@@ -123,7 +123,9 @@ def peaks_file():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 / FP16; it gives no sustained
+    # (power-capped) rate, so the sustained key is absent and the roofline fractions use the data-sheet figure
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W)"
 
 
 # --------------------------------------------------------------------------------------------
@@ -203,7 +205,7 @@ def _instances_key(peaks, stride):
 
 
 def c4_parity(spec, weights, handle, frames, pred16, model16, n_oracle=2, stride=4, thr=0.2, tag="fp16"):
-    """End-to-end parity of the BENCHMARKED path (fp16 activations, tcgen05 convs) on the bench frames themselves:
+    """End-to-end parity of the BENCHMARKED path (fp16 activations, tensor-core convs) on the bench frames themselves:
     against the strict fp32 CUDA path (precision=1, same post-processing kernels) on all frames, and against the fp32
     CPU oracle network (torch) on the first `n_oracle` frames.  Not timed.  Reference being matched:
     sleap/nn/inference.py:2864-3003 (BottomUpInferenceLayer.call)."""
@@ -302,6 +304,24 @@ def analytic_parity(handle, n_frames=8, n_instances=5):
     return {"frames": n_frames, "peaks": n_peaks, "instances": n_inst, "peak_indices_bit_exact": idx_ok,
             "instance_assignments_bit_exact": asg_ok, "max_peak_xy_err_px": max_xy, "max_line_score_err": max_ls,
             "max_instance_score_err": max_sc}
+
+
+def dump_outputs(out_dir, t_rec, max_instances, n_nodes):
+    """The device records of the last timed step, as a caller of sb_infer_bottomup_dev receives them, one .npy per array.
+    The records mark a missing node and an unused instance slot with NaN; here those entries are written as 0 and
+    `node_present` (1 where an instance has the node) says which are real, so every array is finite.  float32, the
+    instance count float64.  The frames are seeded, so two builds can be compared output for output."""
+    import torch
+    from sleap_b200 import parallel
+    torch.cuda.synchronize()
+    peaks, vals, scores, n_valid = (t.cpu().numpy() for t in parallel.unpack_records(t_rec.clone(), max_instances, n_nodes))
+    present = np.isfinite(peaks).all(axis=-1) & np.isfinite(vals)
+    out = {"instance_peaks": np.where(present[..., None], peaks, 0), "instance_peak_vals": np.where(present, vals, 0),
+           "instance_scores": np.where(np.isfinite(scores), scores, 0), "node_present": present}
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+    np.save(os.path.join(out_dir, "n_valid.npy"), n_valid.astype(np.float64))
 
 
 def run_reference(args):
@@ -493,6 +513,8 @@ def run_ours(args):
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_max = float(t.item())
     value = world * B * args.steps / (ms_max / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, t_rec, I, C)
 
     # ---------------- sustained: the same loop for >= --sustained-seconds (power-capped clocks) ----------------
     sustained = None
@@ -562,7 +584,7 @@ def run_ours(args):
             dist.destroy_process_group()
         return
 
-    # ---------------- roofline of the dominant kernel (k_conv_tc) ----------------
+    # ---------------- roofline of the dominant kernel (k_conv_wg) ----------------
     n_ops = c_int32(0)
     cap = 256
     op_ms = np.zeros(cap, np.float32); op_kind = np.zeros(cap, np.int32); op_fl = np.zeros(cap, np.float64)
@@ -582,27 +604,17 @@ def run_ours(args):
     # serialises the forked transposed-conv phases and adds an event per op, so its sum is only the fallback
     tc_ms = float(fwd_ms.mean()) if len(fwd_ms) else per_op_ms
     peaks, peaks_src = peaks_file()
-    # a timed region shorter than ~1 s runs at boost clocks (1965 MHz, ~300 W): the honest denominator is the BURST
-    # cuBLAS figure; the power-capped "sustained" figure belongs to the seconds-long loop reported under `sustained`
+    # a timed region shorter than ~1 s runs at boost clocks: the honest denominator is the BURST figure; the power-capped
+    # "sustained" figure belongs to the seconds-long loop reported under `sustained`
     burst_region = ms_max < 1000.0
     peak_key = "bf16_tflops" if burst_region else "bf16_tflops_sustained"
     peak_tf = float(peaks.get(peak_key, peaks.get("bf16_tflops")))
     achieved_tf = tc_flops / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
     step_ms = ms_max / args.steps
-    traffic, traffic_src = None, None
-    for tname in ("r02_tc_traffic.json",):                               # ncu capture of THIS round's code and autotune picks only
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if os.path.exists(tpath) and B == FRAMES_PER_GPU and prec == 0:  # ncu dram__bytes_read+write of the same launches
-            tj = json.load(open(tpath))
-            traffic = tj.get("traffic_bytes_per_step")
-            traffic_src = (f"profiles/{tname}: ncu dram__bytes_read.sum+dram__bytes_write.sum summed over the conv launches of "
-                           f"{tj.get('steps_captured', 1)} captured step(s), divided by that count")
-            break
-    roofline = {"bound": "tensor", "kernel": "k_conv_tc (tcgen05 implicit-GEMM conv, all %d launches of a step)" % int(tc.sum()),
+    roofline = {"bound": "tensor", "kernel": "k_conv_wg (wgmma implicit-GEMM conv, all %d launches of a step)" % int(tc.sum()),
                 "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
                 "peak_source": f"{peaks_src} {peak_key} ({'timed region < 1 s: boost clocks' if burst_region else 'timed region >= 1 s'})",
                 "frac_of_sustained_peak": achieved_tf / float(peaks.get("bf16_tflops_sustained", peak_tf)),
-                "traffic": traffic, "traffic_source": traffic_src,
                 "kernel_ms_per_step": tc_ms, "kernel_share_of_step": tc_ms / step_ms if step_ms else None,
                 "kernel_timing": (f"CUDA event pair around the conv launches of each of the {len(fwd_ms)} timed steps, on the launching "
                                   "stream (sb_model_forward_times); the previous step's peak / grouping kernels overlap on a second stream"
@@ -615,7 +627,7 @@ def run_ours(args):
 
     # per-layer floors: a layer is bound by the larger of its tensor floor (FLOPs / sustained bf16 peak) and its HBM
     # floor (activation bytes in + out at storage width / measured copy bandwidth); the whole network's attainable
-    # time is the sum of those floors.  Informational (tools/layer_rooflines.py writes the per-layer table).
+    # time is the sum of those floors.  Informational.
     try:
         c4_layers = [(1, 1, 16, 1024, 1024, 9, 1.0, 2), (2, 16, 16, 1024, 1024, 9, 1.25, 2), (4, 16, 32, 512, 512, 9, 1.0, 2),
                      (5, 32, 32, 512, 512, 9, 1.25, 2), (7, 32, 64, 256, 256, 9, 1.0, 2), (8, 64, 64, 256, 256, 9, 1.25, 2),
@@ -683,7 +695,7 @@ def run_ours(args):
                 ev1.record(stream)
             torch.cuda.synchronize()
             ms2 = ev0.elapsed_time(ev1)
-            strict = {"precision": "split fp16 pairs on tcgen05 (hi*Wh + lo*Wh + hi*Wl, fp32 accumulate), precision=2",
+            strict = {"precision": "split fp16 pairs on the tensor cores (hi*Wh + lo*Wh + hi*Wl, fp32 accumulate), precision=2",
                       "value": B * args.steps / (ms2 / 1e3), "unit": "frames/s", "ms_per_step": ms2 / args.steps, "steps": args.steps,
                       "tensor_tflops_issued": 3 * GFLOP_PER_FRAME * 1e9 * B * args.steps / (ms2 / 1e3) / 1e12,
                       "parity": c4_parity(spec, weights, handle, host[0].numpy(), p2, m2, n_oracle=2, tag="split")}
@@ -700,7 +712,7 @@ def run_ours(args):
             "config": {"workload": "C4 bottom-up UNet(f16,r2,ms32,os4,tconv)+PAF 1024x1024x1, 13 nodes/12 edges (flies13)",
                        "frames_per_gpu_per_step": B, "global_batch": world * B, "parallelism": f"frame-shard x{world}",
                        "gflop_per_frame": GFLOP_PER_FRAME,
-                       "l2": "3 rotating input batches; per-step activation working set ~2.9 GB >> 126 MB L2",
+                       "l2": "3 rotating input batches; per-step activation working set ~2.9 GB >> 50 MB L2",
                        "accumulate": "fp32", "head_outputs": "fp32", "mean_instances_per_frame": n_inst_mean, "exchange": exchange,
                        "heads_calibrated_to_peaks_per_channel": TARGET_PEAKS_PER_CHANNEL,
                        "programmatic_dependent_launch": not bool(os.environ.get("SB_DISABLE_PDL"))},
@@ -728,6 +740,8 @@ def main():
     ap.add_argument("--no-parity", action="store_true", help="skip the (untimed) fp16-vs-fp32 parity block")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--ncu-step", action="store_true", help="profiler window (cudaProfilerStart/Stop) around --steps warm steps, no bench line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed step (instance peaks / peak values / scores / node mask / counts) as DIR/<name>.npy")
     args = ap.parse_args()
     # keep stdout clean for the ONE JSON line (NCCL / torchrun print banners on stdout)
     saved_stdout = os.dup(1)

@@ -1,5 +1,5 @@
 /*
- * libsleapb200 -- C-ABI of the B200-native SLEAP inference path.
+ * libsleapb200 -- C-ABI of the H100-native SLEAP inference path.
  *
  * The reference (talmolab/sleap v1.4.1) has no FFI: its seam is the Python class surface
  * sleap.nn.inference.{Predictor, InferenceModel, InferenceLayer} plus the function-level

@@ -1,4 +1,4 @@
-"""sleap_b200: B200-native (sm_100a) batched-frame pose inference path with the
+"""sleap_b200: H100-native (sm_90a) batched-frame pose inference path with the
 ``sleap.nn.inference`` surface.  All device work goes through ``libsleapb200.so`` (C-ABI);
 there is no CPU fallback: using any op without a CUDA device raises."""
 __version__ = "0.1.0"

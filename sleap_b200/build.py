@@ -1,4 +1,4 @@
-"""Builds libsleapb200.so (C-ABI, sm_100a) in-tree with nvcc.  No GPU needed to build."""
+"""Builds libsleapb200.so (C-ABI, sm_90a) in-tree with nvcc.  No GPU needed to build."""
 import hashlib
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsleapb200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 # per-file extra flags: post-processing must not contract multiply-adds (bit-exact parity)
 EXTRA = {"sb_post.cu": ["-fmad=false"]}

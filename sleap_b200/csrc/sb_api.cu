@@ -39,8 +39,8 @@ int sb_create(int device_id, sb_handle_t* out_handle) {
   cudaDeviceProp prop;
   SB_CUDA(h, cudaGetDeviceProperties(&prop, device_id));
   h->sm_count = prop.multiProcessorCount;
-  if (prop.major != 10)
-    fprintf(stderr, "[sleap_b200] warning: device %d is sm_%d%d; kernels are built for sm_100a\n",
+  if (prop.major != 9 || prop.minor != 0)
+    fprintf(stderr, "[sleap_b200] warning: device %d is sm_%d%d; kernels are built for sm_90a\n",
             device_id, prop.major, prop.minor);
   SB_CUDA(h, cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
   h->stream = h->own_stream;

@@ -1,4 +1,4 @@
-// Shared definitions for libsleapb200 (sm_100a).  Internal header; the public C-ABI is
+// Shared definitions for libsleapb200 (sm_90a).  Internal header; the public C-ABI is
 // include/sleap_b200.h.
 #pragma once
 #include <cuda_runtime.h>
@@ -95,7 +95,7 @@ struct sb_handle_s {
   std::vector<void*> owned;                 // generic device allocations freed at destroy
   std::vector<SbModel*> models;
   int gpu_launches = 0;                     // kernels launched by this handle (bench: gpu_launches)
-  int sm_count = 148;
+  int sm_count = 132;
 };
 
 extern thread_local std::string g_sb_last_error;

@@ -1,32 +1,21 @@
-// Fused first encoder block of the UNet for sm_100a: raw frame -> conv0 (3x3, 1 -> 16, bias, ReLU) -> conv1 (3x3,
-// 16 -> 16, bias, ReLU) -> MaxPool2D(2, 2), one persistent kernel.  Neither the 16-channel full-resolution tensor
-// between the two convolutions nor conv1's own full-resolution output ever leaves the SM: per 8-frame C4 step that
-// removes 268 MB of writes + 268 MB of reads (+ 268 MB of dead stores) and two of the three full-resolution epilogues.
+// Fused first encoder block of the UNet for sm_90a: raw frame -> conv0 (3x3, 1 -> 16, bias, ReLU) -> conv1 (3x3,
+// 16 -> 16, bias, ReLU) -> MaxPool2D(2, 2) in one kernel.  Neither the 16-channel full-resolution tensor between the
+// two convolutions nor conv1's own full-resolution output leaves the SM: per 8-frame C4 step that removes 268 MB of
+// writes + 268 MB of reads of the intermediate and conv1's dead full-resolution stores.
 //
 // Replaces, for that block: InferenceLayer.preprocess (sleap/nn/inference.py:940-967, uint8 -> float * 1/255, zero
 // pad to the stride) and the Keras layers stack0_enc0_conv0/act0, conv1/act1 and the pool of enc1
 // (sleap/nn/architectures/encoder_decoder.py:94-144, unet.py:140-205), as dispatched to cuDNN by TensorFlow.
 //
-// Both convolutions run on tcgen05 in the pixel-group ("Toeplitz") form: M = 128 groups of 4 consecutive pixels of one
-// image row (a 512-pixel strip), N = 4 pixels x 16 output channels = 64, and per filter row ky the K dimension is the
-// group's 6-pixel input window:
-//   conv0: K = 16 (6 window pixels, zero padded), A = fp16 window tile built from the frame (SWIZZLE_32B rows);
-//   conv1: K = 6 x 16 = 96, issued as six K = 16 steps whose A operand is conv0's output row in shared memory laid
-//          out as NHWC with 4 pixels (128 B) per SWIZZLE_128B row: group g's window starts 32 B before its own row,
-//          so step j reads with start address row + 96 + 32 j and the standard 128-byte row pitch -- the overlapping
-//          windows cost nothing.  B[ky][j][(p, co)][ci] = w[ky][j - p][ci][co] (zero unless 0 <= j - p <= 2).
-// With N = 64 the shared-memory operand feed and the tensor pipe are balanced (the direct N = 16 form of the same
-// layer is 4x feed-bound); half of B is structural zeros, i.e. 2x the useful MACs on an otherwise idle pipe.
-//
-// Warp roles (448 threads, one CTA per SM, each CTA owns a contiguous range of (frame, strip, row pair) items):
-//   warp 0     frame rows -> staging ring through cp.async (up to 8 rows ahead)
-//   warp 13    the two halo pixels of every conv0 row (x = strip start - 1 and strip end) on the CUDA cores
-//              (32 lanes = 2 pixels x 16 channels)
-//   warps 10-11  staged rows -> conv0 window tiles (fp16, SWIZZLE_32B A operand), two pixel groups per thread
-//   warp 1     conv0 MMA issuer (3 MMAs per row);   warp 12: conv1 MMA issuer (18 MMAs per row); tcgen05.commit hand-offs
-//   warps 2-5  conv0 accumulator (TMEM) -> + bias, ReLU, fp16 -> swizzled ring row (conv1's A operand)
-//   warps 6-9  two conv1 accumulators (rows 2k, 2k+1) -> 2x2 max, + bias, ReLU, fp16 -> pooled NHWC output:
-//              every thread owns 2 pooled pixels x 16 channels = 64 contiguous bytes, a warp 2 KB
+// One CTA = one 16x8-pixel tile of conv1's output (M = 128), two warpgroups:
+//   1. the 20x12 frame patch around the tile -> shared memory (fp16-rounded pixels, zero outside the frame);
+//   2. conv0 on the CUDA cores for the 18x10 pixels conv1 reads, written as fp16 into three 32-byte-swizzled
+//      [160 rows x 16 ch] A tiles, one per filter column of conv1 (tile kx row 16 yy + xx = conv0 pixel
+//      (y0 - 1 + yy, x0 + kx - 1 + xx)), so that filter row ky of that column is the start offset 16 ky rows;
+//   3. conv1 as nine wgmma m64n16k16 per warpgroup (fp32 accumulators in registers), weights [tap][co][ci] in shared memory;
+//   4. accumulators -> shared-memory staging -> bias, ReLU, fp16 rounding, 2x2 max -> pooled NHWC output.
+// The same rounding points as the separate launches (fp16 frame pixels and weights, fp16 intermediate, fp16 conv1
+// output before the pool).
 #include <cuda.h>
 
 #include <algorithm>
@@ -37,465 +26,160 @@ namespace {
 
 #include "sb_tc_prims.cuh"
 
-constexpr int RING_ROW_BYTES = 17 * 1024;   // 130 groups x 128 B = 16640, rounded up to keep every row 1024-aligned
-constexpr int RC = 6;                       // conv0-output ring rows
-constexpr int RI = 6;                       // window-tile ring rows (4 KB each)
-constexpr int STG = 8;                      // staged frame rows (cp.async ring)
-constexpr int STG_ROW = 2112;               // 130 words of 4 pixels (px xs-4 .. xs+515): 520 B (uint8) / 2080 B (float)
-constexpr int S0 = 4, S1 = 4;               // TMEM accumulator stages of conv0 / conv1 (64 columns each): 512 columns
+constexpr int TW = 16, TH = 8;
+constexpr int PW = TW + 4, PH = TH + 4;     // frame patch
+constexpr int CW0 = TW + 2, CH0 = TH + 2;   // conv0 pixels conv1 reads
+constexpr int A_ROWS = CH0 * TW;            // 160 rows of 32 B per A tile
+constexpr int A_BYTES = A_ROWS * 32;        // 5120
+constexpr int SP = 20;                      // staging row pitch (floats)
 
-constexpr int OFF_W1 = 0;                               // 6 x 8 KB
-constexpr int OFF_W0 = 48 * 1024;                       // 3 x 2 KB
-constexpr int OFF_IN = OFF_W0 + 6 * 1024;               // RI x 4 KB
-constexpr int OFF_RING = OFF_IN + RI * 4096;            // RC x 17 KB
-constexpr int OFF_STG = OFF_RING + RC * RING_ROW_BYTES; // STG x STG_ROW
-constexpr int OFF_PAR = OFF_STG + STG * STG_ROW;        // bias0[16] bias1[16] w0h[144] lut[256]
-constexpr int OFF_BAR = OFF_PAR + (176 + 256) * 4;
-constexpr int N_BARS = 1 + 2 * RI + 2 * S0 + 2 * RC + 2 * S1 + 2 * STG;
-constexpr int SMEM_BYTES = OFF_BAR + N_BARS * 8 + 16 + 1024;
-constexpr int SMEM_LAUNCH = SMEM_BYTES > 225 * 1024 ? SMEM_BYTES : 225 * 1024;
+constexpr int OFF_A = 0;                                // 3 A tiles
+constexpr int OFF_W1 = OFF_A + 3 * A_BYTES;             // 9 taps x [16 co][16 ci] fp16 = 9 x 512 B
+constexpr int OFF_STAGE = OFF_W1 + 9 * 512;             // [128][SP] fp32
+constexpr int OFF_PATCH = OFF_STAGE + 128 * SP * 4;     // [PH][PW] fp32
+constexpr int OFF_PAR = OFF_PATCH + PH * PW * 4;        // w0h[144] bias0[16] bias1[16]
+constexpr int SMEM_BYTES = OFF_PAR + (144 + 32) * 4 + 1024;
 
 struct C01Params {
   const void* frames;
   int frames_u8;
-  int Hin, Win, Hnet, Wnet, B, n_strips;
+  int Hin, Win, Hnet, Wnet, tiles_x;
   __half* pool_out;
   int pool_H, pool_W, pool_Ctot, pool_coff;
   const float* bias0;
   const float* bias1;
   const float* w0h;          // conv0 weights rounded to fp16, as float: [9][16]
+  const __half* w1t;         // conv1 weights [9][16 co][16 ci] fp16
   int relu0, relu1;
-  uint32_t idesc;            // M = 128, N = 64, fp16 x fp16 -> fp32
-  long long total_pairs;     // B * n_strips * Hnet / 2
-  long long* dbg;            // profiling only (SB_C01_TIMING): per-role cycles spent in each mbarrier wait, CTA 0
-  int ablate;                // profiling only (SB_C01_ABLATE): 1 no window build, 2 no halo math, 4 no conv1 MMAs, 8 no conv0
-                             // epilogue, 16 no final epilogue, 32 no conv0 MMAs -- results are then garbage
 };
 
-struct Seg { int b, strip, ya, n; };     // conv1 rows [ya, ya + n) of (frame b, strip)
-
-// Walks the segments of this CTA's item range [p0, p1) (items = row pairs in (frame, strip, pair) order).
-struct SegIter {
-  long long p, p1;
-  int PH, n_strips;
-  __device__ __forceinline__ bool next(Seg& s) {
-    if (p >= p1) return false;
-    const long long per = PH;
-    const long long q = p / per;                 // (b, strip) index
-    const int pa = (int)(p - q * per);
-    const long long end = min(p1, (q + 1) * per);
-    s.b = (int)(q / n_strips);
-    s.strip = (int)(q - (long long)s.b * n_strips);
-    s.ya = 2 * pa;
-    s.n = 2 * (int)(end - p);
-    p = end;
-    return true;
-  }
-};
-
-// profiling aid: cycles spent inside a wait are added to slot `k` of this thread's counters
-#define C01_WAIT(k, bar, par, tag)                                        \
-  do {                                                                    \
-    const long long _t0 = P.dbg ? clock64() : 0;                          \
-    mbar_wait((bar), (par), (tag));                                       \
-    if (P.dbg) wcyc[k] += clock64() - _t0;                                \
-  } while (0)
+// byte offset of 16-byte chunk c of row r in a 32-byte-swizzled K-major tile (chunk bit 4 ^= address bit 7)
+__device__ __forceinline__ int sw32(int r, int c) { return r * 32 + ((c ^ ((r >> 2) & 1)) << 4); }
 
 template <typename TI>
-__global__ void __launch_bounds__(448, 1) k_conv01(const __grid_constant__ CUtensorMap mapW0, const __grid_constant__ CUtensorMap mapW1,
-                                                   const __grid_constant__ C01Params P) {
+__global__ void __launch_bounds__(256) k_conv01(const __grid_constant__ C01Params P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* s_b0 = reinterpret_cast<float*>(base + OFF_PAR);
+  float* s_stage = reinterpret_cast<float*>(base + OFF_STAGE);
+  float* s_patch = reinterpret_cast<float*>(base + OFF_PATCH);
+  float* s_w0 = reinterpret_cast<float*>(base + OFF_PAR);
+  float* s_b0 = s_w0 + 144;
   float* s_b1 = s_b0 + 16;
-  float* s_w0 = s_b1 + 16;
-  float* s_lut = s_w0 + 144;          // uint8 pixel -> fp16-rounded (b / 255) as float: what the tensor path multiplies
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + OFF_BAR);
-  uint64_t* wbar = bars;
-  uint64_t* in_full = wbar + 1;
-  uint64_t* in_empty = in_full + RI;
-  uint64_t* c0_full = in_empty + RI;
-  uint64_t* c0_empty = c0_full + S0;
-  uint64_t* ring_full = c0_empty + S0;
-  uint64_t* ring_empty = ring_full + RC;
-  uint64_t* c1_full = ring_empty + RC;
-  uint64_t* c1_empty = c1_full + S1;
-  uint64_t* stg_full = c1_empty + S1;
-  uint64_t* stg_empty = stg_full + STG;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stg_empty + STG);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int x0 = (blockIdx.x % P.tiles_x) * TW, y0 = (blockIdx.x / P.tiles_x) * TH, b = blockIdx.y;
 
-  for (int i = threadIdx.x; i < 176; i += blockDim.x)
-    s_b0[i] = i < 16 ? (P.bias0 ? P.bias0[i] : 0.f) : (i < 32 ? (P.bias1 ? P.bias1[i - 16] : 0.f) : P.w0h[i - 32]);
-  for (int i = threadIdx.x; i < 256; i += blockDim.x)
-    s_lut[i] = __half2float(__float2half_rn(__fmul_rn((float)i, 1.0f / 255.0f)));   // ensure_float (sleap/nn/data/normalization.py:34-49)
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(wbar), 1);
-    for (int i = 0; i < RI; ++i) { mbar_init(smem_u32(in_full + i), 2); mbar_init(smem_u32(in_empty + i), 1); }
-    for (int i = 0; i < STG; ++i) { mbar_init(smem_u32(stg_full + i), 32); mbar_init(smem_u32(stg_empty + i), 3); }
-    for (int i = 0; i < S0; ++i) { mbar_init(smem_u32(c0_full + i), 1); mbar_init(smem_u32(c0_empty + i), 4); }
-    for (int i = 0; i < RC; ++i) { mbar_init(smem_u32(ring_full + i), 5); mbar_init(smem_u32(ring_empty + i), 1); }   // ring_empty: [RC / 2] pairs used
-    for (int i = 0; i < S1; ++i) { mbar_init(smem_u32(c1_full + i), 1); mbar_init(smem_u32(c1_empty + i), 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW0) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapW1) : "memory");
+  // weights / biases (static) and the frame patch
+  for (int i = tid; i < 9 * 16 * 2; i += 256) {        // 9 taps x 16 rows x 2 chunks
+    const int t = i >> 5, r = (i >> 1) & 15, c = i & 1;
+    *reinterpret_cast<uint4*>(base + OFF_W1 + t * 512 + sw32(r, c)) = reinterpret_cast<const uint4*>(P.w1t + (t * 16 + r) * 16)[c];
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+  if (tid < 144) s_w0[tid] = P.w0h[tid];
+  if (tid < 16) { s_b0[tid] = P.bias0 ? P.bias0[tid] : 0.f; s_b1[tid] = P.bias1 ? P.bias1[tid] : 0.f; }
+  const float sc = P.frames_u8 ? (1.0f / 255.0f) : 1.0f;     // ensure_float (normalization.py:34-49)
+  const TI* img = reinterpret_cast<const TI*>(P.frames) + (size_t)b * P.Hin * P.Win;
+  for (int i = tid; i < PH * PW; i += 256) {
+    const int y = y0 - 2 + i / PW, x = x0 - 2 + i % PW;
+    float v = 0.f;
+    if (y >= 0 && y < P.Hin && x >= 0 && x < P.Win) v = __half2float(__float2half_rn(__fmul_rn((float)img[(size_t)y * P.Win + x], sc)));
+    s_patch[i] = v;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  // programmatic dependent launch: this CTA owns the SM (448 threads, ~all of its shared memory), so the next kernel's CTAs
-  // may be scheduled as SMs drain; the pooled output buffer this kernel writes is read by the previous step's second
-  // kernel, so nothing is stored before the previous kernel chain has completed
-  griddep_launch();
-  griddep_wait();
 
-  long long wcyc[3] = {0, 0, 0};
-  const long long t_start = P.dbg ? clock64() : 0;
-  SegIter it;
-  it.PH = P.Hnet / 2; it.n_strips = P.n_strips;
-  it.p = P.total_pairs * blockIdx.x / gridDim.x;
-  it.p1 = P.total_pairs * (blockIdx.x + 1) / gridDim.x;
-  Seg sg;
-
-  // value of staged pixel k of a row as the tensor path sees it (fp16-rounded, as float)
-  auto px = [&](const uint8_t* row, int k) -> float {
-    if (sizeof(TI) == 1) return s_lut[row[k]];
-    return __half2float(__float2half_rn(reinterpret_cast<const float*>(row)[k]));
-  };
-
-  if (warp == 0) {
-    // ---------- frame rows -> staging ring (cp.async; runs ahead of the consumers by up to STG rows) ----------
-    if (lane == 0) {
-      mbar_expect_tx(smem_u32(wbar), 6u * 8192u + 3u * 2048u);
-      for (int ky = 0; ky < 3; ++ky) {
-        tma_load_3d(smem_u32(base + OFF_W1 + (2 * ky) * 8192), &mapW1, smem_u32(wbar), 0, 0, ky);
-        tma_load_3d(smem_u32(base + OFF_W1 + (2 * ky + 1) * 8192), &mapW1, smem_u32(wbar), 64, 0, ky);
-        tma_load_3d(smem_u32(base + OFF_W0 + ky * 2048), &mapW0, smem_u32(wbar), 0, 0, ky);
+  // conv0 for the CH0 x CW0 pixels conv1 reads, 8 channels per item; zero outside the network image (conv1's SAME pad)
+  for (int it = tid; it < CH0 * CW0 * 2; it += 256) {
+    const int half = it & 1, p = it >> 1, yy = p / CW0, cx = p % CW0;
+    const int y = y0 - 1 + yy, x = x0 - 1 + cx;
+    __align__(16) __half h[8];
+    if (y >= 0 && y < P.Hnet && x >= 0 && x < P.Wnet) {
+      float acc[8];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) {
+          const float v = s_patch[(yy + ky) * PW + cx + kx];
+#pragma unroll
+          for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, s_w0[(ky * 3 + kx) * 16 + 8 * half + c], acc[c]);
+        }
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        float v = acc[c] + s_b0[8 * half + c];
+        if (P.relu0) v = fmaxf(v, 0.f);
+        h[c] = __float2half_rn(v);
       }
+    } else {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) h[c] = __float2half_rn(0.f);
     }
-    const TI* frames = reinterpret_cast<const TI*>(P.frames);
-    // A plain load loop here was the whole kernel's critical path (~17 dependent global loads per row on one warp): rows
-    // come in through cp.async.  Words of 4 pixels; a word is entirely inside or outside the frame
-    // (W % 4 == 0, strips start at multiples of 512); outside -> zero fill (zero padding of the frame).
-    unsigned pf_cnt = 0;
-    while (it.next(sg)) {
-      const int xs0 = sg.strip * 512 - 4;
-      for (int ii = 0; ii < sg.n + 4; ++ii, ++pf_cnt) {
-        const unsigned slot = pf_cnt % STG;
-        C01_WAIT(0, smem_u32(stg_empty + slot), ((pf_cnt / STG) & 1) ^ 1, 103);   // builders + halo are done with the row it held
-        const int ri = sg.ya - 2 + ii;
-        const bool row_ok = ri >= 0 && ri < P.Hin;
-        const TI* src_row = frames + ((size_t)sg.b * P.Hin + (row_ok ? ri : 0)) * P.Win;
-        const uint32_t dst_row = smem_u32(base + OFF_STG + slot * STG_ROW);
-        for (int w = lane; w < 130; w += 32) {
-          const int x = xs0 + 4 * w;
-          const bool ok = row_ok && x >= 0 && x < P.Win;
-          const TI* src = src_row + (ok ? x : 0);
-          if (sizeof(TI) == 1)
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst_row + 4 * w), "l"(src), "r"(ok ? 4 : 0) : "memory");
-          else
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst_row + 16 * w), "l"(src), "r"(ok ? 16 : 0) : "memory");
-        }
-        asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(stg_full + slot)) : "memory");   // one arrival per lane
-      }
-    }
-  } else if (warp == 13) {
-    // ------ the two halo pixels of every conv0 row (x = strip start - 1, strip end) on the CUDA cores: 2 px x 16 channels ------
-    unsigned in_cnt = 0, c0_cnt = 0;
-    while (it.next(sg)) {
-      const int xs = sg.strip * 512;
-      for (int ii = 0; ii < sg.n + 4; ++ii, ++in_cnt) {
-        C01_WAIT(1, smem_u32(stg_full + in_cnt % STG), (in_cnt / STG) & 1, 104);
-        // halo pixels of conv0 row i0 = ii - 2 (image row r): frame rows r-1, r, r+1 are items in_cnt-2 .. in_cnt
-        const int i0 = ii - 2;
-        if (i0 >= 0) {
-          const int r = sg.ya - 1 + i0;
-          const int side = lane >> 4, co = lane & 15;
-          const int x = side ? xs + 512 : xs - 1;
-          float acc = 0.f;
-          if (r >= 0 && r < P.Hnet && x >= 0 && x < P.Wnet && !(P.ablate & 2)) {
-            acc = s_b0[co];
 #pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {
-              const uint8_t* rr = base + OFF_STG + ((in_cnt - 2 + ky) % STG) * STG_ROW;
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) acc = fmaf(px(rr, (x - xs + 4) - 1 + kx), s_w0[(ky * 3 + kx) * 16 + co], acc);
-            }
-            if (P.relu0) acc = fmaxf(acc, 0.f);
-          }
-          const unsigned rslot = c0_cnt % RC, rpair = rslot >> 1;
-          C01_WAIT(2, smem_u32(ring_empty + rpair), ((c0_cnt / RC) & 1) ^ 1, 102);
-          uint8_t* row = base + OFF_RING + rslot * RING_ROW_BYTES;
-          // px xs-1 = pixel 3 of ring group 0 (chunks 6, 7; group 0: no swizzle); px xs+512 = pixel 0 of group 129 (129 & 7 = 1)
-          const int off = side ? (129 * 128 + (((co >> 3) ^ 1) * 16) + (co & 7) * 2) : (96 + co * 2);
-          *reinterpret_cast<__half*>(row + off) = __float2half_rn(acc);
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(smem_u32(ring_full + rslot));
-            mbar_arrive(smem_u32(stg_empty + (in_cnt - 2) % STG));    // row in_cnt - 2 is not needed by later halo pixels
-            if (ii == sg.n + 3) {                                      // end of the segment: its last two rows as well
-              mbar_arrive(smem_u32(stg_empty + (in_cnt - 1) % STG));
-              mbar_arrive(smem_u32(stg_empty + in_cnt % STG));
-            }
-          }
-          ++c0_cnt;
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 10 || warp == 11) {
-    // ---------------- staged frame rows -> conv0 window tiles (A operand, SWIZZLE_32B rows of 16 halves) ----------------
-    const int tb = (warp - 10) * 32 + lane;            // 64 builder threads, two pixel groups each
-    unsigned in_cnt = 0;
-    while (it.next(sg)) {
-      for (int ii = 0; ii < sg.n + 4; ++ii, ++in_cnt) {
-        const unsigned slot = in_cnt % RI;
-        C01_WAIT(0, smem_u32(stg_full + in_cnt % STG), (in_cnt / STG) & 1, 105);
-        C01_WAIT(1, smem_u32(in_empty + slot), ((in_cnt / RI) & 1) ^ 1, 101);
-        const uint8_t* stg = base + OFF_STG + (in_cnt % STG) * STG_ROW;
-        uint8_t* tile = base + OFF_IN + slot * 4096;
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          if (P.ablate & 1) break;
-          const int g = tb + 64 * t;
-          __align__(16) __half w[16];
-#pragma unroll
-          for (int j = 0; j < 6; ++j) w[j] = __float2half_rn(px(stg, 4 * g + 3 + j));   // px xs + 4g - 1 + j
-#pragma unroll
-          for (int j = 6; j < 16; ++j) w[j] = __float2half_rn(0.f);
-          const int sw = (g >> 2) & 1;                                                   // SWIZZLE_32B: chunk ^= address bit 7
-          *reinterpret_cast<uint4*>(tile + g * 32 + ((0 ^ sw) * 16)) = *reinterpret_cast<const uint4*>(&w[0]);
-          *reinterpret_cast<uint4*>(tile + g * 32 + ((1 ^ sw) * 16)) = *reinterpret_cast<const uint4*>(&w[8]);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(smem_u32(in_full + slot));
-          mbar_arrive(smem_u32(stg_empty + in_cnt % STG));
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------- conv0 MMA issuer (3 MMAs per row) -------------------------------
-    // Two issuing warps (this one and warp 12 for conv1): with a single issuer every blocking wait of one convolution's
-    // pipeline stalled the other one as well, and the per-row hand-off latency chain, not the tensor pipe, set the pace.
-    mbar_wait(smem_u32(wbar), 0, 111);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint64_t d32 = make_desc(0, 32, 6);
-    const uint32_t in0 = smem_u32(base + OFF_IN), w0a = smem_u32(base + OFF_W0);
-    unsigned in_base = 0, c0_base = 0;
-    while (it.next(sg)) {
-      const int n = sg.n;
-      for (int t = 0; t < n + 2; ++t) {
-        // conv0 row i0 = t: input items in_base + t + ky
-        const unsigned c0 = c0_base + t, st = c0 % S0;
-        C01_WAIT(0, smem_u32(c0_empty + st), ((c0 / S0) & 1) ^ 1, 112);
-        for (int ky = 0; ky < 3; ++ky) {
-          const unsigned ic = in_base + t + ky;
-          if (ky == 2 || t == 0) C01_WAIT(1, smem_u32(in_full + ic % RI), (ic / RI) & 1, 113);   // rows t, t+1 were awaited by row t-1
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-#pragma unroll
-          for (int ky = 0; ky < 3; ++ky) {
-            if (P.ablate & 32) break;
-            const unsigned ic = in_base + t + ky;
-            tc_mma_f16(tmem_base + st * 64, d32 + (uint64_t)((in0 + (ic % RI) * 4096) >> 4), d32 + (uint64_t)((w0a + ky * 2048) >> 4), P.idesc,
-                       ky ? 1u : 0u);
-          }
-          tc_commit(smem_u32(c0_full + st));
-          tc_commit(smem_u32(in_empty + (in_base + t) % RI));
-          if (t == n + 1) {
-            tc_commit(smem_u32(in_empty + (in_base + t + 1) % RI));
-            tc_commit(smem_u32(in_empty + (in_base + t + 2) % RI));
-          }
-        }
-        __syncwarp();
-      }
-      in_base += n + 4; c0_base += n + 2;
-    }
-  } else if (warp == 12) {
-    // ------------------------------- conv1 MMA issuer (18 MMAs per row) -------------------------------
-    mbar_wait(smem_u32(wbar), 0, 116);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint64_t d128 = make_desc(0, 128, 2);
-    const uint32_t w1a = smem_u32(base + OFF_W1), ring0 = smem_u32(base + OFF_RING);
-    unsigned c0_base = 0, c1_base = 0;
-    while (it.next(sg)) {
-      const int n = sg.n;
-      for (int i1 = 0; i1 < n; ++i1) {
-        // conv1 row i1: ring items c0_base + i1 + ky
-        const unsigned c1 = c1_base + i1, st = c1 % S1;
-        C01_WAIT(0, smem_u32(c1_empty + st), ((c1 / S1) & 1) ^ 1, 114);
-        for (int ky = 0; ky < 3; ++ky) {
-          const unsigned rc = c0_base + i1 + ky;
-          if (ky == 2 || i1 == 0) C01_WAIT(1, smem_u32(ring_full + rc % RC), (rc / RC) & 1, 115);
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (elect_one()) {
-#pragma unroll
-          for (int ky = 0; ky < 3; ++ky) {
-            if (P.ablate & 4) break;
-            const unsigned rc = c0_base + i1 + ky;
-            const uint32_t arow = ring0 + (rc % RC) * RING_ROW_BYTES + 96;
-#pragma unroll
-            for (int j = 0; j < 6; ++j) {
-              const uint32_t wt = w1a + (2 * ky + (j >> 2)) * 8192 + (j & 3) * 32;
-              tc_mma_f16(tmem_base + S0 * 64 + st * 64, d128 + (uint64_t)((arow + 32 * j) >> 4), d128 + (uint64_t)(wt >> 4), P.idesc,
-                         (ky | j) ? 1u : 0u);
-            }
-          }
-          // hand-offs once per row PAIR (tcgen05.commit costs the issuing thread a few hundred cycles): the accumulators of rows
-          // 2k, 2k+1 are published by one commit (it covers every MMA issued so far), and ring rows are released two at a time
-          if (i1 & 1) {
-            tc_commit(smem_u32(c1_full + st));
-            tc_commit(smem_u32(ring_empty + ((c0_base + i1) % RC >> 1)));          // ring rows i1 - 1, i1
-            if (i1 == n - 1) tc_commit(smem_u32(ring_empty + ((c0_base + i1 + 2) % RC >> 1)));   // ... and the segment's last two
-          }
-        }
-        __syncwarp();
-      }
-      c0_base += n + 2; c1_base += n;
-    }
-  } else if (warp < 6) {
-    // ------------------- conv0 accumulator -> ring row (conv1's A operand) -------------------
-    const int q = warp & 3;
-    const int g = q * 32 + lane;                       // group = TMEM lane
-    const int gi = g + 1;                              // ring group (group 0 holds the left halo pixel)
-    unsigned c0_cnt = 0;
-    while (it.next(sg)) {
-      const int xs = sg.strip * 512;
-      for (int i0 = 0; i0 < sg.n + 2; ++i0, ++c0_cnt) {
-        const int r = sg.ya - 1 + i0;
-        const unsigned st = c0_cnt % S0, rslot = c0_cnt % RC;
-        C01_WAIT(0, smem_u32(c0_full + st), (c0_cnt / S0) & 1, 121);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        C01_WAIT(1, smem_u32(ring_empty + (rslot >> 1)), ((c0_cnt / RC) & 1) ^ 1, 122);
-        uint8_t* row = base + OFF_RING + rslot * RING_ROW_BYTES + gi * 128;
-        const bool row_ok = r >= 0 && r < P.Hnet;
-        const float lo = P.relu0 ? 0.f : -INFINITY;
-#pragma unroll
-        for (int p = 0; p < 4; ++p) {
-          if (P.ablate & 8) break;
-          uint32_t rr[16];
-          tc_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + st * 64 + p * 16, rr);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          __align__(16) __half2 h[8];
-          const bool ok = row_ok && (xs + 4 * g + p) < P.Wnet;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float a = fmaxf(__uint_as_float(rr[2 * j]) + s_b0[2 * j], lo), b = fmaxf(__uint_as_float(rr[2 * j + 1]) + s_b0[2 * j + 1], lo);
-            h[j] = ok ? __floats2half2_rn(a, b) : __floats2half2_rn(0.f, 0.f);
-          }
-          *reinterpret_cast<uint4*>(row + (((2 * p) ^ (gi & 7)) * 16)) = *reinterpret_cast<const uint4*>(&h[0]);
-          *reinterpret_cast<uint4*>(row + (((2 * p + 1) ^ (gi & 7)) * 16)) = *reinterpret_cast<const uint4*>(&h[4]);
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(smem_u32(ring_full + rslot));
-          mbar_arrive(smem_u32(c0_empty + st));
-        }
-      }
-    }
-  } else {
-    // ------------- two conv1 accumulators -> 2x2 max-pool, bias, ReLU -> pooled NHWC output -------------
-    const int q = warp & 3;
-    const int g = q * 32 + lane;
-    unsigned c1_cnt = 0;
-    const float lo = P.relu1 ? 0.f : -INFINITY;
-    while (it.next(sg)) {
-      const int xs = sg.strip * 512;
-      for (int i1 = 0; i1 < sg.n; i1 += 2, c1_cnt += 2) {
-        const unsigned sa = c1_cnt % S1, sb = (c1_cnt + 1) % S1;
-        C01_WAIT(1, smem_u32(c1_full + sb), ((c1_cnt + 1) / S1) & 1, 132);      // committed after both rows of the pair
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int y = sg.ya + i1;
-        const uint32_t ta = tmem_base + ((uint32_t)(q * 32) << 16) + S0 * 64 + sa * 64, tb = tmem_base + ((uint32_t)(q * 32) << 16) + S0 * 64 + sb * 64;
-#pragma unroll
-        for (int pp = 0; pp < 2; ++pp) {
-          if (P.ablate & 16) break;
-          uint32_t a0[16], a1[16], b0[16], b1[16];
-          tc_ld16(ta + (2 * pp) * 16, a0);
-          tc_ld16(ta + (2 * pp + 1) * 16, a1);
-          tc_ld16(tb + (2 * pp) * 16, b0);
-          tc_ld16(tb + (2 * pp + 1) * 16, b1);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          __align__(16) __half2 h[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            // max over the 2x2 window commutes with "+ bias" and with the fp16 rounding (both monotonic)
-            const float m0 = fmaxf(fmaxf(__uint_as_float(a0[2 * j]), __uint_as_float(a1[2 * j])), fmaxf(__uint_as_float(b0[2 * j]), __uint_as_float(b1[2 * j])));
-            const float m1 = fmaxf(fmaxf(__uint_as_float(a0[2 * j + 1]), __uint_as_float(a1[2 * j + 1])),
-                                   fmaxf(__uint_as_float(b0[2 * j + 1]), __uint_as_float(b1[2 * j + 1])));
-            h[j] = __floats2half2_rn(fmaxf(m0 + s_b1[2 * j], lo), fmaxf(m1 + s_b1[2 * j + 1], lo));
-          }
-          const int x = xs + 4 * g + 2 * pp;
-          if (x < P.Wnet && y < P.Hnet) {
-            __half* dst = P.pool_out + (((size_t)sg.b * P.pool_H + (y >> 1)) * P.pool_W + (x >> 1)) * P.pool_Ctot + P.pool_coff;
-            if (((P.pool_Ctot | P.pool_coff) & 15) == 0) st_global_256(dst, h);
-            else {
-              reinterpret_cast<uint4*>(dst)[0] = *reinterpret_cast<const uint4*>(&h[0]);
-              reinterpret_cast<uint4*>(dst)[1] = *reinterpret_cast<const uint4*>(&h[4]);
-            }
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(smem_u32(c1_empty + sa));
-          mbar_arrive(smem_u32(c1_empty + sb));
-        }
-      }
+    for (int kx = 0; kx < 3; ++kx) {                    // tile kx holds this pixel at column cx - kx
+      const int xx = cx - kx;
+      if (xx >= 0 && xx < TW) *reinterpret_cast<uint4*>(base + OFF_A + kx * A_BYTES + sw32(yy * TW + xx, half)) = *reinterpret_cast<uint4*>(h);
     }
   }
-  __syncwarp();
-  if (P.dbg && blockIdx.x == 0 && lane == 0) {         // [warp][wait 0, wait 1, wait 2, role total]
-    long long* d = P.dbg + warp * 4;
-    d[0] = wcyc[0]; d[1] = wcyc[1]; d[2] = wcyc[2]; d[3] = clock64() - t_start;
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
   __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-  }
-}
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  // conv1: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64)
+  const int wg = warp >> 2;
+  float acc[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  const uint64_t desc_hi = make_desc(0, 32, 3);
+  wgmma_fence();
+  wgmma_reg_fence(acc);
+#pragma unroll
+  for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+    for (int kx = 0; kx < 3; ++kx) {
+      const uint32_t a = smem_u32(base + OFF_A + kx * A_BYTES + (ky * TW + 64 * wg) * 32);
+      const uint32_t w = smem_u32(base + OFF_W1 + (ky * 3 + kx) * 512);
+      wgmma_f16<16>(acc, desc_hi + (a >> 4), desc_hi + (w >> 4), (ky | kx) ? 1u : 0u);
+    }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_reg_fence(acc);
 
-EncodeTiledFn get_encode01() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)p;
+  // accumulators -> staging (fragment rows 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1))
+  const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    *reinterpret_cast<float2*>(s_stage + frow * SP + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(s_stage + (frow + 8) * SP + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
   }
-  return fn;
+  __syncthreads();
+
+  // bias, ReLU, fp16 rounding (conv1's stored value), 2x2 max: thread = (pooled pixel, channel pair)
+  const int pp = tid >> 3, cp = 2 * (tid & 7);
+  const int py = pp / (TW / 2), px = pp % (TW / 2);
+  const int gy = (y0 >> 1) + py, gx = (x0 >> 1) + px;
+  if (gy < P.pool_H && gx < P.pool_W) {
+    __half2 m = __float2half2_rn(-INFINITY);
+#pragma unroll
+    for (int a = 0; a < 2; ++a)
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float* s = s_stage + ((2 * py + a) * TW + 2 * px + c) * SP + cp;
+        float v0 = s[0] + s_b1[cp], v1 = s[1] + s_b1[cp + 1];
+        if (P.relu1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        m = __hmax2(m, __floats2half2_rn(v0, v1));
+      }
+    *reinterpret_cast<__half2*>(P.pool_out + (((size_t)b * P.pool_H + gy) * P.pool_W + gx) * P.pool_Ctot + P.pool_coff + cp) = m;
+  }
 }
 
 }  // namespace
 
 struct SbConv01Plan {
-  CUtensorMap mapW0, mapW1;
   C01Params P;
-  __half* w0t = nullptr;     // [3][64][16]
-  __half* w1t = nullptr;     // [3][64][128]
+  __half* w1t = nullptr;     // [9][16][16]
   float* w0h = nullptr;      // [9][16]
   int conv0_op = -1, conv1_op = -1;
 };
 
 void sb_conv01_release(SbModel* m) {
   if (!m->conv01) return;
-  if (m->conv01->w0t) cudaFree(m->conv01->w0t);
   if (m->conv01->w1t) cudaFree(m->conv01->w1t);
   if (m->conv01->w0h) cudaFree(m->conv01->w0h);
   delete m->conv01;
@@ -514,72 +198,41 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
   if (c1.in_buf() != c0.out_buf() || c1.in_coff() != c0.out_coff() || c1.pool_buf() < 0) return 0;
   const SbBuffer& ob0 = m->buffers[c0.out_buf()];
   const SbBuffer& pb = m->buffers[c1.pool_buf()];
-  if (ob0.f32 || pb.f32 || pb.C % 8 || c1.pool_coff() % 8 || ob0.H % 2 || ob0.W % 4) return 0;
+  if (ob0.f32 || pb.f32 || pb.C % 2 || c1.pool_coff() % 2 || ob0.H % 2 || ob0.W % 2) return 0;
   for (size_t oi = 0; oi < m->ops.size(); ++oi)            // conv0's output must feed conv1 only
     if ((int)oi != conv1_op && m->ops[oi].kind() != SB_OPK_PREPROCESS && (int)oi != conv0_op &&
         (m->ops[oi].in_buf() == c0.out_buf() || (m->ops[oi].kind() == SB_OPK_ADD && m->ops[oi].in2_buf() == c0.out_buf())))
       return 0;
-  EncodeTiledFn enc = get_encode01();
-  if (!enc) return 0;
   SbConv01Plan* pl = new SbConv01Plan();
   pl->conv0_op = conv0_op; pl->conv1_op = conv1_op;
   const float* w0 = m->weights_host.data() + c0.w_off();     // [9][1][16]
   const float* w1 = m->weights_host.data() + c1.w_off();     // [9][16][16]
-  std::vector<__half> w0t((size_t)3 * 64 * 16, __float2half(0.f)), w1t((size_t)3 * 64 * 128, __float2half(0.f));
+  std::vector<__half> w1t((size_t)9 * 16 * 16);
   std::vector<float> w0h(144);
   for (int t = 0; t < 9; ++t)
-    for (int co = 0; co < 16; ++co) w0h[t * 16 + co] = __half2float(__float2half_rn(w0[t * 16 + co]));
-  for (int ky = 0; ky < 3; ++ky)
-    for (int p = 0; p < 4; ++p)
-      for (int co = 0; co < 16; ++co)
-        for (int kx = 0; kx < 3; ++kx) {
-          const int j = p + kx;                              // window pixel index: x_in = x_out + kx - 1 = (4g + p) + kx - 1 = (4g - 1) + j
-          w0t[((size_t)ky * 64 + p * 16 + co) * 16 + j] = __float2half_rn(w0[(ky * 3 + kx) * 16 + co]);
-          for (int ci = 0; ci < 16; ++ci)
-            w1t[((size_t)ky * 64 + p * 16 + co) * 128 + j * 16 + ci] = __float2half_rn(w1[((size_t)(ky * 3 + kx) * 16 + ci) * 16 + co]);
-        }
-  auto fail = [&](const char* what) { sb_conv01_release(m); delete pl; return sb_fail(h, SB_ERR_CUDA, "conv01: %s", what); };
-  if (cudaMalloc((void**)&pl->w0t, w0t.size() * 2) != cudaSuccess || cudaMalloc((void**)&pl->w1t, w1t.size() * 2) != cudaSuccess ||
-      cudaMalloc((void**)&pl->w0h, w0h.size() * 4) != cudaSuccess)
-    return fail("cudaMalloc");
-  cudaMemcpy(pl->w0t, w0t.data(), w0t.size() * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(pl->w1t, w1t.data(), w1t.size() * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(pl->w0h, w0h.data(), w0h.size() * 4, cudaMemcpyHostToDevice);
-  {
-    cuuint64_t dims[3] = {16, 64, 3};
-    cuuint64_t strides[2] = {16 * 2, 64 * 16 * 2};
-    cuuint32_t box[3] = {16, 64, 1}, es[3] = {1, 1, 1};
-    if (enc(&pl->mapW0, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, pl->w0t, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail("cuTensorMapEncodeTiled(W0)");
-  }
-  {
-    cuuint64_t dims[3] = {128, 64, 3};
-    cuuint64_t strides[2] = {128 * 2, 64 * 128 * 2};
-    cuuint32_t box[3] = {64, 64, 1}, es[3] = {1, 1, 1};
-    if (enc(&pl->mapW1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, pl->w1t, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return fail("cuTensorMapEncodeTiled(W1)");
+    for (int co = 0; co < 16; ++co) {
+      w0h[t * 16 + co] = __half2float(__float2half_rn(w0[t * 16 + co]));
+      for (int ci = 0; ci < 16; ++ci) w1t[((size_t)t * 16 + co) * 16 + ci] = __float2half_rn(w1[((size_t)t * 16 + ci) * 16 + co]);
+    }
+  auto fail = [&](const char* what) { delete pl; return sb_fail(h, SB_ERR_CUDA, "conv01: %s", what); };
+  if (cudaMalloc((void**)&pl->w1t, w1t.size() * 2) != cudaSuccess) return fail("cudaMalloc");
+  if (cudaMalloc((void**)&pl->w0h, w0h.size() * 4) != cudaSuccess) { cudaFree(pl->w1t); return fail("cudaMalloc"); }
+  m->conv01 = pl;                                          // released with the model from here on
+  if (cudaMemcpy(pl->w1t, w1t.data(), w1t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(pl->w0h, w0h.data(), w0h.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
+    sb_conv01_release(m);
+    return sb_fail(h, SB_ERR_CUDA, "conv01: weight copy");
   }
   C01Params& P = pl->P;
   memset(&P, 0, sizeof(P));
   P.Hin = m->Hin; P.Win = m->Win; P.Hnet = ob0.H; P.Wnet = ob0.W;
-  P.n_strips = (ob0.W + 511) / 512;
+  P.tiles_x = (ob0.W + TW - 1) / TW;
   P.pool_out = (__half*)pb.dev; P.pool_H = pb.H; P.pool_W = pb.W; P.pool_Ctot = pb.C; P.pool_coff = c1.pool_coff();
   P.bias0 = c0.b_off() >= 0 ? m->weights_dev + c0.b_off() : nullptr;
   P.bias1 = c1.b_off() >= 0 ? m->weights_dev + c1.b_off() : nullptr;
-  P.w0h = pl->w0h;
+  P.w0h = pl->w0h; P.w1t = pl->w1t;
   P.relu0 = (c0.flags() & SB_OPF_RELU) ? 1 : 0;
   P.relu1 = (c1.flags() & SB_OPF_RELU) ? 1 : 0;
-  P.idesc = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  static bool attr = false;
-  if (!attr) {
-    if (cudaFuncSetAttribute(k_conv01<unsigned char>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LAUNCH) != cudaSuccess ||
-        cudaFuncSetAttribute(k_conv01<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LAUNCH) != cudaSuccess)
-      return fail("cudaFuncSetAttribute");
-    attr = true;
-  }
-  m->conv01 = pl;
   return 0;
 }
 
@@ -589,33 +242,10 @@ int sb_conv01_conv1_op(const SbModel* m) { return m->conv01 ? m->conv01->conv1_o
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
   SbConv01Plan* pl = m->conv01;
   C01Params P = pl->P;
-  P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.B = B;
-  P.total_pairs = (long long)B * P.n_strips * (P.Hnet / 2);
-  P.ablate = getenv("SB_C01_ABLATE") ? atoi(getenv("SB_C01_ABLATE")) : 0;
-  static long long* dbg_dev = nullptr;
-  if (getenv("SB_C01_TIMING") && !dbg_dev) cudaMalloc((void**)&dbg_dev, 14 * 4 * sizeof(long long));
-  P.dbg = getenv("SB_C01_TIMING") ? dbg_dev : nullptr;
-  const int grid = (int)std::max<long long>(1, std::min<long long>(h->sm_count, P.total_pairs));
-  // programmatic dependent launch (sb_tc_prims.cuh): padded to the SM's whole shared memory so that no CTA of the next
-  // kernel can become co-resident (and queue on TMEM) once this kernel has triggered its dependents
-  cudaLaunchConfig_t cfg = {};
-  const bool pdl = !getenv("SB_DISABLE_PDL");
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(448); cfg.dynamicSmemBytes = pdl ? (size_t)SMEM_LAUNCH : (size_t)SMEM_BYTES; cfg.stream = h->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-  if (frames_are_u8) cudaLaunchKernelEx(&cfg, k_conv01<unsigned char>, pl->mapW0, pl->mapW1, P);
-  else cudaLaunchKernelEx(&cfg, k_conv01<float>, pl->mapW0, pl->mapW1, P);
+  P.frames = frames_dev; P.frames_u8 = frames_are_u8;
+  const dim3 grid(P.tiles_x * ((P.Hnet + TH - 1) / TH), B);
+  if (frames_are_u8) k_conv01<unsigned char><<<grid, 256, SMEM_BYTES, h->stream>>>(P);
+  else k_conv01<float><<<grid, 256, SMEM_BYTES, h->stream>>>(P);
   SB_CHECK_LAUNCH(h);
-  if (P.dbg) {                                          // profiling aid: where each warp role of CTA 0 waited
-    long long hbuf[14 * 4];
-    cudaStreamSynchronize(h->stream);
-    cudaMemcpy(hbuf, P.dbg, sizeof(hbuf), cudaMemcpyDeviceToHost);
-    const char* names[14] = {"stage+halo", "conv0 issue", "mid 0", "mid 1", "mid 2", "mid 3", "final 0", "final 1", "final 2", "final 3",
-                             "build 0", "build 1", "conv1 issue", "halo"};
-    for (int w = 0; w < 14; ++w)
-      fprintf(stderr, "[k_conv01 timing] warp %2d %-12s total %9lld cyc, waits: %9lld %9lld %9lld\n", w, names[w], hbuf[w * 4 + 3], hbuf[w * 4],
-              hbuf[w * 4 + 1], hbuf[w * 4 + 2]);
-  }
   return 0;
 }

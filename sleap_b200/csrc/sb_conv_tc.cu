@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution for sm_100a: NHWC fp16 activations, fp32 accumulation in TMEM.
+// wgmma implicit-GEMM convolution for sm_90a: NHWC fp16 activations, fp32 accumulation in registers.
 //
 // Replaces cuDNN's Conv2D / Conv2DTranspose as dispatched by the reference's Keras graph
 // (sleap/nn/architectures/encoder_decoder.py:117-131, 304-310, 369-389; hourglass.py:36-45;
@@ -8,16 +8,15 @@
 //   GEMM M = 128 output pixels, N = C_out tile (16..256), K = taps x C_in.
 //   A operand: TMA (cp.async.bulk.tensor.4d) loads an NHWC box [KC ch, 16 px, 8+halo rows] with
 //     hardware zero fill outside the image (= TF "SAME" padding) into 128B/64B/32B-swizzled
-//     shared memory, one pixel per row, i.e. exactly the canonical K-major UMMA layout.  The
+//     shared memory, one pixel per row, i.e. exactly the canonical K-major wgmma layout.  The
 //     x shift of a filter tap is baked into the TMA coordinate (one load per distinct dx); the
 //     y shift is a whole number of 16-pixel rows = a swizzle-atom-aligned start-address offset,
 //     so the three ky taps of one dx share one staged tile.
 //   B operand: weights pre-arranged [tap][C_out][C_in] fp16 (K-major), TMA box [KC, N, 1].
-//   D: TMEM accumulator (128 lanes x N fp32 columns), tcgen05.mma.cta_group::1.kind::f16 issued
-//     by one thread; epilogue tcgen05.ld 32x32b -> bias / ReLU / BN affine -> fp16 (or fp32 for
-//     head outputs) NHWC stores into the consumer's channel slice.
+//   D: two warpgroups, each m64nNk16 wgmma over 64 of the 128 pixels; epilogue through a shared-memory
+//     staging tile -> bias / ReLU / BN affine -> fp16 (or fp32 for head outputs) NHWC stores into the
+//     consumer's channel slice.
 //   Conv2DTranspose(k3,s2) = four sub-pixel phase GEMMs over the input grid with strided stores.
-// Warp roles: warp 0 lane 0 = TMA producer, warp 1 lane 0 = MMA issuer, all 4 warps = epilogue.
 #include <cuda.h>
 
 #include <algorithm>
@@ -27,29 +26,13 @@
 namespace {
 
 constexpr int TW = 16, TH = 8;          // output tile (pixels); M = 128
-constexpr int MAX_GROUPS = 7, MAX_TAPS = 7;   // filter columns / rows of the widest kernel taken (7x7); the 3x3 kernels unroll 3
+constexpr int MAX_GROUPS = 7, MAX_TAPS = 7;   // filter columns / rows of the widest kernel taken (7x7)
 // dynamic shared memory every kernel here is opted in for (cudaFuncAttributeMaxDynamicSharedMemorySize); more than
 // half of the SM's 227 KB, so a launch padded to this size is guaranteed to run one CTA per SM
 constexpr size_t kMaxDynSmem = 225 * 1024;
-// shared memory the persistent / halo / programmed variants plan with (filter bank or weight ring + activation ring);
-// barriers, the TMEM slot and the bias / BN vectors come on top (~2.5 KB).  SB_SMEM_BUDGET_KB overrides (<= 220).
-static size_t tc_budget() {
-  static size_t b = 0;
-  if (!b) {
-    const char* e = getenv("SB_SMEM_BUDGET_KB");
-    b = (size_t)std::min(220, std::max(96, e ? atoi(e) : 196)) * 1024;
-  }
-  return b;
-}
 
 struct TcTap { int row_off, w_tap; };
 struct TcGroup { int dx, n_taps; TcTap taps[MAX_TAPS]; };
-
-struct TcProgEntry {          // one step of the MMA program of k_conv_tc_prog (per input-channel chunk), packed for the
-  uint32_t a_acc;             // single issuing thread: a_off16 (activation start offset in the staged box, >> 4) | acc_col << 16
-  uint32_t w_flags;           // w_off16 (resident slice offset >> 4) | first << 16 | n_same << 20 | w_tap << 26
-};                            // first: first step of its accumulator; n_same: entries from here on that share this weight slice
-struct TcAccOut { int16_t dx, dy, oy_add, ox_add; };   // where accumulator s lands: tile offset + output phase
 
 struct TcParams {
   int H, W;                    // iteration grid (input grid for tconv phases, output grid for convs)
@@ -58,9 +41,7 @@ struct TcParams {
   int n_groups;
   TcGroup groups[MAX_GROUPS];
   int dy0, box_rows;
-  int N, Cout;                 // UMMA N of this launch, valid output channels
-  uint32_t idesc;
-  int tmem_cols;
+  int N, Cout;                 // wgmma N of this launch, valid output channels
   void* out;
   int out_f32, out_H, out_W, out_Ctot, out_coff;
   int oy_mul, oy_add, ox_mul, ox_add;
@@ -72,35 +53,10 @@ struct TcParams {
   int pool_H, pool_W, pool_Ctot, pool_coff;
   int a_slot_bytes, b_slot_bytes, n_a_slots, n_b_slots;
   int a_tx_bytes, b_tx_bytes;
-  int layout_type;             // UMMA LayoutType: 2 = SW128, 4 = SW64, 6 = SW32
+  int layout_type;             // wgmma descriptor layout: 1 = SW128, 2 = SW64, 3 = SW32
   int row_bytes;               // KC * 2
-  // persistent variant (weights resident in shared memory, double-buffered TMEM accumulators)
-  int persistent;
-  int tiles_per_img, n_tiles_total;
-  int n_used_taps, used_taps[9], slot_of_tap[9];
-  int w_slot_bytes;
-  // geometry of the output tile: tw x (128/tw) pixels (16x8 for the per-dx staging, 8x16 for halo staging)
-  int tw;
-  // halo variant: ONE staged tile [KC, tw+2, th+2] per chunk; every tap is a start-address offset
-  int n_htaps;
-  int htap_off_rows[9];        // (tap_dy - dy0) * (tw + 2) + (tap_dx - dx0)   [rows of row_bytes]
-  int htap_w[9];               // weight tap index
-  int dx0;
-  int halo_base_offset;        // 1: put (addr >> 7) & 7 into the descriptor's base-offset field
-  int n_stages;                // TMEM accumulator stages of the persistent kernels (2..8)
-  // halo super-tile: sub_x x sub_y sub-tiles of 8x16 pixels share ONE staged halo box and one
-  // barrier round trip (sub-tile s accumulates in TMEM columns [s*N, (s+1)*N) of the stage)
-  int sub_x, sub_y, pitch;     // pitch = 8*sub_x + 2 (pixels per staged row)
-  int epi_groups;              // 1 or 2 sets of 4 epilogue warps (2 only when sub_x*sub_y >= 2)
-  // filter bank too large for shared memory: stream one [N x KC] slice per (chunk, tap) through a ring
-  // of n_w_ring slots; every slice is used by all sub-tiles of the super-tile before it is released
-  int w_stream, n_w_ring;
-  int n_prog, n_acc;
-  TcProgEntry prog[36];
-  TcAccOut acc_out[4];
-  int ablate;                  // profiling only (SB_ABLATE): 1 no TMA, 2 no MMA, 4 no stores, 8 no TMEM loads
   // 1: the common epilogue shape (fp16 NHWC output, no BN affine, C_out a multiple of 16 covering the whole
-  //    N tile, 32-byte aligned channel slices for the output and the fused pool) runs tc_epilogue_cols_fast
+  //    channel tile, 32-byte aligned channel slices for the output and the fused pool) runs tc_epilogue_cols_fast
   int epi_mode;
   // 1: the full-resolution output of this conv has no reader (only its fused 2x2 max-pool is consumed): skip the stores
   int skip_out;
@@ -108,7 +64,7 @@ struct TcParams {
   // Cout channels apart, from out_coff / pool_coff (sb_kernels_direct.cuh: st_split); 0 for fp32 head outputs
   int split;
   // programmatic dependent launch: 1 = call griddepcontrol.launch_dependents after the prologue (host: only for launches
-  // padded to the whole SM's shared memory, so that no CTA of the successor can become co-resident and queue on TMEM)
+  // that own their SMs, so that the successor's CTAs wait for free SMs instead of sharing them)
   int pdl_trigger;
 };
 
@@ -126,7 +82,7 @@ __device__ __forceinline__ void stage_params(const TcParams& P, float* s_par, in
 }
 
 // Shared epilogue: 16 accumulator columns of this thread's pixel -> bias / ReLU / BN -> stores
-// (+ fused 2x2 max-pool).  q = TMEM lane quadrant of the warp (rows 32q .. 32q+31 of the tile).
+// (+ fused 2x2 max-pool).  q = warp of the epilogue: it holds tile pixels 32q .. 32q+31, one per lane.
 template <int TWC = 0>   // TWC: tile width known at compile time (0 = P.tw)
 __device__ __forceinline__ void tc_epilogue_cols(const TcParams& P, const float* __restrict__ s_par, const uint32_t (&r)[16],
                                                  int n0, int c0, bool valid, size_t pix, int b, int x0, int y0, int q, int lane) {
@@ -190,7 +146,7 @@ __device__ __forceinline__ void tc_epilogue_cols(const TcParams& P, const float*
     if (valid && !(P.pool_out != nullptr && P.skip_out))
       store3(reinterpret_cast<__half*>(P.out) + pix * P.out_Ctot, P.out_Ctot, P.out_coff, v);
     if (P.pool_out != nullptr) {
-      const int tw = TWC ? TWC : P.tw;
+      const int tw = TWC ? TWC : TW;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         v[j] = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
@@ -209,7 +165,7 @@ __device__ __forceinline__ void tc_epilogue_cols(const TcParams& P, const float*
     // (ty = q*(32/tw) + lane/tw, tx = lane%tw); the 2x2 partners are lane^1 (x) and lane^tw (y); lanes with
     // even tx and even ty store.  The max runs on the already rounded, packed halves: rounding is
     // monotonic, so max(round(a), round(b)) == round(max(a, b)) and this equals pooling the stored tensor.
-    const int tw = TWC ? TWC : P.tw;
+    const int tw = TWC ? TWC : TW;
     __align__(16) __half2 h[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) h[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
@@ -282,9 +238,8 @@ __device__ __forceinline__ float4 lds_f4(uint32_t saddr) {
 }
 
 // Specialised form of tc_epilogue_cols for P.epi_mode == 1.  The generic routine re-derives, for every 16
-// columns, facts that are fixed per launch (output dtype, BN, alignment, partial channel tiles): ncu's source
-// view of the 16->16 @1024^2 layer shows ~430 warp instructions per 128-pixel tile and 67 % issue-slot
-// utilisation, i.e. an instruction-issue bound epilogue.  Here the launch-invariant decisions are made on
+// columns, facts that are fixed per launch (output dtype, BN, alignment, partial channel tiles), which makes the
+// epilogue of the low-channel full-resolution layers instruction-issue bound.  Here the launch-invariant decisions are made on
 // the host, the bias comes from shared memory through ld.shared (the generic path emitted generic LDs), ReLU
 // is a branch-free max against 0 / -inf, and the output / pooled row pointers are computed once per tile.
 template <int TWC, bool POOL>
@@ -315,104 +270,67 @@ __device__ __forceinline__ void tc_epilogue_cols_fast(uint32_t s_bias, const uin
   }
 }
 
-template <int TWC, bool PIPE, bool POOL>
-__device__ __forceinline__ void tc_epilogue_acc_fast(const TcParams& P, const float* __restrict__ s_par, uint32_t taddr, int n0, bool valid,
-                                                     size_t pix, int b, int x0, int y0, int q, int lane) {
+constexpr int kConsumerThreads = 256;                 // two warpgroups: tile rows 0-63 / 64-127
+constexpr int kConvThreads = kConsumerThreads + 32;   // + the TMA producer warp
+// fp32 accumulator columns staged through shared memory per epilogue round (must divide N)
+constexpr int stage_cols(int n) { return n % 32 == 0 ? 32 : 16; }
+
+// Epilogue of 16 accumulator columns [c0, c0 + 16) of one tile pixel, read from the fp32 staging rows in shared memory
+// (`src`: this pixel's 16 staged values).  Called by whole warps (the fused max-pool shuffles across lanes): lane l of
+// warp q holds tile pixel 32 q + l.
+__device__ __forceinline__ void tc_epilogue_chunk(const TcParams& P, const float* __restrict__ s_par, const float* src, int n0, int c0,
+                                               bool valid, size_t pix, int b, int x0, int y0, int q, int lane) {
+  uint32_t r[16];
+#pragma unroll
+  for (int j4 = 0; j4 < 4; ++j4) {
+    const float4 v = reinterpret_cast<const float4*>(src)[j4];
+    r[4 * j4 + 0] = __float_as_uint(v.x); r[4 * j4 + 1] = __float_as_uint(v.y);
+    r[4 * j4 + 2] = __float_as_uint(v.z); r[4 * j4 + 3] = __float_as_uint(v.w);
+  }
+  if (P.epi_mode != 1) {
+    tc_epilogue_cols<TW>(P, s_par, r, n0, c0, valid, pix, b, x0, y0, q, lane);
+    return;
+  }
   const float lo = P.relu ? 0.f : -INFINITY;
-  const uint32_t sb = smem_u32(s_par);
-  __half* po = reinterpret_cast<__half*>(P.out) + pix * P.out_Ctot + P.out_coff + n0;
-  __half* pp = nullptr;
-  bool pool_store = false;
-  if (POOL) {
-    const int tw = TWC ? TWC : P.tw;
-    const int lr = lane / tw, lc = lane % tw;
-    pool_store = valid && ((lc | lr) & 1) == 0;
-    const int py = (y0 >> 1) + ((q * (32 / tw) + lr) >> 1), px = (x0 >> 1) + (lc >> 1);
-    pp = reinterpret_cast<__half*>(P.pool_out) + (((size_t)b * P.pool_H + py) * P.pool_W + px) * P.pool_Ctot + P.pool_coff + n0;
-  }
-  if (POOL && P.skip_out) valid = false;               // launch-uniform: only the pooled tensor is consumed
-  if constexpr (!PIPE) {
-    for (int c0 = 0; c0 < P.N; c0 += 16) {
-      uint32_t r16[16];
-      tc_ld16(taddr + (uint32_t)c0, r16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      tc_epilogue_cols_fast<TWC, POOL>(sb + 4u * c0, r16, valid, po + c0, pp + c0, pool_store, lo, P.tw);
-    }
+  __half* po = reinterpret_cast<__half*>(P.out) + pix * P.out_Ctot + P.out_coff + n0 + c0;
+  if (P.pool_out == nullptr) {
+    tc_epilogue_cols_fast<TW, false>(smem_u32(s_par + c0), r, valid, po, nullptr, false, lo, TW);
     return;
   }
-  uint32_t ra[16], rb[16];
-  tc_ld16(taddr, ra);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  for (int c0 = 0; c0 < P.N; c0 += 32) {
-    const bool has_b = c0 + 16 < P.N;
-    if (has_b) tc_ld16(taddr + (uint32_t)(c0 + 16), rb);
-    tc_epilogue_cols_fast<TWC, POOL>(sb + 4u * c0, ra, valid, po + c0, pp + c0, pool_store, lo, P.tw);
-    if (has_b) {
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const bool has_a = c0 + 32 < P.N;
-      if (has_a) tc_ld16(taddr + (uint32_t)(c0 + 32), ra);
-      tc_epilogue_cols_fast<TWC, POOL>(sb + 4u * (c0 + 16), rb, valid, po + c0 + 16, pp + c0 + 16, pool_store, lo, P.tw);
-      if (has_a) asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    }
-  }
+  const int lr = lane / TW, lc = lane % TW;
+  const bool pool_store = valid && ((lc | lr) & 1) == 0;
+  const int py = (y0 >> 1) + ((q * (32 / TW) + lr) >> 1), px = (x0 >> 1) + (lc >> 1);
+  __half* pp = reinterpret_cast<__half*>(P.pool_out) + (((size_t)b * P.pool_H + py) * P.pool_W + px) * P.pool_Ctot + P.pool_coff + n0 + c0;
+  tc_epilogue_cols_fast<TW, true>(smem_u32(s_par + c0), r, valid && !P.skip_out, po, pp, pool_store, lo, TW);
 }
 
-// Epilogue of one accumulator (P.N fp32 columns at TMEM address `taddr`), software pipelined: the
-// tcgen05.ld of chunk i+1 is in flight while chunk i is converted and stored, so the ~100-cycle
-// tcgen05.wait::ld is paid once per accumulator instead of once per 16 columns.
-// PIPE = false keeps the plain load-wait-store loop: the 16/32-input-channel kernels run 3-4 CTAs per SM and
-// the 16 extra registers of the pipelined form would cost them a resident CTA (80 -> 96 registers).
-template <int TWC, bool PIPE>
-__device__ __forceinline__ void tc_epilogue_acc(const TcParams& P, const float* __restrict__ s_par, uint32_t taddr, int n0,
-                                                bool valid, size_t pix, int b, int x0, int y0, int q, int lane) {
-  if (P.epi_mode == 1) {                               // launch-uniform
-    if (P.pool_out != nullptr) tc_epilogue_acc_fast<TWC, PIPE, true>(P, s_par, taddr, n0, valid, pix, b, x0, y0, q, lane);
-    else tc_epilogue_acc_fast<TWC, PIPE, false>(P, s_par, taddr, n0, valid, pix, b, x0, y0, q, lane);
-    return;
-  }
-  if constexpr (!PIPE) {
-    for (int c0 = 0; c0 < P.N; c0 += 16) {
-      uint32_t r16[16];
-      tc_ld16(taddr + (uint32_t)c0, r16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      tc_epilogue_cols<TWC>(P, s_par, r16, n0, c0, valid, pix, b, x0, y0, q, lane);
-    }
-    return;
-  }
-  uint32_t ra[16], rb[16];
-  tc_ld16(taddr, ra);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  for (int c0 = 0; c0 < P.N; c0 += 32) {
-    const bool has_b = c0 + 16 < P.N;                  // warp-uniform
-    if (has_b) tc_ld16(taddr + (uint32_t)(c0 + 16), rb);
-    tc_epilogue_cols<TWC>(P, s_par, ra, n0, c0, valid, pix, b, x0, y0, q, lane);
-    if (has_b) {
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      const bool has_a = c0 + 32 < P.N;
-      if (has_a) tc_ld16(taddr + (uint32_t)(c0 + 32), ra);
-      tc_epilogue_cols<TWC>(P, s_par, rb, n0, c0 + 16, valid, pix, b, x0, y0, q, lane);
-      if (has_a) asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    }
-  }
-}
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 
-template <int KSTEPS, int MAXG = 3>   // MAXG: unroll bound of the filter-column / filter-row loops (3: 1x1 and 3x3, 7: 5x5 and 7x7)
-__global__ void __launch_bounds__(128) k_conv_tc(const __grid_constant__ CUtensorMap mapA,
-                                                 const __grid_constant__ CUtensorMap mapB,
-                                                 const __grid_constant__ TcParams P) {
+// Implicit-GEMM convolution on wgmma.  One CTA = one 16x8-pixel output tile x one N tile of output channels:
+//   warp 8, lane 0: TMA producer -- per (input-channel chunk, filter column) one activation box into the A ring, per filter
+//     tap one [N x KC] weight slice into the B ring (mbarrier full / empty pairs);
+//   warps 0-7 (two warpgroups): warpgroup w multiplies tile rows [64 w, 64 w + 64) -- m64nNk16 wgmma, fp32 accumulators in
+//     registers; a step's slots are released once the NEXT step's wgmma group has been issued and the step's own has
+//     completed (wgmma.wait_group 1), so the tensor cores always have one group queued;
+//   epilogue: accumulators -> shared-memory staging, CW columns at a time -> one pixel per thread, 16 columns per call
+//     (bias / ReLU / BN / fused max-pool / split planes, as the scalar kernels do).
+template <int KSTEPS, int N>
+__global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg(const __grid_constant__ CUtensorMap mapA,
+                                                             const __grid_constant__ CUtensorMap mapB,
+                                                             const __grid_constant__ TcParams P) {
+  constexpr int CW = stage_cols(N), SP = CW + 4;   // staged columns per round, staging row pitch (floats)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve shared memory (ring slots are 1024-aligned: required by the 128B swizzle atoms)
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* a_ring = base;
   uint8_t* b_ring = a_ring + (size_t)P.n_a_slots * P.a_slot_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(b_ring + (size_t)P.n_b_slots * P.b_slot_bytes);
+  float* s_stage = reinterpret_cast<float*>(b_ring + (size_t)P.n_b_slots * P.b_slot_bytes);   // [128][SP]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + 128 * SP);
   uint64_t* fullA = bars;
   uint64_t* emptyA = fullA + P.n_a_slots;
   uint64_t* fullB = emptyA + P.n_a_slots;
   uint64_t* emptyB = fullB + P.n_b_slots;
-  uint64_t* accum = emptyB + P.n_b_slots;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum + 1);
-  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 1) + 15) & ~(uintptr_t)15);
+  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(emptyB + P.n_b_slots) + 15) & ~(uintptr_t)15);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x;
@@ -422,860 +340,105 @@ __global__ void __launch_bounds__(128) k_conv_tc(const __grid_constant__ CUtenso
   stage_params(P, s_par, n0);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), 1); }
-    for (int i = 0; i < P.n_b_slots; ++i) { mbar_init(smem_u32(fullB + i), 1); mbar_init(smem_u32(emptyB + i), 1); }
-    mbar_init(smem_u32(accum), 1);
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), kConsumerThreads / 32); }
+    for (int i = 0; i < P.n_b_slots; ++i) { mbar_init(smem_u32(fullB + i), 1); mbar_init(smem_u32(emptyB + i), kConsumerThreads / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   if (P.pdl_trigger) griddep_launch();
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerThreads / 32) {
     // ------------------------------ TMA producer ------------------------------
-    griddep_wait();                    // activations come from the previous kernel of the stream
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
-    for (int ch = 0; ch < P.n_chunks; ++ch) {
-      for (int g = 0; g < P.n_groups; ++g) {
-        mbar_wait(smem_u32(emptyA + sa), pha ^ 1, 1);
-        mbar_expect_tx(smem_u32(fullA + sa), (uint32_t)P.a_tx_bytes);
-        tma_load_4d(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, smem_u32(fullA + sa), ch * P.KC,
-                    x0 + P.groups[g].dx, y0 + P.dy0, b);
-        for (int t = 0; t < P.groups[g].n_taps; ++t) {
-          mbar_wait(smem_u32(emptyB + sb), phb ^ 1, 2);
-          mbar_expect_tx(smem_u32(fullB + sb), (uint32_t)P.b_tx_bytes);
-          tma_load_3d(smem_u32(b_ring + (size_t)sb * P.b_slot_bytes), &mapB, smem_u32(fullB + sb), ch * P.KC, n0,
-                      P.groups[g].taps[t].w_tap);
-          if (++sb == P.n_b_slots) { sb = 0; phb ^= 1; }
-        }
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    // The whole warp walks the loop (all values are warp-uniform, so descriptors live in uniform
-    // registers); only lane 0 issues tcgen05.mma / tcgen05.commit.
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
-    const uint64_t desc_hi = make_desc(0, P.row_bytes, P.layout_type);
-    for (int ch = 0; ch < P.n_chunks; ++ch) {
-#pragma unroll
-      for (int g = 0; g < MAXG; ++g) {
-        if (g >= P.n_groups) break;
-        mbar_wait(smem_u32(fullA + sa), pha, 3);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_base = smem_u32(a_ring + (size_t)sa * P.a_slot_bytes);
-#pragma unroll
-        for (int t = 0; t < MAXG; ++t) {
-          if (t >= P.groups[g].n_taps) break;
-          mbar_wait(smem_u32(fullB + sb), phb, 4);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t b_base = smem_u32(b_ring + (size_t)sb * P.b_slot_bytes);
-          const uint64_t da = desc_hi + (uint64_t)((a_base + (uint32_t)(P.groups[g].taps[t].row_off * TW * P.row_bytes)) >> 4);
-          const uint64_t db = desc_hi + (uint64_t)(b_base >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < KSTEPS; ++k)
-              tc_mma_f16(tmem_base, da + 2 * k, db + 2 * k, P.idesc, (ch | g | t | k) ? 1u : 0u);
-            tc_commit(smem_u32(emptyB + sb));
-          }
-          __syncwarp();
-          if (++sb == P.n_b_slots) { sb = 0; phb ^= 1; }
-        }
-        if (elect_one()) tc_commit(smem_u32(emptyA + sa));
-        __syncwarp();
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-      }
-    }
-    if (elect_one()) tc_commit(smem_u32(accum));
-  }
-  __syncwarp();
-
-  // ------------------------------ epilogue (all 4 warps) ----------------------
-  mbar_wait(smem_u32(accum), 0, 5);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const int m = warp * 32 + lane;                     // accumulator row = TMEM lane
-  const int iy = y0 + m / TW, ix = x0 + m % TW;
-  const bool valid = (iy < P.H) && (ix < P.W);
-  const int oy = iy * P.oy_mul + P.oy_add, ox = ix * P.ox_mul + P.ox_add;
-  const size_t pix = ((size_t)b * P.out_H + oy) * P.out_W + ox;
-  tc_epilogue_acc<16, KSTEPS == 4>(P, s_par, tmem_base + ((uint32_t)(warp * 32) << 16), n0, valid, pix, b, x0, y0, warp, lane);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
-  }
-}
-
-
-// ---- thread-block cluster helpers (weight slices multicast to the CTAs of a cluster: k_conv_tc_prog<KSTEPS, 2>) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(mask) : "memory");
-}
-// ---- CTA-pair helpers (cta_group::2: one M = 256 MMA over the two CTAs of a cluster; k_conv_tc_prog<KSTEPS, 2, 2>) ----
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {    // shared::cta address -> the same offset in CTA `rank`
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-// TMA loads of a CTA pair: the data lands in the executing CTA, the bytes are counted on the LEADER's barrier
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_pair(uint32_t dst, const CUtensorMap* map, uint32_t bar_cluster, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar) {      // one arrival on the barrier at this offset in BOTH CTAs
-  const uint16_t mask = 3;
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
-
-
-// Persistent, warp-specialised variant for layers whose whole filter bank fits in shared memory:
-// each CTA loads the weights once, then walks output tiles; warp 0 = TMA producer (activation
-// halo tiles), warp 1 = MMA issuer, warps 2..5 = epilogue.  Two TMEM accumulator stages let the
-// epilogue of tile i overlap the MMAs of tile i+1 and the TMA loads of tile i+2.
-template <int KSTEPS>
-__global__ void __launch_bounds__(192) k_conv_tc_persist(const __grid_constant__ CUtensorMap mapA,
-                                                         const __grid_constant__ CUtensorMap mapB,
-                                                         const __grid_constant__ TcParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int n_wslots = P.n_chunks * P.n_used_taps;
-  uint8_t* w_res = base;
-  uint8_t* a_ring = w_res + (size_t)n_wslots * P.w_slot_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_ring + (size_t)P.n_a_slots * P.a_slot_bytes);
-  uint64_t* fullA = bars;
-  uint64_t* emptyA = fullA + P.n_a_slots;
-  uint64_t* tfull = emptyA + P.n_a_slots;     // [n_stages]
-  uint64_t* tempty = tfull + P.n_stages;      // [n_stages]
-  uint64_t* wbar = tempty + P.n_stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
-  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 1) + 15) & ~(uintptr_t)15);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  stage_params(P, s_par, 0);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), 1); }
-    for (int i = 0; i < P.n_stages; ++i) { mbar_init(smem_u32(tfull + i), 1); mbar_init(smem_u32(tempty + i), 4); }
-    mbar_init(smem_u32(wbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (P.pdl_trigger) griddep_launch();
-  if (warp == 0 && lane == 0) {
-    // ------------------------------ TMA producer ------------------------------
-    mbar_expect_tx(smem_u32(wbar), (uint32_t)(n_wslots * P.b_tx_bytes));
-    for (int ch = 0; ch < P.n_chunks; ++ch)
-      for (int u = 0; u < P.n_used_taps; ++u)
-        tma_load_3d(smem_u32(w_res + (size_t)(ch * P.n_used_taps + u) * P.w_slot_bytes), &mapB, smem_u32(wbar), ch * P.KC, 0,
-                    P.used_taps[u]);
-    griddep_wait();                    // the filter bank above does not depend on the previous kernel; the activations do
-    int sa = 0;
-    uint32_t pha = 0;
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x) {
-      const int b = t / P.tiles_per_img, r = t - b * P.tiles_per_img;
-      const int y0 = (r / P.tiles_x) * TH, x0 = (r % P.tiles_x) * TW;
-      for (int ch = 0; ch < P.n_chunks; ++ch)
+    if (lane == 0) {
+      griddep_wait();                  // activations come from the previous kernel of the stream
+      int sa = 0, sb = 0;
+      uint32_t pha = 0, phb = 0;
+      for (int ch = 0; ch < P.n_chunks; ++ch) {
         for (int g = 0; g < P.n_groups; ++g) {
-          mbar_wait(smem_u32(emptyA + sa), pha ^ 1, 11);
+          mbar_wait(smem_u32(emptyA + sa), pha ^ 1);
           mbar_expect_tx(smem_u32(fullA + sa), (uint32_t)P.a_tx_bytes);
           tma_load_4d(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, smem_u32(fullA + sa), ch * P.KC,
                       x0 + P.groups[g].dx, y0 + P.dy0, b);
-          if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-        }
-    }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    // warp-uniform loop (descriptors in uniform registers); lane 0 issues the tcgen05 instructions
-    mbar_wait(smem_u32(wbar), 0, 12);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    int sa = 0, stage = 0;
-    uint32_t pha = 0, eph = 0;
-    const uint64_t desc_hi = make_desc(0, P.row_bytes, P.layout_type);
-    const uint32_t w_base = smem_u32(w_res);
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x) {
-      mbar_wait(smem_u32(tempty + stage), eph ^ 1, 13);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d_tmem = tmem_base + (uint32_t)(stage * P.N);
-      for (int ch = 0; ch < P.n_chunks; ++ch) {
-#pragma unroll
-        for (int g = 0; g < 3; ++g) {
-          if (g >= P.n_groups) break;
-          mbar_wait(smem_u32(fullA + sa), pha, 14);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a_base = smem_u32(a_ring + (size_t)sa * P.a_slot_bytes);
-#pragma unroll
-          for (int tp = 0; tp < 3; ++tp) {
-            if (tp >= P.groups[g].n_taps) break;
-            const int slot = ch * P.n_used_taps + P.slot_of_tap[P.groups[g].taps[tp].w_tap];
-            const uint64_t da = desc_hi + (uint64_t)((a_base + (uint32_t)(P.groups[g].taps[tp].row_off * TW * P.row_bytes)) >> 4);
-            const uint64_t db = desc_hi + (uint64_t)((w_base + (uint32_t)(slot * P.w_slot_bytes)) >> 4);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < KSTEPS; ++k)
-                tc_mma_f16(d_tmem, da + 2 * k, db + 2 * k, P.idesc, (ch | g | tp | k) ? 1u : 0u);
-            }
-            __syncwarp();
+          for (int t = 0; t < P.groups[g].n_taps; ++t) {
+            mbar_wait(smem_u32(emptyB + sb), phb ^ 1);
+            mbar_expect_tx(smem_u32(fullB + sb), (uint32_t)P.b_tx_bytes);
+            tma_load_3d(smem_u32(b_ring + (size_t)sb * P.b_slot_bytes), &mapB, smem_u32(fullB + sb), ch * P.KC, n0,
+                        P.groups[g].taps[t].w_tap);
+            if (++sb == P.n_b_slots) { sb = 0; phb ^= 1; }
           }
-          if (elect_one()) tc_commit(smem_u32(emptyA + sa));
-          __syncwarp();
           if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
         }
       }
-      if (elect_one()) tc_commit(smem_u32(tfull + stage));
-      __syncwarp();
-      if (++stage == P.n_stages) { stage = 0; eph ^= 1; }
     }
-  } else if (warp >= 2) {
-    // ------------------------------ epilogue warps ----------------------------
-    const int q = warp & 3;                       // TMEM lane quadrant this warp may access
-    int stage = 0;
-    uint32_t fph = 0;
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x) {
-      const int b = t / P.tiles_per_img, r = t - b * P.tiles_per_img;
-      const int y0 = (r / P.tiles_x) * TH, x0 = (r % P.tiles_x) * TW;
-      mbar_wait(smem_u32(tfull + stage), fph, 15);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int m = q * 32 + lane;
-      const int iy = y0 + m / TW, ix = x0 + m % TW;
-      const bool valid = (iy < P.H) && (ix < P.W);
-      const size_t pix = ((size_t)b * P.out_H + (iy * P.oy_mul + P.oy_add)) * P.out_W + (ix * P.ox_mul + P.ox_add);
-      tc_epilogue_acc<16, KSTEPS == 4>(P, s_par, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(stage * P.N), 0, valid, pix, b, x0, y0, q, lane);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(tempty + stage));
-      if (++stage == P.n_stages) { stage = 0; fph ^= 1; }
-    }
+    return;
   }
-  __syncwarp();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
-  }
-}
 
-
-
-// Walks the tiles t = first, first + stride, ... of a (batch, tiles_y, tiles_x) grid without
-// integer divisions in the loop (each role warp of the persistent kernels keeps one of these).
-struct TileIter {
-  int b, ty, tx;            // current tile
-  int sb, sy, sx;           // stride decomposed into (batch, tile row, tile col) steps
-  int tiles_x, tiles_y;
-  __device__ __forceinline__ void init(int first, int stride, int tx_n, int ty_n) {
-    tiles_x = tx_n; tiles_y = ty_n;
-    const int per = tx_n * ty_n;
-    b = first / per; int r = first - b * per; ty = r / tx_n; tx = r - ty * tx_n;
-    sb = stride / per; r = stride - sb * per; sy = r / tx_n; sx = r - sy * tx_n;
-  }
-  __device__ __forceinline__ void next() {
-    tx += sx;
-    if (tx >= tiles_x) { tx -= tiles_x; ++ty; }
-    ty += sy;
-    if (ty >= tiles_y) { ty -= tiles_y; ++b; }
-    b += sb;
-  }
-};
-
-// K-major swizzled descriptor whose start address is NOT aligned to the swizzle repeat (8 rows):
-// the matrix base offset field (bits [49,52)) carries the phase (address >> 7) & 7.
-__device__ __forceinline__ uint64_t make_desc_unaligned(uint32_t saddr, int sbo_bytes, int layout_type, int use_base_offset) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  if (use_base_offset) d |= (uint64_t)((saddr >> 7) & 7) << 49;
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-
-// Halo variant of the persistent kernel: output tile 8 px wide x 16 rows (one 8-row swizzle group
-// per tile row), ONE TMA load of the [KC, 10, 18] halo tile per input-channel chunk; the nine
-// taps are pure start-address offsets ((ky*10 + kx) rows) with stride-byte-offset = 10 rows.
-// Cuts the L2->SM traffic of the activation operand from 3.75x to 1.4x of the tile.
-template <int KSTEPS>
-__global__ void __launch_bounds__(192) k_conv_tc_halo(const __grid_constant__ CUtensorMap mapA,
-                                                      const __grid_constant__ CUtensorMap mapB,
-                                                      const __grid_constant__ TcParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int n_wslots = P.n_chunks * P.n_used_taps;
-  uint8_t* w_res = base;
-  uint8_t* a_ring = w_res + (size_t)n_wslots * P.w_slot_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_ring + (size_t)P.n_a_slots * P.a_slot_bytes);
-  uint64_t* fullA = bars;
-  uint64_t* emptyA = fullA + P.n_a_slots;
-  uint64_t* tfull = emptyA + P.n_a_slots;
-  uint64_t* tempty = tfull + P.n_stages;
-  uint64_t* wbar = tempty + P.n_stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
-  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 1) + 15) & ~(uintptr_t)15);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int TWH = 8, THH = 16, PITCH = TWH + 2;
-  stage_params(P, s_par, 0);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), 1); }
-    for (int i = 0; i < P.n_stages; ++i) { mbar_init(smem_u32(tfull + i), 1); mbar_init(smem_u32(tempty + i), 4); }
-    mbar_init(smem_u32(wbar), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (P.pdl_trigger) griddep_launch();
-  if (warp == 0 && lane == 0) {
-    mbar_expect_tx(smem_u32(wbar), (uint32_t)(n_wslots * P.b_tx_bytes));
-    for (int ch = 0; ch < P.n_chunks; ++ch)
-      for (int u = 0; u < P.n_used_taps; ++u)
-        tma_load_3d(smem_u32(w_res + (size_t)(ch * P.n_used_taps + u) * P.w_slot_bytes), &mapB, smem_u32(wbar), ch * P.KC, 0,
-                    P.used_taps[u]);
-    griddep_wait();
-    int sa = 0;
-    uint32_t pha = 0;
-    TileIter it;
-    it.init(blockIdx.x, gridDim.x, P.tiles_x, P.tiles_per_img / P.tiles_x);
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x, it.next()) {
-      const int b = it.b, y0 = it.ty * THH, x0 = it.tx * TWH;
-      for (int ch = 0; ch < P.n_chunks; ++ch) {
-        mbar_wait(smem_u32(emptyA + sa), pha ^ 1, 21);
-        if (P.ablate & 1) { mbar_arrive(smem_u32(fullA + sa)); }
-        else {
-          mbar_expect_tx(smem_u32(fullA + sa), (uint32_t)P.a_tx_bytes);
-          tma_load_4d(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, smem_u32(fullA + sa), ch * P.KC, x0 + P.dx0,
-                      y0 + P.dy0, b);
+  // ------------------------------ MMA (two warpgroups) ------------------------
+  const int wg = warp >> 2;
+  float acc[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  const uint64_t desc_hi = make_desc(0, P.row_bytes, P.layout_type);
+  const uint32_t a_row0 = (uint32_t)(wg * 64 * P.row_bytes);
+  int sa = 0, sb = 0, rel_a = -1, rel_b = -1;
+  uint32_t pha = 0, phb = 0, scale_d = 0;
+  for (int ch = 0; ch < P.n_chunks; ++ch) {
+    for (int g = 0; g < P.n_groups; ++g) {
+      mbar_wait(smem_u32(fullA + sa), pha);
+      const uint32_t a_base = smem_u32(a_ring + (size_t)sa * P.a_slot_bytes) + a_row0;
+      const int n_taps = P.groups[g].n_taps;
+      for (int t = 0; t < n_taps; ++t) {
+        mbar_wait(smem_u32(fullB + sb), phb);
+        const uint64_t da = desc_hi + (uint64_t)((a_base + (uint32_t)(P.groups[g].taps[t].row_off * TW * P.row_bytes)) >> 4);
+        const uint64_t db = desc_hi + (uint64_t)(smem_u32(b_ring + (size_t)sb * P.b_slot_bytes) >> 4);
+        wgmma_fence();
+        wgmma_reg_fence(acc);
+#pragma unroll
+        for (int k = 0; k < KSTEPS; ++k) {
+          wgmma_f16<N>(acc, da + 2 * k, db + 2 * k, scale_d);
+          scale_d = 1;
         }
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    mbar_wait(smem_u32(wbar), 0, 22);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    int sa = 0, stage = 0;
-    uint32_t pha = 0, eph = 0;
-    const uint32_t w_base = smem_u32(w_res);
-    const int sbo = PITCH * P.row_bytes;
-    // per-tap constants, computed once per CTA (fully unrolled -> registers)
-    const uint64_t desca_hi = make_desc_unaligned(0, sbo, P.layout_type, 0);
-    uint32_t tap_aoff[9];      // (start-address offset of the tap inside the halo tile) >> 4
-    uint64_t tap_db[9];        // B descriptor of the tap for chunk 0
-#pragma unroll
-    for (int tp = 0; tp < 9; ++tp) {
-      const int tq = tp < P.n_htaps ? tp : 0;
-      tap_aoff[tp] = (uint32_t)(P.htap_off_rows[tq] * P.row_bytes) >> 4;
-      tap_db[tp] = make_desc(w_base + (uint32_t)(P.slot_of_tap[P.htap_w[tq]] * P.w_slot_bytes), P.row_bytes, P.layout_type);
-    }
-    const uint32_t chunk_db_step = (uint32_t)(P.n_used_taps * P.w_slot_bytes) >> 4;
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x) {
-      mbar_wait(smem_u32(tempty + stage), eph ^ 1, 23);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d_tmem = tmem_base + (uint32_t)(stage * P.N);
-      for (int ch = 0; ch < P.n_chunks; ++ch) {
-        mbar_wait(smem_u32(fullA + sa), pha, 24);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t da0 = desca_hi + (uint64_t)(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes) >> 4);
-        const uint32_t dbo = (uint32_t)ch * chunk_db_step;
-        if (elect_one()) {
-#pragma unroll
-          for (int tp = 0; tp < 9; ++tp) {
-            if (tp < P.n_htaps && !(P.ablate & 2)) {
-              const uint64_t da = da0 + tap_aoff[tp];
-              const uint64_t db = tap_db[tp] + dbo;
-#pragma unroll
-              for (int k = 0; k < KSTEPS; ++k)
-                tc_mma_f16(d_tmem, da + 2 * k, db + 2 * k, P.idesc, (ch | tp | k) ? 1u : 0u);
-            }
-          }
-          tc_commit(smem_u32(emptyA + sa));
-        }
+        wgmma_commit();
+        wgmma_reg_fence(acc);
+        wgmma_wait<1>();               // the previous step's products are done: its slots may be refilled
         __syncwarp();
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-      }
-      if (elect_one()) tc_commit(smem_u32(tfull + stage));
-      __syncwarp();
-      if (++stage == P.n_stages) { stage = 0; eph ^= 1; }
-    }
-  } else if (warp >= 2) {
-    const int q = warp & 3;
-    int stage = 0;
-    uint32_t fph = 0;
-    TileIter it;
-    it.init(blockIdx.x, gridDim.x, P.tiles_x, P.tiles_per_img / P.tiles_x);
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x, it.next()) {
-      const int b = it.b, y0 = it.ty * THH, x0 = it.tx * TWH;
-      mbar_wait(smem_u32(tfull + stage), fph, 25);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int m = q * 32 + lane;
-      const int iy = y0 + (m >> 3), ix = x0 + (m & 7);
-      const bool valid = (iy < P.H) && (ix < P.W);
-      const size_t pix = ((size_t)b * P.out_H + (iy * P.oy_mul + P.oy_add)) * P.out_W + (ix * P.ox_mul + P.ox_add);
-      if (P.ablate & 8) {                              // profiling only: epilogue without TMEM loads
-        for (int c0 = 0; c0 < P.N; c0 += 16) {
-          uint32_t r16[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) r16[j] = (uint32_t)(lane + j);
-          tc_epilogue_cols<8>(P, s_par, r16, 0, c0, valid && !(P.ablate & 4), pix, b, x0, y0, q, lane);
+        if (lane == 0) {
+          if (rel_b >= 0) mbar_arrive(smem_u32(emptyB + rel_b));
+          if (rel_a >= 0) mbar_arrive(smem_u32(emptyA + rel_a));
         }
-      } else {
-        tc_epilogue_acc<8, KSTEPS == 4>(P, s_par, tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(stage * P.N), 0, valid && !(P.ablate & 4), pix,
-                           b, x0, y0, q, lane);
+        rel_b = sb;
+        rel_a = t == n_taps - 1 ? sa : -1;
+        if (++sb == P.n_b_slots) { sb = 0; phb ^= 1; }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(tempty + stage));
-      if (++stage == P.n_stages) { stage = 0; fph ^= 1; }
+      if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
     }
   }
-  __syncwarp();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
-  }
-}
+  wgmma_wait<0>();
+  wgmma_reg_fence(acc);
 
-// Warp-uniform copy of a value (the compiler keeps the result in a uniform register, which is where
-// tcgen05.mma wants its descriptors: no per-instruction R2UR traffic in the single issuing thread).
-__device__ __forceinline__ uint32_t uni(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-
-// "Programmed" halo kernel: one staged halo box [KC, pitch, box_h] per input-channel chunk feeds up
-// to four TMEM accumulators per stage.  The accumulators are either the 8x16-pixel sub-tiles of a
-// super-tile (one barrier round trip and one weight slice for 256/512 pixels) or the four sub-pixel
-// phases of a stride-2 transposed convolution (the whole Conv2DTranspose in ONE launch; every phase
-// reads the same staged activations).  The MMA sequence is a table in the kernel parameters
-// (TcProgEntry: activation start offset, weight slice, accumulator); the filter bank is either
-// resident in shared memory or streamed slice by slice through a ring (w_stream), in which case a
-// slice is consumed by all program entries that use it before the slot is released.
-// CS = 2: the launch is made of clusters of two CTAs (neighbouring tiles of one sweep) that consume the SAME sequence of
-// weight slices: each CTA fetches half of every [N x KC] slice and TMA-multicasts it into the same ring slot of both, so the
-// L2 -> SM weight traffic per output pixel halves (round 1: the >= 128-channel layers and the transposed convs sat on the
-// L2 read bandwidth, 10-28x read amplification, 37-57 % tensor-active).  A ring slot is refilled only when BOTH CTAs'
-// MMAs have consumed it (tcgen05.commit multicast to both empty barriers); every CTA walks the same number of tiles
-// (the host only launches this form when tiles % grid == 0).
-// CG = 2 (with CS = 2): the two CTAs form a cta_group::2 PAIR.  Every MMA is M = 256: the leader (cluster rank 0) issues
-// tcgen05.mma.cta_group::2 over both CTAs' staged activation boxes (128 pixels each, at the same shared-memory offsets) and
-// a weight slice of which each CTA holds N/2 rows; each CTA's TMEM receives the accumulators of its own pixels and its own
-// epilogue warps drain them.  What it buys (tools/probes/mma_probe.cu, DESIGN.md 7): an SM's shared memory serves the TMA
-// fills AND the operand reads of the tensor core; with streamed weights a CTA writes N x KC x 2 bytes per slice that it
-// reads back once per sub-tile -- the pair writes only half a slice per CTA, and reads half of B per MMA.
-//   barriers: all TMA loads of both CTAs count on the LEADER's full barriers (.cta_group::2 loads); the leader's commits
-//   are multicast to both CTAs' empty / accumulator-full barriers; both CTAs' epilogue warps arrive on the leader's
-//   accumulator-empty barrier (the peer remotely).
-template <int KSTEPS, int CS = 1, int CG = 1>
-__global__ void __launch_bounds__(320) k_conv_tc_prog(const __grid_constant__ CUtensorMap mapA,
-                                                      const __grid_constant__ CUtensorMap mapB,
-                                                      const __grid_constant__ TcParams P) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const bool w_stream = P.w_stream != 0;
-  const int n_wslots = w_stream ? P.n_w_ring : P.n_chunks * P.n_used_taps;
-  uint8_t* w_res = base;
-  uint8_t* a_ring = w_res + (size_t)n_wslots * P.w_slot_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(a_ring + (size_t)P.n_a_slots * P.a_slot_bytes);
-  uint64_t* fullA = bars;
-  uint64_t* emptyA = fullA + P.n_a_slots;
-  uint64_t* tfull = emptyA + P.n_a_slots;
-  uint64_t* tempty = tfull + P.n_stages;
-  uint64_t* wbar = tempty + P.n_stages;
-  uint64_t* fullW = wbar + 1;          // [8] (streamed-weights mode only)
-  uint64_t* emptyW = fullW + 8;        // [8]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(emptyW + 8);
-  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 1) + 15) & ~(uintptr_t)15);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int TWH = 8 * P.sub_x, THH = 16 * P.sub_y;
-  constexpr bool PAIR = CG == 2;
-  static_assert(!PAIR || CS == 2, "a cta_group::2 pair is a cluster of two");
-  stage_params(P, s_par, 0);
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), 1); }
-    // pair: the leader's accumulator-empty barrier collects the epilogue warps of both CTAs; a slot's empty barrier gets
-    // ONE multicast commit (the leader's) instead of one per CTA
-    for (int i = 0; i < P.n_stages; ++i) { mbar_init(smem_u32(tfull + i), 1); mbar_init(smem_u32(tempty + i), 4 * P.epi_groups * CG); }
-    mbar_init(smem_u32(wbar), 1);
-    for (int i = 0; i < 8; ++i) { mbar_init(smem_u32(fullW + i), 1); mbar_init(smem_u32(emptyW + i), PAIR ? 1 : CS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
-  }
-  if (warp == 0) {
-    if constexpr (PAIR) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if constexpr (CS > 1) cluster_sync_all();          // every CTA's barriers exist before a peer signals them
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t crank = CS > 1 ? cluster_ctarank() : 0u;
-  constexpr uint16_t kMask = (uint16_t)((1u << CS) - 1u);
-  const uint32_t piece_bytes = (uint32_t)(P.b_tx_bytes / CS);
-
-  if (P.pdl_trigger) griddep_launch();
-  if (warp == 0 && lane == 0) {
-    if (!w_stream) {
-      if constexpr (PAIR) {
-        // resident filter bank split over the pair: each CTA keeps N/2 rows of every (chunk, tap) slice (half the shared
-        // memory -> a deeper activation ring); all loads are counted on the leader's barrier, whose MMA warp waits for it
-        if (crank == 0) mbar_expect_tx(smem_u32(wbar), (uint32_t)(n_wslots * P.b_tx_bytes));
-        for (int ch = 0; ch < P.n_chunks; ++ch)
-          for (int u = 0; u < P.n_used_taps; ++u)
-            tma_load_3d_pair(smem_u32(w_res + (size_t)(ch * P.n_used_taps + u) * P.w_slot_bytes), &mapB, mapa_rank(smem_u32(wbar), 0), ch * P.KC,
-                             (int)crank * (P.N / 2), P.used_taps[u]);
-      } else {
-        mbar_expect_tx(smem_u32(wbar), (uint32_t)(n_wslots * P.b_tx_bytes));
-        for (int ch = 0; ch < P.n_chunks; ++ch)
-          for (int u = 0; u < P.n_used_taps; ++u)
-            tma_load_3d(smem_u32(w_res + (size_t)(ch * P.n_used_taps + u) * P.w_slot_bytes), &mapB, smem_u32(wbar), ch * P.KC, 0,
-                        P.used_taps[u]);
-      }
-    }
-    griddep_wait();                    // resident filter bank (if any) is already in flight; activations need the previous kernel
-    int sa = 0, sw = 0;
-    uint32_t pha = 0, phw = 0;
-    TileIter it;
-    it.init(blockIdx.x, gridDim.x, P.tiles_x, P.tiles_per_img / P.tiles_x);
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x, it.next()) {
-      const int b = it.b, y0 = it.ty * THH, x0 = it.tx * TWH;
-      for (int ch = 0; ch < P.n_chunks; ++ch) {
-        mbar_wait(smem_u32(emptyA + sa), pha ^ 1, 21);
-        if (P.ablate & 1) { mbar_arrive(smem_u32(fullA + sa)); }
-        else {
-          if constexpr (PAIR) {      // both CTAs' boxes are counted on the leader's barrier
-            if (crank == 0) mbar_expect_tx(smem_u32(fullA + sa), 2u * (uint32_t)P.a_tx_bytes);
-            tma_load_4d_pair(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, mapa_rank(smem_u32(fullA + sa), 0), ch * P.KC,
-                             x0 + P.dx0, y0 + P.dy0, b);
-          } else {
-            mbar_expect_tx(smem_u32(fullA + sa), (uint32_t)P.a_tx_bytes);
-            tma_load_4d(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, smem_u32(fullA + sa), ch * P.KC, x0 + P.dx0,
-                        y0 + P.dy0, b);
-          }
-        }
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-        if (w_stream) {
-          for (int i = 0; i < P.n_prog;) {              // same order as the MMA warp consumes the slices
-            const uint32_t ew = P.prog[i].w_flags;
-            mbar_wait(smem_u32(emptyW + sw), phw ^ 1, 26);                 // CS > 1: all CTAs of the cluster are done with this slot
-            if (!PAIR || crank == 0) mbar_expect_tx(smem_u32(fullW + sw), (uint32_t)P.b_tx_bytes);
-            if constexpr (PAIR)                                            // this CTA's N/2 rows of the slice, into its own (half-size) slot
-              tma_load_3d_pair(smem_u32(w_res + (size_t)sw * P.w_slot_bytes), &mapB, mapa_rank(smem_u32(fullW + sw), 0), ch * P.KC,
-                               (int)crank * (P.N / 2), (int)((ew >> 26) & 15));
-            else if constexpr (CS > 1)                                     // this CTA's 1/CS of the slice, into every CTA of the cluster
-              tma_load_3d_mc(smem_u32(w_res + (size_t)sw * P.w_slot_bytes) + crank * piece_bytes, &mapB, smem_u32(fullW + sw), ch * P.KC,
-                             (int)crank * (P.N / CS), (int)((ew >> 26) & 15), kMask);
-            else
-              tma_load_3d(smem_u32(w_res + (size_t)sw * P.w_slot_bytes), &mapB, smem_u32(fullW + sw), ch * P.KC, 0, (int)((ew >> 26) & 15));
-            if (++sw == P.n_w_ring) { sw = 0; phw ^= 1; }
-            i += (int)((ew >> 20) & 63);
-          }
-        }
-      }
-    }
-  } else if (warp == 1 && (!PAIR || crank == 0)) {
-    if (!w_stream) mbar_wait(smem_u32(wbar), 0, 22);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    int sa = 0, stage = 0, sw = 0;
-    uint32_t pha = 0, eph = 0, phw = 0;
-    // descriptor templates (everything but the 14-bit start address); all operands below are warp-uniform
-    const uint64_t desca_t = make_desc_unaligned(0, P.pitch * P.row_bytes, P.layout_type, 0);
-    const uint64_t descb_t = make_desc(0, P.row_bytes, P.layout_type);
-    const uint32_t desca_lo = (uint32_t)desca_t, desca_hi = (uint32_t)(desca_t >> 32);
-    const uint32_t descb_lo = (uint32_t)descb_t, descb_hi = (uint32_t)(descb_t >> 32);
-    const uint32_t a_base16 = uni(smem_u32(a_ring) >> 4), w_base16 = uni(smem_u32(w_res) >> 4);
-    const uint32_t a_slot16 = (uint32_t)P.a_slot_bytes >> 4, w_slot16 = (uint32_t)P.w_slot_bytes >> 4;
-    const uint32_t tm0 = uni(tmem_base);
-    const int n_acc_cols = P.n_acc * P.N;
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x) {
-      mbar_wait(smem_u32(tempty + stage), eph ^ 1, 23);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t d0 = tm0 + (uint32_t)(stage * n_acc_cols);
-      for (int ch = 0; ch < P.n_chunks; ++ch) {
-        mbar_wait(smem_u32(fullA + sa), pha, 24);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_lo0 = desca_lo + uni(a_base16 + (uint32_t)sa * a_slot16);
-        const uint32_t b_lo0 = descb_lo + w_base16 + (uint32_t)(ch * P.n_used_taps) * w_slot16;
-        // entries [i, i + n_same) use one weight slice: a single elected region issues all their MMAs
-        for (int i = 0; i < P.n_prog;) {
-          const int n_same = w_stream ? (int)((P.prog[i].w_flags >> 20) & 63) : P.n_prog;
-          uint32_t b_ring = 0;
-          if (w_stream) {
-            mbar_wait(smem_u32(fullW + sw), phw, 27);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            b_ring = descb_lo + w_base16 + uni((uint32_t)sw) * w_slot16;
-          }
-          if (elect_one()) {
-            if (!(P.ablate & 2)) {
-#pragma unroll 1
-              for (int e = i; e < i + n_same; ++e) {
-                const uint32_t ea = P.prog[e].a_acc, ew = P.prog[e].w_flags;
-                const uint32_t a_lo = a_lo0 + (ea & 0xffffu);
-                const uint32_t b_lo = w_stream ? b_ring : b_lo0 + (ew & 0xffffu);
-                const uint32_t dt = d0 + (ea >> 16);
-                const uint32_t accf = (uint32_t)ch | (((ew >> 16) & 1u) ^ 1u);
+  // ------------------------------ epilogue (all 256 consumer threads) ----------
+  // fragment rows of this thread: 16 (warp % 4) + lane / 4 (+ 8) of its warpgroup's 64; columns 8 j + 2 (lane % 4) (+ 1)
+  const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+  // staging readers: pixel m = threadIdx.x % 128 (warp q = m / 32 as the fused pool expects), column half threadIdx.x / 128
+  const int m = threadIdx.x & 127, half = threadIdx.x >> 7;
+  const int iy = y0 + m / TW, ix = x0 + m % TW;
+  const bool valid = (iy < P.H) && (ix < P.W);
+  const size_t pix = ((size_t)b * P.out_H + (iy * P.oy_mul + P.oy_add)) * P.out_W + (ix * P.ox_mul + P.ox_add);
 #pragma unroll
-                for (int k = 0; k < KSTEPS; ++k) {
-                  const uint64_t da = ((uint64_t)desca_hi << 32) | (uint64_t)(a_lo + 2 * k), db = ((uint64_t)descb_hi << 32) | (uint64_t)(b_lo + 2 * k);
-                  if constexpr (PAIR) tc_mma_f16_pair(dt, da, db, P.idesc, (accf | (uint32_t)k) ? 1u : 0u);
-                  else tc_mma_f16(dt, da, db, P.idesc, (accf | (uint32_t)k) ? 1u : 0u);
-                }
-              }
-            }
-            if (w_stream) {
-              if constexpr (PAIR) tc_commit_pair(smem_u32(emptyW + sw));
-              else if constexpr (CS > 1) tc_commit_mc(smem_u32(emptyW + sw), kMask);   // one arrival on every CTA's empty barrier of this slot
-              else tc_commit(smem_u32(emptyW + sw));
-            }
-          }
-          __syncwarp();
-          if (w_stream) { if (++sw == P.n_w_ring) { sw = 0; phw ^= 1; } }
-          i += n_same;
-        }
-        if (elect_one()) { if constexpr (PAIR) tc_commit_pair(smem_u32(emptyA + sa)); else tc_commit(smem_u32(emptyA + sa)); }
-        __syncwarp();
-        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
-      }
-      if (elect_one()) { if constexpr (PAIR) tc_commit_pair(smem_u32(tfull + stage)); else tc_commit(smem_u32(tfull + stage)); }
-      __syncwarp();
-      if (++stage == P.n_stages) { stage = 0; eph ^= 1; }
+  for (int c0 = 0; c0 < N; c0 += CW) {
+    if (c0 > 0) consumer_sync();     // the previous round's readers are done with the staging rows
+#pragma unroll
+    for (int jj = 0; jj < CW / 8; ++jj) {
+      const int j = c0 / 8 + jj;
+      *reinterpret_cast<float2*>(s_stage + frow * SP + 8 * jj + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_stage + (frow + 8) * SP + 8 * jj + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-  } else if (warp >= 2) {
-    const int q = warp & 3, eg = (warp - 2) >> 2;
-    int stage = 0;
-    uint32_t fph = 0;
-    TileIter it;
-    it.init(blockIdx.x, gridDim.x, P.tiles_x, P.tiles_per_img / P.tiles_x);
-    for (int t = blockIdx.x; t < P.n_tiles_total; t += gridDim.x, it.next()) {
-      const int b = it.b, y0 = it.ty * THH, x0 = it.tx * TWH;
-      mbar_wait(smem_u32(tfull + stage), fph, 25);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int m = q * 32 + lane;
-      for (int s = eg; s < P.n_acc; s += P.epi_groups) {
-        const TcAccOut ao = P.acc_out[s];
-        const int xs = x0 + ao.dx, ys = y0 + ao.dy;
-        const int iy = ys + (m >> 3), ix = xs + (m & 7);
-        const bool valid = (iy < P.H) && (ix < P.W);
-        const size_t pix = ((size_t)b * P.out_H + (iy * P.oy_mul + ao.oy_add)) * P.out_W + (ix * P.ox_mul + ao.ox_add);
-        const uint32_t tcol = (uint32_t)((stage * P.n_acc + s) * P.N);
-        if (P.ablate & 8) {                            // profiling only: epilogue without TMEM loads
-          for (int c0 = 0; c0 < P.N; c0 += 16) {
-            uint32_t r16[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) r16[j] = (uint32_t)(lane + j);
-            tc_epilogue_cols<8>(P, s_par, r16, 0, c0, valid && !(P.ablate & 4), pix, b, xs, ys, q, lane);
-          }
-        } else {
-          tc_epilogue_acc<8, KSTEPS == 4>(P, s_par, tmem_base + ((uint32_t)(q * 32) << 16) + tcol, 0, valid && !(P.ablate & 4), pix, b, xs, ys, q, lane);
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) {
-        if (PAIR && crank != 0) mbar_arrive_cluster(mapa_rank(smem_u32(tempty + stage), 0));   // the leader's MMA warp owns the accumulators
-        else mbar_arrive(smem_u32(tempty + stage));
-      }
-      if (++stage == P.n_stages) { stage = 0; fph ^= 1; }
-    }
-  }
-  __syncwarp();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if constexpr (CS > 1) cluster_sync_all();          // nobody leaves while a peer may still multicast into it / signal its barriers
-  if (warp == 0) {
-    if constexpr (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// First layer on the tensor cores, fused with InferenceLayer.preprocess (inference.py:940-967):
-// raw uint8 / float frame -> * (1/255) -> zero pad -> 3x3 SAME conv + bias + ReLU -> fp16 NHWC.
-// K = 9 taps x CIN (9 or 27) is zero-padded to KPAD = 16 / 32; every thread gathers the 3x3
-// neighbourhood of "its" pixel and writes one K-major row of the A tile straight into the
-// 32B / 64B-swizzled UMMA layout (no TMA: the source is 1-3 bytes per pixel).  One MMA (two for
-// RGB) per 128-pixel tile; the epilogue is the shared tcgen05.ld path.
-template <typename TI, int CIN>
-__global__ void __launch_bounds__(128) k_conv_first_tc(const TI* __restrict__ img, int Hin, int Win, int Hnet, int Wnet,
-                                                       int tiles_x, int tiles_per_img, int n_tiles_total,
-                                                       const __half* __restrict__ wk /*[N][KPAD] fp16*/, int in_is_u8,
-                                                       const __grid_constant__ TcParams P) {
-  constexpr int KPAD = CIN == 1 ? 16 : 32;
-  constexpr int ROWB = KPAD * 2;                       // bytes per A / B row
-  constexpr int LAYOUT = CIN == 1 ? 6 : 4;             // SWIZZLE_32B / SWIZZLE_64B
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sA = base;                                   // 2 x (128 rows x ROWB): double buffered
-  uint8_t* sB = base + 2 * 128 * ROWB;                  // N rows x ROWB
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sB + 64 * ROWB);   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 2);
-  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 1) + 15) & ~(uintptr_t)15);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  stage_params(P, s_par, 0);
-  // weights -> swizzled B tile: 16-byte chunk c of row r lands at chunk c ^ ((row address >> 7) & (ROWB/16 - 1))
-  for (int t = threadIdx.x; t < P.N * (ROWB / 16); t += 128) {
-    const int r = t / (ROWB / 16), c = t % (ROWB / 16);
-    const uint4 v = *reinterpret_cast<const uint4*>(wk + (size_t)r * KPAD + c * 8);
-    const int pc = c ^ (((r * ROWB) >> 7) & (ROWB / 16 - 1));
-    *reinterpret_cast<uint4*>(sB + r * ROWB + pc * 16) = v;
-  }
-  if (threadIdx.x == 0) {
-    mbar_init(smem_u32(bar), 1);
-    mbar_init(smem_u32(bar + 1), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(P.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
-  const int m = threadIdx.x;                            // A row = TMEM lane = tile pixel
-  const int ty = m / TW, tx = m % TW;
-
-  // gathers the 3x3 x CIN neighbourhood of this thread's pixel of tile (b, y0, x0) into A buffer `buf`
-  auto build = [&](int b, int y0, int x0, int buf) {
-    const int oy = y0 + ty, ox = x0 + tx;
-    __align__(16) __half row[KPAD];
-#pragma unroll
-    for (int k = 0; k < KPAD; ++k) row[k] = __float2half(0.f);
-    const TI* im = img + (size_t)b * Hin * Win * CIN;
-#pragma unroll
-    for (int ky = 0; ky < 3; ++ky) {
-      const int iy = oy + ky - 1;
-#pragma unroll
-      for (int kx = 0; kx < 3; ++kx) {
-        const int ix = ox + kx - 1;
-        const bool ok = iy >= 0 && iy < Hin && ix >= 0 && ix < Win;
-#pragma unroll
-        for (int ci = 0; ci < CIN; ++ci) {
-          const float v = ok ? __fmul_rn((float)im[((size_t)iy * Win + ix) * CIN + ci], sc) : 0.f;
-          row[(ky * 3 + kx) * CIN + ci] = __float2half_rn(v);
-        }
-      }
-    }
-    uint8_t* dst = sA + buf * 128 * ROWB;
-#pragma unroll
-    for (int c = 0; c < ROWB / 16; ++c) {
-      const int pc = c ^ (((m * ROWB) >> 7) & (ROWB / 16 - 1));
-      *reinterpret_cast<uint4*>(dst + m * ROWB + pc * 16) = *reinterpret_cast<const uint4*>(&row[c * 8]);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
-  };
-  auto issue = [&](int buf) {            // warp 0: one elected lane issues the MMA(s) of the tile staged in `buf`
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (elect_one()) {
-      const uint64_t da = make_desc(smem_u32(sA + buf * 128 * ROWB), ROWB, LAYOUT);
-      const uint64_t db = make_desc(smem_u32(sB), ROWB, LAYOUT);
-#pragma unroll
-      for (int k = 0; k < KPAD / 16; ++k) tc_mma_f16(tmem_base + (uint32_t)(buf * P.N), da + 2 * k, db + 2 * k, P.idesc, k ? 1u : 0u);
-      tc_commit(smem_u32(bar + buf));
-    }
-    __syncwarp();
-  };
-
-  TileIter it;
-  it.init(blockIdx.x, gridDim.x, tiles_x, tiles_per_img / tiles_x);
-  int t = blockIdx.x;
-  if (t < n_tiles_total) {
-    build(it.b, it.ty * TH, it.tx * TW, 0);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) issue(0);
-  }
-  // software pipeline: gather tile i+1 and issue its MMA while the MMA of tile i completes, then drain tile i
-  for (int i = 0; t < n_tiles_total; ++i, t += gridDim.x) {
-    const int b = it.b, y0 = it.ty * TH, x0 = it.tx * TW;
-    const int cur = i & 1, nxt = cur ^ 1;
-    const bool has_next = t + (int)gridDim.x < n_tiles_total;
-    it.next();
-    if (has_next) build(it.b, it.ty * TH, it.tx * TW, nxt);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();                      // A(i+1) staged; everyone is done reading TMEM stage `nxt` (tile i-1)
-    if (has_next && warp == 0) issue(nxt);
-    mbar_wait(smem_u32(bar + cur), (uint32_t)((i >> 1) & 1), 31);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int oy = y0 + ty, ox = x0 + tx;
-    const bool valid = (oy < Hnet) && (ox < Wnet);
-    const size_t pix = ((size_t)b * P.out_H + oy) * P.out_W + ox;
-    for (int c0 = 0; c0 < P.N; c0 += 16) {
-      uint32_t r16[16];
-      tc_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(cur * P.N + c0), r16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      tc_epilogue_cols(P, s_par, r16, 0, c0, valid, pix, b, x0, y0, warp, lane);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(P.tmem_cols) : "memory");
+    consumer_sync();
+    const int cc = c0 + 16 * half;
+    if (cc < c0 + CW && n0 + cc < P.Cout)     // warp-uniform
+      tc_epilogue_chunk(P, s_par, s_stage + m * SP + 16 * half, n0, cc, valid, pix, b, x0, y0, warp & 3, lane);
   }
 }
 
@@ -1299,12 +462,11 @@ EncodeTiledFn get_encode() {
 
 // ------------------------------------------------------------------------------------------------
 // 1x1 linear head (heads.py:55-63: Conv2D(channels, 1, activation="linear"), fp32 output): C_in x C_out per pixel is a few
-// hundred MACs against C_in * 2 + C_out * 4 bytes of traffic, i.e. an HBM-bound layer.  On the tcgen05 path each of the
-// 4 epilogue warps of an SM wrote 13 (24) strided 4-byte stores per pixel and the launch ran at 0.3-0.45 of its HBM
-// floor (profiles/r01_step_full_summary.md).  Here: warp-level mma.sync m16n8k16 (fp16 x fp16 -> fp32; the layer is not
-// tensor bound, what matters is that the MACs cost no issue slots), 16 pixels x C_in channels per warp staged with 16-byte-per-lane loads (whole 128-byte
-// lines per warp instruction; fragment loads straight from global memory cost 8 L1 wavefronts per 128 useful bytes and
-// ran at 1.7 TB/s) and read back with ldmatrix, weights [N_pad][C_in] fp16 in shared memory, and the 16 x C_out fp32 results of a warp staged through shared memory so that the global stores
+// hundred MACs against C_in * 2 + C_out * 4 bytes of traffic, i.e. an HBM-bound layer: the implicit-GEMM conv kernel would
+// write 13 (24) strided 4-byte stores per pixel.  Here: warp-level mma.sync m16n8k16 (fp16 x fp16 -> fp32; the layer is not
+// tensor bound, what matters is that the MACs cost no issue slots), 16 pixels x C_in channels per warp staged with
+// 16-byte-per-lane loads (whole 128-byte lines per warp instruction) and read back with ldmatrix, weights [N_pad][C_in]
+// fp16 in shared memory, and the 16 x C_out fp32 results of a warp staged through shared memory so that the global stores
 // are contiguous 4-byte-per-lane runs.  64 warps per SM keep ~128 KB of loads in flight.
 template <int NT, int KCH>   // n-tiles of 8 output channels (C_out <= 8 * NT); input channels staged per pass (16 / 32 / 64 / 128)
 __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in, int in_Ctot, int in_coff, int Cin,
@@ -1441,26 +603,15 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
 
 struct TcLaunch {
   CUtensorMap mapA, mapB;
-  TcParams P;          // streaming variant (one CTA per tile, weights streamed through a TMA ring)
+  TcParams P;
   dim3 grid;
   size_t smem;
-  bool has_persist;    // persistent variant available (filter bank resident in shared memory)
-  TcParams PP;
-  size_t smem_p;
-  int occ;
-  int use_persist;     // variant chosen at configure time by timing them on the device: 0 stream, 1 persist, 2 halo
-  // halo variants (variant id 2 + i): super-tiles of sub_x x sub_y 8x16 sub-tiles, box [KC, 8*sub_x+2, 16*sub_y+2, 1]
-  bool pp_valid;       // PP holds the tap/slot tables (the launch covers all output channels with one N)
-  int n_halo;
-  struct Halo { CUtensorMap map; TcParams P; size_t smem; int occ, threads; bool prog; int mc; CUtensorMap mapBpiece; } halo[8];
 };
 
 }  // namespace
 
 struct SbConvTcPlan {
   std::vector<TcLaunch> launches;   // 1 for conv, 4 phases for tconv
-  std::vector<TcLaunch> fused;      // tconv: all phases in one launch (two when 4 accumulators exceed TMEM)
-  bool use_fused = false;
   __half* w16 = nullptr;            // [taps][Cout_pad][Cin]
   int Cout_pad = 0;
   // first layer as a Toeplitz GEMM (sb_first_view_prepare): staged [B][H][W/8][16] fp16 view of the frame
@@ -1472,7 +623,6 @@ struct SbConvTcPlan {
   bool s2d = false;                 // view_in is the space-to-depth view of the frame (7x7 stride-2 stem as a 4x4 conv)
   int s2d_Hs = 0, s2d_Ws = 0;
   bool out_dead = false;            // nobody reads the full-resolution output (only the fused pool): stores are skipped
-  bool skip_now = false;            // out_dead, unless the caller asked for that buffer (sb_model_forward)
 };
 
 static CUtensorMapSwizzle swz_for(int KC) {
@@ -1500,10 +650,7 @@ static bool tc_eligible(const SbModel* m, const SbOp& op) {
   return true;
 }
 
-void sb_conv_first_tc_release(const SbModel* m);
-
 void sb_conv_tc_release(SbModel* m) {
-  sb_conv_first_tc_release(m);
   for (SbConvTcPlan* p : m->tc_plans)
     if (p) {
       if (p->w16) cudaFree(p->w16);
@@ -1537,10 +684,15 @@ struct TcView {
   int out_coff = 0;
 };
 
+// N of the wgmma instantiation that covers `n` output channels (extra rows of the weight box are zero-filled by TMA)
+static int wg_n(int n) {
+  for (int c : {16, 32, 48, 64, 96, 128, 192}) if (n <= c) return c;
+  return 256;
+}
+
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
                        const TcGroup* groups, int dy0, int extra_rows, int n_wtaps, int oy_mul, int oy_add,
-                       int ox_mul, int ox_add, int fused_phases = 0, std::vector<TcLaunch>* dst = nullptr,
-                       const TcView* view = nullptr) {
+                       int ox_mul, int ox_add, const TcView* view = nullptr) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   const SbBuffer& ib = view ? view->ib : m->buffers[op.in_buf()];
@@ -1558,14 +710,8 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   P.n_groups = n_groups;
   for (int g = 0; g < n_groups; ++g) P.groups[g] = groups[g];
   P.dy0 = dy0; P.box_rows = TH + extra_rows;
-  const int N = std::min(plan->Cout_pad, 256);
+  const int N = wg_n(std::min(plan->Cout_pad, 256));
   P.N = N; P.Cout = Cout;
-  // cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b format F16 (0) @7/@10, K-major (0) @15/@16,
-  // n_dim = N>>3 @17, m_dim = M>>4 @24.
-  P.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  int cols = 32;
-  while (cols < N) cols <<= 1;
-  P.tmem_cols = cols;
   P.out = ob.dev; P.out_f32 = ob.f32; P.out_H = ob.H; P.out_W = ob.W; P.out_Ctot = ob.C; P.out_coff = out_coff;
   P.oy_mul = oy_mul; P.oy_add = oy_add; P.ox_mul = ox_mul; P.ox_add = ox_add;
   if (view) {
@@ -1588,295 +734,25 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
       ob.C % 16 == 0 && out_coff % 16 == 0 && (P.pool_out == nullptr || (P.pool_Ctot % 16 == 0 && P.pool_coff % 16 == 0)))
     P.epi_mode = 1;
   P.row_bytes = KC * 2;
-  P.layout_type = KC == 64 ? 2 : (KC == 32 ? 4 : 6);
+  P.layout_type = KC == 64 ? 1 : (KC == 32 ? 2 : 3);     // wgmma descriptor layout: SW128 / SW64 / SW32
   P.a_tx_bytes = P.box_rows * TW * KC * 2;
   P.b_tx_bytes = N * KC * 2;
   P.a_slot_bytes = (P.a_tx_bytes + 1023) / 1024 * 1024;
   P.b_slot_bytes = (P.b_tx_bytes + 1023) / 1024 * 1024;
   int total_steps = 0;
   for (int g = 0; g < n_groups; ++g) total_steps += groups[g].n_taps;
+  // rings: up to 3 activation boxes and 4 weight slices in flight, within what is left of the SM's shared memory after
+  // the accumulator staging rows, the barriers and the bias / BN vectors
+  const size_t stage_bytes = (size_t)128 * (stage_cols(N) + 4) * sizeof(float);
+  const size_t ring_budget = 200 * 1024 - stage_bytes;
   P.n_a_slots = std::min(3, P.n_chunks * n_groups);
   P.n_b_slots = std::min(4, P.n_chunks * total_steps);
-  while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > 200 * 1024 && P.n_b_slots > 2) P.n_b_slots--;
-  while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > 200 * 1024 && P.n_a_slots > 2) P.n_a_slots--;
-  L.smem = (size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes + 1024 /*align slack*/ +
-           (size_t)(2 * P.n_a_slots + 2 * P.n_b_slots + 1) * 8 + 64 + 3 * 256 * sizeof(float);
-  L.grid = dim3(P.tiles_x * tiles_y, plan->Cout_pad / N, 1 /* z = batch, set at launch */);
-  {
-    // never let more CTAs become co-resident than TMEM can serve without waiting inside tcgen05.alloc
-    cudaFuncAttributes fa;
-    const void* fn = KC == 16 ? (const void*)k_conv_tc<1> : (KC == 32 ? (const void*)k_conv_tc<2> : (const void*)k_conv_tc<4>);
-    if (cudaFuncGetAttributes(&fa, fn) == cudaSuccess) {
-      const int by_regs = 65536 / std::max(1, ((fa.numRegs + 7) / 8 * 8) * 128);
-      const int by_smem = (int)((227 * 1024) / (L.smem + fa.sharedSizeBytes + 1024));
-      const int hw_occ = std::max(1, std::min(std::min(by_regs, by_smem), 32));
-      const int tmem_occ = 512 / P.tmem_cols;
-      if (hw_occ > tmem_occ) L.smem = std::max(L.smem, std::min<size_t>(kMaxDynSmem, (size_t)(227 * 1024) / tmem_occ - 2048));
-    }
-  }
-  // persistent variant when the whole filter bank of this launch fits in shared memory
-  P.persistent = 0;
-  P.tw = TW;
-  P.tiles_per_img = P.tiles_x * tiles_y;
-  L.has_persist = false;
-  L.n_halo = 0;
-  const bool small_filter = n_wtaps <= 9 && n_groups <= 3;     // persistent / halo variants: 1x1, 3x3 and the transposed-conv phases
-  if (small_filter) {
-    int used[9], n_used = 0, slot_of[9];
-    for (int i = 0; i < 9; ++i) slot_of[i] = -1;
-    for (int g = 0; g < n_groups; ++g)
-      for (int t = 0; t < groups[g].n_taps; ++t) {
-        const int wt = groups[g].taps[t].w_tap;
-        if (slot_of[wt] < 0) { slot_of[wt] = n_used; used[n_used++] = wt; }
-      }
-    const size_t w_bytes = (size_t)P.n_chunks * n_used * P.b_slot_bytes;
-    const size_t budget = tc_budget();
-    L.pp_valid = plan->Cout_pad == N;
-    {
-      TcParams& Q = L.PP;
-      Q = P;
-      Q.persistent = 1;
-      Q.n_used_taps = n_used;
-      for (int i = 0; i < 9; ++i) { Q.used_taps[i] = i < n_used ? used[i] : 0; Q.slot_of_tap[i] = slot_of[i]; }
-      Q.w_slot_bytes = P.b_slot_bytes;
-    }
-    if (!getenv("SB_DISABLE_PERSISTENT") && plan->Cout_pad == N && 2 * N <= 512 &&
-        w_bytes + 2 * (size_t)P.a_slot_bytes <= budget) {
-      TcParams& Q = L.PP;
-      // activation ring: two tiles of look-ahead (2 x n_groups halo tiles per chunk) when it fits
-      int na = (int)((budget - w_bytes) / P.a_slot_bytes);
-      Q.n_a_slots = std::max(2, std::min(na, std::max(6, 2 * n_groups)));
-      // accumulator stages: as many as TMEM allows (the mbarrier hand-offs between the MMA and the
-      // epilogue warps cost ~0.5 us each; a deep ring keeps both sides from ever sleeping)
-      int ns = getenv("SB_TMEM_STAGES") ? atoi(getenv("SB_TMEM_STAGES")) : 8;
-      while (ns > 2 && ns * N > 512) ns >>= 1;
-      Q.n_stages = ns;
-      int c2 = 32;
-      while (c2 < ns * N) c2 <<= 1;
-      Q.tmem_cols = c2;
-      L.smem_p = w_bytes + (size_t)Q.n_a_slots * P.a_slot_bytes + 1024 + (size_t)(2 * Q.n_a_slots + 2 * 8 + 1) * 8 + 64 + 3 * 256 * sizeof(float);
-      // co-residency the hardware may reach (registers / shared memory); the TMEM demand of that many
-      // CTAs must fit the 512 columns of the SM outright, because a CTA that has to wait inside
-      // tcgen05.alloc for a neighbour to exit was observed to fault on sm_100a
-      cudaFuncAttributes fa;
-      int occ = 1;
-      const void* fn = KC == 16 ? (const void*)k_conv_tc_persist<1> : (KC == 32 ? (const void*)k_conv_tc_persist<2> : (const void*)k_conv_tc_persist<4>);
-      if (cudaFuncGetAttributes(&fa, fn) == cudaSuccess) {
-        const int by_regs = 65536 / std::max(1, ((fa.numRegs + 7) / 8 * 8) * 192);
-        const int by_smem = (int)((227 * 1024) / (L.smem_p + fa.sharedSizeBytes + 1024));
-        occ = std::max(1, std::min(std::min(by_regs, by_smem), 16));
-        auto cols_for = [&](int nst) { int c = 32; while (c < nst * N) c <<= 1; return c; };
-        while (occ * Q.tmem_cols > 512 && Q.n_stages > 2) { Q.n_stages >>= 1; Q.tmem_cols = cols_for(Q.n_stages); }
-        if (occ * Q.tmem_cols > 512) { Q.n_stages = 1; Q.tmem_cols = cols_for(1); }        // last resort: single stage
-        if (occ * Q.tmem_cols > 512) { L.smem_p = std::max(L.smem_p, std::min<size_t>(kMaxDynSmem, (size_t)(227 * 1024) / (512 / Q.tmem_cols) - 2048)); occ = 512 / Q.tmem_cols; }
-      }
-      L.occ = occ;
-      L.has_persist = true;
-    }
-  }
-  // a pair twin is only valid when its half-size weight slot keeps the 1024-byte alignment of the swizzle atoms
-  auto Q_ok = [](const TcLaunch::Halo& Hh) { return Hh.mc != 4 || (Hh.P.w_slot_bytes % 1024 == 0 && Hh.P.n_w_ring >= 2); };
-  L.n_halo = 0;
-  // sub_x, sub_y, epilogue groups; 8x32 (1x2) measured 2-5 % ahead of 16x16 (2x1) on the 64..256-channel layers
-  int kHaloShapes[5][3] = {{1, 1, 1}, {2, 1, 2}, {2, 2, 2}, {1, 2, 2}, {0, 0, 0}};
-  int n_shapes = 4;
-  if (const char* e = getenv("SB_HALO_SHAPES")) {      // experiments: "sx,sy,eg;sx,sy,eg;..."
-    n_shapes = 0;
-    while (*e && n_shapes < 4) {
-      int a = 1, b = 1, c = 1;
-      if (sscanf(e, "%d,%d,%d", &a, &b, &c) == 3) { kHaloShapes[n_shapes][0] = a; kHaloShapes[n_shapes][1] = b; kHaloShapes[n_shapes][2] = c; ++n_shapes; }
-      const char* semi = strchr(e, ';');
-      if (!semi) break;
-      e = semi + 1;
-    }
-  }
-  if (fused_phases) {          // fused transposed conv: ONE candidate, 8x16 input tile, one accumulator per phase
-    kHaloShapes[0][0] = 1; kHaloShapes[0][1] = 1; kHaloShapes[0][2] = 2;
-    n_shapes = 1;
-    L.has_persist = false;
-  }
-  for (int hs = 0; hs < n_shapes && L.n_halo < 8 && L.pp_valid && small_filter && !getenv("SB_DISABLE_HALO"); ++hs) {
-    const int sub_x = kHaloShapes[hs][0], sub_y = kHaloShapes[hs][1], egroups = kHaloShapes[hs][2];
-    const int n_sub = sub_x * sub_y;
-    const int pitch = fused_phases ? 9 : 8 * sub_x + 2, box_h = fused_phases ? 17 : 16 * sub_y + 2;
-    if (ib.W < pitch || ib.H < box_h) continue;
-    if ((n_sub > 1 || fused_phases) && getenv("SB_DISABLE_SUPERTILE")) continue;
-    TcLaunch::Halo& HC = L.halo[L.n_halo];
-    TcParams& Hp = HC.P;
-    Hp = L.PP;
-    Hp.tw = 8;
-    Hp.sub_x = sub_x; Hp.sub_y = sub_y; Hp.pitch = pitch; Hp.epi_groups = egroups;
-    Hp.tiles_x = (ib.W + 8 * sub_x - 1) / (8 * sub_x);
-    Hp.tiles_per_img = Hp.tiles_x * ((ib.H + 16 * sub_y - 1) / (16 * sub_y));
-    Hp.halo_base_offset = getenv("SB_HALO_BASEOFF") ? atoi(getenv("SB_HALO_BASEOFF")) : 0;
-    Hp.ablate = getenv("SB_ABLATE") ? atoi(getenv("SB_ABLATE")) : 0;
-    Hp.n_prog = 0; Hp.n_acc = 0;
-    struct ProgTmp { int a_rows, w_tap, w_slot, acc, first, n_same; } prog_tmp[36];
-    if (fused_phases) {
-      // Conv2DTranspose k3 s2 (see sb_conv_tc_prepare): out[2i+a] gets (ky, row) = a==0 ? {(0,i),(2,i-1)} : {(1,i)};
-      // same along x.  Box origin (x0-1, y0-1); phase (a, bx) accumulates in its own TMEM columns.
-      Hp.dx0 = -1; Hp.dy0 = -1;
-      int n_used = 0;
-      for (int i = 0; i < 9; ++i) Hp.slot_of_tap[i] = -1;
-      for (int a = 0; a < 2; ++a)
-        for (int bx = 0; bx < 2; ++bx) {
-          if (!(fused_phases & (1 << (a * 2 + bx)))) continue;
-          const int acc = Hp.n_acc++;
-          Hp.acc_out[acc] = TcAccOut{0, 0, (int16_t)a, (int16_t)bx};
-          const int kys[2] = {a == 0 ? 0 : 1, 2}, dys[2] = {0, -1}, nky = a == 0 ? 2 : 1;
-          const int kxs[2] = {bx == 0 ? 0 : 1, 2}, dxs[2] = {0, -1}, nkx = bx == 0 ? 2 : 1;
-          bool first = true;
-          for (int qy = 0; qy < nky; ++qy)
-            for (int qx = 0; qx < nkx; ++qx) {
-              const int wt = kys[qy] * 3 + kxs[qx];
-              Hp.used_taps[n_used] = wt; Hp.slot_of_tap[wt] = n_used;
-              prog_tmp[Hp.n_prog++] = ProgTmp{((dys[qy] + 1) * pitch + (dxs[qx] + 1)), wt, n_used++, acc, first ? 1 : 0, 1};
-              first = false;
-            }
-        }
-      Hp.n_used_taps = n_used;
-    } else {
-      int dxmin = 0;
-      for (int g = 0; g < n_groups; ++g) dxmin = std::min(dxmin, groups[g].dx);
-      Hp.dx0 = dxmin;
-      Hp.n_htaps = 0;
-      for (int g = 0; g < n_groups; ++g)
-        for (int t = 0; t < groups[g].n_taps; ++t) {
-          Hp.htap_off_rows[Hp.n_htaps] = groups[g].taps[t].row_off * pitch + (groups[g].dx - dxmin);
-          Hp.htap_w[Hp.n_htaps] = groups[g].taps[t].w_tap;
-          ++Hp.n_htaps;
-        }
-      Hp.n_acc = n_sub;
-      for (int sIdx = 0; sIdx < n_sub; ++sIdx)
-        Hp.acc_out[sIdx] = TcAccOut{(int16_t)((sIdx % sub_x) * 8), (int16_t)((sIdx / sub_x) * 16), (int16_t)oy_add, (int16_t)ox_add};
-      for (int tp = 0; tp < Hp.n_htaps; ++tp)       // taps outermost: a weight slice serves every sub-tile
-        for (int sIdx = 0; sIdx < n_sub; ++sIdx) {
-          const int sub_rows = (sIdx / sub_x) * 16 * pitch + (sIdx % sub_x) * 8;
-          prog_tmp[Hp.n_prog++] = ProgTmp{sub_rows + Hp.htap_off_rows[tp], Hp.htap_w[tp], Hp.slot_of_tap[Hp.htap_w[tp]], sIdx, tp == 0 ? 1 : 0,
-                                          sIdx == 0 ? n_sub : 0};
-        }
-    }
-    for (int i = 0; i < Hp.n_prog; ++i) {
-      const ProgTmp& t = prog_tmp[i];
-      const uint32_t a_off16 = (uint32_t)(t.a_rows * Hp.row_bytes) >> 4, w_off16 = (uint32_t)(t.w_slot * Hp.w_slot_bytes) >> 4;
-      Hp.prog[i].a_acc = (a_off16 & 0xffffu) | ((uint32_t)(t.acc * N) << 16);
-      Hp.prog[i].w_flags = (w_off16 & 0xffffu) | ((uint32_t)t.first << 16) | ((uint32_t)t.n_same << 20) | ((uint32_t)t.w_tap << 26);
-    }
-    if (Hp.n_acc * N > 512) continue;
-    Hp.a_tx_bytes = box_h * pitch * KC * 2;
-    Hp.a_slot_bytes = (Hp.a_tx_bytes + 1023) / 1024 * 1024;
-    size_t w_bytes = (size_t)Hp.n_chunks * Hp.n_used_taps * Hp.w_slot_bytes;
-    const size_t budget = tc_budget();
-    Hp.w_stream = 0; Hp.n_w_ring = 0;
-    const bool resident_fits = !getenv("SB_DISABLE_PERSISTENT") && w_bytes + 2 * (size_t)Hp.a_slot_bytes <= budget;
-    if (!resident_fits || getenv("SB_FORCE_WSTREAM")) {
-      if (getenv("SB_DISABLE_WSTREAM")) continue;
-      if (2 * (size_t)Hp.a_slot_bytes + 2 * (size_t)Hp.w_slot_bytes > budget) continue;
-      Hp.w_stream = 1;
-      Hp.n_a_slots = 2;
-      Hp.n_w_ring = (int)std::min<size_t>(6, (budget - 2 * (size_t)Hp.a_slot_bytes) / Hp.w_slot_bytes);
-      if (Hp.n_w_ring >= 5 && 3 * (size_t)Hp.a_slot_bytes + 4 * (size_t)Hp.w_slot_bytes <= budget) { Hp.n_a_slots = 3; Hp.n_w_ring = 4; }
-      w_bytes = (size_t)Hp.n_w_ring * Hp.w_slot_bytes;
-    } else {
-      const int na = (int)((budget - w_bytes) / Hp.a_slot_bytes);
-      Hp.n_a_slots = std::max(2, std::min(na, n_sub > 1 ? 3 : 6));
-    }
-    HC.prog = Hp.n_acc > 1 || Hp.w_stream;       // the plain 8x16 weights-resident case keeps the unrolled kernel
-    HC.threads = HC.prog ? 64 + 128 * egroups : 192;
-    if (!HC.prog) Hp.epi_groups = 1;
-    if (HC.prog && Hp.n_acc < 2) { Hp.epi_groups = 1; HC.threads = 192; }
-    HC.smem = w_bytes + (size_t)Hp.n_a_slots * Hp.a_slot_bytes + 1024 + (size_t)(2 * Hp.n_a_slots + 2 * 8 + 1 + 16) * 8 + 64 + 3 * 256 * sizeof(float);
-    cudaFuncAttributes fa;
-    int occ = 1;
-    const void* fn = HC.prog ? (KC == 16 ? (const void*)k_conv_tc_prog<1> : (KC == 32 ? (const void*)k_conv_tc_prog<2> : (const void*)k_conv_tc_prog<4>))
-                             : (KC == 16 ? (const void*)k_conv_tc_halo<1> : (KC == 32 ? (const void*)k_conv_tc_halo<2> : (const void*)k_conv_tc_halo<4>));
-    const int NS = Hp.n_acc * N;      // TMEM columns of one accumulator stage
-    auto cols_for = [&](int nst) { int c = 32; while (c < nst * NS) c <<= 1; return c; };
-    Hp.n_stages = getenv("SB_TMEM_STAGES") ? atoi(getenv("SB_TMEM_STAGES")) : (Hp.n_acc > 1 ? 4 : 8);
-    while (Hp.n_stages > 1 && Hp.n_stages * NS > 512) Hp.n_stages >>= 1;
-    Hp.tmem_cols = cols_for(Hp.n_stages);
-    if (cudaFuncGetAttributes(&fa, fn) == cudaSuccess) {
-      const int by_regs = 65536 / std::max(1, ((fa.numRegs + 7) / 8 * 8) * HC.threads);
-      const int by_smem = (int)((227 * 1024) / (HC.smem + fa.sharedSizeBytes + 1024));
-      occ = std::max(1, std::min(std::min(by_regs, by_smem), 16));
-      while (occ * Hp.tmem_cols > 512 && Hp.n_stages > 2) { Hp.n_stages >>= 1; Hp.tmem_cols = cols_for(Hp.n_stages); }
-      if (occ * Hp.tmem_cols > 512) { Hp.n_stages = 1; Hp.tmem_cols = cols_for(1); }
-      if (occ * Hp.tmem_cols > 512) { HC.smem = std::max(HC.smem, std::min<size_t>(kMaxDynSmem, (size_t)(227 * 1024) / (512 / Hp.tmem_cols) - 2048)); occ = 512 / Hp.tmem_cols; }
-    }
-    HC.occ = occ;
-    cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)ib.W, (cuuint64_t)ib.H, (cuuint64_t)m->B};
-    cuuint64_t strides[3] = {(cuuint64_t)ib.C * 2, (cuuint64_t)ib.W * ib.C * 2, (cuuint64_t)ib.H * ib.W * ib.C * 2};
-    cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)pitch, (cuuint32_t)box_h, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    void* gptr = (void*)((__half*)ib.dev + in_coff);
-    CUresult r = enc(&HC.map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, gptr, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A halo) failed: %d", (int)r);
-    HC.mc = 0;
-    ++L.n_halo;
-    // twin of a weight-streamed candidate on clusters of two CTAs.  Default: the cta_group::2 PAIR (mc = 4: M = 256 MMAs,
-    // each CTA stages N/2 rows of every slice in a half-size slot, so the ring is deeper).  SB_ENABLE_MULTICAST=1 selects the
-    // round-2 multicast form instead (mc = 2: full slices in both CTAs, each fetching half) -- measured no faster than
-    // unicast, kept as an experiment (DESIGN.md 5.1).
-    if (Hp.w_stream && HC.prog && N % 16 == 0 && L.n_halo < 8 && !getenv("SB_DISABLE_MULTICAST") && !getenv("SB_DISABLE_PAIR")) {
-      TcLaunch::Halo& H2 = L.halo[L.n_halo];
-      const TcLaunch::Halo& H1 = L.halo[L.n_halo - 1];
-      H2 = H1;
-      H2.mc = getenv("SB_ENABLE_MULTICAST") ? 2 : 4;
-      H2.occ = 1;
-      if (H2.mc == 4) {
-        TcParams& Q = H2.P;
-        Q.w_slot_bytes = H1.P.w_slot_bytes / 2;                      // N/2 rows x KC: stays a multiple of 8 rows (N % 16 == 0)
-        Q.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-        const size_t a_bytes = (size_t)Q.n_a_slots * Q.a_slot_bytes;
-        Q.n_w_ring = (int)std::min<size_t>(8, (tc_budget() - a_bytes) / Q.w_slot_bytes);
-        if (Q.n_a_slots == 2 && Q.n_w_ring >= 7 && 3 * (size_t)Q.a_slot_bytes + 6 * (size_t)Q.w_slot_bytes <= tc_budget()) { Q.n_a_slots = 3; Q.n_w_ring = 6; }
-        H2.smem = (size_t)Q.n_w_ring * Q.w_slot_bytes + (size_t)Q.n_a_slots * Q.a_slot_bytes + 1024 +
-                  (size_t)(2 * Q.n_a_slots + 2 * 8 + 1 + 16) * 8 + 64 + 3 * 256 * sizeof(float);
-      }
-      cuuint64_t wdims[3] = {(cuuint64_t)Cin, (cuuint64_t)plan->Cout_pad, (cuuint64_t)n_wtaps};
-      cuuint64_t wstrides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)plan->Cout_pad * Cin * 2};
-      cuuint32_t pbox[3] = {(cuuint32_t)KC, (cuuint32_t)(N / 2), 1};
-      cuuint32_t wes[3] = {1, 1, 1};
-      if (Q_ok(H2) && enc(&H2.mapBpiece, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, wdims, wstrides, pbox, wes, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
-        ++L.n_halo;
-    } else if (!Hp.w_stream && N % 16 == 0 && L.n_halo < 8 && !getenv("SB_DISABLE_PAIR") && !getenv("SB_DISABLE_RESIDENT_PAIR") &&
-               (size_t)Hp.n_chunks * Hp.n_used_taps * Hp.w_slot_bytes >= 64 * 1024 && (Hp.w_slot_bytes / 2) % 1024 == 0) {
-      // cta_group::2 twin of a weights-RESIDENT candidate whose filter bank takes a large part of shared memory (128 -> 64:
-      // 147 KB, leaving two activation slots = one tile of look-ahead against ~1.5 us of TMA latency per box; ablations in
-      // DESIGN.md 7): the pair splits the bank, each CTA keeps N/2 rows of every slice, the activation ring gets the rest,
-      // and the M = 256 MMAs read half of B per SM (tools/probes/mma_probe.cu: N = 64, 43 instead of 48 clocks).
-      TcLaunch::Halo& H2 = L.halo[L.n_halo];
-      const TcLaunch::Halo& H1 = L.halo[L.n_halo - 1];
-      H2 = H1;
-      H2.mc = 4; H2.occ = 1; H2.prog = true;
-      TcParams& Q = H2.P;
-      Q.w_slot_bytes = H1.P.w_slot_bytes / 2;
-      Q.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      for (int i = 0; i < Q.n_prog; ++i) {           // resident slices are addressed by offset: half-size slots
-        const uint32_t off16 = Q.prog[i].w_flags & 0xffffu;
-        Q.prog[i].w_flags = (Q.prog[i].w_flags & ~0xffffu) | ((off16 / 2) & 0xffffu);
-      }
-      const size_t wb2 = (size_t)Q.n_chunks * Q.n_used_taps * Q.w_slot_bytes;
-      Q.n_a_slots = std::max(2, std::min((int)((budget - wb2) / Q.a_slot_bytes), n_sub > 1 ? 4 : 8));
-      if (Q.n_acc < 2) { Q.epi_groups = 1; H2.threads = 192; } else H2.threads = 64 + 128 * Q.epi_groups;
-      const int NS2 = Q.n_acc * N;
-      Q.n_stages = Q.n_acc > 1 ? 4 : 8;
-      while (Q.n_stages > 1 && Q.n_stages * NS2 > 512) Q.n_stages >>= 1;
-      { int c = 32; while (c < Q.n_stages * NS2) c <<= 1; Q.tmem_cols = c; }
-      H2.smem = wb2 + (size_t)Q.n_a_slots * Q.a_slot_bytes + 1024 + (size_t)(2 * Q.n_a_slots + 2 * 8 + 1 + 16) * 8 + 64 + 3 * 256 * sizeof(float);
-      cuuint64_t wdims[3] = {(cuuint64_t)Cin, (cuuint64_t)plan->Cout_pad, (cuuint64_t)n_wtaps};
-      cuuint64_t wstrides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)plan->Cout_pad * Cin * 2};
-      cuuint32_t pbox[3] = {(cuuint32_t)KC, (cuuint32_t)(N / 2), 1};
-      cuuint32_t wes[3] = {1, 1, 1};
-      if (enc(&H2.mapBpiece, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, wdims, wstrides, pbox, wes, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
-        ++L.n_halo;
-    }
-  }
-  if (fused_phases && L.n_halo == 0) return 1;     // caller falls back to the per-phase launches
-  L.use_persist = 0;
+  while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_b_slots > 2) P.n_b_slots--;
+  while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_a_slots > 2) P.n_a_slots--;
+  L.smem = (size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes + stage_bytes + 1024 /*align slack*/ +
+           (size_t)(2 * P.n_a_slots + 2 * P.n_b_slots) * 8 + 16 + 3 * 256 * sizeof(float);
+  if (L.smem > kMaxDynSmem) return sb_fail(h, SB_ERR_INVALID, "conv tile needs %zu bytes of shared memory", L.smem);
+  L.grid = dim3(P.tiles_x * tiles_y, (plan->Cout_pad + N - 1) / N, 1 /* z = batch, set at launch */);
   // A: NHWC view (slice channels, W, H, batch)
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)ib.W, (cuuint64_t)ib.H, (cuuint64_t)m->B};
@@ -1898,7 +774,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
-  (dst ? *dst : plan->launches).push_back(L);
+  plan->launches.push_back(L);
   return 0;
 }
 
@@ -1907,10 +783,9 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
 // With G[y][g][c] = in[y][8g-1+c] (c = 0..9; c = 10..15 zero) the layer is an ordinary 3x1 convolution
 // over the [H][W/8] grid of groups with 16 "input channels" (the window) and 8*Cout "output channels"
 // (pixel j of the group x filter co): W'[ky][j*Cout+co][c] = w[ky][c-j][co] for 0 <= c-j <= 2.  The
-// output [H][W/8][8*Cout] is byte-identical to NHWC [H][W][Cout], so the stock tcgen05 conv kernels run
+// output [H][W/8][8*Cout] is byte-identical to NHWC [H][W][Cout], so the stock wgmma conv kernel runs
 // it unchanged: each epilogue thread writes 8 pixels (8*Cout*2 contiguous bytes) instead of gathering a
-// 3x3 neighbourhood per pixel, which is what bound the CUDA-core k_conv_first (28% of its FMA pipe, 19%
-// of DRAM write bandwidth in profiles/r01_step_full_summary.md).  Tensor work grows 3.5x (16x8*Cout
+// 3x3 neighbourhood per pixel, which is what bounds the CUDA-core k_conv_first.  Tensor work grows 3.5x (16x8*Cout
 // MACs per tap row instead of 9*Cout per pixel) on a pipe that is otherwise idle in this layer.
 template <typename TI>
 __global__ void __launch_bounds__(256) k_first_view(const TI* __restrict__ img, int Hin, int Win, int Hnet, int Wg,
@@ -1995,7 +870,7 @@ static int first_view_prepare(sb_handle_s* h, SbModel* m, int oi, bool from_buff
   TcGroup g[1];
   g[0].dx = 0; g[0].n_taps = 3;
   for (int ky = 0; ky < 3; ++ky) g[0].taps[ky] = TcTap{ky, ky};
-  const int rc = make_launch(h, m, op, plan, 1, g, -1, 2, 3, 1, 0, 1, 0, 0, nullptr, &V);
+  const int rc = make_launch(h, m, op, plan, 1, g, -1, 2, 3, 1, 0, 1, 0, &V);
   if (rc) {
     cudaFree(plan->w16); cudaFree(plan->view_in); cudaFree(plan->view_bias);
     delete plan;
@@ -2011,7 +886,7 @@ static int first_view_prepare(sb_handle_s* h, SbModel* m, int oi, bool from_buff
 // 2o-2 .. 2o+4.  With the frame regrouped into 2x2 blocks ("space to depth": block (Y, X) holds pixels (2Y+py, 2X+px),
 // 4*Cin values, padded to 16 channels) those are blocks o-1 .. o+2, i.e. a 4x4 stride-1 convolution over the block grid
 // with W'[dy][dx][(py, px, c)][co] = w[2(dy+1)+py][2(dx+1)+px][c][co] (zero where the index reaches 7).  The view kernel
-// does InferenceLayer.preprocess (uint8 -> float * 1/255, zero pad) on the way; the stock streaming tcgen05 kernel runs
+// does InferenceLayer.preprocess (uint8 -> float * 1/255, zero pad) on the way; the stock wgmma conv kernel runs
 // the convolution (K = 16 taps x 16 channels = 256 instead of 147: the stem was on the CUDA cores before).
 template <typename TI>
 __global__ void __launch_bounds__(256) k_s2d_view(const TI* __restrict__ img, int Hin, int Win, int Cin, int Hs, int Ws,
@@ -2095,7 +970,7 @@ static int stem_view_prepare(sb_handle_s* h, SbModel* m, int oi) {
     g[dx].dx = dx - 1; g[dx].n_taps = 4;
     for (int dy = 0; dy < 4; ++dy) g[dx].taps[dy] = TcTap{dy, dy * 4 + dx};
   }
-  const int rc = make_launch(h, m, op, plan, 4, g, -1, 3, 16, 1, 0, 1, 0, 0, nullptr, &V);
+  const int rc = make_launch(h, m, op, plan, 4, g, -1, 3, 16, 1, 0, 1, 0, &V);
   if (rc) {
     cudaFree(plan->w16); cudaFree(plan->view_in);
     delete plan;
@@ -2109,7 +984,7 @@ bool sb_stem_view_can(const SbModel* m, int op_index) {
   return op_index >= 0 && op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] && m->tc_plans[op_index]->s2d;
 }
 
-// frame -> space-to-depth view -> tcgen05 4x4 conv
+// frame -> space-to-depth view -> 4x4 conv on the tensor cores
 int sb_stem_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
   SbConvTcPlan* plan = m->tc_plans[op_index];
   const size_t total = (size_t)B * plan->s2d_Hs * plan->s2d_Ws;
@@ -2129,7 +1004,7 @@ bool sb_first_view_can(const SbModel* m, int op_index) {
 }
 
 // First conv of a model whose frames are resized / converted first (input_scale != 1, rgb -> gray): the PREPROCESS kernel
-// runs as usual and the Toeplitz view is built from ITS one-channel fp16 output, so the layer still runs on tcgen05.
+// runs as usual and the Toeplitz view is built from ITS one-channel fp16 output, so the layer still runs on the tensor cores.
 bool sb_first_buffer_view_can(const SbModel* m, int op_index) {
   return op_index >= 0 && op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] && m->tc_plans[op_index]->view_in &&
          m->tc_plans[op_index]->from_buffer;
@@ -2146,7 +1021,7 @@ int sb_first_buffer_view_launch(sb_handle_s* h, SbModel* m, int op_index, int B)
   return sb_conv_tc_launch(h, m, op_index, B);
 }
 
-// frame -> Toeplitz view -> tcgen05 conv (the launch sb_conv_tc_autotune picked)
+// frame -> Toeplitz view -> tensor-core conv
 int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
   SbConvTcPlan* plan = m->tc_plans[op_index];
   const SbBuffer& ob = m->buffers[m->ops[op_index].out_buf()];
@@ -2161,6 +1036,27 @@ int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* f
   return sb_conv_tc_launch(h, m, op_index, B);
 }
 
+typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, TcParams);
+
+template <int KSTEPS>
+static ConvKernel conv_kernel_n(int N) {
+  switch (N) {
+    case 16: return k_conv_wg<KSTEPS, 16>;
+    case 32: return k_conv_wg<KSTEPS, 32>;
+    case 48: return k_conv_wg<KSTEPS, 48>;
+    case 64: return k_conv_wg<KSTEPS, 64>;
+    case 96: return k_conv_wg<KSTEPS, 96>;
+    case 128: return k_conv_wg<KSTEPS, 128>;
+    case 192: return k_conv_wg<KSTEPS, 192>;
+    default: return k_conv_wg<KSTEPS, 256>;
+  }
+}
+
+// the instantiation for an input-channel chunk of KC (K steps of 16 per staged slice) and a wg_n() tile width N
+static ConvKernel conv_kernel(int KC, int N) {
+  return KC == 16 ? conv_kernel_n<1>(N) : (KC == 32 ? conv_kernel_n<2>(N) : conv_kernel_n<4>(N));
+}
+
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);
 
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
@@ -2170,27 +1066,9 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   const bool split = m->precision == 2;          // physical extent of a conv's output slice: 3 x C_out fp16 planes
   static bool attr_set = false;
   if (!attr_set) {
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc<1, 7>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc<2, 7>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc<4, 7>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_persist<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_persist<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_persist<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_halo<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_prog<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_halo<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_prog<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_halo<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute(k_conv_tc_prog<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<1, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<2, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<4, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<1, 2, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<2, 2, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    SB_CUDA(h, cudaFuncSetAttribute((k_conv_tc_prog<4, 2, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
+    for (int kc : {16, 32, 64})
+      for (int n : {16, 32, 48, 64, 96, 128, 192, 256})
+        SB_CUDA(h, cudaFuncSetAttribute((const void*)conv_kernel(kc, n), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
     attr_set = true;
   }
   for (size_t oi = 0; oi < m->ops.size(); ++oi) {
@@ -2247,21 +1125,6 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
           }
           rc = make_launch(h, m, op, plan, ng, g, a == 0 ? -1 : 0, extra, 9, 2, a, 2, bx);
         }
-      if (!rc && !getenv("SB_DISABLE_FUSED_TCONV")) {
-        // all four phases from one staged activation box; two launches (a = 0 / a = 1) when 4 x N columns exceed TMEM
-        TcGroup g[1];
-        g[0].dx = 0; g[0].n_taps = 1; g[0].taps[0] = TcTap{0, 4};
-        const int N = std::min(plan->Cout_pad, 256);
-        int r2 = 0;
-        if (4 * N <= 512) r2 = make_launch(h, m, op, plan, 1, g, 0, 0, 9, 2, 0, 2, 0, 0xF, &plan->fused);
-        else {
-          r2 = make_launch(h, m, op, plan, 1, g, 0, 0, 9, 2, 0, 2, 0, 0x3, &plan->fused);
-          if (!r2) r2 = make_launch(h, m, op, plan, 1, g, 0, 0, 9, 2, 0, 2, 0, 0xC, &plan->fused);
-        }
-        if (r2 < 0) rc = r2;
-        if (r2 != 0) plan->fused.clear();
-        for (TcLaunch& F : plan->fused) F.use_persist = 2;
-      }
     }
     if (rc) { cudaFree(plan->w16); delete plan; return rc; }
     m->tc_plans[oi] = plan;
@@ -2317,212 +1180,39 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   return sb_conv_tc_autotune(h, m);
 }
 
-// Programmatic dependent launch (sb_tc_prims.cuh): every tcgen05 conv launch carries the attribute (its producer thread
-// waits on the grid dependency before the first activation load); a launch that owns its SMs (one CTA per SM) is padded to
-// the SM's whole shared memory and triggers its dependents right after its prologue, so that the next layer's CTAs set up
-// (barriers, TMEM, descriptors, resident filter bank) while this layer's last tiles drain.  SB_DISABLE_PDL=1 switches it off.
+// Programmatic dependent launch (sb_tc_prims.cuh): every conv launch carries the attribute (its producer thread waits on
+// the grid dependency before the first activation load); a launch that owns its SMs (one CTA per SM) is padded to the
+// SM's whole shared memory and triggers its dependents right after its prologue, so that the next layer's CTAs set up
+// (barriers, bias staging, descriptor prefetch) while this layer's last tiles drain.  SB_DISABLE_PDL=1 switches it off.
 static bool pdl_on() {
   static int v = -1;
   if (v < 0) v = getenv("SB_DISABLE_PDL") ? 0 : 1;
   return v != 0;
 }
 
-template <typename K>
-static void launch_tc(K kern, int grid_x, int grid_y, int grid_z, int threads, size_t smem, cudaStream_t stream, int cluster, bool exclusive,
-                      const CUtensorMap& a, const CUtensorMap& b, TcParams& P) {
+static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
+  TcParams P = L.P;
+  P.skip_out = skip_out;
+  size_t smem = L.smem;
+  P.pdl_trigger = (pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
+  if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing of the successor fits beside it
   cudaLaunchConfig_t cfg = {};
-  P.pdl_trigger = (pdl_on() && exclusive) ? 1 : 0;
-  if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing else fits on the SM: no successor CTA can queue on its TMEM
-  cfg.gridDim = dim3(grid_x, grid_y, grid_z); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute at[2];
-  int na = 0;
-  if (cluster > 1) {
-    at[na].id = cudaLaunchAttributeClusterDimension;
-    at[na].val.clusterDim.x = cluster; at[na].val.clusterDim.y = 1; at[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl_on()) {
-    at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = at; cfg.numAttrs = na;
-  cudaLaunchKernelEx(&cfg, kern, a, b, P);
+  cfg.gridDim = dim3(L.grid.x, L.grid.y, B); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, conv_kernel(P.KC, P.N), L.mapA, L.mapB, P);
 }
 
-static void launch_variant(sb_handle_s* h, TcLaunch& L, int B, int variant, cudaStream_t stream, int skip_out = 0) {
-  if (variant >= 2) {
-    TcLaunch::Halo& HC = L.halo[variant - 2];
-    TcParams P = HC.P;
-    P.skip_out = skip_out;
-    P.n_tiles_total = P.tiles_per_img * B;
-    const int grid = std::max(1, std::min(P.n_tiles_total, h->sm_count * HC.occ));
-    if (getenv("SB_DEBUG_LAUNCH")) fprintf(stderr, "[halo %dx%d] KC=%d N=%d stages=%d cols=%d occ=%d grid=%d slots=%d smem=%zu tiles=%d thr=%d\n", P.sub_x, P.sub_y, P.KC, P.N, P.n_stages, P.tmem_cols, HC.occ, grid, P.n_a_slots, HC.smem, P.n_tiles_total, HC.threads);
-    const bool excl = HC.occ == 1;
-    if (HC.mc) {
-      // clusters of 2: the two CTAs of a cluster walk tiles (t, t + 1), (t + g, t + 1 + g), ... and must make the same number
-      // of steps -> an even grid over an even tile count (cluster ranks are consecutive block indices)
-      const int g2 = std::min(P.n_tiles_total, h->sm_count) & ~1;
-      if (g2 < 2 || (P.n_tiles_total & 1)) {      // odd tile count: the unicast twin
-        launch_variant(h, L, B, variant - 1, stream, skip_out);
-        return;
-      }
-      if (HC.mc == 4) {
-        switch (P.KC) {
-          case 16: launch_tc(k_conv_tc_prog<1, 2, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-          case 32: launch_tc(k_conv_tc_prog<2, 2, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-          default: launch_tc(k_conv_tc_prog<4, 2, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-        }
-        return;
-      }
-      switch (P.KC) {
-        case 16: launch_tc(k_conv_tc_prog<1, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-        case 32: launch_tc(k_conv_tc_prog<2, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-        default: launch_tc(k_conv_tc_prog<4, 2>, g2, 1, 1, HC.threads, HC.smem, stream, 2, true, HC.map, HC.mapBpiece, P); break;
-      }
-      return;
-    }
-    if (HC.prog) {
-      switch (P.KC) {
-        case 16: launch_tc(k_conv_tc_prog<1>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-        case 32: launch_tc(k_conv_tc_prog<2>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-        default: launch_tc(k_conv_tc_prog<4>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-      }
-    } else {
-      switch (P.KC) {
-        case 16: launch_tc(k_conv_tc_halo<1>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-        case 32: launch_tc(k_conv_tc_halo<2>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-        default: launch_tc(k_conv_tc_halo<4>, grid, 1, 1, HC.threads, HC.smem, stream, 1, excl, HC.map, L.mapB, P); break;
-      }
-    }
-  } else if (variant == 1) {
-    TcParams P = L.PP;
-    P.skip_out = skip_out;
-    P.n_tiles_total = P.tiles_per_img * B;
-    const int grid = std::max(1, std::min(P.n_tiles_total, h->sm_count * L.occ));
-    if (getenv("SB_DEBUG_LAUNCH")) fprintf(stderr, "[persist] KC=%d N=%d stages=%d cols=%d occ=%d grid=%d slots=%d smem=%zu tiles=%d\n", P.KC, P.N, P.n_stages, P.tmem_cols, L.occ, grid, P.n_a_slots, L.smem_p, P.n_tiles_total);
-    const bool excl = L.occ == 1;
-    switch (P.KC) {
-      case 16: launch_tc(k_conv_tc_persist<1>, grid, 1, 1, 192, L.smem_p, stream, 1, excl, L.mapA, L.mapB, P); break;
-      case 32: launch_tc(k_conv_tc_persist<2>, grid, 1, 1, 192, L.smem_p, stream, 1, excl, L.mapA, L.mapB, P); break;
-      default: launch_tc(k_conv_tc_persist<4>, grid, 1, 1, 192, L.smem_p, stream, 1, excl, L.mapA, L.mapB, P); break;
-    }
-  } else {
-    dim3 g = L.grid;
-    g.z = B;
-    L.P.skip_out = skip_out;
-    bool wide = L.P.n_groups > 3;                      // 5x5 / 7x7 (and the 4x4 space-to-depth stem): loops unrolled to 7
-    for (int gi = 0; gi < L.P.n_groups; ++gi) wide |= L.P.groups[gi].n_taps > 3;
-    const bool excl = L.smem >= 114 * 1024;            // already one CTA per SM
-    if (wide) {
-      switch (L.P.KC) {
-        case 16: launch_tc((k_conv_tc<1, 7>), g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-        case 32: launch_tc((k_conv_tc<2, 7>), g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-        default: launch_tc((k_conv_tc<4, 7>), g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-      }
-      return;
-    }
-    switch (L.P.KC) {
-      case 16: launch_tc(k_conv_tc<1>, g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-      case 32: launch_tc(k_conv_tc<2>, g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-      default: launch_tc(k_conv_tc<4>, g.x, g.y, g.z, 128, L.smem, stream, 1, excl, L.mapA, L.mapB, L.P); break;
-    }
-  }
-}
-
-static int launch_plan(sb_handle_s* h, SbConvTcPlan* plan, int B, bool fused);
-
-// Pick, per launch, the fastest kernel variant by timing them on the device (buffers are already
-// allocated; their contents do not matter for timing); then, for transposed convs, the fused
-// single-launch form against the four forked per-phase launches.
+// Picks, for a first layer with a Toeplitz view, the faster of the view + tensor-core conv and k_conv_first, and for the
+// first encoder block the fused k_conv01 or the separate launches, by timing both forms on the device (buffers are
+// already allocated; their contents do not matter for timing).
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
-  const char* force = getenv("SB_FORCE_VARIANT");
-  const bool halo_ok = !getenv("SB_DISABLE_HALO");
-  auto avail = [&](const TcLaunch& L, int v) { return v == 0 || (v == 1 && L.has_persist) || (v >= 2 && v - 2 < L.n_halo && halo_ok); };
-  if (force || getenv("SB_DISABLE_AUTOTUNE")) {
-    const int want = force ? atoi(force) : 1;
-    m->conv01_enabled = m->conv01 && (getenv("SB_FORCE_CONV01") ? atoi(getenv("SB_FORCE_CONV01")) != 0 : true);
-    for (SbConvTcPlan* plan : m->tc_plans)
-      if (plan) {
-        for (TcLaunch& L : plan->launches) L.use_persist = avail(L, want) ? want : (avail(L, 1) && !force ? 1 : 0);
-        plan->use_fused = !plan->fused.empty() && (getenv("SB_FORCE_FUSED_TCONV") != nullptr);
-        // SB_FORCE_FUSED_TCONV=2: the cluster twin of the fused transposed conv where it has one
-        const bool twin = getenv("SB_FORCE_FUSED_TCONV") && atoi(getenv("SB_FORCE_FUSED_TCONV")) == 2;
-        for (TcLaunch& F : plan->fused) F.use_persist = (twin && F.n_halo >= 2 && F.halo[1].mc) ? 3 : 2;
-      }
-    return 0;
-  }
-  // SB_TUNE_LOAD=<file>: reuse the picks a previous (un-profiled) run saved with SB_TUNE_SAVE, so a run
-  // under ncu (where event timings are meaningless) launches exactly the kernels the bench timed.
-  if (const char* lf = getenv("SB_TUNE_LOAD")) {
-    if (FILE* f = fopen(lf, "r")) {
-      int oi, li, pick;
-      int applied = 0;
-      while (fscanf(f, "%d %d %d", &oi, &li, &pick) == 3) {
-        if (oi < 0 || oi >= (int)m->tc_plans.size() || !m->tc_plans[oi]) continue;
-        SbConvTcPlan* plan = m->tc_plans[oi];
-        if (li == -3) { m->conv01_enabled = m->conv01 && pick != 0; ++applied; continue; }
-        if (li == -2) { plan->view_enabled = pick != 0; ++applied; continue; }
-        if (li < 0) {
-          plan->use_fused = pick != 0 && !plan->fused.empty();
-          for (TcLaunch& F : plan->fused) F.use_persist = (pick == 2 && F.n_halo >= 2) ? 3 : 2;
-          ++applied;
-          continue;
-        }
-        if (li >= (int)plan->launches.size()) continue;
-        TcLaunch& L = plan->launches[li];
-        L.use_persist = avail(L, pick) ? pick : 0;
-        ++applied;
-      }
-      fclose(f);
-      if (applied > 0) return 0;
-    }
-  }
   cudaEvent_t e0, e1;
   SB_CUDA(h, cudaEventCreate(&e0));
   SB_CUDA(h, cudaEventCreate(&e1));
   const bool dbg = getenv("SB_DEBUG") != nullptr;
-  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
-    SbConvTcPlan* plan = m->tc_plans[oi];
-    if (!plan) continue;
-    for (TcLaunch& L : plan->launches) {
-      if (!L.has_persist && L.n_halo == 0) continue;
-      float best[10] = {1e30f, 1e30f, 1e30f, 1e30f, 1e30f, 1e30f, 1e30f, 1e30f, 1e30f, 1e30f};
-      for (int v = 0; v < 10; ++v) {
-        if (!avail(L, v)) continue;
-        for (int rep = 0; rep < 3; ++rep) {
-          cudaEventRecord(e0, h->stream);
-          launch_variant(h, L, m->B, v, h->stream, plan->out_dead ? 1 : 0);
-          const cudaError_t le = cudaGetLastError();         // launch-configuration errors: the variant is unusable
-          cudaEventRecord(e1, h->stream);
-          cudaError_t e = cudaStreamSynchronize(h->stream);
-          if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (variant %d) failed: %s", v, cudaGetErrorString(e));
-          if (le != cudaSuccess) {
-            if (dbg) fprintf(stderr, "[sb_conv_tc] op %zu variant %d cannot launch: %s\n", oi, v, cudaGetErrorString(le));
-            if (v >= 2) { L.n_halo = std::min(L.n_halo, v - 2); } else if (v == 1) { L.has_persist = false; }
-            best[v] = 1e30f;
-            break;
-          }
-          float ms = 0.f;
-          cudaEventElapsedTime(&ms, e0, e1);
-          if (rep > 0) best[v] = std::min(best[v], ms);
-        }
-      }
-      int pick = 0;
-      for (int v = 1; v < 10; ++v) if (best[v] < best[pick]) pick = v;
-      L.use_persist = pick;
-      if (dbg) {
-        fprintf(stderr, "[sb_conv_tc] op %zu Cin=%d N=%d %dx%d: stream %.1f, persist %.1f (occ %d, %d slots)", oi, L.P.n_chunks * L.P.KC,
-                L.P.N, L.P.H, L.P.W, best[0] * 1e3f, best[1] * 1e3f, L.occ, L.PP.n_a_slots);
-        for (int i = 0; i < L.n_halo; ++i)
-          fprintf(stderr, ", halo%dx%d%s%s %.1f (occ %d, %d slots, %d stages)", L.halo[i].P.sub_x, L.halo[i].P.sub_y,
-                  L.halo[i].P.w_stream ? "w" : "", L.halo[i].mc == 4 ? "-2cta" : (L.halo[i].mc ? "-mc2" : ""), best[2 + i] * 1e3f, L.halo[i].occ, L.halo[i].P.n_a_slots,
-                  L.halo[i].P.n_stages);
-        fprintf(stderr, " us -> %d\n", pick);
-      }
-    }
-  }
-  // first layer: Toeplitz tensor-core form (view kernel + the variant picked above) against k_conv_first
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
     if (!plan || !plan->view_in || plan->s2d || plan->from_buffer || !m->frames_dev) continue;
@@ -2542,7 +1232,7 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
       }
     plan->view_enabled = best[1] < best[0];
     if (const char* fv = getenv("SB_FORCE_FIRST_VIEW")) plan->view_enabled = atoi(fv) != 0;
-    if (dbg) fprintf(stderr, "[sb_conv_tc] op %zu first layer: k_conv_first %.1f us, Toeplitz view + tcgen05 %.1f us -> %s\n", oi,
+    if (dbg) fprintf(stderr, "[sb_conv_tc] op %zu first layer: k_conv_first %.1f us, Toeplitz view + wgmma %.1f us -> %s\n", oi,
                      best[0] * 1e3f, best[1] * 1e3f, plan->view_enabled ? "view" : "direct");
   }
   // fused first block (k_conv01) against its two separate launches (whatever forms were just picked for them)
@@ -2571,58 +1261,12 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
     if (dbg) fprintf(stderr, "[sb_conv_tc] first block: conv0 + conv1 launches %.1f us, fused k_conv01 %.1f us -> %s\n", best[0] * 1e3f,
                      best[1] * 1e3f, m->conv01_enabled ? "fused" : "separate");
   }
-  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
-    SbConvTcPlan* plan = m->tc_plans[oi];
-    if (!plan || plan->fused.empty()) continue;
-    float best[3] = {1e30f, 1e30f, 1e30f};             // 4 phase launches | fused | fused with cluster-multicast weight slices
-    bool has_mc = true;
-    for (TcLaunch& F : plan->fused) has_mc &= F.n_halo >= 2 && F.halo[1].mc != 0;
-    for (int f = 0; f < (has_mc ? 3 : 2); ++f)
-      for (int rep = 0; rep < 4; ++rep) {
-        for (TcLaunch& F : plan->fused) F.use_persist = f == 2 ? 3 : 2;
-        cudaEventRecord(e0, h->stream);
-        int rc = launch_plan(h, plan, m->B, f >= 1);
-        if (rc) return rc;
-        cudaEventRecord(e1, h->stream);
-        cudaError_t e = cudaStreamSynchronize(h->stream);
-        if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (tconv, fused %d) failed: %s", f, cudaGetErrorString(e));
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (rep > 0) best[f] = std::min(best[f], ms);
-      }
-    const bool mc_wins = best[2] < best[1];
-    for (TcLaunch& F : plan->fused) F.use_persist = mc_wins ? 3 : 2;
-    plan->use_fused = std::min(best[1], best[2]) < best[0];
-    if (getenv("SB_FORCE_FUSED_TCONV")) plan->use_fused = atoi(getenv("SB_FORCE_FUSED_TCONV")) != 0;
-    if (dbg) {
-      const TcParams& F = plan->fused[0].halo[0].P;
-      fprintf(stderr, "[sb_conv_tc] op %zu tconv Cin=%d N=%d: 4 phase launches %.1f us, fused x%zu (%s, %d stages, %d slots) %.1f us -> %s\n", oi,
-              F.n_chunks * F.KC, F.N, best[0] * 1e3f, plan->fused.size(), F.w_stream ? "streamed weights" : "resident weights", F.n_stages,
-              F.n_a_slots, best[1] * 1e3f, plan->use_fused ? (mc_wins ? "fused-twin" : "fused") : "phases");
-      if (has_mc) fprintf(stderr, "[sb_conv_tc] op %zu tconv fused, cluster twin (2-CTA pair / multicast): %.1f us\n", oi, best[2] * 1e3f);
-    }
-  }
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  // (a process may configure several models -- bench.py builds the fp16 model, then the precision-2 model for its strict
-  //  block: only the fp16 tensor-core model's picks are recorded, they are what SB_TUNE_LOAD replays under ncu)
-  if (const char* sf = m->precision == 0 ? getenv("SB_TUNE_SAVE") : nullptr) {
-    if (FILE* f = fopen(sf, "w")) {
-      for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
-        SbConvTcPlan* plan = m->tc_plans[oi];
-        if (!plan) continue;
-        for (size_t li = 0; li < plan->launches.size(); ++li) fprintf(f, "%zu %zu %d\n", oi, li, plan->launches[li].use_persist);
-        if (!plan->fused.empty()) fprintf(f, "%zu -1 %d\n", oi, plan->use_fused ? (plan->fused[0].use_persist == 3 ? 2 : 1) : 0);
-        if (plan->view_in) fprintf(f, "%zu -2 %d\n", oi, plan->view_enabled ? 1 : 0);
-        if (m->conv01 && (int)oi == sb_conv01_conv1_op(m)) fprintf(f, "%zu -3 %d\n", oi, m->conv01_enabled ? 1 : 0);
-      }
-      fclose(f);
-    }
-  }
   return 0;
 }
 
-// 1x1 fp32 heads on k_head_1x1 (HBM-bound; see the kernel) instead of the tcgen05 kernels.  SB_DISABLE_HEAD_KERNEL=1 reverts.
+// 1x1 fp32 heads on k_head_1x1 (HBM-bound; see the kernel) instead of the implicit-GEMM conv kernel.  SB_DISABLE_HEAD_KERNEL=1 reverts.
 static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan) {
   if (getenv("SB_DISABLE_HEAD_KERNEL")) return false;
   const SbBuffer& ib = m->buffers[op.in_buf()];
@@ -2679,122 +1323,12 @@ static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
 int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
   SbConvTcPlan* plan = m->tc_plans[op_index];
   if (head_kernel_ok(m, m->ops[op_index], plan)) return head_launch(h, m, m->ops[op_index], plan, B);
-  plan->skip_now = plan->out_dead && !m->keep_dead_stores;
-  return launch_plan(h, plan, B, plan->use_fused);
-}
-
-static int launch_plan(sb_handle_s* h, SbConvTcPlan* plan, int B, bool fused) {
-  if (fused) {
-    for (TcLaunch& L : plan->fused) {
-      launch_variant(h, L, B, L.use_persist >= 2 ? L.use_persist : 2, h->stream);
-      SB_CHECK_LAUNCH(h);
-    }
-    return 0;
-  }
-  const size_t n = plan->launches.size();
-  // with programmatic dependent launch the phases run back to back on the launching stream: each phase's CTAs start as
-  // the previous phase's SMs drain, which fills the GPU like the fork did, without 3 event records + 6 stream waits per
-  // transposed conv on the host's launch path (same device time, +3 % end to end; SB_FORCE_FORK=1 restores the fork)
-  if (n == 1 || getenv("SB_DISABLE_FORK") || (pdl_on() && !getenv("SB_FORCE_FORK"))) {
-    for (TcLaunch& L : plan->launches) {
-      launch_variant(h, L, B, L.use_persist, h->stream, plan->skip_now ? 1 : 0);
-      SB_CHECK_LAUNCH(h);
-    }
-    return 0;
-  }
-  // the sub-pixel phases of a transposed conv are independent: fork them onto side streams so that
-  // their (individually small) grids fill the GPU together, then join
-  SB_CUDA(h, cudaEventRecord(h->fork_ev, h->stream));
-  for (size_t i = 0; i < n; ++i) {
-    cudaStream_t st = (i == 0) ? h->stream : h->aux_stream[(i - 1) % 3];
-    if (i > 0) SB_CUDA(h, cudaStreamWaitEvent(st, h->fork_ev, 0));
-    launch_variant(h, plan->launches[i], B, plan->launches[i].use_persist, st);
+  const int skip = plan->out_dead && !m->keep_dead_stores;
+  // the sub-pixel phases of a transposed conv run back to back on the launching stream: under programmatic dependent
+  // launch each phase's CTAs start as the previous phase's SMs drain
+  for (TcLaunch& L : plan->launches) {
+    launch_conv(L, B, h->stream, skip);
     SB_CHECK_LAUNCH(h);
-    if (i > 0) SB_CUDA(h, cudaEventRecord(h->join_ev[(i - 1) % 3], st));
   }
-  for (size_t i = 1; i < n; ++i) SB_CUDA(h, cudaStreamWaitEvent(h->stream, h->join_ev[(i - 1) % 3], 0));
   return 0;
-}
-
-// ---- first layer on the tensor cores ----------------------------------------------------------
-struct SbFirstTc {
-  __half* wk = nullptr;   // [N][KPAD]
-  TcParams P;
-  int kpad = 16;
-};
-static std::vector<std::pair<const SbModel*, SbFirstTc*>> g_first_plans;
-
-bool sb_conv_first_tc_ok(const SbModel* m, const SbOp& cv) {
-  // same speed as the CUDA-core kernel (both are bound by the 16-channel output write); off by default
-  // because it rounds the input pixel to fp16 before the MAC.  SB_ENABLE_FIRST_TC=1 turns it on.
-  if (!getenv("SB_ENABLE_FIRST_TC") || m->precision != 0) return false;
-  const int co = cv.out_C();
-  return co == 16 || co == 32 || co == 64;
-}
-
-int sb_conv_first_tc_launch(sb_handle_s* h, SbModel* m, const SbOp& op, const void* frames_dev, int frames_are_u8, int B) {
-  SbFirstTc* fp = nullptr;
-  for (auto& pr : g_first_plans) if (pr.first == m) fp = pr.second;
-  const SbBuffer& ob = m->buffers[op.out_buf()];
-  const int Cin = op.in_C(), N = op.out_C();
-  if (!fp) {
-    fp = new SbFirstTc();
-    fp->kpad = Cin == 1 ? 16 : 32;
-    std::vector<__half> wk((size_t)N * fp->kpad, __float2half(0.f));
-    const float* w = m->weights_host.data() + op.w_off();     // [9][Cin][Cout]
-    for (int t = 0; t < 9; ++t)
-      for (int ci = 0; ci < Cin; ++ci)
-        for (int co = 0; co < N; ++co) wk[(size_t)co * fp->kpad + t * Cin + ci] = __float2half_rn(w[((size_t)t * Cin + ci) * N + co]);
-    SB_CUDA(h, cudaMalloc((void**)&fp->wk, wk.size() * sizeof(__half)));
-    SB_CUDA(h, cudaMemcpy(fp->wk, wk.data(), wk.size() * sizeof(__half), cudaMemcpyHostToDevice));
-    TcParams& P = fp->P;
-    memset(&P, 0, sizeof(P));
-    P.H = ob.H; P.W = ob.W; P.N = N; P.Cout = N; P.tw = TW;
-    P.idesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    int cols = 32;
-    while (cols < 2 * N) cols <<= 1;      // two accumulator stages
-    P.tmem_cols = cols;
-    P.out = ob.dev; P.out_f32 = 0; P.out_H = ob.H; P.out_W = ob.W; P.out_Ctot = ob.C; P.out_coff = op.out_coff();
-    P.oy_mul = 1; P.ox_mul = 1;
-    P.bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-    P.relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-    if (op.pool_buf() >= 0 && N % 16 == 0 && ob.H % 2 == 0 && ob.W % 2 == 0) {
-      const SbBuffer& pb = m->buffers[op.pool_buf()];
-      if (pb.C % 8 == 0 && op.pool_coff() % 8 == 0) { P.pool_out = pb.dev; P.pool_H = pb.H; P.pool_W = pb.W; P.pool_Ctot = pb.C; P.pool_coff = op.pool_coff(); }
-    }
-    g_first_plans.push_back({m, fp});
-  }
-  fp->P.out = ob.dev;
-  const int tiles_x = (ob.W + TW - 1) / TW, tiles_y = (ob.H + TH - 1) / TH;
-  const int n_tiles = tiles_x * tiles_y * B;
-  size_t smem = 1024 + 2 * 128 * 64 + 64 * 64 + 64 + 3 * 64 * sizeof(float) + 64;
-  const int occ = std::min(512 / fp->P.tmem_cols, 8);    // 64 regs x 128 threads -> at most 8 co-resident CTAs
-  if (occ < 8) {                                          // keep co-residency within what TMEM serves without waiting
-    smem = std::max(smem, (size_t)(227 * 1024) / occ - 2048);
-    static bool attr_done = false;
-    if (!attr_done) {
-      cudaFuncSetAttribute(k_conv_first_tc<unsigned char, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024);
-      cudaFuncSetAttribute(k_conv_first_tc<unsigned char, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024);
-      cudaFuncSetAttribute(k_conv_first_tc<float, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024);
-      cudaFuncSetAttribute(k_conv_first_tc<float, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 120 * 1024);
-      attr_done = true;
-    }
-  }
-  const int grid = std::max(1, std::min(n_tiles, h->sm_count * occ));
-#define LAUNCH_FIRST(TI, CIN_) k_conv_first_tc<TI, CIN_><<<grid, 128, smem, h->stream>>>((const TI*)frames_dev, m->Hin, m->Win, ob.H, ob.W, tiles_x, tiles_x * tiles_y, n_tiles, fp->wk, frames_are_u8, fp->P)
-  if (frames_are_u8) { if (Cin == 1) LAUNCH_FIRST(unsigned char, 1); else LAUNCH_FIRST(unsigned char, 3); }
-  else { if (Cin == 1) LAUNCH_FIRST(float, 1); else LAUNCH_FIRST(float, 3); }
-#undef LAUNCH_FIRST
-  SB_CHECK_LAUNCH(h);
-  return 0;
-}
-
-void sb_conv_first_tc_release(const SbModel* m) {
-  for (size_t i = 0; i < g_first_plans.size(); ++i)
-    if (g_first_plans[i].first == m) {
-      if (g_first_plans[i].second->wk) cudaFree(g_first_plans[i].second->wk);
-      delete g_first_plans[i].second;
-      g_first_plans.erase(g_first_plans.begin() + i);
-      return;
-    }
 }

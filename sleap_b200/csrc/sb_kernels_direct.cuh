@@ -200,7 +200,6 @@ __global__ void __launch_bounds__(256) k_conv_first(const TI* __restrict__ img, 
       }
       continue;
     }
-    const bool wide = (COUT % 16 == 0) && (((out_Ctot | out_coff) & 15) == 0);     // 32-byte aligned rows
 #pragma unroll
     for (int q = 0; q < COUT / 8; ++q) {
       __align__(16) __half2 h[4];
@@ -210,21 +209,7 @@ __global__ void __launch_bounds__(256) k_conv_first(const TI* __restrict__ img, 
         if (relu) { a = fmaxf(a, 0.f); c2 = fmaxf(c2, 0.f); }
         h[j] = __floats2half2_rn(a, c2);
       }
-      if (wide && (q & 1) == 0 && q + 1 < COUT / 8) {
-        __align__(16) __half2 h2[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float a = acc[p][8 * (q + 1) + 2 * j], c2 = acc[p][8 * (q + 1) + 2 * j + 1];
-          if (relu) { a = fmaxf(a, 0.f); c2 = fmaxf(c2, 0.f); }
-          h2[j] = __floats2half2_rn(a, c2);
-        }
-        const uint32_t* w0 = reinterpret_cast<const uint32_t*>(h);
-        const uint32_t* w1 = reinterpret_cast<const uint32_t*>(h2);
-        asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(po + 8 * q), "r"(w0[0]), "r"(w0[1]),
-                     "r"(w0[2]), "r"(w0[3]), "r"(w1[0]), "r"(w1[1]), "r"(w1[2]), "r"(w1[3]) : "memory");
-      } else if (!(wide && (q & 1) == 1)) {
-        reinterpret_cast<uint4*>(po)[q] = *reinterpret_cast<uint4*>(h);
-      }
+      reinterpret_cast<uint4*>(po)[q] = *reinterpret_cast<uint4*>(h);
     }
   }
 }

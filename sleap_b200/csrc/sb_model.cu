@@ -262,7 +262,7 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
     if ((int)oi == m->guard_op && h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(s, h->post_done_ev, 0));
     if (oi < m->skip_op.size() && m->skip_op[oi]) continue;     // 2x2 max-pool fused into the producing conv
     if ((int)oi == fused_conv1) continue;                       // ran inside the fused first block
-    if ((int)oi == fused_stem) {                                // 7x7 s2 stem: frame -> space-to-depth view -> tcgen05
+    if ((int)oi == fused_stem) {                                // 7x7 s2 stem: frame -> space-to-depth view -> tensor cores
       int rc = sb_stem_view_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
       if (rc) return rc;
       continue;
@@ -275,11 +275,6 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
     }
     if ((int)oi == fused_first && sb_first_view_can(m, (int)oi)) {
       int rc = sb_first_view_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
-      if (rc) return rc;
-      continue;
-    }
-    if ((int)oi == fused_first && sb_conv_first_tc_ok(m, op)) {
-      int rc = sb_conv_first_tc_launch(h, m, op, frames_dev, frames_are_u8, B);
       if (rc) return rc;
       continue;
     }

@@ -121,7 +121,7 @@ int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B);
 
 // first conv fused with the PREPROCESS op before it (sb_model.cu): conv op index or -1
 int sb_first_fusion_op(const SbModel* m, size_t pre_index);
-// first layer as a Toeplitz GEMM on the stock tcgen05 conv kernels (sb_conv_tc.cu)
+// first layer as a Toeplitz GEMM on the stock tensor-core conv kernel (sb_conv_tc.cu)
 bool sb_first_view_can(const SbModel* m, int op_index);
 int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
 bool sb_first_buffer_view_can(const SbModel* m, int op_index);
@@ -139,7 +139,3 @@ void sb_conv01_release(SbModel* m);
 bool sb_conv01_can(const SbModel* m, int conv0_op);
 int sb_conv01_conv1_op(const SbModel* m);
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);
-
-// first layer fused with preprocessing on the tensor cores (sb_conv_tc.cu)
-bool sb_conv_first_tc_ok(const SbModel* m, const SbOp& conv);
-int sb_conv_first_tc_launch(sb_handle_s* h, SbModel* m, const SbOp& op, const void* frames_dev, int frames_are_u8, int B);

@@ -1,4 +1,4 @@
-// Post-processing kernels of the SLEAP inference path for sm_100a: local / global peak finding
+// Post-processing kernels of the SLEAP inference path for sm_90a: local / global peak finding
 // with sub-pixel refinement, PAF line scoring, per-edge assignment and greedy instance grouping.
 //
 // Compiled with -fmad=false: the reference computes these quantities in float32 with separately
@@ -161,8 +161,8 @@ __global__ void __launch_bounds__(256) k_local_scan(const T* __restrict__ cms, i
 }
 
 // Vectorised scan (float maps whose rows are a multiple of 4 elements): a pure streaming pass, no block barrier.
-// Round 1's k_local_scan moved 27 MB in 60 us (0.45 TB/s): one scalar load in flight per thread and a
-// __syncthreads_count per 256 elements.  Here every thread keeps UN 16-byte loads in flight, elements above the
+// A scan with one scalar load in flight per thread and a __syncthreads_count per 256 elements is latency bound.
+// Here every thread keeps UN 16-byte loads in flight, elements above the
 // threshold (a fraction of a percent of the map) take the 8-neighbour slow path, and a peak is appended to its
 // chunk's list with one atomicAdd -- the list is therefore UNORDERED inside a chunk; k_local_emit restores the
 // tf.where order by ranking the (unique) flat indices of a chunk.  chunk_cap can never overflow: strict

@@ -2,7 +2,7 @@
 
 Same function names and argument order.  tf.RaggedTensors become Python lists of per-sample
 NumPy arrays.  Scoring, matching (SciPy-compatible rectangular LSAP) and greedy grouping run as
-sm_100a kernels behind the C-ABI; host code only does index bookkeeping and edge ordering.
+sm_90a kernels behind the C-ABI; host code only does index bookkeeping and edge ordering.
 """
 from typing import List, Tuple
 

@@ -1,7 +1,7 @@
 """Drop-in for ``sleap.nn.peak_finding`` (reference: sleap/nn/peak_finding.py).
 
 Same function names, argument order and return tuples; inputs/outputs are NumPy arrays
-(the reference returns tf.Tensors).  Every function runs as sm_100a CUDA kernels behind the
+(the reference returns tf.Tensors).  Every function runs as sm_90a CUDA kernels behind the
 C-ABI (sleap_b200/csrc/sb_post.cu); nothing is computed on the CPU.
 """
 from ctypes import c_int32, byref

@@ -1,8 +1,8 @@
 """Generates the committed fixtures under tests/golden/ from the reference's own test data.
 
-Run in the build container only (needs /root/reference; the GPU box does not have it):
+Needs a checkout of the reference project (its tests/data directory):
 
-    python tests/golden/make_reference_fixtures.py
+    python tests/golden/make_reference_fixtures.py <reference checkout>
 
 Sources (all data files, no reference code is imported or copied):
   tests/data/models/*/best_model.h5 + training_config.json   (trained fixture models used by
@@ -13,12 +13,15 @@ Sources (all data files, no reference code is imported or copied):
   tests/data/json_format_v1/centered_pair_low_quality.mp4 frame 0, tests/data/videos/small_robot.mp4 frames
 
 Outputs:
+  reference_data/<path>.gz             gzip copies of the data files the CPU tests read directly (.h5 / .slp)
   models/<name>/fixture_config.json    the training config reduced to the keys the inference path reads
   models/<name>/best_model.npz         float32 weights {layer/param} read out of best_model.h5 (optimizer state dropped)
   frames_minimal_instance.npz, frames_robot.npz   uint8 frames + ground-truth points (frame, instance, node, xy)
 """
+import gzip
 import json
 import os
+import shutil
 import sys
 
 import cv2
@@ -29,7 +32,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from sleap_b200.io import h5lite                      # noqa: E402
 from sleap_b200.nn.model import load_weights_h5, save_weights_npz   # noqa: E402
 
-REF = "/root/reference/tests/data"
+REF = None        # <reference checkout>/tests/data, set by main() from the command line
 MODELS = {
     "minimal_instance.bottomup": "minimal_instance.UNet.bottomup",
     "minimal_instance.centroid": "minimal_instance.UNet.centroid",
@@ -91,6 +94,10 @@ def read_frames(path, idxs, grayscale):
 
 
 def main():
+    global REF
+    if len(sys.argv) != 2 or not os.path.isdir(os.path.join(sys.argv[1], "tests", "data")):
+        sys.exit("usage: python tests/golden/make_reference_fixtures.py <reference checkout (with tests/data)>")
+    REF = os.path.join(sys.argv[1], "tests", "data")
     for short, name in MODELS.items():
         src, dst = os.path.join(REF, "models", name), os.path.join(HERE, "models", short)
         os.makedirs(dst, exist_ok=True)
@@ -131,6 +138,14 @@ def main():
     np.savez_compressed(os.path.join(HERE, "frames_tracks_2node.npz"), images=frames, points_gt=np.stack(rows)[None], frame_idx=np.asarray(idxs),
                         track_names=np.asarray(gt_tracks(slp, 1)), video_json=np.asarray(json.dumps(vid)))
     print("tracks_2node", frames.shape, np.stack(rows).shape, idxs, gt_tracks(slp, 1), vid)
+
+    # files the CPU tests read as written by h5py (tests/reference_models.py: ref_path)
+    for rel in ("models/minimal_robot.UNet.single_instance/best_model.h5", "slp_hdf5/minimal_instance.slp",
+                "slp_hdf5/small_robot_minimal.slp", "slp_hdf5/dance.mp4.labels.slp"):
+        dst = os.path.join(HERE, "reference_data", rel + ".gz")
+        os.makedirs(os.path.dirname(dst), exist_ok=True)
+        with open(os.path.join(REF, rel), "rb") as f, gzip.GzipFile(dst, "wb", 9, mtime=0) as g:
+            shutil.copyfileobj(f, g)
 
 
 if __name__ == "__main__":

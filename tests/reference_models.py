@@ -2,8 +2,12 @@
 
 Fixtures under tests/golden/ are made by tests/golden/make_reference_fixtures.py from the
 reference's own test data; the assertions restate tests/nn/test_inference.py:585-800."""
+import atexit
+import gzip
 import json
 import os
+import shutil
+import tempfile
 
 import numpy as np
 
@@ -33,13 +37,22 @@ def frames(name):
     return z["images"], z["points_gt"]
 
 
-REF_DATA = "/root/reference/tests/data"       # present in the build container only; never read by the -m gpu tests
+REF_DATA = os.path.join(GOLDEN, "reference_data")   # gzip copies of data files of the reference's tests/data
+_unpacked = None
 
 
 def ref_path(*parts):
-    """A data file of the reference checkout, or None where the checkout does not exist (GPU box)."""
-    p = os.path.join(REF_DATA, *parts)
-    return p if os.path.exists(p) else None
+    """A data file of the reference's test data, decompressed (once per process) into a temporary directory."""
+    global _unpacked
+    if _unpacked is None:
+        _unpacked = tempfile.mkdtemp(prefix="sb_refdata_")
+        atexit.register(shutil.rmtree, _unpacked, True)
+    dst = os.path.join(_unpacked, *parts)
+    if not os.path.exists(dst):
+        os.makedirs(os.path.dirname(dst), exist_ok=True)
+        with gzip.open(os.path.join(REF_DATA, *parts) + ".gz", "rb") as f, open(dst, "wb") as g:
+            shutil.copyfileobj(f, g)
+    return dst
 
 
 def labels_minimal_instance():

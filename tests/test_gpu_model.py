@@ -79,7 +79,7 @@ def test_unet_forward_resize_and_rgb():
 
 def test_unet_forward_resize_fp16_first_layer_on_tensor_cores():
     """input_scale != 1 (and rgb -> gray): PREPROCESS runs as its own kernel and the first 3x3 conv takes the Toeplitz
-    tcgen05 form from the preprocessed one-channel buffer (sb_first_buffer_view_launch) instead of k_conv_direct."""
+    tensor-core form from the preprocessed one-channel buffer (sb_first_buffer_view_launch) instead of k_conv_direct."""
     from ctypes import byref, c_int, c_void_p
     import torch
     from sleap_b200 import _lib
@@ -265,7 +265,7 @@ def test_topdown_predictor():
 
 
 def test_tc_path_matches_direct_fp16(monkeypatch):
-    """tcgen05 implicit-GEMM convs vs the CUDA-core kernels on identical fp16 activations / weights:
+    """wgmma implicit-GEMM convs vs the CUDA-core kernels on identical fp16 activations / weights:
     only the fp32 accumulation order differs."""
     cfg = dict(filters=64, filters_rate=2, max_stride=8, output_stride=2, middle_block=True, up_interpolate=False)
     heads = [dict(name="MultiInstanceConfmapsHead", channels=13, output_stride=2),
@@ -290,10 +290,9 @@ def test_tc_path_matches_direct_fp16(monkeypatch):
 @pytest.mark.parametrize("fused", [None, "0", "1", "2"])
 @pytest.mark.parametrize("cin,cout", [(16, 16), (64, 32), (128, 64), (256, 128), (512, 256)])
 def test_tc_tconv_layers(cin, cout, fused, monkeypatch):
-    """Conv2DTranspose(k3, s2) on the tensor cores: four forked per-phase launches ("0") or the fused
-    single-launch form with one TMEM accumulator per phase ("1"; weights resident or streamed, two launches
-    when 4 x Cout exceeds the 512 TMEM columns), or whatever the autotuner picks (None) -- against the
-    CUDA-core kernel on the same fp16 activations."""
+    """Conv2DTranspose(k3, s2) on the tensor cores as four sub-pixel phase launches, against the CUDA-core kernel on the
+    same fp16 activations.  The variant / fused-form settings of the parameters select nothing on sm_90a (one kernel
+    form): every case runs the phase launches."""
     from sleap_b200.nn import oplist as ol
     from sleap_b200 import _lib
     from ctypes import c_int, c_void_p, byref
@@ -326,7 +325,7 @@ def test_tc_tconv_layers(cin, cout, fused, monkeypatch):
 
     if fused is not None:
         monkeypatch.setenv("SB_FORCE_VARIANT", "2")
-        if fused in ("1", "2"):            # "2": the cluster twin (cta_group::2 pair) of the fused form where weights are streamed
+        if fused in ("1", "2"):
             monkeypatch.setenv("SB_FORCE_FUSED_TCONV", fused)
     got = run()
     monkeypatch.delenv("SB_FORCE_VARIANT", raising=False)
@@ -339,8 +338,9 @@ def test_tc_tconv_layers(cin, cout, fused, monkeypatch):
 
 @pytest.mark.parametrize("variant,fused", [("2", None), ("3", None), ("4", None), ("5", None), ("2", "1")])
 def test_tc_forced_variants_unet(variant, fused, monkeypatch):
-    """The whole fp16 UNet (transposed-conv phases, fused max-pool, concat-by-slice outputs) with every
-    halo variant forced, against the CUDA-core path."""
+    """The whole fp16 UNet (transposed-conv phases, fused max-pool, concat-by-slice outputs) with each
+    SB_FORCE_VARIANT / SB_FORCE_FUSED_TCONV setting of the parameters, against the CUDA-core path.  On sm_90a there is
+    one kernel form, so the settings select nothing and the runs are identical."""
     cfg = dict(filters=32, filters_rate=2, max_stride=8, output_stride=2, middle_block=True, up_interpolate=False)
     heads = [dict(name="MultiInstanceConfmapsHead", channels=13, output_stride=2),
              dict(name="PartAffinityFieldsHead", channels=24, output_stride=4)]
@@ -373,22 +373,9 @@ def test_tc_single_layers(cin, cout, k, hw, variant, monkeypatch):
     _tc_single_layer(cin, cout, k, hw, variant, monkeypatch)
 
 
-@pytest.mark.parametrize("variant", ["3", "5", "7"])
-@pytest.mark.parametrize("cin,cout,hw", [(256, 128, (53, 70)), (128, 256, (40, 48))])
-def test_tc_multicast_twins(cin, cout, hw, variant, monkeypatch):
-    """The multicast form of the cluster twins (each CTA fetches half of every weight slice and multicasts it to both;
-    SB_ENABLE_MULTICAST=1 -- by default the twin is the cta_group::2 pair, covered by test_tc_single_layers)."""
-    monkeypatch.setenv("SB_ENABLE_MULTICAST", "1")
-    _tc_single_layer(cin, cout, 3, hw, variant, monkeypatch)
-
-
 def _tc_single_layer(cin, cout, k, hw, variant, monkeypatch):
-    """Each swizzle mode / chunk count / N-tile shape of the tensor-core conv on its own, with the
-    kernel variant chosen by the autotuner (None) or forced: 0 streaming, 1 weights-resident,
-    2.. the halo candidates in plan order: 8x16, super-tiles 16x16 / 16x32 / 8x32 (weights resident or streamed), each
-    weight-streamed one followed by its cluster twin (the cta_group::2 pair: M = 256 MMAs over two CTAs; with
-    SB_ENABLE_MULTICAST=1 the multicast form) -- up to six candidates, so 2..7; a forced variant that does not apply to
-    the layer falls back to the streaming kernel."""
+    """Each swizzle mode / chunk count / N-tile shape of the tensor-core conv on its own.  A forced variant
+    (SB_FORCE_VARIANT) that does not exist -- on sm_90a there is one kernel form -- runs that kernel."""
     if variant is not None:
         monkeypatch.setenv("SB_FORCE_VARIANT", variant)
     import torch
@@ -497,7 +484,7 @@ def test_pipelined_predict_matches_per_batch():
 @pytest.mark.parametrize("cout,hw,as_float", [(16, (64, 128), False), (16, (38, 136), False), (8, (48, 256), False),
                                               (32, (64, 128), True), (24, (36, 160), False)])
 def test_first_layer_toeplitz_view(cout, hw, as_float, variant, monkeypatch):
-    """First conv (1 input channel) as a Toeplitz GEMM on the stock tcgen05 kernels (sb_conv_tc.cu,
+    """First conv (1 input channel) as a Toeplitz GEMM on the stock tensor-core kernel (sb_conv_tc.cu,
     first_view_prepare) vs the torch-CPU fp32 conv on the fp16-rounded operands it consumes, and vs the
     CUDA-core k_conv_first (SB_DISABLE_FIRST_VIEW=1).  Covers every kernel variant, widths whose group
     count is not a tile multiple, float frames, and the bottom zero pad (H not a multiple of the stride)."""
@@ -554,8 +541,8 @@ def test_first_layer_toeplitz_view(cout, hw, as_float, variant, monkeypatch):
 def test_conv01_fused_first_block(hw, as_float, relu, monkeypatch):
     """k_conv01 (sb_conv01.cu): frame -> conv0 (1 -> 16) -> conv1 (16 -> 16) -> 2x2 max-pool in ONE kernel, against
     (a) torch fp32 convs on the operands the tensor cores consume (fp16 pixels / weights, fp16-rounded intermediate) and
-    (b) the two separate tcgen05 launches (SB_FORCE_CONV01=0).  Several strips (W > 512, partial last strip), odd row
-    counts per CTA range, float frames, bottom zero padding, no-ReLU."""
+    (b) the two separate tensor-core launches (SB_FORCE_CONV01=0).  Partial edge tiles (W not a multiple of 16,
+    H not a multiple of 8), float frames, bottom zero padding, no-ReLU."""
     from ctypes import byref, c_int, c_void_p
     import torch
     import torch.nn.functional as F
@@ -617,7 +604,7 @@ def test_conv01_fused_first_block(hw, as_float, relu, monkeypatch):
 @pytest.mark.parametrize("cin,cout,hw,as_float,bn", [(3, 32, (64, 96), False, True), (1, 16, (70, 130), False, False), (3, 128, (96, 64), True, True)])
 def test_tc_stem_7x7_stride2(cin, cout, hw, as_float, bn):
     """Hourglass stem (hourglass.py:49-100): 7x7 stride-2 SAME convolution on 1 / 3 input channels as a 4x4 convolution over
-    the space-to-depth view of the frame on the tcgen05 path (sb_conv_tc.cu, stem_view_prepare), conv -> ReLU -> BN affine.
+    the space-to-depth view of the frame on the tensor-core path (sb_conv_tc.cu, stem_view_prepare), conv -> ReLU -> BN affine.
     Reference: torch conv2d with TF SAME padding (2 before, 3 after for even sizes) on the fp16-rounded operands."""
     from ctypes import byref, c_int, c_void_p
     import torch

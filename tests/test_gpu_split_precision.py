@@ -1,4 +1,4 @@
-"""Precision 2 (split-fp16 activations / weights, three tensor-core products per term, fp32 accumulate): the tcgen05
+"""Precision 2 (split-fp16 activations / weights, three tensor-core products per term, fp32 accumulate): the wgmma
 conv path must reproduce the fp32 torch-CPU oracle to the north-star tolerance (1e-4 of the map; measured ~1e-6), so
 that peak indices / instance assignments of the tensor-core path agree with the fp32 reference network."""
 import numpy as np
@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 
 from test_gpu_model import HEADS2, UNET_CASES, _mk, _oracle_forward, _unet_spec  # noqa: E402
 
-TOL = 5e-5     # of max(1, |map|max); measured <= 2.1e-5 on these nets, 2.4e-5 at C4 full size.  The split arithmetic itself
+TOL = 5e-5     # of max(1, |map|max); measured 2.4e-5 at C4 full size on an H100.  The split arithmetic itself
                # is good to ~1e-6 (numpy emulation); what is left is the tensor core's fp32 accumulator, which truncates
                # instead of rounding: a bias of ~n_steps * 2^-25 per accumulation chain (DESIGN.md 5.7)
 
@@ -27,7 +27,7 @@ def _check(got, want, tol=TOL):
 
 @pytest.mark.parametrize("name", list(UNET_CASES))
 def test_unet_forward_split_small(name):
-    """Same nets / frames as test_unet_forward_fp32 (8-filter nets: 24-channel split tensors on tcgen05, the 4-filter
+    """Same nets / frames as test_unet_forward_fp32 (8-filter nets: 24-channel split tensors on the tensor cores, the 4-filter
     net's 12-channel tensors and every first conv on the CUDA-core kernels with split stores; stand-alone pool,
     bilinear upsample, 7x7 stem from the fp32 frame buffer)."""
     cfg = UNET_CASES[name]

@@ -1,6 +1,6 @@
 """Secondary configurations of BASELINE.json (C1, C2, C3, C5) through the public predictors, one
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
-Not the driver's bench (that is bench.py = C4); results are copied into profiles/.
+Secondary to bench.py (C4).
 
   python tools/bench_configs.py [c1] [c2] [c3] [c5] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
 """

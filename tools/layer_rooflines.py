@@ -1,10 +1,10 @@
 """Per-layer floors of the C4 network (8 frames of 1024x1024) next to the measured per-op times.
 
-  python tools/layer_rooflines.py profiles/r01_per_op_fast_epilogue.txt profiles/r01_layer_rooflines.md
+  BENCH_VERBOSE=1 python bench.py 2> per_op.txt; python tools/layer_rooflines.py per_op.txt floors.md
 
-Floors: tensor = algorithmic FLOPs / measured sustained bf16 peak (MEASURED_PEAKS.json, 1377 TF/s);
-HBM = (activations in + out (+ fused pool output) at their storage width) / 6.0 TB/s (profiles/r01_store_probe.txt,
-r01_bw_probe.txt: best streaming rate observed on this part).  The bound of a layer is the larger floor.
+Floors: tensor = algorithmic FLOPs / 989 TFLOP/s (H100 SXM data sheet, dense fp16, 700 W);
+HBM = (activations in + out (+ fused pool output) at their storage width) / 3.35 TB/s (H100 SXM data sheet).
+The bound of a layer is the larger floor.
 """
 import re
 import sys
@@ -74,7 +74,7 @@ def main(src, out):
         rows.append(f"| {op} | {name} @{hin}² | {meas:.1f} | {flops / 1e9:.2f} | {t_tensor:.1f} | {(in_b + out_b) / 1e6:.1f} | {t_hbm:.1f} | "
                     f"{'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} |")
     rows.append(f"| | **all conv layers** | **{tot_m:.1f}** | | | | | | **{tot_f / tot_m:.2f}** (sum of floors {tot_f:.1f} us) |")
-    text = ("# C4 per-layer floors vs measured (8 frames, one B200)\n\nMeasured: CUDA-event per-op times of `bench.py` (`sb_model_profile_ops`), file `" + src +
+    text = ("# C4 per-layer floors vs measured (8 frames, one H100)\n\nMeasured: CUDA-event per-op times of `bench.py` (`sb_model_profile_ops`), file `" + src +
             "`.  Floors: see tools/layer_rooflines.py.\n\n" + "\n".join(rows) + "\n")
     open(out, "w").write(text)
     print(text)

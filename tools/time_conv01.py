@@ -1,4 +1,4 @@
-"""Configure the C4 model (autotune prints the fused first block's time with SB_DEBUG=1); SB_C01_ABLATE masks stages."""
+"""Configure the C4 model (autotune prints the fused first block's time with SB_DEBUG=1)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
