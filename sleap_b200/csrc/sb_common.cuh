@@ -160,3 +160,16 @@ int sbk_local_dir(sb_handle_s* h, const float* patches, int N, float delta, floa
 int sb_post_ws_alloc(sb_handle_s* h, SbPostWs& ws, int B, int H, int W, int C, int max_peaks,
                      int max_node_peaks, int max_instances, int n_edges);
 void sb_post_ws_free(SbPostWs& ws);
+
+// ---- frame preprocessing shared by k_preprocess and the fused first-layer / stem view kernels ----
+// caffe mean of BGR channel c (resnet.py imagenet_preproc_v1)
+__device__ __forceinline__ float sb_imagenet_caffe_mean(int c) { return c == 0 ? 103.939f : (c == 1 ? 116.779f : 123.68f); }
+// ensure_grayscale of one RGB pixel as a [0, 1] float (u8: truncating round trip like tf.image.rgb_to_grayscale)
+template <typename TI>
+__device__ __forceinline__ float sb_gray_pre(const TI* p, int in_is_u8) {
+  const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
+  const float g = __fadd_rn(__fadd_rn(__fmul_rn(__fmul_rn((float)p[0], sc), 0.2989f),
+                                      __fmul_rn(__fmul_rn((float)p[1], sc), 0.5870f)),
+                            __fmul_rn(__fmul_rn((float)p[2], sc), 0.1140f));
+  return in_is_u8 ? __fmul_rn(truncf(fminf(fmaxf(__fmul_rn(g, 255.5f), 0.f), 255.f)), 1.0f / 255.0f) : g;
+}

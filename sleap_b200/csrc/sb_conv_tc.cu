@@ -16,7 +16,11 @@
 //   D: two warpgroups, each m64nNk16 wgmma over 64 of the 128 pixels; epilogue through a shared-memory
 //     staging tile -> bias / ReLU / BN affine -> fp16 (or fp32 for head outputs) NHWC stores into the
 //     consumer's channel slice.
-//   Conv2DTranspose(k3,s2) = four sub-pixel phase GEMMs over the input grid with strided stores.
+//   Conv2DTranspose(k3 / k4, s2) = four sub-pixel phase GEMMs over the input grid with strided stores.
+//   1x1 stride-2 convs (ResNet) = 1x1 stride-1 convs over a subsampled view of the input: the A tensor map gets the
+//     output's H / W and doubled pixel / row pitches (TMA takes any 16-byte-multiple global strides).
+//   Residual blocks (ResNet, add skips): the epilogue adds the shortcut tensor after the bias and applies the ADD's
+//     ReLU, storing into the ADD's output slice.
 #include <cuda.h>
 
 #include <algorithm>
@@ -51,6 +55,10 @@ struct TcParams {
   int relu;
   void* pool_out;               // optional fused MaxPool2D(2,2) output (same dtype as out)
   int pool_H, pool_W, pool_Ctot, pool_coff;
+  // optional residual shortcut (fp16 NHWC slice, same pixel grid as out): added after the bias, before the ReLU;
+  // precision 2: its [lo | hi | hi] planes, Cout channels apart, are summed first
+  const void* res;
+  int res_Ctot, res_coff;
   int a_slot_bytes, b_slot_bytes, n_a_slots, n_b_slots;
   int a_tx_bytes, b_tx_bytes;
   int layout_type;             // wgmma descriptor layout: 1 = SW128, 2 = SW64, 3 = SW32
@@ -275,6 +283,28 @@ constexpr int kConvThreads = kConsumerThreads + 32;   // + the TMA producer warp
 // fp32 accumulator columns staged through shared memory per epilogue round (must divide N)
 constexpr int stage_cols(int n) { return n % 32 == 0 ? 32 : 16; }
 
+// Residual shortcut of output channels [n, n + 16) of pixel `pix`, added to the staged accumulators (before the bias; the
+// epilogue then applies bias, the ADD's ReLU and the store): 16 contiguous fp16 channels of one pixel per thread, two
+// 16-byte loads when the tile is full; precision 2: lo + hi of the [lo | hi | hi] planes, Cout channels apart.
+__device__ __forceinline__ void tc_add_residual(const TcParams& P, uint32_t (&r)[16], size_t pix, int n) {
+  const __half* pr = reinterpret_cast<const __half*>(P.res) + pix * P.res_Ctot + P.res_coff + n;
+  if (!P.split && n + 16 <= P.Cout) {
+    const uint4 q[2] = {reinterpret_cast<const uint4*>(pr)[0], reinterpret_cast<const uint4*>(pr)[1]};
+    const __half2* hq = reinterpret_cast<const __half2*>(q);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 f = __half22float2(hq[j]);
+      r[2 * j] = __float_as_uint(__uint_as_float(r[2 * j]) + f.x);
+      r[2 * j + 1] = __float_as_uint(__uint_as_float(r[2 * j + 1]) + f.y);
+    }
+    return;
+  }
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+    if (n + j < P.Cout)
+      r[j] = __float_as_uint(__uint_as_float(r[j]) + (P.split ? __half2float(pr[j]) + __half2float(pr[P.Cout + j]) : __half2float(pr[j])));
+}
+
 // Epilogue of 16 accumulator columns [c0, c0 + 16) of one tile pixel, read from the fp32 staging rows in shared memory
 // (`src`: this pixel's 16 staged values).  Called by whole warps (the fused max-pool shuffles across lanes): lane l of
 // warp q holds tile pixel 32 q + l.
@@ -287,6 +317,7 @@ __device__ __forceinline__ void tc_epilogue_chunk(const TcParams& P, const float
     r[4 * j4 + 0] = __float_as_uint(v.x); r[4 * j4 + 1] = __float_as_uint(v.y);
     r[4 * j4 + 2] = __float_as_uint(v.z); r[4 * j4 + 3] = __float_as_uint(v.w);
   }
+  if (P.res != nullptr && valid) tc_add_residual(P, r, pix, n0 + c0);
   if (P.epi_mode != 1) {
     tc_epilogue_cols<TW>(P, s_par, r, n0, c0, valid, pix, b, x0, y0, q, lane);
     return;
@@ -622,7 +653,12 @@ struct SbConvTcPlan {
   bool from_buffer = false;         // Toeplitz view built from the (resized / converted) PREPROCESS output instead of the raw frame
   bool s2d = false;                 // view_in is the space-to-depth view of the frame (7x7 stride-2 stem as a 4x4 conv)
   int s2d_Hs = 0, s2d_Ws = 0;
+  int s2d_pre_mode = SB_PRE_PLAIN;   // PREPROCESS mode folded into the space-to-depth view (ImageNet caffe for ResNet)
   bool out_dead = false;            // nobody reads the full-resolution output (only the fused pool): stores are skipped
+  // the residual ADD after this conv runs in its epilogue (launches); plain_launches store the conv's own output
+  // instead, for a forward pass that asks for that tensor (the ADD op then runs)
+  bool res_fused = false;
+  std::vector<TcLaunch> plain_launches;
 };
 
 static CUtensorMapSwizzle swz_for(int KC) {
@@ -637,7 +673,12 @@ static bool tc_eligible(const SbModel* m, const SbOp& op) {
   // chunk that reaches past C_in is zero-filled by TMA on both operands (activations and weights)
   if (!(Cin >= 16 && Cin % 8 == 0)) return false;
   if (getenv("SB_TC_STRICT_CIN") && !(Cin == 16 || Cin == 32 || Cin % 64 == 0)) return false;
-  if (op.kind() == SB_OPK_CONV && !((op.k() == 1 || op.k() == 3 || op.k() == 5 || op.k() == 7) && op.stride() == 1)) return false;
+  if (op.kind() == SB_OPK_CONV && !((op.k() == 1 || op.k() == 3 || op.k() == 5 || op.k() == 7) && op.stride() == 1) &&
+      !(op.k() == 1 && op.stride() == 2))
+    return false;
+  // explicit padding: only the 1x1 VALID convs of ResNet (padding 0, the same as SAME for kernel 1)
+  if (op.kind() == SB_OPK_CONV && op.explicit_pad() && (op.k() != 1 || op.pad_top() != 0 || op.pad_left() != 0)) return false;
+  if (op.kind() == SB_OPK_TCONV && op.k() != 3 && op.k() != 4) return false;
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
   if (ib.f32) return false;
@@ -663,7 +704,7 @@ void sb_conv_tc_release(SbModel* m) {
 
 bool sb_conv_tc_out_dead(const SbModel* m, int buffer_id) {
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi)
-    if (m->tc_plans[oi] && m->tc_plans[oi]->out_dead && m->ops[oi].out_buf() == buffer_id) return true;
+    if (m->tc_plans[oi] && (m->tc_plans[oi]->out_dead || m->tc_plans[oi]->res_fused) && m->ops[oi].out_buf() == buffer_id) return true;
   return false;
 }
 
@@ -690,22 +731,41 @@ static int wg_n(int n) {
   return 256;
 }
 
+// The residual ADD right after conv `oi` can run in its epilogue: the conv's output has no other reader (the compiler
+// only sets SB_OPF_RESIDUAL then), the ADD is flagged, and the shortcut / sum slices are 16-byte aligned fp16.
+static bool res_fusable(const SbModel* m, size_t oi) {
+  const SbOp& op = m->ops[oi];
+  if (op.kind() != SB_OPK_CONV || !op.residual() || oi + 1 >= m->ops.size() || getenv("SB_DISABLE_RES_FUSION")) return false;
+  const SbOp& add = m->ops[oi + 1];
+  if (add.kind() != SB_OPK_ADD || !(add.flags() & SB_OPF_FUSED_ADD) || add.out_buf() != op.sum_buf() || add.out_coff() != op.sum_coff()) return false;
+  const SbBuffer& rb = m->buffers[op.res_buf()];
+  const SbBuffer& sb = m->buffers[op.sum_buf()];
+  const SbBuffer& ob = m->buffers[op.out_buf()];
+  return !rb.f32 && !sb.f32 && !ob.f32 && rb.C % 8 == 0 && op.res_coff() % 8 == 0 && sb.C % 8 == 0 && op.sum_coff() % 8 == 0 &&
+         rb.H == ob.H && rb.W == ob.W && sb.H == ob.H && sb.W == ob.W && op.pool_buf() < 0 && !(op.flags() & (SB_OPF_BN | SB_OPF_RELU));
+}
+
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
                        const TcGroup* groups, int dy0, int extra_rows, int n_wtaps, int oy_mul, int oy_add,
-                       int ox_mul, int ox_add, const TcView* view = nullptr) {
+                       int ox_mul, int ox_add, const TcView* view = nullptr, bool fuse_res = false,
+                       std::vector<TcLaunch>* dst = nullptr) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   const SbBuffer& ib = view ? view->ib : m->buffers[op.in_buf()];
-  const SbBuffer& ob = view ? view->ob : m->buffers[op.out_buf()];
+  const SbBuffer& ob0 = view ? view->ob : m->buffers[op.out_buf()];
+  const SbBuffer& ob = fuse_res ? m->buffers[op.sum_buf()] : ob0;       // the residual sum goes to the ADD's output slice
   const int Cin = view ? view->Cin : op.in_C(), Cout = view ? view->Cout : op.out_C();
-  const int in_coff = view ? 0 : op.in_coff(), out_coff = view ? view->out_coff : op.out_coff();
+  const int in_coff = view ? 0 : op.in_coff(), out_coff = view ? view->out_coff : (fuse_res ? op.sum_coff() : op.out_coff());
   const int KC = Cin > 32 ? 64 : (Cin > 16 ? 32 : 16);
+  // 1x1 stride-2: the GEMM runs over the output grid on a subsampled view of the input (pitches x 2)
+  const int sub = (!view && op.kind() == SB_OPK_CONV) ? op.stride() : 1;
+  const int gH = sub > 1 ? ob.H : ib.H, gW = sub > 1 ? ob.W : ib.W;
   TcLaunch L;
   memset(&L, 0, sizeof(L));
   TcParams& P = L.P;
-  P.H = ib.H; P.W = ib.W;
-  P.tiles_x = (ib.W + TW - 1) / TW;
-  const int tiles_y = (ib.H + TH - 1) / TH;
+  P.H = gH; P.W = gW;
+  P.tiles_x = (gW + TW - 1) / TW;
+  const int tiles_y = (gH + TH - 1) / TH;
   P.n_chunks = (Cin + KC - 1) / KC; P.KC = KC;
   P.n_groups = n_groups;
   for (int g = 0; g < n_groups; ++g) P.groups[g] = groups[g];
@@ -722,6 +782,12 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     P.bn_shift = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_shift_off() : nullptr;
     P.relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
   }
+  P.res = nullptr;
+  if (fuse_res) {                  // + shortcut, then the ADD's ReLU
+    const SbBuffer& rb = m->buffers[op.res_buf()];
+    P.res = (const __half*)rb.dev; P.res_Ctot = rb.C; P.res_coff = op.res_coff();
+    P.relu = (m->ops[&op - m->ops.data() + 1].flags() & SB_OPF_RELU) ? 1 : 0;
+  }
   P.pool_out = nullptr;
   if (!view && op.kind() == SB_OPK_CONV && op.pool_buf() >= 0 && !ob.f32 && Cout % 16 == 0 &&
       m->buffers[op.pool_buf()].C % 8 == 0 && op.pool_coff() % 8 == 0 && ib.H % 2 == 0 && ib.W % 2 == 0) {
@@ -732,7 +798,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   P.epi_mode = 0;
   if (!P.split && !getenv("SB_DISABLE_FAST_EPILOGUE") && !ob.f32 && P.bn_scale == nullptr && Cout % 16 == 0 && plan->Cout_pad == Cout &&
       ob.C % 16 == 0 && out_coff % 16 == 0 && (P.pool_out == nullptr || (P.pool_Ctot % 16 == 0 && P.pool_coff % 16 == 0)))
-    P.epi_mode = 1;
+    P.epi_mode = 1;                // (a residual slice is 16-byte aligned: res_fusable)
   P.row_bytes = KC * 2;
   P.layout_type = KC == 64 ? 1 : (KC == 32 ? 2 : 3);     // wgmma descriptor layout: SW128 / SW64 / SW32
   P.a_tx_bytes = P.box_rows * TW * KC * 2;
@@ -753,10 +819,10 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
            (size_t)(2 * P.n_a_slots + 2 * P.n_b_slots) * 8 + 16 + 3 * 256 * sizeof(float);
   if (L.smem > kMaxDynSmem) return sb_fail(h, SB_ERR_INVALID, "conv tile needs %zu bytes of shared memory", L.smem);
   L.grid = dim3(P.tiles_x * tiles_y, (plan->Cout_pad + N - 1) / N, 1 /* z = batch, set at launch */);
-  // A: NHWC view (slice channels, W, H, batch)
+  // A: NHWC view (slice channels, W, H, batch); pixel and row pitches x sub
   {
-    cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)ib.W, (cuuint64_t)ib.H, (cuuint64_t)m->B};
-    cuuint64_t strides[3] = {(cuuint64_t)ib.C * 2, (cuuint64_t)ib.W * ib.C * 2, (cuuint64_t)ib.H * ib.W * ib.C * 2};
+    cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)gW, (cuuint64_t)gH, (cuuint64_t)m->B};
+    cuuint64_t strides[3] = {(cuuint64_t)ib.C * 2 * sub, (cuuint64_t)ib.W * ib.C * 2 * sub, (cuuint64_t)ib.H * ib.W * ib.C * 2};
     cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)TW, (cuuint32_t)P.box_rows, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     void* gptr = (void*)((__half*)ib.dev + in_coff);
@@ -774,7 +840,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
-  plan->launches.push_back(L);
+  (dst ? *dst : plan->launches).push_back(L);
   return 0;
 }
 
@@ -888,9 +954,14 @@ static int first_view_prepare(sb_handle_s* h, SbModel* m, int oi, bool from_buff
 // with W'[dy][dx][(py, px, c)][co] = w[2(dy+1)+py][2(dx+1)+px][c][co] (zero where the index reaches 7).  The view kernel
 // does InferenceLayer.preprocess (uint8 -> float * 1/255, zero pad) on the way; the stock wgmma conv kernel runs
 // the convolution (K = 16 taps x 16 channels = 256 instead of 147: the stem was on the CUDA cores before).
+// The ResNet stem (ZeroPadding2D(3) + VALID, resnet.py) pads 3|3 instead: output pixel o reads rows 2o-3 .. 2o+3, i.e.
+// blocks o-2 .. o+1 with the zero tap at the top / left (W'[dy][dx][(py, px, c)] = w[2dy+py-1][2dx+px-1]).  Its view
+// carries the pretrained preprocessing too (pre_mode != 0): tile_channels (1 -> 3, or gray -> 3 for a grayscale-trained
+// model fed colour frames), then x * 255, RGB -> BGR, minus the caffe means, on the padded [0, 1] image -- so rows /
+// columns of the net input beyond the frame hold -mean, while the conv's own padding (outside the view) stays 0.
 template <typename TI>
 __global__ void __launch_bounds__(256) k_s2d_view(const TI* __restrict__ img, int Hin, int Win, int Cin, int Hs, int Ws,
-                                                  __half* __restrict__ G, int in_is_u8, size_t total) {
+                                                  __half* __restrict__ G, int in_is_u8, size_t total, int pre_mode = 0) {
   const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
   for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
     const int X = (int)(i % Ws);
@@ -904,9 +975,20 @@ __global__ void __launch_bounds__(256) k_s2d_view(const TI* __restrict__ img, in
 #pragma unroll
       for (int px = 0; px < 2; ++px) {
         const int y = 2 * Y + py, x = 2 * X + px;
-        if (y < Hin && x < Win)
-          for (int c = 0; c < Cin; ++c)
-            v[(py * 2 + px) * Cin + c] = __float2half_rn(__fmul_rn((float)img[(((size_t)b * Hin + y) * Win + x) * Cin + c], sc));
+        const bool in = y < Hin && x < Win;
+        const TI* p = img + (((size_t)b * Hin + y) * Win + x) * Cin;
+        if (pre_mode == SB_PRE_PLAIN) {
+          if (in)
+            for (int c = 0; c < Cin; ++c) v[(py * 2 + px) * Cin + c] = __float2half_rn(__fmul_rn((float)p[c], sc));
+          continue;
+        }
+        const float g = (in && Cin == 3 && pre_mode == SB_PRE_IMAGENET_CAFFE_GRAY) ? sb_gray_pre(p, in_is_u8) : 0.f;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {              // BGR channel c
+          float f = 0.f;
+          if (in) f = (Cin == 3 && pre_mode == SB_PRE_IMAGENET_CAFFE_GRAY) ? g : __fmul_rn((float)p[Cin == 1 ? 0 : 2 - c], sc);
+          v[(py * 2 + px) * 3 + c] = __float2half_rn(__fsub_rn(__fmul_rn(f, 255.f), sb_imagenet_caffe_mean(c)));
+        }
       }
     uint4* dst = reinterpret_cast<uint4*>(G + i * 16);
     dst[0] = *reinterpret_cast<const uint4*>(&v[0]);
@@ -922,6 +1004,7 @@ static int stem_view_prepare(sb_handle_s* h, SbModel* m, int oi) {
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
   const int Cin = op.in_C(), Cout = op.out_C();
+  const int sh = op.explicit_pad() ? 1 : 0;                  // 3|3 padding: the 4x4 block window starts one block earlier
   if (ib.H % 2 || ib.W % 2 || ob.H != ib.H / 2 || ob.W != ib.W / 2) return 0;
   if (ob.f32 || ob.C % 8 || op.out_coff() % 8 || ob.W < TW || ob.H < TH + 3) return 0;
   SbConvTcPlan* plan = new SbConvTcPlan();
@@ -929,14 +1012,15 @@ static int stem_view_prepare(sb_handle_s* h, SbModel* m, int oi) {
   if (cp > 256) cp = (cp + 255) / 256 * 256;
   plan->Cout_pad = cp;
   plan->s2d = true; plan->s2d_Hs = ob.H; plan->s2d_Ws = ob.W;
+  plan->s2d_pre_mode = m->ops[oi - 1].pre_mode();
   std::vector<__half> w16((size_t)16 * cp * 16, __float2half(0.f));
   const float* w = m->weights_host.data() + op.w_off();      // [7*7][Cin][Cout]
   for (int dy = 0; dy < 4; ++dy)
     for (int dx = 0; dx < 4; ++dx)
       for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px) {
-          const int ky = 2 * dy + py, kx = 2 * dx + px;
-          if (ky > 6 || kx > 6) continue;
+          const int ky = 2 * dy + py - sh, kx = 2 * dx + px - sh;
+          if (ky < 0 || kx < 0 || ky > 6 || kx > 6) continue;
           for (int c = 0; c < Cin; ++c)
             for (int co = 0; co < Cout; ++co)
               w16[((size_t)(dy * 4 + dx) * cp + co) * 16 + (py * 2 + px) * Cin + c] = __float2half_rn(w[((size_t)(ky * 7 + kx) * Cin + c) * Cout + co]);
@@ -967,10 +1051,10 @@ static int stem_view_prepare(sb_handle_s* h, SbModel* m, int oi) {
   V.out_coff = op.out_coff();
   TcGroup g[4];
   for (int dx = 0; dx < 4; ++dx) {
-    g[dx].dx = dx - 1; g[dx].n_taps = 4;
+    g[dx].dx = dx - 1 - sh; g[dx].n_taps = 4;
     for (int dy = 0; dy < 4; ++dy) g[dx].taps[dy] = TcTap{dy, dy * 4 + dx};
   }
-  const int rc = make_launch(h, m, op, plan, 4, g, -1, 3, 16, 1, 0, 1, 0, &V);
+  const int rc = make_launch(h, m, op, plan, 4, g, -1 - sh, 3, 16, 1, 0, 1, 0, &V);
   if (rc) {
     cudaFree(plan->w16); cudaFree(plan->view_in);
     delete plan;
@@ -991,9 +1075,10 @@ int sb_stem_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* fr
   const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
   if (frames_are_u8)
     k_s2d_view<unsigned char><<<grid, 256, 0, h->stream>>>((const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, plan->s2d_Hs, plan->s2d_Ws,
-                                                           plan->view_in, 1, total);
+                                                           plan->view_in, 1, total, plan->s2d_pre_mode);
   else
-    k_s2d_view<float><<<grid, 256, 0, h->stream>>>((const float*)frames_dev, m->Hin, m->Win, m->Cin, plan->s2d_Hs, plan->s2d_Ws, plan->view_in, 0, total);
+    k_s2d_view<float><<<grid, 256, 0, h->stream>>>((const float*)frames_dev, m->Hin, m->Win, m->Cin, plan->s2d_Hs, plan->s2d_Ws, plan->view_in, 0,
+                                                   total, plan->s2d_pre_mode);
   SB_CHECK_LAUNCH(h);
   return sb_conv_tc_launch(h, m, op_index, B);
 }
@@ -1098,10 +1183,35 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
         for (int ky = 0; ky < k; ++ky) g[kx].taps[ky] = TcTap{ky, ky * k + kx};
       }
       rc = make_launch(h, m, op, plan, k, g, -(k / 2), k - 1, taps, 1, 0, 1, 0);
-    } else if (op.kind() == SB_OPK_CONV) {   // 1x1
+    } else if (op.kind() == SB_OPK_CONV) {   // 1x1 (stride 1, or stride 2 on the subsampled view)
       TcGroup g[1];
       g[0].dx = 0; g[0].n_taps = 1; g[0].taps[0] = TcTap{0, 0};
-      rc = make_launch(h, m, op, plan, 1, g, 0, 0, 1, 1, 0, 1, 0);
+      if (res_fusable(m, oi)) {
+        rc = make_launch(h, m, op, plan, 1, g, 0, 0, 1, 1, 0, 1, 0, nullptr, false, &plan->plain_launches);
+        if (!rc) rc = make_launch(h, m, op, plan, 1, g, 0, 0, 1, 1, 0, 1, 0, nullptr, true);
+        plan->res_fused = rc == 0;
+      } else {
+        rc = make_launch(h, m, op, plan, 1, g, 0, 0, 1, 1, 0, 1, 0);
+      }
+    } else if (k == 4) {
+      // Conv2DTranspose k4 s2 SAME (forward-conv padding 1): out[2i+a] gets (ky, iy) = a==0 ? {(1,i),(3,i-1)} :
+      // {(0,i+1),(2,i)}; same along x.  Each phase: 2 filter columns x 2 rows, box rows i-1..i+TH-1 (a=0) / i..i+TH (a=1).
+      for (int a = 0; a < 2 && !rc; ++a)
+        for (int bx = 0; bx < 2 && !rc; ++bx) {
+          TcGroup g[2];
+          const int kxs[2] = {bx == 0 ? 1 : 2, bx == 0 ? 3 : 0}, dxs[2] = {0, bx == 0 ? -1 : 1};
+          for (int q = 0; q < 2; ++q) {
+            g[q].dx = dxs[q]; g[q].n_taps = 2;
+            if (a == 0) {             // dy0 = -1: box row 1 = input row i, box row 0 = i-1
+              g[q].taps[0] = TcTap{1, 1 * 4 + kxs[q]};
+              g[q].taps[1] = TcTap{0, 3 * 4 + kxs[q]};
+            } else {                  // dy0 = 0: box row 0 = input row i, box row 1 = i+1
+              g[q].taps[0] = TcTap{0, 2 * 4 + kxs[q]};
+              g[q].taps[1] = TcTap{1, 0 * 4 + kxs[q]};
+            }
+          }
+          rc = make_launch(h, m, op, plan, 2, g, a == 0 ? -1 : 0, 1, 16, 2, a, 2, bx);
+        }
     } else {
       // Conv2DTranspose k3 s2: out[2i+a] gets (ky, iy) = a==0 ? {(0,i),(2,i-1)} : {(1,i)}; same along x.
       for (int a = 0; a < 2 && !rc; ++a)
@@ -1128,6 +1238,7 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
     }
     if (rc) { cudaFree(plan->w16); delete plan; return rc; }
     m->tc_plans[oi] = plan;
+    if (plan->res_fused) m->skip_op[oi + 1] = 2;
     if (op.kind() == SB_OPK_CONV && op.pool_buf() >= 0 && oi + 1 < m->ops.size() &&
         m->ops[oi + 1].kind() == SB_OPK_POOL && (m->ops[oi + 1].flags() & SB_OPF_FUSED_POOL))
       if (plan->launches[0].P.pool_out != nullptr) {
@@ -1326,7 +1437,7 @@ int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
   const int skip = plan->out_dead && !m->keep_dead_stores;
   // the sub-pixel phases of a transposed conv run back to back on the launching stream: under programmatic dependent
   // launch each phase's CTAs start as the previous phase's SMs drain
-  for (TcLaunch& L : plan->launches) {
+  for (TcLaunch& L : (plan->res_fused && m->keep_dead_stores) ? plan->plain_launches : plan->launches) {
     launch_conv(L, B, h->stream, skip);
     SB_CHECK_LAUNCH(h);
   }

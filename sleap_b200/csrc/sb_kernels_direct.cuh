@@ -214,13 +214,16 @@ __global__ void __launch_bounds__(256) k_conv_first(const TI* __restrict__ img, 
   }
 }
 
-// Conv2DTranspose(k=3, strides=2, padding="same"): out (2H, 2W).  Per axis:
-//   out[2i] = in[i]*W[0] + in[i-1]*W[2];  out[2i+1] = in[i]*W[1].   weights [9][Cin][Cout].
+// Conv2DTranspose(k, strides=2, padding="same"), k = 3 or 4: out (2H, 2W), out[o] += in[i] * W[o - 2i + p] with the
+// forward-conv padding p = (k - 2) / 2 (0 for k3, 1 for k4).  Per axis:
+//   k3: out[2i] = in[i]*W[0] + in[i-1]*W[2];            out[2i+1] = in[i]*W[1]
+//   k4: out[2i] = in[i]*W[1] + in[i-1]*W[3];            out[2i+1] = in[i+1]*W[0] + in[i]*W[2]
+// weights [k*k][Cin][Cout].
 template <typename TI, typename TO>
 __global__ void __launch_bounds__(256) k_tconv_direct(
     const TI* __restrict__ in, int Hin, int Win, int in_Ctot, int in_coff, int Cin,
     TO* __restrict__ out, int out_Ctot, int out_coff, int Cout, const float* __restrict__ w,
-    const float* __restrict__ bias, int relu, int split = 0) {
+    const float* __restrict__ bias, int relu, int split = 0, int k = 3) {
   const int Hout = 2 * Hin, Wout = 2 * Win;
   const int b = blockIdx.z;
   const int co0 = blockIdx.y * DC_CO;
@@ -232,14 +235,16 @@ __global__ void __launch_bounds__(256) k_tconv_direct(
 #pragma unroll
   for (int c = 0; c < DC_CO; ++c) acc[c] = 0.f;
   int kys[2], iys[2], nky = 0, kxs[2], ixs[2], nkx = 0;
-  if (oy & 1) { kys[0] = 1; iys[0] = oy >> 1; nky = 1; }
-  else { kys[0] = 0; iys[0] = oy >> 1; nky = 1; if ((oy >> 1) - 1 >= 0) { kys[1] = 2; iys[1] = (oy >> 1) - 1; nky = 2; } }
-  if (ox & 1) { kxs[0] = 1; ixs[0] = ox >> 1; nkx = 1; }
-  else { kxs[0] = 0; ixs[0] = ox >> 1; nkx = 1; if ((ox >> 1) - 1 >= 0) { kxs[1] = 2; ixs[1] = (ox >> 1) - 1; nkx = 2; } }
+  const int p = (k - 2) / 2;
+  for (int kk = 0; kk < k; ++kk) {              // taps with o - kk + p even and the input index inside the map
+    const int ty = oy - kk + p, tx = ox - kk + p;
+    if (!(ty & 1) && ty >= 0 && (ty >> 1) < Hin) { kys[nky] = kk; iys[nky] = ty >> 1; ++nky; }
+    if (!(tx & 1) && tx >= 0 && (tx >> 1) < Win) { kxs[nkx] = kk; ixs[nkx] = tx >> 1; ++nkx; }
+  }
   for (int a = 0; a < nky; ++a)
     for (int bb = 0; bb < nkx; ++bb) {
       const TI* pin = in_b + ((size_t)iys[a] * Win + ixs[bb]) * in_Ctot;
-      const float* pw = w + (size_t)(kys[a] * 3 + kxs[bb]) * Cin * Cout + co0;
+      const float* pw = w + (size_t)(kys[a] * k + kxs[bb]) * Cin * Cout + co0;
       for (int c = 0; c < Cin; ++c) {
         const float v = ld<TI>(pin + c);
 #pragma unroll
@@ -276,6 +281,27 @@ __global__ void k_maxpool2(const T* __restrict__ in, int Hin, int Win, int in_Ct
   }
 }
 
+// ZeroPadding2D(1) + MaxPooling2D(3, strides=2, padding="valid") (ResNet stem): out[o] = max(in[2o-1 .. 2o+1]) with
+// positions outside the map reading 0 (the zero padding), not -inf.
+template <typename T>
+__global__ void k_maxpool3s2(const T* __restrict__ in, int Hin, int Win, int in_Ctot, int in_coff, int C,
+                             T* __restrict__ out, int Hout, int Wout, int out_Ctot, int out_coff, size_t total) {
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(t % C);
+    const int ox = (int)((t / C) % Wout);
+    const int oy = (int)((t / ((size_t)C * Wout)) % Hout);
+    const int b = (int)(t / ((size_t)C * Wout * Hout));
+    const T* pin = in + (size_t)b * Hin * Win * in_Ctot + in_coff + c;
+    float m = -INFINITY;
+    for (int dy = -1; dy <= 1; ++dy)
+      for (int dx = -1; dx <= 1; ++dx) {
+        const int iy = 2 * oy + dy, ix = 2 * ox + dx;
+        m = fmaxf(m, (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) ? ld<T>(pin + ((size_t)iy * Win + ix) * in_Ctot) : 0.f);
+      }
+    st(out + (((size_t)b * Hout + oy) * Wout + ox) * out_Ctot + out_coff + c, m);
+  }
+}
+
 // x2 upsampling: bilinear with half-pixel centres (weights 1/4, 3/4, edge clamp) or nearest.
 template <typename T>
 __global__ void k_upsample2(const T* __restrict__ in, int Hin, int Win, int in_Ctot, int in_coff, int C,
@@ -307,12 +333,13 @@ __global__ void k_upsample2(const T* __restrict__ in, int Hin, int Win, int in_C
 
 template <typename T>
 __global__ void k_add(const T* __restrict__ a, int a_Ctot, int a_coff, const T* __restrict__ bsrc, int b_Ctot,
-                      int b_coff, T* __restrict__ out, int out_Ctot, int out_coff, int C, size_t npix) {
+                      int b_coff, T* __restrict__ out, int out_Ctot, int out_coff, int C, size_t npix, int relu = 0) {
   const size_t total = npix * C;
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(t % C);
     const size_t p = t / C;
-    st(out + p * out_Ctot + out_coff + c, ld<T>(a + p * a_Ctot + a_coff + c) + ld<T>(bsrc + p * b_Ctot + b_coff + c));
+    const float v = ld<T>(a + p * a_Ctot + a_coff + c) + ld<T>(bsrc + p * b_Ctot + b_coff + c);
+    st(out + p * out_Ctot + out_coff + c, relu ? fmaxf(v, 0.f) : v);
   }
 }
 
@@ -329,11 +356,14 @@ __global__ void k_copy(const T* __restrict__ a, int a_Ctot, int a_coff, T* __res
 
 // Preprocess (InferenceLayer.preprocess): gray<->rgb, u8 -> float * (1/255), bilinear resize by
 // input_scale (half-pixel centres, no antialias), zero pad bottom/right to the net input size.
-//   mode_ch: 0 keep, 1 rgb->gray (u8: truncating round trip like tf.image.rgb_to_grayscale), 2 gray->rgb
+//   mode_ch: 0 keep, 1 rgb->gray (u8: truncating round trip like tf.image.rgb_to_grayscale; with Cnet = 3 the gray value
+//            fills all three channels), 2 gray->rgb
+//   imagenet: then imagenet_preproc_v1 (resnet.py) on the padded [0, 1] image: x * 255, RGB -> BGR, minus the caffe
+//             means -- the bottom / right padding becomes -mean, as in the reference, where it runs inside the model
 template <typename TI, typename TO>
 __global__ void k_preprocess(const TI* __restrict__ in, int Hin, int Win, int Cin, TO* __restrict__ out,
                              int Hnet, int Wnet, int Cnet, int Hres, int Wres, int resize, int mode_ch,
-                             int in_is_u8, size_t total) {
+                             int in_is_u8, size_t total, int imagenet = 0) {
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(t % Cnet);
     const int ox = (int)((t / Cnet) % Wnet);
@@ -346,14 +376,9 @@ __global__ void k_preprocess(const TI* __restrict__ in, int Hin, int Win, int Ci
         const TI* p = img + ((size_t)y * Win + x) * Cin;
         float f;
         if (mode_ch == 1) {
-          const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
-          const float g = __fadd_rn(__fadd_rn(__fmul_rn(__fmul_rn((float)p[0], sc), 0.2989f),
-                                              __fmul_rn(__fmul_rn((float)p[1], sc), 0.5870f)),
-                                    __fmul_rn(__fmul_rn((float)p[2], sc), 0.1140f));
-          if (in_is_u8) f = __fmul_rn(truncf(fminf(fmaxf(__fmul_rn(g, 255.5f), 0.f), 255.f)), 1.0f / 255.0f);
-          else f = g;
+          f = sb_gray_pre(p, in_is_u8);
         } else {
-          const int cc = (mode_ch == 2) ? 0 : c;
+          const int cc = (mode_ch == 2) ? 0 : (imagenet ? 2 - c : c);     // imagenet: BGR channel c reads RGB 2 - c
           f = (float)p[cc];
           if (in_is_u8) f = __fmul_rn(f, 1.0f / 255.0f);
         }
@@ -375,6 +400,7 @@ __global__ void k_preprocess(const TI* __restrict__ in, int Hin, int Win, int Ci
         v = __fadd_rn(tp, __fmul_rn(__fadd_rn(bt, -tp), ly));
       }
     }
+    if (imagenet) v = __fsub_rn(__fmul_rn(v, 255.f), sb_imagenet_caffe_mean(c));
     st(out + t, v);
   }
 }
@@ -427,12 +453,31 @@ __global__ void k_upsample2_split(const __half* __restrict__ in, int Hin, int Wi
 }
 
 __global__ void k_add_split(const __half* __restrict__ a, int a_Ctot, int a_coff, const __half* __restrict__ bsrc, int b_Ctot,
-                            int b_coff, __half* __restrict__ out, int out_Ctot, int out_coff, int C, size_t npix) {
+                            int b_coff, __half* __restrict__ out, int out_Ctot, int out_coff, int C, size_t npix, int relu = 0) {
   const size_t total = npix * C;
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(t % C);
     const size_t p = t / C;
-    st_split(out + p * out_Ctot + out_coff + c, ld_split(a + p * a_Ctot + a_coff + c, C) + ld_split(bsrc + p * b_Ctot + b_coff + c, C), C);
+    const float v = ld_split(a + p * a_Ctot + a_coff + c, C) + ld_split(bsrc + p * b_Ctot + b_coff + c, C);
+    st_split(out + p * out_Ctot + out_coff + c, relu ? fmaxf(v, 0.f) : v, C);
+  }
+}
+
+__global__ void k_maxpool3s2_split(const __half* __restrict__ in, int Hin, int Win, int in_Ctot, int in_coff, int C,
+                                   __half* __restrict__ out, int Hout, int Wout, int out_Ctot, int out_coff, size_t total) {
+  for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(t % C);
+    const int ox = (int)((t / C) % Wout);
+    const int oy = (int)((t / ((size_t)C * Wout)) % Hout);
+    const int b = (int)(t / ((size_t)C * Wout * Hout));
+    const __half* pin = in + (size_t)b * Hin * Win * in_Ctot + in_coff + c;
+    float m = -INFINITY;
+    for (int dy = -1; dy <= 1; ++dy)
+      for (int dx = -1; dx <= 1; ++dx) {
+        const int iy = 2 * oy + dy, ix = 2 * ox + dx;
+        m = fmaxf(m, (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) ? ld_split(pin + ((size_t)iy * Win + ix) * in_Ctot, C) : 0.f);
+      }
+    st_split(out + (((size_t)b * Hout + oy) * Wout + ox) * out_Ctot + out_coff + c, m, C);
   }
 }
 

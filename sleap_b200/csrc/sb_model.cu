@@ -101,6 +101,17 @@ int sb_load_model(sb_handle_t h, const int32_t* ops, int n_ops, const float* wei
       if (op.kind() < SB_OPK_CONV || op.kind() > SB_OPK_COPY) { delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: unknown kind %d", i, op.kind()); }
       if (!okbuf(op.out_buf()) || (op.kind() != SB_OPK_PREPROCESS && !okbuf(op.in_buf()))) { delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad buffer id", i); }
       if (op.kind() == SB_OPK_ADD && !okbuf(op.in2_buf())) { delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad second input", i); }
+      if (op.kind() == SB_OPK_CONV && op.residual() && (!okbuf(op.res_buf()) || !okbuf(op.sum_buf()))) {
+        delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad residual buffer id", i);
+      }
+      if (op.kind() == SB_OPK_CONV && op.explicit_pad() && (op.pad_top() < 0 || op.pad_left() < 0 || op.pad_top() >= op.k() || op.pad_left() >= op.k())) {
+        delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad explicit padding", i);
+      }
+      if (op.kind() == SB_OPK_TCONV && op.k() != 3 && op.k() != 4) { delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: transposed conv kernel %d (3 or 4)", i, op.k()); }
+      if (op.kind() == SB_OPK_POOL && op.k() != 0 && op.k() != 3) { delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad pool kind", i); }
+      if (op.kind() == SB_OPK_PREPROCESS && (op.pre_mode() < SB_PRE_PLAIN || op.pre_mode() > SB_PRE_IMAGENET_CAFFE_GRAY)) {
+        delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad preprocess mode", i);
+      }
       auto okoff = [&](int off, int64_t n) { return off < 0 ? true : (int64_t)off + n <= n_weights; };
       if (op.kind() == SB_OPK_CONV || op.kind() == SB_OPK_TCONV) {
         const int64_t nw = (int64_t)op.k() * op.k() * op.in_C() * op.out_C();
@@ -182,8 +193,8 @@ int sb_first_fusion_op(const SbModel* m, size_t pre_index) {
   if (pre_index + 1 >= m->ops.size()) return -1;
   const SbOp& pre = m->ops[pre_index];
   const SbOp& cv = m->ops[pre_index + 1];
-  if (cv.kind() != SB_OPK_CONV || cv.in_buf() != pre.out_buf() || cv.k() != 3 || cv.stride() != 1) return -1;
-  if (pre.input_scale() != 1.0f) return -1;
+  if (cv.kind() != SB_OPK_CONV || cv.in_buf() != pre.out_buf() || cv.k() != 3 || cv.stride() != 1 || cv.explicit_pad()) return -1;
+  if (pre.input_scale() != 1.0f || pre.pre_mode() != SB_PRE_PLAIN) return -1;
   const SbBuffer& ib = m->buffers[pre.out_buf()];
   const SbBuffer& ob = m->buffers[cv.out_buf()];
   if (m->Cin != ib.C || (ib.C != 1 && ib.C != 3) || cv.in_C() != ib.C) return -1;
@@ -202,10 +213,14 @@ int sb_stem_fusion_op(const SbModel* m, size_t pre_index) {
   if (m->precision != 0 || pre_index + 1 >= m->ops.size()) return -1;
   const SbOp& pre = m->ops[pre_index];
   const SbOp& cv = m->ops[pre_index + 1];
+  // SAME padding (hourglass) or the ResNet stem's explicit 3|3 padding after ImageNet preprocessing
   if (cv.kind() != SB_OPK_CONV || cv.in_buf() != pre.out_buf() || cv.k() != 7 || cv.stride() != 2) return -1;
+  if (cv.explicit_pad() && (cv.pad_top() != 3 || cv.pad_left() != 3)) return -1;
   if (pre.input_scale() != 1.0f) return -1;
   const SbBuffer& ib = m->buffers[pre.out_buf()];
-  if (m->Cin != ib.C || (ib.C != 1 && ib.C != 3) || cv.in_C() != ib.C) return -1;
+  if (pre.pre_mode() == SB_PRE_PLAIN ? (m->Cin != ib.C || (ib.C != 1 && ib.C != 3))
+                                     : (ib.C != 3 || (m->Cin != 1 && m->Cin != 3))) return -1;
+  if (cv.in_C() != ib.C) return -1;
   for (size_t i = pre_index + 2; i < m->ops.size(); ++i)      // nobody else may read the preprocessed frame
     if (m->ops[i].kind() != SB_OPK_PREPROCESS && (m->ops[i].in_buf() == pre.out_buf() ||
         (m->ops[i].kind() == SB_OPK_ADD && m->ops[i].in2_buf() == pre.out_buf()))) return -1;
@@ -260,7 +275,9 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
     if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[oi], s);
     SbBuffer& ob = m->buffers[op.out_buf()];
     if ((int)oi == m->guard_op && h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(s, h->post_done_ev, 0));
-    if (oi < m->skip_op.size() && m->skip_op[oi]) continue;     // 2x2 max-pool fused into the producing conv
+    // 2x2 max-pool fused into the producing conv; residual ADD fused into the conv before it (unless that conv's own output
+    // was asked for: it then stores its output and the ADD runs)
+    if (oi < m->skip_op.size() && (m->skip_op[oi] == 1 || (m->skip_op[oi] == 2 && !m->keep_dead_stores))) continue;
     if ((int)oi == fused_conv1) continue;                       // ran inside the fused first block
     if ((int)oi == fused_stem) {                                // 7x7 s2 stem: frame -> space-to-depth view -> tensor cores
       int rc = sb_stem_view_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
@@ -290,21 +307,23 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
         const size_t total = (size_t)B * ob.H * ob.W * ob.C;
         const int resize = op.input_scale() != 1.0f;
         int mode_ch = 0;
-        if (m->Cin == 3 && ob.C == 1) mode_ch = 1;
+        if (m->Cin == 3 && (ob.C == 1 || op.pre_mode() == SB_PRE_IMAGENET_CAFFE_GRAY)) mode_ch = 1;
         if (m->Cin == 1 && ob.C == 3) mode_ch = 2;
+        const int imagenet = op.pre_mode() != SB_PRE_PLAIN;
+        if (imagenet && ob.C != 3) return sb_fail(h, SB_ERR_INVALID, "ImageNet preprocessing needs a 3-channel network input");
         if (ob.f32 && sizeof(T) == 2) {          // precision 2 keeps the preprocessed frame in fp32
           if (frames_are_u8)
             k_preprocess<unsigned char, float><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-                (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total);
+                (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total, imagenet);
           else
             k_preprocess<float, float><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-                (const float*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total);
+                (const float*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total, imagenet);
         } else if (frames_are_u8)
           k_preprocess<unsigned char, T><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-              (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total);
+              (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total, imagenet);
         else
           k_preprocess<float, T><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-              (const float*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total);
+              (const float*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total, imagenet);
         SB_CHECK_LAUNCH(h);
         break;
       }
@@ -324,7 +343,7 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
         const int osplit = (split && !ob.f32) ? op.out_C() : 0;
         const int Hout = ob.H, Wout = ob.W;
         const int tot_h = std::max((Hout - 1) * st + k - ib.H, 0), tot_w = std::max((Wout - 1) * st + k - ib.W, 0);
-        const int pad_top = tot_h / 2, pad_left = tot_w / 2;
+        const int pad_top = op.explicit_pad() ? op.pad_top() : tot_h / 2, pad_left = op.explicit_pad() ? op.pad_left() : tot_w / 2;
         const float* W = m->weights_dev + op.w_off();
         const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
         const float* bs = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_scale_off() : nullptr;
@@ -364,7 +383,8 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
         const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
         dim3 g((ob.H * ob.W + 255) / 256, (op.out_C() + DC_CO - 1) / DC_CO, B);
         k_tconv_direct<T, T><<<g, 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (T*)ob.dev, ob.C,
-                                               op.out_coff(), op.out_C(), W, bias, (op.flags() & SB_OPF_RELU) ? 1 : 0, split ? op.out_C() : 0);
+                                               op.out_coff(), op.out_C(), W, bias, (op.flags() & SB_OPF_RELU) ? 1 : 0, split ? op.out_C() : 0,
+                                               op.k());
         SB_CHECK_LAUNCH(h);
         break;
       }
@@ -372,7 +392,14 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
         SbBuffer& ib = m->buffers[op.in_buf()];
         // precision 2: the record carries the physical channel count (3C); the split kernels work on logical channels
         const size_t total = (size_t)B * ob.H * ob.W * (split ? op.in_C() / 3 : op.in_C());
-        if (split)
+        if (op.k() == 3) {                      // ResNet stem: zero padding 1, 3x3 window, stride 2
+          if (split)
+            k_maxpool3s2_split<<<grid_for(total, h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C() / 3,
+                                                                            (__half*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
+          else
+            k_maxpool3s2<T><<<grid_for(total, h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(),
+                                                                         (T*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
+        } else if (split)
           k_maxpool2_split<<<grid_for(total, h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C() / 3,
                                                                         (__half*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
         else
@@ -399,13 +426,14 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
         SbBuffer& ib = m->buffers[op.in_buf()];
         SbBuffer& ib2 = m->buffers[op.in2_buf()];
         const size_t npix = (size_t)B * ob.H * ob.W;
+        const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
         if (split)
           k_add_split<<<grid_for(npix * (op.in_C() / 3), h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.C, op.in_coff(), (const __half*)ib2.dev,
                                                                                      ib2.C, op.in2_coff(), (__half*)ob.dev, ob.C, op.out_coff(),
-                                                                                     op.in_C() / 3, npix);
+                                                                                     op.in_C() / 3, npix, relu);
         else
         k_add<T><<<grid_for(npix * op.in_C(), h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.C, op.in_coff(), (const T*)ib2.dev, ib2.C,
-                                                                         op.in2_coff(), (T*)ob.dev, ob.C, op.out_coff(), op.in_C(), npix);
+                                                                         op.in2_coff(), (T*)ob.dev, ob.C, op.out_coff(), op.in_C(), npix, relu);
         SB_CHECK_LAUNCH(h);
         break;
       }

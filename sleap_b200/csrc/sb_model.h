@@ -15,7 +15,11 @@ enum {
   SB_OPK_PREPROCESS = 6,
   SB_OPK_COPY = 7,
 };
-enum { SB_OPF_RELU = 1, SB_OPF_BN = 2, SB_OPF_BILINEAR = 8, SB_OPF_FUSED_POOL = 16 };
+enum { SB_OPF_RELU = 1, SB_OPF_BN = 2, SB_OPF_BILINEAR = 8, SB_OPF_FUSED_POOL = 16, SB_OPF_EXPLICIT_PAD = 32,
+       SB_OPF_FUSED_ADD = 64, SB_OPF_RESIDUAL = 128 };
+// PREPROCESS modes: IMAGENET_CAFFE(_GRAY) = pretrained ResNet trained on colour (grayscale) frames; _GRAY converts
+// colour frames to gray before tile_channels
+enum { SB_PRE_PLAIN = 0, SB_PRE_IMAGENET_CAFFE = 1, SB_PRE_IMAGENET_CAFFE_GRAY = 2 };
 
 struct SbOp {
   int32_t w[SB_OP_WORDS];
@@ -40,9 +44,22 @@ struct SbOp {
   //       ran on the tensor-core path.
   int pool_buf() const { return w[18]; }
   int pool_coff() const { return w[19]; }
-  // PREPROCESS: w[16] = float bits of input_scale, w[17] = pad_to_stride
+  // CONV with SB_OPF_EXPLICIT_PAD: w[16] / w[17] = top / left zero padding (otherwise TF SAME, derived from the shapes)
+  bool explicit_pad() const { return (w[11] & SB_OPF_EXPLICIT_PAD) != 0; }
+  int pad_top() const { return w[16]; }
+  int pad_left() const { return w[17]; }
+  // CONV with SB_OPF_RESIDUAL: the ADD op right after it (flag SB_OPF_FUSED_ADD) sums this conv's output and the
+  // shortcut slice (w[20], w[21]) into the sum slice (w[22], w[23]); the tensor-core path does it in the epilogue and
+  // the ADD op is then skipped
+  bool residual() const { return (w[11] & SB_OPF_RESIDUAL) != 0; }
+  int res_buf() const { return w[20]; }
+  int res_coff() const { return w[21]; }
+  int sum_buf() const { return w[22]; }
+  int sum_coff() const { return w[23]; }
+  // PREPROCESS: w[16] = float bits of input_scale, w[17] = pad_to_stride, w[19] = SB_PRE_* mode
   float input_scale() const { float f; memcpy(&f, &w[16], 4); return f; }
   int pad_stride() const { return w[17]; }
+  int pre_mode() const { return w[19]; }
 };
 
 struct SbBuffer {
@@ -68,7 +85,7 @@ struct SbModel {
   size_t act_bytes = 0;
   void* frames_dev = nullptr;
   std::vector<SbConvTcPlan*> tc_plans;  // per op (nullptr = direct path)
-  std::vector<char> skip_op;            // POOL ops fused into the producing tensor-core conv
+  std::vector<char> skip_op;            // 1: POOL fused into the producing tensor-core conv; 2: ADD fused into the conv before it
   std::vector<cudaEvent_t> prof_events; // non-empty only inside sb_model_profile_ops
   std::vector<cudaEvent_t> fwd_events;  // sb_model_forward_times: (start, end) pairs around every forward pass
   int fwd_n = 0;                        // pairs recorded since the last read

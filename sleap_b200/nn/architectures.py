@@ -4,12 +4,19 @@ Restates the *topology* (not the execution) of the reference's Keras graph build
   sleap/nn/architectures/unet.py:43-278          UNet block stacks and from_config
   sleap/nn/architectures/encoder_decoder.py:94-144, 275-399, 508-676
   sleap/nn/architectures/hourglass.py:17-305
+  sleap/nn/architectures/resnet.py:88-702         ResNet50 / 101 / 152 (v1) with the UpsamplingStack decoder
+  sleap/nn/architectures/upsampling.py:90-259
+  sleap/nn/architectures/leap.py:14-131           LeapCNN
   sleap/nn/heads.py:42-63, sleap/nn/model.py:104-364 (head taps by output stride, output order)
 Layer names follow the reference's Keras layer names so that weights exported from a
 ``best_model.h5`` map 1:1 (``{layer_name: {"kernel", "bias", ...}}``, Keras layouts).
 
 Concatenated skip connections are realised by construction: the producer of each part writes
 straight into its channel slice of the concat buffer, so no concat kernel exists.
+
+Backbones: UNet, hourglass, ResNet (v1, ``resnet``) and LEAP (``leap``).  ``pretrained_encoder`` models are not
+supported: their encoders are built by the third-party ``segmentation_models`` package, whose layer graph is not part
+of the reference and so cannot be restated and checked here.
 """
 import math
 from typing import Dict, List, Optional
@@ -19,6 +26,9 @@ import numpy as np
 from sleap_b200.nn import oplist as ol
 
 BN_EPS = 1e-3  # Keras BatchNormalization default
+RESNET_BN_EPS = 1.001e-5   # resnet.py: every BatchNormalization of the ResNet backbone
+RESNET_STACKS = {"ResNet50": (3, 4, 6, 3), "ResNet101": (3, 4, 23, 3), "ResNet152": (3, 8, 36, 3)}
+IMAGENET_CAFFE_MEAN_BGR = (103.939, 116.779, 123.68)   # resnet.py imagenet_preproc_v1
 
 HEAD_CLASS_NAMES = {
     "single_instance": "SingleInstanceConfmapsHead",
@@ -48,23 +58,33 @@ class GraphBuilder:
         self.tensors.append(t)
         return t
 
-    def conv(self, x, filters, k, name, stride=1, relu=True, bn=None, f32_out=False):
+    def conv(self, x, filters, k, name, stride=1, relu=True, bn=None, f32_out=False, bn_pre=None, bn_eps=BN_EPS, pad=None):
+        """``bn``: BatchNormalization AFTER the ReLU (hourglass), applied as the epilogue affine.  ``bn_pre``:
+        BatchNormalization BEFORE the ReLU (ResNet, upsampling stack), folded into the kernel and bias at pack time.
+        ``pad``: explicit (top, left) zero padding (bottom / right follow from the output size), None = TF SAME."""
         y = self.tensor(filters, x.stride * stride, f32_out, name)
-        self.sym_ops.append(("conv", dict(x=x, y=y, k=k, stride=stride, relu=relu, bn=bn, name=name)))
+        self.sym_ops.append(("conv", dict(x=x, y=y, k=k, stride=stride, relu=relu, bn=bn, name=name, pad=pad)))
         self.layers.append(dict(name=name, kind="conv", k=k, cin=x.C, cout=filters))
         if bn:
-            self.layers.append(dict(name=bn, kind="bn", c=filters))
+            self.layers.append(dict(name=bn, kind="bn", c=filters, eps=BN_EPS))
+        if bn_pre:
+            self.layers[-1]["fold_bn"] = bn_pre
+            self.layers.append(dict(name=bn_pre, kind="bn", c=filters, eps=bn_eps, folded=True))
         return y
 
-    def tconv(self, x, filters, name):
+    def tconv(self, x, filters, name, k=3, bn_pre=None, bn_eps=BN_EPS):
         y = self.tensor(filters, x.stride // 2, False, name)
-        self.sym_ops.append(("tconv", dict(x=x, y=y, k=3, name=name)))
-        self.layers.append(dict(name=name, kind="tconv", k=3, cin=x.C, cout=filters))
+        self.sym_ops.append(("tconv", dict(x=x, y=y, k=k, name=name)))
+        self.layers.append(dict(name=name, kind="tconv", k=k, cin=x.C, cout=filters))
+        if bn_pre:
+            self.layers[-1]["fold_bn"] = bn_pre
+            self.layers.append(dict(name=bn_pre, kind="bn", c=filters, eps=bn_eps, folded=True))
         return y
 
-    def pool(self, x, name="pool"):
+    def pool(self, x, name="pool", k=2):
+        """k = 2: MaxPool2D(2, 2, SAME); k = 3: ZeroPadding2D(1) + MaxPool2D(3, 2) (ResNet stem)."""
         y = self.tensor(x.C, x.stride * 2, False, name)
-        self.sym_ops.append(("pool", dict(x=x, y=y)))
+        self.sym_ops.append(("pool", dict(x=x, y=y, k=k)))
         return y
 
     def upsample(self, x, bilinear, name="up"):
@@ -72,9 +92,9 @@ class GraphBuilder:
         self.sym_ops.append(("up", dict(x=x, y=y, bilinear=bilinear)))
         return y
 
-    def add(self, a, b, name="add"):
+    def add(self, a, b, name="add", relu=False):
         y = self.tensor(a.C, a.stride, False, name)
-        self.sym_ops.append(("add", dict(a=a, b=b, y=y)))
+        self.sym_ops.append(("add", dict(a=a, b=b, y=y, relu=relu)))
         return y
 
     def concat(self, parts, name="concat"):
@@ -216,11 +236,126 @@ def build_hourglass(g: GraphBuilder, x: _T, cfg):
     return outs, mids
 
 
+def build_resnet(g: GraphBuilder, x: _T, cfg):
+    """ResNetv1.make_backbone (resnet.py): stem, stacks of bottleneck blocks (block_v1 / stack_v1), optional
+    UpsamplingStack.  Layer names are the flat Keras names (``conv1_conv``, ``conv2_block1_0_conv``, ...)."""
+    version = cfg.get("version", "ResNet50")
+    if version not in RESNET_STACKS:
+        raise ValueError(f"Invalid ResNet version in the configuration: {version}")
+    max_stride = int(cfg.get("max_stride", 32))
+    if max_stride not in (4, 8, 16, 32):
+        raise ValueError(f"ResNet max_stride must be 4, 8, 16 or 32, got {max_stride}.")
+    eps = RESNET_BN_EPS
+
+    def cbn(t, f, k, name, stride=1, relu=True, pad=None):
+        return g.conv(t, f, k, name + "_conv", stride=stride, relu=relu, bn_pre=name + "_bn", bn_eps=eps, pad=pad)
+
+    # stem: ZeroPadding2D(3) + Conv2D(7, s2, VALID) -- 3|3 padding, not SAME's 2|3 -- BN, ReLU; then ZeroPadding2D(1) +
+    # MaxPooling2D(3, s2, VALID)
+    x = cbn(x, 64, 7, "conv1", stride=2, pad=(3, 3))
+    feats = [x]
+    x = g.pool(x, "pool1_pool", k=3)
+    feats.append(x)
+
+    def block(t, filters, stride, shortcut, name):
+        # the 1x1 convs are VALID; with kernel 1 and an even input (every buffer is a multiple of the stride) VALID and
+        # SAME coincide: padding 0|0
+        sc = cbn(t, 4 * filters, 1, name + "_0", stride=stride, relu=False, pad=(0, 0)) if shortcut else t
+        y = cbn(t, filters, 1, name + "_1", stride=stride, pad=(0, 0))
+        y = cbn(y, filters, 3, name + "_2")
+        y = cbn(y, 4 * filters, 1, name + "_3", relu=False)
+        return g.add(sc, y, name + "_add", relu=True)
+
+    cur = 4
+    for si, (filters, n_blocks, stride1) in enumerate(zip((64, 128, 256, 512), RESNET_STACKS[version], (1, 2, 2, 2))):
+        if cur < max_stride:
+            cur *= stride1
+        else:
+            # make_backbone_fn: the stack's stride becomes 1 and its dilation_rate doubles.  The dilation only reaches the
+            # first block's 1x1 convs (_0_conv, _1_conv), where it has no effect, so it is dropped here.
+            stride1 = 1
+        for b in range(1, n_blocks + 1):
+            x = block(x, filters, stride1 if b == 1 else 1, b == 1, f"conv{si + 2}_block{b}")
+        feats.append(x)
+
+    up = cfg.get("upsampling")
+    if not up:
+        return [x], [feats]
+    if int(up.get("block_stride", 2)) != 2:
+        raise ValueError("Upsampling block_stride other than 2 is not supported.")
+    transposed = up.get("method", "interpolation") == "transposed_conv"
+    skip_mode = up.get("skip_connections")
+    filters, rate = up.get("filters", 64), up.get("filters_rate", 1)
+    refine, bn, tk = int(up.get("refine_convs", 2)), bool(up.get("batch_norm", True)), int(up.get("transposed_conv_kernel_size", 4))
+    if transposed and tk not in (3, 4):
+        raise ValueError(f"Transposed convolution kernel size {tk} is not supported (3 or 4).")
+    skip_sources = feats[2:] if skip_mode else []          # the stack outputs (intermediate_feats[2:])
+    mids = [x]
+    cur = max_stride
+    n_up = int(round(math.log2(max_stride / cfg["output_stride"])))
+    for blk in range(n_up):
+        new = cur // 2
+        prefix = f"upsample_s{cur}_to_s{new}"
+        f = int(filters * rate ** blk)
+        if transposed:
+            # Conv2DTranspose -> (BatchNormalization, Keras default eps) -> ReLU: BN folded, ReLU in the epilogue
+            x = g.tconv(x, f, prefix + "_trans_conv", k=tk, bn_pre=prefix + "_bn" if bn else None)
+        else:
+            x = g.upsample(x, True, prefix + "_interp")
+        cur = new
+        skip = next((t for t in skip_sources if t.stride == cur), None)
+        if skip is not None:
+            if skip_mode == "add":
+                src = skip if skip.C == x.C else g.conv(skip, x.C, 1, prefix + "_skip_conv1x1", relu=False)
+                x = g.add(src, x, prefix + "_skip_add")
+            else:
+                x = g.concat([skip, x], prefix + "_skip_concat")
+        for i in range(refine):
+            x = g.conv(x, f, 3, prefix + f"_refine{i}_conv", bn_pre=prefix + f"_refine{i}_bn" if bn else None)
+        mids.append(x)
+    return [x], [mids]
+
+
+def build_leap(g: GraphBuilder, x: _T, cfg):
+    """LeapCNN.from_config (leap.py) on EncoderDecoder: 3 convs + 2x2 max-pool per down block, transposed conv k3 s2
+    (or bilinear x2) + 2 refine convs per up block, no skip connections."""
+    filters, rate = cfg.get("filters", 64), cfg.get("filters_rate", 2)
+    down = int(round(math.log2(cfg["max_stride"])))
+    up = int(round(math.log2(cfg["max_stride"] / cfg["output_stride"])))
+    interp = cfg.get("up_interpolate", False)
+    if cfg.get("stacks", 1) > 1 and cfg["output_stride"] != 1:       # EncoderDecoder.make_backbone (encoder_decoder.py:633-639)
+        raise ValueError("If using a stacked configuration, the backbone must define symmetric encoder and decoder. "
+                         "Create a stem for initial downsampling if an output stride > 1 is desired.")
+    outs, mids = [], []
+    for s in range(cfg.get("stacks", 1)):
+        for i in range(down):
+            for j in range(3):
+                x = g.conv(x, int(filters * rate ** i), 3, f"stack{s}_enc{i}_conv{j}")
+            x = g.pool(x, f"stack{s}_enc{i}_pool")
+        inter = []
+        for i, e in enumerate(range(up, 0, -1)):
+            inter.append(x)
+            f = int(filters * rate ** e)
+            prefix = f"stack{s}_dec{i}_s{x.stride}_to_s{x.stride // 2}"
+            x = g.upsample(x, True, prefix + "_interp_bilinear") if interp else g.tconv(x, f, prefix + "_trans_conv")
+            for j in range(2):
+                x = g.conv(x, f, 3, prefix + f"_refine_conv{j}")
+        outs.append(x)
+        mids.append(inter)
+    return outs, mids
+
+
+def resnet_pretrained(spec) -> bool:
+    """``weights != "random"`` (the default "frozen" included): the graph starts with tile_channels (1 -> 3) and
+    imagenet_preproc_v1."""
+    return spec["backbone"] == "resnet" and spec["backbone_cfg"].get("weights", "frozen") != "random"
+
+
 # ------------------------------------------------------------------------------------------
 def spec_from_config(model_cfg: dict, skeleton_nodes=None, skeleton_edges=None):
     """``training_config.json["model"]`` -> internal spec.
 
-    spec = {"backbone": "unet"|"hourglass", "backbone_cfg": {...}, "head_type": str,
+    spec = {"backbone": "unet"|"hourglass"|"resnet"|"leap", "backbone_cfg": {...}, "head_type": str,
             "heads": [{"name", "channels", "output_stride"}...], "part_names", "edges"}
     Mirrors Model.from_config (model.py:104-305): head list order = [confmaps, pafs, (offsets)].
     """
@@ -228,8 +363,11 @@ def spec_from_config(model_cfg: dict, skeleton_nodes=None, skeleton_edges=None):
     if len(bb) != 1:
         raise ValueError("Backbone architecture (config.model.backbone) was not specified.")
     bname, bcfg = next(iter(bb.items()))
-    if bname not in ("unet", "hourglass"):
-        raise ValueError(f"Backbone '{bname}' is outside the scope of this build (UNet / hourglass only).")
+    if bname == "pretrained_encoder":
+        raise ValueError("Backbone 'pretrained_encoder' is not supported: its encoder is built by the third-party "
+                         "segmentation_models package, whose layer graph this library cannot restate and check.")
+    if bname not in ("unet", "hourglass", "resnet", "leap"):
+        raise ValueError(f"Backbone '{bname}' is outside the scope of this build (UNet / hourglass / ResNet / LEAP only).")
     hd = {k: v for k, v in model_cfg["heads"].items() if v is not None}
     if len(hd) != 1:
         raise ValueError("Head configuration (config.model.heads) was not specified.")
@@ -320,33 +458,53 @@ class CompiledModel:
     def ops_array(self):
         return np.ascontiguousarray(np.stack(self.records).astype(np.int32))
 
+    def folded_kernel_bias(self, L, weights):
+        """Kernel (kh, kw, Cin, Cout) and bias of a conv / transposed conv in float32, with a BatchNormalization that
+        follows it before the activation folded in: W' = W * s, b' = b * s + t (s, t: bn_affine)."""
+        p = weights[L["name"]]
+        kern = np.asarray(p["kernel"], np.float32)
+        if L["kind"] == "tconv":
+            kern = np.transpose(kern, (0, 1, 3, 2))     # (kh,kw,Cout,Cin) -> (kh,kw,Cin,Cout)
+        assert kern.shape == (L["k"], L["k"], L["cin"], L["cout"]), (L["name"], kern.shape)
+        bias = p.get("bias")
+        bias = np.zeros((L["cout"],), np.float32) if bias is None else np.asarray(bias, np.float32)
+        if L.get("fold_bn"):
+            bn = next(B for B in self.layers if B["name"] == L["fold_bn"])
+            scale, shift = bn_affine(weights[bn["name"]], bn["eps"])
+            kern = (kern * scale).astype(np.float32)
+            bias = (bias * scale + shift).astype(np.float32)
+        return kern, bias
+
     def pack_weights(self, weights: Dict[str, Dict[str, np.ndarray]]) -> np.ndarray:
-        """Keras-layout weights dict -> flat float32 blob in the kernel layouts."""
+        """Keras-layout weights dict -> flat float32 blob in the kernel layouts.  BatchNormalization layers before an
+        activation are folded into the conv before them (before precision 2's hi / lo split of the weights)."""
         blob = np.zeros((self.n_weights,), np.float32)
         for L in self.layers:
+            if L.get("folded"):
+                continue
             slot = self._w_slots[L["name"]]
             p = weights[L["name"]]
             if L["kind"] in ("conv", "tconv"):
-                kern = np.asarray(p["kernel"], np.float32)
-                if L["kind"] == "tconv":
-                    kern = np.transpose(kern, (0, 1, 3, 2))     # (kh,kw,Cout,Cin) -> (kh,kw,Cin,Cout)
-                assert kern.shape == (L["k"], L["k"], L["cin"], L["cout"]), (L["name"], kern.shape)
+                kern, bias = self.folded_kernel_bias(L, weights)
                 if "expand" in L:        # precision 2: input rows in the physical order of the split input, [Wh | Wl | Wh]
                     src, part = L["expand"]
                     wh = kern.astype(np.float16).astype(np.float32)
                     wl = (kern - wh).astype(np.float16).astype(np.float32)
                     kern = np.where((part == 1)[None, None, :, None], wl[:, :, src, :], wh[:, :, src, :])
                 blob[slot["w"]:slot["w"] + kern.size] = kern.reshape(-1)
-                bias = p.get("bias")
-                if bias is None:
-                    bias = np.zeros((L["cout"],), np.float32)
-                blob[slot["b"]:slot["b"] + L["cout"]] = np.asarray(bias, np.float32)
+                blob[slot["b"]:slot["b"] + L["cout"]] = bias
             else:  # bn -> affine (scale, shift), exact Keras inference formula
-                scale = (np.asarray(p["gamma"], np.float32) / np.sqrt(np.asarray(p["var"], np.float32) + np.float32(BN_EPS))).astype(np.float32)
-                shift = (np.asarray(p["beta"], np.float32) - np.asarray(p["mean"], np.float32) * scale).astype(np.float32)
+                scale, shift = bn_affine(p, L["eps"])
                 blob[slot["scale"]:slot["scale"] + L["c"]] = scale
                 blob[slot["shift"]:slot["shift"] + L["c"]] = shift
         return blob
+
+
+def bn_affine(p, eps):
+    """BatchNormalization (inference) as a per-channel affine: scale = gamma / sqrt(var + eps), shift = beta - mean * scale."""
+    scale = (np.asarray(p["gamma"], np.float32) / np.sqrt(np.asarray(p["var"], np.float32) + np.float32(eps))).astype(np.float32)
+    shift = (np.asarray(p["beta"], np.float32) - np.asarray(p["mean"], np.float32) * scale).astype(np.float32)
+    return scale, shift
 
 
 def _compile_identity(spec: dict, input_channels: int, input_scale: float, pad_to_stride: Optional[int]) -> CompiledModel:
@@ -377,9 +535,22 @@ def compile_model(spec: dict, input_channels: int, input_scale: float = 1.0, pad
         return _compile_identity(spec, input_channels, input_scale, pad_to_stride)
     g = GraphBuilder()
     net_c = input_channels
+    pre_mode = ol.PRE_PLAIN
+    if resnet_pretrained(spec):
+        # tile_channels + imagenet_preproc_v1: the buffer after PREPROCESS has 3 caffe-normalised BGR channels.
+        # ``input_channels`` is the channel count of the model's Keras input (its training frames): 1 -> colour frames
+        # are converted to gray and the gray plane is tiled (PRE_IMAGENET_CAFFE_GRAY); 3 -> grayscale frames are tiled.
+        net_c = 3
+        pre_mode = ol.PRE_IMAGENET_CAFFE_GRAY if input_channels == 1 else ol.PRE_IMAGENET_CAFFE
     x0 = g.tensor(net_c, 1, False, "input")
     if spec["backbone"] == "unet":
         outs, mids = build_unet(g, x0, spec["backbone_cfg"])
+        max_stride = spec["backbone_cfg"]["max_stride"]
+    elif spec["backbone"] == "resnet":
+        outs, mids = build_resnet(g, x0, spec["backbone_cfg"])
+        max_stride = int(spec["backbone_cfg"].get("max_stride", 32))
+    elif spec["backbone"] == "leap":
+        outs, mids = build_leap(g, x0, spec["backbone_cfg"])
         max_stride = spec["backbone_cfg"]["max_stride"]
     else:
         outs, mids = build_hourglass(g, x0, spec["backbone_cfg"])
@@ -454,7 +625,7 @@ def compile_model(spec: dict, input_channels: int, input_scale: float = 1.0, pad
     cm.n_buffers = len(bufs)
     for i, (C, stride, f32) in enumerate(bufs):
         cm.records.append(ol.buffer_record(i, stride, C, f32, 1 if i == 0 else 0))
-    cm.records.append(ol.preprocess_record(0, net_c, input_scale, pad_to_stride or max_stride))
+    cm.records.append(ol.preprocess_record(0, net_c, input_scale, pad_to_stride or max_stride, pre_mode))
 
     # ---- weights layout ----
     if split:
@@ -465,6 +636,8 @@ def compile_model(spec: dict, input_channels: int, input_scale: float = 1.0, pad
                 by_name[o["name"]]["expand"] = (src, part)
     off = 0
     for L in g.layers:
+        if L.get("folded"):
+            continue
         if L["kind"] in ("conv", "tconv"):
             n = L["k"] * L["k"] * (len(L["expand"][0]) if "expand" in L else L["cin"]) * L["cout"]
             cm._w_slots[L["name"]] = dict(w=off, b=off + n)
@@ -476,8 +649,16 @@ def compile_model(spec: dict, input_channels: int, input_scale: float = 1.0, pad
     cm.n_weights = off
     cm.layers = g.layers
 
+    def n_readers(t):
+        n = 0
+        for kind_, o_ in g.sym_ops:
+            ins = o_["parts"] if kind_ == "concat" else ([o_["a"], o_["b"]] if kind_ == "add" else [o_["x"]])
+            n += sum(1 for u in ins if u is t)
+        return n
+
+    tapped = {t.id for t in vec_t.values()}
     flops = 0.0
-    fused_pools = set()
+    fused_pools, fused_adds = set(), set()
     for idx, (kind, o) in enumerate(g.sym_ops):
         for (src, dbuf, dcoff) in copies_before.get(idx, []):
             cm.records.append(ol.copy_record(src.buf, src.coff, pc(src), dbuf, dcoff))
@@ -493,23 +674,34 @@ def compile_model(spec: dict, input_channels: int, input_scale: float = 1.0, pad
                 py = g.sym_ops[idx + 1][1]["y"]
                 pool_buf, pool_coff = py.buf, py.coff
                 fused_pools.add(idx + 1)
+            # an ADD right after this conv with this conv's output as one operand, which nothing else reads: offered to
+            # the conv's epilogue (residual add + the ADD's ReLU); the ADD record stays, flagged, for the CUDA-core path
+            res = None
+            if idx + 1 < len(g.sym_ops) and g.sym_ops[idx + 1][0] == "add" and not copies_before.get(idx + 1) \
+                    and not y.f32 and not o["relu"] and not o["bn"] and pool_buf < 0:
+                ao = g.sym_ops[idx + 1][1]
+                other = ao["b"] if ao["a"] is y else (ao["a"] if ao["b"] is y else None)
+                if other is not None and other is not y and n_readers(y) == 1 and y.id not in tapped:
+                    res = (other.buf, other.coff, ao["y"].buf, ao["y"].coff)
+                    fused_adds.add(idx + 1)
             cm.records.append(ol.conv_record(x.buf, x.coff, pc(x), y.buf, y.coff, y.C, o["k"], o["stride"],
                                              relu=o["relu"], w_off=slot["w"], b_off=slot["b"],
                                              bn_scale_off=bn["scale"] if bn else -1, bn_shift_off=bn["shift"] if bn else -1,
-                                             pool_buf=pool_buf, pool_coff=pool_coff))
+                                             pool_buf=pool_buf, pool_coff=pool_coff, pad=o.get("pad"), res=res))
             flops += 2.0 * o["k"] * o["k"] * x.C * y.C / (y.stride ** 2)
         elif kind == "tconv":
             x, y = o["x"], o["y"]
             slot = cm._w_slots[o["name"]]
-            cm.records.append(ol.tconv_record(x.buf, x.coff, pc(x), y.buf, y.coff, y.C, w_off=slot["w"], b_off=slot["b"]))
-            flops += 2.0 * 9 * x.C * y.C / (x.stride ** 2)     # 2*9*Cin*Cout MACs per *input* pixel (Keras count)
+            cm.records.append(ol.tconv_record(x.buf, x.coff, pc(x), y.buf, y.coff, y.C, w_off=slot["w"], b_off=slot["b"], k=o["k"]))
+            flops += 2.0 * o["k"] ** 2 * x.C * y.C / (x.stride ** 2)     # 2*k*k*Cin*Cout MACs per *input* pixel (Keras count)
         elif kind == "pool":
             cm.records.append(ol.pool_record(o["x"].buf, o["x"].coff, pc(o["x"]), o["y"].buf, o["y"].coff,
-                                             fused=idx in fused_pools))
+                                             fused=idx in fused_pools, k=o["k"]))
         elif kind == "up":
             cm.records.append(ol.upsample_record(o["x"].buf, o["x"].coff, pc(o["x"]), o["y"].buf, o["y"].coff, o["bilinear"]))
         elif kind == "add":
-            cm.records.append(ol.add_record(o["a"].buf, o["a"].coff, o["b"].buf, o["b"].coff, pc(o["a"]), o["y"].buf, o["y"].coff))
+            cm.records.append(ol.add_record(o["a"].buf, o["a"].coff, o["b"].buf, o["b"].coff, pc(o["a"]), o["y"].buf, o["y"].coff,
+                                            relu=o["relu"], fused=idx in fused_adds))
         elif kind == "concat":
             pass
     cm.flops_per_pixel = flops
@@ -535,8 +727,8 @@ def make_synthetic_weights(cm: CompiledModel, seed: int) -> Dict[str, Dict[str, 
             w[L["name"]] = dict(kernel=(rng.standard_normal((L["k"], L["k"], L["cin"], L["cout"])) * std).astype(np.float32),
                                 bias=np.zeros((L["cout"],), np.float32))
         elif L["kind"] == "tconv":
-            # effective fan-in of a k3 s2 transposed conv is ~ (9/4) * Cin taps per output pixel
-            std = math.sqrt(2.0 / (2.25 * L["cin"]))
+            # effective fan-in of a k s2 transposed conv is ~ (k^2/4) * Cin taps per output pixel
+            std = math.sqrt(2.0 / (L["k"] ** 2 / 4.0 * L["cin"]))
             w[L["name"]] = dict(kernel=(rng.standard_normal((L["k"], L["k"], L["cout"], L["cin"])) * std).astype(np.float32),
                                 bias=np.zeros((L["cout"],), np.float32))
         else:

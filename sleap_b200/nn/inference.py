@@ -944,6 +944,10 @@ class Predictor:
         # ``is_grayscale``); here it is the C_in of the first convolution's kernel.
         first = arch.compile_model(spec, 1).layers[0]["name"]
         in_ch = int(np.asarray(weights[first]["kernel"]).shape[2])
+        if arch.resnet_pretrained(spec):
+            # conv1_conv always sees 3 channels after tile_channels; the model's own input has 1 channel when it was
+            # trained on grayscale frames (colour frames are then converted to gray before the tile, :1477, :3149)
+            in_ch = 1 if pre.get("ensure_grayscale") else 3
         scale = float(pre.get("input_scaling", 1.0) or 1.0)
         model = DeviceModel(spec, weights, input_channels=in_ch, input_scale=scale if resize_in_graph else 1.0,
                             pad_to_stride=pre.get("pad_to_stride"), precision=precision, handle=handle)

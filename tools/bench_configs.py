@@ -2,7 +2,11 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
+
+r50: ResNet50 bottom-up (ImageNet-preprocessed "frozen" weights, upsampling stack to stride 4 with k4 transposed convs,
+BN, two refine convs, concat skips), 1024x1024x1, flies13, B=8 per GPU; it also reports the fp16 maps against the fp32
+path as a fraction of the map maximum.
 """
 import json
 import os
@@ -126,6 +130,45 @@ def hourglass(steps, B=16):
             "clocks": LAST_CLOCKS, "roofline": roofline(gf, B / dt)}
 
 
+def gpu_identity():
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    return q.stdout.strip()
+
+
+def resnet50(steps, B=8):
+    edges = [("head", "thorax"), ("thorax", "abdomen"), ("thorax", "wingL"), ("thorax", "wingR"), ("thorax", "forelegL"),
+             ("thorax", "forelegR"), ("thorax", "midlegL"), ("thorax", "midlegR"), ("thorax", "hindlegL"), ("thorax", "hindlegR"),
+             ("head", "eyeL"), ("head", "eyeR")]
+    up = dict(method="transposed_conv", skip_connections="concatenate", block_stride=2, filters=64, filters_rate=1, refine_convs=2,
+              batch_norm=True, transposed_conv_kernel_size=4)
+    spec = dict(backbone="resnet", backbone_cfg=dict(version="ResNet50", weights="frozen", max_stride=32, output_stride=4, upsampling=up),
+                head_type="multi_instance", part_names=FLIES13, edges=edges,
+                heads=[dict(name="MultiInstanceConfmapsHead", channels=13, output_stride=4),
+                       dict(name="PartAffinityFieldsHead", channels=24, output_stride=8)])
+    cm = A.compile_model(spec, 1)
+    w = A.make_synthetic_weights(cm, 1006)
+    for L in cm.layers:        # keep 16 residual blocks of He-normal weights in a sane range
+        if L["name"].endswith("_3_bn"):
+            w[L["name"]]["gamma"] = np.full(L["c"], 0.3, np.float32)
+    m = DeviceModel(spec, w, input_channels=1, precision=0)
+    fr = frames(B, 1024, 1024, 1, 7)
+    cms, pafs = m.forward(fr[:2])
+    ref = DeviceModel(spec, w, input_channels=1, precision=1).forward(fr[:2])
+    err = [float(np.abs(a - b).max() / np.abs(b).max()) for a, b in zip((cms, pafs), ref)]
+    thr = float(np.quantile(cms, 1 - 5.0 / (256 * 256)))
+    pred = BottomUpPredictor(m, FLIES13, edges, peak_threshold=thr, batch_size=B, max_peaks_per_sample=4096,
+                             max_node_peaks=64, max_instances_per_frame=64)
+    pred.inference_model.predict_on_batch(fr)
+    dt = timed(lambda: pred.inference_model.predict_on_batch(fr), steps, warmup=2)
+    gf = cm.flops_per_pixel * 1024 * 1024 / 1e9
+    tf = gf * B / dt / 1e3
+    return {"config": f"R50 ResNet50 bottom-up 1024x1024x1, flies13, upsampling to stride 4 (k4 tconv + BN + 2 refine, concat skips), B={B}",
+            "metric": "frames/s (predict_on_batch, host frames)", "value": B / dt, "ms_per_step": dt * 1e3, "batch": B,
+            "gflop_per_frame": gf, "tflops": tf, "frac_of_989_dense_fp16_tflops": tf / 989.0, "gpu": gpu_identity(),
+            "fp16_vs_fp32_maps_max_err_frac": err, "dtype": "f16", "clocks": LAST_CLOCKS}
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -136,6 +179,8 @@ if __name__ == "__main__":
             r = single("C2 single-instance UNet 512x512x1, 13 nodes, B=32", 512, FLIES13, 32, steps)
         elif c == "c3":
             r = topdown(steps)
+        elif c == "r50":
+            r = resnet50(steps)
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
