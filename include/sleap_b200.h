@@ -330,6 +330,31 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
                      float* out_centroids, float* out_centroid_vals, float* out_instance_peaks,
                      float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
 
+/* ---- flow shift for the optical-flow trackers ----------------------------------------------
+ * sleap/nn/tracking.py:262-360 FlowCandidateMaker.flow_shift_instances = cv2.calcOpticalFlowPyrLK(prev, next,
+ * pts, winSize=(window, window), maxLevel=max_levels, criteria=(EPS|COUNT, 30, 0.01)) on gray (cv2.COLOR_BGR2GRAY)
+ * frames resized by img_scale.  A flow object keeps the image pyramids and Scharr derivatives of the last `ring`
+ * frames on the device, keyed by frame index t, so that every frame's pyramid is built once however many later
+ * frames shift points out of it.  Gray conversion, resize, pyramid and derivatives are bit-exact with OpenCV; the
+ * LK iteration agrees with it to the size of its stopping step.
+ *   window: 3..41; max_levels >= 0; img_scale: 1 or 0.5 (others return SB_ERR_UNSUPPORTED); ring: 2..64.
+ * frame_host: uint8 (H, W, C), C = 1 or 3 (3 = BGR order, as the reference calls cvtColor).  A frame of another
+ * size than the ring holds empties the ring.  replace = 0 keeps a frame already held under t and skips the upload.
+ * When every slot is taken, the slot used least recently (added or read by a shift) is replaced.
+ * sb_flow_shift: point i (pts[2i], pts[2i+1], in the resized frame's pixels) moves from frame ref_t[i] into frame t.
+ * out_status[i] = 1 when found; out_err[i] = mean |J - I| over the window (defined where found).  A frame index that
+ * is not held returns SB_ERR_INVALID.  One upload, one launch and one download.
+ * sb_flow_fetch_level: level `level` of frame t: img_out (H, W) uint8, deriv_out (H, W, 2) int16 (dx, dy); either
+ * may be NULL; *out_n_levels = levels built (maxLevel actually used + 1). */
+int sb_flow_create(sb_handle_t h, int window, int max_levels, float img_scale, int ring, int* out_flow_id);
+int sb_flow_add_frame(sb_handle_t h, int flow_id, int64_t t, const uint8_t* frame_host, int H, int W, int C,
+                      int replace);
+int sb_flow_shift(sb_handle_t h, int flow_id, int64_t t, int n, const int64_t* ref_t, const float* pts,
+                  float* out_pts, int32_t* out_status, float* out_err);
+int sb_flow_fetch_level(sb_handle_t h, int flow_id, int64_t t, int level, uint8_t* img_out, int16_t* deriv_out,
+                        int* out_H, int* out_W, int* out_n_levels);
+int sb_flow_destroy(sb_handle_t h, int flow_id);
+
 #ifdef __cplusplus
 }
 #endif

@@ -125,6 +125,12 @@ _SIGS = {
     "sb_centroid_configure": [c_void_p, c_int, POINTER(CentroidParams)],
     "sb_infer_centroids": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p],
+    "sb_flow_create": [c_void_p, c_int, c_int, c_float, c_int, POINTER(c_int)],
+    "sb_flow_add_frame": [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_int, c_int],
+    "sb_flow_shift": [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_flow_fetch_level": [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, POINTER(c_int), POINTER(c_int),
+                            POINTER(c_int)],
+    "sb_flow_destroy": [c_void_p, c_int],
 }
 
 EXPORTED_SYMBOLS = sorted(list(_SIGS.keys()) + ["sb_last_error"])

@@ -11,8 +11,9 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
-# per-file extra flags: post-processing must not contract multiply-adds (bit-exact parity)
-EXTRA = {"sb_post.cu": ["-fmad=false"]}
+# per-file extra flags: post-processing must not contract multiply-adds (bit-exact parity); the flow kernels neither,
+# so that their float steps round like OpenCV's (sb_flow.cu header)
+EXTRA = {"sb_post.cu": ["-fmad=false"], "sb_flow.cu": ["-fmad=false"]}
 
 
 def sources():

@@ -12,6 +12,7 @@
 #include "../../include/sleap_b200.h"
 
 struct SbModel;
+struct SbFlow;
 
 // Device workspace for the post-processing stages (capacity-bounded, per sample).
 struct SbPostWs {
@@ -94,6 +95,7 @@ struct sb_handle_s {
   std::string last_error;
   std::vector<void*> owned;                 // generic device allocations freed at destroy
   std::vector<SbModel*> models;
+  std::vector<SbFlow*> flows;               // sb_flow_create objects (sb_flow.cu); index = flow id
   int gpu_launches = 0;                     // kernels launched by this handle (bench: gpu_launches)
   int sm_count = 132;
 };
@@ -102,6 +104,7 @@ extern thread_local std::string g_sb_last_error;
 
 int sb_fail(sb_handle_s* h, int code, const char* fmt, ...);
 void sb_models_free(sb_handle_s* h);
+void sb_flows_free(sb_handle_s* h);
 
 #define SB_CUDA(h, expr)                                                              \
   do {                                                                                \

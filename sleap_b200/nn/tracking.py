@@ -3,7 +3,8 @@
 Restates the default tracker of the reference -- candidates from the last ``track_window`` frames, one similarity
 value per (instance, track), greedy or Hungarian assignment, new tracks for the unmatched, optional cap on the
 number of tracks -- and the optical-flow variant that first shifts the candidates of earlier frames into the current frame
-(Lucas-Kanade through OpenCV, exactly the library call the reference makes); the Kalman variant is not built:
+(Lucas-Kanade through OpenCV, exactly the library call the reference makes, or on a GPU named by ``of_device``:
+sleap_b200/nn/flow.py); the Kalman variant is not built:
   sleap/nn/tracker/components.py:33-196   similarity functions (instance, normalized, object keypoint, centroid, IoU)
   sleap/nn/tracker/components.py:198-226  hungarian_matching / greedy_matching, :637-647 first_choice_matching
   sleap/nn/tracker/components.py:229-313  nms_instances / nms_fast, :316-422 cull_instances / cull_frame_instances
@@ -341,34 +342,51 @@ def _ensure_u8(img: np.ndarray) -> np.ndarray:
     return np.clip(np.rint(img), 0, 255).astype(np.uint8)
 
 
+def shifted_instances_from_flow(ref_instances: list, shifted: np.ndarray, status: np.ndarray, errs: np.ndarray,
+                                min_shifted_points: int = 0) -> list:
+    """tracking.py:340-360: the flow result of the concatenated points of ``ref_instances`` -> one ShiftedInstance per
+    instance that kept more than ``min_shifted_points`` points (lost points NaN, ``shift_score`` = -mean err of the
+    found points)."""
+    sections = np.cumsum([len(_pts(x)) for x in ref_instances])[:-1]
+    out = []
+    for ref, pts, found, err in zip(ref_instances, np.split(shifted, sections, axis=0), np.split(status, sections, axis=0),
+                                    np.split(errs, sections, axis=0)):
+        if found.sum() > min_shifted_points:
+            found = found.reshape(-1).astype(bool)
+            pts = pts.astype(np.float64)
+            pts[~found] = np.nan
+            out.append(ShiftedInstance.from_instance(ref, new_points_array=pts, shift_score=-float(np.mean(err.reshape(-1)[found]))))
+    return out
+
+
 class FlowCandidateMaker:
     """Candidates = the instances of the last ``track_window`` frames, each flow-shifted into the current frame
     (tracking.py:108-360).  ``save_shifted_instances`` chains the shifts frame to frame instead of always starting from
-    the original frame (:139-160)."""
+    the original frame (:139-160).
+
+    ``of_device``: None shifts with ``cv2.calcOpticalFlowPyrLK``, one call per reference frame, as the reference does.
+    A GPU index (or "cuda:N") shifts every reference frame's points with one ``DeviceFlow.shift`` call on that GPU
+    (sleap_b200/nn/flow.py), building each frame's pyramid once."""
 
     uses_image = True
 
     def __init__(self, min_points: int = 0, img_scale: float = 1.0, of_window_size: int = 21, of_max_levels: int = 3,
-                 save_shifted_instances: bool = False, track_window: int = 5):
+                 save_shifted_instances: bool = False, track_window: int = 5, of_device=None):
         self.min_points, self.img_scale = min_points, img_scale
         self.of_window_size, self.of_max_levels = of_window_size, of_max_levels
         self.save_shifted_instances, self.track_window = save_shifted_instances, track_window
-        self.shifted_instances: Dict[Tuple[int, int], tuple] = {}        # (ref_t, t) -> (instances, img)
+        self.of_device = of_device
+        self._device_flow = None
+        self.shifted_instances: Dict[Tuple[int, int], tuple] = {}        # (ref_t, t) -> (instances, img, t)
 
     def get_shifted_instances_from_earlier_time(self, ref_t: int, ref_img, ref_instances: list, t: int):
+        """-> (frame index of the image, image, instances) to shift from."""
         for ti in reversed(range(ref_t, t)):
             if (ref_t, ti) in self.shifted_instances:
-                insts, img = self.shifted_instances[(ref_t, ti)]
+                insts, img, img_t = self.shifted_instances[(ref_t, ti)]
                 if len(insts) > 0:
-                    return img, insts
-        return ref_img, ref_instances
-
-    def get_shifted_instances(self, ref_instances: list, ref_img, ref_t: int, img, t: int) -> list:
-        shifted = self.flow_shift_instances(ref_instances, ref_img, img, min_shifted_points=self.min_points, scale=self.img_scale,
-                                            window_size=self.of_window_size, max_levels=self.of_max_levels)
-        if self.save_shifted_instances:
-            self.shifted_instances[(ref_t, t)] = (shifted, img)
-        return shifted
+                    return img_t, img, insts
+        return ref_t, ref_img, ref_instances
 
     def prune_shifted_instances(self, t: int):
         if not self.save_shifted_instances:
@@ -377,18 +395,68 @@ class FlowCandidateMaker:
             if t - k[0] > self.track_window:
                 del self.shifted_instances[k]
 
+    def add_request(self, requests: list, ref_t: int, ref_img, ref_instances: list, t: int):
+        """Queue the shift of ``ref_instances`` (frame ``ref_t``) into frame ``t``, from the latest saved shift when
+        ``save_shifted_instances`` is on.  Requests are (ref_t, frame index of the image, image, instances)."""
+        img_t = ref_t
+        if self.save_shifted_instances:
+            img_t, ref_img, ref_instances = self.get_shifted_instances_from_earlier_time(ref_t, ref_img, ref_instances, t)
+        if len(ref_instances) > 0:
+            requests.append((ref_t, img_t, ref_img, ref_instances))
+
     def get_candidates(self, track_matching_queue, t: int, img, **kw) -> list:
         if img is None:
             raise ValueError("the flow tracker needs the frame image: Tracker.track(instances, img=frame, ...)")
-        out = []
         self.prune_shifted_instances(t)
+        requests: list = []
         for item in track_matching_queue:
-            ref_t, ref_instances, ref_img = item[0], item[1], item[2]
+            self.add_request(requests, item[0], item[2], item[1], t)
+        return self.resolve_requests(requests, img, t)
+
+    def resolve_requests(self, requests: list, img, t: int) -> list:
+        """Shift every request into frame ``t`` and return the candidates in request order."""
+        if not requests:
+            return []
+        if self.of_device is None:
+            shifted = [self.flow_shift_instances(insts, ref_img, img, min_shifted_points=self.min_points, scale=self.img_scale,
+                                                 window_size=self.of_window_size, max_levels=self.of_max_levels)
+                       for _, _, ref_img, insts in requests]
+        else:
+            shifted = self.device_shift(requests, img, t)
+        out = []
+        for (ref_t, _, _, _), insts in zip(requests, shifted):
             if self.save_shifted_instances:
-                ref_img, ref_instances = self.get_shifted_instances_from_earlier_time(ref_t, ref_img, ref_instances, t)
-            if len(ref_instances) > 0:
-                out.extend(self.get_shifted_instances(ref_instances, ref_img, ref_t, img, t))
+                self.shifted_instances[(ref_t, t)] = (insts, img, t)
+            out.extend(insts)
         return out
+
+    def device_flow(self):
+        """The DeviceFlow of ``of_device``, made on first use (``make_tracker_by_name`` sets the flow options after
+        construction)."""
+        if self._device_flow is None:
+            from sleap_b200.nn.flow import DeviceFlow
+            dev = int(str(self.of_device).split(":")[-1])
+            self._device_flow = DeviceFlow(dev, self.of_window_size, self.of_max_levels, self.img_scale, self.track_window + 2)
+        return self._device_flow
+
+    def device_shift(self, requests: list, img, t: int) -> list:
+        """All requests in one ``DeviceFlow.shift`` call; the frames they read are uploaded unless already held."""
+        flow = self.device_flow()
+        frames: Dict[int, object] = {}
+        for _, img_t, ref_img, _ in requests:
+            frames.setdefault(img_t, ref_img)
+        flow.reserve(len(frames) + 1)
+        flow.add_frame(t, _ensure_u8(img))          # gray conversion and resize run on the device
+        for img_t, ref_img in frames.items():
+            flow.add_frame(img_t, _ensure_u8(ref_img), replace=False)
+        pts = [np.concatenate([_pts(x) for x in insts], axis=0).astype("float32") * self.img_scale for _, _, _, insts in requests]
+        ref_t = np.concatenate([np.full(len(p), img_t, np.int64) for p, (_, img_t, _, _) in zip(pts, requests)])
+        shifted, status, errs = flow.shift(t, ref_t, np.concatenate(pts, axis=0))
+        shifted = shifted / self.img_scale
+        sections = np.cumsum([len(p) for p in pts])[:-1]
+        return [shifted_instances_from_flow(insts, s, st, e, self.min_points)
+                for (_, _, _, insts), s, st, e in zip(requests, np.split(shifted, sections), np.split(status, sections),
+                                                      np.split(errs, sections))]
 
     @staticmethod
     def flow_shift_instances(ref_instances: list, ref_img, new_img, min_shifted_points: int = 0, scale: float = 1.0,
@@ -409,17 +477,7 @@ class FlowCandidateMaker:
             np.ascontiguousarray(ref_img), np.ascontiguousarray(new_img), (np.concatenate(ref_pts, axis=0)).astype("float32") * scale, None,
             winSize=(window_size, window_size), maxLevel=max_levels,
             criteria=(cv2.TERM_CRITERIA_EPS | cv2.TERM_CRITERIA_COUNT, 30, 0.01))
-        shifted = shifted / scale
-        sections = np.cumsum([len(x) for x in ref_pts])[:-1]
-        out = []
-        for ref, pts, found, err in zip(ref_instances, np.split(shifted, sections, axis=0), np.split(status, sections, axis=0),
-                                        np.split(errs, sections, axis=0)):
-            if found.sum() > min_shifted_points:
-                found = found.reshape(-1).astype(bool)
-                pts = pts.astype(np.float64)
-                pts[~found] = np.nan
-                out.append(ShiftedInstance.from_instance(ref, new_points_array=pts, shift_score=-float(np.mean(err.reshape(-1)[found]))))
-        return out
+        return shifted_instances_from_flow(ref_instances, shifted / scale, status, errs, min_shifted_points)
 
 
 class FlowMaxTracksCandidateMaker(FlowCandidateMaker):
@@ -439,19 +497,16 @@ class FlowMaxTracksCandidateMaker(FlowCandidateMaker):
     def get_candidates(self, track_matching_queue_dict, max_tracking: bool, t: int, img, **kw) -> list:
         if img is None:
             raise ValueError("the flow tracker needs the frame image: Tracker.track(instances, img=frame, ...)")
-        out, tracks = [], []
+        requests: list = []
+        tracks = []
         self.prune_shifted_instances(t)
         for track, hist in track_matching_queue_dict.items():
             if not max_tracking or len(tracks) < self.max_tracks:
                 tracks.append(track)
-                for item in hist:
+                for item in hist:                               # one request per track and frame, duplicates included
                     ref_t, ref_img = item[0], item[2]
-                    ref_instances = self.get_ref_instances(ref_t, ref_img, track_matching_queue_dict)
-                    if self.save_shifted_instances:
-                        ref_img, ref_instances = self.get_shifted_instances_from_earlier_time(ref_t, ref_img, ref_instances, t)
-                    if len(ref_instances) > 0:
-                        out.extend(self.get_shifted_instances(ref_instances, ref_img, ref_t, img, t))
-        return out
+                    self.add_request(requests, ref_t, ref_img, self.get_ref_instances(ref_t, ref_img, track_matching_queue_dict), t)
+        return self.resolve_requests(requests, img, t)
 
 
 SIMILARITIES = dict(instance=instance_similarity, centroid=centroid_distance, iou=instance_iou,
@@ -579,7 +634,10 @@ class Tracker:
                              oks_normalization: str = "all", img_scale: float = 1.0, of_window_size: int = 21,
                              of_max_levels: int = 3, save_shifted_instances: bool = False, kf_init_frame_count: int = 0,
                              kf_node_indices: Optional[list] = None, post_connect_single_breaks: bool = False,
-                             clean_instance_count: int = 0, clean_iou_threshold: Optional[float] = None, **kwargs) -> "Tracker":
+                             clean_instance_count: int = 0, clean_iou_threshold: Optional[float] = None, of_device=None,
+                             **kwargs) -> "Tracker":
+        """``of_device``: GPU (index or "cuda:N") that runs the flow shift of the flow trackers; None (default) runs
+        it with cv2 on the CPU, as the reference does."""
         max_tracking = max_tracking if max_tracks else False
         if max_tracking and tracker in ("simple", "flow"):          # :882-884
             tracker += "maxtracks"
@@ -595,6 +653,7 @@ class Tracker:
         if tracker in ("flow", "flowmaxtracks"):                   # :913-918
             maker.img_scale, maker.of_window_size, maker.of_max_levels = img_scale, of_window_size, of_max_levels
             maker.save_shifted_instances, maker.track_window = save_shifted_instances, track_window
+            maker.of_device = of_device
         if tracker in ("simplemaxtracks", "flowmaxtracks"):
             maker.max_tracks = max_tracks
         sim = SIMILARITIES[similarity]

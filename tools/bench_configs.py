@@ -2,11 +2,17 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
 
 r50: ResNet50 bottom-up (ImageNet-preprocessed "frozen" weights, upsampling stack to stride 4 with k4 transposed convs,
 BN, two refine convs, concat skips), 1024x1024x1, flies13, B=8 per GPU; it also reports the fp16 maps against the fp32
 path as a fraction of the map maximum.
+
+track: the flow trackers with the cv2 flow shift and with the device flow shift (one JSON line).  Tracker only: the
+first 500 frames of the tracking clip (tests/golden/tracks, 1024x1024, two flies x two nodes, window 5) for flow, flow
+with save_shifted_instances and flowmaxtracks (max_tracks 2).  End to end: BottomUpPredictor.predict (labels made) of
+the C4 network on 256 clip frames with no tracker, the cv2 flow tracker and the device flow tracker; the heads are
+calibrated as bench.py does (~5 detections per channel), so the tracker shifts ~65 points per reference frame.
 """
 import json
 import os
@@ -169,6 +175,61 @@ def resnet50(steps, B=8):
             "fp16_vs_fp32_maps_max_err_frac": err, "dtype": "f16", "clocks": LAST_CLOCKS}
 
 
+def track_bench():
+    import cv2
+    import torch
+    import bench
+    from sleap_b200.nn import tracking as T
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from flow_clip import clip_frames, clip_labeled_frames
+    n_track, n_e2e = 500, 256
+    clip = clip_frames(n_track)
+    out = {"config": "track: flow trackers, cv2 vs device flow shift, 1024x1024 clip", "gpu": gpu_identity(),
+           "cv2_threads": cv2.getNumThreads(), "cpu_count": os.cpu_count(), "tracker_only_frames_per_s": {}}
+
+    def make(tracker, save, of_device):
+        tr = T.Tracker.make_tracker_by_name(tracker=tracker, similarity="instance", match="greedy", track_window=5, max_tracks=2,
+                                            max_tracking=tracker == "flowmaxtracks", save_shifted_instances=save, of_device=of_device)
+        if of_device is not None:
+            tr.candidate_maker.device_flow()             # handle creation is set-up, not tracking
+        return tr
+
+    variants = [("flow", False), ("flow", True), ("flowmaxtracks", False)]
+    for tracker, save in variants:
+        for dev in (None, 0):
+            T.run_tracker(clip_labeled_frames(20), make(tracker, save, dev), images=lambda t: clip[t])    # warm-up
+            tr, frames = make(tracker, save, dev), clip_labeled_frames(n_track)
+            t0 = time.perf_counter()
+            T.run_tracker(frames, tr, images=lambda t: clip[t])
+            fps = n_track / (time.perf_counter() - t0)
+            out["tracker_only_frames_per_s"][f"{tracker}{'+save' if save else ''} {'device' if dev is not None else 'cv2'}"] = fps
+
+    # end to end: C4 network (bench.py) + post-processing + labels + tracker on the consumer thread
+    spec = bench.c4_spec()
+    cm = A.compile_model(spec, 1)
+    w = A.make_synthetic_weights(cm, bench.SEED)
+    gray = np.ascontiguousarray(clip[:n_e2e, :, :, :1])
+    m0 = DeviceModel(spec, w, input_channels=1, precision=0)
+    cms0, pafs0 = m0.forward(gray[:2])
+    w = bench.calibrate_heads(w, cms0, pafs0, 2)
+    del m0
+    model = DeviceModel(spec, w, input_channels=1, precision=0)
+    frames_e2e = torch.from_numpy(gray).pin_memory().numpy()
+    e2e = {}
+    for name, tracker, dev in (("no tracker", None, None), ("flow cv2", "flow", None), ("flow device", "flow", 0)):
+        pred = BottomUpPredictor(model, bench.NODES, bench.EDGES, peak_threshold=0.2, batch_size=8, integral_refinement=True,
+                                 max_peaks_per_sample=1024, max_node_peaks=32, max_instances_per_frame=32)
+        pred.tracker = make(tracker, False, dev) if tracker else None
+        pred.predict(frames_e2e[:32])                                    # warm-up
+        pred.tracker = make(tracker, False, dev) if tracker else None
+        t0 = time.perf_counter()
+        labeled = pred.predict(frames_e2e)
+        e2e[name] = n_e2e / (time.perf_counter() - t0)
+        e2e[f"{name} instances/frame"] = float(np.mean([len(lf.instances) for lf in labeled]))
+    out["predict_c4_frames_per_s"] = e2e
+    return out
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -181,6 +242,8 @@ if __name__ == "__main__":
             r = topdown(steps)
         elif c == "r50":
             r = resnet50(steps)
+        elif c == "track":
+            r = track_bench()
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
