@@ -74,6 +74,8 @@ struct TcParams {
   // programmatic dependent launch: 1 = call griddepcontrol.launch_dependents after the prologue (host: only for launches
   // that own their SMs, so that the successor's CTAs wait for free SMs instead of sharing them)
   int pdl_trigger;
+  // persistent form (k_conv_wg_p): output tiles of the launch, frames
+  int n_tiles, batch;
 };
 
 #include "sb_tc_prims.cuh"
@@ -337,6 +339,38 @@ __device__ __forceinline__ void tc_epilogue_chunk(const TcParams& P, const float
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
 
+// Epilogue of one 128-pixel tile of k_conv_wg_p (all 256 consumer threads; warp / lane of the calling thread); k_conv_wg
+// runs the same steps written out in its body.  Accumulators -> shared-memory
+// staging, CW columns at a time -> one pixel per thread, 16 columns per call (bias / ReLU / BN / residual / fused max-pool /
+// split planes).  Starts by writing the staging rows: a caller that ran an epilogue before must consumer_sync() first.
+template <int N>
+__device__ __forceinline__ void conv_epilogue(const TcParams& P, const float* __restrict__ s_par, float* s_stage, float (&acc)[N / 2],
+                                              int x0, int y0, int n0, int b, int warp, int lane) {
+  constexpr int CW = stage_cols(N), SP = CW + 4;   // staged columns per round, staging row pitch (floats)
+  const int wg = warp >> 2;
+  // fragment rows of this thread: 16 (warp % 4) + lane / 4 (+ 8) of its warpgroup's 64; columns 8 j + 2 (lane % 4) (+ 1)
+  const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+  // staging readers: pixel m = threadIdx.x % 128 (warp q = m / 32 as the fused pool expects), column half threadIdx.x / 128
+  const int m = threadIdx.x & 127, half = threadIdx.x >> 7;
+  const int iy = y0 + m / TW, ix = x0 + m % TW;
+  const bool valid = (iy < P.H) && (ix < P.W);
+  const size_t pix = ((size_t)b * P.out_H + (iy * P.oy_mul + P.oy_add)) * P.out_W + (ix * P.ox_mul + P.ox_add);
+#pragma unroll
+  for (int c0 = 0; c0 < N; c0 += CW) {
+    if (c0 > 0) consumer_sync();     // the previous round's readers are done with the staging rows
+#pragma unroll
+    for (int jj = 0; jj < CW / 8; ++jj) {
+      const int j = c0 / 8 + jj;
+      *reinterpret_cast<float2*>(s_stage + frow * SP + 8 * jj + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_stage + (frow + 8) * SP + 8 * jj + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    consumer_sync();
+    const int cc = c0 + 16 * half;
+    if (cc < c0 + CW && n0 + cc < P.Cout)     // warp-uniform
+      tc_epilogue_chunk(P, s_par, s_stage + m * SP + 16 * half, n0, cc, valid, pix, b, x0, y0, warp & 3, lane);
+  }
+}
+
 // Implicit-GEMM convolution on wgmma.  One CTA = one 16x8-pixel output tile x one N tile of output channels:
 //   warp 8, lane 0: TMA producer -- per (input-channel chunk, filter column) one activation box into the A ring, per filter
 //     tap one [N x KC] weight slice into the B ring (mbarrier full / empty pairs);
@@ -450,6 +484,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg(const __grid_consta
   wgmma_reg_fence(acc);
 
   // ------------------------------ epilogue (all 256 consumer threads) ----------
+  // (the same steps as conv_epilogue, written out: calling it, even force-inlined, changes this kernel's register allocation
+  // and grows the N = 256 spills from 54 to 90 bytes)
   // fragment rows of this thread: 16 (warp % 4) + lane / 4 (+ 8) of its warpgroup's 64; columns 8 j + 2 (lane % 4) (+ 1)
   const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
   // staging readers: pixel m = threadIdx.x % 128 (warp q = m / 32 as the fused pool expects), column half threadIdx.x / 128
@@ -470,6 +506,123 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg(const __grid_consta
     const int cc = c0 + 16 * half;
     if (cc < c0 + CW && n0 + cc < P.Cout)     // warp-uniform
       tc_epilogue_chunk(P, s_par, s_stage + m * SP + 16 * half, n0, cc, valid, pix, b, x0, y0, warp & 3, lane);
+  }
+}
+
+// Persistent form of k_conv_wg with resident weights (one N tile: C_out_pad <= 128).  The grid holds as many CTAs as fit on
+// the GPU at once; each walks a static list of work items (pixel tile, frame): CTA u takes items u, u + gridDim.x, ...
+// Barrier init, bias staging, descriptor prefetch and the weights happen once per CTA: the whole [chunk][step] bank of
+// weight slices is loaded with the mapB boxes before the grid dependency is waited on, and there is no weight ring.  The
+// activation ring runs on across items, so the producer stages the next tile's boxes while the consumers run the
+// epilogue.  Every item issues exactly the wgmma sequence of k_conv_wg -- same (chunk, filter column, tap, k-step) order on
+// the same operands -- so the outputs are bit-identical.
+template <int KSTEPS, int N>
+__global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(const __grid_constant__ CUtensorMap mapA,
+                                                                          const __grid_constant__ CUtensorMap mapB,
+                                                                          const __grid_constant__ TcParams P) {
+  constexpr int SP = stage_cols(N) + 4;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* a_ring = base;
+  uint8_t* bank = a_ring + (size_t)P.n_a_slots * P.a_slot_bytes;             // n_b_slots = n_chunks x steps weight slices
+  float* s_stage = reinterpret_cast<float*>(bank + (size_t)P.n_b_slots * P.b_slot_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + 128 * SP);
+  uint64_t* fullA = bars;
+  uint64_t* emptyA = fullA + P.n_a_slots;
+  uint64_t* fullB = emptyA + P.n_a_slots;                                    // the bank has landed
+  float* s_par = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(fullB + 1) + 15) & ~(uintptr_t)15);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_work = P.n_tiles * P.batch;
+  stage_params(P, s_par, 0);
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(fullA + i), 1); mbar_init(smem_u32(emptyA + i), kConsumerThreads / 32); }
+    mbar_init(smem_u32(fullB), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
+  }
+  __syncthreads();
+
+  if (warp == kConsumerThreads / 32) {
+    // ------------------------------ TMA producer ------------------------------
+    if (lane == 0) {
+      // weights are static: load the bank while the predecessor drains
+      mbar_expect_tx(smem_u32(fullB), (uint32_t)(P.n_b_slots * P.b_tx_bytes));
+      int s = 0;
+      for (int ch = 0; ch < P.n_chunks; ++ch)
+        for (int g = 0; g < P.n_groups; ++g)
+          for (int t = 0; t < P.groups[g].n_taps; ++t, ++s)
+            tma_load_3d(smem_u32(bank + (size_t)s * P.b_slot_bytes), &mapB, smem_u32(fullB), ch * P.KC, 0, P.groups[g].taps[t].w_tap);
+      griddep_wait();                                   // activations come from the previous kernel of the stream
+      int sa = 0;
+      uint32_t pha = 0;
+      for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+        if (w + (int)gridDim.x >= n_work) griddep_launch();   // last item of this CTA
+        const int tile = w % P.n_tiles, b = w / P.n_tiles;
+        const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+        for (int ch = 0; ch < P.n_chunks; ++ch) {
+          for (int g = 0; g < P.n_groups; ++g) {
+            mbar_wait(smem_u32(emptyA + sa), pha ^ 1);
+            mbar_expect_tx(smem_u32(fullA + sa), (uint32_t)P.a_tx_bytes);
+            tma_load_4d(smem_u32(a_ring + (size_t)sa * P.a_slot_bytes), &mapA, smem_u32(fullA + sa), ch * P.KC,
+                        x0 + P.groups[g].dx, y0 + P.dy0, b);
+            if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------ MMA (two warpgroups) + epilogue ------------------------
+  const int wg = warp >> 2;
+  float acc[N / 2];
+  const uint64_t desc_hi = make_desc(0, P.row_bytes, P.layout_type);
+  const uint32_t a_row0 = (uint32_t)(wg * 64 * P.row_bytes);
+  const uint32_t b_base = smem_u32(bank);
+  mbar_wait(smem_u32(fullB), 0);
+  int sa = 0;
+  uint32_t pha = 0;
+  for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+    const int tile = w % P.n_tiles, b = w / P.n_tiles;
+    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+    int rel_a = -1, s = 0;
+    uint32_t scale_d = 0;
+    for (int ch = 0; ch < P.n_chunks; ++ch) {
+      for (int g = 0; g < P.n_groups; ++g) {
+        mbar_wait(smem_u32(fullA + sa), pha);
+        const uint32_t a_base = smem_u32(a_ring + (size_t)sa * P.a_slot_bytes) + a_row0;
+        const int n_taps = P.groups[g].n_taps;
+        for (int t = 0; t < n_taps; ++t, ++s) {
+          const uint64_t da = desc_hi + (uint64_t)((a_base + (uint32_t)(P.groups[g].taps[t].row_off * TW * P.row_bytes)) >> 4);
+          const uint64_t db = desc_hi + (uint64_t)((b_base + (uint32_t)(s * P.b_slot_bytes)) >> 4);
+          wgmma_fence();
+          wgmma_reg_fence(acc);
+#pragma unroll
+          for (int k = 0; k < KSTEPS; ++k) {
+            wgmma_f16<N>(acc, da + 2 * k, db + 2 * k, scale_d);
+            scale_d = 1;
+          }
+          wgmma_commit();
+          wgmma_reg_fence(acc);
+          wgmma_wait<1>();               // the previous step's products are done: its activation slot may be refilled
+          __syncwarp();
+          if (lane == 0 && rel_a >= 0) mbar_arrive(smem_u32(emptyA + rel_a));
+          rel_a = t == n_taps - 1 ? sa : -1;
+        }
+        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(emptyA + rel_a));   // the item's last box: the producer is filling the next item's
+    if (w != (int)blockIdx.x) consumer_sync();              // the previous item's epilogue readers are done with the staging rows
+    conv_epilogue<N>(P, s_par, s_stage, acc, x0, y0, 0, b, warp, lane);
   }
 }
 
@@ -632,11 +785,24 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
   asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// Kernel forms of one launch: 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with
+// resident weights.  Both give bit-identical outputs; the autotuner keeps the faster eligible one per launch
+// (SB_FORCE_VARIANT=n forces form n where it is eligible).
+constexpr int kForms = 2;
+struct TcForm {
+  int ok;
+  int n_a_slots, n_b_slots;
+  size_t smem;
+  int max_ctas;                // persistent form: CTAs the GPU holds at once
+};
+
 struct TcLaunch {
   CUtensorMap mapA, mapB;
   TcParams P;
   dim3 grid;
   size_t smem;
+  TcForm forms[kForms];        // forms[0] (streaming) uses P's ring sizes and smem
+  int form;
 };
 
 }  // namespace
@@ -731,6 +897,85 @@ static int wg_n(int n) {
   return 256;
 }
 
+typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, TcParams);
+
+template <int KSTEPS>
+static ConvKernel conv_kernel_n(int N) {
+  switch (N) {
+    case 16: return k_conv_wg<KSTEPS, 16>;
+    case 32: return k_conv_wg<KSTEPS, 32>;
+    case 48: return k_conv_wg<KSTEPS, 48>;
+    case 64: return k_conv_wg<KSTEPS, 64>;
+    case 96: return k_conv_wg<KSTEPS, 96>;
+    case 128: return k_conv_wg<KSTEPS, 128>;
+    case 192: return k_conv_wg<KSTEPS, 192>;
+    default: return k_conv_wg<KSTEPS, 256>;
+  }
+}
+
+// the instantiation for an input-channel chunk of KC (K steps of 16 per staged slice) and a wg_n() tile width N
+static ConvKernel conv_kernel(int KC, int N) {
+  return KC == 16 ? conv_kernel_n<1>(N) : (KC == 32 ? conv_kernel_n<2>(N) : conv_kernel_n<4>(N));
+}
+
+// the resident-weight instantiations: N <= 128 (a 192 / 256-wide bank does not fit beside the activation ring at C_in >= 64,
+// and N = 256 leaves no registers for the persistent loop state); nullptr otherwise
+template <int KSTEPS>
+static ConvKernel conv_kernel_p_n(int N) {
+  switch (N) {
+    case 16: return k_conv_wg_p<KSTEPS, 16>;
+    case 32: return k_conv_wg_p<KSTEPS, 32>;
+    case 48: return k_conv_wg_p<KSTEPS, 48>;
+    case 64: return k_conv_wg_p<KSTEPS, 64>;
+    case 96: return k_conv_wg_p<KSTEPS, 96>;
+    case 128: return k_conv_wg_p<KSTEPS, 128>;
+    default: return nullptr;
+  }
+}
+
+static ConvKernel conv_kernel_form(int form, int KC, int N) {
+  if (form == 0) return conv_kernel(KC, N);
+  return KC == 16 ? conv_kernel_p_n<1>(N) : (KC == 32 ? conv_kernel_p_n<2>(N) : conv_kernel_p_n<4>(N));
+}
+
+// shared memory of a k_conv_wg launch: rings, accumulator staging rows, barriers, bias / BN vectors of 256 channels
+static size_t conv_smem(const TcParams& P, int n_a, int n_b) {
+  return (size_t)n_a * P.a_slot_bytes + (size_t)n_b * P.b_slot_bytes + (size_t)128 * (stage_cols(P.N) + 4) * sizeof(float) +
+         1024 /*align slack*/ + (size_t)(2 * n_a + 2 * n_b) * 8 + 16 + 3 * 256 * sizeof(float);
+}
+
+// shared memory of a k_conv_wg_p launch: activation ring, weight bank, staging rows, 2 n_a + 1 barriers, bias / BN vectors
+static size_t conv_smem_resident(const TcParams& P, int n_a, int bank) {
+  return (size_t)n_a * P.a_slot_bytes + (size_t)bank * P.b_slot_bytes + (size_t)128 * (stage_cols(P.N) + 4) * sizeof(float) +
+         1024 /*align slack*/ + (size_t)(2 * n_a + 1) * 8 + 16 + 3 * (size_t)P.N * sizeof(float);
+}
+
+// Eligibility, ring sizes, shared memory and co-resident grid size of the resident form of launch L (forms[0], the
+// streaming form, is always eligible): one N tile, and the whole bank of the launch's weight slices plus at least 2
+// activation slots fit in 225 KB; two CTAs per SM where they fit in 113 KB.
+static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
+  TcParams& P = L.P;
+  L.form = 0;
+  L.forms[0].ok = 1; L.forms[0].n_a_slots = P.n_a_slots; L.forms[0].n_b_slots = P.n_b_slots; L.forms[0].smem = L.smem;
+  TcForm& F = L.forms[1];
+  ConvKernel kern = conv_kernel_form(1, P.KC, P.N);
+  if (!kern || L.grid.y != 1) return;
+  const int bank = P.n_chunks * total_steps;
+  for (size_t budget : {(size_t)113 * 1024, kMaxDynSmem}) {
+    for (int na = 4; na >= 2 && !F.ok; --na)
+      if (conv_smem_resident(P, na, bank) <= budget) { F.ok = 1; F.n_a_slots = na; F.n_b_slots = bank; F.smem = conv_smem_resident(P, na, bank); }
+    if (F.ok) break;
+  }
+  if (!F.ok) return;
+  int nb = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kConvThreads, F.smem) != cudaSuccess || nb < 1) {
+    cudaGetLastError();
+    F.ok = 0;
+    return;
+  }
+  F.max_ctas = nb * h->sm_count;
+}
+
 // The residual ADD right after conv `oi` can run in its epilogue: the conv's output has no other reader (the compiler
 // only sets SB_OPF_RESIDUAL then), the ADD is flagged, and the shortcut / sum slices are 16-byte aligned fp16.
 static bool res_fusable(const SbModel* m, size_t oi) {
@@ -815,8 +1060,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   P.n_b_slots = std::min(4, P.n_chunks * total_steps);
   while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_b_slots > 2) P.n_b_slots--;
   while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_a_slots > 2) P.n_a_slots--;
-  L.smem = (size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes + stage_bytes + 1024 /*align slack*/ +
-           (size_t)(2 * P.n_a_slots + 2 * P.n_b_slots) * 8 + 16 + 3 * 256 * sizeof(float);
+  L.smem = conv_smem(P, P.n_a_slots, P.n_b_slots);
   if (L.smem > kMaxDynSmem) return sb_fail(h, SB_ERR_INVALID, "conv tile needs %zu bytes of shared memory", L.smem);
   L.grid = dim3(P.tiles_x * tiles_y, (plan->Cout_pad + N - 1) / N, 1 /* z = batch, set at launch */);
   // A: NHWC view (slice channels, W, H, batch); pixel and row pitches x sub
@@ -840,6 +1084,8 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
+  P.n_tiles = (int)L.grid.x;
+  setup_forms(h, L, total_steps);
   (dst ? *dst : plan->launches).push_back(L);
   return 0;
 }
@@ -1121,27 +1367,6 @@ int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* f
   return sb_conv_tc_launch(h, m, op_index, B);
 }
 
-typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, TcParams);
-
-template <int KSTEPS>
-static ConvKernel conv_kernel_n(int N) {
-  switch (N) {
-    case 16: return k_conv_wg<KSTEPS, 16>;
-    case 32: return k_conv_wg<KSTEPS, 32>;
-    case 48: return k_conv_wg<KSTEPS, 48>;
-    case 64: return k_conv_wg<KSTEPS, 64>;
-    case 96: return k_conv_wg<KSTEPS, 96>;
-    case 128: return k_conv_wg<KSTEPS, 128>;
-    case 192: return k_conv_wg<KSTEPS, 192>;
-    default: return k_conv_wg<KSTEPS, 256>;
-  }
-}
-
-// the instantiation for an input-channel chunk of KC (K steps of 16 per staged slice) and a wg_n() tile width N
-static ConvKernel conv_kernel(int KC, int N) {
-  return KC == 16 ? conv_kernel_n<1>(N) : (KC == 32 ? conv_kernel_n<2>(N) : conv_kernel_n<4>(N));
-}
-
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);
 
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
@@ -1151,9 +1376,11 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   const bool split = m->precision == 2;          // physical extent of a conv's output slice: 3 x C_out fp16 planes
   static bool attr_set = false;
   if (!attr_set) {
-    for (int kc : {16, 32, 64})
-      for (int n : {16, 32, 48, 64, 96, 128, 192, 256})
-        SB_CUDA(h, cudaFuncSetAttribute((const void*)conv_kernel(kc, n), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
+    for (int f = 0; f < kForms; ++f)
+      for (int kc : {16, 32, 64})
+        for (int n : {16, 32, 48, 64, 96, 128, 192, 256})
+          if (ConvKernel k = conv_kernel_form(f, kc, n))
+            SB_CUDA(h, cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
     attr_set = true;
   }
   for (size_t oi = 0; oi < m->ops.size(); ++oi) {
@@ -1304,6 +1531,21 @@ static bool pdl_on() {
 static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
   TcParams P = L.P;
   P.skip_out = skip_out;
+  if (L.form != 0) {
+    // persistent: as many CTAs as fit at once (capped at the work count), no shared-memory padding; each CTA triggers its
+    // dependents when it starts its last work item
+    const TcForm& F = L.forms[L.form];
+    P.n_a_slots = F.n_a_slots; P.n_b_slots = F.n_b_slots; P.batch = B; P.pdl_trigger = 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(std::min(P.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = F.smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
+    cudaLaunchKernelEx(&cfg, conv_kernel_form(L.form, P.KC, P.N), L.mapA, L.mapB, P);
+    return;
+  }
   size_t smem = L.smem;
   P.pdl_trigger = (pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
   if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing of the successor fits beside it
@@ -1316,14 +1558,54 @@ static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
   cudaLaunchKernelEx(&cfg, conv_kernel(P.KC, P.N), L.mapA, L.mapB, P);
 }
 
-// Picks, for a first layer with a Toeplitz view, the faster of the view + tensor-core conv and k_conv_first, and for the
-// first encoder block the fused k_conv01 or the separate launches, by timing both forms on the device (buffers are
-// already allocated; their contents do not matter for timing).
+static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan);
+
+// Picks, for every tensor-core conv launch (each transposed-conv phase included), the faster eligible kernel form
+// (streaming / resident weights), for a first layer with a Toeplitz view the faster of the view + tensor-core
+// conv and k_conv_first, and for the first encoder block the fused k_conv01 or the separate launches, by timing the
+// forms on the device at the configured batch (buffers are already allocated; their contents do not matter for timing).
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   cudaEvent_t e0, e1;
   SB_CUDA(h, cudaEventCreate(&e0));
   SB_CUDA(h, cudaEventCreate(&e1));
   const bool dbg = getenv("SB_DEBUG") != nullptr;
+  const char* fvar = getenv("SB_FORCE_VARIANT");
+  const int force = fvar ? atoi(fvar) : -1;
+  static const char* const form_name[kForms] = {"streaming", "resident"};
+  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
+    SbConvTcPlan* plan = m->tc_plans[oi];
+    if (!plan || head_kernel_ok(m, m->ops[oi], plan)) continue;
+    for (std::vector<TcLaunch>* list : {&plan->launches, &plan->plain_launches})
+      for (size_t li = 0; li < list->size(); ++li) {
+        TcLaunch& L = (*list)[li];
+        float best[kForms];
+        int pick = 0;
+        for (int f = 0; f < kForms; ++f) {
+          best[f] = 1e30f;
+          if (!L.forms[f].ok) continue;
+          L.form = f;
+          for (int rep = 0; rep < 4; ++rep) {
+            cudaEventRecord(e0, h->stream);
+            launch_conv(L, m->B, h->stream, plan->out_dead && list == &plan->launches);
+            cudaEventRecord(e1, h->stream);
+            cudaError_t e = cudaStreamSynchronize(h->stream);
+            if (e != cudaSuccess)
+              return sb_fail(h, SB_ERR_CUDA, "autotune launch (op %zu, %s form) failed: %s", oi, form_name[f], cudaGetErrorString(e));
+            float ms = 0.f;
+            cudaEventElapsedTime(&ms, e0, e1);
+            if (rep > 0) best[f] = std::min(best[f], ms);
+          }
+          if (best[f] < best[pick]) pick = f;
+        }
+        L.form = (force >= 0 && force < kForms && L.forms[force].ok) ? force : pick;
+        if (dbg) {
+          fprintf(stderr, "[sb_conv_tc] op %zu launch %zu%s:", oi, li, list == &plan->launches ? "" : " (own output)");
+          for (int f = 0; f < kForms; ++f)
+            if (L.forms[f].ok) fprintf(stderr, " %s %.1f us", form_name[f], best[f] * 1e3f);
+          fprintf(stderr, " -> %s\n", form_name[L.form]);
+        }
+      }
+  }
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
     if (!plan || !plan->view_in || plan->s2d || plan->from_buffer || !m->frames_dev) continue;

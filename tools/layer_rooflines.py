@@ -1,16 +1,32 @@
 """Per-layer floors of the C4 network (8 frames of 1024x1024) next to the measured per-op times.
 
-  BENCH_VERBOSE=1 python bench.py 2> per_op.txt; python tools/layer_rooflines.py per_op.txt floors.md
+  BENCH_VERBOSE=1 python bench.py 2> per_op.txt; python tools/layer_rooflines.py per_op.txt floors.md [L2_TBS]
 
 Floors: tensor = algorithmic FLOPs / 989 TFLOP/s (H100 SXM data sheet, dense fp16, 700 W);
 HBM = (activations in + out (+ fused pool output) at their storage width) / 3.35 TB/s (H100 SXM data sheet).
-The bound of a layer is the larger floor.
+`MEASURED_PEAKS.json` at the repository root (`bf16_tflops`, `hbm_gbs`), when present, replaces both figures, as in
+bench.py.  The bound of a layer is the larger floor.
+L2 column (3x3 convs and k3 transposed convs only): the bytes the streaming form of k_conv_wg pulls from L2 into the SMs
+(every 128-pixel CTA loads its activation boxes and its whole weight slice), and, given an L2 read rate in TB/s
+(`tools/bw_probe.py`, "L2-resident"), the time that traffic takes at that rate.
 """
+import json
+import os
 import re
 import sys
 
 B = 8
-PEAK_TF, PEAK_TBS = 1376.9, 6.0
+
+
+def _peaks():
+    p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
+    if os.path.exists(p):
+        d = json.load(open(p))
+        return float(d["bf16_tflops"]), float(d["hbm_gbs"]) / 1e3, "MEASURED_PEAKS.json"
+    return 989.0, 3.35, "H100 SXM data sheet (700 W)"
+
+
+PEAK_TF, PEAK_TBS, PEAK_SRC = _peaks()
 # (op index in the per-op table, name, Cin, Cout, input grid H(=W), output grid, taps, pooled copy, out bytes/elem)
 LAYERS = [
     (1, "conv 1->16 (Toeplitz view)", 1, 16, 1024, 1024, 9, False, 2),
@@ -39,15 +55,39 @@ LAYERS = [
 ]
 
 
-def main(src, out):
+def _wg_n(n):
+    for c in (16, 32, 48, 64, 96, 128, 192):
+        if n <= c:
+            return c
+    return 256
+
+
+def l2_bytes_streaming(cin, cout, hin, taps):
+    """Bytes the streaming k_conv_wg moves from L2 into shared memory for one layer of B frames (None: not modelled)."""
+    kc = 64 if cin > 32 else (32 if cin > 16 else 16)
+    chunks = -(-cin // kc)
+    cp = -(-cout // 16) * 16
+    n = _wg_n(min(cp, 256))
+    n_tiles = -(-cp // n)
+    tiles = -(-hin // 16) * -(-hin // 8)
+    if taps == 9:                # 3 filter columns: one 10-row box each, 9 weight slices
+        rows, slices = 3 * 10, 9
+    elif taps == 2.25:           # k3 transposed conv, 4 phases over the input grid: 3 + 3 boxes of 9 / 8 rows, 9 slices
+        rows, slices = 3 * 9 + 3 * 8, 9
+    else:
+        return None
+    return B * tiles * n_tiles * chunks * (rows * 16 * kc * 2 + slices * n * kc * 2)
+
+
+def main(src, out, l2_tbs=None):
     ms = {}
     for line in open(src):
         m = re.match(r"\[op\s*(\d+)\] kind=\d+\s+([\d.]+) us", line)
         if m:
             ms[int(m.group(1))] = float(m.group(2))
-    rows = ["| op | layer | measured us | GFLOP | tensor floor us | bytes MB | HBM floor us | bound | floor / measured |",
-            "|---|---|---|---|---|---|---|---|---|"]
-    tot_m = tot_f = 0.0
+    rows = ["| op | layer | measured us | GFLOP | tensor floor us | bytes MB | HBM floor us | bound | floor / measured | L2 GB (streaming) | L2 us |",
+            "|---|---|---|---|---|---|---|---|---|---|---|"]
+    tot_m = tot_f = tot_l2 = 0.0
     layers = list(LAYERS)
     if ms.get(2, 1e9) < 10.0:        # fused first block (k_conv01): op 1 holds both convs + the pool, op 2 is an empty slot
         flops = sum(2.0 * 9 * ci * co * 1024 * 1024 * B for ci, co in ((1, 16), (16, 16)))
@@ -59,7 +99,7 @@ def main(src, out):
         tot_m += meas
         tot_f += floor
         rows.append(f"| 1+2 | fused first block 1->16->16 + pool (k_conv01) @1024² | {meas:.1f} | {flops / 1e9:.2f} | {t_tensor:.1f} | {byts / 1e6:.1f} | "
-                    f"{t_hbm:.1f} | {'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} |")
+                    f"{t_hbm:.1f} | {'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} | | |")
         layers = [l for l in layers if l[0] not in (1, 2)]
     for op, name, cin, cout, hin, hout, taps, pool, ob in layers:
         flops = 2.0 * taps * cin * cout * hout * hout * B
@@ -71,14 +111,18 @@ def main(src, out):
         meas = ms.get(op, float("nan"))
         tot_m += meas
         tot_f += floor
+        l2b = None if op == 1 else l2_bytes_streaming(cin, cout, hin, taps)
+        tot_l2 += l2b or 0.0
+        l2_cols = "| |" if l2b is None else f"| {l2b / 1e9:.2f} | " + (f"{l2b / (l2_tbs * 1e12) * 1e6:.1f} |" if l2_tbs else "|")
         rows.append(f"| {op} | {name} @{hin}² | {meas:.1f} | {flops / 1e9:.2f} | {t_tensor:.1f} | {(in_b + out_b) / 1e6:.1f} | {t_hbm:.1f} | "
-                    f"{'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} |")
-    rows.append(f"| | **all conv layers** | **{tot_m:.1f}** | | | | | | **{tot_f / tot_m:.2f}** (sum of floors {tot_f:.1f} us) |")
+                    f"{'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} " + l2_cols)
+    rows.append(f"| | **all conv layers** | **{tot_m:.1f}** | | | | | | **{tot_f / tot_m:.2f}** (sum of floors {tot_f:.1f} us) | "
+                f"**{tot_l2 / 1e9:.2f}** | " + (f"**{tot_l2 / (l2_tbs * 1e12) * 1e6:.1f}** |" if l2_tbs else "|"))
     text = ("# C4 per-layer floors vs measured (8 frames, one H100)\n\nMeasured: CUDA-event per-op times of `bench.py` (`sb_model_profile_ops`), file `" + src +
-            "`.  Floors: see tools/layer_rooflines.py.\n\n" + "\n".join(rows) + "\n")
+            f"`.  Floors: {PEAK_TF:.0f} TFLOP/s and {PEAK_TBS:.2f} TB/s ({PEAK_SRC}); see tools/layer_rooflines.py.\n\n" + "\n".join(rows) + "\n")
     open(out, "w").write(text)
     print(text)
 
 
 if __name__ == "__main__":
-    main(sys.argv[1], sys.argv[2])
+    main(sys.argv[1], sys.argv[2], float(sys.argv[3]) if len(sys.argv) > 3 else None)
