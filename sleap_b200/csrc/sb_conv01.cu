@@ -7,15 +7,20 @@
 // pad to the stride) and the Keras layers stack0_enc0_conv0/act0, conv1/act1 and the pool of enc1
 // (sleap/nn/architectures/encoder_decoder.py:94-144, unet.py:140-205), as dispatched to cuDNN by TensorFlow.
 //
-// One CTA = one 16x8-pixel tile of conv1's output (M = 128), two warpgroups:
-//   1. the 20x12 frame patch around the tile -> shared memory (fp16-rounded pixels, zero outside the frame);
-//   2. conv0 on the CUDA cores for the 18x10 pixels conv1 reads, written as fp16 into three 32-byte-swizzled
-//      [160 rows x 16 ch] A tiles, one per filter column of conv1 (tile kx row 16 yy + xx = conv0 pixel
-//      (y0 - 1 + yy, x0 + kx - 1 + xx)), so that filter row ky of that column is the start offset 16 ky rows;
-//   3. conv1 as nine wgmma m64n16k16 per warpgroup (fp32 accumulators in registers), weights [tap][co][ci] in shared memory;
-//   4. accumulators -> shared-memory staging -> bias, ReLU, fp16 rounding, 2x2 max -> pooled NHWC output.
+// Persistent: one CTA per SM (as many as fit) walks a static list of (32x16-pixel tile of conv1's output, frame) items.
+// The conv1 bank, this thread's conv0 weights and both biases are loaded once, before the grid-dependency wait.  Per item:
+//   1. the 20x36 frame patch around the tile, fetched into registers one item ahead and stored to shared memory as
+//      fp16-rounded pixels (zero outside the frame), double-buffered;
+//   2. conv0 on the CUDA cores for the 18x34 pixels conv1 reads, each written once as fp16 into two non-swizzled 8-channel
+//      planes [18][34][8] (16 bytes per pixel), double-buffered;
+//   3. conv1 as 4 blocks of 8x8 pixels per warpgroup, each nine wgmma m64n16k16.  In the planes every filter tap of a block
+//      is the same operand at start offset (ky * 34 + kx) * 16 bytes (LBO = plane, SBO = one pixel row), so conv0's output
+//      needs no per-tap copies.  The wgmma run asynchronously while the same warps compute conv0 of the next item;
+//   4. bias, ReLU, fp16 rounding and the 2x2 max in registers: a thread's two accumulator rows are vertically adjacent
+//      pixels, the horizontal partner is lane ^ 4.  Each warp store writes four whole pooled pixels (128 bytes).
 // The same rounding points as the separate launches (fp16 frame pixels and weights, fp16 intermediate, fp16 conv1
-// output before the pool).
+// output before the pool), the same conv0 fma order and the same wgmma tap order and operands: results are bit-identical
+// to the one-tile-per-CTA form this replaces.
 #include <cuda.h>
 
 #include <algorithm>
@@ -26,24 +31,25 @@ namespace {
 
 #include "sb_tc_prims.cuh"
 
-constexpr int TW = 16, TH = 8;
-constexpr int PW = TW + 4, PH = TH + 4;     // frame patch
+constexpr int TW = 32, TH = 16;             // conv1 outputs per work item
+constexpr int NBX = TW / 8;                 // 8x8-pixel blocks per warpgroup and item
 constexpr int CW0 = TW + 2, CH0 = TH + 2;   // conv0 pixels conv1 reads
-constexpr int A_ROWS = CH0 * TW;            // 160 rows of 32 B per A tile
-constexpr int A_BYTES = A_ROWS * 32;        // 5120
-constexpr int SP = 20;                      // staging row pitch (floats)
+constexpr int PW = TW + 4, PH = TH + 4;     // frame patch
+constexpr int N_PATCH = PW * PH;
+constexpr int N_C0 = CW0 * CH0;
+constexpr int PATCH_PER_THREAD = (N_PATCH + 255) / 256;
+constexpr int C0_PER_THREAD = (N_C0 + 127) / 128;   // two threads per pixel, one per 8-channel half
+constexpr int PLANE = N_C0 * 16;            // one 8-channel plane [CH0][CW0][8] fp16
 
-constexpr int OFF_A = 0;                                // 3 A tiles
-constexpr int OFF_W1 = OFF_A + 3 * A_BYTES;             // 9 taps x [16 co][16 ci] fp16 = 9 x 512 B
-constexpr int OFF_STAGE = OFF_W1 + 9 * 512;             // [128][SP] fp32
-constexpr int OFF_PATCH = OFF_STAGE + 128 * SP * 4;     // [PH][PW] fp32
-constexpr int OFF_PAR = OFF_PATCH + PH * PW * 4;        // w0h[144] bias0[16] bias1[16]
-constexpr int SMEM_BYTES = OFF_PAR + (144 + 32) * 4 + 1024;
+constexpr int OFF_W1 = 0;                               // 9 taps x [16 co][16 ci] fp16, 32-byte swizzle
+constexpr int OFF_A = OFF_W1 + 9 * 512;                 // 2 buffers x 2 planes
+constexpr int OFF_PATCH = OFF_A + 4 * PLANE;            // 2 buffers x [PH][PW] fp32
+constexpr int SMEM_BYTES = OFF_PATCH + 2 * N_PATCH * 4 + 1024;
 
 struct C01Params {
   const void* frames;
   int frames_u8;
-  int Hin, Win, Hnet, Wnet, tiles_x;
+  int Hin, Win, Hnet, Wnet, tiles_x, n_tiles, batch;
   __half* pool_out;
   int pool_H, pool_W, pool_Ctot, pool_coff;
   const float* bias0;
@@ -57,116 +63,166 @@ struct C01Params {
 __device__ __forceinline__ int sw32(int r, int c) { return r * 32 + ((c ^ ((r >> 2) & 1)) << 4); }
 
 template <typename TI>
-__global__ void __launch_bounds__(256) k_conv01(const __grid_constant__ C01Params P) {
+__global__ void __launch_bounds__(256, 1) k_conv01(const __grid_constant__ C01Params P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* s_stage = reinterpret_cast<float*>(base + OFF_STAGE);
+  // 1024-byte aligned by offsetting the array itself, so that the compiler keeps every access in the shared window
+  uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   float* s_patch = reinterpret_cast<float*>(base + OFF_PATCH);
-  float* s_w0 = reinterpret_cast<float*>(base + OFF_PAR);
-  float* s_b0 = s_w0 + 144;
-  float* s_b1 = s_b0 + 16;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int x0 = (blockIdx.x % P.tiles_x) * TW, y0 = (blockIdx.x / P.tiles_x) * TH, b = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int n_items = P.n_tiles * P.batch, G = gridDim.x;
 
-  // weights / biases (static) and the frame patch
+  // static operands, loaded while the predecessor drains: the conv1 bank to shared memory; this thread's conv0 channel
+  // half (fixed: 256 threads, two per pixel) with its bias, and its conv1 output channels' biases to registers
   for (int i = tid; i < 9 * 16 * 2; i += 256) {        // 9 taps x 16 rows x 2 chunks
     const int t = i >> 5, r = (i >> 1) & 15, c = i & 1;
     *reinterpret_cast<uint4*>(base + OFF_W1 + t * 512 + sw32(r, c)) = reinterpret_cast<const uint4*>(P.w1t + (t * 16 + r) * 16)[c];
   }
-  if (tid < 144) s_w0[tid] = P.w0h[tid];
-  if (tid < 16) { s_b0[tid] = P.bias0 ? P.bias0[tid] : 0.f; s_b1[tid] = P.bias1 ? P.bias1[tid] : 0.f; }
-  const float sc = P.frames_u8 ? (1.0f / 255.0f) : 1.0f;     // ensure_float (normalization.py:34-49)
-  const TI* img = reinterpret_cast<const TI*>(P.frames) + (size_t)b * P.Hin * P.Win;
-  for (int i = tid; i < PH * PW; i += 256) {
-    const int y = y0 - 2 + i / PW, x = x0 - 2 + i % PW;
-    float v = 0.f;
-    if (y >= 0 && y < P.Hin && x >= 0 && x < P.Win) v = __half2float(__float2half_rn(__fmul_rn((float)img[(size_t)y * P.Win + x], sc)));
-    s_patch[i] = v;
-  }
-  __syncthreads();
-
-  // conv0 for the CH0 x CW0 pixels conv1 reads, 8 channels per item; zero outside the network image (conv1's SAME pad)
-  for (int it = tid; it < CH0 * CW0 * 2; it += 256) {
-    const int half = it & 1, p = it >> 1, yy = p / CW0, cx = p % CW0;
-    const int y = y0 - 1 + yy, x = x0 - 1 + cx;
-    __align__(16) __half h[8];
-    if (y >= 0 && y < P.Hnet && x >= 0 && x < P.Wnet) {
-      float acc[8];
+  const int hc = tid & 1;
+  float w0[9][8], b0[8], b1[2][2];
 #pragma unroll
-      for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+  for (int t = 0; t < 9; ++t)
+#pragma unroll
+    for (int c = 0; c < 8; ++c) w0[t][c] = P.w0h[t * 16 + 8 * hc + c];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) b0[c] = P.bias0 ? P.bias0[8 * hc + c] : 0.f;
+  const int fc = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) b1[j][e] = P.bias1 ? P.bias1[8 * j + fc + e] : 0.f;
+  griddep_wait();                                       // frames and the pooled buffer belong to the stream's order
+
+  const float sc = P.frames_u8 ? (1.0f / 255.0f) : 1.0f;     // ensure_float (normalization.py:34-49)
+  TI pf[PATCH_PER_THREAD];
+  auto fetch = [&](int w) {                             // frame patch of item w -> registers (zero outside the frame)
+    const int tile = w % P.n_tiles, b = w / P.n_tiles;
+    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+    const TI* img = reinterpret_cast<const TI*>(P.frames) + (size_t)b * P.Hin * P.Win;
+#pragma unroll
+    for (int k = 0; k < PATCH_PER_THREAD; ++k) {
+      const int e = tid + 256 * k;
+      const int y = y0 - 2 + e / PW, x = x0 - 2 + e % PW;
+      pf[k] = (w < n_items && e < N_PATCH && y >= 0 && y < P.Hin && x >= 0 && x < P.Win) ? img[(size_t)y * P.Win + x] : TI(0);
+    }
+  };
+  auto stash = [&](float* dst) {
+#pragma unroll
+    for (int k = 0; k < PATCH_PER_THREAD; ++k)
+      if (tid + 256 * k < N_PATCH) dst[tid + 256 * k] = __half2float(__float2half_rn(__fmul_rn((float)pf[k], sc)));
+  };
+
+  // conv0 for the CH0 x CW0 pixels conv1 reads, 8 channels per thread; zero outside the network image (conv1's SAME pad)
+  auto conv0 = [&](const float* patch, uint8_t* A, int x0, int y0) {
+#pragma unroll 1
+    for (int k = 0; k < C0_PER_THREAD; ++k) {
+      const int p = (tid >> 1) + 128 * k;
+      if (p >= N_C0) break;
+      const int yy = p / CW0, cx = p % CW0;
+      const int y = y0 - 1 + yy, x = x0 - 1 + cx;
+      uint32_t q[4] = {0u, 0u, 0u, 0u};                 // fp16 +0 outside
+      if (y >= 0 && y < P.Hnet && x >= 0 && x < P.Wnet) {
+        float acc[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+#pragma unroll
+        for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+          for (int kx = 0; kx < 3; ++kx) {
+            const float v = patch[(yy + ky) * PW + cx + kx];
+#pragma unroll
+            for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, w0[ky * 3 + kx][c], acc[c]);
+          }
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          acc[c] += b0[c];
+          if (P.relu0) acc[c] = fmaxf(acc[c], 0.f);
+        }
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const __half2 t = __floats2half2_rn(acc[2 * c], acc[2 * c + 1]);
+          q[c] = *reinterpret_cast<const uint32_t*>(&t);
+        }
+      }
+      *reinterpret_cast<uint4*>(A + hc * PLANE + p * 16) = make_uint4(q[0], q[1], q[2], q[3]);
+    }
+  };
+
+  // conv1: warpgroup wg takes tile rows [8 wg, 8 wg + 8), block bx columns [8 bx, 8 bx + 8); wgmma row m = pixel (m / 8, m % 8)
+  float acc[NBX][8];
+  const uint64_t desc_a = make_desc_interleave(0, PLANE, CW0 * 16);
+  const uint64_t desc_b = make_desc(0, 32, 3);
+  const uint32_t w1_addr = smem_u32(base + OFF_W1);
+  auto mma = [&](const uint8_t* A) {
+    const uint32_t a0 = smem_u32(A) + (uint32_t)(8 * wg * CW0 * 16);
+    wgmma_fence();
+#pragma unroll
+    for (int bx = 0; bx < NBX; ++bx) wgmma_reg_fence(acc[bx]);
+#pragma unroll
+    for (int bx = 0; bx < NBX; ++bx)
 #pragma unroll
       for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
         for (int kx = 0; kx < 3; ++kx) {
-          const float v = s_patch[(yy + ky) * PW + cx + kx];
-#pragma unroll
-          for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, s_w0[(ky * 3 + kx) * 16 + 8 * half + c], acc[c]);
+          const uint32_t a = a0 + (uint32_t)(((ky * CW0) + 8 * bx + kx) * 16);
+          const uint32_t w = w1_addr + (ky * 3 + kx) * 512;
+          wgmma_f16<16>(acc[bx], desc_a + (a >> 4), desc_b + (w >> 4), (ky | kx) ? 1u : 0u);
         }
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        float v = acc[c] + s_b0[8 * half + c];
-        if (P.relu0) v = fmaxf(v, 0.f);
-        h[c] = __float2half_rn(v);
-      }
-    } else {
-#pragma unroll
-      for (int c = 0; c < 8; ++c) h[c] = __float2half_rn(0.f);
-    }
-#pragma unroll
-    for (int kx = 0; kx < 3; ++kx) {                    // tile kx holds this pixel at column cx - kx
-      const int xx = cx - kx;
-      if (xx >= 0 && xx < TW) *reinterpret_cast<uint4*>(base + OFF_A + kx * A_BYTES + sw32(yy * TW + xx, half)) = *reinterpret_cast<uint4*>(h);
-    }
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
-  __syncthreads();
+    wgmma_commit();
+  };
 
-  // conv1: warpgroup wg multiplies tile rows [64 wg, 64 wg + 64)
-  const int wg = warp >> 2;
-  float acc[8];
+  // bias, ReLU, fp16 rounding (conv1's stored value), 2x2 max.  Thread rows: pixels (2 (warp % 4) + a, g) of each block,
+  // a = 0, 1; the even column of a pair pools channels 0-7, the odd one 8-15, after trading the other half with lane ^ 4.
+  auto pool_store = [&](int w) {
+    wgmma_wait<0>();
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-  const uint64_t desc_hi = make_desc(0, 32, 3);
-  wgmma_fence();
-  wgmma_reg_fence(acc);
+    for (int bx = 0; bx < NBX; ++bx) wgmma_reg_fence(acc[bx]);
+    const int tile = w % P.n_tiles, b = w / P.n_tiles;
+    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+    const int g = lane >> 2, odd = g & 1;
+    const int gy = (y0 >> 1) + 4 * wg + (warp & 3);
+    __half* row = P.pool_out + ((size_t)b * P.pool_H + gy) * P.pool_W * P.pool_Ctot + P.pool_coff + 8 * odd + fc;
 #pragma unroll
-  for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-    for (int kx = 0; kx < 3; ++kx) {
-      const uint32_t a = smem_u32(base + OFF_A + kx * A_BYTES + (ky * TW + 64 * wg) * 32);
-      const uint32_t w = smem_u32(base + OFF_W1 + (ky * 3 + kx) * 512);
-      wgmma_f16<16>(acc, desc_hi + (a >> 4), desc_hi + (w >> 4), (ky | kx) ? 1u : 0u);
-    }
-  wgmma_commit();
-  wgmma_wait<0>();
-  wgmma_reg_fence(acc);
-
-  // accumulators -> staging (fragment rows 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1))
-  const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    *reinterpret_cast<float2*>(s_stage + frow * SP + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-    *reinterpret_cast<float2*>(s_stage + (frow + 8) * SP + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-  }
-  __syncthreads();
-
-  // bias, ReLU, fp16 rounding (conv1's stored value), 2x2 max: thread = (pooled pixel, channel pair)
-  const int pp = tid >> 3, cp = 2 * (tid & 7);
-  const int py = pp / (TW / 2), px = pp % (TW / 2);
-  const int gy = (y0 >> 1) + py, gx = (x0 >> 1) + px;
-  if (gy < P.pool_H && gx < P.pool_W) {
-    __half2 m = __float2half2_rn(-INFINITY);
-#pragma unroll
-    for (int a = 0; a < 2; ++a)
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const float* s = s_stage + ((2 * py + a) * TW + 2 * px + c) * SP + cp;
-        float v0 = s[0] + s_b1[cp], v1 = s[1] + s_b1[cp + 1];
+    for (int bx = 0; bx < NBX; ++bx) {
+      auto val = [&](int j, int a) {                    // conv1 output of channel pair (8 j + fc, + 1), row a
+        float v0 = acc[bx][4 * j + 2 * a] + b1[j][0], v1 = acc[bx][4 * j + 2 * a + 1] + b1[j][1];
         if (P.relu1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        m = __hmax2(m, __floats2half2_rn(v0, v1));
-      }
-    *reinterpret_cast<__half2*>(P.pool_out + (((size_t)b * P.pool_H + gy) * P.pool_W + gx) * P.pool_Ctot + P.pool_coff + cp) = m;
+        return __floats2half2_rn(v0, v1);
+      };
+      const __half2 v00 = val(0, 0), v01 = val(0, 1), v10 = val(1, 0), v11 = val(1, 1);
+      const __half2 mine0 = odd ? v10 : v00, mine1 = odd ? v11 : v01;
+      const __half2 theirs0 = __shfl_xor_sync(0xffffffffu, odd ? v00 : v10, 4);
+      const __half2 theirs1 = __shfl_xor_sync(0xffffffffu, odd ? v01 : v11, 4);
+      __half2 m = __float2half2_rn(-INFINITY);          // order (row, column) = (0, 0), (0, 1), (1, 0), (1, 1)
+      m = __hmax2(m, odd ? theirs0 : mine0);
+      m = __hmax2(m, odd ? mine0 : theirs0);
+      m = __hmax2(m, odd ? theirs1 : mine1);
+      m = __hmax2(m, odd ? mine1 : theirs1);
+      const int gx = (x0 >> 1) + 4 * bx + (g >> 1);
+      if (gy < P.pool_H && gx < P.pool_W) *reinterpret_cast<__half2*>(row + (size_t)gx * P.pool_Ctot) = m;
+    }
+  };
+
+  int w = blockIdx.x;
+  fetch(w);
+  stash(s_patch);
+  fetch(w + G);
+  __syncthreads();
+  for (int k = 0; w < n_items; ++k, w += G) {
+    if (w + G >= n_items) griddep_launch();             // last item of this CTA
+    const int buf = k & 1;
+    const int tile = w % P.n_tiles;
+    uint8_t* A = base + OFF_A + buf * 2 * PLANE;
+    // A[buf] was last read by the wgmma of item k - 2, waited for before the previous barrier; so was patch[buf ^ 1]'s
+    // last reader, conv0 of item k - 1
+    conv0(s_patch + buf * N_PATCH, A, (tile % P.tiles_x) * TW, (tile / P.tiles_x) * TH);
+    stash(s_patch + (buf ^ 1) * N_PATCH);
+    fetch(w + 2 * G);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
+    if (k > 0) pool_store(w - G);
+    __syncthreads();
+    mma(A);
   }
+  pool_store(w - G);                                    // every CTA has at least one item (grid <= item count)
 }
 
 }  // namespace
@@ -176,6 +232,7 @@ struct SbConv01Plan {
   __half* w1t = nullptr;     // [9][16][16]
   float* w0h = nullptr;      // [9][16]
   int conv0_op = -1, conv1_op = -1;
+  int max_ctas = 0;          // co-resident CTAs of k_conv01 on this GPU
 };
 
 void sb_conv01_release(SbModel* m) {
@@ -205,6 +262,15 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
       return 0;
   SbConv01Plan* pl = new SbConv01Plan();
   pl->conv0_op = conv0_op; pl->conv1_op = conv1_op;
+  for (auto kern : {k_conv01<unsigned char>, k_conv01<float>}) {
+    int nb = 0;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, 256, SMEM_BYTES) != cudaSuccess || nb < 1) {
+      delete pl;
+      return sb_fail(h, SB_ERR_CUDA, "conv01: kernel attributes / occupancy: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    pl->max_ctas = pl->max_ctas ? std::min(pl->max_ctas, nb * h->sm_count) : nb * h->sm_count;
+  }
   const float* w0 = m->weights_host.data() + c0.w_off();     // [9][1][16]
   const float* w1 = m->weights_host.data() + c1.w_off();     // [9][16][16]
   std::vector<__half> w1t((size_t)9 * 16 * 16);
@@ -227,6 +293,7 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
   memset(&P, 0, sizeof(P));
   P.Hin = m->Hin; P.Win = m->Win; P.Hnet = ob0.H; P.Wnet = ob0.W;
   P.tiles_x = (ob0.W + TW - 1) / TW;
+  P.n_tiles = P.tiles_x * ((ob0.H + TH - 1) / TH);
   P.pool_out = (__half*)pb.dev; P.pool_H = pb.H; P.pool_W = pb.W; P.pool_Ctot = pb.C; P.pool_coff = c1.pool_coff();
   P.bias0 = c0.b_off() >= 0 ? m->weights_dev + c0.b_off() : nullptr;
   P.bias1 = c1.b_off() >= 0 ? m->weights_dev + c1.b_off() : nullptr;
@@ -239,13 +306,21 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
 bool sb_conv01_can(const SbModel* m, int conv0_op) { return m->conv01 && m->conv01->conv0_op == conv0_op && m->conv01_enabled; }
 int sb_conv01_conv1_op(const SbModel* m) { return m->conv01 ? m->conv01->conv1_op : -1; }
 
+// Persistent launch: as many CTAs as are co-resident (capped at the item count), with programmatic stream serialization
+// so that the weight loads overlap the predecessor's tail; each CTA triggers its dependents when it starts its last item.
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
   SbConv01Plan* pl = m->conv01;
   C01Params P = pl->P;
-  P.frames = frames_dev; P.frames_u8 = frames_are_u8;
-  const dim3 grid(P.tiles_x * ((P.Hnet + TH - 1) / TH), B);
-  if (frames_are_u8) k_conv01<unsigned char><<<grid, 256, SMEM_BYTES, h->stream>>>(P);
-  else k_conv01<float><<<grid, 256, SMEM_BYTES, h->stream>>>(P);
+  P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.batch = B;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(P.n_tiles * B, pl->max_ctas)); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.stream = h->stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
+  if (frames_are_u8) cudaLaunchKernelEx(&cfg, k_conv01<unsigned char>, P);
+  else cudaLaunchKernelEx(&cfg, k_conv01<float>, P);
   SB_CHECK_LAUNCH(h);
   return 0;
 }

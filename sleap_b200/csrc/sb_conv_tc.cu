@@ -1522,7 +1522,7 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
 // the grid dependency before the first activation load); a launch that owns its SMs (one CTA per SM) is padded to the
 // SM's whole shared memory and triggers its dependents right after its prologue, so that the next layer's CTAs set up
 // (barriers, bias staging, descriptor prefetch) while this layer's last tiles drain.  SB_DISABLE_PDL=1 switches it off.
-static bool pdl_on() {
+bool sb_pdl_on() {
   static int v = -1;
   if (v < 0) v = getenv("SB_DISABLE_PDL") ? 0 : 1;
   return v != 0;
@@ -1542,19 +1542,19 @@ static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
+    cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
     cudaLaunchKernelEx(&cfg, conv_kernel_form(L.form, P.KC, P.N), L.mapA, L.mapB, P);
     return;
   }
   size_t smem = L.smem;
-  P.pdl_trigger = (pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
+  P.pdl_trigger = (sb_pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
   if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing of the successor fits beside it
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(L.grid.x, L.grid.y, B); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
   cudaLaunchKernelEx(&cfg, conv_kernel(P.KC, P.N), L.mapA, L.mapB, P);
 }
 
@@ -1651,8 +1651,8 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
       }
     m->conv01_enabled = best[1] < best[0];
     if (const char* fv = getenv("SB_FORCE_CONV01")) m->conv01_enabled = atoi(fv) != 0;
-    if (dbg) fprintf(stderr, "[sb_conv_tc] first block: conv0 + conv1 launches %.1f us, fused k_conv01 %.1f us -> %s\n", best[0] * 1e3f,
-                     best[1] * 1e3f, m->conv01_enabled ? "fused" : "separate");
+    if (dbg) fprintf(stderr, "[sb_conv_tc] first block (B = %d): conv0 + conv1 launches %.1f us, fused k_conv01 %.1f us -> %s\n", m->B,
+                     best[0] * 1e3f, best[1] * 1e3f, m->conv01_enabled ? "fused" : "separate");
   }
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
@@ -1694,7 +1694,7 @@ static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = smem; cfg.stream = h->stream;                    \
     cudaLaunchAttribute at[1];                                                                                                  \
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;        \
-    cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;                                                                            \
+    cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;                                                                            \
     cudaLaunchKernelEx(&cfg, k_head_1x1<NT, KC>, (const __half*)ib.dev, ib.C, op.in_coff(), op.in_C(), (const __half*)plan->w16, bias,        \
                        (float*)ob.dev, ob.C, op.out_coff(), op.out_C(), relu, npix, n_ring);                                    \
   }

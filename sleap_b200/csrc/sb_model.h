@@ -156,3 +156,6 @@ void sb_conv01_release(SbModel* m);
 bool sb_conv01_can(const SbModel* m, int conv0_op);
 int sb_conv01_conv1_op(const SbModel* m);
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);
+
+// programmatic dependent launch for the conv kernels (sb_conv_tc.cu); SB_DISABLE_PDL=1 switches it off
+bool sb_pdl_on();

@@ -52,6 +52,16 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, int row_bytes, int
   d |= (uint64_t)layout_type << 62;
   return d;
 }
+// Non-swizzled K-major descriptor (layout type 0) with explicit offsets.  The operand is built from 8-row x 16-byte core
+// matrices whose rows are 16 bytes apart; lbo = distance between the two core matrices of one K = 16 step, sbo = distance
+// between successive 8-row groups along M / N.  The start address only needs 16-byte alignment.
+__device__ __forceinline__ uint64_t make_desc_interleave(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
+  return d;
+}
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
