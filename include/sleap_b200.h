@@ -35,7 +35,10 @@ extern "C" {
 #define SB_REFINE_INTEGRAL 1
 #define SB_REFINE_LOCAL 2
 
-/* overflow flags reported per sample (capacity-bounded device buffers; the reference is unbounded) */
+/* overflow flags reported per sample (capacity-bounded device buffers; the reference is unbounded).  What is kept:
+   PEAKS_TRUNCATED: the first max_peaks_per_sample peaks in tf.where (row-major NHWC) order;
+   NODE_PEAKS_TRUNCATED: grouping sees the first max_node_peaks peaks of each node, in the same order;
+   INSTANCES_TRUNCATED: the first max_instances instances of the reference's output order. */
 #define SB_FLAG_PEAKS_TRUNCATED 1
 #define SB_FLAG_NODE_PEAKS_TRUNCATED 2
 #define SB_FLAG_INSTANCES_TRUNCATED 4

@@ -825,6 +825,7 @@ struct SbConvTcPlan {
   // instead, for a forward pass that asks for that tensor (the ADD op then runs)
   bool res_fused = false;
   std::vector<TcLaunch> plain_launches;
+  bool head_logged = false;         // SB_DEBUG: the k_head_1x1 launch shape of this op was printed
 };
 
 static CUtensorMapSwizzle swz_for(int KC) {
@@ -1659,6 +1660,29 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
+// Shared memory of one k_head_1x1 launch: the weight bank, the output staging and the bias, plus a per-warp ring of n_ring
+// staged items (16 pixels x kch channels each), as deep as fits with two blocks per SM, else with one block per SM
+// (kHeadSmem).  n_ring = 0: not even a ring of 2 fits beside the bank (wide inputs with 17-32 outputs), so the op stays
+// on the implicit-GEMM conv kernel.
+constexpr long long kHeadSmem = 200 * 1024;
+struct HeadShape {
+  int nt, kch, n_ring;
+  size_t smem;
+};
+static HeadShape head_shape(const SbOp& op) {
+  HeadShape s;
+  s.nt = (op.out_C() + 7) / 8;
+  s.kch = std::min(op.in_C(), 128);
+  // signed: the bank alone can exceed the two-blocks-per-SM budget
+  const long long fixed = 8LL * s.nt * (op.in_C() + 8) * 2 + 8LL * 16 * (8 * s.nt + 1) * 4 + 8LL * s.nt * 4;
+  const long long stage = 8LL * 16 * (s.kch + 8) * 2;
+  long long n_ring = std::min<long long>(8, (110 * 1024 - fixed) / stage);
+  if (n_ring < 4) n_ring = std::min<long long>(8, (kHeadSmem - fixed) / stage);
+  s.n_ring = n_ring >= 2 ? (int)n_ring : 0;
+  s.smem = (size_t)(fixed + s.n_ring * stage);
+  return s;
+}
+
 // 1x1 fp32 heads on k_head_1x1 (HBM-bound; see the kernel) instead of the implicit-GEMM conv kernel.  SB_DISABLE_HEAD_KERNEL=1 reverts.
 static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan) {
   if (getenv("SB_DISABLE_HEAD_KERNEL")) return false;
@@ -1666,30 +1690,28 @@ static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan*
   const SbBuffer& ob = m->buffers[op.out_buf()];
   return op.kind() == SB_OPK_CONV && op.k() == 1 && op.stride() == 1 && ob.f32 && !ib.f32 && !(op.flags() & SB_OPF_BN) && op.in_C() % 16 == 0 &&
          (op.in_C() == 16 || op.in_C() == 32 || op.in_C() == 64 || op.in_C() % 128 == 0) && op.out_C() <= 32 && ib.C % 8 == 0 && op.in_coff() % 8 == 0 && plan->w16 != nullptr && plan->Cout_pad >= (op.out_C() + 7) / 8 * 8 &&
-         (size_t)plan->Cout_pad * (op.in_C() + 8) * 2 <= 160 * 1024;
+         (size_t)plan->Cout_pad * (op.in_C() + 8) * 2 <= 160 * 1024 && head_shape(op).n_ring >= 2;
 }
 
 static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int B) {
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
-  const int nt = (op.out_C() + 7) / 8;
+  const HeadShape hs = head_shape(op);
+  const int nt = hs.nt, kch = hs.kch, n_ring = hs.n_ring;
+  const size_t smem = hs.smem;
   const size_t npix = (size_t)B * ob.H * ob.W;
-  const int kch = std::min(op.in_C(), 128);
-  // per-warp ring of n_ring staged items (16 pixels x kch channels each): as deep as shared memory allows with two blocks per SM,
-  // else one block per SM (128-channel passes)
-  const size_t fixed = (size_t)8 * nt * (op.in_C() + 8) * 2 + (size_t)8 * 16 * (8 * nt + 1) * 4 + (size_t)8 * nt * 4;
-  const size_t stage = (size_t)8 * 16 * (kch + 8) * 2;
-  int n_ring = (int)std::min<size_t>(8, (110 * 1024 - fixed) / stage);
-  if (n_ring < 4) n_ring = (int)std::min<size_t>(8, (200 * 1024 - fixed) / stage);
-  n_ring = std::max(2, n_ring);
-  const size_t smem = fixed + (size_t)n_ring * stage;
+  if (!plan->head_logged && getenv("SB_DEBUG")) {
+    fprintf(stderr, "[sb_conv_tc] head k_head_1x1: Cin %d Cout %d NT %d KCH %d n_ring %d smem %zu\n", op.in_C(), op.out_C(), nt, kch,
+            n_ring, smem);
+    plan->head_logged = true;
+  }
   const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
   const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
   const int grid = (int)std::min<size_t>((npix + 127) / 128, (size_t)h->sm_count * 2);
 #define SB_HEAD_LAUNCH(NT, KC)                                                                                                  \
   {                                                                                                                             \
     static bool attr = false;                                                                                                   \
-    if (!attr) { SB_CUDA(h, cudaFuncSetAttribute((k_head_1x1<NT, KC>), cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; } \
+    if (!attr) { SB_CUDA(h, cudaFuncSetAttribute((k_head_1x1<NT, KC>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHeadSmem)); attr = true; } \
     cudaLaunchConfig_t cfg = {};                                                                                                \
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = smem; cfg.stream = h->stream;                    \
     cudaLaunchAttribute at[1];                                                                                                  \
