@@ -76,6 +76,9 @@ struct TcParams {
   int pdl_trigger;
   // persistent form (k_conv_wg_p): output tiles of the launch, frames
   int n_tiles, batch;
+  // halo form (k_conv_wg_h): the input slice (fp16 NHWC, H x W of the iteration grid), its pixel pitch and channel count
+  const void* in;
+  int in_Ctot, in_C;
 };
 
 #include "sb_tc_prims.cuh"
@@ -626,6 +629,196 @@ __global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(con
   }
 }
 
+// Halo form (form 2): persistent, weights resident, for 3x3 stride-1 convs with C_in <= 64 (one K chunk) and one N tile of
+// <= 64 channels in the epi_mode == 1 shape (fp16 out, no BN, no residual).  A work item is a 16 x 8 BY-pixel tile of one
+// frame, cut into 2 x BY blocks of 8x8 pixels (one m64 each).  The producer warp stages the item's (8 BY + 2) x 18-pixel
+// halo patch as KC / 8 non-swizzled 8-channel planes [rows][18][8 ch] (16 bytes per pixel; zero outside the image and
+// beyond C_in) with 16-byte cp.async into a ring of patch slots.  Every tap (ky, kx) of a block is then the same K-major
+// operand at start offset (ky * 18 + kx) * 16 bytes (LBO = one plane, SBO = one patch row): one load serves all nine taps.
+// The two consumer warpgroups take alternate items (ping-pong), so one warpgroup's epilogue overlaps the other's wgmma.
+// The epilogue runs from registers: a thread's two accumulator rows are vertically adjacent pixels, its horizontal pool
+// partner is lane ^ 4, and a 4x4 transpose across the lanes of a quad turns the channel pairs into 16-byte stores.  Every
+// output element gets the wgmma products of k_conv_wg -- the same m64nNk16 shape, (filter column, tap, k-step) order and
+// operand values -- and the bias / ReLU / fp16 rounding / 2x2 max of tc_epilogue_cols_fast in the same order, so the
+// outputs are bit-identical to forms 0 and 1.
+constexpr int kHaloCols = 18;                                  // 16 output columns + 2
+// 8x8 blocks along y per item: 16x16 px where N <= 32 and N x KC <= 1024, else 16x8 (ptxas: 16x16 at N = 32, KC = 64 spills)
+constexpr int halo_by(int n, int kc) { return n <= 32 && n * kc <= 1024 ? 2 : 1; }
+constexpr int halo_plane(int n, int kc) { return (8 * halo_by(n, kc) + 2) * kHaloCols * 16; }
+
+// lane t of each quad holds piece k of chunks 0..3 in v[k]; afterwards it holds pieces 0..3 of chunk t (two xor stages)
+__device__ __forceinline__ void quad_transpose(uint32_t& v0, uint32_t& v1, uint32_t& v2, uint32_t& v3, int t) {
+  const bool o1 = t & 1, o2 = t & 2;
+  uint32_t r = __shfl_xor_sync(0xffffffffu, o1 ? v0 : v1, 1);
+  if (o1) v0 = r; else v1 = r;
+  r = __shfl_xor_sync(0xffffffffu, o1 ? v2 : v3, 1);
+  if (o1) v2 = r; else v3 = r;
+  r = __shfl_xor_sync(0xffffffffu, o2 ? v0 : v2, 2);
+  if (o2) v0 = r; else v2 = r;
+  r = __shfl_xor_sync(0xffffffffu, o2 ? v1 : v3, 2);
+  if (o2) v1 = r; else v3 = r;
+}
+
+__device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
+  const __half2 m = __hmax2(*reinterpret_cast<const __half2*>(&a), *reinterpret_cast<const __half2*>(&b));
+  return *reinterpret_cast<const uint32_t*>(&m);
+}
+
+template <int KSTEPS, int N>
+__global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_constant__ CUtensorMap mapA,
+                                                               const __grid_constant__ CUtensorMap mapB,
+                                                               const __grid_constant__ TcParams P) {
+  constexpr int BY = halo_by(N, 16 * KSTEPS), NB = 2 * BY;                  // blocks per item: 2 along x, BY along y
+  constexpr int NP = 2 * KSTEPS;                               // 8-channel planes of the chunk
+  constexpr int PH = 8 * BY + 2, PW = kHaloCols, PLANE = halo_plane(N, 16 * KSTEPS), SLOT = NP * PLANE;
+  constexpr int NJ = N / 8;                                    // 8-channel groups of the output
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* bank = base;                                        // 9 weight slices, swizzled as in k_conv_wg_p
+  uint8_t* ring = bank + 9 * (size_t)P.b_slot_bytes;
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)P.n_a_slots * SLOT);
+  uint64_t* empty = full + P.n_a_slots;
+  uint64_t* fullB = empty + P.n_a_slots;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_x = (P.W + 15) / 16, n_tiles = tiles_x * ((P.H + 8 * BY - 1) / (8 * BY));
+  const int n_work = n_tiles * P.batch;
+  if (threadIdx.x == 0) {
+    // full: one cp.async arrival per producer lane; empty: one arrival per warp of the consuming warpgroup
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(full + i), 32); mbar_init(smem_u32(empty + i), 4); }
+    mbar_init(smem_u32(fullB), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
+  }
+  __syncthreads();
+
+  if (warp == kConsumerThreads / 32) {
+    // ------------------------------ producer warp ------------------------------
+    if (lane == 0) {
+      // weights are static: load the bank (slice kx * 3 + ky = filter tap (ky, kx)) while the predecessor drains
+      mbar_expect_tx(smem_u32(fullB), (uint32_t)(9 * P.b_tx_bytes));
+      for (int kx = 0; kx < 3; ++kx)
+        for (int ky = 0; ky < 3; ++ky)
+          tma_load_3d(smem_u32(bank + (size_t)(kx * 3 + ky) * P.b_slot_bytes), &mapB, smem_u32(fullB), 0, 0, ky * 3 + kx);
+    }
+    griddep_wait();                                            // activations come from the previous kernel of the stream
+    const __half* in = reinterpret_cast<const __half*>(P.in);
+    for (int i = 0, w = blockIdx.x; w < n_work; ++i, w += gridDim.x) {
+      if (w + (int)gridDim.x >= n_work) griddep_launch();      // last item of this CTA
+      const int s = i % P.n_a_slots;
+      mbar_wait(smem_u32(empty + s), ((i / P.n_a_slots) & 1) ^ 1);
+      const int tile = w % n_tiles, b = w / n_tiles;
+      const int xs = (tile % tiles_x) * 16 - 1, ys = (tile / tiles_x) * (8 * BY) - 1;
+      const uint32_t dst = smem_u32(ring + (size_t)s * SLOT);
+      // piece e = (patch pixel, plane), plane fastest: a warp instruction reads whole pixels
+      for (int e = lane; e < NP * PH * PW; e += 32) {
+        const int pl = e % NP, p = e / NP, y = ys + p / PW, x = xs + p % PW;
+        const bool ok = y >= 0 && y < P.H && x >= 0 && x < P.W && pl * 8 < P.in_C;
+        const __half* src = ok ? in + (((size_t)b * P.H + y) * P.W + x) * P.in_Ctot + pl * 8 : in;
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(pl * PLANE + p * 16)), "l"(src),
+                     "r"(ok ? 16 : 0) : "memory");
+      }
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(full + s)) : "memory");
+    }
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    return;
+  }
+
+  // ------------------------------ consumers: warpgroup wg takes the CTA's items wg, wg + 2, ... ------------------------------
+  const int wg = warp >> 2, q = warp & 3, g = lane >> 2, t = lane & 3;
+  float bias[NJ][2];                                           // channels 8 j + 2 t (+ 1) of this thread's fragment columns
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) bias[j][e] = P.bias ? P.bias[8 * j + 2 * t + e] : 0.f;
+  const float lo = P.relu ? 0.f : -INFINITY;
+  const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
+  const uint64_t desc_b = make_desc(0, P.row_bytes, P.layout_type);
+  const uint32_t b_base = smem_u32(bank);
+  mbar_wait(smem_u32(fullB), 0);
+  float acc[NB][N / 2];
+  for (int i = wg, w = blockIdx.x + wg * (int)gridDim.x; w < n_work; i += 2, w += 2 * (int)gridDim.x) {
+    const int s = i % P.n_a_slots;
+    mbar_wait(smem_u32(full + s), (i / P.n_a_slots) & 1);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async writes (generic proxy) -> wgmma operand reads
+    const uint32_t a_base = smem_u32(ring + (size_t)s * SLOT);
+    wgmma_fence();
+#pragma unroll
+    for (int bk = 0; bk < NB; ++bk) wgmma_reg_fence(acc[bk]);
+#pragma unroll
+    for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int k = 0; k < KSTEPS; ++k) {
+          const uint64_t db = desc_b + (uint64_t)((b_base + (uint32_t)((kx * 3 + ky) * P.b_slot_bytes)) >> 4) + 2 * k;
+#pragma unroll
+          for (int bk = 0; bk < NB; ++bk) {
+            const uint32_t a = a_base + (uint32_t)(((8 * (bk >> 1) + ky) * PW + 8 * (bk & 1) + kx) * 16 + 2 * k * PLANE);
+            wgmma_f16<N>(acc[bk], desc_a + (uint64_t)(a >> 4), db, (kx | ky | k) ? 1u : 0u);
+          }
+        }
+    wgmma_commit();
+#pragma unroll
+    for (int bk = 0; bk < NB; ++bk) wgmma_reg_fence(acc[bk]);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int bk = 0; bk < NB; ++bk) wgmma_reg_fence(acc[bk]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(empty + s));           // the patch slot may be refilled
+
+    const int tile = w % n_tiles, b = w / n_tiles;
+    const int x0 = (tile % tiles_x) * 16, y0 = (tile / tiles_x) * (8 * BY);
+#pragma unroll
+    for (int bk = 0; bk < NB; ++bk) {
+      // this thread's pixels: (y, x) and (y + 1, x); piece r * NJ + j = channels 8 j + 2 t (+ 1) of row r, as half2
+      const int y = y0 + 8 * (bk >> 1) + 2 * q, x = x0 + 8 * (bk & 1) + g;
+      uint32_t hv[2 * NJ];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const __half2 h2 = __floats2half2_rn(fmaxf(acc[bk][4 * j + 2 * r] + bias[j][0], lo), fmaxf(acc[bk][4 * j + 2 * r + 1] + bias[j][1], lo));
+          hv[r * NJ + j] = *reinterpret_cast<const uint32_t*>(&h2);
+        }
+      if (P.pool_out != nullptr) {
+        // 2x2 max on the rounded halves in tc_epilogue_cols_fast's order: max(max(h(y, x), h(y, x + 1)), max(h(y + 1, x),
+        // h(y + 1, x + 1))) on the even-column lane, which stores
+        constexpr int NJ4 = (NJ + 3) / 4 * 4;
+        uint32_t pv[NJ4];
+#pragma unroll
+        for (int j = 0; j < NJ4; ++j) {
+          if (j < NJ) {
+            const uint32_t m0 = hmax2_u32(hv[j], __shfl_xor_sync(0xffffffffu, hv[j], 4));
+            const uint32_t m1 = hmax2_u32(hv[NJ + j], __shfl_xor_sync(0xffffffffu, hv[NJ + j], 4));
+            pv[j] = hmax2_u32(m0, m1);
+          } else {
+            pv[j] = 0u;
+          }
+        }
+        __half* pp = reinterpret_cast<__half*>(P.pool_out) + (((size_t)b * P.pool_H + (y >> 1)) * P.pool_W + (x >> 1)) * P.pool_Ctot +
+                     P.pool_coff;
+        const bool st = (g & 1) == 0 && y < P.H && x < P.W;
+#pragma unroll
+        for (int c0 = 0; c0 < NJ4; c0 += 4) {
+          quad_transpose(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3], t);
+          if (st && c0 + t < NJ) *reinterpret_cast<uint4*>(pp + 8 * (c0 + t)) = make_uint4(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3]);
+        }
+      }
+      if (!P.skip_out) {
+        __half* po = reinterpret_cast<__half*>(P.out) + (((size_t)b * P.out_H + y) * P.out_W + x) * P.out_Ctot + P.out_coff;
+#pragma unroll
+        for (int c0 = 0; c0 < 2 * NJ; c0 += 4) {
+          quad_transpose(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3], t);
+          const int c = c0 + t, r = c / NJ, j = c % NJ;
+          if (y + r < P.H && x < P.W)
+            *reinterpret_cast<uint4*>(po + (size_t)r * P.out_W * P.out_Ctot + 8 * j) = make_uint4(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3]);
+        }
+      }
+    }
+  }
+}
+
 // ------------------------------- host side ---------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -786,14 +979,15 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
 }
 
 // Kernel forms of one launch: 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with
-// resident weights.  Both give bit-identical outputs; the autotuner keeps the faster eligible one per launch
-// (SB_FORCE_VARIANT=n forces form n where it is eligible).
-constexpr int kForms = 2;
+// resident weights, 2 = the persistent halo-patch k_conv_wg_h.  All give bit-identical outputs; the autotuner keeps the
+// faster eligible one per launch (SB_FORCE_VARIANT=n forces form n where it is eligible).
+constexpr int kForms = 3;
 struct TcForm {
   int ok;
-  int n_a_slots, n_b_slots;
+  int n_a_slots, n_b_slots;    // halo form: n_a_slots = patch slots
   size_t smem;
-  int max_ctas;                // persistent form: CTAs the GPU holds at once
+  int max_ctas;                // persistent forms: CTAs the GPU holds at once
+  int n_tiles;                 // persistent forms: work items per frame
 };
 
 struct TcLaunch {
@@ -934,8 +1128,21 @@ static ConvKernel conv_kernel_p_n(int N) {
   }
 }
 
+// the halo instantiations: N <= 64; nullptr otherwise
+template <int KSTEPS>
+static ConvKernel conv_kernel_h_n(int N) {
+  switch (N) {
+    case 16: return k_conv_wg_h<KSTEPS, 16>;
+    case 32: return k_conv_wg_h<KSTEPS, 32>;
+    case 48: return k_conv_wg_h<KSTEPS, 48>;
+    case 64: return k_conv_wg_h<KSTEPS, 64>;
+    default: return nullptr;
+  }
+}
+
 static ConvKernel conv_kernel_form(int form, int KC, int N) {
   if (form == 0) return conv_kernel(KC, N);
+  if (form == 2) return KC == 16 ? conv_kernel_h_n<1>(N) : (KC == 32 ? conv_kernel_h_n<2>(N) : conv_kernel_h_n<4>(N));
   return KC == 16 ? conv_kernel_p_n<1>(N) : (KC == 32 ? conv_kernel_p_n<2>(N) : conv_kernel_p_n<4>(N));
 }
 
@@ -951,13 +1158,51 @@ static size_t conv_smem_resident(const TcParams& P, int n_a, int bank) {
          1024 /*align slack*/ + (size_t)(2 * n_a + 1) * 8 + 16 + 3 * (size_t)P.N * sizeof(float);
 }
 
-// Eligibility, ring sizes, shared memory and co-resident grid size of the resident form of launch L (forms[0], the
-// streaming form, is always eligible): one N tile, and the whole bank of the launch's weight slices plus at least 2
-// activation slots fit in 225 KB; two CTAs per SM where they fit in 113 KB.
+// shared memory of a k_conv_wg_h launch: weight bank (9 slices), n_a patch slots, 2 n_a + 1 barriers
+static size_t conv_smem_halo(const TcParams& P, int n_a) {
+  return 1024 /*align slack*/ + (size_t)9 * P.b_slot_bytes + (size_t)n_a * (P.KC / 8) * halo_plane(P.N, P.KC) + (size_t)(2 * n_a + 1) * 8;
+}
+
+// The halo form takes plain 3x3 stride-1 SAME convs (filter column g = dx + 1, tap ky of it = weight tap 3 ky + g) with one
+// input-channel chunk and the fast-epilogue output shape without a residual.
+static bool halo_eligible(const TcLaunch& L) {
+  const TcParams& P = L.P;
+  if (L.grid.y != 1 || P.n_chunks != 1 || P.N > 64 || P.epi_mode != 1 || P.res != nullptr || P.n_groups != 3 || P.dy0 != -1 ||
+      P.box_rows != TH + 2 || P.oy_mul != 1 || P.oy_add != 0 || P.ox_mul != 1 || P.ox_add != 0)
+    return false;
+  for (int g = 0; g < 3; ++g) {
+    if (P.groups[g].dx != g - 1 || P.groups[g].n_taps != 3) return false;
+    for (int ky = 0; ky < 3; ++ky)
+      if (P.groups[g].taps[ky].row_off != ky || P.groups[g].taps[ky].w_tap != 3 * ky + g) return false;
+  }
+  return true;
+}
+
+// Eligibility, ring sizes, shared memory and co-resident grid size of the persistent forms of launch L (forms[0], the
+// streaming form, is always eligible).  Resident form: one N tile, and the whole bank of the launch's weight slices plus
+// at least 2 activation slots fit in 225 KB; two CTAs per SM where they fit in 113 KB.  Halo form: halo_eligible, and the
+// bank plus at least 4 patch slots (two being read, two prefetched) fit in 225 KB; up to 8 slots, one CTA per SM.
 static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
   TcParams& P = L.P;
   L.form = 0;
   L.forms[0].ok = 1; L.forms[0].n_a_slots = P.n_a_slots; L.forms[0].n_b_slots = P.n_b_slots; L.forms[0].smem = L.smem;
+  auto fit = [&](TcForm& F, ConvKernel kern) {               // co-resident CTAs of an eligible form
+    int nb = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kConvThreads, F.smem) != cudaSuccess || nb < 1) {
+      cudaGetLastError();
+      F.ok = 0;
+      return;
+    }
+    F.max_ctas = nb * h->sm_count;
+  };
+  if (ConvKernel kern = conv_kernel_form(2, P.KC, P.N); kern && halo_eligible(L)) {
+    TcForm& F = L.forms[2];
+    for (int na = 8; na >= 4 && !F.ok; --na)
+      if (conv_smem_halo(P, na) <= kMaxDynSmem) { F.ok = 1; F.n_a_slots = na; F.n_b_slots = 9; F.smem = conv_smem_halo(P, na); }
+    const int by = halo_by(P.N, P.KC);
+    F.n_tiles = ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
+    if (F.ok) fit(F, kern);
+  }
   TcForm& F = L.forms[1];
   ConvKernel kern = conv_kernel_form(1, P.KC, P.N);
   if (!kern || L.grid.y != 1) return;
@@ -967,14 +1212,8 @@ static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
       if (conv_smem_resident(P, na, bank) <= budget) { F.ok = 1; F.n_a_slots = na; F.n_b_slots = bank; F.smem = conv_smem_resident(P, na, bank); }
     if (F.ok) break;
   }
-  if (!F.ok) return;
-  int nb = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kConvThreads, F.smem) != cudaSuccess || nb < 1) {
-    cudaGetLastError();
-    F.ok = 0;
-    return;
-  }
-  F.max_ctas = nb * h->sm_count;
+  F.n_tiles = P.n_tiles;
+  if (F.ok) fit(F, kern);
 }
 
 // The residual ADD right after conv `oi` can run in its epilogue: the conv's output has no other reader (the compiler
@@ -1071,6 +1310,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)TW, (cuuint32_t)P.box_rows, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     void* gptr = (void*)((__half*)ib.dev + in_coff);
+    P.in = gptr; P.in_Ctot = ib.C; P.in_C = Cin;
     CUresult r = enc(&L.mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, gptr, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
@@ -1538,7 +1778,7 @@ static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
     const TcForm& F = L.forms[L.form];
     P.n_a_slots = F.n_a_slots; P.n_b_slots = F.n_b_slots; P.batch = B; P.pdl_trigger = 0;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(std::min(P.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = F.smem;
+    cfg.gridDim = dim3(std::min(F.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = F.smem;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -1572,7 +1812,7 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   const bool dbg = getenv("SB_DEBUG") != nullptr;
   const char* fvar = getenv("SB_FORCE_VARIANT");
   const int force = fvar ? atoi(fvar) : -1;
-  static const char* const form_name[kForms] = {"streaming", "resident"};
+  static const char* const form_name[kForms] = {"streaming", "resident", "halo"};
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
     if (!plan || head_kernel_ok(m, m->ops[oi], plan)) continue;
