@@ -358,6 +358,73 @@ int sb_flow_fetch_level(sb_handle_t h, int flow_id, int64_t t, int level, uint8_
                         int* out_H, int* out_W, int* out_n_levels);
 int sb_flow_destroy(sb_handle_t h, int flow_id);
 
+/* ---- identity tracker on the device ----------------------------------------------------------
+ * sleap/nn/tracking.py:542-844 Tracker.track with the simple / simple-max-tracks candidate makers, one call per frame,
+ * replayed frame by frame by one CTA (k_track): pre-cull (target_instance_count + nms_fast), candidate pool,
+ * similarity matrix (float64), robust per-track reduction (max or np.quantile), greedy or Hungarian matching, new
+ * tracks, and the track_window queues, which stay on the device between calls.
+ * Tie rules: greedy visits pairs in np.argsort(cost, kind="stable") order (ascending flat index among equal costs);
+ * nms_fast orders equal instance scores by ascending index.  The host's default sorts leave these orders
+ * implementation-defined.
+ * Capacities (checked at create, SB_ERR_INVALID): max_instances 1..128 per frame, n_nodes 1..64, track_window 1..64,
+ * track_table 1..65536 (simple-max-tracks: the per-track queues; max_tracking requires track_table >= max_tracks).
+ * sb_track_instances: points (B, I, n_nodes, 2), point confidences (B, I, n_nodes), scores (B, I), counts (B),
+ * img_hw (B, 2) (normalized_instance only; may be NULL otherwise), t (B) frame indices (t < 0: the host's _next_t).
+ * Per frame b the output lists the tracked instances in Tracker.track's order: out_index (B, I) index into the input,
+ * out_track (B, I) track id in spawn order (name track_{id}), out_score (B, I) tracking score (-cost; 0 for a new
+ * track), out_matched (B, I) 1 when matched, out_n (B), out_t (B) the frame index used.  *out_n_done = frames
+ * tracked; *out_flag = SB_TRACK_INFEASIBLE when the Hungarian matcher met a matrix SciPy rejects (frame *out_n_done,
+ * left untracked, state as before it).  A count above I, or a max-tracks queue table that would grow past
+ * track_table, returns SB_ERR_INVALID; the frames before it are tracked (*out_n_done). */
+#define SB_TRACK_SIMPLE 0
+#define SB_TRACK_SIMPLE_MAX_TRACKS 1
+#define SB_TRACK_SIM_INSTANCE 0
+#define SB_TRACK_SIM_NORMALIZED_INSTANCE 1
+#define SB_TRACK_SIM_OBJECT_KEYPOINT 2
+#define SB_TRACK_SIM_CENTROID 3
+#define SB_TRACK_SIM_IOU 4
+#define SB_TRACK_MATCH_GREEDY 0
+#define SB_TRACK_MATCH_HUNGARIAN 1
+#define SB_TRACK_OKS_ALL 0
+#define SB_TRACK_OKS_REF 1
+#define SB_TRACK_OKS_UNION 2
+#define SB_TRACK_INFEASIBLE 1
+typedef struct sb_tracker_params {
+  int32_t maker, similarity, match;         /* SB_TRACK_* */
+  int32_t track_window;
+  int32_t max_tracks, max_tracking;         /* max_tracks <= 0: none */
+  int32_t min_match_points, min_new_track_points;
+  double robust;                            /* 0 < robust < 1: np.quantile, else max */
+  int32_t cull_target;                      /* target_instance_count when pre_cull_to_target, else 0 */
+  int32_t cull_use_iou;                     /* pre_cull_iou_threshold given and nonzero */
+  double cull_iou_threshold;
+  const double* oks_errors;                 /* NULL / n_oks_errors = 0: 1 */
+  int32_t n_oks_errors;
+  int32_t oks_score_weighting, oks_normalization;
+  int32_t n_nodes, max_instances, track_table;
+} sb_tracker_params;
+int sb_tracker_create(sb_handle_t h, const sb_tracker_params* params, int* out_tracker_id);
+int sb_tracker_reset(sb_handle_t h, int tracker_id);
+int sb_tracker_destroy(sb_handle_t h, int tracker_id);
+int sb_track_instances(sb_handle_t h, int tracker_id, int B, int I, const double* points, const double* point_conf,
+                       const double* scores, const int32_t* counts, const double* img_hw, const int64_t* t,
+                       int32_t* out_index, int32_t* out_track, double* out_score, int32_t* out_matched,
+                       int32_t* out_n, int64_t* out_t, int32_t* out_n_done, int32_t* out_flag);
+/* The tracker inside the bottom-up step.  sb_bottomup_attach_tracker(tracker_id = -1 detaches): every later
+ * sb_infer_bottomup / sb_infer_bottomup_dev / sb_bottomup_submit call runs k_track on the post-processing stream right
+ * after the grouping kernel, on the instance list Predictor._frames_from_example builds from each frame (all-NaN rows
+ * skipped; max_instances >= 0: the top scores, stable), with the frame size img_h x img_w (normalized_instance) and
+ * t = the host's _next_t.  The tracker must live on the model's handle, have its n_nodes and at least its
+ * max_instances, and the record exchange must not be connected (one rank).  The per-frame track records
+ * ([B][2 + 3 I] doubles, I = the tracker's max_instances: n, flag, order[I] (index into that instance list), track
+ * id[I], tracking score[I]; flag != 0: the frame was not tracked -- SB_TRACK_INFEASIBLE, or 2 = queue table full)
+ * are a separate buffer: the result records and record_width do not change.  They come back with the result copy:
+ * sb_bottomup_tracks(slot 0 / 1 after sb_bottomup_collect, -1 after sb_infer_bottomup); sb_bottomup_device_tracks
+ * copies the last step's records after sb_infer_bottomup_dev. */
+int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int max_instances, double img_h, double img_w);
+int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks);
+int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tracks);
+
 #ifdef __cplusplus
 }
 #endif

@@ -62,6 +62,15 @@ class TopdownParams(ctypes.Structure):
                 ("max_crops_per_call", c_int32)]
 
 
+class TrackerParams(ctypes.Structure):
+    _fields_ = [("maker", c_int32), ("similarity", c_int32), ("match", c_int32), ("track_window", c_int32),
+                ("max_tracks", c_int32), ("max_tracking", c_int32), ("min_match_points", c_int32),
+                ("min_new_track_points", c_int32), ("robust", ctypes.c_double), ("cull_target", c_int32),
+                ("cull_use_iou", c_int32), ("cull_iou_threshold", ctypes.c_double), ("oks_errors", c_void_p),
+                ("n_oks_errors", c_int32), ("oks_score_weighting", c_int32), ("oks_normalization", c_int32),
+                ("n_nodes", c_int32), ("max_instances", c_int32), ("track_table", c_int32)]
+
+
 # name -> argtypes (restype is always int unless noted)
 _SIGS = {
     "sb_version": [],
@@ -131,6 +140,14 @@ _SIGS = {
     "sb_flow_fetch_level": [c_void_p, c_int, c_int64, c_int, c_void_p, c_void_p, POINTER(c_int), POINTER(c_int),
                             POINTER(c_int)],
     "sb_flow_destroy": [c_void_p, c_int],
+    "sb_tracker_create": [c_void_p, POINTER(TrackerParams), POINTER(c_int)],
+    "sb_tracker_reset": [c_void_p, c_int],
+    "sb_bottomup_attach_tracker": [c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double],
+    "sb_bottomup_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
+    "sb_bottomup_device_tracks": [c_void_p, c_int, c_int, c_void_p],
+    "sb_tracker_destroy": [c_void_p, c_int],
+    "sb_track_instances": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), POINTER(c_int32)],
 }
 
 EXPORTED_SYMBOLS = sorted(list(_SIGS.keys()) + ["sb_last_error"])

@@ -12,8 +12,9 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 # per-file extra flags: post-processing must not contract multiply-adds (bit-exact parity); the flow kernels neither,
-# so that their float steps round like OpenCV's (sb_flow.cu header)
-EXTRA = {"sb_post.cu": ["-fmad=false"], "sb_flow.cu": ["-fmad=false"]}
+# so that their float steps round like OpenCV's (sb_flow.cu header); nor the tracker, whose float64 similarities
+# restate numpy's (sb_track.cu header)
+EXTRA = {"sb_post.cu": ["-fmad=false"], "sb_flow.cu": ["-fmad=false"], "sb_track.cu": ["-fmad=false"]}
 
 
 def sources():

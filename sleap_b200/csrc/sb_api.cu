@@ -62,6 +62,7 @@ int sb_destroy(sb_handle_t h) {
   cudaDeviceSynchronize();
   sb_models_free(h);
   sb_flows_free(h);
+  sb_trackers_free(h);
   for (void* p : h->owned) cudaFree(p);
   for (int i = 0; i < 3; ++i) { if (h->aux_stream[i]) cudaStreamDestroy(h->aux_stream[i]); if (h->join_ev[i]) cudaEventDestroy(h->join_ev[i]); }
   if (h->fork_ev) cudaEventDestroy(h->fork_ev);

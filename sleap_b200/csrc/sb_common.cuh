@@ -13,6 +13,7 @@
 
 struct SbModel;
 struct SbFlow;
+struct SbTracker;
 
 // Device workspace for the post-processing stages (capacity-bounded, per sample).
 struct SbPostWs {
@@ -96,6 +97,7 @@ struct sb_handle_s {
   std::vector<void*> owned;                 // generic device allocations freed at destroy
   std::vector<SbModel*> models;
   std::vector<SbFlow*> flows;               // sb_flow_create objects (sb_flow.cu); index = flow id
+  std::vector<SbTracker*> trackers;         // sb_tracker_create objects (sb_track.cu); index = tracker id
   int gpu_launches = 0;                     // kernels launched by this handle (bench: gpu_launches)
   int sm_count = 132;
 };
@@ -105,6 +107,16 @@ extern thread_local std::string g_sb_last_error;
 int sb_fail(sb_handle_s* h, int code, const char* fmt, ...);
 void sb_models_free(sb_handle_s* h);
 void sb_flows_free(sb_handle_s* h);
+void sb_trackers_free(sb_handle_s* h);
+// ---- device tracker (sb_track.cu) inside the bottom-up step ----
+SbTracker* sb_tracker_get(sb_handle_s* h, int id);
+int sb_tracker_max_instances(const SbTracker* t);
+int sb_tracker_nodes(const SbTracker* t);
+static __host__ __device__ inline size_t sb_track_record_width(int I) { return 2 + 3 * (size_t)I; }
+// k_track on the grouping output of a batch (ws.inst_*), then one track record per frame into out_records
+int sbk_track_step(sb_handle_s* h, SbTracker* tr, int B, const float* inst_peaks, const float* inst_vals,
+                   const float* inst_scores, const int* n_inst, int I_src, int max_instances, double img_h, double img_w,
+                   double* out_records);
 
 #define SB_CUDA(h, expr)                                                              \
   do {                                                                                \

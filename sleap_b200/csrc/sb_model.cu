@@ -38,6 +38,8 @@ void sb_models_free(sb_handle_s* h) {
     if (m->gpoints) cudaFree(m->gpoints);
     if (m->gvals) cudaFree(m->gvals);
     if (m->rec_host) cudaFreeHost(m->rec_host);
+    if (m->trk_dev) cudaFree(m->trk_dev);
+    for (int i = 0; i < 3; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
     for (int i = 0; i < 2; ++i) {
       if (m->frames_slot[i]) cudaFree(m->frames_slot[i]);
       if (m->stage_host[i]) cudaFreeHost(m->stage_host[i]);
@@ -667,7 +669,19 @@ static int bottomup_post_kernels(sb_handle_s* h, SbModel* m, int B) {
     if (!rc) m->gather.step++;
     return rc;
   }
-  return sbk_group(h, B, p.n_nodes, p.min_instance_peaks, p.min_line_scores, p.input_scale, m->ws);
+  if ((rc = sbk_group(h, B, p.n_nodes, p.min_instance_peaks, p.min_line_scores, p.input_scale, m->ws))) return rc;
+  if (!m->trk) return 0;
+  if (B > m->trk_B) return sb_fail(h, SB_ERR_INVALID, "attached tracker was sized for %d frames per step, not %d", m->trk_B, B);
+  return sbk_track_step(h, m->trk, B, m->ws.inst_peaks, m->ws.inst_vals, m->ws.inst_scores, m->ws.n_inst, p.max_instances,
+                        m->trk_cut, m->trk_h, m->trk_w, m->trk_dev);
+}
+
+// The track records of a batch go to the host with its result records, on the same stream.
+static int queue_track_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, int which) {
+  if (!m->trk) return 0;
+  SB_CUDA(h, cudaMemcpyAsync(m->trk_host[which], m->trk_dev, (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double),
+                             cudaMemcpyDeviceToHost, rs));
+  return 0;
 }
 
 // Peak finding / PAF scoring / matching / grouping of this batch on the handle's post-processing
@@ -711,6 +725,7 @@ int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, i
   cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
   if (!m->rec_host) SB_CUDA(h, cudaHostAlloc((void**)&m->rec_host, stage_floats(m) * sizeof(float), cudaHostAllocDefault));
   if ((rc = queue_result_copy(h, m, B, rs, m->rec_host, 3))) return rc;
+  if ((rc = queue_track_copy(h, m, B, rs, 2))) return rc;
   SB_CUDA(h, cudaStreamSynchronize(rs));
   h->post_pending = false;
   m->rec_B = B;
@@ -769,6 +784,7 @@ int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, 
   if ((rc = bottomup_post(h, m, B))) return rc;
   cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
   if ((rc = queue_result_copy(h, m, B, rs, m->stage_host[slot], 1 + slot))) return rc;
+  if ((rc = queue_track_copy(h, m, B, rs, slot))) return rc;
   m->slot_B[slot] = B;
   SB_CUDA(h, cudaEventRecord(m->result_ev[slot], rs));
   m->slot_used[slot] = true;
@@ -810,6 +826,56 @@ int sb_bottomup_device_outputs(sb_handle_t h, int model_id, float** instance_pea
   if (instance_scores_dev) *instance_scores_dev = m->ws.inst_scores;
   if (n_valid_dev) *n_valid_dev = m->ws.n_inst;
   if (flags_dev) *flags_dev = m->ws.flags;
+  return SB_OK;
+}
+
+int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int max_instances, double img_h, double img_w) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if (h->post_pending) SB_CUDA(h, cudaStreamSynchronize(h->post_stream));
+  if (tracker_id < 0) { m->trk = nullptr; return SB_OK; }
+  SbTracker* t = sb_tracker_get(h, tracker_id);
+  if (!t) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_attach_tracker: no tracker %d on this handle", tracker_id);
+  if (m->gather.connected)
+    return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_bottomup_attach_tracker: the record exchange is connected (one rank only)");
+  if (sb_tracker_nodes(t) != m->bu.n_nodes || sb_tracker_max_instances(t) < m->bu.max_instances)
+    return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_attach_tracker: tracker of %d nodes / %d instances, predictor of %d / %d",
+                   sb_tracker_nodes(t), sb_tracker_max_instances(t), m->bu.n_nodes, m->bu.max_instances);
+  if (!(img_h > 0) || !(img_w > 0)) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_attach_tracker: image %g x %g", img_h, img_w);
+  const int I = sb_tracker_max_instances(t);
+  if (m->trk_B < m->B || m->trk_I != I) {
+    cudaFree(m->trk_dev); m->trk_dev = nullptr;
+    for (int i = 0; i < 3; ++i) { cudaFreeHost(m->trk_host[i]); m->trk_host[i] = nullptr; }
+    m->trk_B = 0;
+    const size_t n = (size_t)m->B * sb_track_record_width(I);
+    int rc;
+    if ((rc = sb_dev_alloc(h, &m->trk_dev, n))) return rc;
+    for (int i = 0; i < 3; ++i) SB_CUDA(h, cudaHostAlloc((void**)&m->trk_host[i], n * sizeof(double), cudaHostAllocDefault));
+    m->trk_B = m->B; m->trk_I = I;
+  }
+  m->trk = t; m->trk_cut = max_instances < 0 ? -1 : max_instances; m->trk_h = img_h; m->trk_w = img_w;
+  return SB_OK;
+}
+
+int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: no tracker attached");
+  if (slot < -1 || slot > 1 || B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: bad slot / batch");
+  if (slot >= 0) SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
+  memcpy(out_tracks, m->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double));
+  return SB_OK;
+}
+
+int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tracks) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_device_tracks: no tracker attached");
+  if (B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_device_tracks: bad batch");
+  SB_CUDA(h, cudaSetDevice(h->device));
+  cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
+  SB_CUDA(h, cudaMemcpyAsync(out_tracks, m->trk_dev, (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double),
+                             cudaMemcpyDeviceToHost, rs));
+  SB_CUDA(h, cudaStreamSynchronize(rs));
   return SB_OK;
 }
 

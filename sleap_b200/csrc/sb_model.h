@@ -116,6 +116,13 @@ struct SbModel {
   bool conv01_enabled = false;             // the autotuner measured it faster than the two separate launches
   SbGather gather;                         // peer-memory exchange of the result records (sb_gather.cu)
   bool keep_dead_stores = false;           // sb_model_forward asked for a tensor whose stores are normally elided
+  // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu); its per-frame track records
+  // ([B][sb_track_record_width] doubles) live beside the result records and travel with the result copy
+  SbTracker* trk = nullptr;
+  int trk_B = 0, trk_I = 0, trk_cut = -1;
+  double trk_h = 1.0, trk_w = 1.0;
+  double* trk_dev = nullptr;
+  double* trk_host[3] = {nullptr, nullptr, nullptr};   // pinned: collect slots 0 / 1, sb_infer_bottomup
 };
 
 int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);

@@ -503,6 +503,38 @@ class BottomUpInferenceLayer(InferenceLayer):
         self.max_instances = max_instances
         self._cfg_key = None
         self._keep = None
+        # a Tracker with track_device, run by k_track inside each step (BottomUpPredictor.predict sets it for its span),
+        # and the predictor's max_instances cut of the instance list (-1: none)
+        self.tracker = None
+        self.tracker_cut = -1
+
+    def attach_tracker(self, image_hw):
+        """Attach ``self.tracker`` to the configured model for the frames of size ``image_hw`` (sb_bottomup_attach_tracker)."""
+        if self.tracker is None:
+            return
+        m = self.keras_model
+        dev = self.tracker._device_tracker(self.paf_scorer.n_nodes, handle=m.handle, max_instances=self.max_instances)
+        m.handle.call("sb_bottomup_attach_tracker", m.model_id, dev.id, int(self.tracker_cut), float(image_hw[0]),
+                      float(image_hw[1]))
+
+    def detach_tracker(self):
+        m = self.keras_model
+        if getattr(self.tracker, "_device", None) is not None and self._cfg_key is not None:
+            m.handle.call("sb_bottomup_attach_tracker", m.model_id, -1, -1, 1.0, 1.0)
+
+    def track_fields(self, slot, B):
+        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields:
+        track_order / track_ids / tracking_scores (B, I) (order = index into the frame's instance list, -1 padded),
+        track_n and track_flags (B)."""
+        if self.tracker is None:
+            return {}
+        I = self.tracker._device.max_instances
+        rec = np.zeros((B, 2 + 3 * I), np.float64)
+        m = self.keras_model
+        m.handle.call("sb_bottomup_tracks", m.model_id, slot, B, ptr(rec))
+        return {"track_n": rec[:, 0].astype(np.int64), "track_flags": rec[:, 1].astype(np.int64),
+                "track_order": rec[:, 2:2 + I].astype(np.int64), "track_ids": rec[:, 2 + I:2 + 2 * I].astype(np.int64),
+                "tracking_scores": rec[:, 2 + 2 * I:].copy()}
 
     def params(self) -> BottomUpParams:
         ps = self.paf_scorer
@@ -535,11 +567,13 @@ class BottomUpInferenceLayer(InferenceLayer):
             self._cfg_key = key
 
     def call(self, data):
-        imgs = self._prep(_images_of(data))
+        raw = _images_of(data)
+        imgs = self._prep(raw)
         if imgs.dtype != np.uint8:
             raise ValueError("BottomUpInferenceLayer expects uint8 frames (the fused path reads raw frames).")
         B, H, W, C = imgs.shape
         self._configure(B, H, W, C)
+        self.attach_tracker(np.asarray(raw[0]).shape[:2])
         m = self.keras_model
         I, N = self.max_instances, self.paf_scorer.n_nodes
         ip = np.zeros((B, I, N, 2), np.float32)
@@ -551,6 +585,7 @@ class BottomUpInferenceLayer(InferenceLayer):
         n = int(nv.max()) if B else 0
         out = {"instance_peaks": ip[:, :n].copy(), "instance_peak_vals": iv[:, :n].copy(),
                "instance_scores": isc[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
+        out.update(self.track_fields(-1, B))
         pg = getattr(m, "peer_gather", None)
         if pg is not None:          # multi-GPU: this call was one exchange step; the window came over with the result copy
             out["gathered_records"], out["gathered_counts"] = pg.gathered(-1, B, I, N)
@@ -646,6 +681,7 @@ class BottomUpInferenceModel(InferenceModel):
             return
         _, H, W, C = first.shape
         layer._configure(batch_size, H, W, C)
+        layer.attach_tracker(np.asarray(imgs[0]).shape[:2])
         m = layer.keras_model
         I, N = layer.max_instances, layer.paf_scorer.n_nodes
         starts = list(range(0, n, batch_size))
@@ -668,6 +704,7 @@ class BottomUpInferenceModel(InferenceModel):
             w = int(nv.max()) if B else 0
             out = {"instance_peaks": ip[:, :w], "instance_peak_vals": iv[:, :w], "instance_scores": isc[:, :w],
                    "n_valid": nv.astype(np.int64), "flags": fl}
+            out.update(layer.track_fields(k % 2, B))
             pg = getattr(m, "peer_gather", None)
             if pg is not None:      # multi-GPU: every rank's records of this step came over with the result copy (sb_gather_*)
                 out["gathered_records"], out["gathered_counts"] = pg.gathered(k % 2, B, I, N)
@@ -1136,6 +1173,7 @@ class Predictor:
         """:3230-3343 pattern: a consumer thread builds the objects while the batch loop runs."""
         q: "queue.Queue" = queue.Queue()
         frames: List[LabeledFrame] = []
+        errors: list = []
 
         def worker():
             while True:
@@ -1143,7 +1181,13 @@ class Predictor:
                 if ex is None:
                     return
                 new = self._frames_from_example(ex)
-                if self.tracker is not None:                     # sequential by nature; runs on the consumer thread
+                if "track_ids" in ex:                            # tracked on the device inside the step: map ids to Tracks
+                    try:
+                        self._apply_device_tracks(ex, new)
+                    except Exception as e:                       # raised on the calling thread after the join
+                        errors.append(e)
+                        return
+                elif self.tracker is not None:                   # sequential by nature; runs on the consumer thread
                     hw = tuple(ex.get("image_hw") or (1, 1))
                     for k, lf in enumerate(new):
                         img = ex["image"][k] if "image" in ex else None
@@ -1158,9 +1202,23 @@ class Predictor:
         finally:
             q.put(None)
             t.join()
+        if errors:
+            raise errors[0]
         if self.tracker is not None:                                 # :2702-2703, :3345-3346
             self.tracker.final_pass(frames)
         return frames
+
+    def _apply_device_tracks(self, ex, new):
+        """The frames' tracked lists from the track records of their step (BottomUpPredictor with a device tracker)."""
+        for k, lf in enumerate(new):
+            flag = int(ex["track_flags"][k])
+            if flag == 1:
+                raise ValueError("cost matrix is infeasible")
+            if flag:
+                raise _lib.SleapB200Error(f"the device tracker's track queue table is full (frame {lf.frame_idx})")
+            n = int(ex["track_n"][k])
+            lf.instances = self.tracker.apply_device_tracks(lf.instances, lf.frame_idx, ex["track_order"][k, :n],
+                                                            ex["track_ids"][k, :n], ex["tracking_scores"][k, :n])
 
     def _frames_from_example(self, ex):
         out = []
@@ -1316,6 +1374,28 @@ class BottomUpPredictor(Predictor):
         self.max_instances = max_instances
         self._caps = (max_peaks_per_sample, max_node_peaks, max_instances_per_frame)
         self._initialize_inference_model()
+
+    def predict(self, data, make_labels: bool = True):
+        """As Predictor.predict.  A tracker with ``track_device`` runs inside each bottom-up step (k_track after the
+        grouping kernel, on the model's GPU); the consumer thread only maps its track ids to ``Track`` objects before
+        ``final_pass``.  The tracker's GPU must be the model's, and the run must be on one rank."""
+        tr = self.tracker
+        if tr is None or getattr(tr, "track_device", None) is None or tr.candidate_maker is None:
+            return super().predict(data, make_labels)
+        layer = self.inference_model.bottomup_layer
+        m = layer.keras_model
+        if int(str(tr.track_device).split(":")[-1]) != m.handle.device_id:
+            raise ValueError(f"the tracker's track_device {tr.track_device!r} is not the model's GPU ({m.handle.device_id})")
+        if getattr(m, "peer_gather", None) is not None or int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            raise ValueError("a device tracker tracks one rank's frames: run the multi-rank prediction without track_device")
+        if not make_labels:                          # no labeled frames, nothing to track (as with the host tracker)
+            return super().predict(data, make_labels)
+        layer.tracker, layer.tracker_cut = tr, -1 if self.max_instances is None else int(self.max_instances)
+        try:
+            return super().predict(data, make_labels)
+        finally:
+            layer.detach_tracker()
+            layer.tracker = None
 
     def _initialize_inference_model(self):
         """:3119-3150."""

@@ -17,6 +17,7 @@ Sequential host code by nature (frame t depends on t-1); instances are anything 
 ``score`` and a settable ``track`` (``sleap_b200.nn.inference.PredictedInstance``).
 """
 import copy
+import ctypes
 from collections import deque
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -509,6 +510,67 @@ class FlowMaxTracksCandidateMaker(FlowCandidateMaker):
         return self.resolve_requests(requests, img, t)
 
 
+class DeviceTracker:
+    """The queues and spawned-track counter of one tracker, resident on a GPU (sb_tracker_create), and its per-call
+    step (sb_track_instances: k_track).  ``params``: the fields of sb_tracker_params.  It has a handle of its own, so
+    that a predictor's consumer thread can track while the predictor's handle runs the next batch."""
+
+    def __init__(self, device, params: dict, handle=None):
+        from sleap_b200 import _lib
+        self._lib = _lib
+        self.handle = handle if handle is not None else _lib.Handle(int(str(device).split(":")[-1]))
+        self.params = dict(params)
+        errs = self.params.pop("oks_errors", None)
+        self._errs = None if errs is None or len(errs) == 0 else np.ascontiguousarray(errs, np.float64)
+        p = _lib.TrackerParams(**self.params, oks_errors=None if self._errs is None else _lib.ptr(self._errs),
+                               n_oks_errors=0 if self._errs is None else len(self._errs))
+        out = ctypes.c_int()
+        self.handle.call("sb_tracker_create", ctypes.byref(p), ctypes.byref(out))
+        self.id = out.value
+        self.n_nodes, self.max_instances = int(params["n_nodes"]), int(params["max_instances"])
+
+    def track(self, instance_lists: list, ts: Sequence[Optional[int]], img_hws: Sequence[Tuple[int, int]]) -> list:
+        """-> (per frame done: (input indices, track ids, tracking scores, matched flags, frame index), error).  The
+        error (None when every frame was tracked) is the one the host tracker raises at the first frame not tracked:
+        ValueError for a matrix SciPy's Hungarian matcher rejects, SleapB200Error for a capacity overflow."""
+        B, C = len(instance_lists), self.n_nodes
+        I = max([1] + [len(x) for x in instance_lists])
+        pts = np.full((B, I, C, 2), np.nan)
+        conf = np.ones((B, I, C))
+        scores = np.zeros((B, I))
+        for b, lst in enumerate(instance_lists):
+            for i, x in enumerate(lst):
+                p = _pts(x)
+                if p.shape != (C, 2):
+                    raise ValueError(f"instance with {p.shape[0]} nodes given to a tracker of {C}")
+                pts[b, i] = p
+                conf[b, i] = np.asarray(getattr(x, "point_confidences", np.ones(C)), np.float64)
+                scores[b, i] = x.score
+        counts = np.asarray([len(x) for x in instance_lists], np.int32)
+        hw = np.ascontiguousarray(np.asarray(img_hws, np.float64).reshape(B, 2))
+        t = np.asarray([-1 if x is None else int(x) for x in ts], np.int64)
+        o_idx, o_tid = np.zeros((B, I), np.int32), np.zeros((B, I), np.int32)
+        o_score, o_m = np.zeros((B, I)), np.zeros((B, I), np.int32)
+        o_n, o_t = np.zeros(B, np.int32), np.zeros(B, np.int64)
+        n_done, flag = ctypes.c_int32(), ctypes.c_int32()
+        P = self._lib.ptr
+        rc = self._lib.lib().sb_track_instances(self.handle.h, self.id, B, I, P(pts), P(conf), P(scores), P(counts), P(hw),
+                                                P(t), P(o_idx), P(o_tid), P(o_score), P(o_m), P(o_n), P(o_t),
+                                                ctypes.byref(n_done), ctypes.byref(flag))
+        err = None
+        if rc != 0:
+            err = self._lib.SleapB200Error(f"sb_track_instances failed ({rc}): {self._lib.lib().sb_last_error(self.handle.h).decode()}")
+        elif flag.value != 0:
+            err = ValueError("cost matrix is infeasible")
+        return [(o_idx[b, :o_n[b]].tolist(), o_tid[b, :o_n[b]], o_score[b, :o_n[b]], o_m[b, :o_n[b]], o_t[b])
+                for b in range(n_done.value)], err
+
+
+DEVICE_MAKERS = dict(simple=0, simplemaxtracks=1)
+DEVICE_SIMILARITIES = dict(instance=0, normalized_instance=1, object_keypoint=2, centroid=3, iou=4)
+DEVICE_MATCHERS = dict(greedy=0, hungarian=1)
+DEVICE_OKS_NORMALIZATIONS = dict(all=0, ref=1, union=2)
+
 SIMILARITIES = dict(instance=instance_similarity, centroid=centroid_distance, iou=instance_iou,
                     normalized_instance=normalized_instance_similarity, object_keypoint=factory_object_keypoint_similarity)
 MATCHERS = dict(hungarian=hungarian_matching, greedy=greedy_matching)
@@ -568,6 +630,11 @@ class Tracker:
     def track(self, untracked_instances: list, img_hw: Tuple[int, int] = (1, 1), img=None, t: Optional[int] = None) -> list:
         if self.candidate_maker is None:
             return untracked_instances
+        if self.track_device is not None:
+            out, err = self.track_frames([list(untracked_instances)], [t], [img_hw])
+            if err is not None:
+                raise err
+            return out[0]
         sim = self.similarity_function
         if sim is normalized_instance_similarity:
             sim = lambda a, b: normalized_instance_similarity(a, b, img_hw=img_hw)
@@ -611,6 +678,57 @@ class Tracker:
 
     cleaner: Optional["TrackCleaner"] = None          # deprecated --clean_instance_count path (:924-927)
     post_connect_single_breaks: bool = False
+    # GPU (index or "cuda:N") whose k_track kernel runs the whole per-frame step (make_tracker_by_name(track_device=...))
+    track_device = None
+    device_params: Optional[dict] = None               # the sb_tracker_params of that tracker, set with track_device
+    device_max_instances = 128                         # per-frame capacity of the device tracker (at most 128)
+    device_track_table = 4096                          # max-tracks queue table without a max_tracks cap
+
+    def _device_tracker(self, n_nodes: int, handle=None, max_instances: Optional[int] = None) -> "DeviceTracker":
+        """The device state of this tracker, made on first use: on its own handle of ``track_device``, or on ``handle``
+        (a predictor's, so that the tracker can run inside its bottom-up step)."""
+        dev = getattr(self, "_device", None)
+        if dev is None:
+            table = self.device_track_table
+            if self.has_max_tracking and self.max_tracking:
+                table = int(self.max_tracks)
+            dev = self._device = DeviceTracker(self.track_device, dict(
+                self.device_params, n_nodes=n_nodes, max_instances=max(self.device_max_instances, max_instances or 0),
+                track_table=table), handle=handle)
+            pending, self._pending = getattr(self, "_pending", []), []
+            if pending:                                # empty frames seen before the node count was known
+                dev.track([[] for _ in pending], [t for t, _ in pending], [hw for _, hw in pending])
+        elif handle is not None and dev.handle is not handle:
+            raise ValueError("this tracker's device state lives on another handle than the predictor's; make a new tracker")
+        return dev
+
+    def apply_device_tracks(self, instances: list, frame_idx: int, order, track_ids, scores, matched=None) -> list:
+        """The tracked list of one frame from the device's output: copies of ``instances[order[k]]`` with the ``Track``
+        of ``track_ids[k]`` (made in spawn order, ``spawned_on`` = the frame that spawned it) and, when matched, the
+        tracking score."""
+        tracked = []
+        for k in range(len(order)):
+            tid = int(track_ids[k])
+            while tid >= len(self.spawned_tracks):
+                self.spawned_tracks.append(Track(spawned_on=int(frame_idx), name=f"track_{len(self.spawned_tracks)}"))
+            x = copy.copy(instances[int(order[k])])
+            x.track = self.spawned_tracks[tid]
+            if matched is None or matched[k]:
+                x.tracking_score = float(scores[k])
+            tracked.append(x)
+        return tracked
+
+    def track_frames(self, instance_lists: list, ts: Sequence[Optional[int]], img_hws: Sequence[Tuple[int, int]]):
+        """``track`` of several frames in one ``sb_track_instances`` call on ``track_device`` -> (the tracked list of
+        every frame tracked, in ``track``'s order, error).  As on the host, the frames before an error are tracked
+        and the error (None if there is none) is for the caller to raise."""
+        n_nodes = next((len(_pts(x)) for lst in instance_lists for x in lst), None)
+        if getattr(self, "_device", None) is None and n_nodes is None:
+            self._pending = getattr(self, "_pending", []) + [(t, hw) for t, hw in zip(ts, img_hws)]
+            return [[] for _ in instance_lists], None
+        res, err = self._device_tracker(n_nodes).track(instance_lists, ts, img_hws)
+        return [self.apply_device_tracks(lst, t, idx, tids, scores, matched)
+                for lst, (idx, tids, scores, matched, t) in zip(instance_lists, res)], err
 
     def final_pass(self, frames: list):
         """:816-835: post-processing after the last frame -- the (deprecated) cleaner, or the single-break joining."""
@@ -635,12 +753,24 @@ class Tracker:
                              of_max_levels: int = 3, save_shifted_instances: bool = False, kf_init_frame_count: int = 0,
                              kf_node_indices: Optional[list] = None, post_connect_single_breaks: bool = False,
                              clean_instance_count: int = 0, clean_iou_threshold: Optional[float] = None, of_device=None,
-                             **kwargs) -> "Tracker":
+                             track_device=None, **kwargs) -> "Tracker":
         """``of_device``: GPU (index or "cuda:N") that runs the flow shift of the flow trackers; None (default) runs
-        it with cv2 on the CPU, as the reference does."""
+        it with cv2 on the CPU, as the reference does.
+
+        ``track_device``: GPU (index or "cuda:N") that runs the whole per-frame step of the simple and
+        simple-max-tracks trackers (pre-cull, candidates, similarities, matching, new tracks, queues) in one kernel,
+        the queues staying on the GPU; ``final_pass`` stays on the host.  Ties between equal greedy costs go to the
+        lower flat index (``np.argsort(kind="stable")``), and the pre-cull orders equal scores by ascending instance
+        index (its suppression keeps the higher index of two equal scores first, its score cut drops the lower index
+        first), where the host's default sorts leave these orders implementation-defined.  None (default): the host tracker."""
         max_tracking = max_tracking if max_tracks else False
         if max_tracking and tracker in ("simple", "flow"):          # :882-884
             tracker += "maxtracks"
+        if track_device is not None:
+            if tracker in ("flow", "flowmaxtracks"):
+                raise ValueError("track_device runs the simple and simplemaxtracks trackers; the flow trackers take of_device")
+            if kf_init_frame_count:
+                raise ValueError("track_device does not run the Kalman tracker")
         if tracker.lower() == "none":
             return cls(track_window=track_window, similarity_function=None, matching_function=None, candidate_maker=None)
         if tracker not in CANDIDATE_MAKERS:
@@ -666,6 +796,16 @@ class Tracker:
                           max_tracks=max_tracks, max_tracking=max_tracking, min_new_track_points=min_new_track_points,
                           robust_best_instance=robust, pre_cull_function=pre_cull, target_instance_count=target_instance_count)
         tracker_obj.post_connect_single_breaks = bool(post_connect_single_breaks)
+        if track_device is not None:
+            tracker_obj.track_device = track_device
+            tracker_obj.device_params = dict(
+                maker=DEVICE_MAKERS[tracker], similarity=DEVICE_SIMILARITIES[similarity], match=DEVICE_MATCHERS[match],
+                track_window=int(track_window), max_tracks=int(max_tracks or 0), max_tracking=int(bool(max_tracking)),
+                min_match_points=int(min_match_points), min_new_track_points=int(min_new_track_points), robust=float(robust),
+                cull_target=int(target_instance_count) if (target_instance_count and pre_cull_to_target) else 0,
+                cull_use_iou=int(bool(pre_cull_iou_threshold)), cull_iou_threshold=float(pre_cull_iou_threshold or 0.0),
+                oks_errors=None if oks_errors is None else np.asarray(oks_errors, np.float64).reshape(-1),
+                oks_score_weighting=int(bool(oks_score_weighting)), oks_normalization=DEVICE_OKS_NORMALIZATIONS[oks_normalization])
         if clean_instance_count:
             tracker_obj.cleaner = TrackCleaner(instance_count=int(clean_instance_count), iou_threshold=clean_iou_threshold)
         # Kalman filters on top of the regular tracker (:955-991; sleap_b200/nn/kalman.py)
@@ -686,10 +826,27 @@ class Tracker:
         return tracker_obj
 
 
-def run_tracker(frames: list, tracker: Tracker, images=None) -> list:
+def run_tracker(frames: list, tracker: Tracker, images=None, device_chunk: int = 256) -> list:
     """Track the predicted instances of ``frames`` (sorted by frame index) in place (tracking.py:1542-1580).
-    ``images``: ``frame_idx -> image`` (mapping or callable), needed by the flow trackers."""
+    ``images``: ``frame_idx -> image`` (mapping or callable), needed by the flow trackers.  A tracker with
+    ``track_device`` tracks ``device_chunk`` frames per kernel call."""
     frames = sorted(frames, key=lambda lf: lf.frame_idx)
+    if tracker.track_device is not None and tracker.candidate_maker is not None:
+        for s in range(0, len(frames), device_chunk):
+            chunk = frames[s:s + device_chunk]
+            hws = []
+            for lf in chunk:
+                img = None
+                if images is not None:
+                    img = images(lf.frame_idx) if callable(images) else images[lf.frame_idx]
+                hws.append(tuple(np.asarray(img).shape[:2]) if img is not None else (1, 1))
+            out, err = tracker.track_frames([list(lf.instances) for lf in chunk], [lf.frame_idx for lf in chunk], hws)
+            for lf, tracked in zip(chunk, out):
+                lf.instances = tracked
+            if err is not None:
+                raise err
+        tracker.final_pass(frames)
+        return frames
     for lf in frames:
         img = None
         if images is not None:

@@ -13,6 +13,10 @@ first 500 frames of the tracking clip (tests/golden/tracks, 1024x1024, two flies
 with save_shifted_instances and flowmaxtracks (max_tracks 2).  End to end: BottomUpPredictor.predict (labels made) of
 the C4 network on 256 clip frames with no tracker, the cv2 flow tracker and the device flow tracker; the heads are
 calibrated as bench.py does (~5 detections per channel), so the tracker shifts ~65 points per reference frame.
+The device tracker (track_device=0) against the host tracker: tracker only (run_tracker, 256 frames per kernel call)
+for simple / instance / greedy and simplemaxtracks / centroid / hungarian on the clip predictions (300 frames) and on a
+seeded synthetic set of up to 6 instances x 13 nodes (300 frames); end to end, the same predict with no tracker, the
+host simple tracker and the device simple tracker (k_track inside the step).
 """
 import json
 import os
@@ -227,6 +231,39 @@ def track_bench():
         e2e[name] = n_e2e / (time.perf_counter() - t0)
         e2e[f"{name} instances/frame"] = float(np.mean([len(lf.instances) for lf in labeled]))
     out["predict_c4_frames_per_s"] = e2e
+
+    # device tracker vs host tracker
+    from track_cases import synthetic_frames
+    sets = {"clip": lambda: clip_labeled_frames(300), "synthetic 6x13": lambda: synthetic_frames(7, 300, 6, 13, all_nan=0.0)}
+    configs = {"simple/instance/greedy": dict(tracker="simple", similarity="instance", match="greedy"),
+               "simplemaxtracks/centroid/hungarian": dict(tracker="simplemaxtracks", similarity="centroid", match="hungarian",
+                                                          max_tracks=6, max_tracking=True)}
+    only = {}
+    for sname, make_set in sets.items():
+        for cname, kw in configs.items():
+            for where in ("host", "device"):
+                dev = 0 if where == "device" else None
+                T.run_tracker(make_set()[:20], T.Tracker.make_tracker_by_name(track_device=dev, **kw))     # warm-up
+                frames = make_set()
+                tr = T.Tracker.make_tracker_by_name(track_device=dev, **kw)
+                t0 = time.perf_counter()
+                T.run_tracker(frames, tr)
+                only[f"{sname} {cname} {where}"] = len(frames) / (time.perf_counter() - t0)
+    out["device_tracker_only_frames_per_s"] = only
+    e2e = {}
+    for name, dev in (("no tracker", None), ("simple host", None), ("simple device", 0)):
+        pred = BottomUpPredictor(model, bench.NODES, bench.EDGES, peak_threshold=0.2, batch_size=8, integral_refinement=True,
+                                 max_peaks_per_sample=1024, max_node_peaks=32, max_instances_per_frame=32)
+        mk = (lambda: None) if name == "no tracker" else \
+            (lambda: T.Tracker.make_tracker_by_name(tracker="simple", similarity="instance", match="greedy", track_device=dev))
+        pred.tracker = mk()
+        pred.predict(frames_e2e[:32])                                    # warm-up
+        pred.tracker = mk()
+        t0 = time.perf_counter()
+        labeled = pred.predict(frames_e2e)
+        e2e[name] = n_e2e / (time.perf_counter() - t0)
+        e2e[f"{name} tracks"] = len({id(i.track) for lf in labeled for i in lf.instances if i.track is not None})
+    out["predict_c4_simple_tracker_frames_per_s"] = e2e
     return out
 
 
