@@ -636,8 +636,7 @@ __global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(con
 // beyond C_in) with 16-byte cp.async into a ring of patch slots.  Every tap (ky, kx) of a block is then the same K-major
 // operand at start offset (ky * 18 + kx) * 16 bytes (LBO = one plane, SBO = one patch row): one load serves all nine taps.
 // The two consumer warpgroups take alternate items (ping-pong), so one warpgroup's epilogue overlaps the other's wgmma.
-// The epilogue runs from registers: a thread's two accumulator rows are vertically adjacent pixels, its horizontal pool
-// partner is lane ^ 4, and a 4x4 transpose across the lanes of a quad turns the channel pairs into 16-byte stores.  Every
+// The epilogue runs from registers (halo_block_epilogue): a thread's two accumulator rows are vertically adjacent pixels.  Every
 // output element gets the wgmma products of k_conv_wg -- the same m64nNk16 shape, (filter column, tap, k-step) order and
 // operand values -- and the bias / ReLU / fp16 rounding / 2x2 max of tc_epilogue_cols_fast in the same order, so the
 // outputs are bit-identical to forms 0 and 1.
@@ -664,6 +663,67 @@ __device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
   return *reinterpret_cast<const uint32_t*>(&m);
 }
 
+__device__ __forceinline__ float2 lds_f2(uint32_t saddr) {
+  float2 v;
+  asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
+  return v;
+}
+
+// Register epilogue of one 8x8-pixel block of the halo-patch forms (2 and 3): output channels [n0, n0 + N) of this thread's
+// two fragment rows, the vertically adjacent pixels (y, x) and (y + 1, x) of frame b (g = lane / 4, t = lane % 4; s_bias:
+// shared-memory address of channel n0's bias).  Bias, ReLU and fp16 rounding as in tc_epilogue_cols_fast, then the 2x2 max
+// on the rounded halves in the same order, max(max(h(y, x), h(y, x + 1)), max(h(y + 1, x), h(y + 1, x + 1))), on the
+// even-column lane, which stores (its horizontal partner is lane ^ 4).  A 4x4 transpose across the lanes of a quad turns
+// the channel pairs into 16-byte stores of 8 contiguous channels.
+template <int N>
+__device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const float (&acc)[N / 2], uint32_t s_bias, int n0, int b,
+                                                    int y, int x, int g, int t, float lo) {
+  constexpr int NJ = N / 8;                                    // 8-channel groups of the tile
+  // piece r * NJ + j = channels 8 j + 2 t (+ 1) of row r, as half2
+  uint32_t hv[2 * NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const float2 bb = lds_f2(s_bias + 4u * (8 * j + 2 * t));
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const __half2 h2 = __floats2half2_rn(fmaxf(acc[4 * j + 2 * r] + bb.x, lo), fmaxf(acc[4 * j + 2 * r + 1] + bb.y, lo));
+      hv[r * NJ + j] = *reinterpret_cast<const uint32_t*>(&h2);
+    }
+  }
+  if (P.pool_out != nullptr) {
+    constexpr int NJ4 = (NJ + 3) / 4 * 4;
+    uint32_t pv[NJ4];
+#pragma unroll
+    for (int j = 0; j < NJ4; ++j) {
+      if (j < NJ) {
+        const uint32_t m0 = hmax2_u32(hv[j], __shfl_xor_sync(0xffffffffu, hv[j], 4));
+        const uint32_t m1 = hmax2_u32(hv[NJ + j], __shfl_xor_sync(0xffffffffu, hv[NJ + j], 4));
+        pv[j] = hmax2_u32(m0, m1);
+      } else {
+        pv[j] = 0u;
+      }
+    }
+    __half* pp = reinterpret_cast<__half*>(P.pool_out) + (((size_t)b * P.pool_H + (y >> 1)) * P.pool_W + (x >> 1)) * P.pool_Ctot +
+                 P.pool_coff + n0;
+    const bool st = (g & 1) == 0 && y < P.H && x < P.W;
+#pragma unroll
+    for (int c0 = 0; c0 < NJ4; c0 += 4) {
+      quad_transpose(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3], t);
+      if (st && c0 + t < NJ) *reinterpret_cast<uint4*>(pp + 8 * (c0 + t)) = make_uint4(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3]);
+    }
+  }
+  if (!P.skip_out) {
+    __half* po = reinterpret_cast<__half*>(P.out) + (((size_t)b * P.out_H + y) * P.out_W + x) * P.out_Ctot + P.out_coff + n0;
+#pragma unroll
+    for (int c0 = 0; c0 < 2 * NJ; c0 += 4) {
+      quad_transpose(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3], t);
+      const int c = c0 + t, r = c / NJ, j = c % NJ;
+      if (y + r < P.H && x < P.W)
+        *reinterpret_cast<uint4*>(po + (size_t)r * P.out_W * P.out_Ctot + 8 * j) = make_uint4(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3]);
+    }
+  }
+}
+
 template <int KSTEPS, int N>
 __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_constant__ CUtensorMap mapA,
                                                                const __grid_constant__ CUtensorMap mapB,
@@ -671,7 +731,6 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
   constexpr int BY = halo_by(N, 16 * KSTEPS), NB = 2 * BY;                  // blocks per item: 2 along x, BY along y
   constexpr int NP = 2 * KSTEPS;                               // 8-channel planes of the chunk
   constexpr int PH = 8 * BY + 2, PW = kHaloCols, PLANE = halo_plane(N, 16 * KSTEPS), SLOT = NP * PLANE;
-  constexpr int NJ = N / 8;                                    // 8-channel groups of the output
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* bank = base;                                        // 9 weight slices, swizzled as in k_conv_wg_p
@@ -679,10 +738,12 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
   uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)P.n_a_slots * SLOT);
   uint64_t* empty = full + P.n_a_slots;
   uint64_t* fullB = empty + P.n_a_slots;
+  float* s_bias = reinterpret_cast<float*>(fullB + 1);          // [N]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_x = (P.W + 15) / 16, n_tiles = tiles_x * ((P.H + 8 * BY - 1) / (8 * BY));
   const int n_work = n_tiles * P.batch;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) s_bias[i] = (P.bias && i < P.Cout) ? P.bias[i] : 0.f;
   if (threadIdx.x == 0) {
     // full: one cp.async arrival per producer lane; empty: one arrival per warp of the consuming warpgroup
     for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(full + i), 32); mbar_init(smem_u32(empty + i), 4); }
@@ -726,11 +787,6 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
 
   // ------------------------------ consumers: warpgroup wg takes the CTA's items wg, wg + 2, ... ------------------------------
   const int wg = warp >> 2, q = warp & 3, g = lane >> 2, t = lane & 3;
-  float bias[NJ][2];                                           // channels 8 j + 2 t (+ 1) of this thread's fragment columns
-#pragma unroll
-  for (int j = 0; j < NJ; ++j)
-#pragma unroll
-    for (int e = 0; e < 2; ++e) bias[j][e] = P.bias ? P.bias[8 * j + 2 * t + e] : 0.f;
   const float lo = P.relu ? 0.f : -INFINITY;
   const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
   const uint64_t desc_b = make_desc(0, P.row_bytes, P.layout_type);
@@ -770,52 +826,171 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
     const int tile = w % n_tiles, b = w / n_tiles;
     const int x0 = (tile % tiles_x) * 16, y0 = (tile / tiles_x) * (8 * BY);
 #pragma unroll
-    for (int bk = 0; bk < NB; ++bk) {
-      // this thread's pixels: (y, x) and (y + 1, x); piece r * NJ + j = channels 8 j + 2 t (+ 1) of row r, as half2
-      const int y = y0 + 8 * (bk >> 1) + 2 * q, x = x0 + 8 * (bk & 1) + g;
-      uint32_t hv[2 * NJ];
-#pragma unroll
-      for (int j = 0; j < NJ; ++j)
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const __half2 h2 = __floats2half2_rn(fmaxf(acc[bk][4 * j + 2 * r] + bias[j][0], lo), fmaxf(acc[bk][4 * j + 2 * r + 1] + bias[j][1], lo));
-          hv[r * NJ + j] = *reinterpret_cast<const uint32_t*>(&h2);
-        }
-      if (P.pool_out != nullptr) {
-        // 2x2 max on the rounded halves in tc_epilogue_cols_fast's order: max(max(h(y, x), h(y, x + 1)), max(h(y + 1, x),
-        // h(y + 1, x + 1))) on the even-column lane, which stores
-        constexpr int NJ4 = (NJ + 3) / 4 * 4;
-        uint32_t pv[NJ4];
-#pragma unroll
-        for (int j = 0; j < NJ4; ++j) {
-          if (j < NJ) {
-            const uint32_t m0 = hmax2_u32(hv[j], __shfl_xor_sync(0xffffffffu, hv[j], 4));
-            const uint32_t m1 = hmax2_u32(hv[NJ + j], __shfl_xor_sync(0xffffffffu, hv[NJ + j], 4));
-            pv[j] = hmax2_u32(m0, m1);
-          } else {
-            pv[j] = 0u;
+    for (int bk = 0; bk < NB; ++bk)
+      halo_block_epilogue<N>(P, acc[bk], smem_u32(s_bias), 0, b, y0 + 8 * (bk >> 1) + 2 * q, x0 + 8 * (bk & 1) + g, g, t, lo);
+  }
+}
+
+// Wide form (form 3): persistent, warp-specialized, for the 3x3 stride-1 convs of the 64-512-channel layers, whose weight
+// banks do not fit in shared memory.  The streaming form re-reads every weight slice from L2 for each 128 output pixels;
+// here a work item is 16 x 8 BY output pixels x one N tile (N <= 128) x one frame, cut into 2 x BY blocks of 8x8 pixels,
+// and both consumer warpgroups (BY blocks each) read every weight slice, so one L2 read of a slice feeds 256 (N > 64) or
+// 512 (N <= 64) pixels.  K = 9 taps x C_in runs in chunks of 64 input channels (the last zero-filled beyond C_in).
+//   warpgroup 0 (registers cut to 56): warps 0, 2, 3 stage one halo patch per (item, chunk) in form 2's layout (8 non-swizzled
+//     8-channel planes [8 BY + 2][18][8], 16-byte cp.async, zero outside the image and beyond C_in) into a ring of patch
+//     slots; lane 0 of warp 1 streams the [N x 64] weight slices (SW128, TMA) in (chunk, filter column, tap) order into a
+//     ring of weight slots.  The weights never wait on the grid dependency, so the first ring is in flight while the
+//     predecessor drains.
+//   warpgroups 1, 2 (registers raised to 224): per weight slice, m64nNk16 wgmma over all k-steps and the warpgroup's
+//     blocks as one group; a slice's slot is released (one arrival per consumer warp, 8 in all) once the next slice's
+//     group is issued and its own has completed, a patch slot after the chunk's last slice.  Then the register epilogue of
+//     form 2 (halo_block_epilogue), for channels [n0, n0 + N).
+// Every output element gets the wgmma products of k_conv_wg -- the (chunk, filter column, tap, k-step) order on the same
+// operand values -- and form 2's epilogue arithmetic, so the outputs are bit-identical to forms 0, 1 and 2.
+// The CTA starts with 168 registers per thread (the cap for 384 threads); the consumers can only take what the producer
+// warpgroup gives back: 128 x (168 - 56) = 256 x (224 - 168).  (56 / 224 rather than 40 / 232: at 40 the patch loader spills.)
+constexpr int kWideThreads = 384;
+// threads of the producer warpgroup that stage patches (warps 0, 2 and 3; one warp alone issues the ~2600 16-byte
+// copies of a 64-channel patch too slowly to keep up with the MMAs)
+constexpr int kWidePatchLoaders = 96;
+constexpr int wide_by(int n) { return n <= 64 ? 4 : 2; }       // 8x8 block rows per item: 128 accumulators per consumer thread
+constexpr int wide_plane(int n) { return (8 * wide_by(n) + 2) * kHaloCols * 16; }
+
+template <int N>
+__global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_constant__ CUtensorMap mapA,
+                                                                const __grid_constant__ CUtensorMap mapB,
+                                                                const __grid_constant__ TcParams P) {
+  constexpr int BY = wide_by(N), NP = 8, PH = 8 * BY + 2, PW = kHaloCols, PLANE = wide_plane(N), SLOT = NP * PLANE;
+  constexpr int WSLOT = N * 128;                               // one [N x 64-channel] weight slice
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* wring = base;                                       // n_b_slots weight slices (1024-aligned: SW128 atoms)
+  uint8_t* pring = wring + (size_t)P.n_b_slots * WSLOT;        // n_a_slots patches
+  uint64_t* pfull = reinterpret_cast<uint64_t*>(pring + (size_t)P.n_a_slots * SLOT);
+  uint64_t* pempty = pfull + P.n_a_slots;
+  uint64_t* wfull = pempty + P.n_a_slots;
+  uint64_t* wempty = wfull + P.n_b_slots;
+  float* s_bias = reinterpret_cast<float*>(wempty + P.n_b_slots);   // [Cout]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // work item w = (N tile fastest, pixel tile, frame): the N tiles of one pixel tile run side by side and share its patches in L2
+  const int tiles_x = (P.W + 15) / 16, n_pt = tiles_x * ((P.H + 8 * BY - 1) / (8 * BY));
+  const int n_nt = P.Cout / N, n_work = n_nt * n_pt * P.batch;
+  for (int i = threadIdx.x; i < P.Cout; i += blockDim.x) s_bias[i] = P.bias ? P.bias[i] : 0.f;
+  if (threadIdx.x == 0) {
+    // full: one cp.async arrival per patch loader thread / one TMA transaction; empty: one arrival per consumer warp
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(pfull + i), kWidePatchLoaders); mbar_init(smem_u32(pempty + i), 8); }
+    for (int i = 0; i < P.n_b_slots; ++i) { mbar_init(smem_u32(wfull + i), 1); mbar_init(smem_u32(wempty + i), 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ------------------------------ producer warpgroup ------------------------------
+    setmaxnreg_dec<56>();
+    if (warp != 1) {
+      griddep_wait();                                          // activations come from the previous kernel of the stream
+      const __half* in = reinterpret_cast<const __half*>(P.in);
+      const int pid = (warp == 0 ? 0 : 32 * (warp - 1)) + lane;   // patch loader thread 0..95 (warps 0, 2, 3)
+      for (int i = 0, w = blockIdx.x; w < n_work; w += gridDim.x) {
+        if (w + (int)gridDim.x >= n_work) griddep_launch();    // last item of this CTA
+        const int pt = (w / n_nt) % n_pt, b = w / (n_nt * n_pt);
+        const int xs = (pt % tiles_x) * 16 - 1, ys = (pt / tiles_x) * (8 * BY) - 1;
+        for (int ch = 0; ch < P.n_chunks; ++ch, ++i) {
+          const int s = i % P.n_a_slots;
+          mbar_wait(smem_u32(pempty + s), ((i / P.n_a_slots) & 1) ^ 1);
+          // loader thread = (patch pixel % 12, plane): a warp instruction reads four whole 128-byte pixel runs
+          const int pl = pid & 7, c = ch * 64 + pl * 8;
+          const bool c_ok = c < P.in_C;
+          const __half* in_c = in + (size_t)b * P.H * P.W * P.in_Ctot + c;
+          const uint32_t dst = smem_u32(pring + (size_t)s * SLOT) + (uint32_t)(pl * PLANE);
+          for (int p = pid >> 3; p < PH * PW; p += kWidePatchLoaders / 8) {
+            const int y = ys + p / PW, x = xs + p % PW;
+            const bool ok = c_ok && y >= 0 && y < P.H && x >= 0 && x < P.W;
+            const __half* src = ok ? in_c + ((size_t)y * P.W + x) * P.in_Ctot : in;
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(p * 16)), "l"(src), "r"(ok ? 16 : 0)
+                         : "memory");
           }
-        }
-        __half* pp = reinterpret_cast<__half*>(P.pool_out) + (((size_t)b * P.pool_H + (y >> 1)) * P.pool_W + (x >> 1)) * P.pool_Ctot +
-                     P.pool_coff;
-        const bool st = (g & 1) == 0 && y < P.H && x < P.W;
-#pragma unroll
-        for (int c0 = 0; c0 < NJ4; c0 += 4) {
-          quad_transpose(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3], t);
-          if (st && c0 + t < NJ) *reinterpret_cast<uint4*>(pp + 8 * (c0 + t)) = make_uint4(pv[c0], pv[c0 + 1], pv[c0 + 2], pv[c0 + 3]);
+          asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(pfull + s)) : "memory");
         }
       }
-      if (!P.skip_out) {
-        __half* po = reinterpret_cast<__half*>(P.out) + (((size_t)b * P.out_H + y) * P.out_W + x) * P.out_Ctot + P.out_coff;
-#pragma unroll
-        for (int c0 = 0; c0 < 2 * NJ; c0 += 4) {
-          quad_transpose(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3], t);
-          const int c = c0 + t, r = c / NJ, j = c % NJ;
-          if (y + r < P.H && x < P.W)
-            *reinterpret_cast<uint4*>(po + (size_t)r * P.out_W * P.out_Ctot + 8 * j) = make_uint4(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3]);
-        }
+      asm volatile("cp.async.wait_all;" ::: "memory");
+    } else if (warp == 1 && lane == 0) {
+      // weights are static: no grid-dependency wait
+      for (int j = 0, w = blockIdx.x; w < n_work; w += gridDim.x) {
+        const int n0 = (w % n_nt) * N;
+        for (int ch = 0; ch < P.n_chunks; ++ch)
+          for (int kx = 0; kx < 3; ++kx)
+            for (int ky = 0; ky < 3; ++ky, ++j) {
+              const int s = j % P.n_b_slots;
+              mbar_wait(smem_u32(wempty + s), ((j / P.n_b_slots) & 1) ^ 1);
+              mbar_expect_tx(smem_u32(wfull + s), (uint32_t)WSLOT);
+              tma_load_3d(smem_u32(wring + (size_t)s * WSLOT), &mapB, smem_u32(wfull + s), ch * 64, n0, ky * 3 + kx);
+            }
       }
     }
+    return;
+  }
+
+  // ------------------------------ consumers: warpgroup cw multiplies block rows [cw BY / 2, (cw + 1) BY / 2) ----------------
+  setmaxnreg_inc<224>();
+  const int cw = (warp >> 2) - 1, q = warp & 3, g = lane >> 2, t = lane & 3;
+  const float lo = P.relu ? 0.f : -INFINITY;
+  const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
+  const uint64_t desc_b = make_desc(0, 128, 1);
+  const uint32_t p_base = smem_u32(pring) + (uint32_t)(cw * (BY / 2) * 8 * PW * 16), w_base = smem_u32(wring);
+  float acc[BY][N / 2];
+  int ps = 0, ws = 0;
+  uint32_t pph = 0, wph = 0;
+  for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
+    int rel_w = -1, rel_p = -1;
+    for (int ch = 0; ch < P.n_chunks; ++ch) {
+      mbar_wait(smem_u32(pfull + ps), pph);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async writes (generic proxy) -> wgmma operand reads
+      const uint32_t a_base = p_base + (uint32_t)(ps * SLOT);
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+        for (int ky = 0; ky < 3; ++ky) {
+          mbar_wait(smem_u32(wfull + ws), wph);
+          const uint64_t db = desc_b + (uint64_t)((w_base + (uint32_t)(ws * WSLOT)) >> 4);
+          wgmma_fence();
+#pragma unroll
+          for (int i = 0; i < BY; ++i) wgmma_reg_fence(acc[i]);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int i = 0; i < BY; ++i) {
+              const uint32_t a = a_base + (uint32_t)(((8 * (i >> 1) + ky) * PW + 8 * (i & 1) + kx) * 16 + 2 * k * PLANE);
+              wgmma_f16<N>(acc[i], desc_a + (uint64_t)(a >> 4), db + 2 * k, (ch | kx | ky | k) ? 1u : 0u);
+            }
+          wgmma_commit();
+#pragma unroll
+          for (int i = 0; i < BY; ++i) wgmma_reg_fence(acc[i]);
+          wgmma_wait<1>();               // the previous slice's products are done: its slots may be refilled
+          __syncwarp();
+          if (lane == 0) {
+            if (rel_w >= 0) mbar_arrive(smem_u32(wempty + rel_w));
+            if (rel_p >= 0) mbar_arrive(smem_u32(pempty + rel_p));
+          }
+          rel_w = ws;
+          rel_p = (kx == 2 && ky == 2) ? ps : -1;
+          if (++ws == P.n_b_slots) { ws = 0; wph ^= 1; }
+        }
+      if (++ps == P.n_a_slots) { ps = 0; pph ^= 1; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < BY; ++i) wgmma_reg_fence(acc[i]);
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(smem_u32(wempty + rel_w)); mbar_arrive(smem_u32(pempty + rel_p)); }
+
+    const int n0 = (w % n_nt) * N, pt = (w / n_nt) % n_pt, b = w / (n_nt * n_pt);
+    const int x0 = (pt % tiles_x) * 16, y0 = (pt / tiles_x) * (8 * BY) + cw * (BY / 2) * 8;
+#pragma unroll
+    for (int i = 0; i < BY; ++i)
+      halo_block_epilogue<N>(P, acc[i], smem_u32(s_bias + n0), n0, b, y0 + 8 * (i >> 1) + 2 * q, x0 + 8 * (i & 1) + g, g, t, lo);
   }
 }
 
@@ -979,15 +1154,19 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
 }
 
 // Kernel forms of one launch: 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with
-// resident weights, 2 = the persistent halo-patch k_conv_wg_h.  All give bit-identical outputs; the autotuner keeps the
-// faster eligible one per launch (SB_FORCE_VARIANT=n forces form n where it is eligible).
-constexpr int kForms = 3;
+// resident weights, 2 = the persistent halo-patch k_conv_wg_h, 3 = the persistent halo-patch k_conv_wg_hw with streamed
+// weights and N tiles of at most 128.  All give bit-identical outputs; the autotuner keeps the fastest eligible one per
+// launch (SB_FORCE_VARIANT=n forces form n where it is eligible).
+constexpr int kForms = 4;
 struct TcForm {
   int ok;
-  int n_a_slots, n_b_slots;    // halo form: n_a_slots = patch slots
+  int n_a_slots, n_b_slots;    // halo forms: n_a_slots = patch slots
   size_t smem;
+  int threads;                 // CTA size
+  int N;                       // wgmma N of the form's tiles (form 3: at most 128; the others: the launch's P.N)
   int max_ctas;                // persistent forms: CTAs the GPU holds at once
   int n_tiles;                 // persistent forms: work items per frame
+  CUtensorMap mapB;            // form 3: weight map with a [64, N, 1] box (the others use TcLaunch::mapB)
 };
 
 struct TcLaunch {
@@ -1140,8 +1319,22 @@ static ConvKernel conv_kernel_h_n(int N) {
   }
 }
 
+// the wide instantiations: K chunks of 64 channels, N tiles 32..128; nullptr otherwise
+static ConvKernel conv_kernel_hw(int KC, int N) {
+  if (KC != 64) return nullptr;
+  switch (N) {
+    case 32: return k_conv_wg_hw<32>;
+    case 48: return k_conv_wg_hw<48>;
+    case 64: return k_conv_wg_hw<64>;
+    case 96: return k_conv_wg_hw<96>;
+    case 128: return k_conv_wg_hw<128>;
+    default: return nullptr;
+  }
+}
+
 static ConvKernel conv_kernel_form(int form, int KC, int N) {
   if (form == 0) return conv_kernel(KC, N);
+  if (form == 3) return conv_kernel_hw(KC, N);
   if (form == 2) return KC == 16 ? conv_kernel_h_n<1>(N) : (KC == 32 ? conv_kernel_h_n<2>(N) : conv_kernel_h_n<4>(N));
   return KC == 16 ? conv_kernel_p_n<1>(N) : (KC == 32 ? conv_kernel_p_n<2>(N) : conv_kernel_p_n<4>(N));
 }
@@ -1160,15 +1353,21 @@ static size_t conv_smem_resident(const TcParams& P, int n_a, int bank) {
 
 // shared memory of a k_conv_wg_h launch: weight bank (9 slices), n_a patch slots, 2 n_a + 1 barriers
 static size_t conv_smem_halo(const TcParams& P, int n_a) {
-  return 1024 /*align slack*/ + (size_t)9 * P.b_slot_bytes + (size_t)n_a * (P.KC / 8) * halo_plane(P.N, P.KC) + (size_t)(2 * n_a + 1) * 8;
+  return 1024 /*align slack*/ + (size_t)9 * P.b_slot_bytes + (size_t)n_a * (P.KC / 8) * halo_plane(P.N, P.KC) + (size_t)(2 * n_a + 1) * 8 +
+         (size_t)P.N * sizeof(float);
 }
 
-// The halo form takes plain 3x3 stride-1 SAME convs (filter column g = dx + 1, tap ky of it = weight tap 3 ky + g) with one
-// input-channel chunk and the fast-epilogue output shape without a residual.
-static bool halo_eligible(const TcLaunch& L) {
-  const TcParams& P = L.P;
-  if (L.grid.y != 1 || P.n_chunks != 1 || P.N > 64 || P.epi_mode != 1 || P.res != nullptr || P.n_groups != 3 || P.dy0 != -1 ||
-      P.box_rows != TH + 2 || P.oy_mul != 1 || P.oy_add != 0 || P.ox_mul != 1 || P.ox_add != 0)
+// shared memory of a k_conv_wg_hw launch with N tiles of n: n_b weight slots, n_a patch slots, 2 (n_a + n_b) barriers, the bias
+static size_t conv_smem_wide(const TcParams& P, int n, int n_a, int n_b) {
+  return 1024 /*align slack*/ + (size_t)n_b * n * 128 + (size_t)n_a * 8 * wide_plane(n) + (size_t)(2 * n_a + 2 * n_b) * 8 +
+         (size_t)P.Cout * sizeof(float);
+}
+
+// The halo forms take plain 3x3 stride-1 SAME convs (filter column g = dx + 1, tap ky of it = weight tap 3 ky + g) in the
+// fast-epilogue output shape without a residual.
+static bool halo_shape(const TcParams& P) {
+  if (P.epi_mode != 1 || P.res != nullptr || P.n_groups != 3 || P.dy0 != -1 || P.box_rows != TH + 2 || P.oy_mul != 1 ||
+      P.oy_add != 0 || P.ox_mul != 1 || P.ox_add != 0)
     return false;
   for (int g = 0; g < 3; ++g) {
     if (P.groups[g].dx != g - 1 || P.groups[g].n_taps != 3) return false;
@@ -1178,23 +1377,46 @@ static bool halo_eligible(const TcLaunch& L) {
   return true;
 }
 
+// form 2: one input-channel chunk and one N tile of at most 64 channels
+static bool halo_eligible(const TcLaunch& L) {
+  return L.grid.y == 1 && L.P.n_chunks == 1 && L.P.N <= 64 && halo_shape(L.P);
+}
+
+// form 3: chunks of 64 input channels, and N tiles of min(N, 128) channels that cover C_out exactly
+static int wide_n(const TcParams& P) { return std::min(P.N, 128); }
+static bool wide_eligible(const TcLaunch& L) {
+  return L.P.KC == 64 && L.P.Cout % wide_n(L.P) == 0 && halo_shape(L.P);
+}
+
 // Eligibility, ring sizes, shared memory and co-resident grid size of the persistent forms of launch L (forms[0], the
 // streaming form, is always eligible).  Resident form: one N tile, and the whole bank of the launch's weight slices plus
 // at least 2 activation slots fit in 225 KB; two CTAs per SM where they fit in 113 KB.  Halo form: halo_eligible, and the
-// bank plus at least 4 patch slots (two being read, two prefetched) fit in 225 KB; up to 8 slots, one CTA per SM.
+// bank plus at least 4 patch slots (two being read, two prefetched) fit in 225 KB; up to 8 slots, one CTA per SM.  Wide
+// form: wide_eligible, 2 patch slots and 4-8 weight slots in 225 KB, one CTA per SM.
 static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
   TcParams& P = L.P;
   L.form = 0;
   L.forms[0].ok = 1; L.forms[0].n_a_slots = P.n_a_slots; L.forms[0].n_b_slots = P.n_b_slots; L.forms[0].smem = L.smem;
+  for (int f = 0; f < kForms; ++f) { L.forms[f].threads = kConvThreads; L.forms[f].N = P.N; }
   auto fit = [&](TcForm& F, ConvKernel kern) {               // co-resident CTAs of an eligible form
     int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kConvThreads, F.smem) != cudaSuccess || nb < 1) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, F.threads, F.smem) != cudaSuccess || nb < 1) {
       cudaGetLastError();
       F.ok = 0;
       return;
     }
     F.max_ctas = nb * h->sm_count;
   };
+  if (ConvKernel kern = conv_kernel_form(3, P.KC, wide_n(P)); kern && wide_eligible(L)) {
+    TcForm& F = L.forms[3];
+    F.threads = kWideThreads;
+    F.N = wide_n(P);
+    for (int nb = 8; nb >= 4 && !F.ok; --nb)
+      if (conv_smem_wide(P, F.N, 2, nb) <= kMaxDynSmem) { F.ok = 1; F.n_a_slots = 2; F.n_b_slots = nb; F.smem = conv_smem_wide(P, F.N, 2, nb); }
+    const int by = wide_by(F.N);
+    F.n_tiles = (P.Cout / F.N) * ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
+    if (F.ok) fit(F, kern);
+  }
   if (ConvKernel kern = conv_kernel_form(2, P.KC, P.N); kern && halo_eligible(L)) {
     TcForm& F = L.forms[2];
     for (int na = 8; na >= 4 && !F.ok; --na)
@@ -1315,18 +1537,21 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
   }
-  {
+  // B: [tap][Cout_pad][Cin] weights, box [KC, box_n, 1]
+  auto encode_b = [&](CUtensorMap* map, int box_n) {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)plan->Cout_pad, (cuuint64_t)n_wtaps};
     cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)plan->Cout_pad * Cin * 2};
-    cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)N, 1};
+    cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)box_n, 1};
     cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&L.mapB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
-  }
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  };
+  if (CUresult r = encode_b(&L.mapB, N); r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   P.n_tiles = (int)L.grid.x;
   setup_forms(h, L, total_steps);
+  if (L.forms[3].ok)
+    if (CUresult r = encode_b(&L.forms[3].mapB, L.forms[3].N); r != CUDA_SUCCESS)
+      return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, wide form) failed: %d", (int)r);
   (dst ? *dst : plan->launches).push_back(L);
   return 0;
 }
@@ -1776,15 +2001,15 @@ static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
     // persistent: as many CTAs as fit at once (capped at the work count), no shared-memory padding; each CTA triggers its
     // dependents when it starts its last work item
     const TcForm& F = L.forms[L.form];
-    P.n_a_slots = F.n_a_slots; P.n_b_slots = F.n_b_slots; P.batch = B; P.pdl_trigger = 0;
+    P.n_a_slots = F.n_a_slots; P.n_b_slots = F.n_b_slots; P.batch = B; P.pdl_trigger = 0; P.N = F.N;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(std::min(F.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = F.smem;
+    cfg.gridDim = dim3(std::min(F.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(F.threads); cfg.dynamicSmemBytes = F.smem;
     cfg.stream = stream;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, conv_kernel_form(L.form, P.KC, P.N), L.mapA, L.mapB, P);
+    cudaLaunchKernelEx(&cfg, conv_kernel_form(L.form, P.KC, P.N), L.mapA, L.form == 3 ? F.mapB : L.mapB, P);
     return;
   }
   size_t smem = L.smem;
@@ -1812,7 +2037,7 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   const bool dbg = getenv("SB_DEBUG") != nullptr;
   const char* fvar = getenv("SB_FORCE_VARIANT");
   const int force = fvar ? atoi(fvar) : -1;
-  static const char* const form_name[kForms] = {"streaming", "resident", "halo"};
+  static const char* const form_name[kForms] = {"streaming", "resident", "halo", "wide"};
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
     if (!plan || head_kernel_ok(m, m->ops[oi], plan)) continue;

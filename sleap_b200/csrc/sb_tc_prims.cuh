@@ -168,6 +168,13 @@ __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t a_desc,
       : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
 }
 
+// Warp-specialized register split: every warp of a warpgroup executes these together.  dec releases registers of the
+// calling warpgroup down to R per thread, inc blocks until R per thread are free (R a multiple of 8 in [24, 256]).
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // 32-byte global store of 16 halves (two 16-byte stores; the destination is 32-byte aligned)
 __device__ __forceinline__ void st_global_256(void* p, const __half2 (&h)[8]) {
   reinterpret_cast<uint4*>(p)[0] = *reinterpret_cast<const uint4*>(&h[0]);

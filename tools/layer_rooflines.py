@@ -6,9 +6,10 @@ Floors: tensor = algorithmic FLOPs / 989 TFLOP/s (H100 SXM data sheet, dense fp1
 HBM = (activations in + out (+ fused pool output) at their storage width) / 3.35 TB/s (H100 SXM data sheet).
 `MEASURED_PEAKS.json` at the repository root (`bf16_tflops`, `hbm_gbs`), when present, replaces both figures, as in
 bench.py.  The bound of a layer is the larger floor.
-L2 column (3x3 convs and k3 transposed convs only): the bytes the streaming form of k_conv_wg pulls from L2 into the SMs
+L2 columns (3x3 convs and k3 transposed convs only): the bytes the streaming form of k_conv_wg pulls from L2 into the SMs
 (every 128-pixel CTA loads its activation boxes and its whole weight slice), and, given an L2 read rate in TB/s
-(`tools/bw_probe.py`, "L2-resident"), the time that traffic takes at that rate.
+(`tools/bw_probe.py`, "L2-resident"), the time that traffic takes at that rate; then the same for the wide form
+k_conv_wg_hw where it is eligible.
 """
 import json
 import os
@@ -79,15 +80,34 @@ def l2_bytes_streaming(cin, cout, hin, taps):
     return B * tiles * n_tiles * chunks * (rows * 16 * kc * 2 + slices * n * kc * 2)
 
 
+def l2_bytes_wide(cin, cout, hin, taps):
+    """The same for the wide form k_conv_wg_hw (3x3 convs with C_in > 32; None: not eligible): per item (16 x 8 by pixels,
+    one N tile of n <= 128 channels) and 64-channel chunk, one (8 by + 2) x 18-pixel halo patch and 9 weight slices."""
+    if taps != 9 or cin <= 32:
+        return None
+    n = min(_wg_n(-(-cout // 16) * 16), 128)
+    if cout % n:
+        return None
+    by = 4 if n <= 64 else 2
+    items = -(-hin // 16) * -(-hin // (8 * by))
+    return B * items * (cout // n) * -(-cin // 64) * ((8 * by + 2) * 18 * 64 * 2 + 9 * n * 64 * 2)
+
+
 def main(src, out, l2_tbs=None):
     ms = {}
     for line in open(src):
         m = re.match(r"\[op\s*(\d+)\] kind=\d+\s+([\d.]+) us", line)
         if m:
             ms[int(m.group(1))] = float(m.group(2))
-    rows = ["| op | layer | measured us | GFLOP | tensor floor us | bytes MB | HBM floor us | bound | floor / measured | L2 GB (streaming) | L2 us |",
-            "|---|---|---|---|---|---|---|---|---|---|---|"]
+    rows = ["| op | layer | measured us | GFLOP | tensor floor us | bytes MB | HBM floor us | bound | floor / measured | L2 GB (streaming) | L2 us "
+            "| L2 GB (wide) | L2 us (wide) |",
+            "|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
     tot_m = tot_f = tot_l2 = 0.0
+
+    def l2_cols(b):
+        if b is None:
+            return "| | |"
+        return f"| {b / 1e9:.2f} | " + (f"{b / (l2_tbs * 1e12) * 1e6:.1f} |" if l2_tbs else "|")
     layers = list(LAYERS)
     if ms.get(2, 1e9) < 10.0:        # fused first block (k_conv01): op 1 holds both convs + the pool, op 2 is an empty slot
         flops = sum(2.0 * 9 * ci * co * 1024 * 1024 * B for ci, co in ((1, 16), (16, 16)))
@@ -99,7 +119,7 @@ def main(src, out, l2_tbs=None):
         tot_m += meas
         tot_f += floor
         rows.append(f"| 1+2 | fused first block 1->16->16 + pool (k_conv01) @1024² | {meas:.1f} | {flops / 1e9:.2f} | {t_tensor:.1f} | {byts / 1e6:.1f} | "
-                    f"{t_hbm:.1f} | {'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} | | |")
+                    f"{t_hbm:.1f} | {'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} | | | | |")
         layers = [l for l in layers if l[0] not in (1, 2)]
     for op, name, cin, cout, hin, hout, taps, pool, ob in layers:
         flops = 2.0 * taps * cin * cout * hout * hout * B
@@ -113,11 +133,10 @@ def main(src, out, l2_tbs=None):
         tot_f += floor
         l2b = None if op == 1 else l2_bytes_streaming(cin, cout, hin, taps)
         tot_l2 += l2b or 0.0
-        l2_cols = "| |" if l2b is None else f"| {l2b / 1e9:.2f} | " + (f"{l2b / (l2_tbs * 1e12) * 1e6:.1f} |" if l2_tbs else "|")
         rows.append(f"| {op} | {name} @{hin}² | {meas:.1f} | {flops / 1e9:.2f} | {t_tensor:.1f} | {(in_b + out_b) / 1e6:.1f} | {t_hbm:.1f} | "
-                    f"{'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} " + l2_cols)
+                    f"{'tensor' if t_tensor >= t_hbm else 'HBM'} | {floor / meas:.2f} " + l2_cols(l2b) + l2_cols(l2_bytes_wide(cin, cout, hin, taps))[1:])
     rows.append(f"| | **all conv layers** | **{tot_m:.1f}** | | | | | | **{tot_f / tot_m:.2f}** (sum of floors {tot_f:.1f} us) | "
-                f"**{tot_l2 / 1e9:.2f}** | " + (f"**{tot_l2 / (l2_tbs * 1e12) * 1e6:.1f}** |" if l2_tbs else "|"))
+                f"**{tot_l2 / 1e9:.2f}** | " + (f"**{tot_l2 / (l2_tbs * 1e12) * 1e6:.1f}** |" if l2_tbs else "|") + " | |")
     text = ("# C4 per-layer floors vs measured (8 frames, one H100)\n\nMeasured: CUDA-event per-op times of `bench.py` (`sb_model_profile_ops`), file `" + src +
             f"`.  Floors: {PEAK_TF:.0f} TFLOP/s and {PEAK_TBS:.2f} TB/s ({PEAK_SRC}); see tools/layer_rooflines.py.\n\n" + "\n".join(rows) + "\n")
     open(out, "w").write(text)
