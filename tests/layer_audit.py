@@ -14,6 +14,9 @@ Operands are the ones each kernel actually uses (``sb_model_profile_ops`` kind 1
 Precision 2 works on the physical ``[lo | hi | hi]`` layout: records carry physical input channels, the blob holds the
 expanded ``[Wh | Wl | Wh]`` rows, a producer's slice is decoded as lo + hi (planes ``out_C`` apart) and its layout
 invariants are asserted exactly.
+Precision 1 (the fp32 CUDA-core path) keeps every buffer in fp32 and runs every conv on ``k_conv_direct`` /
+``k_tconv_direct`` with the fp32 blob: no first-conv fusion, no tensor-core plan, so no fused pool or ADD either.  Its
+elementwise ops have their own bounds (``elementwise_bound``).
 """
 import math
 
@@ -68,6 +71,29 @@ def elem_bound(A, mag, n_steps, prop=0.0, bn_scale=None, bn_mag=None):
     if bn_scale is not None:
         e = np.abs(bn_scale) * e + 2.0 * 2.0 ** -24 * bn_mag
     return e
+
+
+def elementwise_bound(kind, ref, x=None):
+    """(e_pre, store kind) of an elementwise op of the fp32 path (k_maxpool2 / k_maxpool3s2 / k_upsample2 / k_add with
+    T = float, sb_kernels_direct.cuh) whose float64 reference from the fp32 device inputs is ``ref``.  u = 2^-24, one
+    fp32 rounding.
+      * pool, pool3s2, nearest: the output is one of the inputs (fmaxf, a copy): exact, no store rounding;
+      * add: v = a + b, one rounding of |a + b| (the 'f32' store term); a ReLU after it keeps the sign, so is exact;
+      * bilinear: per axis lerp t = l + (r - l) w with w in {1/4, 3/4} (0 where the edge clamp makes l = r).  With M the
+        largest |corner|: r - l rounds (<= u 2M), (r - l) w rounds (<= u 3/4 2M; exact for w = 1/4), the add rounds
+        (<= u M), so each of tp, bt is within 2u M + 3/4 2u M + u M < 4u M; the outer lerp carries that (weights 1 - w, w)
+        and adds 3/4 2u M + 3/4 2u M + u M = 4u M.  So e_pre = 8u M = 2^-21 M, which already holds the final add's
+        rounding; the 'f32' store term on top absorbs the second-order terms.  nvcc may contract (r - l) w + l into one
+        FMA, which drops a rounding.
+    ``x`` is the bilinear upsample's input map (M is taken over its 3 x 3 neighbourhood, which holds all four corners)."""
+    if kind in ("pool", "pool3s2", "nearest"):
+        return np.zeros_like(ref), "exact"
+    if kind == "add":
+        return np.zeros_like(ref), "f32"
+    m = np.abs(x)
+    m = np.maximum(np.maximum(m, np.roll(m, 1, 1)), np.roll(m, -1, 1))
+    m = np.maximum(np.maximum(m, np.roll(m, 1, 2)), np.roll(m, -1, 2))
+    return 2.0 ** -21 * upsample64(m, False), "f32"
 
 
 def check(dev, ref, e_pre, out, lo=None):
@@ -233,12 +259,14 @@ class Audit:
     """One forward pass of a compiled op list.
 
     ``kinds[i]``: per-op kind of ``sb_model_profile_ops`` (1 tensor core, 2 CUDA core, 0 other); ``conv01``: the fused first
-    block ran (``SB_DEBUG`` line "-> fused").  ``precision`` 0 or 2."""
+    block ran (``SB_DEBUG`` line "-> fused").  ``precision`` 0, 1 or 2; in precision 1 every buffer is fp32
+    (``elem_size`` in sb_model.cu), so it is marked ``f32`` here whatever its record says."""
 
     def __init__(self, cm, blob, precision, frames, kinds, conv01=False):
         self.cm = cm
         recs = [np.asarray(r) for r in cm.records]
-        self.bufs = {int(r[1]): dict(stride=int(r[2]), C=int(r[3]), f32=bool(r[4])) for r in recs if r[0] == ol.BUFFER}
+        self.bufs = {int(r[1]): dict(stride=int(r[2]), C=int(r[3]), f32=bool(r[4]) or precision == 1)
+                     for r in recs if r[0] == ol.BUFFER}
         self.ops = [r for r in recs if r[0] != ol.BUFFER]
         self.blob = np.asarray(blob, np.float32)
         self.precision = precision
@@ -265,7 +293,7 @@ class Audit:
         return True
 
     def _first_fusion(self):
-        if self.pre_i + 1 >= len(self.ops):
+        if self.precision == 1 or self.pre_i + 1 >= len(self.ops):
             return -1
         pre, cv = self.ops[self.pre_i], self.ops[self.pre_i + 1]
         ib, ob = self.bufs[int(pre[6])], self.bufs[int(cv[6])]
@@ -293,9 +321,12 @@ class Audit:
         return ()
 
     def _pool_dead(self, i):
-        """CONV i feeds a fused 2x2 pool and nothing else reads its output slice."""
+        """CONV i runs on the tensor cores, feeds a fused 2x2 pool and nothing else reads its output slice (a CUDA-core
+        conv stores its output and the pool runs as its own kernel)."""
         o = self.ops[i]
         if o[0] != ol.CONV or o[18] < 0 or i + 1 >= len(self.ops) or self.ops[i + 1][0] != ol.POOL or not self.ops[i + 1][11] & ol.F_FUSED_POOL:
+            return False
+        if self.kinds[i] != 1:
             return False
         ext = (3 if self.split else 1) * int(o[8])
         for j, p in enumerate(self.ops):
@@ -481,23 +512,27 @@ class Audit:
                     continue
                 x = self.decode(dev[int(op[1])].astype(np.float64), int(op[2]), C)
                 ref = pool3s2(x) if op[9] == 3 else pool2(x)
-                rows.append(self._row(i, "pool3s2" if op[9] == 3 else "pool2", *self._slice(dev, ob, int(op[7]), C), ref,
-                                      self.decode_err(np.abs(ref)), self.out_kind(ob)))
+                e, ok = (self.decode_err(np.abs(ref)), self.out_kind(ob)) if self.precision != 1 else elementwise_bound("pool", ref)
+                rows.append(self._row(i, "pool3s2" if op[9] == 3 else "pool2", *self._slice(dev, ob, int(op[7]), C), ref, e, ok))
                 continue
             if kind == ol.UPSAMPLE:
                 C = int(op[3]) // (3 if self.split else 1)
                 x = self.decode(dev[int(op[1])].astype(np.float64), int(op[2]), C)
                 bil = bool(op[11] & ol.F_BILINEAR)
                 ref = upsample64(x, bil)
-                e = np.zeros_like(ref)
-                if bil:                    # three fp32 lerps: a few roundings of the largest of the four corners
-                    m = np.abs(x)
-                    m = np.maximum(np.maximum(m, np.roll(m, 1, 1)), np.roll(m, -1, 1))
-                    m = np.maximum(np.maximum(m, np.roll(m, 1, 2)), np.roll(m, -1, 2))
-                    e = 2.0 ** -21 * upsample64(m, False)
-                e = e + self.decode_err(upsample64(np.abs(x), False) if not bil else upsample64(m, False))
+                if self.precision == 1:
+                    e, ok = elementwise_bound("bilinear" if bil else "nearest", ref, x)
+                else:
+                    e = np.zeros_like(ref)
+                    if bil:                    # three fp32 lerps: a few roundings of the largest of the four corners
+                        m = np.abs(x)
+                        m = np.maximum(np.maximum(m, np.roll(m, 1, 1)), np.roll(m, -1, 1))
+                        m = np.maximum(np.maximum(m, np.roll(m, 1, 2)), np.roll(m, -1, 2))
+                        e = 2.0 ** -21 * upsample64(m, False)
+                    e = e + self.decode_err(upsample64(np.abs(x), False) if not bil else upsample64(m, False))
+                    ok = self.out_kind(ob)
                 rows.append(self._row(i, "upsample-" + ("bilinear" if bil else "nearest"), *self._slice(dev, ob, int(op[7]), C),
-                                      ref, e, self.out_kind(ob)))
+                                      ref, e, ok))
                 continue
             if kind == ol.ADD:
                 if production and i > 0 and self._res_fused(i - 1):
@@ -509,7 +544,10 @@ class Audit:
                 e = 2.0 ** -24 * (np.abs(a) + np.abs(b)) + self.decode_err(np.abs(a) + np.abs(b))
                 if op[11] & ol.F_RELU:
                     ref = np.maximum(ref, 0)
-                rows.append(self._row(i, "add", *self._slice(dev, ob, int(op[7]), C), ref, e, self.out_kind(ob)))
+                ok = self.out_kind(ob)
+                if self.precision == 1:
+                    e, ok = elementwise_bound("add", ref)
+                rows.append(self._row(i, "add", *self._slice(dev, ob, int(op[7]), C), ref, e, ok))
                 continue
             if kind == ol.COPY:
                 C = int(op[3])

@@ -71,14 +71,16 @@ def _gate(rows, label):
             assert abs(r["bias"]) <= BIAS_MAX, f"{tag}: mean signed error {r['bias']:.4f} ulp"
 
 
-def _audit(spec, in_ch, imgs, precision, capfd, monkeypatch, env=(), expect=None, all_buffers=True, input_scale=1.0, seed=5):
+def _audit(spec, in_ch, imgs, precision, capfd, monkeypatch, env=(), expect=None, all_buffers=True, input_scale=1.0, seed=5,
+           weights=None):
+    """``weights``: a weight dict (e.g. a trained model's); None = la.synthetic_weights(seed)."""
     from sleap_b200.nn import architectures as A
     from sleap_b200.nn.model import DeviceModel
     t0 = time.time()
     monkeypatch.setenv("SB_DEBUG", "1")
     for k, v in dict(env).items():
         monkeypatch.setenv(k, v)
-    w = la.synthetic_weights(A.compile_model(spec, in_ch, input_scale, split=precision == 2), seed)
+    w = weights if weights is not None else la.synthetic_weights(A.compile_model(spec, in_ch, input_scale, split=precision == 2), seed)
     model = DeviceModel(spec, w, input_channels=in_ch, input_scale=input_scale, precision=precision)
     B, H, W, C = imgs.shape
     capfd.readouterr()
