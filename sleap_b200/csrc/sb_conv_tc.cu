@@ -16,7 +16,8 @@
 //   D: two warpgroups, each m64nNk16 wgmma over 64 of the 128 pixels; epilogue through a shared-memory
 //     staging tile -> bias / ReLU / BN affine -> fp16 (or fp32 for head outputs) NHWC stores into the
 //     consumer's channel slice.
-//   Conv2DTranspose(k3 / k4, s2) = four sub-pixel phase GEMMs over the input grid with strided stores.
+//   Conv2DTranspose(k3 / k4, s2) = four sub-pixel phase GEMMs over the input grid with strided stores: four launches, or
+//     one persistent k_tconv_wg_hw launch over all four.
 //   1x1 stride-2 convs (ResNet) = 1x1 stride-1 convs over a subsampled view of the input: the A tensor map gets the
 //     output's H / W and doubled pixel / row pitches (TMA takes any 16-byte-multiple global strides).
 //   Residual blocks (ResNet, add skips): the epilogue adds the shortcut tensor after the bias and applies the ADD's
@@ -669,18 +670,12 @@ __device__ __forceinline__ float2 lds_f2(uint32_t saddr) {
   return v;
 }
 
-// Register epilogue of one 8x8-pixel block of the halo-patch forms (2 and 3): output channels [n0, n0 + N) of this thread's
-// two fragment rows, the vertically adjacent pixels (y, x) and (y + 1, x) of frame b (g = lane / 4, t = lane % 4; s_bias:
-// shared-memory address of channel n0's bias).  Bias, ReLU and fp16 rounding as in tc_epilogue_cols_fast, then the 2x2 max
-// on the rounded halves in the same order, max(max(h(y, x), h(y, x + 1)), max(h(y + 1, x), h(y + 1, x + 1))), on the
-// even-column lane, which stores (its horizontal partner is lane ^ 4).  A 4x4 transpose across the lanes of a quad turns
-// the channel pairs into 16-byte stores of 8 contiguous channels.
+// Bias, ReLU and fp16 rounding of a thread's two wgmma fragment rows (columns 8 j + 2 t (+ 1), t = lane % 4), as in
+// tc_epilogue_cols_fast: piece r * N / 8 + j of hv = channels 8 j + 2 t (+ 1) of row r, as half2 (s_bias: shared-memory
+// address of the bias of the tile's first channel).
 template <int N>
-__device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const float (&acc)[N / 2], uint32_t s_bias, int n0, int b,
-                                                    int y, int x, int g, int t, float lo) {
+__device__ __forceinline__ void frag_rows_f16(const float (&acc)[N / 2], uint32_t s_bias, int t, float lo, uint32_t (&hv)[N / 4]) {
   constexpr int NJ = N / 8;                                    // 8-channel groups of the tile
-  // piece r * NJ + j = channels 8 j + 2 t (+ 1) of row r, as half2
-  uint32_t hv[2 * NJ];
 #pragma unroll
   for (int j = 0; j < NJ; ++j) {
     const float2 bb = lds_f2(s_bias + 4u * (8 * j + 2 * t));
@@ -690,6 +685,32 @@ __device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const flo
       hv[r * NJ + j] = *reinterpret_cast<const uint32_t*>(&h2);
     }
   }
+}
+
+// Stores of frag_rows_f16's pieces: a 4x4 transpose across the lanes of a quad turns the channel pairs into 16-byte stores of
+// 8 contiguous channels; row r's channels [8 j, 8 j + 8) go to po + r * row_step + 8 j, where ok[r].
+template <int N>
+__device__ __forceinline__ void frag_rows_store(uint32_t (&hv)[N / 4], __half* po, size_t row_step, bool ok0, bool ok1, int t) {
+  constexpr int NJ = N / 8;
+#pragma unroll
+  for (int c0 = 0; c0 < 2 * NJ; c0 += 4) {
+    quad_transpose(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3], t);
+    const int c = c0 + t, r = c / NJ, j = c % NJ;
+    if (r ? ok1 : ok0) *reinterpret_cast<uint4*>(po + r * row_step + 8 * j) = make_uint4(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3]);
+  }
+}
+
+// Register epilogue of one 8x8-pixel block of the halo-patch forms (2 and 3): output channels [n0, n0 + N) of this thread's
+// two fragment rows, the vertically adjacent pixels (y, x) and (y + 1, x) of frame b (g = lane / 4, t = lane % 4; s_bias:
+// shared-memory address of channel n0's bias).  Bias, ReLU and fp16 rounding as in tc_epilogue_cols_fast, then the 2x2 max
+// on the rounded halves in the same order, max(max(h(y, x), h(y, x + 1)), max(h(y + 1, x), h(y + 1, x + 1))), on the
+// even-column lane, which stores (its horizontal partner is lane ^ 4).
+template <int N>
+__device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const float (&acc)[N / 2], uint32_t s_bias, int n0, int b,
+                                                    int y, int x, int g, int t, float lo) {
+  constexpr int NJ = N / 8;                                    // 8-channel groups of the tile
+  uint32_t hv[2 * NJ];
+  frag_rows_f16<N>(acc, s_bias, t, lo, hv);
   if (P.pool_out != nullptr) {
     constexpr int NJ4 = (NJ + 3) / 4 * 4;
     uint32_t pv[NJ4];
@@ -714,13 +735,7 @@ __device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const flo
   }
   if (!P.skip_out) {
     __half* po = reinterpret_cast<__half*>(P.out) + (((size_t)b * P.out_H + y) * P.out_W + x) * P.out_Ctot + P.out_coff + n0;
-#pragma unroll
-    for (int c0 = 0; c0 < 2 * NJ; c0 += 4) {
-      quad_transpose(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3], t);
-      const int c = c0 + t, r = c / NJ, j = c % NJ;
-      if (y + r < P.H && x < P.W)
-        *reinterpret_cast<uint4*>(po + (size_t)r * P.out_W * P.out_Ctot + 8 * j) = make_uint4(hv[c0], hv[c0 + 1], hv[c0 + 2], hv[c0 + 3]);
-    }
+    frag_rows_store<N>(hv, po, (size_t)P.out_W * P.out_Ctot, y < P.H && x < P.W, y + 1 < P.H && x < P.W, t);
   }
 }
 
@@ -994,6 +1009,182 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
   }
 }
 
+// Fused transposed-conv form (form 4): all four sub-pixel phases of one Conv2DTranspose (k3 or k4, stride 2) in a single
+// persistent, warp-specialized launch.  The phase launches of form 0 each run a short K (1-4 weight slices per 64-channel
+// chunk) over 128-pixel tiles and end in their own half-empty wave; here a work item is (phase, 16x16 input tile, N tile
+// of at most 128 channels, frame), and both consumer warpgroups read every weight slice, so one L2 read of a slice feeds
+// 256 pixels.  The phases keep their own filter columns and taps (the TcGroup lists of the four phase launches):
+//   warpgroup 0 (registers cut to 56): lane 0 of warp 0 loads, per (item, chunk, filter column), one [64 ch, 16 px, 17 rows]
+//     SW128 box by TMA -- exactly form 0's box with 8 more rows; the taps are whole-row start offsets inside it and TMA's
+//     zero fill is the padding -- into a ring of box slots; lane 0 of warp 1 streams the [N x 64] weight slices in
+//     (item, chunk, filter column, tap) order into a ring of weight slots, without waiting on the grid dependency.
+//   warpgroups 1, 2 (registers raised to 224): warpgroup cw multiplies tile rows [8 cw, 8 cw + 8) as two m64 blocks of
+//     4 x 16 pixels, one wgmma group per weight slice; slots are released as in k_conv_wg.  Then a register epilogue
+//     (frag_rows_f16 / frag_rows_store): a thread's two fragment rows are input pixels (y, x) and (y, x + 8), stored to
+//     output pixels (2 y + a, 2 x + b) and (2 y + a, 2 x + 16 + b) of phase (a, b).
+// Items are dealt in rounds of gridDim.x, alternately forward and backward; the list is cut into blocks of gridDim.x
+// (N tile, input tile, frame) units x 4 phases, phase-major with the heaviest phase first, so that the rounds even out
+// the phases' unequal costs and the four phases of one input tile read its boxes while they are still in L2.
+// Within each phase an output element gets form 0's products in form 0's order ((chunk, filter column, tap, k-step) on the
+// same operand values) and tc_epilogue_cols_fast's arithmetic, so the outputs are bit-identical to forms 0 and 1.
+constexpr int kTconvBoxRows = 17;                              // 16 input rows + the one-row halo of a dy0 = -1 phase
+constexpr int kTconvBox = kTconvBoxRows * 16 * 128;            // one [64 ch, 16 px, 17 rows] box: 34 KB, 1024-aligned
+struct TcPhases {                                              // the four phase launches' tap lists, (a, b) = (p / 2, p % 2)
+  int n_groups[4], dy0[4], oy_add[4], ox_add[4];
+  TcGroup groups[4][2];
+};
+
+// the item of round r of this CTA
+__device__ __forceinline__ int tconv_item(int r) {
+  const int G = gridDim.x;
+  return r * G + ((r & 1) ? G - 1 - (int)blockIdx.x : (int)blockIdx.x);
+}
+
+// item w -> (phase, unit); units are (N tile fastest, input tile, frame)
+__device__ __forceinline__ int2 tconv_decode(int w, int n_units) {
+  const int G = gridDim.x, blk = w / (4 * G), r = w - blk * 4 * G, s = min(G, n_units - blk * G);
+  return make_int2(r / s, blk * G + r % s);
+}
+
+template <int N>
+__global__ void __launch_bounds__(kWideThreads, 1) k_tconv_wg_hw(const __grid_constant__ CUtensorMap mapA,
+                                                                 const __grid_constant__ CUtensorMap mapB,
+                                                                 const __grid_constant__ TcParams P,
+                                                                 const __grid_constant__ TcPhases Q) {
+  constexpr int WSLOT = N * 128;                               // one [N x 64-channel] weight slice
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t* wring = base;                                       // n_b_slots weight slices (1024-aligned: SW128 atoms)
+  uint8_t* aring = wring + (size_t)P.n_b_slots * WSLOT;        // n_a_slots activation boxes
+  uint64_t* afull = reinterpret_cast<uint64_t*>(aring + (size_t)P.n_a_slots * kTconvBox);
+  uint64_t* aempty = afull + P.n_a_slots;
+  uint64_t* wfull = aempty + P.n_a_slots;
+  uint64_t* wempty = wfull + P.n_b_slots;
+  float* s_bias = reinterpret_cast<float*>(wempty + P.n_b_slots);   // [Cout]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_x = (P.W + 15) / 16, n_pt = tiles_x * ((P.H + 15) / 16);
+  const int n_nt = P.Cout / N, n_units = n_nt * n_pt * P.batch, n_work = 4 * n_units;
+  for (int i = threadIdx.x; i < P.Cout; i += blockDim.x) s_bias[i] = P.bias ? P.bias[i] : 0.f;
+  if (threadIdx.x == 0) {
+    // full: one TMA transaction; empty: one arrival per consumer warp
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(afull + i), 1); mbar_init(smem_u32(aempty + i), 8); }
+    for (int i = 0; i < P.n_b_slots; ++i) { mbar_init(smem_u32(wfull + i), 1); mbar_init(smem_u32(wempty + i), 8); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ------------------------------ producer warpgroup ------------------------------
+    setmaxnreg_dec<56>();
+    if (warp == 0 && lane == 0) {
+      griddep_wait();                                          // activations come from the previous kernel of the stream
+      int s = 0;
+      uint32_t ph = 0;
+      for (int r = 0, w = tconv_item(0); w < n_work; w = tconv_item(++r)) {
+        if (tconv_item(r + 1) >= n_work) griddep_launch();     // last item of this CTA
+        const int2 it = tconv_decode(w, n_units);
+        const int pt = (it.y / n_nt) % n_pt, b = it.y / (n_nt * n_pt);
+        const int x0 = (pt % tiles_x) * 16, y0 = (pt / tiles_x) * 16 + Q.dy0[it.x];
+        for (int ch = 0; ch < P.n_chunks; ++ch)
+          for (int g = 0; g < Q.n_groups[it.x]; ++g) {
+            mbar_wait(smem_u32(aempty + s), ph ^ 1);
+            mbar_expect_tx(smem_u32(afull + s), (uint32_t)kTconvBox);
+            tma_load_4d(smem_u32(aring + (size_t)s * kTconvBox), &mapA, smem_u32(afull + s), ch * 64, x0 + Q.groups[it.x][g].dx, y0, b);
+            if (++s == P.n_a_slots) { s = 0; ph ^= 1; }
+          }
+      }
+    } else if (warp == 1 && lane == 0) {
+      // weights are static: no grid-dependency wait
+      int s = 0;
+      uint32_t ph = 0;
+      for (int r = 0, w = tconv_item(0); w < n_work; w = tconv_item(++r)) {
+        const int2 it = tconv_decode(w, n_units);
+        const int n0 = (it.y % n_nt) * N;
+        for (int ch = 0; ch < P.n_chunks; ++ch)
+          for (int g = 0; g < Q.n_groups[it.x]; ++g)
+            for (int t = 0; t < Q.groups[it.x][g].n_taps; ++t) {
+              mbar_wait(smem_u32(wempty + s), ph ^ 1);
+              mbar_expect_tx(smem_u32(wfull + s), (uint32_t)WSLOT);
+              tma_load_3d(smem_u32(wring + (size_t)s * WSLOT), &mapB, smem_u32(wfull + s), ch * 64, n0, Q.groups[it.x][g].taps[t].w_tap);
+              if (++s == P.n_b_slots) { s = 0; ph ^= 1; }
+            }
+      }
+    }
+    return;
+  }
+
+  // ------------------------------ consumers: warpgroup cw multiplies tile rows [8 cw, 8 cw + 8) ------------------------------
+  setmaxnreg_inc<224>();
+  const int cw = (warp >> 2) - 1, q = warp & 3, g = lane >> 2, t = lane & 3;
+  const float lo = P.relu ? 0.f : -INFINITY;
+  const uint64_t desc = make_desc(0, 128, 1);
+  const uint32_t a_row0 = smem_u32(aring) + (uint32_t)(cw * 8 * 16 * 128), w_base = smem_u32(wring);
+  constexpr uint32_t kBlockStep = (4 * 16 * 128) >> 4;         // descriptor start-address step of one m64 block (4 rows)
+  float acc[2][N / 2];
+  int sa = 0, sb = 0;
+  uint32_t pha = 0, phb = 0;
+  for (int r = 0, w = tconv_item(0); w < n_work; w = tconv_item(++r)) {
+    const int2 it = tconv_decode(w, n_units);
+    const int ph = it.x;
+    int rel_a = -1, rel_b = -1;
+    uint32_t scale_d = 0;
+    for (int ch = 0; ch < P.n_chunks; ++ch) {
+      for (int gi = 0; gi < Q.n_groups[ph]; ++gi) {
+        mbar_wait(smem_u32(afull + sa), pha);
+        const uint32_t a_base = a_row0 + (uint32_t)(sa * kTconvBox);
+        const int n_taps = Q.groups[ph][gi].n_taps;
+        for (int tt = 0; tt < n_taps; ++tt) {
+          mbar_wait(smem_u32(wfull + sb), phb);
+          const uint64_t da = desc + (uint64_t)((a_base + (uint32_t)(Q.groups[ph][gi].taps[tt].row_off * 16 * 128)) >> 4);
+          const uint64_t db = desc + (uint64_t)((w_base + (uint32_t)(sb * WSLOT)) >> 4);
+          wgmma_fence();
+          wgmma_reg_fence(acc[0]);
+          wgmma_reg_fence(acc[1]);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) wgmma_f16<N>(acc[i], da + i * kBlockStep + 2 * k, db + 2 * k, scale_d);
+            scale_d = 1;
+          }
+          wgmma_commit();
+          wgmma_reg_fence(acc[0]);
+          wgmma_reg_fence(acc[1]);
+          wgmma_wait<1>();               // the previous slice's products are done: its slots may be refilled
+          __syncwarp();
+          if (lane == 0) {
+            if (rel_b >= 0) mbar_arrive(smem_u32(wempty + rel_b));
+            if (rel_a >= 0) mbar_arrive(smem_u32(aempty + rel_a));
+          }
+          rel_b = sb;
+          rel_a = tt == n_taps - 1 ? sa : -1;
+          if (++sb == P.n_b_slots) { sb = 0; phb ^= 1; }
+        }
+        if (++sa == P.n_a_slots) { sa = 0; pha ^= 1; }
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc[0]);
+    wgmma_reg_fence(acc[1]);
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(smem_u32(wempty + rel_b)); mbar_arrive(smem_u32(aempty + rel_a)); }
+
+    const int n0 = (it.y % n_nt) * N, pt = (it.y / n_nt) % n_pt, b = it.y / (n_nt * n_pt);
+    const int x = (pt % tiles_x) * 16 + g;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int y = (pt / tiles_x) * 16 + 8 * cw + 4 * i + q;
+      uint32_t hv[N / 4];
+      frag_rows_f16<N>(acc[i], smem_u32(s_bias + n0), t, lo, hv);
+      __half* po = reinterpret_cast<__half*>(P.out) +
+                   (((size_t)b * P.out_H + y * P.oy_mul + Q.oy_add[ph]) * P.out_W + x * P.ox_mul + Q.ox_add[ph]) * P.out_Ctot + P.out_coff + n0;
+      frag_rows_store<N>(hv, po, (size_t)8 * P.ox_mul * P.out_Ctot, y < P.H && x < P.W, y < P.H && x + 8 < P.W, t);
+    }
+  }
+}
+
 // ------------------------------- host side ---------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1156,7 +1347,8 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
 // Kernel forms of one launch: 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with
 // resident weights, 2 = the persistent halo-patch k_conv_wg_h, 3 = the persistent halo-patch k_conv_wg_hw with streamed
 // weights and N tiles of at most 128.  All give bit-identical outputs; the autotuner keeps the fastest eligible one per
-// launch (SB_FORCE_VARIANT=n forces form n where it is eligible).
+// launch (SB_FORCE_VARIANT=n forces form n where it is eligible).  Form 4 (k_tconv_wg_hw) spans the four phase launches
+// of a transposed conv and is chosen per op (TcTconv); SB_FORCE_VARIANT=4 forces it, any other forced form the phases.
 constexpr int kForms = 4;
 struct TcForm {
   int ok;
@@ -1178,10 +1370,24 @@ struct TcLaunch {
   int form;
 };
 
+// Form 4 of a transposed conv: its four phase launches as one k_tconv_wg_hw launch (P: the first phase's parameters with
+// the ring sizes and N of this form; mapA: a [64, 16, 17, 1] activation box; mapB: a [64, N, 1] weight box)
+struct TcTconv {
+  int ok;
+  int max_ctas;
+  int n_units;                 // (N tile, input tile) units per frame
+  size_t smem;
+  CUtensorMap mapA, mapB;
+  TcParams P;
+  TcPhases Q;
+};
+
 }  // namespace
 
 struct SbConvTcPlan {
   std::vector<TcLaunch> launches;   // 1 for conv, 4 phases for tconv
+  TcTconv tconv = {};               // tconv: the fused form of the four phases (tconv.ok: eligible)
+  bool tconv_fused = false;         // the autotuner picked the fused form over the phase launches
   __half* w16 = nullptr;            // [taps][Cout_pad][Cin]
   int Cout_pad = 0;
   // first layer as a Toeplitz GEMM (sb_first_view_prepare): staged [B][H][W/8][16] fp16 view of the frame
@@ -1339,6 +1545,20 @@ static ConvKernel conv_kernel_form(int form, int KC, int N) {
   return KC == 16 ? conv_kernel_p_n<1>(N) : (KC == 32 ? conv_kernel_p_n<2>(N) : conv_kernel_p_n<4>(N));
 }
 
+typedef void (*TconvKernel)(CUtensorMap, CUtensorMap, TcParams, TcPhases);
+
+// the fused transposed-conv instantiations: N tiles 32..128; nullptr otherwise
+static TconvKernel tconv_kernel(int N) {
+  switch (N) {
+    case 32: return k_tconv_wg_hw<32>;
+    case 48: return k_tconv_wg_hw<48>;
+    case 64: return k_tconv_wg_hw<64>;
+    case 96: return k_tconv_wg_hw<96>;
+    case 128: return k_tconv_wg_hw<128>;
+    default: return nullptr;
+  }
+}
+
 // shared memory of a k_conv_wg launch: rings, accumulator staging rows, barriers, bias / BN vectors of 256 channels
 static size_t conv_smem(const TcParams& P, int n_a, int n_b) {
   return (size_t)n_a * P.a_slot_bytes + (size_t)n_b * P.b_slot_bytes + (size_t)128 * (stage_cols(P.N) + 4) * sizeof(float) +
@@ -1360,6 +1580,12 @@ static size_t conv_smem_halo(const TcParams& P, int n_a) {
 // shared memory of a k_conv_wg_hw launch with N tiles of n: n_b weight slots, n_a patch slots, 2 (n_a + n_b) barriers, the bias
 static size_t conv_smem_wide(const TcParams& P, int n, int n_a, int n_b) {
   return 1024 /*align slack*/ + (size_t)n_b * n * 128 + (size_t)n_a * 8 * wide_plane(n) + (size_t)(2 * n_a + 2 * n_b) * 8 +
+         (size_t)P.Cout * sizeof(float);
+}
+
+// shared memory of a k_tconv_wg_hw launch with N tiles of n: n_b weight slots, n_a box slots, 2 (n_a + n_b) barriers, the bias
+static size_t tconv_smem(const TcParams& P, int n, int n_a, int n_b) {
+  return 1024 /*align slack*/ + (size_t)n_b * n * 128 + (size_t)n_a * kTconvBox + (size_t)(2 * n_a + 2 * n_b) * 8 +
          (size_t)P.Cout * sizeof(float);
 }
 
@@ -1452,6 +1678,16 @@ static bool res_fusable(const SbModel* m, size_t oi) {
          rb.H == ob.H && rb.W == ob.W && sb.H == ob.H && sb.W == ob.W && op.pool_buf() < 0 && !(op.flags() & (SB_OPF_BN | SB_OPF_RELU));
 }
 
+// [tap][Cout_pad][Cin] weights of a plan, box [KC, box_n, 1]
+static CUresult encode_weights(EncodeTiledFn enc, const SbConvTcPlan* plan, int Cin, int n_wtaps, int KC, int box_n, CUtensorMap* map) {
+  cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)plan->Cout_pad, (cuuint64_t)n_wtaps};
+  cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)plan->Cout_pad * Cin * 2};
+  cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)box_n, 1};
+  cuuint32_t es[3] = {1, 1, 1};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
                        const TcGroup* groups, int dy0, int extra_rows, int n_wtaps, int oy_mul, int oy_add,
                        int ox_mul, int ox_add, const TcView* view = nullptr, bool fuse_res = false,
@@ -1537,22 +1773,68 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
   }
-  // B: [tap][Cout_pad][Cin] weights, box [KC, box_n, 1]
-  auto encode_b = [&](CUtensorMap* map, int box_n) {
-    cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)plan->Cout_pad, (cuuint64_t)n_wtaps};
-    cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)plan->Cout_pad * Cin * 2};
-    cuuint32_t box[3] = {(cuuint32_t)KC, (cuuint32_t)box_n, 1};
-    cuuint32_t es[3] = {1, 1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-               swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  };
-  if (CUresult r = encode_b(&L.mapB, N); r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
+  if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, N, &L.mapB); r != CUDA_SUCCESS)
+    return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   P.n_tiles = (int)L.grid.x;
   setup_forms(h, L, total_steps);
   if (L.forms[3].ok)
-    if (CUresult r = encode_b(&L.forms[3].mapB, L.forms[3].N); r != CUDA_SUCCESS)
+    if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, L.forms[3].N, &L.forms[3].mapB); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, wide form) failed: %d", (int)r);
   (dst ? *dst : plan->launches).push_back(L);
+  return 0;
+}
+
+// Form 4 of the transposed conv `op`, whose four phase launches are plan->launches: chunks of 64 input channels, N tiles of
+// min(N, 128) channels that cover C_out exactly, the fp16 fast-epilogue shape (so not precision 2), and phases whose taps
+// all lie in one 17-row box (dy0 of -1 or 0, start rows 0 or 1: the k3 and k4 phases); 4 box slots and 4-8 weight slots
+// in 225 KB, one CTA per SM.  Leaves plan->tconv.ok = 0 where the op is not eligible.
+static int tconv_setup(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan) {
+  TcTconv& T = plan->tconv;
+  T.ok = 0;
+  if (plan->launches.size() != 4) return 0;
+  const TcParams& P0 = plan->launches[0].P;
+  const int N = std::min(P0.N, 128);
+  TconvKernel kern = tconv_kernel(N);
+  if (!kern || P0.KC != 64 || P0.Cout % N) return 0;
+  for (int p = 0; p < 4; ++p) {
+    const TcParams& P = plan->launches[p].P;
+    if (P.epi_mode != 1 || P.n_groups > 2 || P.dy0 < -1 || P.dy0 > 0) return 0;
+    T.Q.n_groups[p] = P.n_groups; T.Q.dy0[p] = P.dy0; T.Q.oy_add[p] = P.oy_add; T.Q.ox_add[p] = P.ox_add;
+    for (int g = 0; g < P.n_groups; ++g) {
+      for (int t = 0; t < P.groups[g].n_taps; ++t)
+        if (P.groups[g].taps[t].row_off < 0 || P.groups[g].taps[t].row_off > 1) return 0;
+      T.Q.groups[p][g] = P.groups[g];
+    }
+  }
+  T.P = P0;
+  T.P.N = N; T.P.n_a_slots = 4; T.P.skip_out = 0; T.P.pdl_trigger = 0;
+  T.P.n_b_slots = 0;
+  for (int nb = 8; nb >= 4 && !T.P.n_b_slots; --nb)
+    if (tconv_smem(P0, N, 4, nb) <= kMaxDynSmem) T.P.n_b_slots = nb;
+  if (!T.P.n_b_slots) return 0;
+  T.smem = tconv_smem(P0, N, 4, T.P.n_b_slots);
+  int nb = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kWideThreads, T.smem) != cudaSuccess || nb < 1) {
+    cudaGetLastError();
+    return 0;
+  }
+  T.max_ctas = nb * h->sm_count;
+  T.n_units = (P0.Cout / N) * ((P0.W + 15) / 16) * ((P0.H + 15) / 16);
+  EncodeTiledFn enc = get_encode();
+  {
+    // the phase launches' activation view (slice channels, W, H, batch) with a [64, 16, 17, 1] box
+    cuuint64_t dims[4] = {(cuuint64_t)P0.in_C, (cuuint64_t)P0.W, (cuuint64_t)P0.H, (cuuint64_t)m->B};
+    cuuint64_t strides[3] = {(cuuint64_t)P0.in_Ctot * 2, (cuuint64_t)P0.W * P0.in_Ctot * 2, (cuuint64_t)P0.H * P0.W * P0.in_Ctot * 2};
+    cuuint32_t box[4] = {64, 16, (cuuint32_t)kTconvBoxRows, 1};
+    cuuint32_t es[4] = {1, 1, 1, 1};
+    CUresult r = enc(&T.mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(P0.in), dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A, fused tconv) failed: %d", (int)r);
+  }
+  if (CUresult r = encode_weights(enc, plan, op.in_C(), op.k() * op.k(), 64, N, &T.mapB); r != CUDA_SUCCESS)
+    return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, fused tconv) failed: %d", (int)r);
+  T.ok = 1;
   return 0;
 }
 
@@ -1847,6 +2129,8 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
         for (int n : {16, 32, 48, 64, 96, 128, 192, 256})
           if (ConvKernel k = conv_kernel_form(f, kc, n))
             SB_CUDA(h, cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
+    for (int n : {32, 48, 64, 96, 128})
+      SB_CUDA(h, cudaFuncSetAttribute((const void*)tconv_kernel(n), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
     attr_set = true;
   }
   for (size_t oi = 0; oi < m->ops.size(); ++oi) {
@@ -1929,6 +2213,7 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
           rc = make_launch(h, m, op, plan, ng, g, a == 0 ? -1 : 0, extra, 9, 2, a, 2, bx);
         }
     }
+    if (!rc && op.kind() == SB_OPK_TCONV) rc = tconv_setup(h, m, op, plan);
     if (rc) { cudaFree(plan->w16); delete plan; return rc; }
     m->tc_plans[oi] = plan;
     if (plan->res_fused) m->skip_op[oi + 1] = 2;
@@ -2024,11 +2309,27 @@ static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
   cudaLaunchKernelEx(&cfg, conv_kernel(P.KC, P.N), L.mapA, L.mapB, P);
 }
 
+// form 4: the four phases of a transposed conv in one persistent launch of as many CTAs as fit at once (capped at the work
+// count); each CTA triggers its dependents when it starts its last work item
+static void launch_tconv_fused(const TcTconv& T, int B, cudaStream_t stream) {
+  TcParams P = T.P;
+  P.batch = B;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(std::min(4 * T.n_units * B, T.max_ctas)); cfg.blockDim = dim3(kWideThreads); cfg.dynamicSmemBytes = T.smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, tconv_kernel(P.N), T.mapA, T.mapB, P, T.Q);
+}
+
 static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan);
 
 // Picks, for every tensor-core conv launch (each transposed-conv phase included), the faster eligible kernel form
 // (streaming / resident weights), for a first layer with a Toeplitz view the faster of the view + tensor-core
-// conv and k_conv_first, and for the first encoder block the fused k_conv01 or the separate launches, by timing the
+// conv and k_conv_first, for a transposed conv its four phase launches or the fused form 4, and for the first encoder
+// block the fused k_conv01 or the separate launches, by timing the
 // forms on the device at the configured batch (buffers are already allocated; their contents do not matter for timing).
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   cudaEvent_t e0, e1;
@@ -2071,6 +2372,31 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
           fprintf(stderr, " -> %s\n", form_name[L.form]);
         }
       }
+  }
+  // transposed convs: the four phase launches (whatever forms were just picked for them) against the fused form 4
+  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
+    SbConvTcPlan* plan = m->tc_plans[oi];
+    if (!plan || !plan->tconv.ok) continue;
+    float best[2] = {1e30f, 1e30f};
+    for (int f = 0; f < 2; ++f) {
+      plan->tconv_fused = f == 1;
+      for (int rep = 0; rep < 4; ++rep) {
+        cudaEventRecord(e0, h->stream);
+        const int rc = sb_conv_tc_launch(h, m, (int)oi, m->B);
+        if (rc) return rc;
+        cudaEventRecord(e1, h->stream);
+        cudaError_t e = cudaStreamSynchronize(h->stream);
+        if (e != cudaSuccess)
+          return sb_fail(h, SB_ERR_CUDA, "autotune launch (op %zu, %s) failed: %s", oi, f ? "fused tconv" : "tconv phases", cudaGetErrorString(e));
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, e0, e1);
+        if (rep > 0) best[f] = std::min(best[f], ms);
+      }
+    }
+    plan->tconv_fused = force >= 0 ? force == 4 : best[1] < best[0];
+    if (dbg)
+      fprintf(stderr, "[sb_conv_tc] op %zu launches (4 tconv phases) %.1f us, fused k_tconv_wg_hw %.1f us -> %s\n", oi, best[0] * 1e3f,
+              best[1] * 1e3f, plan->tconv_fused ? "tconv-fused" : "phases");
   }
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
@@ -2203,6 +2529,11 @@ static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
 int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
   SbConvTcPlan* plan = m->tc_plans[op_index];
   if (head_kernel_ok(m, m->ops[op_index], plan)) return head_launch(h, m, m->ops[op_index], plan, B);
+  if (plan->tconv_fused) {
+    launch_tconv_fused(plan->tconv, B, h->stream);
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  }
   const int skip = plan->out_dead && !m->keep_dead_stores;
   // the sub-pixel phases of a transposed conv run back to back on the launching stream: under programmatic dependent
   // launch each phase's CTAs start as the previous phase's SMs drain

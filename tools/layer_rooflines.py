@@ -9,7 +9,7 @@ bench.py.  The bound of a layer is the larger floor.
 L2 columns (3x3 convs and k3 transposed convs only): the bytes the streaming form of k_conv_wg pulls from L2 into the SMs
 (every 128-pixel CTA loads its activation boxes and its whole weight slice), and, given an L2 read rate in TB/s
 (`tools/bw_probe.py`, "L2-resident"), the time that traffic takes at that rate; then the same for the wide form
-k_conv_wg_hw where it is eligible.
+k_conv_wg_hw (3x3 convs) or the fused transposed-conv form k_tconv_wg_hw (k3 transposed convs) where it is eligible.
 """
 import json
 import os
@@ -82,12 +82,17 @@ def l2_bytes_streaming(cin, cout, hin, taps):
 
 def l2_bytes_wide(cin, cout, hin, taps):
     """The same for the wide form k_conv_wg_hw (3x3 convs with C_in > 32; None: not eligible): per item (16 x 8 by pixels,
-    one N tile of n <= 128 channels) and 64-channel chunk, one (8 by + 2) x 18-pixel halo patch and 9 weight slices."""
-    if taps != 9 or cin <= 32:
+    one N tile of n <= 128 channels) and 64-channel chunk, one (8 by + 2) x 18-pixel halo patch and 9 weight slices.
+    For a k3 transposed conv, the fused form k_tconv_wg_hw: per 16 x 16 input tile, N tile and 64-channel chunk, the four
+    phases load 2 + 1 + 2 + 1 activation boxes of 17 x 16 pixels and 4 + 2 + 2 + 1 weight slices."""
+    if taps not in (9, 2.25) or cin <= 32:
         return None
     n = min(_wg_n(-(-cout // 16) * 16), 128)
     if cout % n:
         return None
+    if taps == 2.25:
+        tiles = (-(-hin // 16)) ** 2
+        return B * tiles * (cout // n) * -(-cin // 64) * (6 * 17 * 16 * 64 * 2 + 9 * n * 64 * 2)
     by = 4 if n <= 64 else 2
     items = -(-hin // 16) * -(-hin // (8 * by))
     return B * items * (cout // n) * -(-cin // 64) * ((8 * by + 2) * 18 * 64 * 2 + 9 * n * 64 * 2)
@@ -100,7 +105,7 @@ def main(src, out, l2_tbs=None):
         if m:
             ms[int(m.group(1))] = float(m.group(2))
     rows = ["| op | layer | measured us | GFLOP | tensor floor us | bytes MB | HBM floor us | bound | floor / measured | L2 GB (streaming) | L2 us "
-            "| L2 GB (wide) | L2 us (wide) |",
+            "| L2 GB (wide / fused tconv) | L2 us (wide / fused tconv) |",
             "|---|---|---|---|---|---|---|---|---|---|---|---|---|"]
     tot_m = tot_f = tot_l2 = 0.0
 
