@@ -312,15 +312,9 @@ int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
   SbConv01Plan* pl = m->conv01;
   C01Params P = pl->P;
   P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.batch = B;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(std::min(P.n_tiles * B, pl->max_ctas)); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = SMEM_BYTES;
-  cfg.stream = h->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
-  if (frames_are_u8) cudaLaunchKernelEx(&cfg, k_conv01<unsigned char>, P);
-  else cudaLaunchKernelEx(&cfg, k_conv01<float>, P);
+  void* args[] = {&P};
+  sb_launch_pdl(frames_are_u8 ? (const void*)k_conv01<unsigned char> : (const void*)k_conv01<float>,
+                dim3(std::min(P.n_tiles * B, pl->max_ctas)), dim3(256), SMEM_BYTES, h->stream, args);
   SB_CHECK_LAUNCH(h);
   return 0;
 }

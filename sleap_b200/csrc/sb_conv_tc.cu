@@ -1344,50 +1344,38 @@ __global__ void __launch_bounds__(256) k_head_1x1(const __half* __restrict__ in,
   asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
-// Kernel forms of one launch: 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with
-// resident weights, 2 = the persistent halo-patch k_conv_wg_h, 3 = the persistent halo-patch k_conv_wg_hw with streamed
-// weights and N tiles of at most 128.  All give bit-identical outputs; the autotuner keeps the fastest eligible one per
-// launch (SB_FORCE_VARIANT=n forces form n where it is eligible).  Form 4 (k_tconv_wg_hw) spans the four phase launches
-// of a transposed conv and is chosen per op (TcTconv); SB_FORCE_VARIANT=4 forces it, any other forced form the phases.
-constexpr int kForms = 4;
+// Kernel forms of a tensor-core conv, all bit-identical.  Forms 0-3 run one launch (a conv, or one sub-pixel phase of a
+// transposed conv): 0 = k_conv_wg (streaming, one CTA per tile and N tile), 1 = the persistent k_conv_wg_p with resident
+// weights, 2 = the persistent halo-patch k_conv_wg_h, 3 = the persistent halo-patch k_conv_wg_hw with streamed weights
+// and N tiles of at most 128.  Form 4 = the persistent k_tconv_wg_hw runs all four phases of a transposed conv in one
+// launch; it is kept in the first phase's TcLaunch and, when picked, stands for the whole op.  The autotuner first keeps
+// the fastest eligible form 0-3 per launch, then for each transposed conv the faster of its phase launches and form 4.
+// SB_FORCE_VARIANT=n with n = 0-3 forces form n on every launch where it is eligible and keeps the phase launches; n = 4
+// keeps the autotuned launch forms and forces form 4 where it is eligible; any other n >= 0 keeps the autotuned launch
+// forms and the phase launches.
+constexpr int kForms = 5, kTconvForm = 4;
 struct TcForm {
   int ok;
-  int n_a_slots, n_b_slots;    // halo forms: n_a_slots = patch slots
-  size_t smem;
   int threads;                 // CTA size
-  int N;                       // wgmma N of the form's tiles (form 3: at most 128; the others: the launch's P.N)
+  size_t smem;
   int max_ctas;                // persistent forms: CTAs the GPU holds at once
-  int n_tiles;                 // persistent forms: work items per frame
-  CUtensorMap mapB;            // form 3: weight map with a [64, N, 1] box (the others use TcLaunch::mapB)
+  int n_items;                 // persistent forms: work items per frame
+  TcParams P;                  // the launch's parameters with this form's ring sizes and N
+  CUtensorMap mapA, mapB;      // form 3: a [64, N, 1] weight box; form 4: a [64, 16, 17, 1] activation box too
+  TcPhases Q;                  // form 4: the four phases' filter columns and taps
 };
 
 struct TcLaunch {
-  CUtensorMap mapA, mapB;
-  TcParams P;
-  dim3 grid;
-  size_t smem;
-  TcForm forms[kForms];        // forms[0] (streaming) uses P's ring sizes and smem
+  dim3 grid;                   // form 0: tiles x N tiles (z = batch, set at launch)
+  TcForm forms[kForms];
   int form;
-};
-
-// Form 4 of a transposed conv: its four phase launches as one k_tconv_wg_hw launch (P: the first phase's parameters with
-// the ring sizes and N of this form; mapA: a [64, 16, 17, 1] activation box; mapB: a [64, N, 1] weight box)
-struct TcTconv {
-  int ok;
-  int max_ctas;
-  int n_units;                 // (N tile, input tile) units per frame
-  size_t smem;
-  CUtensorMap mapA, mapB;
-  TcParams P;
-  TcPhases Q;
 };
 
 }  // namespace
 
 struct SbConvTcPlan {
   std::vector<TcLaunch> launches;   // 1 for conv, 4 phases for tconv
-  TcTconv tconv = {};               // tconv: the fused form of the four phases (tconv.ok: eligible)
-  bool tconv_fused = false;         // the autotuner picked the fused form over the phase launches
+  const void* head = nullptr;       // the k_head_1x1 instantiation that runs this 1x1 fp32 head instead of the launches
   __half* w16 = nullptr;            // [taps][Cout_pad][Cin]
   int Cout_pad = 0;
   // first layer as a Toeplitz GEMM (sb_first_view_prepare): staged [B][H][W/8][16] fp16 view of the frame
@@ -1418,7 +1406,6 @@ static bool tc_eligible(const SbModel* m, const SbOp& op) {
   // any channel count that keeps 16-byte aligned NHWC rows: K is cut into chunks of 16 / 32 / 64 channels and a
   // chunk that reaches past C_in is zero-filled by TMA on both operands (activations and weights)
   if (!(Cin >= 16 && Cin % 8 == 0)) return false;
-  if (getenv("SB_TC_STRICT_CIN") && !(Cin == 16 || Cin == 32 || Cin % 64 == 0)) return false;
   if (op.kind() == SB_OPK_CONV && !((op.k() == 1 || op.k() == 3 || op.k() == 5 || op.k() == 7) && op.stride() == 1) &&
       !(op.k() == 1 && op.stride() == 2))
     return false;
@@ -1428,10 +1415,8 @@ static bool tc_eligible(const SbModel* m, const SbOp& op) {
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
   if (ib.f32) return false;
-  // feature maps smaller than the TMA box (16 px x 8 + k - 1 rows): the box simply hangs over the tensor, the overhang is
-  // zero-filled like every other out-of-image tap (SB_TC_MIN_BOX=1 restores round 1's rule that kept e.g. the 10x10 middle
-  // block of a 160x160 crop network -- 2/3 of its step time -- on the CUDA-core kernel)
-  if (getenv("SB_TC_MIN_BOX") && (ib.W < TW || ib.H < TH + std::max(2, op.k() - 1))) return false;
+  // feature maps smaller than the TMA box (16 px x 8 + k - 1 rows) are taken too: the box simply hangs over the tensor,
+  // the overhang is zero-filled like every other out-of-image tap
   if (ib.C % 8 || op.in_coff() % 8) return false;
   if (!ob.f32 && (ob.C % 8 || op.out_coff() % 8)) return false;
   return true;
@@ -1471,92 +1456,41 @@ struct TcView {
   int out_coff = 0;
 };
 
+// the wgmma tile widths N that have instantiations
+constexpr int kWgN[8] = {16, 32, 48, 64, 96, 128, 192, 256};
+
 // N of the wgmma instantiation that covers `n` output channels (extra rows of the weight box are zero-filled by TMA)
 static int wg_n(int n) {
-  for (int c : {16, 32, 48, 64, 96, 128, 192}) if (n <= c) return c;
+  for (int c : kWgN) if (n <= c) return c;
   return 256;
 }
 
-typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, TcParams);
-
-template <int KSTEPS>
-static ConvKernel conv_kernel_n(int N) {
-  switch (N) {
-    case 16: return k_conv_wg<KSTEPS, 16>;
-    case 32: return k_conv_wg<KSTEPS, 32>;
-    case 48: return k_conv_wg<KSTEPS, 48>;
-    case 64: return k_conv_wg<KSTEPS, 64>;
-    case 96: return k_conv_wg<KSTEPS, 96>;
-    case 128: return k_conv_wg<KSTEPS, 128>;
-    case 192: return k_conv_wg<KSTEPS, 192>;
-    default: return k_conv_wg<KSTEPS, 256>;
-  }
+// Instantiations of each form for K steps of 16 per staged slice of KS x 16 channels, by N (kWgN).  Resident: N <= 128
+// (a 192 / 256-wide bank does not fit beside the activation ring at C_in >= 64, and N = 256 leaves no registers for the
+// persistent loop state).  Halo: N <= 64.  Wide and fused tconv: chunks of 64 channels only, N of 32..128.
+template <int KS>
+static const void* form_kernel_ks(int form, int ni) {
+  static const void* const kernels[kForms][8] = {
+      {(const void*)k_conv_wg<KS, 16>, (const void*)k_conv_wg<KS, 32>, (const void*)k_conv_wg<KS, 48>,
+       (const void*)k_conv_wg<KS, 64>, (const void*)k_conv_wg<KS, 96>, (const void*)k_conv_wg<KS, 128>,
+       (const void*)k_conv_wg<KS, 192>, (const void*)k_conv_wg<KS, 256>},
+      {(const void*)k_conv_wg_p<KS, 16>, (const void*)k_conv_wg_p<KS, 32>, (const void*)k_conv_wg_p<KS, 48>,
+       (const void*)k_conv_wg_p<KS, 64>, (const void*)k_conv_wg_p<KS, 96>, (const void*)k_conv_wg_p<KS, 128>, nullptr, nullptr},
+      {(const void*)k_conv_wg_h<KS, 16>, (const void*)k_conv_wg_h<KS, 32>, (const void*)k_conv_wg_h<KS, 48>,
+       (const void*)k_conv_wg_h<KS, 64>, nullptr, nullptr, nullptr, nullptr},
+      {nullptr, (const void*)k_conv_wg_hw<32>, (const void*)k_conv_wg_hw<48>, (const void*)k_conv_wg_hw<64>,
+       (const void*)k_conv_wg_hw<96>, (const void*)k_conv_wg_hw<128>, nullptr, nullptr},
+      {nullptr, (const void*)k_tconv_wg_hw<32>, (const void*)k_tconv_wg_hw<48>, (const void*)k_tconv_wg_hw<64>,
+       (const void*)k_tconv_wg_hw<96>, (const void*)k_tconv_wg_hw<128>, nullptr, nullptr}};
+  return form >= 3 && KS != 4 ? nullptr : kernels[form][ni];
 }
 
-// the instantiation for an input-channel chunk of KC (K steps of 16 per staged slice) and a wg_n() tile width N
-static ConvKernel conv_kernel(int KC, int N) {
-  return KC == 16 ? conv_kernel_n<1>(N) : (KC == 32 ? conv_kernel_n<2>(N) : conv_kernel_n<4>(N));
-}
-
-// the resident-weight instantiations: N <= 128 (a 192 / 256-wide bank does not fit beside the activation ring at C_in >= 64,
-// and N = 256 leaves no registers for the persistent loop state); nullptr otherwise
-template <int KSTEPS>
-static ConvKernel conv_kernel_p_n(int N) {
-  switch (N) {
-    case 16: return k_conv_wg_p<KSTEPS, 16>;
-    case 32: return k_conv_wg_p<KSTEPS, 32>;
-    case 48: return k_conv_wg_p<KSTEPS, 48>;
-    case 64: return k_conv_wg_p<KSTEPS, 64>;
-    case 96: return k_conv_wg_p<KSTEPS, 96>;
-    case 128: return k_conv_wg_p<KSTEPS, 128>;
-    default: return nullptr;
-  }
-}
-
-// the halo instantiations: N <= 64; nullptr otherwise
-template <int KSTEPS>
-static ConvKernel conv_kernel_h_n(int N) {
-  switch (N) {
-    case 16: return k_conv_wg_h<KSTEPS, 16>;
-    case 32: return k_conv_wg_h<KSTEPS, 32>;
-    case 48: return k_conv_wg_h<KSTEPS, 48>;
-    case 64: return k_conv_wg_h<KSTEPS, 64>;
-    default: return nullptr;
-  }
-}
-
-// the wide instantiations: K chunks of 64 channels, N tiles 32..128; nullptr otherwise
-static ConvKernel conv_kernel_hw(int KC, int N) {
-  if (KC != 64) return nullptr;
-  switch (N) {
-    case 32: return k_conv_wg_hw<32>;
-    case 48: return k_conv_wg_hw<48>;
-    case 64: return k_conv_wg_hw<64>;
-    case 96: return k_conv_wg_hw<96>;
-    case 128: return k_conv_wg_hw<128>;
-    default: return nullptr;
-  }
-}
-
-static ConvKernel conv_kernel_form(int form, int KC, int N) {
-  if (form == 0) return conv_kernel(KC, N);
-  if (form == 3) return conv_kernel_hw(KC, N);
-  if (form == 2) return KC == 16 ? conv_kernel_h_n<1>(N) : (KC == 32 ? conv_kernel_h_n<2>(N) : conv_kernel_h_n<4>(N));
-  return KC == 16 ? conv_kernel_p_n<1>(N) : (KC == 32 ? conv_kernel_p_n<2>(N) : conv_kernel_p_n<4>(N));
-}
-
-typedef void (*TconvKernel)(CUtensorMap, CUtensorMap, TcParams, TcPhases);
-
-// the fused transposed-conv instantiations: N tiles 32..128; nullptr otherwise
-static TconvKernel tconv_kernel(int N) {
-  switch (N) {
-    case 32: return k_tconv_wg_hw<32>;
-    case 48: return k_tconv_wg_hw<48>;
-    case 64: return k_tconv_wg_hw<64>;
-    case 96: return k_tconv_wg_hw<96>;
-    case 128: return k_tconv_wg_hw<128>;
-    default: return nullptr;
-  }
+// The kernel of `form` for input-channel chunks of KC and a wg_n() tile width N, or nullptr where the form has none.
+// Forms 0-3 take (mapA, mapB, TcParams), form 4 (mapA, mapB, TcParams, TcPhases).
+static const void* form_kernel(int form, int KC, int N) {
+  const int ni = (int)(std::find(std::begin(kWgN), std::end(kWgN), N) - std::begin(kWgN));
+  if (ni == 8) return nullptr;
+  return KC == 16 ? form_kernel_ks<1>(form, ni) : (KC == 32 ? form_kernel_ks<2>(form, ni) : form_kernel_ks<4>(form, ni));
 }
 
 // shared memory of a k_conv_wg launch: rings, accumulator staging rows, barriers, bias / BN vectors of 256 channels
@@ -1577,16 +1511,27 @@ static size_t conv_smem_halo(const TcParams& P, int n_a) {
          (size_t)P.N * sizeof(float);
 }
 
-// shared memory of a k_conv_wg_hw launch with N tiles of n: n_b weight slots, n_a patch slots, 2 (n_a + n_b) barriers, the bias
-static size_t conv_smem_wide(const TcParams& P, int n, int n_a, int n_b) {
-  return 1024 /*align slack*/ + (size_t)n_b * n * 128 + (size_t)n_a * 8 * wide_plane(n) + (size_t)(2 * n_a + 2 * n_b) * 8 +
-         (size_t)P.Cout * sizeof(float);
+// Rings of a k_conv_wg_hw / k_tconv_wg_hw launch (forms 3 and 4, N tiles of F.P.N): n_a activation slots of a_slot bytes
+// and the deepest ring of 8 down to 4 weight slices that fits in 225 KB beside them, 2 (n_a + n_b) barriers and the bias.
+// Sets F.ok where one fits.
+static void fit_weight_ring(TcForm& F, int n_a, size_t a_slot) {
+  for (int nb = 8; nb >= 4 && !F.ok; --nb) {
+    const size_t smem = 1024 /*align slack*/ + (size_t)nb * F.P.N * 128 + (size_t)n_a * a_slot + (size_t)(2 * n_a + 2 * nb) * 8 +
+                        (size_t)F.P.Cout * sizeof(float);
+    if (smem <= kMaxDynSmem) { F.ok = 1; F.P.n_a_slots = n_a; F.P.n_b_slots = nb; F.smem = smem; }
+  }
 }
 
-// shared memory of a k_tconv_wg_hw launch with N tiles of n: n_b weight slots, n_a box slots, 2 (n_a + n_b) barriers, the bias
-static size_t tconv_smem(const TcParams& P, int n, int n_a, int n_b) {
-  return 1024 /*align slack*/ + (size_t)n_b * n * 128 + (size_t)n_a * kTconvBox + (size_t)(2 * n_a + 2 * n_b) * 8 +
-         (size_t)P.Cout * sizeof(float);
+// Co-resident CTAs of persistent form f where it fits (F.ok); clears F.ok where not even one CTA per SM does.
+static void fit_ctas(sb_handle_s* h, TcForm& F, int f) {
+  if (!F.ok) return;
+  int nb = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, form_kernel(f, F.P.KC, F.P.N), F.threads, F.smem) != cudaSuccess || nb < 1) {
+    cudaGetLastError();
+    F.ok = 0;
+    return;
+  }
+  F.max_ctas = nb * h->sm_count;
 }
 
 // The halo forms take plain 3x3 stride-1 SAME convs (filter column g = dx + 1, tap ky of it = weight tap 3 ky + g) in the
@@ -1605,63 +1550,52 @@ static bool halo_shape(const TcParams& P) {
 
 // form 2: one input-channel chunk and one N tile of at most 64 channels
 static bool halo_eligible(const TcLaunch& L) {
-  return L.grid.y == 1 && L.P.n_chunks == 1 && L.P.N <= 64 && halo_shape(L.P);
+  const TcParams& P = L.forms[0].P;
+  return L.grid.y == 1 && P.n_chunks == 1 && P.N <= 64 && halo_shape(P);
 }
 
 // form 3: chunks of 64 input channels, and N tiles of min(N, 128) channels that cover C_out exactly
 static int wide_n(const TcParams& P) { return std::min(P.N, 128); }
-static bool wide_eligible(const TcLaunch& L) {
-  return L.P.KC == 64 && L.P.Cout % wide_n(L.P) == 0 && halo_shape(L.P);
-}
+static bool wide_eligible(const TcParams& P) { return P.KC == 64 && P.Cout % wide_n(P) == 0 && halo_shape(P); }
 
-// Eligibility, ring sizes, shared memory and co-resident grid size of the persistent forms of launch L (forms[0], the
-// streaming form, is always eligible).  Resident form: one N tile, and the whole bank of the launch's weight slices plus
-// at least 2 activation slots fit in 225 KB; two CTAs per SM where they fit in 113 KB.  Halo form: halo_eligible, and the
-// bank plus at least 4 patch slots (two being read, two prefetched) fit in 225 KB; up to 8 slots, one CTA per SM.  Wide
-// form: wide_eligible, 2 patch slots and 4-8 weight slots in 225 KB, one CTA per SM.
+// Forms 1-4 of launch L as copies of its streaming form 0 (always eligible), and the eligibility, ring sizes, shared
+// memory and co-resident grid size of forms 1-3 (form 4 is set up per op: setup_tconv_form).  Resident form: one N tile,
+// and the whole bank of the launch's weight slices plus at least 2 activation slots fit in 225 KB; two CTAs per SM where
+// they fit in 113 KB.  Halo form: halo_eligible, and the bank plus at least 4 patch slots (two being read, two
+// prefetched) fit in 225 KB; up to 8 slots, one CTA per SM.  Wide form: wide_eligible, 2 patch slots and 4-8 weight
+// slots in 225 KB, one CTA per SM.
 static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
-  TcParams& P = L.P;
+  const TcParams& P = L.forms[0].P;
   L.form = 0;
-  L.forms[0].ok = 1; L.forms[0].n_a_slots = P.n_a_slots; L.forms[0].n_b_slots = P.n_b_slots; L.forms[0].smem = L.smem;
-  for (int f = 0; f < kForms; ++f) { L.forms[f].threads = kConvThreads; L.forms[f].N = P.N; }
-  auto fit = [&](TcForm& F, ConvKernel kern) {               // co-resident CTAs of an eligible form
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, F.threads, F.smem) != cudaSuccess || nb < 1) {
-      cudaGetLastError();
-      F.ok = 0;
-      return;
-    }
-    F.max_ctas = nb * h->sm_count;
-  };
-  if (ConvKernel kern = conv_kernel_form(3, P.KC, wide_n(P)); kern && wide_eligible(L)) {
-    TcForm& F = L.forms[3];
-    F.threads = kWideThreads;
-    F.N = wide_n(P);
-    for (int nb = 8; nb >= 4 && !F.ok; --nb)
-      if (conv_smem_wide(P, F.N, 2, nb) <= kMaxDynSmem) { F.ok = 1; F.n_a_slots = 2; F.n_b_slots = nb; F.smem = conv_smem_wide(P, F.N, 2, nb); }
-    const int by = wide_by(F.N);
-    F.n_tiles = (P.Cout / F.N) * ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
-    if (F.ok) fit(F, kern);
+  for (int f = 1; f < kForms; ++f) {
+    L.forms[f] = L.forms[0];
+    L.forms[f].ok = 0;
   }
-  if (ConvKernel kern = conv_kernel_form(2, P.KC, P.N); kern && halo_eligible(L)) {
-    TcForm& F = L.forms[2];
+  if (TcForm& F = L.forms[3]; form_kernel(3, P.KC, wide_n(P)) && wide_eligible(P)) {
+    F.threads = kWideThreads;
+    F.P.N = wide_n(P);
+    fit_weight_ring(F, 2, (size_t)8 * wide_plane(F.P.N));
+    const int by = wide_by(F.P.N);
+    F.n_items = (P.Cout / F.P.N) * ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
+    fit_ctas(h, F, 3);
+  }
+  if (TcForm& F = L.forms[2]; form_kernel(2, P.KC, P.N) && halo_eligible(L)) {
     for (int na = 8; na >= 4 && !F.ok; --na)
-      if (conv_smem_halo(P, na) <= kMaxDynSmem) { F.ok = 1; F.n_a_slots = na; F.n_b_slots = 9; F.smem = conv_smem_halo(P, na); }
+      if (conv_smem_halo(P, na) <= kMaxDynSmem) { F.ok = 1; F.P.n_a_slots = na; F.P.n_b_slots = 9; F.smem = conv_smem_halo(P, na); }
     const int by = halo_by(P.N, P.KC);
-    F.n_tiles = ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
-    if (F.ok) fit(F, kern);
+    F.n_items = ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
+    fit_ctas(h, F, 2);
   }
   TcForm& F = L.forms[1];
-  ConvKernel kern = conv_kernel_form(1, P.KC, P.N);
-  if (!kern || L.grid.y != 1) return;
+  if (!form_kernel(1, P.KC, P.N) || L.grid.y != 1) return;
   const int bank = P.n_chunks * total_steps;
   for (size_t budget : {(size_t)113 * 1024, kMaxDynSmem}) {
     for (int na = 4; na >= 2 && !F.ok; --na)
-      if (conv_smem_resident(P, na, bank) <= budget) { F.ok = 1; F.n_a_slots = na; F.n_b_slots = bank; F.smem = conv_smem_resident(P, na, bank); }
+      if (conv_smem_resident(P, na, bank) <= budget) { F.ok = 1; F.P.n_a_slots = na; F.P.n_b_slots = bank; F.smem = conv_smem_resident(P, na, bank); }
     if (F.ok) break;
   }
-  F.n_tiles = P.n_tiles;
-  if (F.ok) fit(F, kern);
+  F.n_items = P.n_tiles;
+  fit_ctas(h, F, 1);
 }
 
 // The residual ADD right after conv `oi` can run in its epilogue: the conv's output has no other reader (the compiler
@@ -1705,7 +1639,8 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   const int gH = sub > 1 ? ob.H : ib.H, gW = sub > 1 ? ob.W : ib.W;
   TcLaunch L;
   memset(&L, 0, sizeof(L));
-  TcParams& P = L.P;
+  TcForm& F0 = L.forms[0];
+  TcParams& P = F0.P;
   P.H = gH; P.W = gW;
   P.tiles_x = (gW + TW - 1) / TW;
   const int tiles_y = (gH + TH - 1) / TH;
@@ -1739,7 +1674,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   }
   P.split = (m->precision == 2 && !ob.f32) ? 1 : 0;
   P.epi_mode = 0;
-  if (!P.split && !getenv("SB_DISABLE_FAST_EPILOGUE") && !ob.f32 && P.bn_scale == nullptr && Cout % 16 == 0 && plan->Cout_pad == Cout &&
+  if (!P.split && !ob.f32 && P.bn_scale == nullptr && Cout % 16 == 0 && plan->Cout_pad == Cout &&
       ob.C % 16 == 0 && out_coff % 16 == 0 && (P.pool_out == nullptr || (P.pool_Ctot % 16 == 0 && P.pool_coff % 16 == 0)))
     P.epi_mode = 1;                // (a residual slice is 16-byte aligned: res_fusable)
   P.row_bytes = KC * 2;
@@ -1758,8 +1693,10 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
   P.n_b_slots = std::min(4, P.n_chunks * total_steps);
   while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_b_slots > 2) P.n_b_slots--;
   while ((size_t)P.n_a_slots * P.a_slot_bytes + (size_t)P.n_b_slots * P.b_slot_bytes > ring_budget && P.n_a_slots > 2) P.n_a_slots--;
-  L.smem = conv_smem(P, P.n_a_slots, P.n_b_slots);
-  if (L.smem > kMaxDynSmem) return sb_fail(h, SB_ERR_INVALID, "conv tile needs %zu bytes of shared memory", L.smem);
+  F0.ok = 1;
+  F0.threads = kConvThreads;
+  F0.smem = conv_smem(P, P.n_a_slots, P.n_b_slots);
+  if (F0.smem > kMaxDynSmem) return sb_fail(h, SB_ERR_INVALID, "conv tile needs %zu bytes of shared memory", F0.smem);
   L.grid = dim3(P.tiles_x * tiles_y, (plan->Cout_pad + N - 1) / N, 1 /* z = batch, set at launch */);
   // A: NHWC view (slice channels, W, H, batch); pixel and row pitches x sub
   {
@@ -1769,35 +1706,34 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     cuuint32_t es[4] = {1, 1, 1, 1};
     void* gptr = (void*)((__half*)ib.dev + in_coff);
     P.in = gptr; P.in_Ctot = ib.C; P.in_C = Cin;
-    CUresult r = enc(&L.mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, gptr, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = enc(&F0.mapA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, gptr, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A) failed: %d", (int)r);
   }
-  if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, N, &L.mapB); r != CUDA_SUCCESS)
+  if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, N, &F0.mapB); r != CUDA_SUCCESS)
     return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   P.n_tiles = (int)L.grid.x;
   setup_forms(h, L, total_steps);
   if (L.forms[3].ok)
-    if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, L.forms[3].N, &L.forms[3].mapB); r != CUDA_SUCCESS)
+    if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, L.forms[3].P.N, &L.forms[3].mapB); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, wide form) failed: %d", (int)r);
   (dst ? *dst : plan->launches).push_back(L);
   return 0;
 }
 
-// Form 4 of the transposed conv `op`, whose four phase launches are plan->launches: chunks of 64 input channels, N tiles of
-// min(N, 128) channels that cover C_out exactly, the fp16 fast-epilogue shape (so not precision 2), and phases whose taps
-// all lie in one 17-row box (dy0 of -1 or 0, start rows 0 or 1: the k3 and k4 phases); 4 box slots and 4-8 weight slots
-// in 225 KB, one CTA per SM.  Leaves plan->tconv.ok = 0 where the op is not eligible.
-static int tconv_setup(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan) {
-  TcTconv& T = plan->tconv;
-  T.ok = 0;
+// Form 4 of the transposed conv `op`, kept in the first of its four phase launches (plan->launches): chunks of 64 input
+// channels, N tiles of min(N, 128) channels that cover C_out exactly, the fp16 fast-epilogue shape (so not precision 2),
+// and phases whose taps all lie in one 17-row box (dy0 of -1 or 0, start rows 0 or 1: the k3 and k4 phases); 4 box
+// slots and 4-8 weight slots in 225 KB, one CTA per SM.  The form stays ineligible where the op does not qualify.
+static int setup_tconv_form(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan) {
   if (plan->launches.size() != 4) return 0;
-  const TcParams& P0 = plan->launches[0].P;
-  const int N = std::min(P0.N, 128);
-  TconvKernel kern = tconv_kernel(N);
-  if (!kern || P0.KC != 64 || P0.Cout % N) return 0;
+  TcForm& T = plan->launches[0].forms[kTconvForm];      // setup_forms: a copy of the first phase's form 0, not ok
+  const TcParams& P0 = plan->launches[0].forms[0].P;
+  T.threads = kWideThreads;
+  T.P.N = std::min(P0.N, 128);
+  if (!form_kernel(kTconvForm, P0.KC, T.P.N) || P0.Cout % T.P.N) return 0;
   for (int p = 0; p < 4; ++p) {
-    const TcParams& P = plan->launches[p].P;
+    const TcParams& P = plan->launches[p].forms[0].P;
     if (P.epi_mode != 1 || P.n_groups > 2 || P.dy0 < -1 || P.dy0 > 0) return 0;
     T.Q.n_groups[p] = P.n_groups; T.Q.dy0[p] = P.dy0; T.Q.oy_add[p] = P.oy_add; T.Q.ox_add[p] = P.ox_add;
     for (int g = 0; g < P.n_groups; ++g) {
@@ -1806,20 +1742,10 @@ static int tconv_setup(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
       T.Q.groups[p][g] = P.groups[g];
     }
   }
-  T.P = P0;
-  T.P.N = N; T.P.n_a_slots = 4; T.P.skip_out = 0; T.P.pdl_trigger = 0;
-  T.P.n_b_slots = 0;
-  for (int nb = 8; nb >= 4 && !T.P.n_b_slots; --nb)
-    if (tconv_smem(P0, N, 4, nb) <= kMaxDynSmem) T.P.n_b_slots = nb;
-  if (!T.P.n_b_slots) return 0;
-  T.smem = tconv_smem(P0, N, 4, T.P.n_b_slots);
-  int nb = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kWideThreads, T.smem) != cudaSuccess || nb < 1) {
-    cudaGetLastError();
-    return 0;
-  }
-  T.max_ctas = nb * h->sm_count;
-  T.n_units = (P0.Cout / N) * ((P0.W + 15) / 16) * ((P0.H + 15) / 16);
+  fit_weight_ring(T, 4, kTconvBox);
+  T.n_items = 4 * (P0.Cout / T.P.N) * ((P0.W + 15) / 16) * ((P0.H + 15) / 16);   // (phase, N tile, input tile)
+  fit_ctas(h, T, kTconvForm);
+  if (!T.ok) return 0;
   EncodeTiledFn enc = get_encode();
   {
     // the phase launches' activation view (slice channels, W, H, batch) with a [64, 16, 17, 1] box
@@ -1832,9 +1758,8 @@ static int tconv_setup(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(A, fused tconv) failed: %d", (int)r);
   }
-  if (CUresult r = encode_weights(enc, plan, op.in_C(), op.k() * op.k(), 64, N, &T.mapB); r != CUDA_SUCCESS)
+  if (CUresult r = encode_weights(enc, plan, op.in_C(), op.k() * op.k(), 64, T.P.N, &T.mapB); r != CUDA_SUCCESS)
     return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, fused tconv) failed: %d", (int)r);
-  T.ok = 1;
   return 0;
 }
 
@@ -2115,6 +2040,51 @@ int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* f
   return sb_conv_tc_launch(h, m, op_index, B);
 }
 
+// Shared memory of one k_head_1x1 launch: the weight bank, the output staging and the bias, plus a per-warp ring of n_ring
+// staged items (16 pixels x kch channels each), as deep as fits with two blocks per SM, else with one block per SM
+// (kHeadSmem).  n_ring = 0: not even a ring of 2 fits beside the bank (wide inputs with 17-32 outputs), so the op stays
+// on the implicit-GEMM conv kernel.
+constexpr long long kHeadSmem = 200 * 1024;
+struct HeadShape {
+  int nt, kch, n_ring;
+  size_t smem;
+};
+static HeadShape head_shape(const SbOp& op) {
+  HeadShape s;
+  s.nt = (op.out_C() + 7) / 8;
+  s.kch = std::min(op.in_C(), 128);
+  // signed: the bank alone can exceed the two-blocks-per-SM budget
+  const long long fixed = 8LL * s.nt * (op.in_C() + 8) * 2 + 8LL * 16 * (8 * s.nt + 1) * 4 + 8LL * s.nt * 4;
+  const long long stage = 8LL * 16 * (s.kch + 8) * 2;
+  long long n_ring = std::min<long long>(8, (110 * 1024 - fixed) / stage);
+  if (n_ring < 4) n_ring = std::min<long long>(8, (kHeadSmem - fixed) / stage);
+  s.n_ring = n_ring >= 2 ? (int)n_ring : 0;
+  s.smem = (size_t)(fixed + s.n_ring * stage);
+  return s;
+}
+
+// 1x1 fp32 heads on k_head_1x1 (HBM-bound; see the kernel) instead of the implicit-GEMM conv kernel
+static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan) {
+  const SbBuffer& ib = m->buffers[op.in_buf()];
+  const SbBuffer& ob = m->buffers[op.out_buf()];
+  return op.kind() == SB_OPK_CONV && op.k() == 1 && op.stride() == 1 && ob.f32 && !ib.f32 && !(op.flags() & SB_OPF_BN) && op.in_C() % 16 == 0 &&
+         (op.in_C() == 16 || op.in_C() == 32 || op.in_C() == 64 || op.in_C() % 128 == 0) && op.out_C() <= 32 && ib.C % 8 == 0 && op.in_coff() % 8 == 0 && plan->w16 != nullptr && plan->Cout_pad >= (op.out_C() + 7) / 8 * 8 &&
+         (size_t)plan->Cout_pad * (op.in_C() + 8) * 2 <= 160 * 1024 && head_shape(op).n_ring >= 2;
+}
+
+// the k_head_1x1 instantiation for NT x 8 output channels (NT <= 4: head_kernel_ok) and staged chunks of KCH channels
+static const void* head_kernel(int nt, int kch) {
+#define SB_HEAD_CASE(NT)                                                                                                 \
+  case NT:                                                                                                               \
+    return kch == 16 ? (const void*)k_head_1x1<NT, 16> : kch == 32 ? (const void*)k_head_1x1<NT, 32>                     \
+         : kch == 64 ? (const void*)k_head_1x1<NT, 64> : (const void*)k_head_1x1<NT, 128>;
+  switch (nt) {
+    SB_HEAD_CASE(1) SB_HEAD_CASE(2) SB_HEAD_CASE(3) SB_HEAD_CASE(4)
+    default: return nullptr;
+  }
+#undef SB_HEAD_CASE
+}
+
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);
 
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
@@ -2126,11 +2096,9 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   if (!attr_set) {
     for (int f = 0; f < kForms; ++f)
       for (int kc : {16, 32, 64})
-        for (int n : {16, 32, 48, 64, 96, 128, 192, 256})
-          if (ConvKernel k = conv_kernel_form(f, kc, n))
-            SB_CUDA(h, cudaFuncSetAttribute((const void*)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
-    for (int n : {32, 48, 64, 96, 128})
-      SB_CUDA(h, cudaFuncSetAttribute((const void*)tconv_kernel(n), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
+        for (int n : kWgN)
+          if (const void* k = form_kernel(f, kc, n))
+            SB_CUDA(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem));
     attr_set = true;
   }
   for (size_t oi = 0; oi < m->ops.size(); ++oi) {
@@ -2213,13 +2181,18 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
           rc = make_launch(h, m, op, plan, ng, g, a == 0 ? -1 : 0, extra, 9, 2, a, 2, bx);
         }
     }
-    if (!rc && op.kind() == SB_OPK_TCONV) rc = tconv_setup(h, m, op, plan);
+    if (!rc && op.kind() == SB_OPK_TCONV) rc = setup_tconv_form(h, m, op, plan);
     if (rc) { cudaFree(plan->w16); delete plan; return rc; }
     m->tc_plans[oi] = plan;
+    if (head_kernel_ok(m, op, plan)) {
+      const HeadShape hs = head_shape(op);
+      plan->head = head_kernel(hs.nt, hs.kch);
+      SB_CUDA(h, cudaFuncSetAttribute(plan->head, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHeadSmem));
+    }
     if (plan->res_fused) m->skip_op[oi + 1] = 2;
     if (op.kind() == SB_OPK_CONV && op.pool_buf() >= 0 && oi + 1 < m->ops.size() &&
         m->ops[oi + 1].kind() == SB_OPK_POOL && (m->ops[oi + 1].flags() & SB_OPF_FUSED_POOL))
-      if (plan->launches[0].P.pool_out != nullptr) {
+      if (plan->launches[0].forms[0].P.pool_out != nullptr) {
         m->skip_op[oi + 1] = 1;
         // dead-store elimination: with the pool fused, the conv's own output is written only for other readers
         // (skip connections into the decoder, heads).  The two finest encoder blocks of a UNet with output_stride 4
@@ -2235,7 +2208,7 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
                                  op.out_coff() < o2.in2_coff() + o2.in_C();
           read = overl_in || overl_in2;
         }
-        plan->out_dead = !read && !getenv("SB_DISABLE_DEAD_STORE_ELIM");
+        plan->out_dead = !read;
       }
   }
   for (size_t oi = 0; oi + 1 < m->ops.size() && !split; ++oi)   // precision 2: the first conv runs on k_conv_first / k_conv_direct in fp32
@@ -2279,95 +2252,79 @@ bool sb_pdl_on() {
   return v != 0;
 }
 
-static void launch_conv(TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
-  TcParams P = L.P;
+// Launches form L.form of L for B frames (form 4: all four phases of the op).  Form 0 runs one CTA per tile, N tile and
+// frame.  The persistent forms run as many CTAs as fit at once (capped at the work count), without shared-memory padding;
+// each CTA triggers its dependents when it starts its last work item.
+static void launch_form(const TcLaunch& L, int B, cudaStream_t stream, int skip_out) {
+  const TcForm& F = L.forms[L.form];
+  TcParams P = F.P;
   P.skip_out = skip_out;
-  if (L.form != 0) {
-    // persistent: as many CTAs as fit at once (capped at the work count), no shared-memory padding; each CTA triggers its
-    // dependents when it starts its last work item
-    const TcForm& F = L.forms[L.form];
-    P.n_a_slots = F.n_a_slots; P.n_b_slots = F.n_b_slots; P.batch = B; P.pdl_trigger = 0; P.N = F.N;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(std::min(F.n_tiles * B, F.max_ctas)); cfg.blockDim = dim3(F.threads); cfg.dynamicSmemBytes = F.smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
-    cudaLaunchKernelEx(&cfg, conv_kernel_form(L.form, P.KC, P.N), L.mapA, L.form == 3 ? F.mapB : L.mapB, P);
-    return;
+  dim3 grid(std::min(F.n_items * B, F.max_ctas));
+  size_t smem = F.smem;
+  if (L.form == 0) {
+    grid = dim3(L.grid.x, L.grid.y, B);
+    P.pdl_trigger = (sb_pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
+    if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing of the successor fits beside it
+  } else {
+    P.batch = B;
   }
-  size_t smem = L.smem;
-  P.pdl_trigger = (sb_pdl_on() && smem >= 114 * 1024) ? 1 : 0;   // already one CTA per SM
-  if (P.pdl_trigger) smem = std::max(smem, kMaxDynSmem);       // nothing of the successor fits beside it
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(L.grid.x, L.grid.y, B); cfg.blockDim = dim3(kConvThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, conv_kernel(P.KC, P.N), L.mapA, L.mapB, P);
+  void* args[4] = {const_cast<CUtensorMap*>(&F.mapA), const_cast<CUtensorMap*>(&F.mapB), &P, const_cast<TcPhases*>(&F.Q)};
+  sb_launch_pdl(form_kernel(L.form, P.KC, P.N), grid, dim3(F.threads), smem, stream, args);
 }
 
-// form 4: the four phases of a transposed conv in one persistent launch of as many CTAs as fit at once (capped at the work
-// count); each CTA triggers its dependents when it starts its last work item
-static void launch_tconv_fused(const TcTconv& T, int B, cudaStream_t stream) {
-  TcParams P = T.P;
-  P.batch = B;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(std::min(4 * T.n_units * B, T.max_ctas)); cfg.blockDim = dim3(kWideThreads); cfg.dynamicSmemBytes = T.smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, tconv_kernel(P.N), T.mapA, T.mapB, P, T.Q);
-}
-
-static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan);
-
-// Picks, for every tensor-core conv launch (each transposed-conv phase included), the faster eligible kernel form
-// (streaming / resident weights), for a first layer with a Toeplitz view the faster of the view + tensor-core
-// conv and k_conv_first, for a transposed conv its four phase launches or the fused form 4, and for the first encoder
-// block the fused k_conv01 or the separate launches, by timing the
-// forms on the device at the configured batch (buffers are already allocated; their contents do not matter for timing).
+// Picks, for every tensor-core conv launch (each transposed-conv phase included), the fastest eligible kernel form 0-3,
+// for a transposed conv its four phase launches or the fused form 4, for a first layer with a Toeplitz view the faster
+// of the view + tensor-core conv and k_conv_first, and for the first encoder block the fused k_conv01 or the separate
+// launches, by timing them on the device at the configured batch (buffers are already allocated; their contents do not
+// matter for timing).
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   cudaEvent_t e0, e1;
   SB_CUDA(h, cudaEventCreate(&e0));
   SB_CUDA(h, cudaEventCreate(&e1));
+  // the time of run() in ms: 4 synchronised runs, the first dropped, the minimum of the others
+  char what[64];
+  auto time_min = [&](float& best, auto run) -> int {
+    best = 1e30f;
+    for (int rep = 0; rep < 4; ++rep) {
+      cudaEventRecord(e0, h->stream);
+      if (const int rc = run()) return rc;
+      cudaEventRecord(e1, h->stream);
+      cudaError_t e = cudaStreamSynchronize(h->stream);
+      if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (%s) failed: %s", what, cudaGetErrorString(e));
+      float ms = 0.f;
+      cudaEventElapsedTime(&ms, e0, e1);
+      if (rep > 0) best = std::min(best, ms);
+    }
+    return 0;
+  };
   const bool dbg = getenv("SB_DEBUG") != nullptr;
   const char* fvar = getenv("SB_FORCE_VARIANT");
   const int force = fvar ? atoi(fvar) : -1;
-  static const char* const form_name[kForms] = {"streaming", "resident", "halo", "wide"};
+  static const char* const form_name[kForms] = {"streaming", "resident", "halo", "wide", "tconv-fused"};
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
-    if (!plan || head_kernel_ok(m, m->ops[oi], plan)) continue;
+    if (!plan || plan->head) continue;
     for (std::vector<TcLaunch>* list : {&plan->launches, &plan->plain_launches})
       for (size_t li = 0; li < list->size(); ++li) {
         TcLaunch& L = (*list)[li];
-        float best[kForms];
+        float best[kTconvForm];
         int pick = 0;
-        for (int f = 0; f < kForms; ++f) {
+        for (int f = 0; f < kTconvForm; ++f) {
           best[f] = 1e30f;
           if (!L.forms[f].ok) continue;
           L.form = f;
-          for (int rep = 0; rep < 4; ++rep) {
-            cudaEventRecord(e0, h->stream);
-            launch_conv(L, m->B, h->stream, plan->out_dead && list == &plan->launches);
-            cudaEventRecord(e1, h->stream);
-            cudaError_t e = cudaStreamSynchronize(h->stream);
-            if (e != cudaSuccess)
-              return sb_fail(h, SB_ERR_CUDA, "autotune launch (op %zu, %s form) failed: %s", oi, form_name[f], cudaGetErrorString(e));
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, e0, e1);
-            if (rep > 0) best[f] = std::min(best[f], ms);
-          }
+          snprintf(what, sizeof what, "op %zu, %s form", oi, form_name[f]);
+          const int rc = time_min(best[f], [&] {
+            launch_form(L, m->B, h->stream, plan->out_dead && list == &plan->launches);
+            return 0;
+          });
+          if (rc) return rc;
           if (best[f] < best[pick]) pick = f;
         }
-        L.form = (force >= 0 && force < kForms && L.forms[force].ok) ? force : pick;
+        L.form = (force >= 0 && force < kTconvForm && L.forms[force].ok) ? force : pick;
         if (dbg) {
           fprintf(stderr, "[sb_conv_tc] op %zu launch %zu%s:", oi, li, list == &plan->launches ? "" : " (own output)");
-          for (int f = 0; f < kForms; ++f)
+          for (int f = 0; f < kTconvForm; ++f)
             if (L.forms[f].ok) fprintf(stderr, " %s %.1f us", form_name[f], best[f] * 1e3f);
           fprintf(stderr, " -> %s\n", form_name[L.form]);
         }
@@ -2376,71 +2333,50 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   // transposed convs: the four phase launches (whatever forms were just picked for them) against the fused form 4
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
-    if (!plan || !plan->tconv.ok) continue;
-    float best[2] = {1e30f, 1e30f};
+    if (!plan || plan->launches.empty() || !plan->launches[0].forms[kTconvForm].ok) continue;
+    TcLaunch& L0 = plan->launches[0];
+    const int phase_form = L0.form;
+    float best[2];
     for (int f = 0; f < 2; ++f) {
-      plan->tconv_fused = f == 1;
-      for (int rep = 0; rep < 4; ++rep) {
-        cudaEventRecord(e0, h->stream);
-        const int rc = sb_conv_tc_launch(h, m, (int)oi, m->B);
-        if (rc) return rc;
-        cudaEventRecord(e1, h->stream);
-        cudaError_t e = cudaStreamSynchronize(h->stream);
-        if (e != cudaSuccess)
-          return sb_fail(h, SB_ERR_CUDA, "autotune launch (op %zu, %s) failed: %s", oi, f ? "fused tconv" : "tconv phases", cudaGetErrorString(e));
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (rep > 0) best[f] = std::min(best[f], ms);
-      }
+      L0.form = f ? kTconvForm : phase_form;
+      snprintf(what, sizeof what, "op %zu, %s", oi, f ? "fused tconv" : "tconv phases");
+      if (const int rc = time_min(best[f], [&] { return sb_conv_tc_launch(h, m, (int)oi, m->B); })) return rc;
     }
-    plan->tconv_fused = force >= 0 ? force == 4 : best[1] < best[0];
+    L0.form = (force >= 0 ? force == kTconvForm : best[1] < best[0]) ? kTconvForm : phase_form;
     if (dbg)
       fprintf(stderr, "[sb_conv_tc] op %zu launches (4 tconv phases) %.1f us, fused k_tconv_wg_hw %.1f us -> %s\n", oi, best[0] * 1e3f,
-              best[1] * 1e3f, plan->tconv_fused ? "tconv-fused" : "phases");
+              best[1] * 1e3f, L0.form == kTconvForm ? "tconv-fused" : "phases");
   }
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
     SbConvTcPlan* plan = m->tc_plans[oi];
     if (!plan || !plan->view_in || plan->s2d || plan->from_buffer || !m->frames_dev) continue;
-    float best[2] = {1e30f, 1e30f};
-    for (int f = 0; f < 2; ++f)
-      for (int rep = 0; rep < 4; ++rep) {
-        cudaEventRecord(e0, h->stream);
-        const int rc = f == 0 ? sb_first_direct_launch(h, m, (int)oi, m->frames_dev, 1, m->B)
-                              : sb_first_view_launch(h, m, (int)oi, m->frames_dev, 1, m->B);
-        if (rc) return rc;
-        cudaEventRecord(e1, h->stream);
-        cudaError_t e = cudaStreamSynchronize(h->stream);
-        if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (first layer, form %d) failed: %s", f, cudaGetErrorString(e));
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (rep > 0) best[f] = std::min(best[f], ms);
-      }
+    float best[2];
+    for (int f = 0; f < 2; ++f) {
+      snprintf(what, sizeof what, "first layer, form %d", f);
+      const int rc = time_min(best[f], [&] {
+        return f == 0 ? sb_first_direct_launch(h, m, (int)oi, m->frames_dev, 1, m->B)
+                      : sb_first_view_launch(h, m, (int)oi, m->frames_dev, 1, m->B);
+      });
+      if (rc) return rc;
+    }
     plan->view_enabled = best[1] < best[0];
-    if (const char* fv = getenv("SB_FORCE_FIRST_VIEW")) plan->view_enabled = atoi(fv) != 0;
     if (dbg) fprintf(stderr, "[sb_conv_tc] op %zu first layer: k_conv_first %.1f us, Toeplitz view + wgmma %.1f us -> %s\n", oi,
                      best[0] * 1e3f, best[1] * 1e3f, plan->view_enabled ? "view" : "direct");
   }
   // fused first block (k_conv01) against its two separate launches (whatever forms were just picked for them)
   if (m->conv01 && m->frames_dev) {
     const int c1op = sb_conv01_conv1_op(m), c0op = c1op - 1;
-    float best[2] = {1e30f, 1e30f};
-    for (int f = 0; f < 2; ++f)
-      for (int rep = 0; rep < 4; ++rep) {
-        cudaEventRecord(e0, h->stream);
-        int rc = 0;
-        if (f == 1) rc = sb_conv01_launch(h, m, m->frames_dev, 1, m->B);
-        else {
-          rc = sb_first_view_can(m, c0op) ? sb_first_view_launch(h, m, c0op, m->frames_dev, 1, m->B) : sb_first_direct_launch(h, m, c0op, m->frames_dev, 1, m->B);
-          if (!rc) rc = sb_conv_tc_launch(h, m, c1op, m->B);
-        }
-        if (rc) return rc;
-        cudaEventRecord(e1, h->stream);
-        cudaError_t e = cudaStreamSynchronize(h->stream);
-        if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (first block, fused %d) failed: %s", f, cudaGetErrorString(e));
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        if (rep > 0) best[f] = std::min(best[f], ms);
-      }
+    float best[2];
+    for (int f = 0; f < 2; ++f) {
+      snprintf(what, sizeof what, "first block, fused %d", f);
+      const int rc = time_min(best[f], [&] {
+        if (f == 1) return sb_conv01_launch(h, m, m->frames_dev, 1, m->B);
+        const int rc0 = sb_first_view_can(m, c0op) ? sb_first_view_launch(h, m, c0op, m->frames_dev, 1, m->B)
+                                                   : sb_first_direct_launch(h, m, c0op, m->frames_dev, 1, m->B);
+        return rc0 ? rc0 : sb_conv_tc_launch(h, m, c1op, m->B);
+      });
+      if (rc) return rc;
+    }
     m->conv01_enabled = best[1] < best[0];
     if (const char* fv = getenv("SB_FORCE_CONV01")) m->conv01_enabled = atoi(fv) != 0;
     if (dbg) fprintf(stderr, "[sb_conv_tc] first block (B = %d): conv0 + conv1 launches %.1f us, fused k_conv01 %.1f us -> %s\n", m->B,
@@ -2451,95 +2387,40 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
-// Shared memory of one k_head_1x1 launch: the weight bank, the output staging and the bias, plus a per-warp ring of n_ring
-// staged items (16 pixels x kch channels each), as deep as fits with two blocks per SM, else with one block per SM
-// (kHeadSmem).  n_ring = 0: not even a ring of 2 fits beside the bank (wide inputs with 17-32 outputs), so the op stays
-// on the implicit-GEMM conv kernel.
-constexpr long long kHeadSmem = 200 * 1024;
-struct HeadShape {
-  int nt, kch, n_ring;
-  size_t smem;
-};
-static HeadShape head_shape(const SbOp& op) {
-  HeadShape s;
-  s.nt = (op.out_C() + 7) / 8;
-  s.kch = std::min(op.in_C(), 128);
-  // signed: the bank alone can exceed the two-blocks-per-SM budget
-  const long long fixed = 8LL * s.nt * (op.in_C() + 8) * 2 + 8LL * 16 * (8 * s.nt + 1) * 4 + 8LL * s.nt * 4;
-  const long long stage = 8LL * 16 * (s.kch + 8) * 2;
-  long long n_ring = std::min<long long>(8, (110 * 1024 - fixed) / stage);
-  if (n_ring < 4) n_ring = std::min<long long>(8, (kHeadSmem - fixed) / stage);
-  s.n_ring = n_ring >= 2 ? (int)n_ring : 0;
-  s.smem = (size_t)(fixed + s.n_ring * stage);
-  return s;
-}
-
-// 1x1 fp32 heads on k_head_1x1 (HBM-bound; see the kernel) instead of the implicit-GEMM conv kernel.  SB_DISABLE_HEAD_KERNEL=1 reverts.
-static bool head_kernel_ok(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan) {
-  if (getenv("SB_DISABLE_HEAD_KERNEL")) return false;
-  const SbBuffer& ib = m->buffers[op.in_buf()];
-  const SbBuffer& ob = m->buffers[op.out_buf()];
-  return op.kind() == SB_OPK_CONV && op.k() == 1 && op.stride() == 1 && ob.f32 && !ib.f32 && !(op.flags() & SB_OPF_BN) && op.in_C() % 16 == 0 &&
-         (op.in_C() == 16 || op.in_C() == 32 || op.in_C() == 64 || op.in_C() % 128 == 0) && op.out_C() <= 32 && ib.C % 8 == 0 && op.in_coff() % 8 == 0 && plan->w16 != nullptr && plan->Cout_pad >= (op.out_C() + 7) / 8 * 8 &&
-         (size_t)plan->Cout_pad * (op.in_C() + 8) * 2 <= 160 * 1024 && head_shape(op).n_ring >= 2;
-}
-
 static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int B) {
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
   const HeadShape hs = head_shape(op);
-  const int nt = hs.nt, kch = hs.kch, n_ring = hs.n_ring;
-  const size_t smem = hs.smem;
-  const size_t npix = (size_t)B * ob.H * ob.W;
+  int n_ring = hs.n_ring;
+  size_t npix = (size_t)B * ob.H * ob.W;
   if (!plan->head_logged && getenv("SB_DEBUG")) {
-    fprintf(stderr, "[sb_conv_tc] head k_head_1x1: Cin %d Cout %d NT %d KCH %d n_ring %d smem %zu\n", op.in_C(), op.out_C(), nt, kch,
-            n_ring, smem);
+    fprintf(stderr, "[sb_conv_tc] head k_head_1x1: Cin %d Cout %d NT %d KCH %d n_ring %d smem %zu\n", op.in_C(), op.out_C(), hs.nt,
+            hs.kch, n_ring, hs.smem);
     plan->head_logged = true;
   }
+  const __half* in = (const __half*)ib.dev;
+  const __half* w = plan->w16;
   const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-  const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
+  float* out = (float*)ob.dev;
+  int in_Ctot = ib.C, in_coff = op.in_coff(), Cin = op.in_C(), out_Ctot = ob.C, out_coff = op.out_coff(), Cout = op.out_C();
+  int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
+  void* args[] = {&in, &in_Ctot, &in_coff, &Cin, &w, &bias, &out, &out_Ctot, &out_coff, &Cout, &relu, &npix, &n_ring};
   const int grid = (int)std::min<size_t>((npix + 127) / 128, (size_t)h->sm_count * 2);
-#define SB_HEAD_LAUNCH(NT, KC)                                                                                                  \
-  {                                                                                                                             \
-    static bool attr = false;                                                                                                   \
-    if (!attr) { SB_CUDA(h, cudaFuncSetAttribute((k_head_1x1<NT, KC>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHeadSmem)); attr = true; } \
-    cudaLaunchConfig_t cfg = {};                                                                                                \
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = smem; cfg.stream = h->stream;                    \
-    cudaLaunchAttribute at[1];                                                                                                  \
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;        \
-    cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;                                                                            \
-    cudaLaunchKernelEx(&cfg, k_head_1x1<NT, KC>, (const __half*)ib.dev, ib.C, op.in_coff(), op.in_C(), (const __half*)plan->w16, bias,        \
-                       (float*)ob.dev, ob.C, op.out_coff(), op.out_C(), relu, npix, n_ring);                                    \
-  }
-#define SB_HEAD_CASE(NT)                                                                                                        \
-  case NT:                                                                                                                      \
-    if (kch == 16) SB_HEAD_LAUNCH(NT, 16) else if (kch == 32) SB_HEAD_LAUNCH(NT, 32) else if (kch == 64) SB_HEAD_LAUNCH(NT, 64)   \
-    else SB_HEAD_LAUNCH(NT, 128)                                                                                                \
-    break;
-  switch (nt) {
-    SB_HEAD_CASE(1) SB_HEAD_CASE(2) SB_HEAD_CASE(3) SB_HEAD_CASE(4)
-    default: return sb_fail(h, SB_ERR_INVALID, "head kernel: %d output channels", op.out_C());
-  }
-#undef SB_HEAD_CASE
-#undef SB_HEAD_LAUNCH
+  sb_launch_pdl(plan->head, dim3(grid), dim3(256), hs.smem, h->stream, args);
   SB_CHECK_LAUNCH(h);
   return 0;
 }
 
 int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
   SbConvTcPlan* plan = m->tc_plans[op_index];
-  if (head_kernel_ok(m, m->ops[op_index], plan)) return head_launch(h, m, m->ops[op_index], plan, B);
-  if (plan->tconv_fused) {
-    launch_tconv_fused(plan->tconv, B, h->stream);
-    SB_CHECK_LAUNCH(h);
-    return 0;
-  }
+  if (plan->head) return head_launch(h, m, m->ops[op_index], plan, B);
   const int skip = plan->out_dead && !m->keep_dead_stores;
   // the sub-pixel phases of a transposed conv run back to back on the launching stream: under programmatic dependent
-  // launch each phase's CTAs start as the previous phase's SMs drain
+  // launch each phase's CTAs start as the previous phase's SMs drain.  Form 4 runs all four phases in the first launch.
   for (TcLaunch& L : (plan->res_fused && m->keep_dead_stores) ? plan->plain_launches : plan->launches) {
-    launch_conv(L, B, h->stream, skip);
+    launch_form(L, B, h->stream, skip);
     SB_CHECK_LAUNCH(h);
+    if (L.form == kTconvForm) break;
   }
   return 0;
 }

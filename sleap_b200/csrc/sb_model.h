@@ -166,3 +166,15 @@ int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
 
 // programmatic dependent launch for the conv kernels (sb_conv_tc.cu); SB_DISABLE_PDL=1 switches it off
 bool sb_pdl_on();
+
+// Launches `kernel` (args: pointers to its arguments, as for cudaLaunchKernelExC) with programmatic stream
+// serialization while sb_pdl_on(): its CTAs may start while the kernel before it on the stream drains.
+inline cudaError_t sb_launch_pdl(const void* kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t stream, void** args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at; cfg.numAttrs = sb_pdl_on() ? 1 : 0;
+  return cudaLaunchKernelExC(&cfg, kernel, args);
+}

@@ -287,72 +287,43 @@ def test_tc_path_matches_direct_fp16(monkeypatch):
     assert launches_tc > 0
 
 
-@pytest.mark.parametrize("fused", [None, "0", "1", "2"])
+@pytest.mark.parametrize("variant", [None, "0", "1", "2", "4"])
 @pytest.mark.parametrize("cin,cout", [(16, 16), (64, 32), (128, 64), (256, 128), (512, 256)])
-def test_tc_tconv_layers(cin, cout, fused, monkeypatch):
-    """Conv2DTranspose(k3, s2) on the tensor cores as four sub-pixel phase launches, against the CUDA-core kernel on the
-    same fp16 activations.  The variant / fused-form settings of the parameters select nothing on sm_90a (one kernel
-    form): every case runs the phase launches."""
-    from sleap_b200.nn import oplist as ol
-    from sleap_b200 import _lib
-    from ctypes import c_int, c_void_p, byref
-    rng = np.random.default_rng(cin * 3 + cout)
-    B, H, W = 2, 88, 72            # tconv input grid 44 x 36 -> output 88 x 72
-    recs = [ol.buffer_record(0, 1, 1, 0, 1), ol.buffer_record(1, 1, cin, 0, 0), ol.buffer_record(2, 2, cin, 0, 0),
-            ol.buffer_record(3, 1, cout, 0, 0), ol.preprocess_record(0, 1, 1.0, 2)]   # fp16 output (the CUDA-core tconv writes halves)
-    w0 = (rng.standard_normal((3, 3, 1, cin)) * 0.5).astype(np.float32)
-    b0 = rng.normal(0, 0.1, cin).astype(np.float32)
-    w1 = (rng.standard_normal((3, 3, cin, cout)) * np.sqrt(2.0 / (4 * cin))).astype(np.float32)
-    b1 = rng.normal(0, 0.1, cout).astype(np.float32)
-    blob = np.concatenate([w0.reshape(-1), b0, w1.reshape(-1), b1]).astype(np.float32)
-    o0, o1 = 0, w0.size + cin
-    recs.append(ol.conv_record(0, 0, 1, 1, 0, cin, 3, 1, True, o0, o0 + w0.size))
-    recs.append(ol.pool_record(1, 0, cin, 2, 0))
-    recs.append(ol.tconv_record(2, 0, cin, 3, 0, cout, o1, o1 + w1.size))
-    ops = np.ascontiguousarray(np.stack(recs).astype(np.int32))
-    imgs = rng.uniform(0, 1, size=(B, H, W, 1)).astype(np.float32)
-
-    def run():
-        h = _lib.default_handle()
-        mid = c_int(-1)
-        h.call("sb_load_model", _lib.ptr(ops), ops.shape[0], _lib.ptr(blob), int(blob.size), 0, byref(mid))
-        h.call("sb_model_configure", mid.value, B, H, W, 1)
-        out = np.zeros((B, H, W, cout), np.float32)
-        ids = np.asarray([3], np.int32)
-        ptrs = (c_void_p * 1)(out.ctypes.data)
-        h.call("sb_model_forward", mid.value, _lib.ptr(imgs), 0, B, 1, _lib.ptr(ids), ptrs)
-        return out
-
-    if fused is not None:
-        monkeypatch.setenv("SB_FORCE_VARIANT", "2")
-        if fused in ("1", "2"):
-            monkeypatch.setenv("SB_FORCE_FUSED_TCONV", fused)
-    got = run()
+def test_tc_tconv_layers(cin, cout, variant, monkeypatch):
+    """Conv2DTranspose(k3, s2) on the tensor cores, against the CUDA-core kernel on the same fp16 activations, with
+    SB_FORCE_VARIANT = variant: None autotuned; 0 / 1 the four sub-pixel phase launches in the streaming / resident form
+    (a phase the form does not take stays autotuned); 2 the phase launches in their autotuned forms (no phase takes the
+    halo form); 4 the fused form where it is eligible."""
+    from conv_forms import tconv_layer
+    layer = tconv_layer(cin, cout, (88, 72), 2)          # tconv input grid 44 x 36 -> output 88 x 72, fp16
+    if variant is not None:
+        monkeypatch.setenv("SB_FORCE_VARIANT", variant)
+    got = layer()[0]
     monkeypatch.delenv("SB_FORCE_VARIANT", raising=False)
-    monkeypatch.delenv("SB_FORCE_FUSED_TCONV", raising=False)
     monkeypatch.setenv("SB_DISABLE_TC", "1")
-    want = run()
+    want = layer()[0]
     assert np.abs(want).max() > 0.1
     assert_allclose(got, want, atol=3e-3 * max(1.0, np.abs(want).max()), rtol=3e-3)
 
 
-@pytest.mark.parametrize("variant,fused", [("2", None), ("3", None), ("4", None), ("5", None), ("2", "1")])
-def test_tc_forced_variants_unet(variant, fused, monkeypatch):
-    """The whole fp16 UNet (transposed-conv phases, fused max-pool, concat-by-slice outputs) with each
-    SB_FORCE_VARIANT / SB_FORCE_FUSED_TCONV setting of the parameters, against the CUDA-core path.  On sm_90a there is
-    one kernel form, so the settings select nothing and the runs are identical."""
+@pytest.mark.parametrize("variant,no_first_view", [("2", None), ("3", None), ("4", None), ("5", None), ("2", "1")])
+def test_tc_forced_variants_unet(variant, no_first_view, monkeypatch):
+    """The whole fp16 UNet (transposed convs, fused max-pool, concat-by-slice outputs) with SB_FORCE_VARIANT = variant,
+    against the CUDA-core path: 2 / 3 the halo / wide form wherever it is eligible and the phase launches; 4 the autotuned
+    launch forms and the fused transposed convs; 5 the autotuned launch forms and the phase launches.  no_first_view:
+    SB_DISABLE_FIRST_VIEW, so the first layer runs on k_conv_first instead of its Toeplitz view (None: autotuned)."""
     cfg = dict(filters=32, filters_rate=2, max_stride=8, output_stride=2, middle_block=True, up_interpolate=False)
     heads = [dict(name="MultiInstanceConfmapsHead", channels=13, output_stride=2),
              dict(name="PartAffinityFieldsHead", channels=24, output_stride=4)]
     spec = _unet_spec(cfg, heads)
     imgs = np.random.default_rng(12).integers(0, 256, size=(2, 288, 304, 1), dtype=np.uint8)
     monkeypatch.setenv("SB_FORCE_VARIANT", variant)
-    if fused:
-        monkeypatch.setenv("SB_FORCE_FUSED_TCONV", fused)
+    if no_first_view:
+        monkeypatch.setenv("SB_DISABLE_FIRST_VIEW", no_first_view)
     tc_model, w, cm = _mk(spec, 1, 17, precision=0)
     got_tc = tc_model.forward(imgs)
     monkeypatch.delenv("SB_FORCE_VARIANT")
-    monkeypatch.delenv("SB_FORCE_FUSED_TCONV", raising=False)
+    monkeypatch.delenv("SB_DISABLE_FIRST_VIEW", raising=False)
     monkeypatch.setenv("SB_DISABLE_TC", "1")
     dm, _, _ = _mk(spec, 1, 17, precision=0)
     got_direct = dm.forward(imgs)
@@ -370,54 +341,33 @@ def test_tc_forced_variants_unet(variant, fused, monkeypatch):
                                            (32, 32, 5, (40, 48)), (64, 48, 7, (53, 70)), (128, 64, 5, (40, 48)), (16, 16, 7, (40, 48)),
                                            (192, 384, 3, (10, 10)), (384, 384, 3, (5, 7)), (64, 64, 3, (12, 20)), (96, 24, 1, (3, 3))])
 def test_tc_single_layers(cin, cout, k, hw, variant, monkeypatch):
-    _tc_single_layer(cin, cout, k, hw, variant, monkeypatch)
-
-
-def _tc_single_layer(cin, cout, k, hw, variant, monkeypatch):
-    """Each swizzle mode / chunk count / N-tile shape of the tensor-core conv on its own.  A forced variant
-    (SB_FORCE_VARIANT) that does not exist -- on sm_90a there is one kernel form -- runs that kernel."""
+    """Each swizzle mode / chunk count / N-tile shape of the tensor-core conv on its own, autotuned (None) and with each
+    launch form 0-3 forced (SB_FORCE_VARIANT; a form that is not eligible for the layer leaves it autotuned).  4 (the
+    fused transposed conv) and 5-9 name no launch form of a conv: the layer must run its autotuned forms."""
     if variant is not None:
         monkeypatch.setenv("SB_FORCE_VARIANT", variant)
     import torch
     import torch.nn.functional as F
-    from sleap_b200.nn import oplist as ol
+    from ctypes import byref, c_int, c_void_p
     from sleap_b200 import _lib
-    from ctypes import c_int, c_void_p, byref
-    rng = np.random.default_rng(cin + cout)
-    B, (H, W) = 2, hw
-    # op-list: input(1ch) -> conv3x3 1->cin (direct, relu) -> [layer under test] (f32 out)
-    recs = [ol.buffer_record(0, 1, 1, 0, 1), ol.buffer_record(1, 1, cin, 0, 0), ol.buffer_record(2, 1, cout, 1, 0),
-            ol.preprocess_record(0, 1, 1.0, 1)]
-    w0 = (rng.standard_normal((3, 3, 1, cin)) * 0.5).astype(np.float32)
-    b0 = rng.normal(0, 0.1, cin).astype(np.float32)
-    w1 = (rng.standard_normal((k, k, cin, cout)) * np.sqrt(2.0 / (k * k * cin))).astype(np.float32)
-    b1 = rng.normal(0, 0.1, cout).astype(np.float32)
-    blob = np.concatenate([w0.reshape(-1), b0, w1.reshape(-1), b1]).astype(np.float32)
-    o0, o1 = 0, w0.size + cin
-    recs.append(ol.conv_record(0, 0, 1, 1, 0, cin, 3, 1, True, o0, o0 + w0.size))
-    recs.append(ol.conv_record(1, 0, cin, 2, 0, cout, k, 1, False, o1, o1 + w1.size))
-    ops = np.ascontiguousarray(np.stack(recs).astype(np.int32))
-    h = _lib.default_handle()
-    mid = c_int(-1)
-    h.call("sb_load_model", _lib.ptr(ops), ops.shape[0], _lib.ptr(blob), int(blob.size), 0, byref(mid))
-    h.call("sb_model_configure", mid.value, B, H, W, 1)
-    imgs = rng.uniform(0, 1, size=(B, H, W, 1)).astype(np.float32)
-    mids = np.zeros((B, H, W, cin), np.float32)
-    outs = np.zeros((B, H, W, cout), np.float32)
-    ids = np.asarray([1, 2], np.int32)
-    ptrs = (c_void_p * 2)(mids.ctypes.data, outs.ctypes.data)
-    h.call("sb_model_forward", mid.value, _lib.ptr(imgs), 0, B, 2, _lib.ptr(ids), ptrs)
-    # the layer must have run on the tensor-core path (kind 1 in the per-op profile), not on the CUDA-core fallback
-    dev = torch.zeros((B, H, W, 1), dtype=torch.uint8, device="cuda")
-    op_ms = np.zeros(16, np.float32); op_kind = np.zeros(16, np.int32); op_fl = np.zeros(16, np.float64)
-    n_ops = c_int(0)
-    h.call("sb_model_profile_ops", mid.value, c_void_p(dev.data_ptr()), B, 16, _lib.ptr(op_ms), _lib.ptr(op_kind), _lib.ptr(op_fl),
-           byref(n_ops))
-    assert op_kind[n_ops.value - 1] == 1, list(op_kind[:n_ops.value])
+    from conv_forms import conv_layer
+    layer = conv_layer(cin, cout, hw, 2, k=k, relu=False, f32_out=True)
+    B, H, W, _ = layer.imgs.shape
+
+    def op_kinds(h, mid):
+        """the per-op profile's kinds: the layer must run on the tensor-core path (kind 1), not on the CUDA-core fallback"""
+        dev = torch.zeros((B, H, W, 1), dtype=torch.uint8, device="cuda")
+        op_ms = np.zeros(16, np.float32); op_kind = np.zeros(16, np.int32); op_fl = np.zeros(16, np.float64)
+        n_ops = c_int(0)
+        h.call("sb_model_profile_ops", mid, c_void_p(dev.data_ptr()), B, 16, _lib.ptr(op_ms), _lib.ptr(op_kind), _lib.ptr(op_fl),
+               byref(n_ops))
+        return list(op_kind[:n_ops.value])
+    (mids, outs), kinds = layer.run(ids=[1, 2], probe=op_kinds)
+    assert kinds[-1] == 1, kinds
     # reference from the *device's* fp16 intermediate so only this layer is under test
     x = torch.from_numpy(mids).permute(0, 3, 1, 2)
-    w16 = torch.from_numpy(w1.astype(np.float16).astype(np.float32)).permute(3, 2, 0, 1)
-    y = F.conv2d(x, w16, torch.from_numpy(b1), padding=k // 2).permute(0, 2, 3, 1).numpy()
+    w16 = torch.from_numpy(layer.w1.astype(np.float16).astype(np.float32)).permute(3, 2, 0, 1)
+    y = F.conv2d(x, w16, torch.from_numpy(layer.b1), padding=k // 2).permute(0, 2, 3, 1).numpy()
     assert_allclose(outs, y, atol=2e-3 * max(1.0, np.abs(y).max()), rtol=2e-3)
 
 
