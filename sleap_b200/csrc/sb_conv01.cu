@@ -7,20 +7,22 @@
 // pad to the stride) and the Keras layers stack0_enc0_conv0/act0, conv1/act1 and the pool of enc1
 // (sleap/nn/architectures/encoder_decoder.py:94-144, unet.py:140-205), as dispatched to cuDNN by TensorFlow.
 //
-// Persistent: one CTA per SM (as many as fit) walks a static list of (32x16-pixel tile of conv1's output, frame) items.
-// The conv1 bank, this thread's conv0 weights and both biases are loaded once, before the grid-dependency wait.  Per item:
-//   1. the 20x36 frame patch around the tile, fetched into registers one item ahead and stored to shared memory as
-//      fp16-rounded pixels (zero outside the frame), double-buffered;
-//   2. conv0 on the CUDA cores for the 18x34 pixels conv1 reads, each written once as fp16 into two non-swizzled 8-channel
-//      planes [18][34][8] (16 bytes per pixel), double-buffered;
-//   3. conv1 as 4 blocks of 8x8 pixels per warpgroup, each nine wgmma m64n16k16.  In the planes every filter tap of a block
-//      is the same operand at start offset (ky * 34 + kx) * 16 bytes (LBO = plane, SBO = one pixel row), so conv0's output
-//      needs no per-tap copies.  The wgmma run asynchronously while the same warps compute conv0 of the next item;
-//   4. bias, ReLU, fp16 rounding and the 2x2 max in registers: a thread's two accumulator rows are vertically adjacent
-//      pixels, the horizontal partner is lane ^ 4.  Each warp store writes four whole pooled pixels (128 bytes).
+// Persistent and warp-specialized: one CTA per SM (as many as fit) walks a static list of (64x16-pixel tile of conv1's
+// output, frame) items.  The conv1 bank, the conv0 weights and both biases are loaded once, before the grid-dependency
+// wait.  Two roles hand conv0's output over through a ring of NSLOT plane slots with full / empty mbarriers:
+//   * conv0 warpgroups (0, 1), on the CUDA cores: the 20x68 frame patch around the next item is fetched into registers
+//     one item ahead and stored to shared memory as fp16-rounded pixels (zero outside the frame), double-buffered; conv0
+//     for the 18x66 pixels conv1 reads is written once as fp16 into the slot's two non-swizzled 8-channel planes
+//     [18][66][8] (16 bytes per pixel).  A named barrier among these 256 threads orders the patch buffers.
+//   * the MMA warpgroup (2): conv1 as register-A wgmma over image rows.  An m64 block is the item's 64 pixels of one
+//     output row.  Per plane row r, each warp loads three A fragments with ldmatrix.x4 (one per kx: +16 bytes on the row
+//     addresses); each fragment feeds the ky = 0, 1, 2 taps of output rows r, r - 1, r - 2, whose accumulators rotate
+//     through four sets.  Every A element is read from shared memory once, not once per tap.  Bias, ReLU, fp16 rounding
+//     and the 2x2 max in registers: an even row's half2 values wait in registers for the odd row; the horizontal partner
+//     is lane ^ 4.  Each warp store writes four whole pooled pixels (128 bytes).
 // The same rounding points as the separate launches (fp16 frame pixels and weights, fp16 intermediate, fp16 conv1
-// output before the pool), the same conv0 fma order and the same wgmma tap order and operands: results are bit-identical
-// to the one-tile-per-CTA form this replaces.
+// output before the pool), the same conv0 fma order, and every output pixel gets its nine wgmma products in (ky, kx)
+// order on the same operand values as before: results are bit-identical to the 32x16 shared-A form this replaces.
 #include <cuda.h>
 
 #include <algorithm>
@@ -31,20 +33,25 @@ namespace {
 
 #include "sb_tc_prims.cuh"
 
-constexpr int TW = 32, TH = 16;             // conv1 outputs per work item
-constexpr int NBX = TW / 8;                 // 8x8-pixel blocks per warpgroup and item
+constexpr int TW = 64, TH = 16;             // conv1 outputs per work item; TW = one wgmma M block
 constexpr int CW0 = TW + 2, CH0 = TH + 2;   // conv0 pixels conv1 reads
 constexpr int PW = TW + 4, PH = TH + 4;     // frame patch
 constexpr int N_PATCH = PW * PH;
 constexpr int N_C0 = CW0 * CH0;
-constexpr int PATCH_PER_THREAD = (N_PATCH + 255) / 256;
-constexpr int C0_PER_THREAD = (N_C0 + 127) / 128;   // two threads per pixel, one per 8-channel half
+constexpr int N_CONV0 = 256;                // conv0 threads (warpgroups 0, 1); the MMA warpgroup follows
+constexpr int N_THREADS = N_CONV0 + 128;
+constexpr int PATCH_PER_THREAD = (N_PATCH + N_CONV0 - 1) / N_CONV0;
+constexpr int C0_PER_THREAD = (N_C0 + N_CONV0 / 2 - 1) / (N_CONV0 / 2);   // two threads per pixel, one per 8-channel half
 constexpr int PLANE = N_C0 * 16;            // one 8-channel plane [CH0][CW0][8] fp16
+constexpr int NSLOT = 3;                    // conv0 -> conv1 ring
 
 constexpr int OFF_W1 = 0;                               // 9 taps x [16 co][16 ci] fp16, 32-byte swizzle
-constexpr int OFF_A = OFF_W1 + 9 * 512;                 // 2 buffers x 2 planes
-constexpr int OFF_PATCH = OFF_A + 4 * PLANE;            // 2 buffers x [PH][PW] fp32
-constexpr int SMEM_BYTES = OFF_PATCH + 2 * N_PATCH * 4 + 1024;
+constexpr int OFF_A = OFF_W1 + 9 * 512;                 // NSLOT slots x 2 planes
+constexpr int OFF_PATCH = OFF_A + NSLOT * 2 * PLANE;    // 2 buffers x [PH][PW] fp32
+constexpr int OFF_BAR = OFF_PATCH + 2 * N_PATCH * 4;    // NSLOT full + NSLOT empty mbarriers
+constexpr int SMEM_BYTES = OFF_BAR + 2 * NSLOT * 8 + 1024;
+// plane stores of a quarter warp (4 pixels x 2 planes) and ldmatrix phases (8 consecutive pixels) are conflict-free
+static_assert(PLANE % 128 == 64, "the two planes of a pixel must sit in different bank halves");
 
 struct C01Params {
   const void* frames;
@@ -62,167 +69,217 @@ struct C01Params {
 // byte offset of 16-byte chunk c of row r in a 32-byte-swizzled K-major tile (chunk bit 4 ^= address bit 7)
 __device__ __forceinline__ int sw32(int r, int c) { return r * 32 + ((c ^ ((r >> 2) & 1)) << 4); }
 
+__device__ __forceinline__ void conv0_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(N_CONV0) : "memory"); }
+
 template <typename TI>
-__global__ void __launch_bounds__(256, 1) k_conv01(const __grid_constant__ C01Params P) {
+__global__ void __launch_bounds__(N_THREADS, 1) k_conv01(const __grid_constant__ C01Params P) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte aligned by offsetting the array itself, so that the compiler keeps every access in the shared window
   uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* s_patch = reinterpret_cast<float*>(base + OFF_PATCH);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int tid = threadIdx.x;
   const int n_items = P.n_tiles * P.batch, G = gridDim.x;
+  const uint32_t full0 = smem_u32(base + OFF_BAR), empty0 = full0 + 8 * NSLOT;
 
-  // static operands, loaded while the predecessor drains: the conv1 bank to shared memory; this thread's conv0 channel
-  // half (fixed: 256 threads, two per pixel) with its bias, and its conv1 output channels' biases to registers
-  for (int i = tid; i < 9 * 16 * 2; i += 256) {        // 9 taps x 16 rows x 2 chunks
+  // static operands, loaded while the predecessor drains
+  for (int i = tid; i < 9 * 16 * 2; i += N_THREADS) {   // conv1 bank: 9 taps x 16 rows x 2 chunks
     const int t = i >> 5, r = (i >> 1) & 15, c = i & 1;
     *reinterpret_cast<uint4*>(base + OFF_W1 + t * 512 + sw32(r, c)) = reinterpret_cast<const uint4*>(P.w1t + (t * 16 + r) * 16)[c];
   }
-  const int hc = tid & 1;
-  float w0[9][8], b0[8], b1[2][2];
+  if (tid == 0)
+    for (int s = 0; s < NSLOT; ++s) {
+      mbar_init(full0 + 8 * s, N_CONV0);
+      mbar_init(empty0 + 8 * s, 128);
+    }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the conv1 bank -> visible to wgmma
+  __syncthreads();
+
+  if (tid < N_CONV0) {
+    // ---- conv0 warpgroups: frame patch and conv0 of every item of this CTA into the plane ring ----
+    const int hc = tid & 1;                             // this thread's 8-channel half (fixed: two threads per pixel)
+    float w0[9][8], b0[8];
 #pragma unroll
-  for (int t = 0; t < 9; ++t)
+    for (int t = 0; t < 9; ++t)
 #pragma unroll
-    for (int c = 0; c < 8; ++c) w0[t][c] = P.w0h[t * 16 + 8 * hc + c];
+      for (int c = 0; c < 8; ++c) w0[t][c] = P.w0h[t * 16 + 8 * hc + c];
 #pragma unroll
-  for (int c = 0; c < 8; ++c) b0[c] = P.bias0 ? P.bias0[8 * hc + c] : 0.f;
-  const int fc = 2 * (lane & 3);
+    for (int c = 0; c < 8; ++c) b0[c] = P.bias0 ? P.bias0[8 * hc + c] : 0.f;
+    float* s_patch = reinterpret_cast<float*>(base + OFF_PATCH);
+    griddep_wait();                                     // frames belong to the stream's order
+
+    const float sc = P.frames_u8 ? (1.0f / 255.0f) : 1.0f;     // ensure_float (normalization.py:34-49)
+    TI pf[PATCH_PER_THREAD];
+    auto fetch = [&](int w) {                           // frame patch of item w -> registers (zero outside the frame)
+      const int tile = w % P.n_tiles, b = w / P.n_tiles;
+      const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+      const TI* img = reinterpret_cast<const TI*>(P.frames) + (size_t)b * P.Hin * P.Win;
+#pragma unroll
+      for (int k = 0; k < PATCH_PER_THREAD; ++k) {
+        const int e = tid + N_CONV0 * k;
+        const int y = y0 - 2 + e / PW, x = x0 - 2 + e % PW;
+        pf[k] = (w < n_items && e < N_PATCH && y >= 0 && y < P.Hin && x >= 0 && x < P.Win) ? img[(size_t)y * P.Win + x] : TI(0);
+      }
+    };
+    auto stash = [&](float* dst) {
+#pragma unroll
+      for (int k = 0; k < PATCH_PER_THREAD; ++k)
+        if (tid + N_CONV0 * k < N_PATCH) dst[tid + N_CONV0 * k] = __half2float(__float2half_rn(__fmul_rn((float)pf[k], sc)));
+    };
+    // conv0 for the CH0 x CW0 pixels conv1 reads, 8 channels per thread; zero outside the network image (conv1's SAME pad)
+    auto conv0 = [&](const float* patch, uint8_t* A, int x0, int y0) {
+#pragma unroll 1
+      for (int k = 0; k < C0_PER_THREAD; ++k) {
+        const int p = (tid >> 1) + (N_CONV0 / 2) * k;
+        if (p >= N_C0) break;
+        const int yy = p / CW0, cx = p % CW0;
+        const int y = y0 - 1 + yy, x = x0 - 1 + cx;
+        uint32_t q[4] = {0u, 0u, 0u, 0u};               // fp16 +0 outside
+        if (y >= 0 && y < P.Hnet && x >= 0 && x < P.Wnet) {
+          float acc[8];
+#pragma unroll
+          for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+#pragma unroll
+          for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+            for (int kx = 0; kx < 3; ++kx) {
+              const float v = patch[(yy + ky) * PW + cx + kx];
+#pragma unroll
+              for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, w0[ky * 3 + kx][c], acc[c]);
+            }
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            acc[c] += b0[c];
+            if (P.relu0) acc[c] = fmaxf(acc[c], 0.f);
+          }
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const __half2 t = __floats2half2_rn(acc[2 * c], acc[2 * c + 1]);
+            q[c] = *reinterpret_cast<const uint32_t*>(&t);
+          }
+        }
+        *reinterpret_cast<uint4*>(A + hc * PLANE + p * 16) = make_uint4(q[0], q[1], q[2], q[3]);
+      }
+    };
+
+    int w = blockIdx.x;
+    fetch(w);
+    stash(s_patch);
+    fetch(w + G);
+    conv0_bar_sync();
+    for (int k = 0; w < n_items; ++k, w += G) {
+      if (w + G >= n_items) griddep_launch();           // last item of this CTA
+      const int slot = k % NSLOT, use = k / NSLOT;
+      if (use > 0) mbar_wait(empty0 + 8 * slot, (use - 1) & 1);   // the MMA warpgroup has read the slot's last item
+      const int tile = w % P.n_tiles;
+      conv0(s_patch + (k & 1) * N_PATCH, base + OFF_A + slot * 2 * PLANE, (tile % P.tiles_x) * TW, (tile / P.tiles_x) * TH);
+      mbar_arrive(full0 + 8 * slot);
+      // patch[k & 1] was last read by conv0 above; patch[(k + 1) & 1]'s last reader, conv0 of item k - 1, finished
+      // before the previous barrier
+      stash(s_patch + ((k + 1) & 1) * N_PATCH);
+      fetch(w + 2 * G);
+      conv0_bar_sync();
+    }
+    return;
+  }
+
+  // ---- MMA warpgroup: conv1 + bias + ReLU + pool of every item of this CTA ----
+  const int ctid = tid - N_CONV0, warp = ctid >> 5, lane = ctid & 31;
+  const int g = lane >> 2, odd = g & 1, fc = 2 * (lane & 3);
+  float b1[2][2];
 #pragma unroll
   for (int j = 0; j < 2; ++j)
 #pragma unroll
     for (int e = 0; e < 2; ++e) b1[j][e] = P.bias1 ? P.bias1[8 * j + fc + e] : 0.f;
-  griddep_wait();                                       // frames and the pooled buffer belong to the stream's order
+  const uint64_t desc_b = make_desc(0, 32, 3) + (uint64_t)(smem_u32(base + OFF_W1) >> 4);
+  // ldmatrix row address of this lane in plane row 0, kx = 0: pixel 16 warp + lane % 16, 8-channel plane lane / 16
+  const uint32_t a_lane = smem_u32(base + OFF_A) + (uint32_t)((lane >> 4) * PLANE + (16 * warp + (lane & 15)) * 16);
+  griddep_wait();                                       // the pooled buffer belongs to the stream's order
 
-  const float sc = P.frames_u8 ? (1.0f / 255.0f) : 1.0f;     // ensure_float (normalization.py:34-49)
-  TI pf[PATCH_PER_THREAD];
-  auto fetch = [&](int w) {                             // frame patch of item w -> registers (zero outside the frame)
-    const int tile = w % P.n_tiles, b = w / P.n_tiles;
-    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
-    const TI* img = reinterpret_cast<const TI*>(P.frames) + (size_t)b * P.Hin * P.Win;
+  float acc[4][8];                                      // output row y accumulates in set y % 4
+  uint32_t fr[3][3][4];                                 // A fragments of plane row r in set r % 3, one per kx
+  __half2 even[2][2];                                   // an even output row's values (channel group j, pixel half a)
+
+  // bias, ReLU, fp16 rounding (conv1's stored value) of output row y, then for an odd row the 2x2 max with the row above.
+  // Thread pixels: 16 warp + g + 8 a, a = 0, 1; the even column of a pair pools channels 0-7, the odd one 8-15, after
+  // trading the other half with lane ^ 4.
+  auto epilogue = [&](int y, const float (&d)[8], __half* pool_row, int gx0) {
+    auto val = [&](int j, int a) {                      // conv1 output of channel pair (8 j + fc, + 1), pixel half a
+      float v0 = d[4 * j + 2 * a] + b1[j][0], v1 = d[4 * j + 2 * a + 1] + b1[j][1];
+      if (P.relu1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      return __floats2half2_rn(v0, v1);
+    };
+    if ((y & 1) == 0) {
 #pragma unroll
-    for (int k = 0; k < PATCH_PER_THREAD; ++k) {
-      const int e = tid + 256 * k;
-      const int y = y0 - 2 + e / PW, x = x0 - 2 + e % PW;
-      pf[k] = (w < n_items && e < N_PATCH && y >= 0 && y < P.Hin && x >= 0 && x < P.Win) ? img[(size_t)y * P.Win + x] : TI(0);
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int a = 0; a < 2; ++a) even[j][a] = val(j, a);
+      return;
     }
-  };
-  auto stash = [&](float* dst) {
 #pragma unroll
-    for (int k = 0; k < PATCH_PER_THREAD; ++k)
-      if (tid + 256 * k < N_PATCH) dst[tid + 256 * k] = __half2float(__float2half_rn(__fmul_rn((float)pf[k], sc)));
-  };
-
-  // conv0 for the CH0 x CW0 pixels conv1 reads, 8 channels per thread; zero outside the network image (conv1's SAME pad)
-  auto conv0 = [&](const float* patch, uint8_t* A, int x0, int y0) {
-#pragma unroll 1
-    for (int k = 0; k < C0_PER_THREAD; ++k) {
-      const int p = (tid >> 1) + 128 * k;
-      if (p >= N_C0) break;
-      const int yy = p / CW0, cx = p % CW0;
-      const int y = y0 - 1 + yy, x = x0 - 1 + cx;
-      uint32_t q[4] = {0u, 0u, 0u, 0u};                 // fp16 +0 outside
-      if (y >= 0 && y < P.Hnet && x >= 0 && x < P.Wnet) {
-        float acc[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) acc[c] = 0.f;
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) {
-            const float v = patch[(yy + ky) * PW + cx + kx];
-#pragma unroll
-            for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, w0[ky * 3 + kx][c], acc[c]);
-          }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          acc[c] += b0[c];
-          if (P.relu0) acc[c] = fmaxf(acc[c], 0.f);
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const __half2 t = __floats2half2_rn(acc[2 * c], acc[2 * c + 1]);
-          q[c] = *reinterpret_cast<const uint32_t*>(&t);
-        }
-      }
-      *reinterpret_cast<uint4*>(A + hc * PLANE + p * 16) = make_uint4(q[0], q[1], q[2], q[3]);
-    }
-  };
-
-  // conv1: warpgroup wg takes tile rows [8 wg, 8 wg + 8), block bx columns [8 bx, 8 bx + 8); wgmma row m = pixel (m / 8, m % 8)
-  float acc[NBX][8];
-  const uint64_t desc_a = make_desc_interleave(0, PLANE, CW0 * 16);
-  const uint64_t desc_b = make_desc(0, 32, 3);
-  const uint32_t w1_addr = smem_u32(base + OFF_W1);
-  auto mma = [&](const uint8_t* A) {
-    const uint32_t a0 = smem_u32(A) + (uint32_t)(8 * wg * CW0 * 16);
-    wgmma_fence();
-#pragma unroll
-    for (int bx = 0; bx < NBX; ++bx) wgmma_reg_fence(acc[bx]);
-#pragma unroll
-    for (int bx = 0; bx < NBX; ++bx)
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const uint32_t a = a0 + (uint32_t)(((ky * CW0) + 8 * bx + kx) * 16);
-          const uint32_t w = w1_addr + (ky * 3 + kx) * 512;
-          wgmma_f16<16>(acc[bx], desc_a + (a >> 4), desc_b + (w >> 4), (ky | kx) ? 1u : 0u);
-        }
-    wgmma_commit();
-  };
-
-  // bias, ReLU, fp16 rounding (conv1's stored value), 2x2 max.  Thread rows: pixels (2 (warp % 4) + a, g) of each block,
-  // a = 0, 1; the even column of a pair pools channels 0-7, the odd one 8-15, after trading the other half with lane ^ 4.
-  auto pool_store = [&](int w) {
-    wgmma_wait<0>();
-#pragma unroll
-    for (int bx = 0; bx < NBX; ++bx) wgmma_reg_fence(acc[bx]);
-    const int tile = w % P.n_tiles, b = w / P.n_tiles;
-    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
-    const int g = lane >> 2, odd = g & 1;
-    const int gy = (y0 >> 1) + 4 * wg + (warp & 3);
-    __half* row = P.pool_out + ((size_t)b * P.pool_H + gy) * P.pool_W * P.pool_Ctot + P.pool_coff + 8 * odd + fc;
-#pragma unroll
-    for (int bx = 0; bx < NBX; ++bx) {
-      auto val = [&](int j, int a) {                    // conv1 output of channel pair (8 j + fc, + 1), row a
-        float v0 = acc[bx][4 * j + 2 * a] + b1[j][0], v1 = acc[bx][4 * j + 2 * a + 1] + b1[j][1];
-        if (P.relu1) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        return __floats2half2_rn(v0, v1);
-      };
-      const __half2 v00 = val(0, 0), v01 = val(0, 1), v10 = val(1, 0), v11 = val(1, 1);
-      const __half2 mine0 = odd ? v10 : v00, mine1 = odd ? v11 : v01;
-      const __half2 theirs0 = __shfl_xor_sync(0xffffffffu, odd ? v00 : v10, 4);
-      const __half2 theirs1 = __shfl_xor_sync(0xffffffffu, odd ? v01 : v11, 4);
+    for (int a = 0; a < 2; ++a) {
+      const __half2 o0 = val(0, a), o1 = val(1, a);
+      const __half2 mine0 = odd ? even[1][a] : even[0][a], mine1 = odd ? o1 : o0;
+      const __half2 theirs0 = __shfl_xor_sync(0xffffffffu, odd ? even[0][a] : even[1][a], 4);
+      const __half2 theirs1 = __shfl_xor_sync(0xffffffffu, odd ? o0 : o1, 4);
       __half2 m = __float2half2_rn(-INFINITY);          // order (row, column) = (0, 0), (0, 1), (1, 0), (1, 1)
       m = __hmax2(m, odd ? theirs0 : mine0);
       m = __hmax2(m, odd ? mine0 : theirs0);
       m = __hmax2(m, odd ? theirs1 : mine1);
       m = __hmax2(m, odd ? mine1 : theirs1);
-      const int gx = (x0 >> 1) + 4 * bx + (g >> 1);
-      if (gy < P.pool_H && gx < P.pool_W) *reinterpret_cast<__half2*>(row + (size_t)gx * P.pool_Ctot) = m;
+      const int gx = gx0 + 4 * a;
+      if (pool_row && gx < P.pool_W) *reinterpret_cast<__half2*>(pool_row + (size_t)gx * P.pool_Ctot) = m;
     }
   };
 
   int w = blockIdx.x;
-  fetch(w);
-  stash(s_patch);
-  fetch(w + G);
-  __syncthreads();
   for (int k = 0; w < n_items; ++k, w += G) {
     if (w + G >= n_items) griddep_launch();             // last item of this CTA
-    const int buf = k & 1;
-    const int tile = w % P.n_tiles;
-    uint8_t* A = base + OFF_A + buf * 2 * PLANE;
-    // A[buf] was last read by the wgmma of item k - 2, waited for before the previous barrier; so was patch[buf ^ 1]'s
-    // last reader, conv0 of item k - 1
-    conv0(s_patch + buf * N_PATCH, A, (tile % P.tiles_x) * TW, (tile / P.tiles_x) * TH);
-    stash(s_patch + (buf ^ 1) * N_PATCH);
-    fetch(w + 2 * G);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
-    if (k > 0) pool_store(w - G);
-    __syncthreads();
-    mma(A);
+    const int slot = k % NSLOT;
+    mbar_wait(full0 + 8 * slot, (k / NSLOT) & 1);
+    const uint32_t a0 = a_lane + (uint32_t)(slot * 2 * PLANE);
+    const int tile = w % P.n_tiles, b = w / P.n_tiles;
+    const int x0 = (tile % P.tiles_x) * TW, y0 = (tile / P.tiles_x) * TH;
+    const int gx0 = (x0 >> 1) + 8 * warp + (g >> 1);
+    __half* pool_img = P.pool_out + (size_t)b * P.pool_H * P.pool_W * P.pool_Ctot + P.pool_coff + 8 * odd + fc;
+    auto row_of = [&](int y) -> __half* {               // pooled row of output row y (nullptr below the map)
+      const int gy = (y0 + y) >> 1;
+      return gy < P.pool_H ? pool_img + (size_t)gy * P.pool_W * P.pool_Ctot : nullptr;
+    };
+#pragma unroll
+    for (int kx = 0; kx < 3; ++kx) ldmatrix_x4(fr[0][kx], a0 + 16 * kx);
+#pragma unroll
+    for (int r = 0; r < CH0; ++r) {
+      // group r: plane row r's fragments into the ky = 0, 1, 2 taps of output rows r, r - 1, r - 2
+      wgmma_fence();
+#pragma unroll
+      for (int s = 0; s < 4; ++s) wgmma_reg_fence(acc[s]);
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky) {
+        const int y = r - ky;
+        if (y < 0 || y >= TH) continue;
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx)
+          wgmma_f16_rs16(acc[y & 3], fr[r % 3][kx], desc_b + 32 * (ky * 3 + kx), (ky | kx) ? 1u : 0u);
+      }
+      wgmma_commit();
+      if (r + 1 < CH0) {
+        // set (r + 1) % 3 was last read by group r - 2, complete since the previous wait
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) ldmatrix_x4(fr[(r + 1) % 3][kx], a0 + (uint32_t)((r + 1) * CW0 * 16) + 16 * kx);
+      } else {
+        mbar_arrive(empty0 + 8 * slot);                 // every ldmatrix of this slot has returned
+      }
+#pragma unroll
+      for (int s = 0; s < 4; ++s) wgmma_reg_fence(acc[s]);
+      wgmma_wait<1>();                                  // groups <= r - 1 done: output row r - 3 is complete
+      if (r >= 3) {
+        wgmma_reg_fence(acc[(r - 3) & 3]);
+        epilogue(r - 3, acc[(r - 3) & 3], row_of(r - 3), gx0);
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc[(TH - 1) & 3]);
+    epilogue(TH - 1, acc[(TH - 1) & 3], row_of(TH - 1), gx0);
   }
-  pool_store(w - G);                                    // every CTA has at least one item (grid <= item count)
 }
 
 }  // namespace
@@ -265,7 +322,7 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
   for (auto kern : {k_conv01<unsigned char>, k_conv01<float>}) {
     int nb = 0;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, 256, SMEM_BYTES) != cudaSuccess || nb < 1) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, N_THREADS, SMEM_BYTES) != cudaSuccess || nb < 1) {
       delete pl;
       return sb_fail(h, SB_ERR_CUDA, "conv01: kernel attributes / occupancy: %s", cudaGetErrorString(cudaGetLastError()));
     }
@@ -314,7 +371,7 @@ int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
   P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.batch = B;
   void* args[] = {&P};
   sb_launch_pdl(frames_are_u8 ? (const void*)k_conv01<unsigned char> : (const void*)k_conv01<float>,
-                dim3(std::min(P.n_tiles * B, pl->max_ctas)), dim3(256), SMEM_BYTES, h->stream, args);
+                dim3(std::min(P.n_tiles * B, pl->max_ctas)), dim3(N_THREADS), SMEM_BYTES, h->stream, args);
   SB_CHECK_LAUNCH(h);
   return 0;
 }

@@ -168,6 +168,25 @@ __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint64_t a_desc,
       : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
 }
 
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T with A in registers: warp w of the warpgroup holds rows [16 w, 16 w + 16) as
+// the four 8x8 fp16 matrices (rows 0-7 | 8-15) x (k 0-7 | 8-15) in the order ldmatrix_x4 loads them when lane l gives
+// the address of row l % 16, k half l / 16.  B is K-major in shared memory; accumulators as in wgmma_f16<16>.
+__device__ __forceinline__ void wgmma_f16_rs16(float (&d)[8], const uint32_t (&a)[4], uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "{%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(scale_d) : "memory");
+}
+// four 8x8 b16 matrices from shared memory; lanes 8 i .. 8 i + 7 give the 16-byte row addresses of matrix i
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr) : "memory");
+}
+
 // Warp-specialized register split: every warp of a warpgroup executes these together.  dec releases registers of the
 // calling warpgroup down to R per thread, inc blocks until R per thread are free (R a multiple of 8 in [24, 256]).
 template <int R>
