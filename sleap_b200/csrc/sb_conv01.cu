@@ -288,37 +288,25 @@ struct SbConv01Plan {
   C01Params P;
   __half* w1t = nullptr;     // [9][16][16]
   float* w0h = nullptr;      // [9][16]
-  int conv0_op = -1, conv1_op = -1;
   int max_ctas = 0;          // co-resident CTAs of k_conv01 on this GPU
 };
 
 void sb_conv01_release(SbModel* m) {
-  if (!m->conv01) return;
-  if (m->conv01->w1t) cudaFree(m->conv01->w1t);
-  if (m->conv01->w0h) cudaFree(m->conv01->w0h);
-  delete m->conv01;
-  m->conv01 = nullptr;
+  SbConv01Plan*& pl = m->entry.conv01;
+  if (!pl) return;
+  if (pl->w1t) cudaFree(pl->w1t);
+  if (pl->w0h) cudaFree(pl->w0h);
+  delete pl;
+  pl = nullptr;
 }
 
-// The block qualifies when: 1-channel frames, no resize; conv0 = 3x3 s1 1 -> 16 (+ReLU) fused with PREPROCESS;
-// conv1 = 3x3 s1 16 -> 16 whose 2x2 max-pool is fused and whose own output has no other reader (sb_conv_tc.cu marks it).
-int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bool conv1_out_dead) {
-  sb_conv01_release(m);
-  if (getenv("SB_DISABLE_CONV01") || m->precision != 0 || !conv1_out_dead) return 0;
+// The parameters of k_conv01 over conv0_op -> conv1_op -> pool, a block the input stage found it takes (sb_entry.cu).
+int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op) {
   const SbOp& c0 = m->ops[conv0_op];
   const SbOp& c1 = m->ops[conv1_op];
-  if (m->Cin != 1 || c0.in_C() != 1 || c0.out_C() != 16 || c0.k() != 3 || c0.stride() != 1 || (c0.flags() & SB_OPF_BN)) return 0;
-  if (c1.in_C() != 16 || c1.out_C() != 16 || c1.k() != 3 || c1.stride() != 1 || (c1.flags() & SB_OPF_BN)) return 0;
-  if (c1.in_buf() != c0.out_buf() || c1.in_coff() != c0.out_coff() || c1.pool_buf() < 0) return 0;
   const SbBuffer& ob0 = m->buffers[c0.out_buf()];
   const SbBuffer& pb = m->buffers[c1.pool_buf()];
-  if (ob0.f32 || pb.f32 || pb.C % 2 || c1.pool_coff() % 2 || ob0.H % 2 || ob0.W % 2) return 0;
-  for (size_t oi = 0; oi < m->ops.size(); ++oi)            // conv0's output must feed conv1 only
-    if ((int)oi != conv1_op && m->ops[oi].kind() != SB_OPK_PREPROCESS && (int)oi != conv0_op &&
-        (m->ops[oi].in_buf() == c0.out_buf() || (m->ops[oi].kind() == SB_OPK_ADD && m->ops[oi].in2_buf() == c0.out_buf())))
-      return 0;
   SbConv01Plan* pl = new SbConv01Plan();
-  pl->conv0_op = conv0_op; pl->conv1_op = conv1_op;
   for (auto kern : {k_conv01<unsigned char>, k_conv01<float>}) {
     int nb = 0;
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
@@ -340,7 +328,7 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
   auto fail = [&](const char* what) { delete pl; return sb_fail(h, SB_ERR_CUDA, "conv01: %s", what); };
   if (cudaMalloc((void**)&pl->w1t, w1t.size() * 2) != cudaSuccess) return fail("cudaMalloc");
   if (cudaMalloc((void**)&pl->w0h, w0h.size() * 4) != cudaSuccess) { cudaFree(pl->w1t); return fail("cudaMalloc"); }
-  m->conv01 = pl;                                          // released with the model from here on
+  m->entry.conv01 = pl;                                    // released with the model from here on
   if (cudaMemcpy(pl->w1t, w1t.data(), w1t.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMemcpy(pl->w0h, w0h.data(), w0h.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
     sb_conv01_release(m);
@@ -360,13 +348,10 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bo
   return 0;
 }
 
-bool sb_conv01_can(const SbModel* m, int conv0_op) { return m->conv01 && m->conv01->conv0_op == conv0_op && m->conv01_enabled; }
-int sb_conv01_conv1_op(const SbModel* m) { return m->conv01 ? m->conv01->conv1_op : -1; }
-
 // Persistent launch: as many CTAs as are co-resident (capped at the item count), with programmatic stream serialization
 // so that the weight loads overlap the predecessor's tail; each CTA triggers its dependents when it starts its last item.
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
-  SbConv01Plan* pl = m->conv01;
+  SbConv01Plan* pl = m->entry.conv01;
   C01Params P = pl->P;
   P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.batch = B;
   void* args[] = {&P};

@@ -1378,15 +1378,6 @@ struct SbConvTcPlan {
   const void* head = nullptr;       // the k_head_1x1 instantiation that runs this 1x1 fp32 head instead of the launches
   __half* w16 = nullptr;            // [taps][Cout_pad][Cin]
   int Cout_pad = 0;
-  // first layer as a Toeplitz GEMM (sb_first_view_prepare): staged [B][H][W/8][16] fp16 view of the frame
-  __half* view_in = nullptr;
-  float* view_bias = nullptr;       // bias replicated over the 8 pixels of a group: [8 * Cout]
-  int view_Wg = 0;
-  bool view_enabled = true;         // false: the autotuner measured k_conv_first faster for this shape
-  bool from_buffer = false;         // Toeplitz view built from the (resized / converted) PREPROCESS output instead of the raw frame
-  bool s2d = false;                 // view_in is the space-to-depth view of the frame (7x7 stride-2 stem as a 4x4 conv)
-  int s2d_Hs = 0, s2d_Ws = 0;
-  int s2d_pre_mode = SB_PRE_PLAIN;   // PREPROCESS mode folded into the space-to-depth view (ImageNet caffe for ResNet)
   bool out_dead = false;            // nobody reads the full-resolution output (only the fused pool): stores are skipped
   // the residual ADD after this conv runs in its epilogue (launches); plain_launches store the conv's own output
   // instead, for a forward pass that asks for that tensor (the ADD op then runs)
@@ -1422,39 +1413,27 @@ static bool tc_eligible(const SbModel* m, const SbOp& op) {
   return true;
 }
 
+void sb_conv_tc_drop(SbModel* m, int op_index) {
+  SbConvTcPlan*& p = m->tc_plans[op_index];
+  if (p->w16) cudaFree(p->w16);
+  delete p;
+  p = nullptr;
+}
+
 void sb_conv_tc_release(SbModel* m) {
-  for (SbConvTcPlan* p : m->tc_plans)
-    if (p) {
-      if (p->w16) cudaFree(p->w16);
-      if (p->view_in) cudaFree(p->view_in);
-      if (p->view_bias) cudaFree(p->view_bias);
-      delete p;
-    }
+  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi)
+    if (m->tc_plans[oi]) sb_conv_tc_drop(m, (int)oi);
   m->tc_plans.clear();
 }
 
-bool sb_conv_tc_out_dead(const SbModel* m, int buffer_id) {
-  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi)
-    if (m->tc_plans[oi] && (m->tc_plans[oi]->out_dead || m->tc_plans[oi]->res_fused) && m->ops[oi].out_buf() == buffer_id) return true;
-  return false;
+bool sb_conv_tc_out_dead(const SbModel* m, int op_index) {
+  const SbConvTcPlan* p = op_index < (int)m->tc_plans.size() ? m->tc_plans[op_index] : nullptr;
+  return p && (p->out_dead || p->res_fused);
 }
 
 bool sb_conv_tc_can(const SbModel* m, int op_index) {
-  return op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] != nullptr &&
-         (!m->tc_plans[op_index]->view_in || m->tc_plans[op_index]->view_enabled);
+  return op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] != nullptr;
 }
-
-// A launch over tensors that are not op-list buffers (the Toeplitz view of the first layer): every
-// quantity make_launch would read from the op / its buffers.
-struct TcView {
-  SbBuffer ib, ob;
-  int Cin, Cout;
-  const float* bias;
-  int relu;
-  const float* bn_scale = nullptr;
-  const float* bn_shift = nullptr;
-  int out_coff = 0;
-};
 
 // the wgmma tile widths N that have instantiations
 constexpr int kWgN[8] = {16, 32, 48, 64, 96, 128, 192, 256};
@@ -1624,14 +1603,14 @@ static CUresult encode_weights(EncodeTiledFn enc, const SbConvTcPlan* plan, int 
 
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
                        const TcGroup* groups, int dy0, int extra_rows, int n_wtaps, int oy_mul, int oy_add,
-                       int ox_mul, int ox_add, const TcView* view = nullptr, bool fuse_res = false,
+                       int ox_mul, int ox_add, const SbTcView* view = nullptr, bool fuse_res = false,
                        std::vector<TcLaunch>* dst = nullptr) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  const SbBuffer& ib = view ? view->ib : m->buffers[op.in_buf()];
-  const SbBuffer& ob0 = view ? view->ob : m->buffers[op.out_buf()];
+  const SbBuffer& ib = view ? view->in : m->buffers[op.in_buf()];
+  const SbBuffer& ob0 = view ? view->out : m->buffers[op.out_buf()];
   const SbBuffer& ob = fuse_res ? m->buffers[op.sum_buf()] : ob0;       // the residual sum goes to the ADD's output slice
-  const int Cin = view ? view->Cin : op.in_C(), Cout = view ? view->Cout : op.out_C();
+  const int Cin = view ? view->in.C : op.in_C(), Cout = view ? view->Cout : op.out_C();
   const int in_coff = view ? 0 : op.in_coff(), out_coff = view ? view->out_coff : (fuse_res ? op.sum_coff() : op.out_coff());
   const int KC = Cin > 32 ? 64 : (Cin > 16 ? 32 : 16);
   // 1x1 stride-2: the GEMM runs over the output grid on a subsampled view of the input (pitches x 2)
@@ -1763,281 +1742,35 @@ static int setup_tconv_form(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTc
   return 0;
 }
 
-// ---- first layer (1 input channel, 3x3) as a Toeplitz GEMM over groups of 8 output pixels ----------
-// out[y][8g+j][co] = sum_{ky,kx} in[y+ky-1][8g+j+kx-1] * w[ky][kx][co]   (SAME padding)
-// With G[y][g][c] = in[y][8g-1+c] (c = 0..9; c = 10..15 zero) the layer is an ordinary 3x1 convolution
-// over the [H][W/8] grid of groups with 16 "input channels" (the window) and 8*Cout "output channels"
-// (pixel j of the group x filter co): W'[ky][j*Cout+co][c] = w[ky][c-j][co] for 0 <= c-j <= 2.  The
-// output [H][W/8][8*Cout] is byte-identical to NHWC [H][W][Cout], so the stock wgmma conv kernel runs
-// it unchanged: each epilogue thread writes 8 pixels (8*Cout*2 contiguous bytes) instead of gathering a
-// 3x3 neighbourhood per pixel, which is what bounds the CUDA-core k_conv_first.  Tensor work grows 3.5x (16x8*Cout
-// MACs per tap row instead of 9*Cout per pixel) on a pipe that is otherwise idle in this layer.
-template <typename TI>
-__global__ void __launch_bounds__(256) k_first_view(const TI* __restrict__ img, int Hin, int Win, int Hnet, int Wg,
-                                                    __half* __restrict__ G, int in_is_u8, size_t total) {
-  const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;       // ensure_float (normalization.py:34-49)
-  for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
-    const int g = (int)(i % Wg);
-    const size_t r = i / Wg;
-    const int y = (int)(r % Hnet), b = (int)(r / Hnet);
-    __align__(16) __half v[16];
-#pragma unroll
-    for (int c = 0; c < 16; ++c) v[c] = __float2half_rn(0.f);
-    if (y < Hin) {                                           // rows below the frame: bottom zero pad (resizing.py:34-68)
-      const TI* row = img + ((size_t)b * Hin + y) * Win;
-#pragma unroll
-      for (int c = 0; c < 10; ++c) {
-        const int x = 8 * g - 1 + c;
-        if (x >= 0 && x < Win) v[c] = __float2half_rn(__fmul_rn((float)row[x], sc));
-      }
-    }
-    uint4* dst = reinterpret_cast<uint4*>(G + i * 16);
-    dst[0] = *reinterpret_cast<const uint4*>(&v[0]);
-    dst[1] = *reinterpret_cast<const uint4*>(&v[8]);
-  }
-}
-
-int sb_first_fusion_op(const SbModel* m, size_t pre_index);   // sb_model.cu
-
-// Builds the plan of the first conv (op `oi`, fused with the PREPROCESS op before it) when the shape
-// allows the Toeplitz form; leaves m->tc_plans[oi] null otherwise (k_conv_first then runs the layer).
-static int first_view_prepare(sb_handle_s* h, SbModel* m, int oi, bool from_buffer = false) {
-  if (getenv("SB_DISABLE_FIRST_VIEW") || getenv("SB_DISABLE_TC")) return 0;
-  const SbOp& op = m->ops[oi];
-  const SbBuffer& ob = m->buffers[op.out_buf()];
-  const int Cout = op.out_C();
-  if ((!from_buffer && m->Cin != 1) || op.in_C() != 1 || op.k() != 3 || op.stride() != 1) return 0;
-  if (from_buffer && (m->buffers[op.in_buf()].C != 1 || m->buffers[op.in_buf()].f32 || op.in_coff() != 0)) return 0;
-  if (!(Cout == 8 || Cout == 16 || Cout == 24 || Cout == 32)) return 0;           // N = 8*Cout <= 256, multiple of 16
-  if (ob.f32 || ob.C != Cout || op.out_coff() != 0 || op.pool_buf() >= 0 || (op.flags() & SB_OPF_BN)) return 0;
-  if (ob.W % 8 || ob.W / 8 < TW || ob.H < TH + 2) return 0;                        // the streaming TMA box must fit inside the view
-  const int Wg = ob.W / 8, N = 8 * Cout;
+int sb_conv_tc_view_prepare(sb_handle_s* h, SbModel* m, int op_index, const SbTcView& v, const std::vector<float>& w) {
+  if (v.in.W < TW || v.in.H < TH + v.R - 1) return 0;         // the streaming TMA box must fit inside the view
   SbConvTcPlan* plan = new SbConvTcPlan();
-  plan->Cout_pad = N;
-  plan->view_Wg = Wg;
-  plan->from_buffer = from_buffer;
-  std::vector<__half> w16((size_t)3 * N * 16, __float2half(0.f));
-  const float* w = m->weights_host.data() + op.w_off();                            // [9][1][Cout]
-  for (int ky = 0; ky < 3; ++ky)
-    for (int j = 0; j < 8; ++j)
-      for (int kx = 0; kx < 3; ++kx)
-        for (int co = 0; co < Cout; ++co)
-          w16[((size_t)ky * N + j * Cout + co) * 16 + j + kx] = __float2half_rn(w[(size_t)(ky * 3 + kx) * Cout + co]);
-  std::vector<float> brep(N, 0.f);
-  if (op.b_off() >= 0)
-    for (int n = 0; n < N; ++n) brep[n] = m->weights_host[op.b_off() + n % Cout];
-  auto fail = [&](const char* what, cudaError_t e) {
-    if (plan->w16) cudaFree(plan->w16);
-    if (plan->view_in) cudaFree(plan->view_in);
-    if (plan->view_bias) cudaFree(plan->view_bias);
-    delete plan;
-    return sb_fail(h, SB_ERR_CUDA, "first-layer view: %s: %s", what, cudaGetErrorString(e));
-  };
-  cudaError_t e = cudaMalloc((void**)&plan->w16, w16.size() * sizeof(__half));
-  if (e != cudaSuccess) return fail("cudaMalloc w16", e);
-  e = cudaMemcpy(plan->w16, w16.data(), w16.size() * sizeof(__half), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail("copy w16", e);
-  e = cudaMalloc((void**)&plan->view_bias, N * sizeof(float));
-  if (e != cudaSuccess) return fail("cudaMalloc bias", e);
-  e = cudaMemcpy(plan->view_bias, brep.data(), N * sizeof(float), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail("copy bias", e);
-  const size_t vbytes = (size_t)m->B * ob.H * Wg * 16 * sizeof(__half);
-  e = cudaMalloc((void**)&plan->view_in, vbytes + 256);
-  if (e != cudaSuccess) return fail("cudaMalloc view", e);
-  e = cudaMemset(plan->view_in, 0, vbytes + 256);
-  if (e != cudaSuccess) return fail("memset view", e);
-  TcView V;
-  V.ib = SbBuffer(); V.ib.C = 16; V.ib.H = ob.H; V.ib.W = Wg; V.ib.dev = plan->view_in;
-  V.ob = SbBuffer(); V.ob.C = N; V.ob.H = ob.H; V.ob.W = Wg; V.ob.dev = ob.dev; V.ob.f32 = 0;
-  V.Cin = 16; V.Cout = N;
-  V.bias = plan->view_bias;
-  V.relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-  TcGroup g[1];
-  g[0].dx = 0; g[0].n_taps = 3;
-  for (int ky = 0; ky < 3; ++ky) g[0].taps[ky] = TcTap{ky, ky};
-  const int rc = make_launch(h, m, op, plan, 1, g, -1, 2, 3, 1, 0, 1, 0, &V);
-  if (rc) {
-    cudaFree(plan->w16); cudaFree(plan->view_in); cudaFree(plan->view_bias);
-    delete plan;
-    return rc < 0 ? rc : 0;
-  }
-  m->tc_plans[oi] = plan;
-  return 0;
-}
-
-
-// ---- 7x7 stride-2 stem (hourglass.py:49-100; 1 or 3 input channels) on the tensor cores -----------------------
-// SAME padding of an even-sized input puts 2 rows / columns before and 3 after: output pixel o reads input rows
-// 2o-2 .. 2o+4.  With the frame regrouped into 2x2 blocks ("space to depth": block (Y, X) holds pixels (2Y+py, 2X+px),
-// 4*Cin values, padded to 16 channels) those are blocks o-1 .. o+2, i.e. a 4x4 stride-1 convolution over the block grid
-// with W'[dy][dx][(py, px, c)][co] = w[2(dy+1)+py][2(dx+1)+px][c][co] (zero where the index reaches 7).  The view kernel
-// does InferenceLayer.preprocess (uint8 -> float * 1/255, zero pad) on the way; the stock wgmma conv kernel runs
-// the convolution (K = 16 taps x 16 channels = 256 instead of 147: the stem was on the CUDA cores before).
-// The ResNet stem (ZeroPadding2D(3) + VALID, resnet.py) pads 3|3 instead: output pixel o reads rows 2o-3 .. 2o+3, i.e.
-// blocks o-2 .. o+1 with the zero tap at the top / left (W'[dy][dx][(py, px, c)] = w[2dy+py-1][2dx+px-1]).  Its view
-// carries the pretrained preprocessing too (pre_mode != 0): tile_channels (1 -> 3, or gray -> 3 for a grayscale-trained
-// model fed colour frames), then x * 255, RGB -> BGR, minus the caffe means, on the padded [0, 1] image -- so rows /
-// columns of the net input beyond the frame hold -mean, while the conv's own padding (outside the view) stays 0.
-template <typename TI>
-__global__ void __launch_bounds__(256) k_s2d_view(const TI* __restrict__ img, int Hin, int Win, int Cin, int Hs, int Ws,
-                                                  __half* __restrict__ G, int in_is_u8, size_t total, int pre_mode = 0) {
-  const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
-  for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (size_t)gridDim.x * 256) {
-    const int X = (int)(i % Ws);
-    const size_t r = i / Ws;
-    const int Y = (int)(r % Hs), b = (int)(r / Hs);
-    __align__(16) __half v[16];
-#pragma unroll
-    for (int c = 0; c < 16; ++c) v[c] = __float2half_rn(0.f);
-#pragma unroll
-    for (int py = 0; py < 2; ++py)
-#pragma unroll
-      for (int px = 0; px < 2; ++px) {
-        const int y = 2 * Y + py, x = 2 * X + px;
-        const bool in = y < Hin && x < Win;
-        const TI* p = img + (((size_t)b * Hin + y) * Win + x) * Cin;
-        if (pre_mode == SB_PRE_PLAIN) {
-          if (in)
-            for (int c = 0; c < Cin; ++c) v[(py * 2 + px) * Cin + c] = __float2half_rn(__fmul_rn((float)p[c], sc));
-          continue;
-        }
-        const float g = (in && Cin == 3 && pre_mode == SB_PRE_IMAGENET_CAFFE_GRAY) ? sb_gray_pre(p, in_is_u8) : 0.f;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {              // BGR channel c
-          float f = 0.f;
-          if (in) f = (Cin == 3 && pre_mode == SB_PRE_IMAGENET_CAFFE_GRAY) ? g : __fmul_rn((float)p[Cin == 1 ? 0 : 2 - c], sc);
-          v[(py * 2 + px) * 3 + c] = __float2half_rn(__fsub_rn(__fmul_rn(f, 255.f), sb_imagenet_caffe_mean(c)));
-        }
-      }
-    uint4* dst = reinterpret_cast<uint4*>(G + i * 16);
-    dst[0] = *reinterpret_cast<const uint4*>(&v[0]);
-    dst[1] = *reinterpret_cast<const uint4*>(&v[8]);
-  }
-}
-
-int sb_stem_fusion_op(const SbModel* m, size_t pre_index);   // sb_model.cu
-
-static int stem_view_prepare(sb_handle_s* h, SbModel* m, int oi) {
-  if (getenv("SB_DISABLE_STEM_VIEW") || getenv("SB_DISABLE_TC")) return 0;
-  const SbOp& op = m->ops[oi];
-  const SbBuffer& ib = m->buffers[op.in_buf()];
-  const SbBuffer& ob = m->buffers[op.out_buf()];
-  const int Cin = op.in_C(), Cout = op.out_C();
-  const int sh = op.explicit_pad() ? 1 : 0;                  // 3|3 padding: the 4x4 block window starts one block earlier
-  if (ib.H % 2 || ib.W % 2 || ob.H != ib.H / 2 || ob.W != ib.W / 2) return 0;
-  if (ob.f32 || ob.C % 8 || op.out_coff() % 8 || ob.W < TW || ob.H < TH + 3) return 0;
-  SbConvTcPlan* plan = new SbConvTcPlan();
-  int cp = (Cout + 15) / 16 * 16;
+  int cp = (v.Cout + 15) / 16 * 16;
   if (cp > 256) cp = (cp + 255) / 256 * 256;
   plan->Cout_pad = cp;
-  plan->s2d = true; plan->s2d_Hs = ob.H; plan->s2d_Ws = ob.W;
-  plan->s2d_pre_mode = m->ops[oi - 1].pre_mode();
-  std::vector<__half> w16((size_t)16 * cp * 16, __float2half(0.f));
-  const float* w = m->weights_host.data() + op.w_off();      // [7*7][Cin][Cout]
-  for (int dy = 0; dy < 4; ++dy)
-    for (int dx = 0; dx < 4; ++dx)
-      for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-          const int ky = 2 * dy + py - sh, kx = 2 * dx + px - sh;
-          if (ky < 0 || kx < 0 || ky > 6 || kx > 6) continue;
-          for (int c = 0; c < Cin; ++c)
-            for (int co = 0; co < Cout; ++co)
-              w16[((size_t)(dy * 4 + dx) * cp + co) * 16 + (py * 2 + px) * Cin + c] = __float2half_rn(w[((size_t)(ky * 7 + kx) * Cin + c) * Cout + co]);
-        }
-  auto fail = [&](const char* what, cudaError_t e) {
-    if (plan->w16) cudaFree(plan->w16);
-    if (plan->view_in) cudaFree(plan->view_in);
-    delete plan;
-    return sb_fail(h, SB_ERR_CUDA, "stem view: %s: %s", what, cudaGetErrorString(e));
-  };
+  std::vector<__half> w16((size_t)v.R * v.S * cp * 16, __float2half(0.f));
+  for (int t = 0; t < v.R * v.S; ++t)
+    for (int co = 0; co < v.Cout; ++co)
+      for (int c = 0; c < 16; ++c) w16[((size_t)t * cp + co) * 16 + c] = __float2half_rn(w[((size_t)t * v.Cout + co) * 16 + c]);
   cudaError_t e = cudaMalloc((void**)&plan->w16, w16.size() * sizeof(__half));
-  if (e != cudaSuccess) return fail("cudaMalloc w16", e);
-  e = cudaMemcpy(plan->w16, w16.data(), w16.size() * sizeof(__half), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) return fail("copy w16", e);
-  const size_t vbytes = (size_t)m->B * ob.H * ob.W * 16 * sizeof(__half);
-  e = cudaMalloc((void**)&plan->view_in, vbytes + 256);
-  if (e != cudaSuccess) return fail("cudaMalloc view", e);
-  e = cudaMemset(plan->view_in, 0, vbytes + 256);
-  if (e != cudaSuccess) return fail("memset view", e);
-  TcView V;
-  V.ib = SbBuffer(); V.ib.C = 16; V.ib.H = ob.H; V.ib.W = ob.W; V.ib.dev = plan->view_in;
-  V.ob = ob;
-  V.Cin = 16; V.Cout = Cout;
-  V.bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-  V.relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-  V.bn_scale = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_scale_off() : nullptr;
-  V.bn_shift = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_shift_off() : nullptr;
-  V.out_coff = op.out_coff();
-  TcGroup g[4];
-  for (int dx = 0; dx < 4; ++dx) {
-    g[dx].dx = dx - 1 - sh; g[dx].n_taps = 4;
-    for (int dy = 0; dy < 4; ++dy) g[dx].taps[dy] = TcTap{dy, dy * 4 + dx};
-  }
-  const int rc = make_launch(h, m, op, plan, 4, g, -1 - sh, 3, 16, 1, 0, 1, 0, &V);
-  if (rc) {
-    cudaFree(plan->w16); cudaFree(plan->view_in);
+  if (e == cudaSuccess) e = cudaMemcpy(plan->w16, w16.data(), w16.size() * sizeof(__half), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    if (plan->w16) cudaFree(plan->w16);
     delete plan;
-    return rc < 0 ? rc : 0;
+    return sb_fail(h, SB_ERR_CUDA, "view conv weights: %s", cudaGetErrorString(e));
   }
-  m->tc_plans[oi] = plan;
+  TcGroup g[MAX_GROUPS];                                      // filter column s, its rows r
+  for (int s = 0; s < v.S; ++s) {
+    g[s].dx = v.dx0 + s; g[s].n_taps = v.R;
+    for (int r = 0; r < v.R; ++r) g[s].taps[r] = TcTap{r, r * v.S + s};
+  }
+  if (const int rc = make_launch(h, m, m->ops[op_index], plan, v.S, g, v.dy0, v.R - 1, v.R * v.S, 1, 0, 1, 0, &v)) {
+    cudaFree(plan->w16);
+    delete plan;
+    return rc;
+  }
+  m->tc_plans[op_index] = plan;
   return 0;
-}
-
-bool sb_stem_view_can(const SbModel* m, int op_index) {
-  return op_index >= 0 && op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] && m->tc_plans[op_index]->s2d;
-}
-
-// frame -> space-to-depth view -> 4x4 conv on the tensor cores
-int sb_stem_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
-  SbConvTcPlan* plan = m->tc_plans[op_index];
-  const size_t total = (size_t)B * plan->s2d_Hs * plan->s2d_Ws;
-  const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
-  if (frames_are_u8)
-    k_s2d_view<unsigned char><<<grid, 256, 0, h->stream>>>((const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, plan->s2d_Hs, plan->s2d_Ws,
-                                                           plan->view_in, 1, total, plan->s2d_pre_mode);
-  else
-    k_s2d_view<float><<<grid, 256, 0, h->stream>>>((const float*)frames_dev, m->Hin, m->Win, m->Cin, plan->s2d_Hs, plan->s2d_Ws, plan->view_in, 0,
-                                                   total, plan->s2d_pre_mode);
-  SB_CHECK_LAUNCH(h);
-  return sb_conv_tc_launch(h, m, op_index, B);
-}
-
-bool sb_first_view_can(const SbModel* m, int op_index) {
-  return op_index >= 0 && op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] && m->tc_plans[op_index]->view_in &&
-         !m->tc_plans[op_index]->s2d && !m->tc_plans[op_index]->from_buffer && m->tc_plans[op_index]->view_enabled;
-}
-
-// First conv of a model whose frames are resized / converted first (input_scale != 1, rgb -> gray): the PREPROCESS kernel
-// runs as usual and the Toeplitz view is built from ITS one-channel fp16 output, so the layer still runs on the tensor cores.
-bool sb_first_buffer_view_can(const SbModel* m, int op_index) {
-  return op_index >= 0 && op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] && m->tc_plans[op_index]->view_in &&
-         m->tc_plans[op_index]->from_buffer;
-}
-
-int sb_first_buffer_view_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
-  SbConvTcPlan* plan = m->tc_plans[op_index];
-  const SbBuffer& ib = m->buffers[m->ops[op_index].in_buf()];
-  const SbBuffer& ob = m->buffers[m->ops[op_index].out_buf()];
-  const size_t total = (size_t)B * ob.H * plan->view_Wg;
-  const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
-  k_first_view<__half><<<grid, 256, 0, h->stream>>>((const __half*)ib.dev, ib.H, ib.W, ob.H, plan->view_Wg, plan->view_in, 0, total);
-  SB_CHECK_LAUNCH(h);
-  return sb_conv_tc_launch(h, m, op_index, B);
-}
-
-// frame -> Toeplitz view -> tensor-core conv
-int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
-  SbConvTcPlan* plan = m->tc_plans[op_index];
-  const SbBuffer& ob = m->buffers[m->ops[op_index].out_buf()];
-  const size_t total = (size_t)B * ob.H * plan->view_Wg;
-  const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
-  if (frames_are_u8)
-    k_first_view<unsigned char><<<grid, 256, 0, h->stream>>>((const unsigned char*)frames_dev, m->Hin, m->Win, ob.H, plan->view_Wg,
-                                                             plan->view_in, 1, total);
-  else
-    k_first_view<float><<<grid, 256, 0, h->stream>>>((const float*)frames_dev, m->Hin, m->Win, ob.H, plan->view_Wg, plan->view_in, 0, total);
-  SB_CHECK_LAUNCH(h);
-  return sb_conv_tc_launch(h, m, op_index, B);
 }
 
 // Shared memory of one k_head_1x1 launch: the weight bank, the output staging and the bias, plus a per-warp ring of n_ring
@@ -2084,8 +1817,6 @@ static const void* head_kernel(int nt, int kch) {
   }
 #undef SB_HEAD_CASE
 }
-
-int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);
 
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   m->tc_plans.assign(m->ops.size(), nullptr);
@@ -2211,35 +1942,7 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
         plan->out_dead = !read;
       }
   }
-  for (size_t oi = 0; oi + 1 < m->ops.size() && !split; ++oi)   // precision 2: the first conv runs on k_conv_first / k_conv_direct in fp32
-    if (m->ops[oi].kind() == SB_OPK_PREPROCESS) {
-      const int cv = sb_first_fusion_op(m, oi);
-      if (cv >= 0 && !m->tc_plans[cv]) {
-        const int rc = first_view_prepare(h, m, cv);
-        if (rc) return rc;
-      }
-      // not fusable with PREPROCESS (resize / channel conversion first): Toeplitz view of the preprocessed one-channel buffer
-      if (cv < 0 && oi + 1 < m->ops.size() && m->ops[oi + 1].kind() == SB_OPK_CONV && m->ops[oi + 1].in_buf() == m->ops[oi].out_buf() &&
-          m->ops[oi + 1].in_C() == 1 && !m->tc_plans[oi + 1]) {
-        const int rc = first_view_prepare(h, m, (int)oi + 1, true);
-        if (rc) return rc;
-      }
-      const int sv = sb_stem_fusion_op(m, oi);
-      if (sv >= 0 && !m->tc_plans[sv]) {
-        const int rc = stem_view_prepare(h, m, sv);
-        if (rc) return rc;
-      }
-    }
-  // fused first encoder block: frame -> conv0 -> conv1 -> pool in one kernel (sb_conv01.cu) when conv1's own output is dead
-  for (size_t oi = 0; oi + 2 < m->ops.size() && !split; ++oi)
-    if (m->ops[oi].kind() == SB_OPK_PREPROCESS) {
-      const int cv = sb_first_fusion_op(m, oi);
-      if (cv >= 0 && cv + 1 < (int)m->ops.size() && m->ops[cv + 1].kind() == SB_OPK_CONV && m->tc_plans[cv + 1]) {
-        const int rc = sb_conv01_prepare(h, m, cv, cv + 1, m->tc_plans[cv + 1]->out_dead);
-        if (rc) return rc;
-      }
-    }
-  return sb_conv_tc_autotune(h, m);
+  return 0;
 }
 
 // Programmatic dependent launch (sb_tc_prims.cuh): every conv launch carries the attribute (its producer thread waits on
@@ -2272,31 +1975,32 @@ static void launch_form(const TcLaunch& L, int B, cudaStream_t stream, int skip_
   sb_launch_pdl(form_kernel(L.form, P.KC, P.N), grid, dim3(F.threads), smem, stream, args);
 }
 
-// Picks, for every tensor-core conv launch (each transposed-conv phase included), the fastest eligible kernel form 0-3,
-// for a transposed conv its four phase launches or the fused form 4, for a first layer with a Toeplitz view the faster
-// of the view + tensor-core conv and k_conv_first, and for the first encoder block the fused k_conv01 or the separate
-// launches, by timing them on the device at the configured batch (buffers are already allocated; their contents do not
-// matter for timing).
-int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
+int sb_time_min(sb_handle_s* h, const char* what, float& best, const std::function<int()>& run) {
   cudaEvent_t e0, e1;
   SB_CUDA(h, cudaEventCreate(&e0));
   SB_CUDA(h, cudaEventCreate(&e1));
-  // the time of run() in ms: 4 synchronised runs, the first dropped, the minimum of the others
+  best = 1e30f;
+  int rc = 0;
+  for (int rep = 0; rep < 4 && !rc; ++rep) {
+    cudaEventRecord(e0, h->stream);
+    if ((rc = run())) break;
+    cudaEventRecord(e1, h->stream);
+    if (cudaError_t e = cudaStreamSynchronize(h->stream); e != cudaSuccess)
+      rc = sb_fail(h, SB_ERR_CUDA, "autotune launch (%s) failed: %s", what, cudaGetErrorString(e));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    if (rep > 0) best = std::min(best, ms);
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  return rc;
+}
+
+// Picks, for every tensor-core conv launch (each transposed-conv phase included), the fastest eligible kernel form 0-3,
+// then for a transposed conv its four phase launches or the fused form 4, by timing them on the device at the
+// configured batch (buffers are already allocated; their contents do not matter for timing).
+int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   char what[64];
-  auto time_min = [&](float& best, auto run) -> int {
-    best = 1e30f;
-    for (int rep = 0; rep < 4; ++rep) {
-      cudaEventRecord(e0, h->stream);
-      if (const int rc = run()) return rc;
-      cudaEventRecord(e1, h->stream);
-      cudaError_t e = cudaStreamSynchronize(h->stream);
-      if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "autotune launch (%s) failed: %s", what, cudaGetErrorString(e));
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, e0, e1);
-      if (rep > 0) best = std::min(best, ms);
-    }
-    return 0;
-  };
   const bool dbg = getenv("SB_DEBUG") != nullptr;
   const char* fvar = getenv("SB_FORCE_VARIANT");
   const int force = fvar ? atoi(fvar) : -1;
@@ -2314,7 +2018,7 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
           if (!L.forms[f].ok) continue;
           L.form = f;
           snprintf(what, sizeof what, "op %zu, %s form", oi, form_name[f]);
-          const int rc = time_min(best[f], [&] {
+          const int rc = sb_time_min(h, what, best[f], [&] {
             launch_form(L, m->B, h->stream, plan->out_dead && list == &plan->launches);
             return 0;
           });
@@ -2340,50 +2044,13 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
     for (int f = 0; f < 2; ++f) {
       L0.form = f ? kTconvForm : phase_form;
       snprintf(what, sizeof what, "op %zu, %s", oi, f ? "fused tconv" : "tconv phases");
-      if (const int rc = time_min(best[f], [&] { return sb_conv_tc_launch(h, m, (int)oi, m->B); })) return rc;
+      if (const int rc = sb_time_min(h, what, best[f], [&] { return sb_conv_tc_launch(h, m, (int)oi, m->B); })) return rc;
     }
     L0.form = (force >= 0 ? force == kTconvForm : best[1] < best[0]) ? kTconvForm : phase_form;
     if (dbg)
       fprintf(stderr, "[sb_conv_tc] op %zu launches (4 tconv phases) %.1f us, fused k_tconv_wg_hw %.1f us -> %s\n", oi, best[0] * 1e3f,
               best[1] * 1e3f, L0.form == kTconvForm ? "tconv-fused" : "phases");
   }
-  for (size_t oi = 0; oi < m->tc_plans.size(); ++oi) {
-    SbConvTcPlan* plan = m->tc_plans[oi];
-    if (!plan || !plan->view_in || plan->s2d || plan->from_buffer || !m->frames_dev) continue;
-    float best[2];
-    for (int f = 0; f < 2; ++f) {
-      snprintf(what, sizeof what, "first layer, form %d", f);
-      const int rc = time_min(best[f], [&] {
-        return f == 0 ? sb_first_direct_launch(h, m, (int)oi, m->frames_dev, 1, m->B)
-                      : sb_first_view_launch(h, m, (int)oi, m->frames_dev, 1, m->B);
-      });
-      if (rc) return rc;
-    }
-    plan->view_enabled = best[1] < best[0];
-    if (dbg) fprintf(stderr, "[sb_conv_tc] op %zu first layer: k_conv_first %.1f us, Toeplitz view + wgmma %.1f us -> %s\n", oi,
-                     best[0] * 1e3f, best[1] * 1e3f, plan->view_enabled ? "view" : "direct");
-  }
-  // fused first block (k_conv01) against its two separate launches (whatever forms were just picked for them)
-  if (m->conv01 && m->frames_dev) {
-    const int c1op = sb_conv01_conv1_op(m), c0op = c1op - 1;
-    float best[2];
-    for (int f = 0; f < 2; ++f) {
-      snprintf(what, sizeof what, "first block, fused %d", f);
-      const int rc = time_min(best[f], [&] {
-        if (f == 1) return sb_conv01_launch(h, m, m->frames_dev, 1, m->B);
-        const int rc0 = sb_first_view_can(m, c0op) ? sb_first_view_launch(h, m, c0op, m->frames_dev, 1, m->B)
-                                                   : sb_first_direct_launch(h, m, c0op, m->frames_dev, 1, m->B);
-        return rc0 ? rc0 : sb_conv_tc_launch(h, m, c1op, m->B);
-      });
-      if (rc) return rc;
-    }
-    m->conv01_enabled = best[1] < best[0];
-    if (const char* fv = getenv("SB_FORCE_CONV01")) m->conv01_enabled = atoi(fv) != 0;
-    if (dbg) fprintf(stderr, "[sb_conv_tc] first block (B = %d): conv0 + conv1 launches %.1f us, fused k_conv01 %.1f us -> %s\n", m->B,
-                     best[0] * 1e3f, best[1] * 1e3f, m->conv01_enabled ? "fused" : "separate");
-  }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   return 0;
 }
 

@@ -121,99 +121,6 @@ __global__ void __launch_bounds__(256) k_conv_direct(
   }
 }
 
-// First layer fused with InferenceLayer.preprocess (inference.py:940-967) for the common case
-// "no channel conversion, no resize": raw uint8 (or float) frame -> * (1/255) -> zero pad to the
-// net size -> 3x3 SAME conv + bias + ReLU -> fp16 NHWC.  One output pixel per thread, all COUT
-// channels in registers; the frame is read once from HBM (neighbour re-reads hit L1), the output
-// is written once, so the kernel runs at HBM speed instead of paying a separate preprocess pass.
-template <typename TI, int CIN, int COUT, int PX>
-__global__ void __launch_bounds__(256) k_conv_first(const TI* __restrict__ img, int Hin, int Win, int Hnet, int Wnet,
-                                                    __half* __restrict__ out, int out_Ctot, int out_coff,
-                                                    const float* __restrict__ w /*[9][CIN][COUT]*/,
-                                                    const float* __restrict__ bias, int relu, int in_is_u8, int split = 0) {
-  // each thread: PX horizontally adjacent output pixels x COUT channels (weights read once from
-  // shared memory per PX pixels; the thread's PX*COUT fp16 outputs are contiguous in NHWC)
-  __shared__ __align__(16) float s_w[9 * CIN * COUT];
-  __shared__ float s_b[COUT];
-  for (int t = threadIdx.y * 32 + threadIdx.x; t < 9 * CIN * COUT; t += 256) s_w[t] = w[t];
-  for (int t = threadIdx.y * 32 + threadIdx.x; t < COUT; t += 256) s_b[t] = bias ? bias[t] : 0.f;
-  __syncthreads();
-  const int ox0 = (blockIdx.x * 32 + threadIdx.x) * PX, oy = blockIdx.y * 8 + threadIdx.y, b = blockIdx.z;
-  if (ox0 >= Wnet || oy >= Hnet) return;
-  const TI* im = img + (size_t)b * Hin * Win * CIN;
-  const float sc = in_is_u8 ? (1.0f / 255.0f) : 1.0f;
-  float acc[PX][COUT];
-#pragma unroll
-  for (int p = 0; p < PX; ++p)
-#pragma unroll
-    for (int c = 0; c < COUT; ++c) acc[p][c] = s_b[c];
-#pragma unroll
-  for (int ky = 0; ky < 3; ++ky) {
-    const int iy = oy + ky - 1;
-    if (iy < 0 || iy >= Hin) continue;                       // SAME padding / bottom zero pad
-    float in[PX + 2][CIN];
-#pragma unroll
-    for (int j = 0; j < PX + 2; ++j) {
-      const int ix = ox0 + j - 1;
-      const bool ok = ix >= 0 && ix < Win;
-#pragma unroll
-      for (int ci = 0; ci < CIN; ++ci)
-        in[j][ci] = ok ? __fmul_rn((float)im[((size_t)iy * Win + ix) * CIN + ci], sc) : 0.f;
-    }
-#pragma unroll
-    for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-      for (int ci = 0; ci < CIN; ++ci) {
-        const float4* w4 = reinterpret_cast<const float4*>(s_w + ((ky * 3 + kx) * CIN + ci) * COUT);
-#pragma unroll
-        for (int q = 0; q < COUT / 4; ++q) {
-          const float4 ww = w4[q];
-#pragma unroll
-          for (int p = 0; p < PX; ++p) {
-            const float v = in[p + kx][ci];
-            acc[p][4 * q + 0] = fmaf(v, ww.x, acc[p][4 * q + 0]);
-            acc[p][4 * q + 1] = fmaf(v, ww.y, acc[p][4 * q + 1]);
-            acc[p][4 * q + 2] = fmaf(v, ww.z, acc[p][4 * q + 2]);
-            acc[p][4 * q + 3] = fmaf(v, ww.w, acc[p][4 * q + 3]);
-          }
-        }
-      }
-  }
-#pragma unroll
-  for (int p = 0; p < PX; ++p) {
-    if (ox0 + p >= Wnet) break;
-    __half* po = out + (((size_t)b * Hnet + oy) * Wnet + ox0 + p) * out_Ctot + out_coff;
-    if (split) {                                             // precision 2: [lo | hi | hi] planes, COUT channels apart
-#pragma unroll
-      for (int q = 0; q < COUT / 8; ++q) {
-        __align__(16) __half hh[8], ll[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float a = acc[p][8 * q + j];
-          if (relu) a = fmaxf(a, 0.f);
-          hh[j] = __float2half_rn(a);
-          ll[j] = __float2half_rn(a - __half2float(hh[j]));
-        }
-        reinterpret_cast<uint4*>(po)[q] = *reinterpret_cast<uint4*>(ll);
-        reinterpret_cast<uint4*>(po + COUT)[q] = *reinterpret_cast<uint4*>(hh);
-        reinterpret_cast<uint4*>(po + 2 * COUT)[q] = *reinterpret_cast<uint4*>(hh);
-      }
-      continue;
-    }
-#pragma unroll
-    for (int q = 0; q < COUT / 8; ++q) {
-      __align__(16) __half2 h[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float a = acc[p][8 * q + 2 * j], c2 = acc[p][8 * q + 2 * j + 1];
-        if (relu) { a = fmaxf(a, 0.f); c2 = fmaxf(c2, 0.f); }
-        h[j] = __floats2half2_rn(a, c2);
-      }
-      reinterpret_cast<uint4*>(po)[q] = *reinterpret_cast<uint4*>(h);
-    }
-  }
-}
-
 // Conv2DTranspose(k, strides=2, padding="same"), k = 3 or 4: out (2H, 2W), out[o] += in[i] * W[o - 2i + p] with the
 // forward-conv padding p = (k - 2) / 2 (0 for k3, 1 for k4).  Per axis:
 //   k3: out[2i] = in[i]*W[0] + in[i-1]*W[2];            out[2i+1] = in[i]*W[1]

@@ -52,7 +52,7 @@ void sb_models_free(sb_handle_s* h) {
     sb_post_ws_free(m->ws);
     sb_gather_free(m);
     sb_topdown_free(m);
-    sb_conv01_release(m);
+    sb_entry_release(m);
     sb_conv_tc_release(m);
     delete m;
   }
@@ -114,6 +114,9 @@ int sb_load_model(sb_handle_t h, const int32_t* ops, int n_ops, const float* wei
       if (op.kind() == SB_OPK_PREPROCESS && (op.pre_mode() < SB_PRE_PLAIN || op.pre_mode() > SB_PRE_IMAGENET_CAFFE_GRAY)) {
         delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: bad preprocess mode", i);
       }
+      if (op.kind() == SB_OPK_PREPROCESS && std::any_of(m->ops.begin(), m->ops.end(), [](const SbOp& o) { return o.kind() == SB_OPK_PREPROCESS; })) {
+        delete m; return sb_fail(h, SB_ERR_INVALID, "op %d: a second preprocess op", i);
+      }
       auto okoff = [&](int off, int64_t n) { return off < 0 ? true : (int64_t)off + n <= n_weights; };
       if (op.kind() == SB_OPK_CONV || op.kind() == SB_OPK_TCONV) {
         const int64_t nw = (int64_t)op.k() * op.k() * op.in_C() * op.out_C();
@@ -166,8 +169,7 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes): re-init after a reconfigure
   m->configured = false;
   m->bu_configured = false; m->gl_configured = false; m->ce_configured = false; m->td_configured = false;
-  sb_conv01_release(m);
-  m->conv01_enabled = false;
+  sb_entry_release(m);
   sb_conv_tc_release(m);
   m->B = max_batch; m->Hin = H; m->Win = W; m->Cin = C_in; m->Hres = Hres; m->Wres = Wres; m->Hnet = Hnet; m->Wnet = Wnet;
   size_t total = 0;
@@ -181,6 +183,9 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   m->act_bytes = total;
   SB_CUDA(h, cudaMalloc(&m->frames_dev, (size_t)max_batch * H * W * C_in * sizeof(float)));
   int rc = sb_conv_tc_prepare(h, m);
+  if (!rc) rc = sb_entry_prepare(h, m);
+  if (!rc) rc = sb_conv_tc_autotune(h, m);
+  if (!rc) rc = sb_entry_autotune(h, m);
   if (rc) return rc;
   m->configured = true;
   return SB_OK;
@@ -188,90 +193,11 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
 
 }  // extern "C"
 
-// First conv fused with preprocessing (fp16 path): returns the conv op index or -1.
-static int first_fusion_op(const SbModel* m, size_t pre_index) { return sb_first_fusion_op(m, pre_index); }
-int sb_first_fusion_op(const SbModel* m, size_t pre_index) {
-  if (m->precision == 1 || getenv("SB_DISABLE_FIRST_FUSION")) return -1;
-  if (pre_index + 1 >= m->ops.size()) return -1;
-  const SbOp& pre = m->ops[pre_index];
-  const SbOp& cv = m->ops[pre_index + 1];
-  if (cv.kind() != SB_OPK_CONV || cv.in_buf() != pre.out_buf() || cv.k() != 3 || cv.stride() != 1 || cv.explicit_pad()) return -1;
-  if (pre.input_scale() != 1.0f || pre.pre_mode() != SB_PRE_PLAIN) return -1;
-  const SbBuffer& ib = m->buffers[pre.out_buf()];
-  const SbBuffer& ob = m->buffers[cv.out_buf()];
-  if (m->Cin != ib.C || (ib.C != 1 && ib.C != 3) || cv.in_C() != ib.C) return -1;
-  if (ob.f32 || (cv.flags() & SB_OPF_BN) || ob.C % 8 || cv.out_coff() % 8) return -1;
-  const int co = cv.out_C();
-  if (!(co == 8 || co == 16 || co == 24 || co == 32 || co == 64)) return -1;
-  for (size_t i = pre_index + 2; i < m->ops.size(); ++i)      // nobody else may read the preprocessed frame
-    if (m->ops[i].kind() != SB_OPK_PREPROCESS && (m->ops[i].in_buf() == pre.out_buf() ||
-        (m->ops[i].kind() == SB_OPK_ADD && m->ops[i].in2_buf() == pre.out_buf()))) return -1;
-  return (int)pre_index + 1;
-}
-
-// 7x7 stride-2 stem right after PREPROCESS (hourglass.py:49-100) with 1 / 3 input channels and no resize: the conv op
-// index when the tensor-core space-to-depth form can take it (the PREPROCESS op is then fused into the view kernel).
-int sb_stem_fusion_op(const SbModel* m, size_t pre_index) {
-  if (m->precision != 0 || pre_index + 1 >= m->ops.size()) return -1;
-  const SbOp& pre = m->ops[pre_index];
-  const SbOp& cv = m->ops[pre_index + 1];
-  // SAME padding (hourglass) or the ResNet stem's explicit 3|3 padding after ImageNet preprocessing
-  if (cv.kind() != SB_OPK_CONV || cv.in_buf() != pre.out_buf() || cv.k() != 7 || cv.stride() != 2) return -1;
-  if (cv.explicit_pad() && (cv.pad_top() != 3 || cv.pad_left() != 3)) return -1;
-  if (pre.input_scale() != 1.0f) return -1;
-  const SbBuffer& ib = m->buffers[pre.out_buf()];
-  if (pre.pre_mode() == SB_PRE_PLAIN ? (m->Cin != ib.C || (ib.C != 1 && ib.C != 3))
-                                     : (ib.C != 3 || (m->Cin != 1 && m->Cin != 3))) return -1;
-  if (cv.in_C() != ib.C) return -1;
-  for (size_t i = pre_index + 2; i < m->ops.size(); ++i)      // nobody else may read the preprocessed frame
-    if (m->ops[i].kind() != SB_OPK_PREPROCESS && (m->ops[i].in_buf() == pre.out_buf() ||
-        (m->ops[i].kind() == SB_OPK_ADD && m->ops[i].in2_buf() == pre.out_buf()))) return -1;
-  return (int)pre_index + 1;
-}
-
-template <typename TI, int CIN>
-static void launch_first(int co, int B, cudaStream_t s, const TI* img, int Hin, int Win, int Hnet, int Wnet, __half* out,
-                         int Ctot, int coff, const float* w, const float* b, int relu, int is_u8, int split) {
-  dim3 blk(32, 8);
-  auto grid = [&](int px) { return dim3((Wnet + 32 * px - 1) / (32 * px), (Hnet + 7) / 8, B); };
-  switch (co) {
-    case 8: k_conv_first<TI, CIN, 8, 4><<<grid(4), blk, 0, s>>>(img, Hin, Win, Hnet, Wnet, out, Ctot, coff, w, b, relu, is_u8, split); break;
-    case 16: k_conv_first<TI, CIN, 16, 4><<<grid(4), blk, 0, s>>>(img, Hin, Win, Hnet, Wnet, out, Ctot, coff, w, b, relu, is_u8, split); break;
-    case 24: k_conv_first<TI, CIN, 24, 2><<<grid(2), blk, 0, s>>>(img, Hin, Win, Hnet, Wnet, out, Ctot, coff, w, b, relu, is_u8, split); break;
-    case 32: k_conv_first<TI, CIN, 32, 2><<<grid(2), blk, 0, s>>>(img, Hin, Win, Hnet, Wnet, out, Ctot, coff, w, b, relu, is_u8, split); break;
-    default: k_conv_first<TI, CIN, 64, 1><<<grid(1), blk, 0, s>>>(img, Hin, Win, Hnet, Wnet, out, Ctot, coff, w, b, relu, is_u8, split); break;
-  }
-}
-
-// CUDA-core first layer fused with preprocessing (k_conv_first): the fallback of, and the timing rival
-// to, the Toeplitz tensor-core form (sb_first_view_launch).
-int sb_first_direct_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
-  const SbOp& op = m->ops[op_index];
-  SbBuffer& ob = m->buffers[op.out_buf()];
-  cudaStream_t s = h->stream;
-  const float* Wt = m->weights_dev + op.w_off();
-  const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-  const int g = B;
-  const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-  const int split = m->precision == 2 ? op.out_C() : 0;
-  // rows/cols beyond the resized frame (Hres, Wres) are the bottom/right zero padding
-  if (frames_are_u8) {
-    if (m->Cin == 1) launch_first<unsigned char, 1>(op.out_C(), g, s, (const unsigned char*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 1, split);
-    else launch_first<unsigned char, 3>(op.out_C(), g, s, (const unsigned char*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 1, split);
-  } else {
-    if (m->Cin == 1) launch_first<float, 1>(op.out_C(), g, s, (const float*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 0, split);
-    else launch_first<float, 3>(op.out_C(), g, s, (const float*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 0, split);
-  }
-  SB_CHECK_LAUNCH(h);
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------
 template <typename T>
 static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
   cudaStream_t s = h->stream;
   const bool split = m->precision == 2;         // split-fp16 activations: [lo | hi | hi] channel planes (sb_kernels_direct.cuh)
-  int fused_first = -1, fused_conv1 = -1, fused_stem = -1;
   for (size_t oi = 0; oi < m->ops.size(); ++oi) {
     const SbOp& op = m->ops[oi];
     if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[oi], s);
@@ -280,32 +206,13 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
     // 2x2 max-pool fused into the producing conv; residual ADD fused into the conv before it (unless that conv's own output
     // was asked for: it then stores its output and the ADD runs)
     if (oi < m->skip_op.size() && (m->skip_op[oi] == 1 || (m->skip_op[oi] == 2 && !m->keep_dead_stores))) continue;
-    if ((int)oi == fused_conv1) continue;                       // ran inside the fused first block
-    if ((int)oi == fused_stem) {                                // 7x7 s2 stem: frame -> space-to-depth view -> tensor cores
-      int rc = sb_stem_view_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
-      if (rc) return rc;
-      continue;
-    }
-    if ((int)oi == fused_first && sb_conv01_can(m, (int)oi) && !m->keep_dead_stores) {
-      int rc = sb_conv01_launch(h, m, frames_dev, frames_are_u8, B);
-      if (rc) return rc;
-      fused_conv1 = sb_conv01_conv1_op(m);
-      continue;
-    }
-    if ((int)oi == fused_first && sb_first_view_can(m, (int)oi)) {
-      int rc = sb_first_view_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
-      if (rc) return rc;
-      continue;
-    }
-    if ((int)oi == fused_first) {
-      int rc = sb_first_direct_launch(h, m, (int)oi, frames_dev, frames_are_u8, B);
+    if (m->entry.covers((int)oi)) {                             // the input stage (sb_entry.cu)
+      int rc = sb_entry_run(h, m, (int)oi, frames_dev, frames_are_u8, B);
       if (rc) return rc;
       continue;
     }
     switch (op.kind()) {
       case SB_OPK_PREPROCESS: {
-        if (sizeof(T) == 2 && (fused_first = first_fusion_op(m, oi)) >= 0) break;
-        if (sizeof(T) == 2 && sb_stem_view_can(m, sb_stem_fusion_op(m, oi))) { fused_stem = sb_stem_fusion_op(m, oi); break; }
         const size_t total = (size_t)B * ob.H * ob.W * ob.C;
         const int resize = op.input_scale() != 1.0f;
         int mode_ch = 0;
@@ -331,11 +238,6 @@ static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int fra
       }
       case SB_OPK_CONV: {
         SbBuffer& ib = m->buffers[op.in_buf()];
-        if (m->precision == 0 && sb_first_buffer_view_can(m, (int)oi)) {
-          int rc = sb_first_buffer_view_launch(h, m, (int)oi, B);
-          if (rc) return rc;
-          break;
-        }
         if (m->precision != 1 && sb_conv_tc_can(m, (int)oi)) {
           int rc = sb_conv_tc_launch(h, m, (int)oi, B);
           if (rc) return rc;
@@ -471,6 +373,14 @@ __global__ void k_half_to_float(const __half* __restrict__ in, float* __restrict
     out[t] = __half2float(in[t]);
 }
 
+// Buffer `id` is not always written: a tensor-core conv's dead output, or a tensor inside the fused first block.
+static bool stores_elided(const SbModel* m, int id) {
+  for (size_t oi = 0; oi < m->ops.size(); ++oi)
+    if (sb_conv_tc_out_dead(m, (int)oi) && m->ops[oi].out_buf() == id) return true;
+  const SbEntryPlan& e = m->entry;
+  return e.conv01 && (id == m->ops[e.conv_op].out_buf() || id == m->ops[e.conv_op + 1].out_buf());
+}
+
 static int upload_frames(sb_handle_s* h, SbModel* m, const void* images_host, int is_u8, int B) {
   const size_t bytes = (size_t)B * m->Hin * m->Win * m->Cin * (is_u8 ? 1 : 4);
   SB_CUDA(h, cudaMemcpyAsync(m->frames_dev, images_host, bytes, cudaMemcpyHostToDevice, h->stream));
@@ -488,12 +398,8 @@ int sb_model_forward(sb_handle_t h, int model_id, const void* images_host, int i
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
   if (rc) return rc;
-  for (int i = 0; i < n_outputs; ++i) {                  // a tensor nobody reads inside the graph is only written on request
-    if (output_buffer_ids[i] >= 0 && sb_conv_tc_out_dead(m, output_buffer_ids[i])) m->keep_dead_stores = true;
-    if (m->conv01 && output_buffer_ids[i] >= 0 && output_buffer_ids[i] < (int)m->buffers.size() &&
-        (output_buffer_ids[i] == m->ops[sb_conv01_conv1_op(m)].in_buf() || output_buffer_ids[i] == m->ops[sb_conv01_conv1_op(m)].out_buf()))
-      m->keep_dead_stores = true;                          // tensors internal to the fused first block
-  }
+  for (int i = 0; i < n_outputs; ++i)                    // a tensor nobody reads inside the graph is only written on request
+    if (stores_elided(m, output_buffer_ids[i])) m->keep_dead_stores = true;
   rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B);
   m->keep_dead_stores = false;
   if (rc) return rc;

@@ -1,6 +1,7 @@
-// Internal model structures (op-list, buffers) shared by sb_model.cu and sb_conv_tc.cu.
+// Internal model structures (op-list, buffers) shared by sb_model.cu, sb_entry.cu, sb_conv_tc.cu and sb_conv01.cu.
 // The int32 record layout must match sleap_b200/nn/oplist.py.
 #pragma once
+#include <functional>
 #include <vector>
 
 #include "sb_common.cuh"
@@ -72,6 +73,29 @@ struct SbConvTcPlan;  // sb_conv_tc.cu
 struct SbConv01Plan;  // sb_conv01.cu
 struct SbTopdown;     // sb_topdown.cu
 
+// The input stage (sb_entry.cu): how a forward pass gets from the raw frame to the first activation the op loop reads.
+// Resolved and timed once by sb_model_configure; run_ops_t hands every op it covers to sb_entry_run.
+enum {
+  SB_ENTRY_GENERIC = 0,    // k_preprocess as an ordinary op, then the op loop
+  SB_ENTRY_DIRECT,         // k_conv_first: the first conv on the CUDA cores, preprocessing fused
+  SB_ENTRY_FRAME_VIEW,     // k_first_view of the frame, then the first conv as a Toeplitz GEMM on the tensor cores
+  SB_ENTRY_BUFFER_VIEW,    // k_preprocess, k_first_view of its one-channel output, then the Toeplitz GEMM
+  SB_ENTRY_STEM_VIEW,      // k_s2d_view of the frame, then the 7x7 stride-2 stem as a 4x4 GEMM on the tensor cores
+};
+struct SbEntryPlan {
+  int route = SB_ENTRY_GENERIC;
+  int pre_op = -1;                 // the PREPROCESS op when the first conv's launch preprocesses the frame (an empty slot)
+  int conv_op = -1;                // the first conv, unless the route is generic
+  int conv1_op = -1;               // conv1 when the fused first block won: an empty slot, k_conv01 runs in conv_op's
+                                   // (unless the forward asks for a tensor inside the block: keep_dead_stores)
+  SbConv01Plan* conv01 = nullptr;  // fused first encoder block k_conv01 over conv_op and conv_op + 1 (sb_conv01.cu)
+  __half* view = nullptr;          // view routes: the [B][view_H][view_W][16] fp16 view the GEMM reads
+  float* view_bias = nullptr;      // Toeplitz view: the bias replicated over the 8 pixels of a group
+  int view_H = 0, view_W = 0;
+  int pre_mode = SB_PRE_PLAIN;     // stem view: the PREPROCESS mode k_s2d_view applies
+  bool covers(int oi) const { return oi == pre_op || oi == conv_op || oi == conv1_op; }
+};
+
 struct SbModel {
   int precision = 0;  // 0: fp16 activations + tensor-core convs; 1: fp32 CUDA-core path
   std::vector<SbOp> ops;
@@ -112,8 +136,7 @@ struct SbModel {
   bool ce_configured = false;
   bool td_configured = false;              // fused top-down pipeline (sb_topdown_configure); state lives on the centroid model
   SbTopdown* td = nullptr;
-  SbConv01Plan* conv01 = nullptr;          // fused first encoder block (frame -> conv0 -> conv1 -> pool), sb_conv01.cu
-  bool conv01_enabled = false;             // the autotuner measured it faster than the two separate launches
+  SbEntryPlan entry;                       // input stage (sb_entry.cu)
   SbGather gather;                         // peer-memory exchange of the result records (sb_gather.cu)
   bool keep_dead_stores = false;           // sb_model_forward asked for a tensor whose stores are normally elided
   // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu); its per-frame track records
@@ -138,30 +161,36 @@ void sb_pipeline_slots_free(SbModel* m);
 
 // tensor-core conv path (sb_conv_tc.cu)
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m);      // after buffers are allocated
+int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);     // launch forms of every plan, the input stage's included
 void sb_conv_tc_release(SbModel* m);
 bool sb_conv_tc_can(const SbModel* m, int op_index);
-bool sb_conv_tc_out_dead(const SbModel* m, int buffer_id);   // its stores are elided unless keep_dead_stores is set
+bool sb_conv_tc_out_dead(const SbModel* m, int op_index);    // its stores are elided unless keep_dead_stores is set
 int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B);
+// A stride-1 R x S convolution over a [B][H][W][16] fp16 view that is not an op-list buffer, as the plan of op
+// `op_index`: output pixel (y, x) takes tap (r, s) from view pixel (y + dy0 + r, x + dx0 + s), with the weights
+// w[r * S + s] ([R * S][Cout][16]).  Leaves the op without a plan where the view is smaller than one TMA box.
+struct SbTcView {
+  SbBuffer in;                     // the view (C = 16)
+  SbBuffer out;                    // the output tensor as the GEMM sees it (C = its row pitch)
+  int Cout = 0, out_coff = 0;
+  int R = 0, S = 0, dy0 = 0, dx0 = 0;
+  const float *bias = nullptr, *bn_scale = nullptr, *bn_shift = nullptr;
+  int relu = 0;
+};
+int sb_conv_tc_view_prepare(sb_handle_s* h, SbModel* m, int op_index, const SbTcView& v, const std::vector<float>& w);
+void sb_conv_tc_drop(SbModel* m, int op_index);          // frees the op's plan
+// configure-time timing: the time of run() in ms, 4 synchronised runs, the first dropped, the minimum of the others
+int sb_time_min(sb_handle_s* h, const char* what, float& best, const std::function<int()>& run);
 
-// first conv fused with the PREPROCESS op before it (sb_model.cu): conv op index or -1
-int sb_first_fusion_op(const SbModel* m, size_t pre_index);
-// first layer as a Toeplitz GEMM on the stock tensor-core conv kernel (sb_conv_tc.cu)
-bool sb_first_view_can(const SbModel* m, int op_index);
-int sb_first_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
-bool sb_first_buffer_view_can(const SbModel* m, int op_index);
-int sb_first_buffer_view_launch(sb_handle_s* h, SbModel* m, int op_index, int B);
-int sb_first_direct_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
+// input stage (sb_entry.cu)
+int sb_entry_prepare(sb_handle_s* h, SbModel* m);       // after sb_conv_tc_prepare: route, views, fused block
+int sb_entry_autotune(sb_handle_s* h, SbModel* m);      // after sb_conv_tc_autotune: direct vs view, fused vs separate
+int sb_entry_run(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
+void sb_entry_release(SbModel* m);
 
-// 7x7 stride-2 stem through a space-to-depth view of the frame (sb_conv_tc.cu); conv op index or -1 (sb_model.cu)
-int sb_stem_fusion_op(const SbModel* m, size_t pre_index);
-bool sb_stem_view_can(const SbModel* m, int op_index);
-int sb_stem_view_launch(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
-
-// fused first encoder block (sb_conv01.cu)
-int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op, bool conv1_out_dead);
+// fused first encoder block, run by the input stage (sb_conv01.cu)
+int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op);   // sets m->entry.conv01
 void sb_conv01_release(SbModel* m);
-bool sb_conv01_can(const SbModel* m, int conv0_op);
-int sb_conv01_conv1_op(const SbModel* m);
 int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);
 
 // programmatic dependent launch for the conv kernels (sb_conv_tc.cu); SB_DISABLE_PDL=1 switches it off

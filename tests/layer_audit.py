@@ -283,7 +283,7 @@ class Audit:
         self.conv01_ops = self._conv01_ops()
         self.production = True
 
-    # ---- which kernels run (mirrors sb_first_fusion_op / sb_stem_fusion_op / the k_conv01 plan) ----
+    # ---- which kernels run (mirrors the input stage's rules in sb_entry.cu: first_fusable, stem_fusable, conv01_fusable) ----
     def _only_reader(self, buf, reader):
         for j, o in enumerate(self.ops):
             if j == reader or o[0] == ol.PREPROCESS:

@@ -79,7 +79,7 @@ def test_unet_forward_resize_and_rgb():
 
 def test_unet_forward_resize_fp16_first_layer_on_tensor_cores():
     """input_scale != 1 (and rgb -> gray): PREPROCESS runs as its own kernel and the first 3x3 conv takes the Toeplitz
-    tensor-core form from the preprocessed one-channel buffer (sb_first_buffer_view_launch) instead of k_conv_direct."""
+    tensor-core form from the preprocessed one-channel buffer (sb_entry.cu, buffer view route) instead of k_conv_direct."""
     from ctypes import byref, c_int, c_void_p
     import torch
     from sleap_b200 import _lib
@@ -434,8 +434,8 @@ def test_pipelined_predict_matches_per_batch():
 @pytest.mark.parametrize("cout,hw,as_float", [(16, (64, 128), False), (16, (38, 136), False), (8, (48, 256), False),
                                               (32, (64, 128), True), (24, (36, 160), False)])
 def test_first_layer_toeplitz_view(cout, hw, as_float, variant, monkeypatch):
-    """First conv (1 input channel) as a Toeplitz GEMM on the stock tensor-core kernel (sb_conv_tc.cu,
-    first_view_prepare) vs the torch-CPU fp32 conv on the fp16-rounded operands it consumes, and vs the
+    """First conv (1 input channel) as a Toeplitz GEMM on the stock tensor-core kernel (sb_entry.cu,
+    toeplitz_prepare) vs the torch-CPU fp32 conv on the fp16-rounded operands it consumes, and vs the
     CUDA-core k_conv_first (SB_DISABLE_FIRST_VIEW=1).  Covers every kernel variant, widths whose group
     count is not a tile multiple, float frames, and the bottom zero pad (H not a multiple of the stride)."""
     from ctypes import byref, c_int, c_void_p
@@ -484,6 +484,27 @@ def test_first_layer_toeplitz_view(cout, hw, as_float, variant, monkeypatch):
     scale = max(1.0, float(np.abs(want).max()))
     assert_allclose(got, want, atol=1.5e-3 * scale, rtol=0)          # fp16 output rounding (2^-11 relative)
     assert_allclose(got, direct, atol=4e-3 * scale, rtol=0)          # direct kernel keeps fp32 pixels / weights
+
+
+@pytest.mark.gpu
+def test_load_model_rejects_second_preprocess_op():
+    """The network has one input stage: an op list with a second PREPROCESS op is refused at load time."""
+    from ctypes import byref, c_int
+    from sleap_b200 import _lib
+    from sleap_b200.nn import oplist as ol
+    blob = np.zeros(9 * 8 + 8, np.float32)
+    recs = [ol.buffer_record(0, 1, 1, 0, 1), ol.buffer_record(1, 1, 8, 0, 0), ol.preprocess_record(0, 1, 1.0, 1),
+            ol.conv_record(0, 0, 1, 1, 0, 8, 3, 1, True, 0, 72)]
+    h = _lib.Handle(0)
+    try:
+        mid = c_int(-1)
+        ops = np.ascontiguousarray(np.stack(recs).astype(np.int32))
+        h.call("sb_load_model", _lib.ptr(ops), ops.shape[0], _lib.ptr(blob), int(blob.size), 0, byref(mid))
+        ops = np.ascontiguousarray(np.stack(recs + [ol.preprocess_record(0, 1, 1.0, 1)]).astype(np.int32))
+        with pytest.raises(_lib.SleapB200Error, match="second preprocess"):
+            h.call("sb_load_model", _lib.ptr(ops), ops.shape[0], _lib.ptr(blob), int(blob.size), 0, byref(mid))
+    finally:
+        h.close()
 
 
 @pytest.mark.parametrize("hw,as_float,relu", [((64, 64), False, True), ((34, 1056), False, True), ((96, 520), True, True),
@@ -554,7 +575,7 @@ def test_conv01_fused_first_block(hw, as_float, relu, monkeypatch):
 @pytest.mark.parametrize("cin,cout,hw,as_float,bn", [(3, 32, (64, 96), False, True), (1, 16, (70, 130), False, False), (3, 128, (96, 64), True, True)])
 def test_tc_stem_7x7_stride2(cin, cout, hw, as_float, bn):
     """Hourglass stem (hourglass.py:49-100): 7x7 stride-2 SAME convolution on 1 / 3 input channels as a 4x4 convolution over
-    the space-to-depth view of the frame on the tensor-core path (sb_conv_tc.cu, stem_view_prepare), conv -> ReLU -> BN affine.
+    the space-to-depth view of the frame on the tensor-core path (sb_entry.cu, stem_prepare), conv -> ReLU -> BN affine.
     Reference: torch conv2d with TF SAME padding (2 before, 3 after for even sizes) on the fp16-rounded operands."""
     from ctypes import byref, c_int, c_void_p
     import torch
