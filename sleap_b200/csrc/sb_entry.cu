@@ -455,7 +455,8 @@ int sb_entry_autotune(sb_handle_s* h, SbModel* m) {
       });
       if (rc) return rc;
     }
-    const bool view = best[1] < best[0];
+    bool view = best[1] < best[0];
+    if (const char* fv = getenv("SB_FORCE_FIRST_VIEW")) view = atoi(fv) != 0;
     if (dbg) fprintf(stderr, "[sb_conv_tc] op %d first layer: k_conv_first %.1f us, Toeplitz view + wgmma %.1f us -> %s\n", e.conv_op,
                      best[0] * 1e3f, best[1] * 1e3f, view ? "view" : "direct");
     if (!view) {

@@ -101,7 +101,8 @@ def check(dev, ref, e_pre, out, lo=None):
     worst = max |dev - ref| / (e_pre + rounding of the store), which must be <= 1;
     undecided-rounding misses: where [ref - e_pre, ref + e_pre] holds no fp16 rounding boundary, a correct kernel stores
     exactly fp16(ref) (hi for split outputs); any other value is counted in ``missed``;
-    exact = fraction equal to fp16(ref), bias = mean (dev - ref) / ulp16(ref) (fp16 outputs);
+    exact = fraction equal to fp16(ref), bias = mean (dev - ref) / ulp16(ref) (fp16 outputs; elements 0 on one side only
+    count 0), bias_at = its largest term as (index, device, reference, e_pre, ulps);
     lo_bias (split, reported): mean of sign(lo) (dev - ref) / ulp16(lo) over lo != 0."""
     dev = np.asarray(dev, np.float64)
     bound = e_pre + out_rounding(ref, e_pre, out)
@@ -119,7 +120,14 @@ def check(dev, ref, e_pre, out, lo=None):
             r["miss_at"] = (tuple(int(t) for t in k), float(dev[tuple(k)]), float(ref[tuple(k)]), float(e_pre[tuple(k)]))
     if out == "f16":
         r["exact"] = float((dev == f16(ref)).mean()) if dev.size else 1.0
-        r["bias"] = float(((dev - ref) / ulp16(ref)).mean()) if dev.size else 0.0
+        # An element that is 0 on one side only is a ReLU whose pre-activation lies within e_pre of 0: its error in ulps of
+        # a reference of 0 (2^-24) runs to thousands however small, and says nothing about the store's rounding direction;
+        # the bound gates it.  So the bias leaves those out.
+        u = np.where((dev == 0) == (ref == 0), (dev - ref) / ulp16(ref), 0.0)
+        r["bias"] = float(u.mean()) if dev.size else 0.0
+        if dev.size:
+            k = np.unravel_index(int(np.abs(u).argmax()), u.shape)
+            r["bias_at"] = (tuple(int(t) for t in k), float(dev[k]), float(ref[k]), float(e_pre[k]), float(u[k]))
     if out == "split" and lo is not None:
         nz = lo != 0
         r["lo_bias"] = float((np.sign(lo[nz]) * (dev[nz] - ref[nz]) / ulp16(lo[nz])).mean()) if nz.any() else 0.0

@@ -45,7 +45,7 @@ def _op_kinds(model, B, H, W, C):
 
 def _fetch(model, aud, imgs, ids):
     from sleap_b200._lib import ptr
-    outs = [np.zeros(aud.shape(b), np.float32) for b in ids]
+    outs = [np.zeros((imgs.shape[0],) + aud.shape(b)[1:], np.float32) for b in ids]
     ptrs = (c_void_p * len(outs))(*[o.ctypes.data for o in outs])
     model.handle.call("sb_model_forward", model.model_id, ptr(np.ascontiguousarray(imgs)), int(imgs.dtype == np.uint8),
                       imgs.shape[0], len(outs), ptr(np.asarray(ids, np.int32)), ptrs)
@@ -68,12 +68,15 @@ def _gate(rows, label):
         assert r.get("missed", 0) == 0, f"{tag}: {r['missed']} elements differ from fp16(reference) where the bound decides the rounding, first (index, device, reference, e_pre) = {r.get('miss_at')}"
         if r.get("out") == "f16" and r["n"] >= STAT_MIN_N:
             assert r["exact"] >= EXACT_MIN, f"{tag}: exact-match fraction {r['exact']:.4f}"
-            assert abs(r["bias"]) <= BIAS_MAX, f"{tag}: mean signed error {r['bias']:.4f} ulp"
+            assert abs(r["bias"]) <= BIAS_MAX, f"{tag}: mean signed error {r['bias']:.4f} ulp, largest (index, device, reference, e_pre, ulps) = {r.get('bias_at')}"
 
 
 def _audit(spec, in_ch, imgs, precision, capfd, monkeypatch, env=(), expect=None, all_buffers=True, input_scale=1.0, seed=5,
-           weights=None):
-    """``weights``: a weight dict (e.g. a trained model's); None = la.synthetic_weights(seed)."""
+           weights=None, max_batch=None):
+    """``weights``: a weight dict (e.g. a trained model's); None = la.synthetic_weights(seed).
+    ``max_batch``: configure (and autotune) at this batch and audit ``imgs`` at their own, smaller batch, after a poison
+    forward of ``max_batch`` other frames (constant 255, or floats around 50) with every buffer fetched, so that every
+    slot past the audited frames, the fusion-internal buffers included, holds stale data of another magnitude."""
     from sleap_b200.nn import architectures as A
     from sleap_b200.nn.model import DeviceModel
     t0 = time.time()
@@ -84,7 +87,7 @@ def _audit(spec, in_ch, imgs, precision, capfd, monkeypatch, env=(), expect=None
     model = DeviceModel(spec, w, input_channels=in_ch, input_scale=input_scale, precision=precision)
     B, H, W, C = imgs.shape
     capfd.readouterr()
-    model.configure(B, H, W, C)
+    model.configure(max_batch or B, H, W, C)
     err = capfd.readouterr().err
     if expect:
         assert expect in err, f"{expect!r} never ran"
@@ -95,6 +98,12 @@ def _audit(spec, in_ch, imgs, precision, capfd, monkeypatch, env=(), expect=None
     aud = la.Audit(model.cm, model.cm.pack_weights(w), precision, imgs, kinds, conv01="-> fused" in err)
     forms = _forms(err)
     label = f"{spec['backbone']} p{precision} {dict(env)}"
+    if max_batch:
+        assert max_batch > B
+        label += f" {imgs.dtype} B {max_batch} -> {B}"
+        poison = (np.full((max_batch, H, W, C), 255, np.uint8) if imgs.dtype == np.uint8 else
+                  np.random.default_rng(seed).uniform(45, 55, (max_batch, H, W, C)).astype(np.float32))
+        _fetch(model, aud, poison, list(aud.bufs))
 
     # (a) production run: the benchmark's kernels
     internal = aud.internal_buffers(True)

@@ -139,6 +139,10 @@ def emulate(fault=None, fault_op=-1):
             Hin, Win = x.shape[1:3]
             pt = int(op[16]) if op[11] & ol.F_EXPLICIT_PAD else max((ob[1] - 1) * st + k - Hin, 0) // 2
             pl = int(op[17]) if op[11] & ol.F_EXPLICIT_PAD else max((ob[2] - 1) * st + k - Win, 0) // 2
+            if i == fault_op and fault == "cross_frame":      # frame 0's bottom SAME-pad row read from frame 1's first row
+                x = np.concatenate([x, np.concatenate([x[1:2, :1], np.zeros_like(x[1:, :1])])], axis=1)
+            elif i == fault_op and fault == "wrong_frame":    # frame 1's input read from frame 0's slot
+                x = np.concatenate([x[:1], x[:1], x[2:]])
             acc = np.zeros(ob[:3] + (w.shape[3],))
             for ky in range(k):
                 for kx in range(k):
@@ -227,12 +231,15 @@ def test_checker_passes_faithful_emulation():
         assert r["worst"] <= 1 and r.get("missed", 0) == 0, r
 
 
-@pytest.mark.parametrize("fault", ["tap", "bias", "rz", "pool_partner", "slice_off", "double_round"])
+@pytest.mark.parametrize("fault", ["tap", "bias", "rz", "pool_partner", "slice_off", "double_round", "cross_frame",
+                                   "wrong_frame"])
 def test_checker_catches_planted_fault(fault):
+    """cross_frame / wrong_frame: the bugs a run below the configured batch can hide, where the slots past the last frame
+    hold an earlier call's data -- a SAME-pad row read from the next frame, a frame's input read from another slot."""
     cm, blob, frames, kinds = _toy()
     aud = la.Audit(cm, blob, 0, frames, kinds, conv01=True)
     op_c, op_d = 4, 5
-    if fault in ("tap", "bias", "rz"):
+    if fault in ("tap", "bias", "rz", "cross_frame", "wrong_frame"):
         dev = _dev(aud, fault, op_c)
     elif fault == "double_round":
         dev = _dev(aud, fault, op_d)
@@ -246,6 +253,21 @@ def test_checker_catches_planted_fault(fault):
             dev[3][..., 8:24] = buf[3][..., 16:32]
     assert _passes(aud, _dev(aud)), "the faithful emulation must pass"
     assert not _passes(aud, dev), f"planted fault {fault!r} not caught"
+
+
+def test_bias_ignores_relu_zero_crossings():
+    """A ReLU output whose pre-activation lies within the bound of 0 is 0 on one side and small on the other: that is not
+    a rounding bias, and one such element must not swamp the mean signed error; round toward zero still shows in it."""
+    ref = np.maximum(np.random.default_rng(0).normal(0, 1, 8192), 0)
+    e_pre = np.full_like(ref, 1e-3)
+    dev = la.f16(ref)
+    z = np.flatnonzero(ref == 0)
+    dev[z[0]] = la.f16(5e-4)                              # reference 0, device just above
+    r = la.check(dev, ref, e_pre, "f16")
+    assert r["worst"] <= 1 and abs(r["bias"]) < 0.01, r
+    h = la.f16(ref)
+    rz = np.where(np.abs(h) > np.abs(ref), np.nextafter(h.astype(np.float16), np.float16(0)).astype(np.float64), h)
+    assert la.check(rz, ref, e_pre, "f16")["bias"] < -0.2
 
 
 def test_checker_catches_dropped_lo_plane():
