@@ -350,8 +350,7 @@ int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op) {
 
 // Persistent launch: as many CTAs as are co-resident (capped at the item count), with programmatic stream serialization
 // so that the weight loads overlap the predecessor's tail; each CTA triggers its dependents when it starts its last item.
-int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
-  SbConv01Plan* pl = m->entry.conv01;
+int sb_conv01_launch(sb_handle_s* h, const SbConv01Plan* pl, const void* frames_dev, int frames_are_u8, int B) {
   C01Params P = pl->P;
   P.frames = frames_dev; P.frames_u8 = frames_are_u8; P.batch = B;
   void* args[] = {&P};

@@ -1378,12 +1378,12 @@ struct SbConvTcPlan {
   const void* head = nullptr;       // the k_head_1x1 instantiation that runs this 1x1 fp32 head instead of the launches
   __half* w16 = nullptr;            // [taps][Cout_pad][Cin]
   int Cout_pad = 0;
+  bool pool_fused = false;          // the launches write the 2x2 max-pool of the POOL op after this conv
   bool out_dead = false;            // nobody reads the full-resolution output (only the fused pool): stores are skipped
   // the residual ADD after this conv runs in its epilogue (launches); plain_launches store the conv's own output
   // instead, for a forward pass that asks for that tensor (the ADD op then runs)
   bool res_fused = false;
   std::vector<TcLaunch> plain_launches;
-  bool head_logged = false;         // SB_DEBUG: the k_head_1x1 launch shape of this op was printed
 };
 
 static CUtensorMapSwizzle swz_for(int KC) {
@@ -1424,15 +1424,6 @@ void sb_conv_tc_release(SbModel* m) {
   for (size_t oi = 0; oi < m->tc_plans.size(); ++oi)
     if (m->tc_plans[oi]) sb_conv_tc_drop(m, (int)oi);
   m->tc_plans.clear();
-}
-
-bool sb_conv_tc_out_dead(const SbModel* m, int op_index) {
-  const SbConvTcPlan* p = op_index < (int)m->tc_plans.size() ? m->tc_plans[op_index] : nullptr;
-  return p && (p->out_dead || p->res_fused);
-}
-
-bool sb_conv_tc_can(const SbModel* m, int op_index) {
-  return op_index < (int)m->tc_plans.size() && m->tc_plans[op_index] != nullptr;
 }
 
 // the wgmma tile widths N that have instantiations
@@ -1820,7 +1811,6 @@ static const void* head_kernel(int nt, int kch) {
 
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
   m->tc_plans.assign(m->ops.size(), nullptr);
-  m->skip_op.assign(m->ops.size(), 0);
   if (m->precision == 1) return 0;
   const bool split = m->precision == 2;          // physical extent of a conv's output slice: 3 x C_out fp16 planes
   static bool attr_set = false;
@@ -1920,11 +1910,10 @@ int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m) {
       plan->head = head_kernel(hs.nt, hs.kch);
       SB_CUDA(h, cudaFuncSetAttribute(plan->head, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kHeadSmem));
     }
-    if (plan->res_fused) m->skip_op[oi + 1] = 2;
     if (op.kind() == SB_OPK_CONV && op.pool_buf() >= 0 && oi + 1 < m->ops.size() &&
         m->ops[oi + 1].kind() == SB_OPK_POOL && (m->ops[oi + 1].flags() & SB_OPF_FUSED_POOL))
       if (plan->launches[0].forms[0].P.pool_out != nullptr) {
-        m->skip_op[oi + 1] = 1;
+        plan->pool_fused = true;
         // dead-store elimination: with the pool fused, the conv's own output is written only for other readers
         // (skip connections into the decoder, heads).  The two finest encoder blocks of a UNet with output_stride 4
         // have none: 268 + 134 MB of stores per 8-frame C4 step.
@@ -1973,6 +1962,18 @@ static void launch_form(const TcLaunch& L, int B, cudaStream_t stream, int skip_
   }
   void* args[4] = {const_cast<CUtensorMap*>(&F.mapA), const_cast<CUtensorMap*>(&F.mapB), &P, const_cast<TcPhases*>(&F.Q)};
   sb_launch_pdl(form_kernel(L.form, P.KC, P.N), grid, dim3(F.threads), smem, stream, args);
+}
+
+// The launches of one op: the sub-pixel phases of a transposed conv run back to back on the launching stream, and under
+// programmatic dependent launch each phase's CTAs start as the previous phase's SMs drain.  Form 4 runs all four phases
+// in the first launch.
+static int tc_launch(sb_handle_s* h, const std::vector<TcLaunch>& launches, int B, int skip_out) {
+  for (const TcLaunch& L : launches) {
+    launch_form(L, B, h->stream, skip_out);
+    SB_CHECK_LAUNCH(h);
+    if (L.form == kTconvForm) break;
+  }
+  return 0;
 }
 
 int sb_time_min(sb_handle_s* h, const char* what, float& best, const std::function<int()>& run) {
@@ -2044,7 +2045,7 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
     for (int f = 0; f < 2; ++f) {
       L0.form = f ? kTconvForm : phase_form;
       snprintf(what, sizeof what, "op %zu, %s", oi, f ? "fused tconv" : "tconv phases");
-      if (const int rc = sb_time_min(h, what, best[f], [&] { return sb_conv_tc_launch(h, m, (int)oi, m->B); })) return rc;
+      if (const int rc = sb_time_min(h, what, best[f], [&] { return tc_launch(h, plan->launches, m->B, 0); })) return rc;
     }
     L0.form = (force >= 0 ? force == kTconvForm : best[1] < best[0]) ? kTconvForm : phase_form;
     if (dbg)
@@ -2054,40 +2055,47 @@ int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
-static int head_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int B) {
+// k_head_1x1 over the op's pixels.  `log`: SB_DEBUG prints the launch shape (the production program's slot).
+static SbLaunchFn head_entry(const SbModel* m, const SbOp& op, const SbConvTcPlan* plan, bool log) {
   const SbBuffer& ib = m->buffers[op.in_buf()];
   const SbBuffer& ob = m->buffers[op.out_buf()];
   const HeadShape hs = head_shape(op);
-  int n_ring = hs.n_ring;
-  size_t npix = (size_t)B * ob.H * ob.W;
-  if (!plan->head_logged && getenv("SB_DEBUG")) {
+  if (log && getenv("SB_DEBUG"))
     fprintf(stderr, "[sb_conv_tc] head k_head_1x1: Cin %d Cout %d NT %d KCH %d n_ring %d smem %zu\n", op.in_C(), op.out_C(), hs.nt,
-            hs.kch, n_ring, hs.smem);
-    plan->head_logged = true;
-  }
+            hs.kch, hs.n_ring, hs.smem);
+  const void* kern = plan->head;
   const __half* in = (const __half*)ib.dev;
   const __half* w = plan->w16;
   const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
   float* out = (float*)ob.dev;
   int in_Ctot = ib.C, in_coff = op.in_coff(), Cin = op.in_C(), out_Ctot = ob.C, out_coff = op.out_coff(), Cout = op.out_C();
-  int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-  void* args[] = {&in, &in_Ctot, &in_coff, &Cin, &w, &bias, &out, &out_Ctot, &out_coff, &Cout, &relu, &npix, &n_ring};
-  const int grid = (int)std::min<size_t>((npix + 127) / 128, (size_t)h->sm_count * 2);
-  sb_launch_pdl(plan->head, dim3(grid), dim3(256), hs.smem, h->stream, args);
-  SB_CHECK_LAUNCH(h);
-  return 0;
+  int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0, n_ring = hs.n_ring;
+  const size_t frame_pix = (size_t)ob.H * ob.W;
+  return [=](sb_handle_s* h, const void*, int, int B) mutable {
+    size_t npix = (size_t)B * frame_pix;
+    void* args[] = {&in, &in_Ctot, &in_coff, &Cin, &w, &bias, &out, &out_Ctot, &out_coff, &Cout, &relu, &npix, &n_ring};
+    const int grid = (int)std::min<size_t>((npix + 127) / 128, (size_t)h->sm_count * 2);
+    sb_launch_pdl(kern, dim3(grid), dim3(256), hs.smem, h->stream, args);
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  };
 }
 
-int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B) {
-  SbConvTcPlan* plan = m->tc_plans[op_index];
-  if (plan->head) return head_launch(h, m, m->ops[op_index], plan, B);
-  const int skip = plan->out_dead && !m->keep_dead_stores;
-  // the sub-pixel phases of a transposed conv run back to back on the launching stream: under programmatic dependent
-  // launch each phase's CTAs start as the previous phase's SMs drain.  Form 4 runs all four phases in the first launch.
-  for (TcLaunch& L : (plan->res_fused && m->keep_dead_stores) ? plan->plain_launches : plan->launches) {
-    launch_form(L, B, h->stream, skip);
-    SB_CHECK_LAUNCH(h);
-    if (L.form == kTconvForm) break;
+// Production: a dead output is not stored, and a fused residual ADD runs in the epilogue.  All stores: the output is
+// stored, by the plain launches where the ADD was fused (the ADD op then runs in its own slot).  A fused pool is written
+// by both.  The slot refers to the plan's launches: the programs go before the plans.
+SbTcEntry sb_conv_tc_entry(const SbModel* m, int op_index, bool all_stores) {
+  const SbConvTcPlan* plan = m->tc_plans[op_index];
+  SbTcEntry e;
+  if (plan->head) {
+    e.run = head_entry(m, m->ops[op_index], plan, !all_stores);
+    return e;
   }
-  return 0;
+  const bool res = plan->res_fused && !all_stores;
+  const int skip = plan->out_dead && !all_stores;
+  const std::vector<TcLaunch>* launches = plan->res_fused && all_stores ? &plan->plain_launches : &plan->launches;
+  e.run = [launches, skip](sb_handle_s* h, const void*, int, int B) { return tc_launch(h, *launches, B, skip); };
+  if (plan->pool_fused || res) e.absorbs = op_index + 1;
+  e.elides_out = skip || res;
+  return e;
 }

@@ -1,7 +1,7 @@
 // The input stage: everything from the raw frame to the first activation the generic op loop reads.  One of five routes
 // (SbEntryPlan) takes the PREPROCESS op and the first conv, and the fused first encoder block k_conv01 may take conv1
 // too.  sb_entry_prepare resolves the route from the op list and builds its views, sb_entry_autotune times the
-// candidates once at configure time, and run_ops_t hands every op the plan covers to sb_entry_run.
+// candidates once at configure time, and sb_entry_build fills the slots the plan covers in both programs.
 //
 // Replaces InferenceLayer.preprocess (sleap/nn/inference.py:940-967, uint8 -> float * 1/255, zero pad to the stride)
 // fused with the first conv of the backbone (encoder_decoder.py:117-131; hourglass.py:49-100; resnet.py's stem).
@@ -251,7 +251,7 @@ bool stem_fusable(const SbModel* m, int p) {
 // 3x3 s1 16 -> 16 reading all of conv0's output, no BN, conv1's 2x2 max-pool fused on the tensor-core path with its own
 // output dead (so no residual either), even extents, fp16 tensors, and conv1 the only reader of conv0's output.
 bool conv01_fusable(const SbModel* m, int c0i) {
-  if (m->precision != 0 || c0i + 1 >= (int)m->ops.size() || !sb_conv_tc_out_dead(m, c0i + 1)) return false;
+  if (m->precision != 0 || c0i + 1 >= (int)m->ops.size()) return false;
   const SbOp& c0 = m->ops[c0i];
   const SbOp& c1 = m->ops[c0i + 1];
   if (m->Cin != 1 || c0.in_C() != 1 || c0.out_C() != 16 || c0.k() != 3 || c0.stride() != 1 || (c0.flags() & SB_OPF_BN)) return false;
@@ -260,7 +260,7 @@ bool conv01_fusable(const SbModel* m, int c0i) {
   const SbBuffer& ob0 = m->buffers[c0.out_buf()];
   const SbBuffer& pb = m->buffers[c1.pool_buf()];
   if (ob0.f32 || pb.f32 || pb.C % 2 || c1.pool_coff() % 2 || ob0.H % 2 || ob0.W % 2) return false;
-  return only_reader(m, c0.out_buf(), c0i + 1);
+  return m->tc_plans[c0i + 1] && sb_conv_tc_entry(m, c0i + 1, false).elides_out && only_reader(m, c0.out_buf(), c0i + 1);
 }
 
 // ---- views -----------------------------------------------------------------------------------------------------------
@@ -362,55 +362,69 @@ void launch_first(int co, int B, cudaStream_t s, const TI* img, int Hin, int Win
 }
 
 // The direct route: k_conv_first (precision 2: its split store).
-int launch_direct(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
+SbLaunchFn direct_entry(const SbModel* m) {
   const SbOp& op = m->ops[m->entry.conv_op];
-  SbBuffer& ob = m->buffers[op.out_buf()];
-  cudaStream_t s = h->stream;
+  const SbBuffer ob = m->buffers[op.out_buf()];
   const float* Wt = m->weights_dev + op.w_off();
   const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
   const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
   const int split = m->precision == 2 ? op.out_C() : 0;
+  const int Cin = m->Cin, Hin = m->Hin, Win = m->Win, co = op.out_C(), coff = op.out_coff();
   // rows/cols beyond the resized frame (Hres, Wres) are the bottom/right zero padding
-  if (frames_are_u8) {
-    if (m->Cin == 1) launch_first<unsigned char, 1>(op.out_C(), B, s, (const unsigned char*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 1, split);
-    else launch_first<unsigned char, 3>(op.out_C(), B, s, (const unsigned char*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 1, split);
-  } else {
-    if (m->Cin == 1) launch_first<float, 1>(op.out_C(), B, s, (const float*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 0, split);
-    else launch_first<float, 3>(op.out_C(), B, s, (const float*)frames_dev, m->Hin, m->Win, ob.H, ob.W, (__half*)ob.dev, ob.C, op.out_coff(), Wt, bias, relu, 0, split);
-  }
-  SB_CHECK_LAUNCH(h);
-  return 0;
+  return [=](sb_handle_s* h, const void* frames_dev, int frames_are_u8, int B) {
+    cudaStream_t s = h->stream;
+    if (frames_are_u8) {
+      if (Cin == 1) launch_first<unsigned char, 1>(co, B, s, (const unsigned char*)frames_dev, Hin, Win, ob.H, ob.W, (__half*)ob.dev, ob.C, coff, Wt, bias, relu, 1, split);
+      else launch_first<unsigned char, 3>(co, B, s, (const unsigned char*)frames_dev, Hin, Win, ob.H, ob.W, (__half*)ob.dev, ob.C, coff, Wt, bias, relu, 1, split);
+    } else {
+      if (Cin == 1) launch_first<float, 1>(co, B, s, (const float*)frames_dev, Hin, Win, ob.H, ob.W, (__half*)ob.dev, ob.C, coff, Wt, bias, relu, 0, split);
+      else launch_first<float, 3>(co, B, s, (const float*)frames_dev, Hin, Win, ob.H, ob.W, (__half*)ob.dev, ob.C, coff, Wt, bias, relu, 0, split);
+    }
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  };
 }
 
-// The view routes: the route's view kernel, then the GEMM over the view.
-int launch_view(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
+// The view routes: the route's view kernel, then the GEMM over the view (its plan stores its whole output in both programs).
+SbLaunchFn view_entry(SbModel* m) {
   const SbEntryPlan& e = m->entry;
-  const size_t total = (size_t)B * e.view_H * e.view_W;
-  const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
-  cudaStream_t s = h->stream;
-  if (e.route == SB_ENTRY_BUFFER_VIEW) {
-    const SbBuffer& ib = m->buffers[m->ops[e.conv_op].in_buf()];
-    k_first_view<__half><<<grid, 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, e.view_H, e.view_W, e.view, 0, total);
-  } else if (e.route == SB_ENTRY_STEM_VIEW) {
-    if (frames_are_u8)
-      k_s2d_view<unsigned char><<<grid, 256, 0, s>>>((const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, e.view_H, e.view_W,
-                                                     e.view, 1, total, e.pre_mode);
-    else
-      k_s2d_view<float><<<grid, 256, 0, s>>>((const float*)frames_dev, m->Hin, m->Win, m->Cin, e.view_H, e.view_W, e.view, 0,
-                                             total, e.pre_mode);
-  } else if (frames_are_u8) {
-    k_first_view<unsigned char><<<grid, 256, 0, s>>>((const unsigned char*)frames_dev, m->Hin, m->Win, e.view_H, e.view_W, e.view, 1, total);
-  } else {
-    k_first_view<float><<<grid, 256, 0, s>>>((const float*)frames_dev, m->Hin, m->Win, e.view_H, e.view_W, e.view, 0, total);
-  }
-  SB_CHECK_LAUNCH(h);
-  return sb_conv_tc_launch(h, m, e.conv_op, B);
+  const int route = e.route, view_H = e.view_H, view_W = e.view_W, pre_mode = e.pre_mode;
+  const int Cin = m->Cin, Hin = m->Hin, Win = m->Win;
+  __half* view = e.view;
+  const SbBuffer ib = m->buffers[m->ops[e.conv_op].in_buf()];
+  const SbLaunchFn gemm = sb_conv_tc_entry(m, e.conv_op, false).run;
+  return [=](sb_handle_s* h, const void* frames_dev, int frames_are_u8, int B) {
+    const size_t total = (size_t)B * view_H * view_W;
+    const int grid = (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16);
+    cudaStream_t s = h->stream;
+    if (route == SB_ENTRY_BUFFER_VIEW) {
+      k_first_view<__half><<<grid, 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, view_H, view_W, view, 0, total);
+    } else if (route == SB_ENTRY_STEM_VIEW) {
+      if (frames_are_u8)
+        k_s2d_view<unsigned char><<<grid, 256, 0, s>>>((const unsigned char*)frames_dev, Hin, Win, Cin, view_H, view_W, view, 1,
+                                                       total, pre_mode);
+      else
+        k_s2d_view<float><<<grid, 256, 0, s>>>((const float*)frames_dev, Hin, Win, Cin, view_H, view_W, view, 0, total, pre_mode);
+    } else if (frames_are_u8) {
+      k_first_view<unsigned char><<<grid, 256, 0, s>>>((const unsigned char*)frames_dev, Hin, Win, view_H, view_W, view, 1, total);
+    } else {
+      k_first_view<float><<<grid, 256, 0, s>>>((const float*)frames_dev, Hin, Win, view_H, view_W, view, 0, total);
+    }
+    SB_CHECK_LAUNCH(h);
+    return gemm(h, frames_dev, frames_are_u8, B);
+  };
 }
 
 // The first conv as picked, without the fused block.
-int launch_first_conv(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
-  return m->entry.route == SB_ENTRY_DIRECT ? launch_direct(h, m, frames_dev, frames_are_u8, B)
-                                           : launch_view(h, m, frames_dev, frames_are_u8, B);
+SbLaunchFn first_conv_entry(SbModel* m) {
+  return m->entry.route == SB_ENTRY_DIRECT ? direct_entry(m) : view_entry(m);
+}
+
+// The fused first block.
+SbLaunchFn conv01_entry(const SbConv01Plan* pl) {
+  return [pl](sb_handle_s* h, const void* frames_dev, int frames_are_u8, int B) {
+    return sb_conv01_launch(h, pl, frames_dev, frames_are_u8, B);
+  };
 }
 
 }  // namespace
@@ -447,12 +461,11 @@ int sb_entry_autotune(sb_handle_s* h, SbModel* m) {
   const bool dbg = getenv("SB_DEBUG") != nullptr;
   char what[64];
   if (e.route == SB_ENTRY_FRAME_VIEW) {
+    const SbLaunchFn cand[2] = {direct_entry(m), view_entry(m)};
     float best[2];
     for (int f = 0; f < 2; ++f) {
       snprintf(what, sizeof what, "first layer, form %d", f);
-      const int rc = sb_time_min(h, what, best[f], [&] {
-        return f == 0 ? launch_direct(h, m, m->frames_dev, 1, m->B) : launch_view(h, m, m->frames_dev, 1, m->B);
-      });
+      const int rc = sb_time_min(h, what, best[f], [&] { return cand[f](h, m->frames_dev, 1, m->B); });
       if (rc) return rc;
     }
     bool view = best[1] < best[0];
@@ -466,13 +479,14 @@ int sb_entry_autotune(sb_handle_s* h, SbModel* m) {
     }
   }
   if (e.conv01) {
+    const SbLaunchFn conv0 = first_conv_entry(m), conv1 = sb_conv_tc_entry(m, e.conv_op + 1, false).run, fused_block = conv01_entry(e.conv01);
     float best[2];
     for (int f = 0; f < 2; ++f) {
       snprintf(what, sizeof what, "first block, fused %d", f);
       const int rc = sb_time_min(h, what, best[f], [&] {
-        if (f == 1) return sb_conv01_launch(h, m, m->frames_dev, 1, m->B);
-        const int rc0 = launch_first_conv(h, m, m->frames_dev, 1, m->B);
-        return rc0 ? rc0 : sb_conv_tc_launch(h, m, e.conv_op + 1, m->B);
+        if (f == 1) return fused_block(h, m->frames_dev, 1, m->B);
+        const int rc0 = conv0(h, m->frames_dev, 1, m->B);
+        return rc0 ? rc0 : conv1(h, m->frames_dev, 1, m->B);
       });
       if (rc) return rc;
     }
@@ -485,16 +499,18 @@ int sb_entry_autotune(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
-// An op the plan covers: the PREPROCESS op is an empty slot (the first conv's launch preprocesses), the first conv runs
-// its route or the fused block, conv1 is an empty slot when the fused block ran.  A forward that asks for a tensor
-// internal to the fused block (keep_dead_stores) runs the separate launches.
-int sb_entry_run(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B) {
+// The PREPROCESS op's slot is empty where the first conv's launch preprocesses the frame.  The first conv runs its route,
+// or in the production program the fused block, whose conv1 and pool slots are then empty.  The all-stores program runs
+// the separate launches instead (conv1 as an ordinary tensor-core conv), which store the block's two tensors.
+void sb_entry_build(SbModel* m, bool all_stores, std::vector<char>& taken) {
   const SbEntryPlan& e = m->entry;
-  const bool fused = e.conv1_op >= 0 && !m->keep_dead_stores;
-  if (op_index == e.pre_op) return 0;
-  if (op_index == e.conv1_op) return fused ? 0 : sb_conv_tc_launch(h, m, op_index, B);
-  if (fused) return sb_conv01_launch(h, m, frames_dev, frames_are_u8, B);
-  return launch_first_conv(h, m, frames_dev, frames_are_u8, B);
+  if (e.pre_op >= 0) taken[e.pre_op] = 1;
+  if (e.conv_op < 0) return;
+  const bool fused = e.conv1_op >= 0 && !all_stores;
+  m->prog[all_stores][e.conv_op] = fused ? conv01_entry(e.conv01) : first_conv_entry(m);
+  taken[e.conv_op] = 1;
+  if (fused) taken[e.conv1_op] = taken[e.conv1_op + 1] = 1;
+  if (e.conv01) m->buf_elided[m->ops[e.conv_op].out_buf()] = m->buf_elided[m->ops[e.conv_op + 1].out_buf()] = 1;
 }
 
 // The views and the fused block's plan; the view's GEMM plan goes with the tensor-core plans (sb_conv_tc_release).

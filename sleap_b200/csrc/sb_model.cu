@@ -24,6 +24,8 @@ int grid_for(size_t total, int sm) {
   return (int)std::max<size_t>(1, std::min(g, cap));
 }
 
+int build_programs(sb_handle_s* h, SbModel* m);   // the last step of sb_model_configure (below, with the op slots)
+
 }  // namespace
 
 void sb_models_free(sb_handle_s* h) {
@@ -52,6 +54,7 @@ void sb_models_free(sb_handle_s* h) {
     sb_post_ws_free(m->ws);
     sb_gather_free(m);
     sb_topdown_free(m);
+    for (auto& p : m->prog) p.clear();
     sb_entry_release(m);
     sb_conv_tc_release(m);
     delete m;
@@ -169,6 +172,7 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes): re-init after a reconfigure
   m->configured = false;
   m->bu_configured = false; m->gl_configured = false; m->ce_configured = false; m->td_configured = false;
+  for (auto& p : m->prog) p.clear();             // the programs refer to the plans
   sb_entry_release(m);
   sb_conv_tc_release(m);
   m->B = max_batch; m->Hin = H; m->Win = W; m->Cin = C_in; m->Hres = Hres; m->Wres = Wres; m->Hnet = Hnet; m->Wnet = Wnet;
@@ -186,6 +190,7 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   if (!rc) rc = sb_entry_prepare(h, m);
   if (!rc) rc = sb_conv_tc_autotune(h, m);
   if (!rc) rc = sb_entry_autotune(h, m);
+  if (!rc) rc = build_programs(h, m);
   if (rc) return rc;
   m->configured = true;
   return SB_OK;
@@ -194,176 +199,210 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------
-template <typename T>
-static int run_ops_t(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
-  cudaStream_t s = h->stream;
-  const bool split = m->precision == 2;         // split-fp16 activations: [lo | hi | hi] channel planes (sb_kernels_direct.cuh)
-  for (size_t oi = 0; oi < m->ops.size(); ++oi) {
-    const SbOp& op = m->ops[oi];
-    if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[oi], s);
-    SbBuffer& ob = m->buffers[op.out_buf()];
-    if ((int)oi == m->guard_op && h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(s, h->post_done_ev, 0));
-    // 2x2 max-pool fused into the producing conv; residual ADD fused into the conv before it (unless that conv's own output
-    // was asked for: it then stores its output and the ADD runs)
-    if (oi < m->skip_op.size() && (m->skip_op[oi] == 1 || (m->skip_op[oi] == 2 && !m->keep_dead_stores))) continue;
-    if (m->entry.covers((int)oi)) {                             // the input stage (sb_entry.cu)
-      int rc = sb_entry_run(h, m, (int)oi, frames_dev, frames_are_u8, B);
-      if (rc) return rc;
-      continue;
-    }
-    switch (op.kind()) {
-      case SB_OPK_PREPROCESS: {
-        const size_t total = (size_t)B * ob.H * ob.W * ob.C;
-        const int resize = op.input_scale() != 1.0f;
-        int mode_ch = 0;
-        if (m->Cin == 3 && (ob.C == 1 || op.pre_mode() == SB_PRE_IMAGENET_CAFFE_GRAY)) mode_ch = 1;
-        if (m->Cin == 1 && ob.C == 3) mode_ch = 2;
-        const int imagenet = op.pre_mode() != SB_PRE_PLAIN;
-        if (imagenet && ob.C != 3) return sb_fail(h, SB_ERR_INVALID, "ImageNet preprocessing needs a 3-channel network input");
-        if (ob.f32 && sizeof(T) == 2) {          // precision 2 keeps the preprocessed frame in fp32
-          if (frames_are_u8)
-            k_preprocess<unsigned char, float><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-                (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total, imagenet);
-          else
-            k_preprocess<float, float><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-                (const float*)frames_dev, m->Hin, m->Win, m->Cin, (float*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total, imagenet);
-        } else if (frames_are_u8)
-          k_preprocess<unsigned char, T><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-              (const unsigned char*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 1, total, imagenet);
-        else
-          k_preprocess<float, T><<<grid_for(total, h->sm_count), 256, 0, s>>>(
-              (const float*)frames_dev, m->Hin, m->Win, m->Cin, (T*)ob.dev, ob.H, ob.W, ob.C, m->Hres, m->Wres, resize, mode_ch, 0, total, imagenet);
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_CONV: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        if (m->precision != 1 && sb_conv_tc_can(m, (int)oi)) {
-          int rc = sb_conv_tc_launch(h, m, (int)oi, B);
-          if (rc) return rc;
-          break;
-        }
-        const int k = op.k(), st = op.stride();
-        const int osplit = (split && !ob.f32) ? op.out_C() : 0;
-        const int Hout = ob.H, Wout = ob.W;
-        const int tot_h = std::max((Hout - 1) * st + k - ib.H, 0), tot_w = std::max((Wout - 1) * st + k - ib.W, 0);
-        const int pad_top = op.explicit_pad() ? op.pad_top() : tot_h / 2, pad_left = op.explicit_pad() ? op.pad_left() : tot_w / 2;
-        const float* W = m->weights_dev + op.w_off();
-        const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-        const float* bs = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_scale_off() : nullptr;
-        const float* bh = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_shift_off() : nullptr;
-        const int in_tile = (DC_TILE - 1) * st + k;
-        const size_t sm = ((size_t)in_tile * in_tile * DC_CK + (size_t)k * k * DC_CK * DC_CO) * sizeof(float);
-        dim3 g(((Wout + DC_TILE - 1) / DC_TILE) * ((Hout + DC_TILE - 1) / DC_TILE), (op.out_C() + DC_CO - 1) / DC_CO, B);
-        const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-        if (ib.f32 && sizeof(T) == 2) {              // precision 2: first conv straight from the fp32 preprocessed frame
-          if (ob.f32) return sb_fail(h, SB_ERR_INVALID, "conv from the fp32 input buffer to an fp32 head is not supported in precision 2");
-          auto kern = k_conv_direct<float, __half>;
-          if (sm > 48 * 1024) SB_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-          kern<<<g, 256, sm, s>>>((const float*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (__half*)ob.dev, Hout, Wout,
-                                  ob.C, op.out_coff(), op.out_C(), W, bias, bs, bh, k, st, pad_top, pad_left, relu, osplit);
-        } else if (ob.f32 && sizeof(T) == 2) {
-          auto kern = k_conv_direct<T, float>;
-          if (sm > 48 * 1024) SB_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-          kern<<<g, 256, sm, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (float*)ob.dev, Hout, Wout,
-                                  ob.C, op.out_coff(), op.out_C(), W, bias, bs, bh, k, st, pad_top, pad_left, relu, 0);
-        } else {
-          auto kern = k_conv_direct<T, T>;
-          if (sm > 48 * 1024) SB_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-          kern<<<g, 256, sm, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (T*)ob.dev, Hout, Wout,
-                                  ob.C, op.out_coff(), op.out_C(), W, bias, bs, bh, k, st, pad_top, pad_left, relu, osplit);
-        }
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_TCONV: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        if (m->precision != 1 && sb_conv_tc_can(m, (int)oi)) {
-          int rc = sb_conv_tc_launch(h, m, (int)oi, B);
-          if (rc) return rc;
-          break;
-        }
-        const float* W = m->weights_dev + op.w_off();
-        const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
-        dim3 g((ob.H * ob.W + 255) / 256, (op.out_C() + DC_CO - 1) / DC_CO, B);
-        k_tconv_direct<T, T><<<g, 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (T*)ob.dev, ob.C,
-                                               op.out_coff(), op.out_C(), W, bias, (op.flags() & SB_OPF_RELU) ? 1 : 0, split ? op.out_C() : 0,
-                                               op.k());
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_POOL: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        // precision 2: the record carries the physical channel count (3C); the split kernels work on logical channels
-        const size_t total = (size_t)B * ob.H * ob.W * (split ? op.in_C() / 3 : op.in_C());
-        if (op.k() == 3) {                      // ResNet stem: zero padding 1, 3x3 window, stride 2
-          if (split)
-            k_maxpool3s2_split<<<grid_for(total, h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C() / 3,
-                                                                            (__half*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
-          else
-            k_maxpool3s2<T><<<grid_for(total, h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(),
-                                                                         (T*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
-        } else if (split)
-          k_maxpool2_split<<<grid_for(total, h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C() / 3,
-                                                                        (__half*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
-        else
-        k_maxpool2<T><<<grid_for(total, h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(),
-                                                                   (T*)ob.dev, ob.H, ob.W, ob.C, op.out_coff(), total);
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_UPSAMPLE: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        const size_t total = (size_t)B * ob.H * ob.W * (split ? op.in_C() / 3 : op.in_C());
-        if (split)
-          k_upsample2_split<<<grid_for(total, h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C() / 3,
-                                                                         (__half*)ob.dev, ob.C, op.out_coff(),
-                                                                         (op.flags() & SB_OPF_BILINEAR) ? 1 : 0, total);
-        else
-        k_upsample2<T><<<grid_for(total, h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(),
-                                                                    (T*)ob.dev, ob.C, op.out_coff(),
-                                                                    (op.flags() & SB_OPF_BILINEAR) ? 1 : 0, total);
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_ADD: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        SbBuffer& ib2 = m->buffers[op.in2_buf()];
-        const size_t npix = (size_t)B * ob.H * ob.W;
-        const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
-        if (split)
-          k_add_split<<<grid_for(npix * (op.in_C() / 3), h->sm_count), 256, 0, s>>>((const __half*)ib.dev, ib.C, op.in_coff(), (const __half*)ib2.dev,
-                                                                                     ib2.C, op.in2_coff(), (__half*)ob.dev, ob.C, op.out_coff(),
-                                                                                     op.in_C() / 3, npix, relu);
-        else
-        k_add<T><<<grid_for(npix * op.in_C(), h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.C, op.in_coff(), (const T*)ib2.dev, ib2.C,
-                                                                         op.in2_coff(), (T*)ob.dev, ob.C, op.out_coff(), op.in_C(), npix, relu);
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      case SB_OPK_COPY: {
-        SbBuffer& ib = m->buffers[op.in_buf()];
-        const size_t npix = (size_t)B * ob.H * ob.W;
-        k_copy<T><<<grid_for(npix * op.in_C(), h->sm_count), 256, 0, s>>>((const T*)ib.dev, ib.C, op.in_coff(), (T*)ob.dev, ob.C,
-                                                                          op.out_coff(), op.in_C(), npix);
-        SB_CHECK_LAUNCH(h);
-        break;
-      }
-      default:
-        return sb_fail(h, SB_ERR_INVALID, "unknown op kind %d", op.kind());
-    }
+// The slots of the generic ops, in the activation type T of the model's precision.  Precision 2 keeps the preprocessed
+// frame in fp32 and its activations as split-fp16 [lo | hi | hi] channel planes (sb_kernels_direct.cuh).
+namespace {
+
+template <typename TO>
+SbLaunchFn preprocess_entry(const SbModel* m, const SbOp& op, const SbBuffer& ob) {
+  const int Hin = m->Hin, Win = m->Win, Cin = m->Cin, Hres = m->Hres, Wres = m->Wres;
+  const int resize = op.input_scale() != 1.0f;
+  int mode_ch = 0;
+  if (Cin == 3 && (ob.C == 1 || op.pre_mode() == SB_PRE_IMAGENET_CAFFE_GRAY)) mode_ch = 1;
+  if (Cin == 1 && ob.C == 3) mode_ch = 2;
+  const int imagenet = op.pre_mode() != SB_PRE_PLAIN;
+  return [=](sb_handle_s* h, const void* frames_dev, int frames_are_u8, int B) {
+    const size_t total = (size_t)B * ob.H * ob.W * ob.C;
+    if (frames_are_u8)
+      k_preprocess<unsigned char, TO><<<grid_for(total, h->sm_count), 256, 0, h->stream>>>(
+          (const unsigned char*)frames_dev, Hin, Win, Cin, (TO*)ob.dev, ob.H, ob.W, ob.C, Hres, Wres, resize, mode_ch, 1, total, imagenet);
+    else
+      k_preprocess<float, TO><<<grid_for(total, h->sm_count), 256, 0, h->stream>>>(
+          (const float*)frames_dev, Hin, Win, Cin, (TO*)ob.dev, ob.H, ob.W, ob.C, Hres, Wres, resize, mode_ch, 0, total, imagenet);
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  };
+}
+
+template <typename TI, typename TO>
+int conv_entry(sb_handle_s* h, const SbModel* m, const SbOp& op, int osplit, SbLaunchFn& slot) {
+  const SbBuffer& ib = m->buffers[op.in_buf()];
+  const SbBuffer& ob = m->buffers[op.out_buf()];
+  const int k = op.k(), st = op.stride();
+  const int tot_h = std::max((ob.H - 1) * st + k - ib.H, 0), tot_w = std::max((ob.W - 1) * st + k - ib.W, 0);
+  const int pad_top = op.explicit_pad() ? op.pad_top() : tot_h / 2, pad_left = op.explicit_pad() ? op.pad_left() : tot_w / 2;
+  const float* W = m->weights_dev + op.w_off();
+  const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
+  const float* bs = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_scale_off() : nullptr;
+  const float* bh = (op.flags() & SB_OPF_BN) ? m->weights_dev + op.bn_shift_off() : nullptr;
+  const int in_tile = (DC_TILE - 1) * st + k;
+  const size_t sm = ((size_t)in_tile * in_tile * DC_CK + (size_t)k * k * DC_CK * DC_CO) * sizeof(float);
+  const dim3 g(((ob.W + DC_TILE - 1) / DC_TILE) * ((ob.H + DC_TILE - 1) / DC_TILE), (op.out_C() + DC_CO - 1) / DC_CO);
+  const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
+  auto kern = k_conv_direct<TI, TO>;
+  if (sm > 48 * 1024) {          // raised, never lowered: other ops and models launch this instantiation with their own sizes
+    cudaFuncAttributes fa;
+    SB_CUDA(h, cudaFuncGetAttributes(&fa, kern));
+    if ((int)sm > fa.maxDynamicSharedSizeBytes) SB_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
   }
-  if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[m->ops.size()], s);
+  slot = [=](sb_handle_s* h, const void*, int, int B) {
+    kern<<<dim3(g.x, g.y, B), 256, sm, h->stream>>>((const TI*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (TO*)ob.dev, ob.H, ob.W,
+                                                    ob.C, op.out_coff(), op.out_C(), W, bias, bs, bh, k, st, pad_top, pad_left, relu, osplit);
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  };
   return 0;
 }
 
-int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B) {
+// The slot of a generic op: one that has no tensor-core plan and that the input stage does not cover.
+template <typename T>
+int op_entry_t(sb_handle_s* h, const SbModel* m, const SbOp& op, SbLaunchFn& slot) {
+  const bool split = m->precision == 2;
+  const SbBuffer& ob = m->buffers[op.out_buf()];
+  const SbBuffer ib = op.kind() == SB_OPK_PREPROCESS ? SbBuffer() : m->buffers[op.in_buf()];
+  const SbBuffer ib2 = op.kind() == SB_OPK_ADD ? m->buffers[op.in2_buf()] : SbBuffer();
+  // POOL, UPSAMPLE, ADD in precision 2: the record carries the physical channel count (3C); the split kernels work on
+  // logical channels
+  const int C = split ? op.in_C() / 3 : op.in_C();
+  const int relu = (op.flags() & SB_OPF_RELU) ? 1 : 0;
+  const float* W = m->weights_dev + op.w_off();
+  const float* bias = op.b_off() >= 0 ? m->weights_dev + op.b_off() : nullptr;
+  switch (op.kind()) {
+    case SB_OPK_PREPROCESS:
+      if (op.pre_mode() != SB_PRE_PLAIN && ob.C != 3) return sb_fail(h, SB_ERR_INVALID, "ImageNet preprocessing needs a 3-channel network input");
+      slot = (ob.f32 && sizeof(T) == 2) ? preprocess_entry<float>(m, op, ob) : preprocess_entry<T>(m, op, ob);
+      return 0;
+    case SB_OPK_CONV: {
+      const int osplit = (split && !ob.f32) ? op.out_C() : 0;
+      if (ib.f32 && sizeof(T) == 2) {              // precision 2: first conv straight from the fp32 preprocessed frame
+        if (ob.f32) return sb_fail(h, SB_ERR_INVALID, "conv from the fp32 input buffer to an fp32 head is not supported in precision 2");
+        return conv_entry<float, __half>(h, m, op, osplit, slot);
+      }
+      if (ob.f32 && sizeof(T) == 2) return conv_entry<T, float>(h, m, op, 0, slot);
+      return conv_entry<T, T>(h, m, op, osplit, slot);
+    }
+    case SB_OPK_TCONV:
+      slot = [=](sb_handle_s* h, const void*, int, int B) {
+        dim3 g((ob.H * ob.W + 255) / 256, (op.out_C() + DC_CO - 1) / DC_CO, B);
+        k_tconv_direct<T, T><<<g, 256, 0, h->stream>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), op.in_C(), (T*)ob.dev, ob.C,
+                                                       op.out_coff(), op.out_C(), W, bias, relu, split ? op.out_C() : 0, op.k());
+        SB_CHECK_LAUNCH(h);
+        return 0;
+      };
+      return 0;
+    case SB_OPK_POOL:
+      slot = [=](sb_handle_s* h, const void*, int, int B) {
+        const size_t total = (size_t)B * ob.H * ob.W * C;
+        const int grid = grid_for(total, h->sm_count);
+        if (op.k() == 3) {                      // ResNet stem: zero padding 1, 3x3 window, stride 2
+          if (split)
+            k_maxpool3s2_split<<<grid, 256, 0, h->stream>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C, (__half*)ob.dev, ob.H,
+                                                            ob.W, ob.C, op.out_coff(), total);
+          else
+            k_maxpool3s2<T><<<grid, 256, 0, h->stream>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C, (T*)ob.dev, ob.H, ob.W, ob.C,
+                                                         op.out_coff(), total);
+        } else if (split)
+          k_maxpool2_split<<<grid, 256, 0, h->stream>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C, (__half*)ob.dev, ob.H, ob.W,
+                                                        ob.C, op.out_coff(), total);
+        else
+          k_maxpool2<T><<<grid, 256, 0, h->stream>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C, (T*)ob.dev, ob.H, ob.W, ob.C,
+                                                     op.out_coff(), total);
+        SB_CHECK_LAUNCH(h);
+        return 0;
+      };
+      return 0;
+    case SB_OPK_UPSAMPLE:
+      slot = [=](sb_handle_s* h, const void*, int, int B) {
+        const size_t total = (size_t)B * ob.H * ob.W * C;
+        const int bilinear = (op.flags() & SB_OPF_BILINEAR) ? 1 : 0;
+        if (split)
+          k_upsample2_split<<<grid_for(total, h->sm_count), 256, 0, h->stream>>>((const __half*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C,
+                                                                                 (__half*)ob.dev, ob.C, op.out_coff(), bilinear, total);
+        else
+          k_upsample2<T><<<grid_for(total, h->sm_count), 256, 0, h->stream>>>((const T*)ib.dev, ib.H, ib.W, ib.C, op.in_coff(), C,
+                                                                              (T*)ob.dev, ob.C, op.out_coff(), bilinear, total);
+        SB_CHECK_LAUNCH(h);
+        return 0;
+      };
+      return 0;
+    case SB_OPK_ADD:
+      slot = [=](sb_handle_s* h, const void*, int, int B) {
+        const size_t npix = (size_t)B * ob.H * ob.W;
+        if (split)
+          k_add_split<<<grid_for(npix * C, h->sm_count), 256, 0, h->stream>>>((const __half*)ib.dev, ib.C, op.in_coff(), (const __half*)ib2.dev,
+                                                                              ib2.C, op.in2_coff(), (__half*)ob.dev, ob.C, op.out_coff(), C, npix, relu);
+        else
+          k_add<T><<<grid_for(npix * C, h->sm_count), 256, 0, h->stream>>>((const T*)ib.dev, ib.C, op.in_coff(), (const T*)ib2.dev, ib2.C,
+                                                                           op.in2_coff(), (T*)ob.dev, ob.C, op.out_coff(), C, npix, relu);
+        SB_CHECK_LAUNCH(h);
+        return 0;
+      };
+      return 0;
+    case SB_OPK_COPY:
+      slot = [=](sb_handle_s* h, const void*, int, int B) {
+        const size_t npix = (size_t)B * ob.H * ob.W;
+        k_copy<T><<<grid_for(npix * op.in_C(), h->sm_count), 256, 0, h->stream>>>((const T*)ib.dev, ib.C, op.in_coff(), (T*)ob.dev, ob.C,
+                                                                                  op.out_coff(), op.in_C(), npix);
+        SB_CHECK_LAUNCH(h);
+        return 0;
+      };
+      return 0;
+    default:
+      return sb_fail(h, SB_ERR_INVALID, "unknown op kind %d", op.kind());
+  }
+}
+
+// Both programs, one slot per op: the input stage's slots first, then each tensor-core conv (and the POOL or ADD slot it
+// absorbs), then the generic ops.  Also the per-op kinds and the buffers the production program may not store.
+int build_programs(sb_handle_s* h, SbModel* m) {
+  const size_t n = m->ops.size();
+  m->op_kind.assign(n, 0);
+  for (size_t oi = 0; oi < n; ++oi)
+    if (m->ops[oi].kind() == SB_OPK_CONV || m->ops[oi].kind() == SB_OPK_TCONV) m->op_kind[oi] = m->tc_plans[oi] ? 1 : 2;
+  m->buf_elided.assign(m->buffers.size(), 0);
+  for (int all_stores = 0; all_stores < 2; ++all_stores) {
+    m->prog[all_stores].assign(n, nullptr);
+    std::vector<char> taken(n, 0);
+    sb_entry_build(m, all_stores, taken);
+    for (size_t oi = 0; oi < n; ++oi) {
+      if (taken[oi]) continue;
+      if (m->tc_plans[oi]) {
+        const SbTcEntry e = sb_conv_tc_entry(m, (int)oi, all_stores);
+        m->prog[all_stores][oi] = e.run;
+        if (e.absorbs >= 0) taken[e.absorbs] = 1;
+        if (e.elides_out) m->buf_elided[m->ops[oi].out_buf()] = 1;
+        continue;
+      }
+      const int rc = m->precision == 1 ? op_entry_t<float>(h, m, m->ops[oi], m->prog[all_stores][oi])
+                                       : op_entry_t<__half>(h, m, m->ops[oi], m->prog[all_stores][oi]);
+      if (rc) return rc;
+    }
+  }
+  return 0;
+}
+
+// One forward pass of `prog`: per op its profiling event, the wait before the first op that overwrites a head buffer the
+// post-processing stream may still read, then its slot.
+int run_program(sb_handle_s* h, SbModel* m, const std::vector<SbLaunchFn>& prog, const void* frames_dev, int frames_are_u8, int B) {
+  cudaStream_t s = h->stream;
+  for (size_t oi = 0; oi < prog.size(); ++oi) {
+    if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[oi], s);
+    if ((int)oi == m->guard_op && h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(s, h->post_done_ev, 0));
+    if (prog[oi])
+      if (const int rc = prog[oi](h, frames_dev, frames_are_u8, B)) return rc;
+  }
+  if (!m->prof_events.empty()) cudaEventRecord(m->prof_events[prog.size()], s);
+  return 0;
+}
+
+}  // namespace
+
+int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B, bool all_stores) {
   if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "model not configured");
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "batch %d exceeds configured max %d", B, m->B);
   const bool timed = m->fwd_timing && 2 * (m->fwd_n + 1) <= (int)m->fwd_events.size();
   if (timed) cudaEventRecord(m->fwd_events[2 * m->fwd_n], h->stream);
-  const int rc = m->precision == 1 ? run_ops_t<float>(h, m, frames_dev, frames_are_u8, B)
-                                   : run_ops_t<__half>(h, m, frames_dev, frames_are_u8, B);
+  const int rc = run_program(h, m, m->prog[all_stores], frames_dev, frames_are_u8, B);
   if (timed) { cudaEventRecord(m->fwd_events[2 * m->fwd_n + 1], h->stream); ++m->fwd_n; }
   return rc;
 }
@@ -371,14 +410,6 @@ int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_ar
 __global__ void k_half_to_float(const __half* __restrict__ in, float* __restrict__ out, size_t n) {
   for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (size_t)gridDim.x * blockDim.x)
     out[t] = __half2float(in[t]);
-}
-
-// Buffer `id` is not always written: a tensor-core conv's dead output, or a tensor inside the fused first block.
-static bool stores_elided(const SbModel* m, int id) {
-  for (size_t oi = 0; oi < m->ops.size(); ++oi)
-    if (sb_conv_tc_out_dead(m, (int)oi) && m->ops[oi].out_buf() == id) return true;
-  const SbEntryPlan& e = m->entry;
-  return e.conv01 && (id == m->ops[e.conv_op].out_buf() || id == m->ops[e.conv_op + 1].out_buf());
 }
 
 static int upload_frames(sb_handle_s* h, SbModel* m, const void* images_host, int is_u8, int B) {
@@ -398,11 +429,12 @@ int sb_model_forward(sb_handle_t h, int model_id, const void* images_host, int i
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
   if (rc) return rc;
-  for (int i = 0; i < n_outputs; ++i)                    // a tensor nobody reads inside the graph is only written on request
-    if (stores_elided(m, output_buffer_ids[i])) m->keep_dead_stores = true;
-  rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B);
-  m->keep_dead_stores = false;
-  if (rc) return rc;
+  bool all_stores = false;                               // a tensor nobody reads inside the graph is only written on request
+  for (int i = 0; i < n_outputs; ++i) {
+    const int id = output_buffer_ids[i];
+    if (id >= 0 && id < (int)m->buffers.size() && m->buf_elided[id]) all_stores = true;
+  }
+  if ((rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B, all_stores))) return rc;
   for (int i = 0; i < n_outputs; ++i) {
     const int id = output_buffer_ids[i];
     if (id < 0 || id >= (int)m->buffers.size()) return sb_fail(h, SB_ERR_INVALID, "bad output buffer id %d", id);
@@ -442,9 +474,8 @@ int sb_model_profile_ops(sb_handle_t h, int model_id, const uint8_t* frames_dev,
   for (int i = 0; i < n && !rc; ++i) {
     cudaEventElapsedTime(&out_ms[i], m->prof_events[i], m->prof_events[i + 1]);
     const SbOp& op = m->ops[i];
-    out_kind[i] = 0; out_flops[i] = 0.0;
+    out_kind[i] = m->op_kind[i]; out_flops[i] = 0.0;
     if (op.kind() == SB_OPK_CONV || op.kind() == SB_OPK_TCONV) {
-      out_kind[i] = sb_conv_tc_can(m, i) ? 1 : 2;
       const SbBuffer& ib = m->buffers[op.in_buf()];
       const SbBuffer& ob = m->buffers[op.out_buf()];
       const double pix = op.kind() == SB_OPK_TCONV ? (double)ib.H * ib.W : (double)ob.H * ob.W;

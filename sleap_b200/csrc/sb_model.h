@@ -73,8 +73,12 @@ struct SbConvTcPlan;  // sb_conv_tc.cu
 struct SbConv01Plan;  // sb_conv01.cu
 struct SbTopdown;     // sb_topdown.cu
 
+// One op's slot of a program: its launches for a batch of B frames (the frames feed the input stage), everything else
+// fixed at configure time.  An empty slot launches nothing: its op runs inside a neighbour's launch.
+using SbLaunchFn = std::function<int(sb_handle_s* h, const void* frames_dev, int frames_are_u8, int B)>;
+
 // The input stage (sb_entry.cu): how a forward pass gets from the raw frame to the first activation the op loop reads.
-// Resolved and timed once by sb_model_configure; run_ops_t hands every op it covers to sb_entry_run.
+// Resolved and timed once by sb_model_configure, which then fills the slots it covers in both programs.
 enum {
   SB_ENTRY_GENERIC = 0,    // k_preprocess as an ordinary op, then the op loop
   SB_ENTRY_DIRECT,         // k_conv_first: the first conv on the CUDA cores, preprocessing fused
@@ -86,14 +90,13 @@ struct SbEntryPlan {
   int route = SB_ENTRY_GENERIC;
   int pre_op = -1;                 // the PREPROCESS op when the first conv's launch preprocesses the frame (an empty slot)
   int conv_op = -1;                // the first conv, unless the route is generic
-  int conv1_op = -1;               // conv1 when the fused first block won: an empty slot, k_conv01 runs in conv_op's
-                                   // (unless the forward asks for a tensor inside the block: keep_dead_stores)
+  int conv1_op = -1;               // conv1 when the fused first block won: in the production program, k_conv01 runs in
+                                   // conv_op's slot and the slots of conv1 and its pool are empty
   SbConv01Plan* conv01 = nullptr;  // fused first encoder block k_conv01 over conv_op and conv_op + 1 (sb_conv01.cu)
   __half* view = nullptr;          // view routes: the [B][view_H][view_W][16] fp16 view the GEMM reads
   float* view_bias = nullptr;      // Toeplitz view: the bias replicated over the 8 pixels of a group
   int view_H = 0, view_W = 0;
   int pre_mode = SB_PRE_PLAIN;     // stem view: the PREPROCESS mode k_s2d_view applies
-  bool covers(int oi) const { return oi == pre_op || oi == conv_op || oi == conv1_op; }
 };
 
 struct SbModel {
@@ -109,7 +112,12 @@ struct SbModel {
   size_t act_bytes = 0;
   void* frames_dev = nullptr;
   std::vector<SbConvTcPlan*> tc_plans;  // per op (nullptr = direct path)
-  std::vector<char> skip_op;            // 1: POOL fused into the producing tensor-core conv; 2: ADD fused into the conv before it
+  // The forward pass, one slot per op, built at the end of sb_model_configure: prog[0] is the production program (stores
+  // nobody reads inside the network elided, fused POOL and ADD slots empty, k_conv01 where it won), prog[1] stores every
+  // tensor (a fused residual ADD and the first block's convs as their own launches) for a forward that asks for one of them
+  std::vector<SbLaunchFn> prog[2];
+  std::vector<int> op_kind;             // per op, as sb_model_profile_ops reports it
+  std::vector<char> buf_elided;         // per buffer: the production program may not store it
   std::vector<cudaEvent_t> prof_events; // non-empty only inside sb_model_profile_ops
   std::vector<cudaEvent_t> fwd_events;  // sb_model_forward_times: (start, end) pairs around every forward pass
   int fwd_n = 0;                        // pairs recorded since the last read
@@ -138,7 +146,6 @@ struct SbModel {
   SbTopdown* td = nullptr;
   SbEntryPlan entry;                       // input stage (sb_entry.cu)
   SbGather gather;                         // peer-memory exchange of the result records (sb_gather.cu)
-  bool keep_dead_stores = false;           // sb_model_forward asked for a tensor whose stores are normally elided
   // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu); its per-frame track records
   // ([B][sb_track_record_width] doubles) live beside the result records and travel with the result copy
   SbTracker* trk = nullptr;
@@ -148,7 +155,8 @@ struct SbModel {
   double* trk_host[3] = {nullptr, nullptr, nullptr};   // pinned: collect slots 0 / 1, sb_infer_bottomup
 };
 
-int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);
+// one forward pass: the production program, or the all-stores one
+int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B, bool all_stores = false);
 
 void sb_topdown_free(SbModel* m);        // sb_topdown.cu
 
@@ -163,9 +171,13 @@ void sb_pipeline_slots_free(SbModel* m);
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m);      // after buffers are allocated
 int sb_conv_tc_autotune(sb_handle_s* h, SbModel* m);     // launch forms of every plan, the input stage's included
 void sb_conv_tc_release(SbModel* m);
-bool sb_conv_tc_can(const SbModel* m, int op_index);
-bool sb_conv_tc_out_dead(const SbModel* m, int op_index);    // its stores are elided unless keep_dead_stores is set
-int sb_conv_tc_launch(sb_handle_s* h, SbModel* m, int op_index, int B);
+// The slot of op `op_index` (which has a plan) in the production program or, all_stores, in the all-stores program
+struct SbTcEntry {
+  SbLaunchFn run;
+  int absorbs = -1;         // the op after it (a fused POOL, or a fused residual ADD in production) whose slot is empty
+  bool elides_out = false;  // its own output is not stored
+};
+SbTcEntry sb_conv_tc_entry(const SbModel* m, int op_index, bool all_stores);
 // A stride-1 R x S convolution over a [B][H][W][16] fp16 view that is not an op-list buffer, as the plan of op
 // `op_index`: output pixel (y, x) takes tap (r, s) from view pixel (y + dy0 + r, x + dx0 + s), with the weights
 // w[r * S + s] ([R * S][Cout][16]).  Leaves the op without a plan where the view is smaller than one TMA box.
@@ -185,13 +197,15 @@ int sb_time_min(sb_handle_s* h, const char* what, float& best, const std::functi
 // input stage (sb_entry.cu)
 int sb_entry_prepare(sb_handle_s* h, SbModel* m);       // after sb_conv_tc_prepare: route, views, fused block
 int sb_entry_autotune(sb_handle_s* h, SbModel* m);      // after sb_conv_tc_autotune: direct vs view, fused vs separate
-int sb_entry_run(sb_handle_s* h, SbModel* m, int op_index, const void* frames_dev, int frames_are_u8, int B);
+// fills the slots the input stage covers in m->prog[all_stores], marks them (and the fused block's pool) in `taken`;
+// flags the fused block's two tensors in m->buf_elided
+void sb_entry_build(SbModel* m, bool all_stores, std::vector<char>& taken);
 void sb_entry_release(SbModel* m);
 
 // fused first encoder block, run by the input stage (sb_conv01.cu)
 int sb_conv01_prepare(sb_handle_s* h, SbModel* m, int conv0_op, int conv1_op);   // sets m->entry.conv01
 void sb_conv01_release(SbModel* m);
-int sb_conv01_launch(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B);
+int sb_conv01_launch(sb_handle_s* h, const SbConv01Plan* pl, const void* frames_dev, int frames_are_u8, int B);
 
 // programmatic dependent launch for the conv kernels (sb_conv_tc.cu); SB_DISABLE_PDL=1 switches it off
 bool sb_pdl_on();

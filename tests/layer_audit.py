@@ -291,7 +291,8 @@ class Audit:
         self.conv01_ops = self._conv01_ops()
         self.production = True
 
-    # ---- which kernels run (mirrors the input stage's rules in sb_entry.cu: first_fusable, stem_fusable, conv01_fusable) ----
+    # ---- which kernels run (mirrors the input stage's rules in sb_entry.cu: first_fusable, stem_fusable, conv01_fusable,
+    # and the fused pool / ADD slots of sb_conv_tc_entry in sb_conv_tc.cu) ----
     def _only_reader(self, buf, reader):
         for j, o in enumerate(self.ops):
             if j == reader or o[0] == ol.PREPROCESS:
