@@ -623,9 +623,10 @@ static int queue_track_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, 
 
 // Peak finding / PAF scoring / matching / grouping of this batch on the handle's post-processing
 // stream: it only depends on the head outputs, so it overlaps the network of the next batch
-// (run_ops waits on post_done_ev right before it overwrites a head buffer).
+// (run_ops waits on post_done_ev right before it overwrites a head buffer).  Without the overlap
+// (SB_DISABLE_POST_OVERLAP: no guard op) it still runs there, so that work a caller queues on the
+// post-processing stream stays behind it, and the handle's stream waits for it at once.
 static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
-  if (m->guard_op < 0) return bottomup_post_kernels(h, m, B);
   cudaStream_t main_stream = h->stream;
   SB_CUDA(h, cudaEventRecord(h->fwd_done_ev, main_stream));
   SB_CUDA(h, cudaStreamWaitEvent(h->post_stream, h->fwd_done_ev, 0));
@@ -635,7 +636,8 @@ static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
   h->stream = main_stream;
   if (rc) return rc;
   if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "event record: %s", cudaGetErrorString(e));
-  h->post_pending = true;
+  if (m->guard_op < 0) SB_CUDA(h, cudaStreamWaitEvent(main_stream, h->post_done_ev, 0));
+  else h->post_pending = true;
   return 0;
 }
 
