@@ -247,6 +247,40 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* params, const
                           int cap_cands, int32_t* edge_inds, int32_t* edge_peak_inds,
                           float* line_scores, int32_t* cand_offsets);
 
+/* ---- bottom-up multi-class (identity) step -----------------------------------------------------------
+ * sleap/nn/inference.py:3351-3589 BottomUpMultiClassInferenceLayer.call: preprocess -> net -> local peaks
+ * -> * cm_output_stride -> class probability at each peak (sigmoid of the class-map logit at the rounded class-map cell,
+ * 0 outside the map) -> per (frame, node) SciPy assignment of peaks to classes on -probability, a match kept only where
+ * it is the peak's most probable class -> (/input_scale + 0.5).  One record per frame comes back.
+ * A model runs one post-processing chain at a time: sb_multiclass_configure drops the plain bottom-up chain (with its
+ * tracker and record exchange) and sb_bottomup_configure drops this one. */
+#define SB_MAX_CLASSES 128
+typedef struct sb_multiclass_params {
+  int32_t cms_buffer, class_maps_buffer, offsets_buffer; /* op-list buffer ids (offsets: -1 if none) */
+  int32_t cm_output_stride, class_maps_output_stride;
+  float peak_threshold;
+  int32_t refinement, integral_patch_size;
+  int32_t n_nodes, n_classes;          /* n_classes <= SB_MAX_CLASSES */
+  float input_scale;
+  int32_t max_peaks_per_sample, max_node_peaks;
+} sb_multiclass_params;
+
+int sb_multiclass_configure(sb_handle_t h, int model_id, const sb_multiclass_params* params);
+/* frames (B,H,W,C_in) uint8 or float32.  Outputs, class-indexed and NaN where no peak was assigned:
+ * out_points (B,n_classes,n_nodes,2), out_vals (B,n_classes,n_nodes) peak values,
+ * out_class_probs (B,n_classes,n_nodes), out_flags (B) SB_FLAG_* (may be NULL). */
+int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B,
+                        float* out_points, float* out_vals, float* out_class_probs, int32_t* out_flags);
+/* The double-buffered form, as sb_bottomup_submit / sb_bottomup_collect (uint8 frames). */
+int sb_multiclass_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
+int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals,
+                          float* out_class_probs, int32_t* out_flags);
+/* The same post-processing on caller-supplied maps (no network): cms (B,H,W,n_nodes), class-map logits
+ * (B,Hc,Wc,n_classes), optional learned offsets (B,H,W,2*n_nodes).  params->*_buffer fields are ignored. */
+int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* params, const float* cms_host, int B, int H, int W,
+                            const float* class_logits_host, int Hc, int Wc, const float* offsets_host, float* out_points,
+                            float* out_vals, float* out_class_probs, int32_t* out_flags);
+
 /* ---- multi-GPU: exchange of the per-frame result records over NVLink peer memory -----------------
  * The reference runs on one GPU (sleap/nn/system.py:29-46 rejects more than one visible device); its consumer of the
  * per-frame results is Predictor._make_labeled_frames_from_generator (sleap/nn/inference.py:3230-3343).  Here frames

@@ -40,6 +40,19 @@ class BottomUpParams(ctypes.Structure):
     ]
 
 
+class MultiClassParams(ctypes.Structure):
+    _fields_ = [
+        ("cms_buffer", c_int32), ("class_maps_buffer", c_int32), ("offsets_buffer", c_int32),
+        ("cm_output_stride", c_int32), ("class_maps_output_stride", c_int32),
+        ("peak_threshold", c_float), ("refinement", c_int32), ("integral_patch_size", c_int32),
+        ("n_nodes", c_int32), ("n_classes", c_int32), ("input_scale", c_float),
+        ("max_peaks_per_sample", c_int32), ("max_node_peaks", c_int32),
+    ]
+
+
+MAX_CLASSES = 128           # SB_MAX_CLASSES (include/sleap_b200.h)
+
+
 class GlobalParams(ctypes.Structure):
     _fields_ = [
         ("cms_buffer", c_int32), ("offsets_buffer", c_int32), ("output_stride", c_int32),
@@ -118,6 +131,12 @@ _SIGS = {
     "sb_bottomup_from_maps": [c_void_p, POINTER(BottomUpParams), c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int,
                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_multiclass_configure": [c_void_p, c_int, POINTER(MultiClassParams)],
+    "sb_infer_multiclass": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_multiclass_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
+    "sb_multiclass_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_multiclass_from_maps": [c_void_p, POINTER(MultiClassParams), c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sb_gather_init": [c_void_p, c_int, c_int, c_int, c_int, c_void_p],
     "sb_gather_connect": [c_void_p, c_int, c_void_p],
     "sb_gather_enabled": [c_void_p, c_int],

@@ -20,6 +20,7 @@ struct SbPostWs {
   int B = 0, H = 0, W = 0, C = 0;          // confidence-map shape the workspace was sized for
   int rows_per_chunk = 0, n_chunks = 0, chunk_cap = 0;
   int max_peaks = 0, max_node_peaks = 0, max_instances = 0, n_edges = 0;
+  bool node_lists = false;                  // k_local_emit builds node_cnt / node_peaks (PAF matching, class grouping)
   // local peaks
   int* chunk_cnt = nullptr;                 // [B][n_chunks]
   uint2* chunk_items = nullptr;             // [B][n_chunks][chunk_cap]  (flat idx, val bits)
@@ -43,7 +44,8 @@ struct SbPostWs {
   int* n_inst = nullptr;                    // [B]
   int* flags = nullptr;                     // [B]  overflow bit flags
   // contiguous per-frame result records written by the grouping kernel's epilogue:
-  // [B][I*C*2 peaks | I*C vals | I scores | n_valid | flags]  (sb_record_width floats per frame)
+  // [B][I*C*2 peaks | I*C vals | I scores | n_valid | flags]  (sb_record_width floats per frame),
+  // or by k_class_group: [B][sb_class_record_width floats]
   float* records = nullptr;
   uint2* sorted_items = nullptr;            // [B][max_peaks]  scanned items in tf.where order (k_local_emit scratch)
   int* edges_dev = nullptr;                 // [E][2]
@@ -81,6 +83,11 @@ struct SbGather {
 static __host__ __device__ inline size_t sb_record_width(int max_instances, int n_nodes) {
   // peaks | values | scores | n_valid | flags, padded to a multiple of 4 floats (16-byte rows for vector copies)
   return (((size_t)max_instances * n_nodes * 3 + max_instances + 2) + 3) & ~(size_t)3;
+}
+static __host__ __device__ inline size_t sb_class_record_width(int n_classes, int n_nodes) {
+  // points [n_classes][n_nodes][2] | values [n_classes][n_nodes] | class probabilities [n_classes][n_nodes] | flags,
+  // padded to a multiple of 4 floats
+  return (((size_t)n_classes * n_nodes * 4 + 1) + 3) & ~(size_t)3;
 }
 
 struct sb_handle_s {
@@ -157,6 +164,10 @@ int sbk_score_match(sb_handle_s* h, const float* pafs, int B, int Hp, int Wp, in
                     SbPostWs& ws);
 int sbk_group(sb_handle_s* h, int B, int n_nodes, int min_instance_peaks, float min_line_scores,
               float input_scale, SbPostWs& ws, const SbGatherDev* gather = nullptr);
+// identity grouping of the multi-class step on ws's per-node peak lists and the class-map logits (B,Hc,Wc,n_classes):
+// one record per frame into ws.records (sb_class_record_width); ws must have node_lists and records
+int sbk_class_group(sb_handle_s* h, const float* class_maps, int B, int Hc, int Wc, int n_classes, float class_stride,
+                    float input_scale, SbPostWs& ws);
 int sbk_lsap_batch(sb_handle_s* h, const float* scores, const int* n_src, const int* n_dst,
                    const int* offsets, int n_problems, int max_k, int* out_rows, int* out_cols,
                    float* out_scores, int* out_counts);

@@ -171,7 +171,7 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   sb_pipeline_slots_free(m);
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes): re-init after a reconfigure
   m->configured = false;
-  m->bu_configured = false; m->gl_configured = false; m->ce_configured = false; m->td_configured = false;
+  m->bu_configured = false; m->mc_configured = false; m->gl_configured = false; m->ce_configured = false; m->td_configured = false;
   for (auto& p : m->prog) p.clear();             // the programs refer to the plans
   sb_entry_release(m);
   sb_conv_tc_release(m);
@@ -506,7 +506,30 @@ int sb_model_forward_times(sb_handle_t h, int model_id, int enable, int cap, flo
   return SB_OK;
 }
 
+}  // extern "C"
+
 // ---------------------------------- bottom-up ------------------------------------------------
+// A model's bottom-up step runs one post-processing chain: the PAF chain (sb_bottomup_configure) or the multi-class
+// chain (sb_multiclass_configure).  Both share the workspace, the result records, the pinned staging, the copy stream
+// and the slot events; what differs is the record width and the kernels queued after the network.
+
+// The first op that overwrites one of the head buffers the post-processing reads (-1: none, or SB_DISABLE_POST_OVERLAP):
+// the network of the next step waits for the previous step's post-processing right before it.
+static int post_guard_op(const SbModel* m, int b0, int b1, int b2) {
+  if (getenv("SB_DISABLE_POST_OVERLAP")) return -1;
+  for (size_t i = 0; i < m->ops.size(); ++i) {
+    const int ob = m->ops[i].out_buf();
+    if (ob == b0 || ob == b1 || (b2 >= 0 && ob == b2)) return (int)i;
+  }
+  return -1;
+}
+
+static size_t record_width(const SbModel* m) {
+  return m->mc_configured ? sb_class_record_width(m->mc.n_classes, m->mc.n_nodes) : sb_record_width(m->bu.max_instances, m->bu.n_nodes);
+}
+
+extern "C" {
+
 int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params* p) {
   SbModel* m = get_model(h, model_id);
   if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
@@ -528,6 +551,7 @@ int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params*
   SB_CUDA(h, cudaDeviceSynchronize());          // in-flight post-processing / result copies still use the old workspace
   h->post_pending = false;
   m->bu_configured = false;
+  m->mc_configured = false;
   sb_pipeline_slots_free(m);                      // staging records are sized from max_instances / n_nodes
   sb_gather_free(m);
   sb_post_ws_free(m->ws);
@@ -540,31 +564,64 @@ int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params*
   m->bu = *p;
   m->bu.edges = nullptr; m->bu.sorted_edge_inds = nullptr;
   m->bu_edges.assign(p->edges, p->edges + 2 * p->n_edges);
-  m->guard_op = -1;
-  if (!getenv("SB_DISABLE_POST_OVERLAP"))
-    for (size_t i = 0; i < m->ops.size(); ++i) {
-      const int ob = m->ops[i].out_buf();
-      if (ob == p->cms_buffer || ob == p->pafs_buffer || (p->offsets_buffer >= 0 && ob == p->offsets_buffer)) { m->guard_op = (int)i; break; }
-    }
+  m->guard_op = post_guard_op(m, p->cms_buffer, p->pafs_buffer, p->offsets_buffer);
   m->bu_configured = true;
   return SB_OK;
 }
 
+int sb_multiclass_configure(sb_handle_t h, int model_id, const sb_multiclass_params* p) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
+  if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first");
+  SB_CUDA(h, cudaSetDevice(h->device));
+  const int nb = (int)m->buffers.size();
+  if (p->cms_buffer < 0 || p->cms_buffer >= nb || p->class_maps_buffer < 0 || p->class_maps_buffer >= nb)
+    return sb_fail(h, SB_ERR_INVALID, "cms / class-map buffer ids out of range");
+  SbBuffer& cb = m->buffers[p->cms_buffer];
+  SbBuffer& kb = m->buffers[p->class_maps_buffer];
+  if (!cb.f32 || !kb.f32) return sb_fail(h, SB_ERR_INVALID, "cms / class-map buffers must be f32 head outputs");
+  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES)
+    return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
+  if (cb.C != p->n_nodes || kb.C != p->n_classes) return sb_fail(h, SB_ERR_INVALID, "head channels do not match nodes / classes");
+  if (p->offsets_buffer >= 0 && (p->offsets_buffer >= nb || !m->buffers[p->offsets_buffer].f32 || m->buffers[p->offsets_buffer].C != 2 * p->n_nodes))
+    return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
+  if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
+      p->max_node_peaks <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "bad strides / input scale / capacities");
+  SB_CUDA(h, cudaDeviceSynchronize());          // in-flight post-processing / result copies still use the old workspace
+  h->post_pending = false;
+  m->bu_configured = false;
+  m->mc_configured = false;
+  m->trk = nullptr;                               // the tracker and the record exchange belong to the PAF chain
+  sb_pipeline_slots_free(m);
+  sb_gather_free(m);
+  sb_post_ws_free(m->ws);
+  int rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0);
+  if (rc) return rc;
+  m->ws.node_lists = true;
+  const size_t nrec = (size_t)m->B * sb_class_record_width(p->n_classes, p->n_nodes);
+  if ((rc = sb_dev_alloc(h, &m->ws.records, nrec))) return rc;
+  m->ws.bytes += nrec * sizeof(float);
+  m->mc = *p;
+  m->guard_op = post_guard_op(m, p->cms_buffer, p->class_maps_buffer, p->offsets_buffer);
+  m->mc_configured = true;
+  return SB_OK;
+}
+
 static size_t stage_floats(const SbModel* m) {          // [world][B][width] when the exchange is connected
-  return (size_t)(m->gather.connected ? m->gather.world : 1) * m->B * sb_record_width(m->bu.max_instances, m->bu.n_nodes);
+  return (size_t)(m->gather.connected ? m->gather.world : 1) * m->B * record_width(m);
 }
 
 // One D2H copy of a batch's results into pinned `dst`: the rank's own records, or -- exchange connected -- the whole gather
 // window of the step just pushed (device-side wait for the peers, copy, acknowledge; all on stream rs).
 static int queue_result_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, float* dst, int counts_slot) {
-  const size_t w = sb_record_width(m->bu.max_instances, m->bu.n_nodes);
   if (m->gather.connected)
     return sb_gather_queue_collect(h, m, m->gather.step - 1, B, dst, m->gather.counts_dev + counts_slot * SB_GATHER_MAX_WORLD, rs);
-  SB_CUDA(h, cudaMemcpyAsync(dst, m->ws.records, (size_t)B * w * sizeof(float), cudaMemcpyDeviceToHost, rs));
+  SB_CUDA(h, cudaMemcpyAsync(dst, m->ws.records, (size_t)B * record_width(m) * sizeof(float), cudaMemcpyDeviceToHost, rs));
   return 0;
 }
 static const float* own_slice(const SbModel* m, const float* staged, int B) {
-  return staged + (m->gather.connected ? (size_t)m->gather.rank * B * sb_record_width(m->bu.max_instances, m->bu.n_nodes) : 0);
+  return staged + (m->gather.connected ? (size_t)m->gather.rank * B * record_width(m) : 0);
 }
 static int check_exchange(sb_handle_s* h, SbModel* m) {
   if (m->gather.connected && *m->gather.status_host != 0) {
@@ -613,6 +670,30 @@ static int bottomup_post_kernels(sb_handle_s* h, SbModel* m, int B) {
                         m->trk_cut, m->trk_h, m->trk_w, m->trk_dev);
 }
 
+// The multi-class chain: local peaks with their per-node lists, then the identity grouping into the records.
+static int multiclass_post_kernels(sb_handle_s* h, SbModel* m, int B) {
+  const sb_multiclass_params& p = m->mc;
+  SbBuffer& cb = m->buffers[p.cms_buffer];
+  SbBuffer& kb = m->buffers[p.class_maps_buffer];
+  const float* off = p.offsets_buffer >= 0 ? (const float*)m->buffers[p.offsets_buffer].dev : nullptr;
+  SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
+  int rc = sbk_local_peaks(h, cb.dev, 0, off, B, cb.H, cb.W, cb.C, pp, m->ws);
+  if (rc) return rc;
+  return sbk_class_group(h, (const float*)kb.dev, B, kb.H, kb.W, kb.C, (float)p.class_maps_output_stride, p.input_scale, m->ws);
+}
+
+static void unpack_class_records(const float* rec, size_t w, int B, int n_classes, int n_nodes, float* out_points,
+                                 float* out_vals, float* out_class_probs, int32_t* out_flags) {
+  const size_t n1 = (size_t)n_classes * n_nodes;
+  for (int b = 0; b < B; ++b) {
+    const float* r = rec + (size_t)b * w;
+    memcpy(out_points + (size_t)b * n1 * 2, r, n1 * 2 * sizeof(float));
+    memcpy(out_vals + (size_t)b * n1, r + n1 * 2, n1 * sizeof(float));
+    memcpy(out_class_probs + (size_t)b * n1, r + n1 * 3, n1 * sizeof(float));
+    if (out_flags) out_flags[b] = (int32_t)r[n1 * 4];
+  }
+}
+
 // The track records of a batch go to the host with its result records, on the same stream.
 static int queue_track_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, int which) {
   if (!m->trk) return 0;
@@ -621,7 +702,8 @@ static int queue_track_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, 
   return 0;
 }
 
-// Peak finding / PAF scoring / matching / grouping of this batch on the handle's post-processing
+// The configured chain's post-processing of this batch (peak finding, then PAF scoring / matching /
+// grouping or the identity grouping) on the handle's post-processing
 // stream: it only depends on the head outputs, so it overlaps the network of the next batch
 // (run_ops waits on post_done_ev right before it overwrites a head buffer).  Without the overlap
 // (SB_DISABLE_POST_OVERLAP: no guard op) it still runs there, so that work a caller queues on the
@@ -631,7 +713,7 @@ static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
   SB_CUDA(h, cudaEventRecord(h->fwd_done_ev, main_stream));
   SB_CUDA(h, cudaStreamWaitEvent(h->post_stream, h->fwd_done_ev, 0));
   h->stream = h->post_stream;
-  int rc = bottomup_post_kernels(h, m, B);
+  int rc = m->mc_configured ? multiclass_post_kernels(h, m, B) : bottomup_post_kernels(h, m, B);
   cudaError_t e = cudaEventRecord(h->post_done_ev, h->post_stream);
   h->stream = main_stream;
   if (rc) return rc;
@@ -650,16 +732,13 @@ int sb_infer_bottomup_dev(sb_handle_t h, int model_id, const uint8_t* frames_dev
   return bottomup_post(h, m, B);
 }
 
-int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, float* out_instance_peaks,
-                      float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
-                      int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+// One synchronous step of the configured chain: upload, network, post-processing, one result copy into rec_host.
+static int step_sync(sb_handle_s* h, SbModel* m, const void* frames_host, int frames_are_u8, int B) {
   SB_CUDA(h, cudaSetDevice(h->device));
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
-  int rc = upload_frames(h, m, frames_host, 1, B);
+  int rc = upload_frames(h, m, frames_host, frames_are_u8, B);
   if (rc) return rc;
-  if ((rc = sb_run_ops(h, m, m->frames_dev, 1, B))) return rc;
+  if ((rc = sb_run_ops(h, m, m->frames_dev, frames_are_u8, B))) return rc;
   if ((rc = bottomup_post(h, m, B))) return rc;
   cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
   if (!m->rec_host) SB_CUDA(h, cudaHostAlloc((void**)&m->rec_host, stage_floats(m) * sizeof(float), cudaHostAllocDefault));
@@ -668,8 +747,26 @@ int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, i
   SB_CUDA(h, cudaStreamSynchronize(rs));
   h->post_pending = false;
   m->rec_B = B;
-  if ((rc = check_exchange(h, m))) return rc;
+  return check_exchange(h, m);
+}
+
+int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, float* out_instance_peaks,
+                      float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
+                      int32_t* out_flags) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  if (const int rc = step_sync(h, m, frames_host, 1, B)) return rc;
   unpack_records(m, own_slice(m, m->rec_host, B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
+  return SB_OK;
+}
+
+int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B, float* out_points,
+                        float* out_vals, float* out_class_probs, int32_t* out_flags) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
+  if (!frames_host || !out_points || !out_vals || !out_class_probs) return sb_fail(h, SB_ERR_INVALID, "sb_infer_multiclass: null argument");
+  if (const int rc = step_sync(h, m, frames_host, frames_are_u8 ? 1 : 0, B)) return rc;
+  unpack_class_records(m->rec_host, record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -694,9 +791,7 @@ int sb_get_post_stream(sb_handle_t h, void** out_stream) {
 // batch i+1 (its H2D copy runs on a copy stream) while batch i computes, then collect batch i.
 // Layout of the pinned staging record per slot: peaks | vals | scores | n_valid | flags.
 
-int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot) {
   if (slot < 0 || slot > 1 || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
   SB_CUDA(h, cudaSetDevice(h->device));
   if (!m->copy_stream) {
@@ -730,16 +825,42 @@ int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, 
   return SB_OK;
 }
 
+// Blocks until the records of the batch submitted into `slot` are in its pinned staging.
+static int step_collect(sb_handle_s* h, SbModel* m, int slot, int B) {
+  if (slot < 0 || slot > 1 || !m->slot_used[slot] || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
+  SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
+  return check_exchange(h, m);
+}
+
+int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  return step_submit(h, m, frames_host, B, slot);
+}
+
 int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out_instance_peaks,
                         float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
                         int32_t* out_flags) {
   SbModel* m = get_model(h, model_id);
   if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
-  if (slot < 0 || slot > 1 || !m->slot_used[slot] || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
-  SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
-  int rc = check_exchange(h, m);
-  if (rc) return rc;
+  if (const int rc = step_collect(h, m, slot, B)) return rc;
   unpack_records(m, own_slice(m, m->stage_host[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
+  return SB_OK;
+}
+
+int sb_multiclass_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
+  return step_submit(h, m, frames_host, B, slot);
+}
+
+int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals,
+                          float* out_class_probs, int32_t* out_flags) {
+  SbModel* m = get_model(h, model_id);
+  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
+  if (const int rc = step_collect(h, m, slot, B)) return rc;
+  unpack_class_records(m->stage_host[slot], record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals,
+                       out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -926,6 +1047,51 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const floa
   if (peaks)
     return fetch_graph_ws(h, ws, p->edges, B, cap_peaks, peaks, peak_vals, peak_channel_inds, peak_offsets, cap_cands,
                           edge_inds, edge_peak_inds, line_scores, cand_offsets);
+  return SB_OK;
+}
+
+int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const float* cms_host, int B, int H, int W,
+                            const float* class_logits_host, int Hc, int Wc, const float* offsets_host, float* out_points,
+                            float* out_vals, float* out_class_probs, int32_t* out_flags) {
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "null handle / params");
+  if (!cms_host || !class_logits_host || !out_points || !out_vals || !out_class_probs)
+    return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: null argument");
+  if (B <= 0 || H <= 0 || W <= 0 || Hc <= 0 || Wc <= 0 || p->n_nodes <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: bad shape");
+  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES) return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
+  if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
+      p->max_node_peaks <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: bad strides / input scale / capacities");
+  SB_CUDA(h, cudaSetDevice(h->device));
+  const int C = p->n_nodes, NC = p->n_classes;
+  SbPostWs ws;
+  struct Guard { SbPostWs& w; std::vector<void*> bufs; ~Guard() { sb_post_ws_free(w); for (void* q : bufs) cudaFree(q); } } guard{ws, {}};
+  int rc = sb_post_ws_alloc(h, ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0);
+  if (rc) return rc;
+  ws.node_lists = true;
+  const size_t w = sb_class_record_width(NC, C);
+  if ((rc = sb_dev_alloc(h, &ws.records, (size_t)B * w))) return rc;
+  auto dalloc = [&](void** q, size_t bytes) -> int {
+    cudaError_t e = cudaMalloc(q, bytes + 16);
+    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc: %s", cudaGetErrorString(e));
+    guard.bufs.push_back(*q);
+    return 0;
+  };
+  void *d_cms = nullptr, *d_cls = nullptr, *d_off = nullptr;
+  const size_t ncm = (size_t)B * H * W * C, ncl = (size_t)B * Hc * Wc * NC;
+  if ((rc = dalloc(&d_cms, ncm * 4)) || (rc = dalloc(&d_cls, ncl * 4))) return rc;
+  SB_CUDA(h, cudaMemcpyAsync(d_cms, cms_host, ncm * 4, cudaMemcpyHostToDevice, h->stream));
+  SB_CUDA(h, cudaMemcpyAsync(d_cls, class_logits_host, ncl * 4, cudaMemcpyHostToDevice, h->stream));
+  if (offsets_host) {
+    if ((rc = dalloc(&d_off, 2 * ncm * 4))) return rc;
+    SB_CUDA(h, cudaMemcpyAsync(d_off, offsets_host, 2 * ncm * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  SbPeakParams pp{p->peak_threshold, p->refinement, p->integral_patch_size, (float)p->cm_output_stride, 1.0f};
+  if ((rc = sbk_local_peaks(h, d_cms, 0, (const float*)d_off, B, H, W, C, pp, ws))) return rc;
+  if ((rc = sbk_class_group(h, (const float*)d_cls, B, Hc, Wc, NC, (float)p->class_maps_output_stride, p->input_scale, ws))) return rc;
+  std::vector<float> rec((size_t)B * w);
+  SB_CUDA(h, cudaMemcpyAsync(rec.data(), ws.records, rec.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  SB_CUDA(h, cudaStreamSynchronize(h->stream));
+  unpack_class_records(rec.data(), w, B, NC, C, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 

@@ -127,8 +127,10 @@ struct SbModel {
   sb_bottomup_params bu{};
   std::vector<int> bu_edges;
   bool bu_configured = false;
+  sb_multiclass_params mc{};
+  bool mc_configured = false;              // the multi-class chain (k_class_group) instead of the PAF chain; one at a time
   int guard_op = -1;
-  // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect)
+  // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect, sb_multiclass_submit / _collect)
   void* frames_slot[2] = {nullptr, nullptr};
   float* stage_host[2] = {nullptr, nullptr};     // pinned result staging (per-frame records)
   int slot_B[2] = {0, 0}, rec_B = 0;            // frames of the batch last staged in each slot / in rec_host

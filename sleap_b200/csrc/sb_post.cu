@@ -16,6 +16,7 @@
 //   k_group       : sleap/nn/paf_grouping.py:799-914, :917-981, :984-1112
 #include "sb_common.cuh"
 
+#include <algorithm>
 #include <math_constants.h>
 #include "sb_lsap.cuh"
 
@@ -856,6 +857,95 @@ __global__ void __launch_bounds__(128) k_group(
 }
 
 // ------------------------------------------------------------------------------------------
+// Identity grouping of the bottom-up multi-class step: one CTA per (node, sample).  The threads read the class-map
+// logits of the node's peaks (k_local_emit's per-node list, tf.where order) at the rounded class-map cell, apply the
+// sigmoid to those values only, and NaN-fill the node's cells of the frame's record; thread 0 then solves SciPy's
+// assignment on -probability (rows: peaks, columns: classes) and keeps a match only where its probability is the
+// peak's best over all classes.  The CTA of node 0 writes the frame's flags and padding.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) k_class_group(
+    const float* __restrict__ class_maps /*[B][Hc][Wc][NC] logits*/, int Hc, int Wc, int NC, float class_stride,
+    float input_scale, int C, int K, int max_peaks, const float* __restrict__ peaks, const float* __restrict__ peak_vals,
+    const int* __restrict__ node_cnt, const int* __restrict__ node_peaks, const int* __restrict__ flags,
+    float* __restrict__ records /*[B][sb_class_record_width(NC, C)]*/) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int c = blockIdx.x, b = blockIdx.y;
+  const int n = min(node_cnt[b * C + c], K);
+  const int L = max(K, NC), M = min(K, NC);
+  unsigned char* s_lsap = smem_raw;                                                        // LSAP scratch for max(K, NC)
+  float* s_prob = reinterpret_cast<float*>(smem_raw + ((lsap_scratch_bytes(L) + 15) & ~(size_t)15));   // [K][NC]
+  float* s_pt = s_prob + K * NC;                                                           // [K][2] output points
+  int* s_cell = reinterpret_cast<int*>(s_pt + 2 * K);                                      // [K] class-map cell or -1
+  int* s_rows = s_cell + K;                                                                // [M]
+  int* s_cols = s_rows + M;                                                                // [M]
+  const int* lst = node_peaks + ((size_t)b * C + c) * K;
+  const float* pk = peaks + (size_t)b * max_peaks * 2;
+  const float* pv = peak_vals + (size_t)b * max_peaks;
+  const float* cmap = class_maps + (size_t)b * Hc * Wc * NC;
+  // (1) per peak: its class-map cell and its output point, ((peak / cs) * cs) [/ input_scale + 0.5] in separate fp32 ops
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const int pi = lst[i];
+    const float xs = pk[2 * pi] / class_stride, ys = pk[2 * pi + 1] / class_stride;
+    const float col = rintf(xs), row = rintf(ys);            // tf.round: half to even
+    // a cell outside the class map reads 0 (gather_nd on the GPU), not sigmoid(0)
+    s_cell[i] = (row >= 0.f && row < (float)Hc && col >= 0.f && col < (float)Wc) ? (int)row * Wc + (int)col : -1;
+    float x = xs * class_stride, y = ys * class_stride;
+    if (input_scale != 1.0f) {           // inference.py:3555-3577
+      x = x / input_scale + 0.5f;
+      y = y / input_scale + 0.5f;
+    }
+    s_pt[2 * i] = x;
+    s_pt[2 * i + 1] = y;
+  }
+  const int n1 = NC * C;
+  const int w = (int)sb_class_record_width(NC, C);
+  float* rec = records + (size_t)b * w;
+  for (int k = threadIdx.x; k < NC; k += blockDim.x) {
+    const int cell = k * C + c;
+    rec[2 * cell] = CUDART_NAN_F;
+    rec[2 * cell + 1] = CUDART_NAN_F;
+    rec[2 * n1 + cell] = CUDART_NAN_F;
+    rec[3 * n1 + cell] = CUDART_NAN_F;
+  }
+  if (c == 0 && threadIdx.x == 0) {
+    rec[4 * n1] = (float)flags[b];
+    for (int t = 4 * n1 + 1; t < w; ++t) rec[t] = 0.f;   // padding
+  }
+  __syncthreads();
+  // (2) the class probabilities of the node's peaks: the sigmoid of the sampled logits only
+  for (int t = threadIdx.x; t < n * NC; t += blockDim.x) {
+    const int i = t / NC;
+    const int cell = s_cell[i];
+    float p = 0.f;
+    if (cell >= 0) {
+      const double z = (double)cmap[(size_t)cell * NC + (t - i * NC)];
+      p = (float)(1.0 / (1.0 + exp(-z)));                   // identity.class_probabilities
+    }
+    s_prob[t] = p;
+  }
+  __syncthreads();                       // probabilities staged; this CTA's NaN fill ordered before thread 0's stores
+  if (threadIdx.x != 0 || n == 0) return;
+  // (3) SciPy's assignment on -p, then the keep rule
+  LsapScratch s = carve_lsap(s_lsap, L);
+  const int nm = lsap_solve_cost([s_prob, NC](int i, int k) { return -(double)s_prob[i * NC + k]; }, n, NC, s, s_rows, s_cols);
+  for (int q = 0; q < nm; ++q) {
+    const int i = s_rows[q], k = s_cols[q];
+    const float p = s_prob[i * NC + k];
+    float best = s_prob[i * NC];
+    for (int j = 1; j < NC; ++j) {       // np.max: a NaN propagates
+      const float v = s_prob[i * NC + j];
+      best = (v > best || v != v) ? v : best;
+    }
+    if (!(p == best)) continue;
+    const int cell = k * C + c;
+    rec[2 * cell] = s_pt[2 * i];
+    rec[2 * cell + 1] = s_pt[2 * i + 1];
+    rec[2 * n1 + cell] = pv[lst[i]];
+    rec[3 * n1 + cell] = p;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // Centred bilinear crops (top-down): crop_bboxes(make_centered_bboxes(centroid, h, w)).
 // ------------------------------------------------------------------------------------------
 template <typename TI, typename TO, bool TRUNC_U8>
@@ -1002,6 +1092,7 @@ int sb_post_ws_alloc(sb_handle_s* h, SbPostWs& ws, int B, int H, int W, int C, i
   ws.B = B; ws.H = H; ws.W = W; ws.C = C;
   ws.max_peaks = max_peaks; ws.max_node_peaks = max_node_peaks; ws.max_instances = max_instances;
   ws.n_edges = n_edges;
+  ws.node_lists = n_edges > 0;
   // streaming scan: ~8 CTAs of 256 threads per SM over the batch, each with >= ~16 KB of map to walk
   int target_chunks = (8 * h->sm_count + B - 1) / B;
   int rpc = (H + target_chunks - 1) / target_chunks;
@@ -1071,7 +1162,7 @@ int sbk_local_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const floa
                                                   ws.chunk_cap, p.threshold, ws.chunk_cnt, ws.chunk_items);
   SB_CHECK_LAUNCH(h);
   const size_t sm = (size_t)(ws.n_chunks + 1) * sizeof(int);
-  int* ncnt = ws.n_edges > 0 ? ws.node_cnt : nullptr;
+  int* ncnt = ws.node_lists ? ws.node_cnt : nullptr;
   if (cms_is_half)
     k_local_emit<__half><<<B, EMIT_THREADS, sm, h->stream>>>(
         (const __half*)cms, offsets, H, W, C, ws.n_chunks, ws.chunk_cap, p.refinement, p.patch,
@@ -1146,6 +1237,23 @@ int sbk_group(sb_handle_s* h, int B, int n_nodes, int min_instance_peaks, float 
                                      ws.node_peaks, ws.match_cnt, ws.match_src, ws.match_dst, ws.match_score,
                                      min_instance_peaks, min_line_scores, input_scale, ws.inst_peaks,
                                      ws.inst_vals, ws.inst_scores, ws.n_inst, ws.flags, ws.records, gx);
+  SB_CHECK_LAUNCH(h);
+  return 0;
+}
+
+int sbk_class_group(sb_handle_s* h, const float* class_maps, int B, int Hc, int Wc, int n_classes, float class_stride,
+                    float input_scale, SbPostWs& ws) {
+  if (!ws.node_lists || !ws.records || B > ws.B) return sb_fail(h, SB_ERR_INVALID, "class grouping: workspace not sized for it");
+  const int K = ws.max_node_peaks, L = std::max(K, n_classes), M = std::min(K, n_classes);
+  const size_t sm = ((lsap_scratch_bytes(L) + 15) & ~(size_t)15) + ((size_t)K * n_classes + 2 * (size_t)K) * sizeof(float) +
+                    ((size_t)K + 2 * (size_t)M) * sizeof(int);
+  if (sm > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(k_class_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "class group smem %zu: %s", sm, cudaGetErrorString(e));
+  }
+  k_class_group<<<dim3(ws.C, B), 128, sm, h->stream>>>(class_maps, Hc, Wc, n_classes, class_stride, input_scale, ws.C, K,
+                                                        ws.max_peaks, ws.peaks, ws.peak_vals, ws.node_cnt, ws.node_peaks,
+                                                        ws.flags, ws.records);
   SB_CHECK_LAUNCH(h);
   return 0;
 }

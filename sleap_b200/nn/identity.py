@@ -1,6 +1,7 @@
 """Grouping of peaks into identity classes (multi-class models): host-side logic, as in the reference, where these
 functions run as TensorFlow ops around a SciPy ``numpy_function`` (sleap/nn/identity.py, sleap/nn/utils.py:79-98).
 
+  class_probabilities          the class maps' sigmoid (float64, rounded once to float32)
   group_class_peaks            sleap/nn/identity.py:13-94
   classify_peaks_from_maps     sleap/nn/identity.py:97-179
   classify_peaks_from_vectors  sleap/nn/identity.py:182-254
@@ -11,6 +12,13 @@ from typing import Tuple
 
 import numpy as np
 from scipy.optimize import linear_sum_assignment
+
+
+def class_probabilities(logits) -> np.ndarray:
+    """The class maps' sigmoid (heads.py:336-338 of the reference applies it in the graph), evaluated in float64 and
+    rounded once to float32: the one definition the device's multi-class step uses for the logits it samples."""
+    with np.errstate(over="ignore"):         # exp(+large) = inf -> 1 / inf = 0: the limit the sigmoid has there
+        return (1.0 / (1.0 + np.exp(-np.asarray(logits).astype(np.float64)))).astype(np.float32)
 
 
 def group_class_peaks(peak_class_probs, peak_sample_inds, peak_channel_inds, n_samples: int,

@@ -19,7 +19,7 @@ from typing import Dict, List, Optional
 import numpy as np
 
 from sleap_b200 import _lib
-from sleap_b200._lib import BottomUpParams, CentroidParams, GlobalParams, TopdownParams, f32, i32, ptr
+from sleap_b200._lib import BottomUpParams, CentroidParams, GlobalParams, MultiClassParams, TopdownParams, f32, i32, ptr
 from sleap_b200.nn import architectures as arch
 from sleap_b200.nn import paf_grouping, peak_finding
 from sleap_b200.nn.model import DeviceModel, PRECISION_FP16, PRECISION_FP32, load_weights, load_weights_npz
@@ -718,64 +718,98 @@ class BottomUpInferenceModel(InferenceModel):
 # ------------------------------------------------------------------------------------------
 class BottomUpMultiClassInferenceLayer(InferenceLayer):
     """sleap/nn/inference.py:3351-3589: network (confidence maps + class maps) -> local peaks -> identity grouping by the
-    class-map probability at each peak (sleap_b200.nn.identity.classify_peaks_from_maps).  The network and the peak
-    finder run on the device; the grouping is host logic in the reference too (TensorFlow ops around a SciPy callback)."""
+    class-map probability at each peak, executed as one device step (``sb_infer_multiclass``): k_class_group samples
+    the class-map logits at the rounded peak cells, applies the sigmoid (``identity.class_probabilities``) and solves
+    each (frame, node) assignment of peaks to classes, as ``identity.classify_peaks_from_maps`` does on the host."""
+
+    CMS, CLASS_MAPS, OFFSETS = "MultiInstanceConfmapsHead", "ClassMapsHead", "OffsetRefinementHead"
 
     def __init__(self, keras_model, input_scale=1.0, pad_to_stride=1, cm_output_stride=None, class_maps_output_stride=None,
                  peak_threshold=0.2, refinement="integral", integral_patch_size=5, return_confmaps=False,
-                 return_class_maps=False, **kwargs):
+                 return_class_maps=False, max_peaks_per_sample=1024, max_node_peaks=32, **kwargs):
         super().__init__(keras_model, input_scale=input_scale, pad_to_stride=pad_to_stride, **kwargs)
         heads = keras_model.cm.head_buffers
-        if "MultiInstanceConfmapsHead" not in heads:
+        if self.CMS not in heads:
             raise ValueError("Index of the confidence maps output tensor must be specified if not named 'MultiInstanceConfmapsHead'.")
-        if "ClassMapsHead" not in heads:
+        if self.CLASS_MAPS not in heads:
             raise ValueError("Index of the class maps output tensor must be specified if not named 'ClassMapsHead'.")
-        self.has_offsets = "OffsetRefinementHead" in heads
-        self.cm_output_stride = cm_output_stride or keras_model.cm.head_strides["MultiInstanceConfmapsHead"]
-        self.class_maps_output_stride = class_maps_output_stride or keras_model.cm.head_strides["ClassMapsHead"]
+        self.has_offsets = self.OFFSETS in heads
+        self.cm_output_stride = cm_output_stride or keras_model.cm.head_strides[self.CMS]
+        self.class_maps_output_stride = class_maps_output_stride or keras_model.cm.head_strides[self.CLASS_MAPS]
         self.peak_threshold = peak_threshold
         self.refinement = refinement
         self.integral_patch_size = integral_patch_size
         self.return_confmaps = return_confmaps
         self.return_class_maps = return_class_maps
+        self.max_peaks_per_sample = max_peaks_per_sample
+        self.max_node_peaks = max_node_peaks
+        channels = {h["name"]: h["channels"] for h in keras_model.spec["heads"]}
+        self.n_nodes, self.n_classes = int(channels[self.CMS]), int(channels[self.CLASS_MAPS])
+        self._cfg_key = None
 
-    def forward_pass(self, data):
-        """:3462-3490 (the class maps come out of a linear 1x1 head; their sigmoid, heads.py:336-338, is applied here)."""
-        imgs = self._prep(_images_of(data))
-        names = ["MultiInstanceConfmapsHead", "ClassMapsHead"] + (["OffsetRefinementHead"] if self.has_offsets else [])
-        outs = self.keras_model.forward(imgs, names)
-        cms, class_maps = outs[0], outs[1]
-        with np.errstate(over="ignore"):         # exp(+large) = inf -> 1 / inf = 0: the limit the sigmoid has there
-            class_maps = (np.float32(1) / (np.float32(1) + np.exp(-class_maps, dtype=np.float32))).astype(np.float32)
-        return cms, class_maps, (outs[2] if self.has_offsets else None)
+    def params(self) -> MultiClassParams:
+        heads = self.keras_model.cm.head_buffers
+        return MultiClassParams(heads[self.CMS], heads[self.CLASS_MAPS], heads[self.OFFSETS] if self.has_offsets else -1,
+                                int(self.cm_output_stride), int(self.class_maps_output_stride), float(self.peak_threshold),
+                                REFINE.get(self.refinement, 0), int(self.integral_patch_size), self.n_nodes, self.n_classes,
+                                float(self.input_scale), int(self.max_peaks_per_sample), int(self.max_node_peaks))
 
-    def find_peaks(self, cms, offsets):
-        """:3492-3528."""
-        h = self.keras_model.handle
-        if offsets is None:
-            peaks, vals, s_inds, c_inds = peak_finding.find_local_peaks(cms, threshold=self.peak_threshold, refinement=self.refinement,
-                                                                        integral_patch_size=self.integral_patch_size, handle=h)
-        else:
-            peaks, vals, s_inds, c_inds = peak_finding.find_local_peaks_with_offsets(cms, offsets, threshold=self.peak_threshold, handle=h)
-        return (peaks * np.float32(self.cm_output_stride)).astype(np.float32), vals, s_inds, c_inds
+    def _configure(self, B, H, W, C):
+        m = self.keras_model
+        if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
+            m.configure(B, H, W, C)
+            self._cfg_key = None
+        key = (m.configured_for, self.peak_threshold, self.refinement, self.integral_patch_size, self.input_scale,
+               self.cm_output_stride, self.class_maps_output_stride, self.max_peaks_per_sample, self.max_node_peaks)
+        if self._cfg_key != key:
+            p = self.params()
+            m.handle.call("sb_multiclass_configure", m.model_id, byref(p))
+            self._cfg_key = key
+
+    def _outputs(self, B):
+        K, N = self.n_classes, self.n_nodes
+        return (np.zeros((B, K, N, 2), np.float32), np.zeros((B, K, N), np.float32), np.zeros((B, K, N), np.float32),
+                np.zeros((B,), np.int32))
 
     def call(self, data):
         """:3530-3589."""
         from sleap_b200.nn import identity
-        cms, class_maps, offsets = self.forward_pass(data)
-        peaks, peak_vals, s_inds, c_inds = self.find_peaks(cms, offsets)
-        peaks = (peaks / np.float32(self.class_maps_output_stride)).astype(np.float32)
-        inst, inst_vals, inst_scores = identity.classify_peaks_from_maps(class_maps, peaks, peak_vals, s_inds, c_inds,
-                                                                         n_channels=cms.shape[3])
-        inst = (inst * np.float32(self.class_maps_output_stride)).astype(np.float32)
-        if self.input_scale != 1.0:
-            inst = (inst / np.float32(self.input_scale) + np.float32(0.5)).astype(np.float32)
-        out = {"instance_peaks": inst, "instance_peak_vals": inst_vals, "instance_scores": inst_scores}
-        if self.return_confmaps:
-            out["confmaps"] = cms
-        if self.return_class_maps:
-            out["class_maps"] = class_maps
+        imgs = self._prep(_images_of(data))
+        B, H, W, C = imgs.shape
+        self._configure(B, H, W, C)
+        m = self.keras_model
+        pts, vals, probs, fl = self._outputs(B)
+        m.handle.call("sb_infer_multiclass", m.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(pts), ptr(vals),
+                      ptr(probs), ptr(fl))
+        out = {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+        if self.return_confmaps or self.return_class_maps:
+            cms, logits = m.forward(imgs, [self.CMS, self.CLASS_MAPS])
+            if self.return_confmaps:
+                out["confmaps"] = cms
+            if self.return_class_maps:
+                out["class_maps"] = identity.class_probabilities(logits)
         return out
+
+
+def bottomup_multiclass_from_maps(cms, class_logits, cm_output_stride, class_maps_output_stride, peak_threshold=0.2,
+                                  refinement="integral", integral_patch_size=5, offsets=None, input_scale=1.0,
+                                  max_peaks_per_sample=1024, max_node_peaks=32, handle=None):
+    """The BottomUpMultiClassInferenceLayer post-processing (local peaks + k_class_group) on caller-supplied confidence
+    maps (B,H,W,n_nodes) and class-map logits (B,Hc,Wc,n_classes), before the sigmoid -- the parity entry point.  Returns
+    the layer's keys: instance_peaks (B,n_classes,n_nodes,2), instance_peak_vals, instance_scores, flags."""
+    h = handle or _lib.default_handle()
+    cms, class_logits = f32(cms), f32(class_logits)
+    B, H, W, N = cms.shape
+    _, Hc, Wc, K = class_logits.shape
+    p = MultiClassParams(-1, -1, -1, int(cm_output_stride), int(class_maps_output_stride), float(peak_threshold),
+                         REFINE.get(refinement, 0), int(integral_patch_size), N, K, float(input_scale), int(max_peaks_per_sample),
+                         int(max_node_peaks))
+    pts = np.zeros((B, K, N, 2), np.float32); vals = np.zeros((B, K, N), np.float32); probs = np.zeros((B, K, N), np.float32)
+    fl = np.zeros((B,), np.int32)
+    off = None if offsets is None else f32(offsets)
+    h.call("sb_multiclass_from_maps", byref(p), ptr(cms), B, H, W, ptr(class_logits), Hc, Wc, ptr(off), ptr(pts), ptr(vals),
+           ptr(probs), ptr(fl))
+    return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
 
 
 class BottomUpMultiClassInferenceModel(InferenceModel):
@@ -786,6 +820,44 @@ class BottomUpMultiClassInferenceModel(InferenceModel):
 
     def call(self, example):
         return self.inference_layer.call(example)
+
+    def predict_batches(self, data, batch_size: int = 4):
+        """Generator over per-batch result dicts, double-buffered as BottomUpInferenceModel.predict_batches: the upload
+        of batch i+1 overlaps the compute of batch i (uint8 frames; otherwise one predict_on_batch per batch)."""
+        layer = self.inference_layer
+        imgs = _images_of(data)
+        n = len(imgs)
+        if n == 0:
+            return
+        first = layer._prep(np.asarray(imgs[0:min(n, batch_size)]))
+        if first.dtype != np.uint8 or layer.return_confmaps or layer.return_class_maps:
+            for i in range(0, n, batch_size):        # generic (synchronous) path
+                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
+            return
+        _, H, W, C = first.shape
+        layer._configure(batch_size, H, W, C)
+        m = layer.keras_model
+        starts = list(range(0, n, batch_size))
+        keep = {}
+
+        def submit(k):
+            batch = layer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
+            keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
+            m.handle.call("sb_multiclass_submit", m.model_id, ptr(batch), batch.shape[0], k % 2)
+            return batch.shape[0]
+
+        sizes = {0: submit(0)}
+        for k in range(len(starts)):
+            if k + 1 < len(starts):
+                sizes[k + 1] = submit(k + 1)
+            B = sizes.pop(k)
+            pts, vals, probs, fl = layer._outputs(B)
+            m.handle.call("sb_multiclass_collect", m.model_id, k % 2, B, ptr(pts), ptr(vals), ptr(probs), ptr(fl))
+            yield {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+
+    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
+        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
+        return _merge_batches(list(self.predict_batches(data, batch_size)))
 
 
 class TopDownMultiClassFindPeaks(InferenceLayer):
@@ -954,7 +1026,8 @@ class Predictor:
         if "multi_instance" in cfgs:
             return BottomUpPredictor.from_trained_models(cfgs["multi_instance"], max_instances=max_instances, **kw)
         if "multi_class_bottomup" in cfgs:
-            mk = {k: kw[k] for k in ("peak_threshold", "integral_refinement", "integral_patch_size", "batch_size", "precision", "handle")}
+            mk = {k: kw[k] for k in ("peak_threshold", "integral_refinement", "integral_patch_size", "batch_size", "precision", "handle",
+                                     "max_peaks_per_sample", "max_node_peaks") if k in kw}
             return BottomUpMultiClassPredictor.from_trained_models(cfgs["multi_class_bottomup"], **mk)
         raise ValueError("Could not create predictor from model paths:" + "\n".join(model_paths))
 
@@ -1052,7 +1125,7 @@ class Predictor:
                 imgs_all = _images_of(data)
                 hw = tuple(np.asarray(imgs_all[0]).shape[:2]) if len(imgs_all) else (1, 1)
                 for ex in self.inference_model.predict_batches(imgs_all, self.batch_size):
-                    n = len(ex["n_valid"])
+                    n = len(ex["instance_peaks"])
                     ex["frame_ind"] = frame_inds(i0, i0 + n)
                     ex["video_ind"] = np.zeros(n, np.int64)
                     ex["image_hw"] = hw
@@ -1433,7 +1506,8 @@ class BottomUpMultiClassPredictor(Predictor):
     class, in class order; each gets the ``Track`` named after its class (:3781-3790), ``score`` = mean point confidence and
     ``tracking_score`` = mean class probability (:3818-3826)."""
 
-    def __init__(self, model, classes, peak_threshold=0.2, batch_size=4, integral_refinement=True, integral_patch_size=5, tracks=None):
+    def __init__(self, model, classes, peak_threshold=0.2, batch_size=4, integral_refinement=True, integral_patch_size=5, tracks=None,
+                 max_peaks_per_sample=1024, max_node_peaks=32):
         super().__init__(batch_size)
         self.model = model
         self.classes = list(classes)
@@ -1441,6 +1515,7 @@ class BottomUpMultiClassPredictor(Predictor):
         self.integral_refinement = integral_refinement
         self.integral_patch_size = integral_patch_size
         self.tracks = tracks
+        self._caps = (max_peaks_per_sample, max_node_peaks)
         self._initialize_inference_model()
 
     def _initialize_inference_model(self):
@@ -1450,15 +1525,19 @@ class BottomUpMultiClassPredictor(Predictor):
             keras_model=m, input_scale=m.input_scale, pad_to_stride=m.cm.max_stride, peak_threshold=self.peak_threshold,
             refinement="integral" if self.integral_refinement else "local", integral_patch_size=self.integral_patch_size,
             cm_output_stride=m.cm.head_strides["MultiInstanceConfmapsHead"],
-            class_maps_output_stride=m.cm.head_strides["ClassMapsHead"]))
+            class_maps_output_stride=m.cm.head_strides["ClassMapsHead"], max_peaks_per_sample=self._caps[0],
+            max_node_peaks=self._caps[1]))
 
     @classmethod
     def from_trained_models(cls, model_path, batch_size=4, peak_threshold=0.2, integral_refinement=True, integral_patch_size=5,
-                            resize_input_layer=True, precision=PRECISION_FP16, handle=None, **_):
-        """:3699-3745."""
+                            resize_input_layer=True, precision=PRECISION_FP16, handle=None, max_peaks_per_sample=1024,
+                            max_node_peaks=32, **_):
+        """:3699-3745.  ``max_peaks_per_sample`` / ``max_node_peaks`` size the device workspace (the reference's ragged
+        tensors are unbounded); a frame that reaches one is reported through ``on_overflow``."""
         _, spec, model = cls._load(model_path, precision, handle)
         return cls(model, spec["classes"], peak_threshold=peak_threshold, batch_size=batch_size,
-                   integral_refinement=integral_refinement, integral_patch_size=integral_patch_size)
+                   integral_refinement=integral_refinement, integral_patch_size=integral_patch_size,
+                   max_peaks_per_sample=max_peaks_per_sample, max_node_peaks=max_node_peaks)
 
     def _frames_from_example(self, ex):
         """:3781-3838."""

@@ -2,7 +2,8 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [--steps K] [--c5-batch B]   (C5 default: 16 frames per GPU and step)
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [--steps K] [--c5-batch B]
+  (C5 default: 16 frames per GPU and step)
 
 r50: ResNet50 bottom-up (ImageNet-preprocessed "frozen" weights, upsampling stack to stride 4 with k4 transposed convs,
 BN, two refine convs, concat skips), 1024x1024x1, flies13, B=8 per GPU; it also reports the fp16 maps against the fp32
@@ -17,6 +18,14 @@ The device tracker (track_device=0) against the host tracker: tracker only (run_
 for simple / instance / greedy and simplemaxtracks / centroid / hungarian on the clip predictions (300 frames) and on a
 seeded synthetic set of up to 6 instances x 13 nodes (300 frames); end to end, the same predict with no tracker, the
 host simple tracker and the device simple tracker (k_track inside the step).
+
+multiclass: the bottom-up multi-class (identity) predictor, three arms on the same frames, alternating in one process:
+the host chain composed from public calls (forward -> identity.class_probabilities -> find_local_peaks ->
+classify_peaks_from_maps), the fused step (predict_on_batch) and the pipelined submit/collect loop (predict).  Workloads:
+the trained fixture model (min_tracks_2node, 1024x1024 at input scale 0.5, 2 nodes, 2 classes) on 256 clip frames, and a
+C4-sized UNet with 13 nodes and 4 classes at stride 4 (synthetic weights, confidence head calibrated to ~5 detections
+per node as bench.py does), 1024x1024, B=8.  The line reports frames/s per arm and whether the arms agree (assignments
+identical, points, values and class probabilities bit for bit).
 """
 import json
 import os
@@ -267,6 +276,110 @@ def track_bench():
     return out
 
 
+def _mc_host_arm(layer, batch):
+    """The parent commit's host chain for one batch, from public calls."""
+    from sleap_b200.nn import identity, peak_finding
+    m = layer.keras_model
+    names = [layer.CMS, layer.CLASS_MAPS] + ([layer.OFFSETS] if layer.has_offsets else [])
+    outs = m.forward(batch, names)
+    probs = identity.class_probabilities(outs[1])
+    if layer.has_offsets:
+        pk, pv, si, ci = peak_finding.find_local_peaks_with_offsets(outs[0], outs[2], threshold=layer.peak_threshold, handle=m.handle)
+    else:
+        pk, pv, si, ci = peak_finding.find_local_peaks(outs[0], threshold=layer.peak_threshold, refinement=layer.refinement,
+                                                       integral_patch_size=layer.integral_patch_size, handle=m.handle)
+    cs = np.float32(layer.class_maps_output_stride)
+    pk = ((pk * np.float32(layer.cm_output_stride)).astype(np.float32) / cs).astype(np.float32)
+    pts, vals, cp = identity.classify_peaks_from_maps(probs, pk, pv, si, ci, n_channels=outs[0].shape[3])
+    pts = (pts * cs).astype(np.float32)
+    if layer.input_scale != 1.0:
+        pts = (pts / np.float32(layer.input_scale) + np.float32(0.5)).astype(np.float32)
+    return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": cp}
+
+
+def _mc_agree(a, b):
+    """Assignments identical (NaN pattern) and every value bit for bit."""
+    for k in ("instance_peaks", "instance_peak_vals", "instance_scores"):
+        x, y = np.asarray(a[k], np.float32), np.asarray(b[k], np.float32)
+        if x.shape != y.shape or not np.array_equal(np.isnan(x), np.isnan(y)):
+            return False
+        if not np.array_equal(x[~np.isnan(x)].view(np.uint32), y[~np.isnan(y)].view(np.uint32)):
+            return False
+    return True
+
+
+def _mc_workload(pred, fr, B, reps):
+    layer = pred.inference_model.inference_layer
+    im = pred.inference_model
+    arms = {
+        "host chain (forward, class_probabilities, find_local_peaks, classify_peaks_from_maps)":
+            lambda: _merge([_mc_host_arm(layer, fr[i:i + B]) for i in range(0, len(fr), B)]),
+        "fused predict_on_batch": lambda: _merge([im.predict_on_batch(fr[i:i + B]) for i in range(0, len(fr), B)]),
+        "fused predict (pipelined submit/collect loop)": lambda: im.predict(fr, batch_size=B),
+    }
+    outs = {k: f() for k, f in arms.items()}                             # warm-up, and the outputs compared
+    times = {k: [] for k in arms}
+    for _ in range(reps):                                                # arms alternate
+        for k, f in arms.items():
+            t0 = time.perf_counter()
+            f()
+            times[k].append(time.perf_counter() - t0)
+    names = list(arms)
+    res = {"frames": len(fr), "batch": B, "frames_per_s": {k: len(fr) / float(np.median(v)) for k, v in times.items()},
+           "frames_per_s_spread": {k: [len(fr) / max(v), len(fr) / min(v)] for k, v in times.items()},
+           "agree_fused_vs_host": _mc_agree(outs[names[1]], outs[names[0]]),
+           "agree_pipelined_vs_host": _mc_agree(outs[names[2]], outs[names[0]]),
+           "assigned_points_per_frame": float(np.isfinite(outs[names[1]]["instance_scores"]).sum() / len(fr))}
+    return res
+
+
+def _merge(chunks):
+    return {k: np.concatenate([c[k] for c in chunks]) for k in ("instance_peaks", "instance_peak_vals", "instance_scores")}
+
+
+def multiclass_bench(steps):
+    import torch
+    import bench
+    from sleap_b200.nn.inference import BottomUpMultiClassPredictor, Predictor
+    tests = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests")
+    sys.path.insert(0, tests)
+    from flow_clip import clip_frames
+    reps = max(3, steps // 2)
+    out = {"config": "multiclass: bottom-up identity predictor, host chain vs fused step vs pipelined loop", "gpu": gpu_identity(),
+           "metric": "frames/s (median of alternating repetitions; host frames in, results on the host)", "repetitions": reps}
+    clip = torch.from_numpy(np.ascontiguousarray(clip_frames(256))).pin_memory().numpy()
+    fx = os.path.join(tests, "golden", "models", "min_tracks_2node.bottomup_multiclass", "fixture_config.json")
+    pred = Predictor.from_model_paths([fx], batch_size=8)
+    out["fixture min_tracks_2node (1024x1024 at scale 0.5, 2 nodes, 2 classes, maps at stride 2), 256 clip frames"] = \
+        _mc_workload(pred, clip, 8, reps)
+    # C4-sized identity network: the C4 UNet, 13 confidence maps and 4 class maps at stride 4
+    spec = dict(backbone="unet", backbone_cfg=dict(bench.UNET_CFG), head_type="multi_class_bottomup",
+                heads=[dict(name="MultiInstanceConfmapsHead", channels=13, output_stride=4),
+                       dict(name="ClassMapsHead", channels=4, output_stride=4, activation="sigmoid")],
+                part_names=bench.NODES, edges=None, classes=["c0", "c1", "c2", "c3"])
+    cm = A.compile_model(spec, 1)
+    w = A.make_synthetic_weights(cm, bench.SEED)
+    fr = frames(8, 1024, 1024, 1, 11)
+    m0 = DeviceModel(spec, w, input_channels=1, precision=0)
+    cms = m0.forward(fr[:2], ["MultiInstanceConfmapsHead"])[0]
+    del m0
+    k = np.asarray(w["MultiInstanceConfmapsHead"]["kernel"]).copy()
+    b = np.asarray(w["MultiInstanceConfmapsHead"]["bias"]).copy()
+    for c in range(cms.shape[-1]):                                       # bench.calibrate_heads on the confidence head
+        vals = np.sort(np.concatenate([bench.local_max_values(cms[i, :, :, c]) for i in range(cms.shape[0])]))[::-1]
+        kth = min(len(vals) - 1, bench.TARGET_PEAKS_PER_CHANNEL * cms.shape[0])
+        t, top = float(vals[kth]), float(vals[0])
+        g = 0.8 / max(top - t, 1e-6)
+        k[..., c] *= g
+        b[c] = (b[c] - t) * g + 0.2
+    w["MultiInstanceConfmapsHead"] = dict(kernel=k, bias=b)
+    model = DeviceModel(spec, w, input_channels=1, precision=0)
+    pred = BottomUpMultiClassPredictor(model, spec["classes"], peak_threshold=0.2, batch_size=8)
+    out["C4-sized UNet (13 nodes, 4 classes at stride 4, synthetic weights), 1024x1024, B=8"] = \
+        _mc_workload(pred, np.concatenate([fr] * 4), 8, reps)
+    return out
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -281,6 +394,8 @@ if __name__ == "__main__":
             r = resnet50(steps)
         elif c == "track":
             r = track_bench()
+        elif c == "multiclass":
+            r = multiclass_bench(steps)
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
