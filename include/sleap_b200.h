@@ -252,8 +252,11 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* params, const
  * -> * cm_output_stride -> class probability at each peak (sigmoid of the class-map logit at the rounded class-map cell,
  * 0 outside the map) -> per (frame, node) SciPy assignment of peaks to classes on -probability, a match kept only where
  * it is the peak's most probable class -> (/input_scale + 0.5).  One record per frame comes back.
- * A model runs one post-processing chain at a time: sb_multiclass_configure drops the plain bottom-up chain (with its
- * tracker and record exchange) and sb_bottomup_configure drops this one. */
+ * A model runs one post-processing chain at a time (bottom-up, multi-class, global peaks or centroids): any of their
+ * configure calls drops the model's previous chain, with its tracker and record exchange, and so does
+ * sb_model_configure.  A call for another chain than the model's is refused.  A configure call refused for its
+ * arguments leaves the previous chain in place.  The fused top-down pipeline must be configured again
+ * (sb_topdown_configure) after either of its models is reconfigured. */
 #define SB_MAX_CLASSES 128
 typedef struct sb_multiclass_params {
   int32_t cms_buffer, class_maps_buffer, offsets_buffer; /* op-list buffer ids (offsets: -1 if none) */

@@ -65,11 +65,6 @@ __global__ void k_gather_ack(SbGatherDev g, unsigned long long step) {
 
 }  // namespace
 
-static SbModel* gmodel(sb_handle_s* h, int id) {
-  if (!h || id < 0 || id >= (int)h->models.size()) return nullptr;
-  return h->models[id];
-}
-
 static size_t win_data_bytes(const SbGather& g) { return (size_t)g.G * g.world * g.Bmax * g.width * sizeof(float); }
 static size_t win_bytes(const SbGather& g) {
   return win_data_bytes(g) + ((size_t)g.G * g.world + g.world) * sizeof(unsigned long long) + 64;
@@ -122,8 +117,8 @@ int sb_gather_queue_collect(sb_handle_s* h, SbModel* m, long long step, int B, f
 extern "C" {
 
 int sb_gather_init(sb_handle_t h, int model_id, int rank, int world, int generations, void* out_ipc_handle) {
-  SbModel* m = gmodel(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "sb_gather_init: bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_gather_init: bottom-up predictor not configured");
+  if (!m) return SB_ERR_INVALID;
   if (world < 1 || world > SB_GATHER_MAX_WORLD || rank < 0 || rank >= world || generations < 2 || generations > 64 || !out_ipc_handle)
     return sb_fail(h, SB_ERR_INVALID, "sb_gather_init: bad arguments (world <= %d, 2 <= generations <= 64)", SB_GATHER_MAX_WORLD);
   if (m->B > 255) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_gather_init: more than 255 frames per rank and step");
@@ -151,7 +146,7 @@ int sb_gather_init(sb_handle_t h, int model_id, int rank, int world, int generat
 }
 
 int sb_gather_connect(sb_handle_t h, int model_id, const void* all_ipc_handles) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m || !m->gather.local || !all_ipc_handles) return sb_fail(h, SB_ERR_INVALID, "sb_gather_connect: call sb_gather_init first");
   SB_CUDA(h, cudaSetDevice(h->device));
   SbGather& g = m->gather;
@@ -173,7 +168,7 @@ int sb_gather_connect(sb_handle_t h, int model_id, const void* all_ipc_handles) 
 }
 
 int sb_gather_enabled(sb_handle_t h, int model_id) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   return (m && m->gather.connected) ? 1 : 0;
 }
 
@@ -181,7 +176,7 @@ int sb_gather_enabled(sb_handle_t h, int model_id) {
 // for all ranks' records of that step (bounded), then acknowledges the generation.  The window of the step stays
 // readable by later work on that stream until `generations` more steps have been pushed by every rank.
 int sb_gather_consume_dev(sb_handle_t h, int model_id, int64_t step) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m || !m->gather.connected) return sb_fail(h, SB_ERR_INVALID, "sb_gather_consume_dev: exchange not connected");
   if (step < 0) step = m->gather.consumed;        // next unconsumed step
   if (step >= m->gather.step) return sb_fail(h, SB_ERR_INVALID, "sb_gather_consume_dev: step %lld was not pushed", (long long)step);
@@ -193,7 +188,7 @@ int sb_gather_consume_dev(sb_handle_t h, int model_id, int64_t step) {
 }
 
 int sb_gather_window(sb_handle_t h, int model_id, int64_t step, float** out_dev_ptr, int64_t* out_floats) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m || !m->gather.local || !out_dev_ptr) return sb_fail(h, SB_ERR_INVALID, "sb_gather_window: exchange not initialised");
   const SbGather& g = m->gather;
   *out_dev_ptr = (float*)g.local + (size_t)(step % g.G) * g.world * g.Bmax * g.width;
@@ -204,7 +199,7 @@ int sb_gather_window(sb_handle_t h, int model_id, int64_t step, float** out_dev_
 // Host consumer: blocks until the records of `step` from every rank are in out_records_host
 // ([world][B][width] float32, rank-major = frame order for contiguous shards); out_counts[r] = frames rank r pushed.
 int sb_gather_collect(sb_handle_t h, int model_id, int64_t step, int B, float* out_records_host, int32_t* out_counts) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m || !m->gather.connected || !out_records_host) return sb_fail(h, SB_ERR_INVALID, "sb_gather_collect: exchange not connected");
   SbGather& g = m->gather;
   if (step < 0 || step >= g.step) return sb_fail(h, SB_ERR_INVALID, "sb_gather_collect: step %lld was not pushed", (long long)step);
@@ -225,7 +220,7 @@ int sb_gather_collect(sb_handle_t h, int model_id, int64_t step, int B, float* o
 }
 
 int sb_gather_status(sb_handle_t h, int model_id, int32_t* out_status, int64_t* out_steps_pushed, int64_t* out_steps_consumed) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m || !m->gather.local) return sb_fail(h, SB_ERR_INVALID, "sb_gather_status: exchange not initialised");
   if (out_status) *out_status = *m->gather.status_host;
   if (out_steps_pushed) *out_steps_pushed = m->gather.step;
@@ -234,7 +229,7 @@ int sb_gather_status(sb_handle_t h, int model_id, int32_t* out_status, int64_t* 
 }
 
 int sb_gather_close(sb_handle_t h, int model_id) {
-  SbModel* m = gmodel(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
   if (!m) return sb_fail(h, SB_ERR_INVALID, "bad model id");
   SB_CUDA(h, cudaSetDevice(h->device));
   SB_CUDA(h, cudaDeviceSynchronize());

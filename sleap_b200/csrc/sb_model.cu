@@ -26,6 +26,11 @@ int grid_for(size_t total, int sm) {
 
 int build_programs(sb_handle_s* h, SbModel* m);   // the last step of sb_model_configure (below, with the op slots)
 
+void global_scratch_free(SbGlobalScratch& g) {
+  for (float* p : {g.part, g.points, g.vals, g.crop_off}) if (p) cudaFree(p);
+  g = SbGlobalScratch();
+}
+
 }  // namespace
 
 void sb_models_free(sb_handle_s* h) {
@@ -35,10 +40,7 @@ void sb_models_free(sb_handle_s* h) {
     if (m->weights_dev) cudaFree(m->weights_dev);
     if (m->weights_tc_dev) cudaFree(m->weights_tc_dev);
     if (m->frames_dev) cudaFree(m->frames_dev);
-    if (m->crop_off_dev) cudaFree(m->crop_off_dev);
-    if (m->gpart) cudaFree(m->gpart);
-    if (m->gpoints) cudaFree(m->gpoints);
-    if (m->gvals) cudaFree(m->gvals);
+    global_scratch_free(m->gs);
     if (m->rec_host) cudaFreeHost(m->rec_host);
     if (m->trk_dev) cudaFree(m->trk_dev);
     for (int i = 0; i < 3; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
@@ -73,9 +75,35 @@ void sb_pipeline_slots_free(SbModel* m) {
   if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
 }
 
-static SbModel* get_model(sb_handle_s* h, int id) {
-  if (!h || id < 0 || id >= (int)h->models.size()) return nullptr;
-  return h->models[id];
+SbModel* chain_model(sb_handle_s* h, int id, int kind, const char* what) {
+  SbModel* m = (h && id >= 0 && id < (int)h->models.size()) ? h->models[id] : nullptr;
+  if (m && (kind == SB_CHAIN_ANY || m->chain == kind)) return m;
+  sb_fail(h, SB_ERR_INVALID, "%s", what);
+  return nullptr;
+}
+
+// Releases the model's post-processing chain and everything sized or attached for it; the only code that does.  The
+// device is drained first: post-processing and result copies of earlier steps may still read the workspace.
+static int chain_drop(sb_handle_s* h, SbModel* m) {
+  SB_CUDA(h, cudaDeviceSynchronize());
+  h->post_pending = false;
+  sb_post_ws_free(m->ws);
+  sb_pipeline_slots_free(m);                     // staging is sized from the chain's record width
+  sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes)
+  m->trk = nullptr;                              // its checks (nodes, instance capacity) were made against the old chain
+  global_scratch_free(m->gs);
+  sb_topdown_free(m);
+  m->chain = SB_CHAIN_NONE;
+  ++m->chain_gen;
+  return 0;
+}
+
+// The model a per-model configure call sets up: a valid id, non-null params and a configured network
+static SbModel* configure_target(sb_handle_s* h, int id, const void* p) {
+  SbModel* m = chain_model(h, id, SB_CHAIN_ANY, "bad model id / params");
+  if (!m || !p) { sb_fail(h, SB_ERR_INVALID, "bad model id / params"); return nullptr; }
+  if (!m->configured) { sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first"); return nullptr; }
+  return m;
 }
 
 extern "C" {
@@ -143,8 +171,8 @@ int sb_load_model(sb_handle_t h, const int32_t* ops, int n_ops, const float* wei
 }
 
 int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W, int C_in) {
-  SbModel* m = get_model(h, model_id);
-  if (!m) return sb_fail(h, SB_ERR_INVALID, "bad model id");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
+  if (!m) return SB_ERR_INVALID;
   if (max_batch <= 0 || H <= 0 || W <= 0 || (C_in != 1 && C_in != 3)) return sb_fail(h, SB_ERR_INVALID, "sb_model_configure: bad shape");
   SB_CUDA(h, cudaSetDevice(h->device));
   // preprocess op defines the net input size
@@ -161,17 +189,12 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
     if (Hnet % b.stride_den || Wnet % b.stride_den)
       return sb_fail(h, SB_ERR_INVALID, "net input %dx%d not divisible by stride %d (pad_to_stride too small)", Hnet, Wnet, b.stride_den);
   }
-  // a reconfigure invalidates everything sized from the old shape: drain the device first, then drop the
-  // activation buffers, the double-buffer pipeline slots and the predictor workspaces (their configure
-  // calls must be repeated; the C-ABI refuses to run a predictor on a stale workspace)
-  SB_CUDA(h, cudaDeviceSynchronize());
-  h->post_pending = false;
+  // a reconfigure invalidates everything sized from the old shape: the post-processing chain (its configure call must be
+  // repeated; the C-ABI refuses to run a chain the model does not have), then the activation buffers and the plans
+  if (const int rc = chain_drop(h, m)) return rc;
   for (auto& b : m->buffers) { if (b.dev) { cudaFree(b.dev); b.dev = nullptr; } }
   if (m->frames_dev) { cudaFree(m->frames_dev); m->frames_dev = nullptr; }
-  sb_pipeline_slots_free(m);
-  sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes): re-init after a reconfigure
   m->configured = false;
-  m->bu_configured = false; m->mc_configured = false; m->gl_configured = false; m->ce_configured = false; m->td_configured = false;
   for (auto& p : m->prog) p.clear();             // the programs refer to the plans
   sb_entry_release(m);
   sb_conv_tc_release(m);
@@ -422,8 +445,8 @@ extern "C" {
 
 int sb_model_forward(sb_handle_t h, int model_id, const void* images_host, int images_are_u8, int B,
                      int n_outputs, const int32_t* output_buffer_ids, float** out_host_ptrs) {
-  SbModel* m = get_model(h, model_id);
-  if (!m) return sb_fail(h, SB_ERR_INVALID, "bad model id");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "model not configured");
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
@@ -462,7 +485,7 @@ int sb_model_forward(sb_handle_t h, int model_id, const void* images_host, int i
 // 0 other, 1 tensor-core conv, 2 CUDA-core conv; out_flops[i] = 2*MACs of the op for batch B.
 int sb_model_profile_ops(sb_handle_t h, int model_id, const uint8_t* frames_dev, int B, int cap, float* out_ms,
                          int32_t* out_kind, double* out_flops, int32_t* out_n_ops) {
-  SbModel* m = get_model(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "model not configured");
   if (!m || !m->configured) return sb_fail(h, SB_ERR_INVALID, "model not configured");
   SB_CUDA(h, cudaSetDevice(h->device));
   const int n = (int)m->ops.size();
@@ -489,8 +512,8 @@ int sb_model_profile_ops(sb_handle_t h, int model_id, const uint8_t* frames_dev,
 }
 
 int sb_model_forward_times(sb_handle_t h, int model_id, int enable, int cap, float* out_ms, int32_t* out_n) {
-  SbModel* m = get_model(h, model_id);
-  if (!m) return sb_fail(h, SB_ERR_INVALID, "bad model id");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_ANY, "bad model id");
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
   int n = 0;
@@ -525,38 +548,60 @@ static int post_guard_op(const SbModel* m, int b0, int b1, int b2) {
 }
 
 static size_t record_width(const SbModel* m) {
-  return m->mc_configured ? sb_class_record_width(m->mc.n_classes, m->mc.n_nodes) : sb_record_width(m->bu.max_instances, m->bu.n_nodes);
+  return m->chain == SB_CHAIN_CLASS ? sb_class_record_width(m->mc.n_classes, m->mc.n_nodes) : sb_record_width(m->bu.max_instances, m->bu.n_nodes);
+}
+
+// One map a chain reads: device pointer and NHWC shape (a head buffer, or a from-maps call's upload)
+struct SbMap {
+  const float* dev;
+  int H, W, C;
+};
+static SbMap head_map(const SbModel* m, int buf) {
+  const SbBuffer& b = m->buffers[buf];
+  return {(const float*)b.dev, b.H, b.W, b.C};
+}
+static const float* head_offsets(const SbModel* m, int buf) { return buf >= 0 ? (const float*)m->buffers[buf].dev : nullptr; }
+
+// A head buffer id a configure call names: in range, an f32 head output of C channels
+static bool f32_head(const SbModel* m, int buf, int C) {
+  return buf >= 0 && buf < (int)m->buffers.size() && m->buffers[buf].f32 && m->buffers[buf].C == C;
+}
+
+// The PAF chain's parameters, checked by sb_bottomup_configure and sb_bottomup_from_maps alike (not the buffer ids)
+static int check_paf_params(sb_handle_s* h, const sb_bottomup_params* p) {
+  if (p->n_nodes <= 0 || p->n_edges <= 0 || !p->edges) return sb_fail(h, SB_ERR_INVALID, "bad skeleton");
+  if (p->n_sorted > p->n_edges || p->max_peaks_per_sample <= 0 || p->max_node_peaks <= 0 || p->max_instances <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "bad capacities");
+  for (int e = 0; e < 2 * p->n_edges; ++e)
+    if (p->edges[e] < 0 || p->edges[e] >= p->n_nodes) return sb_fail(h, SB_ERR_INVALID, "edge node index out of range");
+  return 0;
+}
+
+// The multi-class chain's parameters, checked by sb_multiclass_configure and sb_multiclass_from_maps alike
+static int check_class_params(sb_handle_s* h, const sb_multiclass_params* p) {
+  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES)
+    return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
+  if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
+      p->max_node_peaks <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "bad strides / input scale / capacities");
+  return 0;
 }
 
 extern "C" {
 
 int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params* p) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
-  if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first");
+  SbModel* m = configure_target(h, model_id, p);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
-  const int nb = (int)m->buffers.size();
-  if (p->cms_buffer < 0 || p->cms_buffer >= nb || p->pafs_buffer < 0 || p->pafs_buffer >= nb)
-    return sb_fail(h, SB_ERR_INVALID, "cms/pafs buffer ids out of range");
-  SbBuffer& cb = m->buffers[p->cms_buffer];
-  SbBuffer& pb = m->buffers[p->pafs_buffer];
-  if (!cb.f32 || !pb.f32) return sb_fail(h, SB_ERR_INVALID, "cms / pafs buffers must be f32 head outputs");
-  if (cb.C != p->n_nodes || pb.C != 2 * p->n_edges) return sb_fail(h, SB_ERR_INVALID, "head channels do not match skeleton");
-  if (p->offsets_buffer >= 0 && (p->offsets_buffer >= nb || !m->buffers[p->offsets_buffer].f32 || m->buffers[p->offsets_buffer].C != 2 * p->n_nodes))
-    return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
-  if (p->n_sorted > p->n_edges || p->max_peaks_per_sample <= 0 || p->max_node_peaks <= 0 || p->max_instances <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "bad capacities");
-  for (int e = 0; e < 2 * p->n_edges; ++e)
-    if (p->edges[e] < 0 || p->edges[e] >= p->n_nodes) return sb_fail(h, SB_ERR_INVALID, "edge node index out of range");
-  SB_CUDA(h, cudaDeviceSynchronize());          // in-flight post-processing / result copies still use the old workspace
-  h->post_pending = false;
-  m->bu_configured = false;
-  m->mc_configured = false;
-  sb_pipeline_slots_free(m);                      // staging records are sized from max_instances / n_nodes
-  sb_gather_free(m);
-  sb_post_ws_free(m->ws);
-  int rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges);
+  if (int rc = check_paf_params(h, p)) return rc;
+  if (!f32_head(m, p->cms_buffer, p->n_nodes) || !f32_head(m, p->pafs_buffer, 2 * p->n_edges))
+    return sb_fail(h, SB_ERR_INVALID, "cms / pafs buffers must be f32 head outputs of n_nodes / 2 * n_edges channels");
+  if (p->offsets_buffer >= 0 && !f32_head(m, p->offsets_buffer, 2 * p->n_nodes)) return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
+  int rc = chain_drop(h, m);
   if (rc) return rc;
+  const SbBuffer& cb = m->buffers[p->cms_buffer];
+  if ((rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges)))
+    return rc;
   SB_CUDA(h, cudaMemcpy(m->ws.edges_dev, p->edges, (size_t)p->n_edges * 2 * sizeof(int), cudaMemcpyHostToDevice));
   if (p->n_sorted > 0)
     SB_CUDA(h, cudaMemcpy(m->ws.sorted_edges_dev, p->sorted_edge_inds, (size_t)p->n_sorted * sizeof(int), cudaMemcpyHostToDevice));
@@ -565,46 +610,29 @@ int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params*
   m->bu.edges = nullptr; m->bu.sorted_edge_inds = nullptr;
   m->bu_edges.assign(p->edges, p->edges + 2 * p->n_edges);
   m->guard_op = post_guard_op(m, p->cms_buffer, p->pafs_buffer, p->offsets_buffer);
-  m->bu_configured = true;
+  m->chain = SB_CHAIN_PAF;
   return SB_OK;
 }
 
 int sb_multiclass_configure(sb_handle_t h, int model_id, const sb_multiclass_params* p) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
-  if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first");
+  SbModel* m = configure_target(h, model_id, p);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
-  const int nb = (int)m->buffers.size();
-  if (p->cms_buffer < 0 || p->cms_buffer >= nb || p->class_maps_buffer < 0 || p->class_maps_buffer >= nb)
-    return sb_fail(h, SB_ERR_INVALID, "cms / class-map buffer ids out of range");
-  SbBuffer& cb = m->buffers[p->cms_buffer];
-  SbBuffer& kb = m->buffers[p->class_maps_buffer];
-  if (!cb.f32 || !kb.f32) return sb_fail(h, SB_ERR_INVALID, "cms / class-map buffers must be f32 head outputs");
-  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES)
-    return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
-  if (cb.C != p->n_nodes || kb.C != p->n_classes) return sb_fail(h, SB_ERR_INVALID, "head channels do not match nodes / classes");
-  if (p->offsets_buffer >= 0 && (p->offsets_buffer >= nb || !m->buffers[p->offsets_buffer].f32 || m->buffers[p->offsets_buffer].C != 2 * p->n_nodes))
-    return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
-  if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
-      p->max_node_peaks <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "bad strides / input scale / capacities");
-  SB_CUDA(h, cudaDeviceSynchronize());          // in-flight post-processing / result copies still use the old workspace
-  h->post_pending = false;
-  m->bu_configured = false;
-  m->mc_configured = false;
-  m->trk = nullptr;                               // the tracker and the record exchange belong to the PAF chain
-  sb_pipeline_slots_free(m);
-  sb_gather_free(m);
-  sb_post_ws_free(m->ws);
-  int rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0);
+  if (int rc = check_class_params(h, p)) return rc;
+  if (!f32_head(m, p->cms_buffer, p->n_nodes) || !f32_head(m, p->class_maps_buffer, p->n_classes))
+    return sb_fail(h, SB_ERR_INVALID, "cms / class-map buffers must be f32 head outputs of n_nodes / n_classes channels");
+  if (p->offsets_buffer >= 0 && !f32_head(m, p->offsets_buffer, 2 * p->n_nodes)) return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
+  int rc = chain_drop(h, m);
   if (rc) return rc;
+  const SbBuffer& cb = m->buffers[p->cms_buffer];
+  if ((rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0))) return rc;
   m->ws.node_lists = true;
   const size_t nrec = (size_t)m->B * sb_class_record_width(p->n_classes, p->n_nodes);
   if ((rc = sb_dev_alloc(h, &m->ws.records, nrec))) return rc;
   m->ws.bytes += nrec * sizeof(float);
   m->mc = *p;
   m->guard_op = post_guard_op(m, p->cms_buffer, p->class_maps_buffer, p->offsets_buffer);
-  m->mc_configured = true;
+  m->chain = SB_CHAIN_CLASS;
   return SB_OK;
 }
 
@@ -646,40 +674,50 @@ static void unpack_records(const SbModel* m, const float* rec, int B, float* out
   }
 }
 
-static int bottomup_post_kernels(sb_handle_s* h, SbModel* m, int B) {
-  const sb_bottomup_params& p = m->bu;
-  SbBuffer& cb = m->buffers[p.cms_buffer];
-  SbBuffer& pb = m->buffers[p.pafs_buffer];
-  const float* off = p.offsets_buffer >= 0 ? (const float*)m->buffers[p.offsets_buffer].dev : nullptr;
+// The PAF chain: local peaks, PAF scoring and matching, grouping into ws's instance arrays and records (and, gx given,
+// every peer's gather window).
+static int bottomup_post_kernels(sb_handle_s* h, const sb_bottomup_params& p, SbPostWs& ws, const SbMap& cms, const SbMap& pafs,
+                                 const float* off, int B, const SbGatherDev* gx = nullptr) {
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
-  int rc = sbk_local_peaks(h, cb.dev, 0, off, B, cb.H, cb.W, cb.C, pp, m->ws);
+  int rc = sbk_local_peaks(h, cms.dev, 0, off, B, cms.H, cms.W, cms.C, pp, ws);
   if (rc) return rc;
-  const float max_len = p.max_edge_length_ratio * (float)std::max(std::max(pb.H, pb.W), pb.C) * (float)p.paf_output_stride;
-  if ((rc = sbk_score_match(h, (const float*)pb.dev, B, pb.H, pb.W, pb.C, p.n_line_points, p.paf_output_stride, max_len,
-                            p.dist_penalty_weight, m->ws))) return rc;
-  if (m->gather.connected) {               // fused exchange: k_group's epilogue pushes the records to every peer
+  const float max_len = p.max_edge_length_ratio * (float)std::max(std::max(pafs.H, pafs.W), pafs.C) * (float)p.paf_output_stride;
+  if ((rc = sbk_score_match(h, pafs.dev, B, pafs.H, pafs.W, pafs.C, p.n_line_points, p.paf_output_stride, max_len,
+                            p.dist_penalty_weight, ws))) return rc;
+  return sbk_group(h, B, p.n_nodes, p.min_instance_peaks, p.min_line_scores, p.input_scale, ws, gx);
+}
+
+// The multi-class chain: local peaks with their per-node lists, then the identity grouping into the records.
+static int multiclass_post_kernels(sb_handle_s* h, const sb_multiclass_params& p, SbPostWs& ws, const SbMap& cms,
+                                   const SbMap& cls, const float* off, int B) {
+  SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
+  int rc = sbk_local_peaks(h, cms.dev, 0, off, B, cms.H, cms.W, cms.C, pp, ws);
+  if (rc) return rc;
+  return sbk_class_group(h, cls.dev, B, cls.H, cls.W, cls.C, (float)p.class_maps_output_stride, p.input_scale, ws);
+}
+
+// The step's chain on the head buffers: the multi-class one, or the PAF one with the record exchange pushed from k_group's
+// epilogue when connected, else the attached tracker after it.
+static int step_post_kernels(sb_handle_s* h, SbModel* m, int B) {
+  if (m->chain == SB_CHAIN_CLASS) {
+    const sb_multiclass_params& p = m->mc;
+    return multiclass_post_kernels(h, p, m->ws, head_map(m, p.cms_buffer), head_map(m, p.class_maps_buffer),
+                                   head_offsets(m, p.offsets_buffer), B);
+  }
+  const sb_bottomup_params& p = m->bu;
+  const SbMap cms = head_map(m, p.cms_buffer), pafs = head_map(m, p.pafs_buffer);
+  const float* off = head_offsets(m, p.offsets_buffer);
+  if (m->gather.connected) {
     const SbGatherDev gx = sb_gather_dev(m, (unsigned long long)m->gather.step);
-    rc = sbk_group(h, B, p.n_nodes, p.min_instance_peaks, p.min_line_scores, p.input_scale, m->ws, &gx);
+    const int rc = bottomup_post_kernels(h, p, m->ws, cms, pafs, off, B, &gx);
     if (!rc) m->gather.step++;
     return rc;
   }
-  if ((rc = sbk_group(h, B, p.n_nodes, p.min_instance_peaks, p.min_line_scores, p.input_scale, m->ws))) return rc;
+  if (const int rc = bottomup_post_kernels(h, p, m->ws, cms, pafs, off, B)) return rc;
   if (!m->trk) return 0;
   if (B > m->trk_B) return sb_fail(h, SB_ERR_INVALID, "attached tracker was sized for %d frames per step, not %d", m->trk_B, B);
   return sbk_track_step(h, m->trk, B, m->ws.inst_peaks, m->ws.inst_vals, m->ws.inst_scores, m->ws.n_inst, p.max_instances,
                         m->trk_cut, m->trk_h, m->trk_w, m->trk_dev);
-}
-
-// The multi-class chain: local peaks with their per-node lists, then the identity grouping into the records.
-static int multiclass_post_kernels(sb_handle_s* h, SbModel* m, int B) {
-  const sb_multiclass_params& p = m->mc;
-  SbBuffer& cb = m->buffers[p.cms_buffer];
-  SbBuffer& kb = m->buffers[p.class_maps_buffer];
-  const float* off = p.offsets_buffer >= 0 ? (const float*)m->buffers[p.offsets_buffer].dev : nullptr;
-  SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
-  int rc = sbk_local_peaks(h, cb.dev, 0, off, B, cb.H, cb.W, cb.C, pp, m->ws);
-  if (rc) return rc;
-  return sbk_class_group(h, (const float*)kb.dev, B, kb.H, kb.W, kb.C, (float)p.class_maps_output_stride, p.input_scale, m->ws);
 }
 
 static void unpack_class_records(const float* rec, size_t w, int B, int n_classes, int n_nodes, float* out_points,
@@ -713,7 +751,7 @@ static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
   SB_CUDA(h, cudaEventRecord(h->fwd_done_ev, main_stream));
   SB_CUDA(h, cudaStreamWaitEvent(h->post_stream, h->fwd_done_ev, 0));
   h->stream = h->post_stream;
-  int rc = m->mc_configured ? multiclass_post_kernels(h, m, B) : bottomup_post_kernels(h, m, B);
+  int rc = step_post_kernels(h, m, B);
   cudaError_t e = cudaEventRecord(h->post_done_ev, h->post_stream);
   h->stream = main_stream;
   if (rc) return rc;
@@ -723,9 +761,12 @@ static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
   return 0;
 }
 
+static const char* const kNoPaf = "bottom-up predictor not configured";
+static const char* const kNoClass = "multi-class predictor not configured";
+
 int sb_infer_bottomup_dev(sb_handle_t h, int model_id, const uint8_t* frames_dev, int B) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   int rc = sb_run_ops(h, m, frames_dev, 1, B);
   if (rc) return rc;
@@ -753,8 +794,8 @@ static int step_sync(sb_handle_s* h, SbModel* m, const void* frames_host, int fr
 int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, float* out_instance_peaks,
                       float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
                       int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   if (const int rc = step_sync(h, m, frames_host, 1, B)) return rc;
   unpack_records(m, own_slice(m, m->rec_host, B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
   return SB_OK;
@@ -762,8 +803,8 @@ int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, i
 
 int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B, float* out_points,
                         float* out_vals, float* out_class_probs, int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
+  if (!m) return SB_ERR_INVALID;
   if (!frames_host || !out_points || !out_vals || !out_class_probs) return sb_fail(h, SB_ERR_INVALID, "sb_infer_multiclass: null argument");
   if (const int rc = step_sync(h, m, frames_host, frames_are_u8 ? 1 : 0, B)) return rc;
   unpack_class_records(m->rec_host, record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals, out_class_probs, out_flags);
@@ -773,8 +814,8 @@ int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, in
 // Makes the handle's main stream wait (on the device, no host sync) for the post-processing of the
 // last sb_infer_bottomup_dev call, e.g. before recording an end-of-work event or reading the results.
 int sb_bottomup_wait_results(sb_handle_t h, int model_id) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   if (h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(h->stream, h->post_done_ev, 0));
   return SB_OK;
 }
@@ -833,31 +874,29 @@ static int step_collect(sb_handle_s* h, SbModel* m, int slot, int B) {
 }
 
 int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
-  return step_submit(h, m, frames_host, B, slot);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
 }
 
 int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out_instance_peaks,
                         float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
                         int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   if (const int rc = step_collect(h, m, slot, B)) return rc;
   unpack_records(m, own_slice(m, m->stage_host[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
   return SB_OK;
 }
 
 int sb_multiclass_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
-  return step_submit(h, m, frames_host, B, slot);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
+  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
 }
 
 int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals,
                           float* out_class_probs, int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->mc_configured) return sb_fail(h, SB_ERR_INVALID, "multi-class predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
+  if (!m) return SB_ERR_INVALID;
   if (const int rc = step_collect(h, m, slot, B)) return rc;
   unpack_class_records(m->stage_host[slot], record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals,
                        out_class_probs, out_flags);
@@ -865,8 +904,8 @@ int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* o
 }
 
 int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* out_records, int32_t* out_counts) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured || !m->gather.connected) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: exchange not connected");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_gathered: exchange not connected");
+  if (!m || !m->gather.connected) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: exchange not connected");
   if (slot < -1 || slot > 1 || !out_records) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: bad slot");
   const float* src = slot < 0 ? m->rec_host : m->stage_host[slot];
   const int have = slot < 0 ? m->rec_B : m->slot_B[slot];
@@ -879,8 +918,8 @@ int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* ou
 
 int sb_bottomup_device_outputs(sb_handle_t h, int model_id, float** instance_peaks_dev, float** instance_peak_vals_dev,
                                float** instance_scores_dev, int32_t** n_valid_dev, int32_t** flags_dev) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   if (instance_peaks_dev) *instance_peaks_dev = m->ws.inst_peaks;
   if (instance_peak_vals_dev) *instance_peak_vals_dev = m->ws.inst_vals;
   if (instance_scores_dev) *instance_scores_dev = m->ws.inst_scores;
@@ -890,8 +929,8 @@ int sb_bottomup_device_outputs(sb_handle_t h, int model_id, float** instance_pea
 }
 
 int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int max_instances, double img_h, double img_w) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (h->post_pending) SB_CUDA(h, cudaStreamSynchronize(h->post_stream));
   if (tracker_id < 0) { m->trk = nullptr; return SB_OK; }
@@ -919,7 +958,7 @@ int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int 
 }
 
 int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks) {
-  SbModel* m = get_model(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_tracks: no tracker attached");
   if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: no tracker attached");
   if (slot < -1 || slot > 1 || B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: bad slot / batch");
   if (slot >= 0) SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
@@ -928,7 +967,7 @@ int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out
 }
 
 int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tracks) {
-  SbModel* m = get_model(h, model_id);
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_device_tracks: no tracker attached");
   if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_device_tracks: no tracker attached");
   if (B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_device_tracks: bad batch");
   SB_CUDA(h, cudaSetDevice(h->device));
@@ -940,13 +979,13 @@ int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tr
 }
 
 int sb_bottomup_device_records(sb_handle_t h, int model_id, float** records_dev) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured || !records_dev) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m || !records_dev) return sb_fail(h, SB_ERR_INVALID, kNoPaf);
   *records_dev = m->ws.records;
   return SB_OK;
 }
 
-static int fetch_graph_ws(sb_handle_s* h, SbPostWs& ws, const int* edges_host, int B, int cap_peaks, float* peaks,
+static int fetch_graph_ws(sb_handle_s* h, const SbPostWs& ws, const int* edges_host, int B, int cap_peaks, float* peaks,
                           float* peak_vals, int32_t* peak_channel_inds, int32_t* peak_offsets, int cap_cands,
                           int32_t* edge_inds, int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets) {
   const int C = ws.C, K = ws.max_node_peaks, E = ws.n_edges, MP = ws.max_peaks;
@@ -991,12 +1030,34 @@ static int fetch_graph_ws(sb_handle_s* h, SbPostWs& ws, const int* edges_host, i
 int sb_bottomup_fetch_graph(sb_handle_t h, int model_id, int B, int cap_peaks, float* peaks, float* peak_vals,
                             int32_t* peak_channel_inds, int32_t* peak_offsets, int cap_cands, int32_t* edge_inds,
                             int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->bu_configured) return sb_fail(h, SB_ERR_INVALID, "bottom-up predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   return fetch_graph_ws(h, m->ws, m->bu_edges.data(), B, cap_peaks, peaks, peak_vals, peak_channel_inds, peak_offsets,
                         cap_cands, edge_inds, edge_peak_inds, line_scores, cand_offsets);
 }
+
+// The scratch of a *_from_maps call, freed when it returns: its workspace and device copies of the caller's maps.
+struct MapsScratch {
+  SbPostWs ws;
+  std::vector<void*> bufs;
+  ~MapsScratch() {
+    sb_post_ws_free(ws);
+    for (void* q : bufs) cudaFree(q);
+  }
+  // queues the upload of n floats from `host` on the handle's stream; host NULL (no such map): *dev = NULL
+  int upload(sb_handle_s* h, const float* host, size_t n, const float** dev) {
+    *dev = nullptr;
+    if (!host) return 0;
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, n * 4 + 16);
+    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc: %s", cudaGetErrorString(e));
+    bufs.push_back(q);
+    *dev = (const float*)q;
+    SB_CUDA(h, cudaMemcpyAsync(q, host, n * 4, cudaMemcpyHostToDevice, h->stream));
+    return 0;
+  }
+};
 
 int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const float* cms_host, int B, int H, int W,
                           const float* pafs_host, int Hp, int Wp, const float* offsets_host,
@@ -1005,38 +1066,26 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const floa
                           int32_t* peak_channel_inds, int32_t* peak_offsets, int cap_cands, int32_t* edge_inds,
                           int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "null handle / params");
-  if (B <= 0 || H <= 0 || W <= 0 || Hp <= 0 || Wp <= 0 || p->n_nodes <= 0 || p->n_edges <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_from_maps: bad shape");
+  if (!cms_host || !pafs_host || !out_instance_peaks || !out_instance_peak_vals || !out_instance_scores || !out_n_valid)
+    return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_from_maps: null argument");
+  if (B <= 0 || H <= 0 || W <= 0 || Hp <= 0 || Wp <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_from_maps: bad shape");
+  int rc = check_paf_params(h, p);
+  if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, C2 = 2 * p->n_edges;
-  SbPostWs ws;
-  struct Guard { SbPostWs& w; std::vector<void*> bufs; ~Guard() { sb_post_ws_free(w); for (void* q : bufs) cudaFree(q); } } guard{ws, {}};
-  int rc = sb_post_ws_alloc(h, ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges);
-  if (rc) return rc;
-  auto dalloc = [&](void** q, size_t bytes) -> int {
-    cudaError_t e = cudaMalloc(q, bytes + 16);
-    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc: %s", cudaGetErrorString(e));
-    guard.bufs.push_back(*q);
-    return 0;
-  };
-  void *d_cms = nullptr, *d_pafs = nullptr, *d_off = nullptr;
-  const size_t ncm = (size_t)B * H * W * C, npf = (size_t)B * Hp * Wp * C2;
-  if ((rc = dalloc(&d_cms, ncm * 4)) || (rc = dalloc(&d_pafs, npf * 4))) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(d_cms, cms_host, ncm * 4, cudaMemcpyHostToDevice, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(d_pafs, pafs_host, npf * 4, cudaMemcpyHostToDevice, h->stream));
-  if (offsets_host) {
-    if ((rc = dalloc(&d_off, 2 * ncm * 4))) return rc;
-    SB_CUDA(h, cudaMemcpyAsync(d_off, offsets_host, 2 * ncm * 4, cudaMemcpyHostToDevice, h->stream));
-  }
-  SB_CUDA(h, cudaMemcpyAsync(ws.edges_dev, p->edges, (size_t)p->n_edges * 8, cudaMemcpyHostToDevice, h->stream));
-  if (p->n_sorted > 0) SB_CUDA(h, cudaMemcpyAsync(ws.sorted_edges_dev, p->sorted_edge_inds, (size_t)p->n_sorted * 4, cudaMemcpyHostToDevice, h->stream));
-  ws.n_sorted = p->n_sorted;
-  SbPeakParams pp{p->peak_threshold, p->refinement, p->integral_patch_size, (float)p->cm_output_stride, 1.0f};
-  if ((rc = sbk_local_peaks(h, d_cms, 0, (const float*)d_off, B, H, W, C, pp, ws))) return rc;
-  const float max_len = p->max_edge_length_ratio * (float)std::max(std::max(Hp, Wp), C2) * (float)p->paf_output_stride;
-  if ((rc = sbk_score_match(h, (const float*)d_pafs, B, Hp, Wp, C2, p->n_line_points, p->paf_output_stride, max_len,
-                            p->dist_penalty_weight, ws))) return rc;
-  if ((rc = sbk_group(h, B, C, p->min_instance_peaks, p->min_line_scores, p->input_scale, ws))) return rc;
+  MapsScratch s;
+  if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges))) return rc;
+  SbMap cms{nullptr, H, W, C}, pafs{nullptr, Hp, Wp, C2};
+  const float* off = nullptr;
+  const size_t ncm = (size_t)B * H * W * C;
+  if ((rc = s.upload(h, cms_host, ncm, &cms.dev)) || (rc = s.upload(h, pafs_host, (size_t)B * Hp * Wp * C2, &pafs.dev)) ||
+      (rc = s.upload(h, offsets_host, 2 * ncm, &off)))
+    return rc;
+  SB_CUDA(h, cudaMemcpyAsync(s.ws.edges_dev, p->edges, (size_t)p->n_edges * 8, cudaMemcpyHostToDevice, h->stream));
+  if (p->n_sorted > 0) SB_CUDA(h, cudaMemcpyAsync(s.ws.sorted_edges_dev, p->sorted_edge_inds, (size_t)p->n_sorted * 4, cudaMemcpyHostToDevice, h->stream));
+  s.ws.n_sorted = p->n_sorted;
+  if ((rc = bottomup_post_kernels(h, *p, s.ws, cms, pafs, off, B))) return rc;
+  const SbPostWs& ws = s.ws;
   const size_t I = p->max_instances;
   SB_CUDA(h, cudaMemcpyAsync(out_instance_peaks, ws.inst_peaks, (size_t)B * I * C * 8, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaMemcpyAsync(out_instance_peak_vals, ws.inst_vals, (size_t)B * I * C * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1057,39 +1106,24 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
   if (!cms_host || !class_logits_host || !out_points || !out_vals || !out_class_probs)
     return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: null argument");
   if (B <= 0 || H <= 0 || W <= 0 || Hc <= 0 || Wc <= 0 || p->n_nodes <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: bad shape");
-  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES) return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
-  if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
-      p->max_node_peaks <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: bad strides / input scale / capacities");
+  int rc = check_class_params(h, p);
+  if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, NC = p->n_classes;
-  SbPostWs ws;
-  struct Guard { SbPostWs& w; std::vector<void*> bufs; ~Guard() { sb_post_ws_free(w); for (void* q : bufs) cudaFree(q); } } guard{ws, {}};
-  int rc = sb_post_ws_alloc(h, ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0);
-  if (rc) return rc;
-  ws.node_lists = true;
+  MapsScratch s;
+  if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0))) return rc;
+  s.ws.node_lists = true;
   const size_t w = sb_class_record_width(NC, C);
-  if ((rc = sb_dev_alloc(h, &ws.records, (size_t)B * w))) return rc;
-  auto dalloc = [&](void** q, size_t bytes) -> int {
-    cudaError_t e = cudaMalloc(q, bytes + 16);
-    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc: %s", cudaGetErrorString(e));
-    guard.bufs.push_back(*q);
-    return 0;
-  };
-  void *d_cms = nullptr, *d_cls = nullptr, *d_off = nullptr;
-  const size_t ncm = (size_t)B * H * W * C, ncl = (size_t)B * Hc * Wc * NC;
-  if ((rc = dalloc(&d_cms, ncm * 4)) || (rc = dalloc(&d_cls, ncl * 4))) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(d_cms, cms_host, ncm * 4, cudaMemcpyHostToDevice, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(d_cls, class_logits_host, ncl * 4, cudaMemcpyHostToDevice, h->stream));
-  if (offsets_host) {
-    if ((rc = dalloc(&d_off, 2 * ncm * 4))) return rc;
-    SB_CUDA(h, cudaMemcpyAsync(d_off, offsets_host, 2 * ncm * 4, cudaMemcpyHostToDevice, h->stream));
-  }
-  SbPeakParams pp{p->peak_threshold, p->refinement, p->integral_patch_size, (float)p->cm_output_stride, 1.0f};
-  if ((rc = sbk_local_peaks(h, d_cms, 0, (const float*)d_off, B, H, W, C, pp, ws))) return rc;
-  if ((rc = sbk_class_group(h, (const float*)d_cls, B, Hc, Wc, NC, (float)p->class_maps_output_stride, p->input_scale, ws))) return rc;
+  if ((rc = sb_dev_alloc(h, &s.ws.records, (size_t)B * w))) return rc;
+  SbMap cms{nullptr, H, W, C}, cls{nullptr, Hc, Wc, NC};
+  const float* off = nullptr;
+  const size_t ncm = (size_t)B * H * W * C;
+  if ((rc = s.upload(h, cms_host, ncm, &cms.dev)) || (rc = s.upload(h, class_logits_host, (size_t)B * Hc * Wc * NC, &cls.dev)) ||
+      (rc = s.upload(h, offsets_host, 2 * ncm, &off)))
+    return rc;
+  if ((rc = multiclass_post_kernels(h, *p, s.ws, cms, cls, off, B))) return rc;
   std::vector<float> rec((size_t)B * w);
-  SB_CUDA(h, cudaMemcpyAsync(rec.data(), ws.records, rec.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  SB_CUDA(h, cudaMemcpyAsync(rec.data(), s.ws.records, rec.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
   unpack_class_records(rec.data(), w, B, NC, C, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
@@ -1097,75 +1131,72 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
 
 // ---------------------------------- global peaks (single / centered instance) ----------------
 int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* p) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
-  if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first");
+  SbModel* m = configure_target(h, model_id, p);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int nb = (int)m->buffers.size();
   if (p->cms_buffer < 0 || p->cms_buffer >= nb || !m->buffers[p->cms_buffer].f32) return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
   if (p->offsets_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
-  SbBuffer& cb = m->buffers[p->cms_buffer];
+  const SbBuffer& cb = m->buffers[p->cms_buffer];
   if (cb.C > 256) return sb_fail(h, SB_ERR_UNSUPPORTED, "more than 256 confidence-map channels");
-  int target = (2 * h->sm_count + m->B - 1) / m->B;
-  m->g_rpc = std::max(1, (cb.H + target - 1) / target);
-  m->g_chunks = (cb.H + m->g_rpc - 1) / m->g_rpc;
-  if (m->gpart) cudaFree(m->gpart);
-  if (m->gpoints) cudaFree(m->gpoints);
-  if (m->gvals) cudaFree(m->gvals);
-  if (m->crop_off_dev) cudaFree(m->crop_off_dev);
-  SB_CUDA(h, cudaMalloc((void**)&m->gpart, (size_t)m->B * m->g_chunks * cb.C * 3 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&m->gpoints, (size_t)m->B * cb.C * 2 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&m->gvals, (size_t)m->B * cb.C * 4));
-  SB_CUDA(h, cudaMalloc((void**)&m->crop_off_dev, (size_t)m->B * 2 * 4));
+  if (const int rc = chain_drop(h, m)) return rc;
+  SbGlobalScratch& g = m->gs;
+  const int target = (2 * h->sm_count + m->B - 1) / m->B;
+  g.rpc = std::max(1, (cb.H + target - 1) / target);
+  g.chunks = (cb.H + g.rpc - 1) / g.rpc;
+  SB_CUDA(h, cudaMalloc((void**)&g.part, (size_t)m->B * g.chunks * cb.C * 3 * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.points, (size_t)m->B * cb.C * 2 * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.vals, (size_t)m->B * cb.C * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.crop_off, (size_t)m->B * 2 * 4));
   m->gl = *p;
-  m->gl_configured = true;
+  m->chain = SB_CHAIN_GLOBAL;
   return SB_OK;
 }
 
 int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int images_are_u8, int B,
                     const float* crop_offsets_host, float* out_points, float* out_vals) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->gl_configured) return sb_fail(h, SB_ERR_INVALID, "global-peak predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, "global-peak predictor not configured");
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
   if (rc) return rc;
-  if (crop_offsets_host) SB_CUDA(h, cudaMemcpyAsync(m->crop_off_dev, crop_offsets_host, (size_t)B * 8, cudaMemcpyHostToDevice, h->stream));
+  const SbGlobalScratch& g = m->gs;
+  if (crop_offsets_host) SB_CUDA(h, cudaMemcpyAsync(g.crop_off, crop_offsets_host, (size_t)B * 8, cudaMemcpyHostToDevice, h->stream));
   if ((rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B))) return rc;
   const sb_global_params& p = m->gl;
   SbBuffer& cb = m->buffers[p.cms_buffer];
-  const float* off = p.offsets_buffer >= 0 ? (const float*)m->buffers[p.offsets_buffer].dev : nullptr;
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-  if ((rc = sbk_global_peaks(h, cb.dev, 0, off, B, cb.H, cb.W, cb.C, pp, crop_offsets_host ? m->crop_off_dev : nullptr,
-                             m->gpart, m->g_chunks, m->g_rpc, m->gpoints, m->gvals))) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(out_points, m->gpoints, (size_t)B * cb.C * 8, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(out_vals, m->gvals, (size_t)B * cb.C * 4, cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = sbk_global_peaks(h, cb.dev, 0, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp,
+                             crop_offsets_host ? g.crop_off : nullptr, g.part, g.chunks, g.rpc, g.points, g.vals))) return rc;
+  SB_CUDA(h, cudaMemcpyAsync(out_points, g.points, (size_t)B * cb.C * 8, cudaMemcpyDeviceToHost, h->stream));
+  SB_CUDA(h, cudaMemcpyAsync(out_vals, g.vals, (size_t)B * cb.C * 4, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
   return SB_OK;
 }
 
 // ---------------------------------- centroids (top-down stage 1) ------------------------------
 int sb_centroid_configure(sb_handle_t h, int model_id, const sb_centroid_params* p) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !p) return sb_fail(h, SB_ERR_INVALID, "bad model id / params");
-  if (!m->configured) return sb_fail(h, SB_ERR_INVALID, "call sb_model_configure first");
+  SbModel* m = configure_target(h, model_id, p);
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int nb = (int)m->buffers.size();
   if (p->cms_buffer < 0 || p->cms_buffer >= nb || !m->buffers[p->cms_buffer].f32) return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
-  SbBuffer& cb = m->buffers[p->cms_buffer];
-  sb_post_ws_free(m->ws);
-  int rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, 1, 1, 0);
+  if (p->offsets_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
+  int rc = chain_drop(h, m);
   if (rc) return rc;
+  const SbBuffer& cb = m->buffers[p->cms_buffer];
+  if ((rc = sb_post_ws_alloc(h, m->ws, m->B, cb.H, cb.W, cb.C, p->max_peaks_per_sample, 1, 1, 0))) return rc;
   m->ce = *p;
-  m->ce_configured = true;
+  m->chain = SB_CHAIN_CENTROID;
   return SB_OK;
 }
 
 int sb_infer_centroids(sb_handle_t h, int model_id, const void* images_host, int images_are_u8, int B,
                        float* out_centroids, float* out_vals, int32_t* out_sample_inds, int32_t* out_n,
                        int32_t* out_flags) {
-  SbModel* m = get_model(h, model_id);
-  if (!m || !m->ce_configured) return sb_fail(h, SB_ERR_INVALID, "centroid predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_CENTROID, "centroid predictor not configured");
+  if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
@@ -1173,9 +1204,8 @@ int sb_infer_centroids(sb_handle_t h, int model_id, const void* images_host, int
   if ((rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B))) return rc;
   const sb_centroid_params& p = m->ce;
   SbBuffer& cb = m->buffers[p.cms_buffer];
-  const float* off = p.offsets_buffer >= 0 ? (const float*)m->buffers[p.offsets_buffer].dev : nullptr;
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-  if ((rc = sbk_local_peaks(h, cb.dev, 0, off, B, cb.H, cb.W, cb.C, pp, m->ws))) return rc;
+  if ((rc = sbk_local_peaks(h, cb.dev, 0, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, m->ws))) return rc;
   std::vector<int> cnt(B), fl(B);
   SB_CUDA(h, cudaMemcpyAsync(cnt.data(), m->ws.n_peaks, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaMemcpyAsync(fl.data(), m->ws.flags, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -99,6 +99,17 @@ struct SbEntryPlan {
   int pre_mode = SB_PRE_PLAIN;     // stem view: the PREPROCESS mode k_s2d_view applies
 };
 
+// The post-processing chain a model runs after its network (include/sleap_b200.h): one at a time.  Every configure call,
+// sb_model_configure's included, drops the previous chain with its tracker and record exchange.  The fused top-down
+// pipeline is a layer over a centroid chain and a global chain, valid while neither model's chain_gen moves.
+enum { SB_CHAIN_ANY = -1, SB_CHAIN_NONE = 0, SB_CHAIN_PAF, SB_CHAIN_CLASS, SB_CHAIN_GLOBAL, SB_CHAIN_CENTROID };
+
+// Global-peak scratch of the global chain (per frame of the configured batch)
+struct SbGlobalScratch {
+  float *part = nullptr, *points = nullptr, *vals = nullptr, *crop_off = nullptr;
+  int rpc = 1, chunks = 1;   // rows per chunk of the partial maxima, chunks per frame
+};
+
 struct SbModel {
   int precision = 0;  // 0: fp16 activations + tensor-core convs; 1: fp32 CUDA-core path
   std::vector<SbOp> ops;
@@ -122,13 +133,14 @@ struct SbModel {
   std::vector<cudaEvent_t> fwd_events;  // sb_model_forward_times: (start, end) pairs around every forward pass
   int fwd_n = 0;                        // pairs recorded since the last read
   bool fwd_timing = false;
-  // predictors
+  // post-processing chain: `chain` says which of the parameter structs bu / mc / gl / ce is live; chain_gen counts the
+  // drops (sb_topdown_configure records it)
+  int chain = SB_CHAIN_NONE;
+  unsigned chain_gen = 0;
   SbPostWs ws;
   sb_bottomup_params bu{};
   std::vector<int> bu_edges;
-  bool bu_configured = false;
   sb_multiclass_params mc{};
-  bool mc_configured = false;              // the multi-class chain (k_class_group) instead of the PAF chain; one at a time
   int guard_op = -1;
   // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect, sb_multiclass_submit / _collect)
   void* frames_slot[2] = {nullptr, nullptr};
@@ -139,13 +151,9 @@ struct SbModel {
   bool slot_used[2] = {false, false};
   cudaStream_t copy_stream = nullptr;      // first op that overwrites a head buffer the post-processing stream may still read
   sb_global_params gl{};
-  bool gl_configured = false;
-  float *gpart = nullptr, *gpoints = nullptr, *gvals = nullptr, *crop_off_dev = nullptr;
-  int g_rpc = 1, g_chunks = 1;
+  SbGlobalScratch gs;
   sb_centroid_params ce{};
-  bool ce_configured = false;
-  bool td_configured = false;              // fused top-down pipeline (sb_topdown_configure); state lives on the centroid model
-  SbTopdown* td = nullptr;
+  SbTopdown* td = nullptr;                 // fused top-down pipeline (sb_topdown_configure), held by its centroid model
   SbEntryPlan entry;                       // input stage (sb_entry.cu)
   SbGather gather;                         // peer-memory exchange of the result records (sb_gather.cu)
   // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu); its per-frame track records
@@ -159,6 +167,9 @@ struct SbModel {
 
 // one forward pass: the production program, or the all-stores one
 int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B, bool all_stores = false);
+
+// Model `id` of the handle when its chain is `kind` (SB_CHAIN_ANY: any chain); otherwise fails with `what`, nullptr
+SbModel* chain_model(sb_handle_s* h, int id, int kind, const char* what);
 
 void sb_topdown_free(SbModel* m);        // sb_topdown.cu
 

@@ -107,6 +107,7 @@ __global__ void __launch_bounds__(128) k_td_pack(const float* __restrict__ sel_c
 struct SbTopdown {
   sb_topdown_params p{};
   SbModel* inst = nullptr;
+  unsigned gen_c = 0, gen_i = 0;    // chain_gen of the centroid and the instance model when it was configured
   int K = 0, nodes = 0, width = 0, Bmax = 0, crop_elem = 1;
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
@@ -124,21 +125,16 @@ void sb_topdown_free(SbModel* m) {
   if (t->total_host) cudaFreeHost(t->total_host);
   delete t;
   m->td = nullptr;
-  m->td_configured = false;
-}
-
-static SbModel* tmodel(sb_handle_s* h, int id) {
-  if (!h || id < 0 || id >= (int)h->models.size()) return nullptr;
-  return h->models[id];
 }
 
 extern "C" {
 
 int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: null argument");
-  SbModel* mc = tmodel(h, p->centroid_model);
-  SbModel* mi = tmodel(h, p->instance_model);
-  if (!mc || !mi || mc == mi) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: bad model ids");
+  static const char* const bad_ids = "sb_topdown_configure: bad model ids";
+  SbModel* mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
+  SbModel* mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
+  if (!mc || !mi || mc == mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
   if (p->crop_size <= 0 || p->max_centroids_per_frame <= 0 || p->max_crops_per_call <= 0 || max_batch <= 0)
     return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: bad sizes");
   if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_configure: more than 1024 frames per batch");
@@ -148,10 +144,10 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batc
   if ((rc = sb_model_configure(h, p->instance_model, p->max_crops_per_call, p->crop_size, p->crop_size, C_in))) return rc;
   if ((rc = sb_centroid_configure(h, p->centroid_model, &p->centroid))) return rc;
   if ((rc = sb_global_configure(h, p->instance_model, &p->instance))) return rc;
-  sb_topdown_free(mc);
-  SbTopdown* t = new SbTopdown();
+  SbTopdown* t = new SbTopdown();           // the centroid configure dropped the previous one
   mc->td = t;
   t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
+  t->gen_c = mc->chain_gen; t->gen_i = mi->chain_gen;
   t->nodes = mi->buffers[p->instance.cms_buffer].C;
   t->width = t->K * (3 + t->nodes * 3) + 2;
   t->crop_elem = 1;                                                    // uint8 frames (float frames: 4, decided per call)
@@ -168,18 +164,18 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batc
     sb_topdown_free(mc);
     return sb_fail(h, SB_ERR_CUDA, "sb_topdown_configure: allocation failed");
   }
-  mc->td_configured = true;
   return SB_OK;
 }
 
 int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B, float* out_centroids,
                      float* out_centroid_vals, float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid,
                      int32_t* out_flags) {
-  SbModel* mc = tmodel(h, centroid_model_id);
-  if (!mc || !mc->td_configured || !mc->td) return sb_fail(h, SB_ERR_INVALID, "top-down pipeline not configured");
+  SbModel* mc = chain_model(h, centroid_model_id, SB_CHAIN_ANY, "top-down pipeline not configured");
+  if (!mc || !mc->td) return sb_fail(h, SB_ERR_INVALID, "top-down pipeline not configured");
   SbTopdown* t = mc->td;
   SbModel* mi = t->inst;
-  if (!mc->configured || !mc->ce_configured || !mi->configured || !mi->gl_configured)
+  // a configure call on either model outside sb_topdown_configure moved its chain_gen (sb_model_configure included)
+  if (mc->chain != SB_CHAIN_CENTROID || mc->chain_gen != t->gen_c || mi->chain != SB_CHAIN_GLOBAL || mi->chain_gen != t->gen_i)
     return sb_fail(h, SB_ERR_INVALID, "top-down pipeline: a model was reconfigured; call sb_topdown_configure again");
   if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   SB_CUDA(h, cudaSetDevice(h->device));
@@ -218,7 +214,7 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
     if ((rc = sbk_crop(h, mc->frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
                        cs, cs, t->crops, frames_are_u8))) return rc;
     if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n))) return rc;
-    if ((rc = sbk_global_peaks(h, ib.dev, 0, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gpart, mi->g_chunks, mi->g_rpc,
+    if ((rc = sbk_global_peaks(h, ib.dev, 0, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
                                t->ipts + (size_t)c0 * t->nodes * 2, t->ivals + (size_t)c0 * t->nodes))) return rc;
   }
   k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags, t->record,

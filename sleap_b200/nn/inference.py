@@ -22,7 +22,7 @@ from sleap_b200 import _lib
 from sleap_b200._lib import BottomUpParams, CentroidParams, GlobalParams, MultiClassParams, TopdownParams, f32, i32, ptr
 from sleap_b200.nn import architectures as arch
 from sleap_b200.nn import paf_grouping, peak_finding
-from sleap_b200.nn.model import DeviceModel, PRECISION_FP16, PRECISION_FP32, load_weights, load_weights_npz
+from sleap_b200.nn.model import DeviceModel, PRECISION_FP16, PRECISION_FP32, chain_key, load_weights, load_weights_npz
 
 REFINE = peak_finding.REFINE
 
@@ -142,20 +142,17 @@ class SingleInstanceInferenceLayer(InferenceLayer):
         self.refinement = refinement
         self.integral_patch_size = integral_patch_size
         self.return_confmaps = return_confmaps
-        self._cfg_key = None
+
+    def params(self) -> GlobalParams:
+        return GlobalParams(self.confmaps_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer,
+                            int(self.output_stride), float(self.peak_threshold), REFINE.get(self.refinement, 0),
+                            int(self.integral_patch_size), float(self.input_scale))
 
     def _configure(self, B, H, W, C):
         m = self.keras_model
         if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
             m.configure(B, H, W, C)
-            self._cfg_key = None
-        key = (m.configured_for, self.peak_threshold, self.refinement, self.integral_patch_size, self.input_scale)
-        if self._cfg_key != key:
-            p = GlobalParams(self.confmaps_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer,
-                             int(self.output_stride), float(self.peak_threshold), REFINE.get(self.refinement, 0),
-                             int(self.integral_patch_size), float(self.input_scale))
-            m.handle.call("sb_global_configure", m.model_id, byref(p))
-            self._cfg_key = key
+        m.configure_chain("sb_global_configure", self.params())
 
     def call(self, data, crop_offsets=None):
         imgs = self._prep(_images_of(data))
@@ -208,21 +205,18 @@ class CentroidCrop(InferenceLayer):
         self.max_instances = max_instances
         self.precrop_resize = precrop_resize
         self.max_peaks_per_sample = max_peaks_per_sample
-        self._cfg_key = None
         self._resizer = None
+
+    def params(self) -> CentroidParams:
+        return CentroidParams(self.confmaps_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer,
+                              int(self.output_stride), float(self.peak_threshold), REFINE.get(self.refinement, 0),
+                              int(self.integral_patch_size), float(self.input_scale), int(self.max_peaks_per_sample))
 
     def call(self, inputs):
         full_imgs = self._prep(_images_of(inputs))
         B, H, W, C = full_imgs.shape
         m = self.keras_model
-        m.configure(B, H, W, C)
-        key = (m.configured_for, self.peak_threshold, self.refinement, self.integral_patch_size, self.input_scale)
-        if self._cfg_key != key:
-            p = CentroidParams(self.confmaps_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer,
-                               int(self.output_stride), float(self.peak_threshold), REFINE.get(self.refinement, 0),
-                               int(self.integral_patch_size), float(self.input_scale), int(self.max_peaks_per_sample))
-            m.handle.call("sb_centroid_configure", m.model_id, byref(p))
-            self._cfg_key = key
+        m.configure(B, H, W, C).configure_chain("sb_centroid_configure", self.params())
         cap = B * self.max_peaks_per_sample
         pts = np.zeros((cap, 2), np.float32)
         vals = np.zeros((cap,), np.float32)
@@ -403,7 +397,6 @@ class TopDownInferenceModel(InferenceModel):
         self.centroid_crop = centroid_crop
         self.instance_peaks = instance_peaks
         self.fused = True            # one device pipeline (sb_infer_topdown) when both stages are device models
-        self._td_key = None
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
@@ -419,24 +412,17 @@ class TopDownInferenceModel(InferenceModel):
         B, H, W, C = imgs.shape
         mc, mi = cc.keras_model, fp.keras_model
         K = int(cc.max_instances) if cc.max_instances else int(cc.max_peaks_per_sample)
-        cap = max(B, self._td_key[0]) if self._td_key else B
-        key = (cap, H, W, C, K, cc.peak_threshold, cc.refinement, cc.integral_patch_size, cc.input_scale, cc.max_peaks_per_sample,
-               cc.max_instances, cc.crop_size, fp.peak_threshold, fp.refinement, fp.integral_patch_size, fp.input_scale,
-               fp.max_crops_per_call)
-        if self._td_key != key or mc.configured_for != (cap, H, W, C) or mi.configured_for != (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C):
-            p = TopdownParams(
-                mc.model_id, mi.model_id,
-                CentroidParams(cc.confmaps_buffer, -1 if cc.offsets_buffer is None else cc.offsets_buffer, int(cc.output_stride),
-                               float(cc.peak_threshold), REFINE.get(cc.refinement, 0), int(cc.integral_patch_size), float(cc.input_scale),
-                               int(cc.max_peaks_per_sample)),
-                GlobalParams(fp.confmaps_buffer, -1 if fp.offsets_buffer is None else fp.offsets_buffer, int(fp.output_stride),
-                             float(fp.peak_threshold), REFINE.get(fp.refinement, 0), int(fp.integral_patch_size), float(fp.input_scale)),
-                int(cc.crop_size), int(cc.max_instances or 0), K, int(fp.max_crops_per_call))
+        p = TopdownParams(mc.model_id, mi.model_id, cc.params(), fp.params(), int(cc.crop_size), int(cc.max_instances or 0), K,
+                          int(fp.max_crops_per_call))
+        # the pipeline's record on both models: a staged call on either one reconfigures its own chain, and this one again
+        record = ("sb_topdown_configure", chain_key(p))
+        cap = max(B, mc.configured_for[0]) if mc.chain == record else B
+        if mc.chain != record or mi.chain != record or mc.configured_for != (cap, H, W, C):
+            mc.chain = mi.chain = None
             mc.handle.call("sb_topdown_configure", byref(p), cap, H, W, C)
             mc.configured_for = (cap, H, W, C)
             mi.configured_for = (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C)
-            cc._cfg_key = fp._cfg_key = None
-            self._td_key = key
+            mc.chain = mi.chain = record
         n_nodes = next(h["channels"] for h in mi.spec["heads"] if h["name"] == fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
@@ -501,7 +487,6 @@ class BottomUpInferenceLayer(InferenceLayer):
         self.max_peaks_per_sample = max_peaks_per_sample
         self.max_node_peaks = max_node_peaks
         self.max_instances = max_instances
-        self._cfg_key = None
         self._keep = None
         # a Tracker with track_device, run by k_track inside each step (BottomUpPredictor.predict sets it for its span),
         # and the predictor's max_instances cut of the instance list (-1: none)
@@ -519,7 +504,7 @@ class BottomUpInferenceLayer(InferenceLayer):
 
     def detach_tracker(self):
         m = self.keras_model
-        if getattr(self.tracker, "_device", None) is not None and self._cfg_key is not None:
+        if getattr(self.tracker, "_device", None) is not None and m.chain and m.chain[0] == "sb_bottomup_configure":
             m.handle.call("sb_bottomup_attach_tracker", m.model_id, -1, -1, 1.0, 1.0)
 
     def track_fields(self, slot, B):
@@ -537,34 +522,18 @@ class BottomUpInferenceLayer(InferenceLayer):
                 "tracking_scores": rec[:, 2 + 2 * I:].copy()}
 
     def params(self) -> BottomUpParams:
-        ps = self.paf_scorer
-        edges = i32(ps.edge_inds).reshape(-1, 2)
-        sorted_e = i32(list(ps.sorted_edge_inds))
-        mip = ps.min_instance_peaks
-        if isinstance(mip, float):
-            mip = int(mip * ps.n_nodes)
-        self._keep = (edges, sorted_e)
-        return BottomUpParams(
-            self.confmaps_buffer, self.pafs_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer,
-            int(self.cm_output_stride), int(self.paf_output_stride), float(self.peak_threshold),
-            REFINE.get(self.refinement, 0), int(self.integral_patch_size), ps.n_nodes, ps.n_edges,
-            edges.ctypes.data, sorted_e.ctypes.data, len(sorted_e), int(ps.n_points), float(ps.max_edge_length_ratio),
-            float(ps.dist_penalty_weight), float(ps.min_line_scores), int(mip), float(self.input_scale),
-            int(self.max_peaks_per_sample), int(self.max_node_peaks), int(self.max_instances))
+        """The chain's parameters; their edge arrays stay alive in ``self._keep``."""
+        p, self._keep = paf_params(
+            self.paf_scorer, (self.confmaps_buffer, self.pafs_buffer, -1 if self.offsets_buffer is None else self.offsets_buffer),
+            self.cm_output_stride, self.paf_output_stride, self.peak_threshold, self.refinement, self.integral_patch_size,
+            self.input_scale, self.max_peaks_per_sample, self.max_node_peaks, self.max_instances)
+        return p
 
     def _configure(self, B, H, W, C):
         m = self.keras_model
         if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
             m.configure(B, H, W, C)
-            self._cfg_key = None
-        ps = self.paf_scorer
-        key = (m.configured_for, self.peak_threshold, self.refinement, self.integral_patch_size, self.input_scale,
-               ps.n_points, ps.max_edge_length_ratio, ps.dist_penalty_weight, ps.min_line_scores, ps.min_instance_peaks,
-               self.max_peaks_per_sample, self.max_node_peaks, self.max_instances)
-        if self._cfg_key != key:
-            p = self.params()
-            m.handle.call("sb_bottomup_configure", m.model_id, byref(p))
-            self._cfg_key = key
+        m.configure_chain("sb_bottomup_configure", self.params(), *self._keep)
 
     def call(self, data):
         raw = _images_of(data)
@@ -614,6 +583,22 @@ class BottomUpInferenceLayer(InferenceLayer):
                 "edge_inds": rows(ei, co), "edge_peak_inds": rows(epi, co), "line_scores": rows(ls, co)}
 
 
+def paf_params(ps, buffers, cm_output_stride, paf_output_stride, peak_threshold, refinement, integral_patch_size, input_scale,
+               max_peaks_per_sample, max_node_peaks, max_instances):
+    """BottomUpParams of the PAF chain of PAFScorer ``ps`` reading head ``buffers`` (cms, pafs, offsets), and the
+    (edges, sorted edges) arrays its pointers point to, to keep alive while it is used."""
+    edges = i32(ps.edge_inds).reshape(-1, 2)
+    sorted_e = i32(list(ps.sorted_edge_inds))
+    mip = ps.min_instance_peaks
+    if isinstance(mip, float):
+        mip = int(mip * ps.n_nodes)
+    p = BottomUpParams(*buffers, int(cm_output_stride), int(paf_output_stride), float(peak_threshold), REFINE.get(refinement, 0),
+                       int(integral_patch_size), ps.n_nodes, ps.n_edges, edges.ctypes.data, sorted_e.ctypes.data, len(sorted_e),
+                       int(ps.n_points), float(ps.max_edge_length_ratio), float(ps.dist_penalty_weight), float(ps.min_line_scores),
+                       int(mip), float(input_scale), int(max_peaks_per_sample), int(max_node_peaks), int(max_instances))
+    return p, (edges, sorted_e)
+
+
 def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0.2, refinement="integral",
                        integral_patch_size=5, offsets=None, input_scale=1.0, max_peaks_per_sample=1024,
                        max_node_peaks=32, max_instances=64, return_paf_graph=True, handle=None):
@@ -624,16 +609,8 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
     B, H, W, C = cms.shape
     _, Hp, Wp, C2 = pafs.shape
     ps = paf_scorer
-    edges = i32(ps.edge_inds).reshape(-1, 2)
-    sorted_e = i32(list(ps.sorted_edge_inds))
-    mip = ps.min_instance_peaks
-    if isinstance(mip, float):
-        mip = int(mip * ps.n_nodes)
-    p = BottomUpParams(-1, -1, -1, int(cm_output_stride), int(ps.pafs_stride), float(peak_threshold),
-                       REFINE.get(refinement, 0), int(integral_patch_size), ps.n_nodes, ps.n_edges, edges.ctypes.data,
-                       sorted_e.ctypes.data, len(sorted_e), int(ps.n_points), float(ps.max_edge_length_ratio),
-                       float(ps.dist_penalty_weight), float(ps.min_line_scores), int(mip), float(input_scale),
-                       int(max_peaks_per_sample), int(max_node_peaks), int(max_instances))
+    p, keep = paf_params(ps, (-1, -1, -1), cm_output_stride, ps.pafs_stride, peak_threshold, refinement, integral_patch_size,
+                         input_scale, max_peaks_per_sample, max_node_peaks, max_instances)
     I, N = max_instances, ps.n_nodes
     ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32); isc = np.zeros((B, I), np.float32)
     nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
@@ -655,6 +632,27 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
         out.update({"peaks": rows(peaks, po), "peak_vals": rows(pv, po), "peak_channel_inds": rows(pc, po),
                     "edge_inds": rows(ei, co), "edge_peak_inds": rows(epi, co), "line_scores": rows(ls, co)})
     return out
+
+
+def _pipelined_batches(layer, imgs, batch_size, submit_fn, collect):
+    """The double-buffered batch loop of the bottom-up models (uint8 frames, chain configured): batch i+1 is submitted
+    (``submit_fn``: its upload on the copy stream, network and post-processing queued) into slot (i+1) % 2 before
+    ``collect(slot, B)`` waits for batch i and returns its result dict."""
+    m = layer.keras_model
+    starts = list(range(0, len(imgs), batch_size))
+    keep = {}
+
+    def submit(k):
+        batch = layer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
+        keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
+        m.handle.call(submit_fn, m.model_id, ptr(batch), batch.shape[0], k % 2)
+        return batch.shape[0]
+
+    sizes = {0: submit(0)}
+    for k in range(len(starts)):
+        if k + 1 < len(starts):
+            sizes[k + 1] = submit(k + 1)
+        yield collect(k % 2, sizes.pop(k))
 
 
 class BottomUpInferenceModel(InferenceModel):
@@ -684,31 +682,21 @@ class BottomUpInferenceModel(InferenceModel):
         layer.attach_tracker(np.asarray(imgs[0]).shape[:2])
         m = layer.keras_model
         I, N = layer.max_instances, layer.paf_scorer.n_nodes
-        starts = list(range(0, n, batch_size))
-        keep = {}
 
-        def submit(k):
-            batch = layer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
-            keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
-            m.handle.call("sb_bottomup_submit", m.model_id, ptr(batch), batch.shape[0], k % 2)
-            return batch.shape[0]
-
-        sizes = {0: submit(0)}
-        for k in range(len(starts)):
-            if k + 1 < len(starts):
-                sizes[k + 1] = submit(k + 1)
-            B = sizes.pop(k)
+        def collect(slot, B):
             ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32)
             isc = np.zeros((B, I), np.float32); nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
-            m.handle.call("sb_bottomup_collect", m.model_id, k % 2, B, ptr(ip), ptr(iv), ptr(isc), ptr(nv), ptr(fl))
+            m.handle.call("sb_bottomup_collect", m.model_id, slot, B, ptr(ip), ptr(iv), ptr(isc), ptr(nv), ptr(fl))
             w = int(nv.max()) if B else 0
             out = {"instance_peaks": ip[:, :w], "instance_peak_vals": iv[:, :w], "instance_scores": isc[:, :w],
                    "n_valid": nv.astype(np.int64), "flags": fl}
-            out.update(layer.track_fields(k % 2, B))
+            out.update(layer.track_fields(slot, B))
             pg = getattr(m, "peer_gather", None)
             if pg is not None:      # multi-GPU: every rank's records of this step came over with the result copy (sb_gather_*)
-                out["gathered_records"], out["gathered_counts"] = pg.gathered(k % 2, B, I, N)
-            yield out
+                out["gathered_records"], out["gathered_counts"] = pg.gathered(slot, B, I, N)
+            return out
+
+        yield from _pipelined_batches(layer, imgs, batch_size, "sb_bottomup_submit", collect)
 
     def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
         """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
@@ -745,26 +733,19 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
         self.max_node_peaks = max_node_peaks
         channels = {h["name"]: h["channels"] for h in keras_model.spec["heads"]}
         self.n_nodes, self.n_classes = int(channels[self.CMS]), int(channels[self.CLASS_MAPS])
-        self._cfg_key = None
 
     def params(self) -> MultiClassParams:
         heads = self.keras_model.cm.head_buffers
-        return MultiClassParams(heads[self.CMS], heads[self.CLASS_MAPS], heads[self.OFFSETS] if self.has_offsets else -1,
-                                int(self.cm_output_stride), int(self.class_maps_output_stride), float(self.peak_threshold),
-                                REFINE.get(self.refinement, 0), int(self.integral_patch_size), self.n_nodes, self.n_classes,
-                                float(self.input_scale), int(self.max_peaks_per_sample), int(self.max_node_peaks))
+        return class_params((heads[self.CMS], heads[self.CLASS_MAPS], heads[self.OFFSETS] if self.has_offsets else -1),
+                            self.cm_output_stride, self.class_maps_output_stride, self.peak_threshold, self.refinement,
+                            self.integral_patch_size, self.n_nodes, self.n_classes, self.input_scale, self.max_peaks_per_sample,
+                            self.max_node_peaks)
 
     def _configure(self, B, H, W, C):
         m = self.keras_model
         if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
             m.configure(B, H, W, C)
-            self._cfg_key = None
-        key = (m.configured_for, self.peak_threshold, self.refinement, self.integral_patch_size, self.input_scale,
-               self.cm_output_stride, self.class_maps_output_stride, self.max_peaks_per_sample, self.max_node_peaks)
-        if self._cfg_key != key:
-            p = self.params()
-            m.handle.call("sb_multiclass_configure", m.model_id, byref(p))
-            self._cfg_key = key
+        m.configure_chain("sb_multiclass_configure", self.params())
 
     def _outputs(self, B):
         K, N = self.n_classes, self.n_nodes
@@ -791,6 +772,14 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
         return out
 
 
+def class_params(buffers, cm_output_stride, class_maps_output_stride, peak_threshold, refinement, integral_patch_size, n_nodes,
+                 n_classes, input_scale, max_peaks_per_sample, max_node_peaks):
+    """MultiClassParams of the identity chain reading head ``buffers`` (cms, class maps, offsets)."""
+    return MultiClassParams(*buffers, int(cm_output_stride), int(class_maps_output_stride), float(peak_threshold),
+                            REFINE.get(refinement, 0), int(integral_patch_size), int(n_nodes), int(n_classes), float(input_scale),
+                            int(max_peaks_per_sample), int(max_node_peaks))
+
+
 def bottomup_multiclass_from_maps(cms, class_logits, cm_output_stride, class_maps_output_stride, peak_threshold=0.2,
                                   refinement="integral", integral_patch_size=5, offsets=None, input_scale=1.0,
                                   max_peaks_per_sample=1024, max_node_peaks=32, handle=None):
@@ -801,9 +790,8 @@ def bottomup_multiclass_from_maps(cms, class_logits, cm_output_stride, class_map
     cms, class_logits = f32(cms), f32(class_logits)
     B, H, W, N = cms.shape
     _, Hc, Wc, K = class_logits.shape
-    p = MultiClassParams(-1, -1, -1, int(cm_output_stride), int(class_maps_output_stride), float(peak_threshold),
-                         REFINE.get(refinement, 0), int(integral_patch_size), N, K, float(input_scale), int(max_peaks_per_sample),
-                         int(max_node_peaks))
+    p = class_params((-1, -1, -1), cm_output_stride, class_maps_output_stride, peak_threshold, refinement, integral_patch_size,
+                     N, K, input_scale, max_peaks_per_sample, max_node_peaks)
     pts = np.zeros((B, K, N, 2), np.float32); vals = np.zeros((B, K, N), np.float32); probs = np.zeros((B, K, N), np.float32)
     fl = np.zeros((B,), np.int32)
     off = None if offsets is None else f32(offsets)
@@ -837,23 +825,13 @@ class BottomUpMultiClassInferenceModel(InferenceModel):
         _, H, W, C = first.shape
         layer._configure(batch_size, H, W, C)
         m = layer.keras_model
-        starts = list(range(0, n, batch_size))
-        keep = {}
 
-        def submit(k):
-            batch = layer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
-            keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
-            m.handle.call("sb_multiclass_submit", m.model_id, ptr(batch), batch.shape[0], k % 2)
-            return batch.shape[0]
-
-        sizes = {0: submit(0)}
-        for k in range(len(starts)):
-            if k + 1 < len(starts):
-                sizes[k + 1] = submit(k + 1)
-            B = sizes.pop(k)
+        def collect(slot, B):
             pts, vals, probs, fl = layer._outputs(B)
-            m.handle.call("sb_multiclass_collect", m.model_id, k % 2, B, ptr(pts), ptr(vals), ptr(probs), ptr(fl))
-            yield {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+            m.handle.call("sb_multiclass_collect", m.model_id, slot, B, ptr(pts), ptr(vals), ptr(probs), ptr(fl))
+            return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+
+        yield from _pipelined_batches(layer, imgs, batch_size, "sb_multiclass_submit", collect)
 
     def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
         """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""

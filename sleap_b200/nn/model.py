@@ -1,6 +1,7 @@
 """Device model: compiled op-list + weights resident on one GPU (replaces the Keras model of
 sleap/nn/model.py:312-364 and ``tf.keras.models.load_model`` at sleap/nn/inference.py:3203-3213)."""
 import ctypes
+import functools
 import json
 import os
 from ctypes import c_int, c_void_p
@@ -35,6 +36,9 @@ class DeviceModel:
                          ctypes.byref(mid))
         self.model_id = mid.value
         self.configured_for = None
+        # (configure call, chain_key) of the post-processing chain the device model runs (None: none, or not known).
+        # Any configure call drops the previous chain, the network's included (include/sleap_b200.h).
+        self.chain = None
         self.peer_gather = None      # sleap_b200.parallel.PeerGather once the multi-GPU record exchange is connected
 
     def head_buffer(self, name):
@@ -45,7 +49,18 @@ class DeviceModel:
         if self.configured_for != key:
             self.handle.call("sb_model_configure", self.model_id, *key)
             self.configured_for = key
-            self._post_cfg = None
+            self.chain = None
+        return self
+
+    def configure_chain(self, fn_name, params, *arrays):
+        """Configures the post-processing chain with ``fn_name`` (``sb_bottomup_configure``, ``sb_multiclass_configure``,
+        ``sb_global_configure`` or ``sb_centroid_configure``) unless the model already runs it with these parameters;
+        ``arrays`` are the ones the pointer fields of ``params`` point to."""
+        record = (fn_name, chain_key(params, *arrays))
+        if self.chain != record:
+            self.chain = None                     # a refused call may have dropped the previous chain
+            self.handle.call(fn_name, self.model_id, ctypes.byref(params))
+            self.chain = record
         return self
 
     def net_hw(self, H, W):
@@ -93,6 +108,26 @@ class DeviceModel:
             feat = buf[..., c0:c0 + Cl]
         head = next(h for h in self.spec["heads"] if h["name"] == name)
         return class_vectors_from_features(feat, head, self.dense_weights)
+
+
+def chain_key(params, *arrays):
+    """Cache key of a chain's ctypes parameter struct: its bytes with the pointer fields zeroed, then the bytes of the
+    ``arrays`` those fields point to -- a key of the values, whichever copy of them the pointers name.  It is computed
+    on every predictor call, so a struct without pointer fields is not copied."""
+    pointers = _pointer_fields(type(params))
+    if pointers:
+        params = type(params).from_buffer_copy(params)
+        for name in pointers:
+            setattr(params, name, None)
+    key = bytes(params)
+    for a in arrays:
+        key += np.ascontiguousarray(a).tobytes()
+    return key
+
+
+@functools.lru_cache(maxsize=None)
+def _pointer_fields(cls):
+    return tuple(name for name, typ in cls._fields_ if typ is c_void_p)
 
 
 def class_vectors_from_features(feat, head, weights):

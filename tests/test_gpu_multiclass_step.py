@@ -341,6 +341,6 @@ def test_errors():
     out = np.zeros(64, np.uint8)
     with pytest.raises(SleapB200Error):                           # the record exchange is the PAF chain's
         m.handle.call("sb_gather_init", m.model_id, 0, 1, 2, out.ctypes.data_as(c_void_p))
-    layer._cfg_key = None
+    m.chain = None
     res = pred.inference_model.predict_on_batch(imgs)             # a refused configure leaves a usable model after a good one
     assert np.isfinite(res["instance_peaks"]).any()

@@ -203,7 +203,7 @@ class C4:
 
     def reconfigure(self):
         """sb_bottomup_configure again (it reads SB_DISABLE_POST_OVERLAP); the network keeps its configuration."""
-        self.layer._cfg_key = None
+        self.model.chain = None
         self.layer._configure(B, *self.hw, 1)
 
     def refs(self):
