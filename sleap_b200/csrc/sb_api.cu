@@ -97,28 +97,30 @@ int sb_set_stream(sb_handle_t h, void* cuda_stream) {
 
 }  // extern "C"
 
-namespace {
-
-struct DevBuf {  // RAII temporary device buffer for the stage-level calls
-  void* p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-  int alloc(sb_handle_s* h, size_t bytes) {
-    cudaError_t e = cudaMalloc(&p, bytes ? bytes : 16);
-    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc(%zu): %s", bytes, cudaGetErrorString(e));
-    return 0;
+int sb_peaks_to_host(sb_handle_s* h, const SbPostWs& ws, int B, float* out_points, float* out_vals, int32_t* out_channel_inds,
+                     int32_t* out_sample_inds, int32_t* out_n, int32_t* out_flags) {
+  SbScratch s(h);
+  std::vector<int> cnt(B), flags(B);
+  int rc;
+  if ((rc = s.to_host(cnt.data(), ws.n_peaks, (size_t)B)) || (rc = s.to_host(flags.data(), ws.flags, (size_t)B)) || (rc = s.sync()))
+    return rc;
+  const size_t MP = ws.max_peaks;
+  int total = 0;
+  for (int b = 0; b < B; ++b) {
+    const size_t nb = cnt[b];
+    if (nb > 0) {
+      if ((rc = s.to_host(out_points + 2 * (size_t)total, ws.peaks + b * MP * 2, nb * 2)) ||
+          (rc = s.to_host(out_vals + total, ws.peak_vals + b * MP, nb)) ||
+          (rc = s.to_host(out_channel_inds ? out_channel_inds + total : nullptr, ws.peak_ch + b * MP, nb, true)))
+        return rc;
+      for (size_t i = 0; i < nb; ++i) out_sample_inds[total + i] = b;
+    }
+    total += cnt[b];
+    if (out_flags) out_flags[b] = flags[b];
   }
-  template <typename T> T* as() { return (T*)p; }
-};
-
-struct WsGuard {
-  SbPostWs ws;
-  ~WsGuard() { sb_post_ws_free(ws); }
-};
-
-#define H2D(h, dst, src, bytes) SB_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, (h)->stream))
-#define D2H(h, dst, src, bytes) SB_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, (h)->stream))
-
-}  // namespace
+  *out_n = total;
+  return s.sync();
+}
 
 extern "C" {
 
@@ -132,38 +134,14 @@ int sb_find_local_peaks(sb_handle_t h, const float* cms_host, int B, int H, int 
     return sb_fail(h, SB_ERR_INVALID, "sb_find_local_peaks: bad shape");
   if ((long long)H * W * C >= (1ll << 31)) return sb_fail(h, SB_ERR_UNSUPPORTED, "map too large");
   SB_CUDA(h, cudaSetDevice(h->device));
-  WsGuard g;
-  int rc = sb_post_ws_alloc(h, g.ws, B, H, W, C, max_peaks_per_sample, 1, 1, 0);
-  if (rc) return rc;
+  SbScratch s(h);
   const size_t n = (size_t)B * H * W * C;
-  DevBuf d_cms, d_off;
-  if ((rc = d_cms.alloc(h, n * sizeof(float)))) return rc;
-  H2D(h, d_cms.p, cms_host, n * sizeof(float));
-  if (offsets_host) {
-    if ((rc = d_off.alloc(h, 2 * n * sizeof(float)))) return rc;
-    H2D(h, d_off.p, offsets_host, 2 * n * sizeof(float));
-  }
+  const float *d_cms, *d_off;
+  int rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, max_peaks_per_sample, 1, 1, 0);
+  if (rc || (rc = s.upload(cms_host, n, &d_cms)) || (rc = s.upload(offsets_host, 2 * n, &d_off, true))) return rc;
   SbPeakParams p{threshold, refinement, integral_patch_size, 1.0f, 1.0f};
-  if ((rc = sbk_local_peaks(h, d_cms.p, 0, offsets_host ? d_off.as<float>() : nullptr, B, H, W, C, p, g.ws))) return rc;
-  std::vector<int> cnt(B), flags(B);
-  D2H(h, cnt.data(), g.ws.n_peaks, B * sizeof(int));
-  D2H(h, flags.data(), g.ws.flags, B * sizeof(int));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  int total = 0;
-  for (int b = 0; b < B; ++b) {
-    const int nb = cnt[b];
-    if (nb > 0) {
-      D2H(h, out_points + 2 * (size_t)total, g.ws.peaks + (size_t)b * max_peaks_per_sample * 2, nb * 2 * sizeof(float));
-      D2H(h, out_vals + total, g.ws.peak_vals + (size_t)b * max_peaks_per_sample, nb * sizeof(float));
-      D2H(h, out_channel_inds + total, g.ws.peak_ch + (size_t)b * max_peaks_per_sample, nb * sizeof(int));
-      for (int i = 0; i < nb; ++i) out_sample_inds[total + i] = b;
-    }
-    total += nb;
-    if (out_flags) out_flags[b] = flags[b];
-  }
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  *out_n_peaks = total;
-  return SB_OK;
+  if ((rc = sbk_local_peaks(h, d_cms, d_off, B, H, W, C, p, s.ws))) return rc;
+  return sb_peaks_to_host(h, s.ws, B, out_points, out_vals, out_channel_inds, out_sample_inds, out_n_peaks, out_flags);
 }
 
 int sb_find_global_peaks(sb_handle_t h, const float* cms_host, int B, int H, int W, int C,
@@ -172,28 +150,17 @@ int sb_find_global_peaks(sb_handle_t h, const float* cms_host, int B, int H, int
   if (!h) return sb_fail(nullptr, SB_ERR_INVALID, "null handle");
   if (B <= 0 || H <= 0 || W <= 0 || C <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_find_global_peaks: bad shape");
   SB_CUDA(h, cudaSetDevice(h->device));
+  SbScratch s(h);
   const size_t n = (size_t)B * H * W * C;
-  int rc;
-  DevBuf d_cms, d_off, d_part, d_pts, d_vals;
-  int target = (2 * h->sm_count + B - 1) / B;
-  int rpc = std::max(1, (H + target - 1) / target);
-  const int n_chunks = (H + rpc - 1) / rpc;
-  if ((rc = d_cms.alloc(h, n * sizeof(float)))) return rc;
-  if ((rc = d_part.alloc(h, (size_t)B * n_chunks * C * 3 * sizeof(float)))) return rc;
-  if ((rc = d_pts.alloc(h, (size_t)B * C * 2 * sizeof(float)))) return rc;
-  if ((rc = d_vals.alloc(h, (size_t)B * C * sizeof(float)))) return rc;
-  H2D(h, d_cms.p, cms_host, n * sizeof(float));
-  if (offsets_host) {
-    if ((rc = d_off.alloc(h, 2 * n * sizeof(float)))) return rc;
-    H2D(h, d_off.p, offsets_host, 2 * n * sizeof(float));
-  }
+  const float *d_cms, *d_off;
+  int rc = sb_global_scratch_alloc(h, s.gs, B, H, C);
+  if (rc || (rc = s.upload(cms_host, n, &d_cms)) || (rc = s.upload(offsets_host, 2 * n, &d_off, true))) return rc;
   SbPeakParams p{threshold, refinement, integral_patch_size, 1.0f, 1.0f};
-  if ((rc = sbk_global_peaks(h, d_cms.p, 0, offsets_host ? d_off.as<float>() : nullptr, B, H, W, C, p, nullptr,
-                             d_part.as<float>(), n_chunks, rpc, d_pts.as<float>(), d_vals.as<float>()))) return rc;
-  D2H(h, out_points, d_pts.p, (size_t)B * C * 2 * sizeof(float));
-  D2H(h, out_vals, d_vals.p, (size_t)B * C * sizeof(float));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  const SbGlobalScratch& g = s.gs;
+  if ((rc = sbk_global_peaks(h, d_cms, d_off, B, H, W, C, p, nullptr, g.part, g.chunks, g.rpc, g.points, g.vals)) ||
+      (rc = s.to_host(out_points, g.points, (size_t)B * C * 2)) || (rc = s.to_host(out_vals, g.vals, (size_t)B * C)))
+    return rc;
+  return s.sync();
 }
 
 int sb_crop_centered(sb_handle_t h, const void* images_host, int images_are_u8, int B, int H, int W,
@@ -204,24 +171,25 @@ int sb_crop_centered(sb_handle_t h, const void* images_host, int images_are_u8, 
   SB_CUDA(h, cudaSetDevice(h->device));
   const size_t esz = images_are_u8 ? 1 : 4;
   const size_t nimg = (size_t)B * H * W * C * esz, nout = (size_t)n * crop_h * crop_w * C * esz;
+  SbScratch s(h);
+  const uint8_t* d_img;
+  const float* d_c;
+  const int* d_s;
+  uint8_t* d_out;
   int rc;
-  DevBuf d_img, d_c, d_s, d_out;
-  if ((rc = d_img.alloc(h, nimg)) || (rc = d_c.alloc(h, (size_t)n * 2 * sizeof(float))) ||
-      (rc = d_s.alloc(h, (size_t)n * sizeof(int))) || (rc = d_out.alloc(h, nout))) return rc;
-  H2D(h, d_img.p, images_host, nimg);
-  H2D(h, d_c.p, centroids, (size_t)n * 2 * sizeof(float));
-  H2D(h, d_s.p, sample_inds, (size_t)n * sizeof(int));
-  if ((rc = sbk_crop(h, d_img.p, images_are_u8, B, H, W, C, d_c.as<float>(), d_s.as<int>(), n, crop_h, crop_w,
-                     d_out.p, images_are_u8))) return rc;
-  D2H(h, out_crops, d_out.p, nout);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  if ((rc = s.upload((const uint8_t*)images_host, nimg, &d_img)) || (rc = s.upload(centroids, (size_t)n * 2, &d_c)) ||
+      (rc = s.upload(sample_inds, (size_t)n, &d_s)) || (rc = s.alloc(&d_out, nout)) ||
+      (rc = sbk_crop(h, d_img, images_are_u8, B, H, W, C, d_c, d_s, n, crop_h, crop_w, d_out, images_are_u8)) ||
+      (rc = s.to_host((uint8_t*)out_crops, d_out, nout)))
+    return rc;
+  return s.sync();
 }
 
 // Builds the per-node ascending peak lists on the host (stable argsort by channel,
 // paf_grouping.py:106-109) for the stage-level calls that receive caller-supplied peaks.
-static int upload_peaks(sb_handle_s* h, SbPostWs& ws, int B, int n_nodes, const float* peaks,
-                        const float* peak_vals, const int32_t* ch, const int32_t* off) {
+static int upload_peaks(SbScratch& s, int B, int n_nodes, const float* peaks, const float* peak_vals, const int32_t* ch,
+                        const int32_t* off) {
+  SbPostWs& ws = s.ws;
   const int K = ws.max_node_peaks, MP = ws.max_peaks;
   std::vector<float> pk((size_t)B * MP * 2, 0.f), pv((size_t)B * MP, 0.f);
   std::vector<int> cnt((size_t)B * n_nodes, 0), lst((size_t)B * n_nodes * K, 0), np(B, 0);
@@ -233,20 +201,19 @@ static int upload_peaks(sb_handle_s* h, SbPostWs& ws, int B, int n_nodes, const 
       pk[((size_t)b * MP + i) * 2 + 1] = peaks[2 * (size_t)(off[b] + i) + 1];
       if (peak_vals) pv[(size_t)b * MP + i] = peak_vals[off[b] + i];
       const int c = ch[off[b] + i];
-      if (c < 0 || c >= n_nodes) return sb_fail(h, SB_ERR_INVALID, "peak channel %d out of range", c);
+      if (c < 0 || c >= n_nodes) return sb_fail(s.h, SB_ERR_INVALID, "peak channel %d out of range", c);
       int& k = cnt[(size_t)b * n_nodes + c];
       lst[((size_t)b * n_nodes + c) * K + k] = i;
       ++k;
     }
   }
-  H2D(h, ws.peaks, pk.data(), pk.size() * sizeof(float));
-  H2D(h, ws.peak_vals, pv.data(), pv.size() * sizeof(float));
-  H2D(h, ws.node_cnt, cnt.data(), cnt.size() * sizeof(int));
-  H2D(h, ws.node_peaks, lst.data(), lst.size() * sizeof(int));
-  H2D(h, ws.n_peaks, np.data(), np.size() * sizeof(int));
-  SB_CUDA(h, cudaMemsetAsync(ws.flags, 0, B * sizeof(int), h->stream));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return 0;
+  int rc;
+  if ((rc = s.to_dev(ws.peaks, pk.data(), pk.size())) || (rc = s.to_dev(ws.peak_vals, pv.data(), pv.size())) ||
+      (rc = s.to_dev(ws.node_cnt, cnt.data(), cnt.size())) || (rc = s.to_dev(ws.node_peaks, lst.data(), lst.size())) ||
+      (rc = s.to_dev(ws.n_peaks, np.data(), np.size())))
+    return rc;
+  SB_CUDA(s.h, cudaMemsetAsync(ws.flags, 0, B * sizeof(int), s.h->stream));
+  return s.sync();
 }
 
 static void node_caps(int B, int n_nodes, const int32_t* ch, const int32_t* off, int* max_peaks, int* max_node) {
@@ -273,46 +240,21 @@ int sb_score_paf_lines_batch(sb_handle_t h, const float* pafs_host, int B, int H
   SB_CUDA(h, cudaSetDevice(h->device));
   int MP, K;
   node_caps(B, n_nodes, peak_channel_inds, peak_offsets, &MP, &K);
-  WsGuard g;
-  int rc = sb_post_ws_alloc(h, g.ws, B, 1, 1, n_nodes, MP, K, 1, n_edges);
-  if (rc) return rc;
-  if ((rc = upload_peaks(h, g.ws, B, n_nodes, peaks, nullptr, peak_channel_inds, peak_offsets))) return rc;
-  H2D(h, g.ws.edges_dev, skeleton_edges, (size_t)n_edges * 2 * sizeof(int));
-  DevBuf d_pafs;
-  const size_t npaf = (size_t)B * Hp * Wp * C2;
-  if ((rc = d_pafs.alloc(h, npaf * sizeof(float)))) return rc;
-  H2D(h, d_pafs.p, pafs_host, npaf * sizeof(float));
+  SbScratch s(h);
+  const float* d_pafs;
+  int rc = sb_post_ws_alloc(h, s.ws, B, 1, 1, n_nodes, MP, K, 1, n_edges);
+  if (rc || (rc = upload_peaks(s, B, n_nodes, peaks, nullptr, peak_channel_inds, peak_offsets)) ||
+      (rc = s.to_dev(s.ws.edges_dev, skeleton_edges, (size_t)n_edges * 2)) ||
+      (rc = s.upload(pafs_host, (size_t)B * Hp * Wp * C2, &d_pafs)))
+    return rc;
   // max_edge_length = ratio * max(Hp, Wp, C2) * stride  (paf_grouping.py:469-473), in f32
   const float max_len = max_edge_length_ratio * (float)std::max(std::max(Hp, Wp), C2) * (float)pafs_stride;
-  if ((rc = sbk_score_match(h, d_pafs.as<float>(), B, Hp, Wp, C2, n_line_points, pafs_stride, max_len,
-                            dist_penalty_weight, g.ws))) return rc;
-  std::vector<float> mat((size_t)B * n_edges * K * K);
-  D2H(h, mat.data(), g.ws.score_mat, mat.size() * sizeof(float));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  // flatten: (sample, edge, src-major) using the same node lists
-  int total = 0;
-  std::vector<std::vector<int>> lists(n_nodes);
-  for (int b = 0; b < B; ++b) {
-    out_cand_offsets[b] = total;
-    for (auto& l : lists) l.clear();
-    for (int i = peak_offsets[b]; i < peak_offsets[b + 1]; ++i) lists[peak_channel_inds[i]].push_back(i - peak_offsets[b]);
-    for (int e = 0; e < n_edges; ++e) {
-      const auto& s = lists[skeleton_edges[2 * e]];
-      const auto& d = lists[skeleton_edges[2 * e + 1]];
-      const int nd = (int)d.size();
-      for (size_t i = 0; i < s.size(); ++i)
-        for (int j = 0; j < nd; ++j) {
-          if (total >= cap) return sb_fail(h, SB_ERR_INVALID, "candidate capacity %d exceeded", cap);
-          out_edge_inds[total] = e;
-          out_edge_peak_inds[2 * total] = s[i];
-          out_edge_peak_inds[2 * total + 1] = d[j];
-          out_line_scores[total] = mat[((size_t)b * n_edges + e) * K * K + i * nd + j];
-          ++total;
-        }
-    }
-  }
-  out_cand_offsets[B] = total;
-  return SB_OK;
+  SbGraphHost g;
+  if ((rc = sbk_score_match(h, d_pafs, B, Hp, Wp, C2, n_line_points, pafs_stride, max_len, dist_penalty_weight, s.ws)) ||
+      (rc = s.sync()) || (rc = sb_graph_download(h, s.ws, B, g)))
+    return rc;
+  // the node lists are the ones upload_peaks built: (sample, edge, src-major) order
+  return sb_graph_flatten(h, s.ws, g, skeleton_edges, B, cap, out_edge_inds, out_edge_peak_inds, out_line_scores, out_cand_offsets);
 }
 
 int sb_paf_lines(sb_handle_t h, const float* pafs_sample, int Hp, int Wp, int C2,
@@ -326,32 +268,23 @@ int sb_paf_lines(sb_handle_t h, const float* pafs_sample, int Hp, int Wp, int C2
   for (int i = 0; i < 2 * n; ++i)
     if (edge_peak_inds[i] < 0 || edge_peak_inds[i] >= n_peaks) return sb_fail(h, SB_ERR_INVALID, "peak index out of range");
   SB_CUDA(h, cudaSetDevice(h->device));
-  int rc;
   const size_t P = n_line_points;
-  DevBuf d_paf, d_lin, d_pk, d_epi, d_ei, d_subs, d_ol, d_os;
-  if (pafs_sample) {
-    if ((rc = d_paf.alloc(h, (size_t)Hp * Wp * C2 * 4))) return rc;
-    H2D(h, d_paf.p, pafs_sample, (size_t)Hp * Wp * C2 * 4);
-  }
-  if (lines_in) {
-    if ((rc = d_lin.alloc(h, (size_t)n * P * 2 * 4))) return rc;
-    H2D(h, d_lin.p, lines_in, (size_t)n * P * 2 * 4);
-  }
-  if ((rc = d_pk.alloc(h, (size_t)n_peaks * 2 * 4)) || (rc = d_epi.alloc(h, (size_t)n * 2 * 4)) ||
-      (rc = d_ei.alloc(h, (size_t)n * 4)) || (rc = d_subs.alloc(h, (size_t)n * P * 2 * 4)) ||
-      (rc = d_ol.alloc(h, (size_t)n * P * 2 * 4)) || (rc = d_os.alloc(h, (size_t)n * 4))) return rc;
-  H2D(h, d_pk.p, peaks, (size_t)n_peaks * 2 * 4);
-  H2D(h, d_epi.p, edge_peak_inds, (size_t)n * 2 * 4);
-  if (edge_inds) H2D(h, d_ei.p, edge_inds, (size_t)n * 4);
-  if ((rc = sbk_lines(h, pafs_sample ? d_paf.as<float>() : nullptr, Hp, Wp, C2, lines_in ? d_lin.as<float>() : nullptr,
-                      d_pk.as<float>(), d_epi.as<int>(), edge_inds ? d_ei.as<int>() : nullptr, n, n_line_points,
-                      (float)pafs_stride, max_edge_length, dist_penalty_weight, d_subs.as<int>(), d_ol.as<float>(),
-                      d_os.as<float>()))) return rc;
-  if (out_subs) D2H(h, out_subs, d_subs.p, (size_t)n * P * 2 * 4);
-  if (out_lines) D2H(h, out_lines, d_ol.p, (size_t)n * P * 2 * 4);
-  if (out_scores) D2H(h, out_scores, d_os.p, (size_t)n * 4);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  SbScratch s(h);
+  const float *d_paf, *d_lin, *d_pk;
+  const int *d_epi, *d_ei;
+  int* d_subs;
+  float *d_ol, *d_os;
+  int rc;
+  if ((rc = s.upload(pafs_sample, (size_t)Hp * Wp * C2, &d_paf, true)) || (rc = s.upload(lines_in, n * P * 2, &d_lin, true)) ||
+      (rc = s.upload(peaks, (size_t)n_peaks * 2, &d_pk)) || (rc = s.upload(edge_peak_inds, (size_t)n * 2, &d_epi)) ||
+      (rc = s.upload(edge_inds, (size_t)n, &d_ei, true)) || (rc = s.alloc(&d_subs, n * P * 2)) ||
+      (rc = s.alloc(&d_ol, n * P * 2)) || (rc = s.alloc(&d_os, (size_t)n)) ||
+      (rc = sbk_lines(h, d_paf, Hp, Wp, C2, d_lin, d_pk, d_epi, d_ei, n, n_line_points, (float)pafs_stride, max_edge_length,
+                      dist_penalty_weight, d_subs, d_ol, d_os)) ||
+      (rc = s.to_host(out_subs, d_subs, n * P * 2, true)) || (rc = s.to_host(out_lines, d_ol, n * P * 2, true)) ||
+      (rc = s.to_host(out_scores, d_os, (size_t)n, true)))
+    return rc;
+  return s.sync();
 }
 
 int sb_integral_regression(sb_handle_t h, const float* cms, int N, int Hh, int Ww, int C,
@@ -359,19 +292,17 @@ int sb_integral_regression(sb_handle_t h, const float* cms, int N, int Hh, int W
   if (!h) return sb_fail(nullptr, SB_ERR_INVALID, "null handle");
   if (N <= 0) return SB_OK;
   SB_CUDA(h, cudaSetDevice(h->device));
-  int rc;
-  DevBuf d_c, d_x, d_y, d_ox, d_oy;
+  SbScratch s(h);
+  const float *d_c, *d_x, *d_y;
+  float *d_ox, *d_oy;
   const size_t n = (size_t)N * Hh * Ww * C;
-  if ((rc = d_c.alloc(h, n * 4)) || (rc = d_x.alloc(h, Ww * 4)) || (rc = d_y.alloc(h, Hh * 4)) ||
-      (rc = d_ox.alloc(h, (size_t)N * C * 4)) || (rc = d_oy.alloc(h, (size_t)N * C * 4))) return rc;
-  H2D(h, d_c.p, cms, n * 4);
-  H2D(h, d_x.p, xv, Ww * 4);
-  H2D(h, d_y.p, yv, Hh * 4);
-  if ((rc = sbk_integral(h, d_c.as<float>(), N, Hh, Ww, C, d_x.as<float>(), d_y.as<float>(), d_ox.as<float>(), d_oy.as<float>()))) return rc;
-  D2H(h, x_hat, d_ox.p, (size_t)N * C * 4);
-  D2H(h, y_hat, d_oy.p, (size_t)N * C * 4);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  int rc;
+  if ((rc = s.upload(cms, n, &d_c)) || (rc = s.upload(xv, (size_t)Ww, &d_x)) || (rc = s.upload(yv, (size_t)Hh, &d_y)) ||
+      (rc = s.alloc(&d_ox, (size_t)N * C)) || (rc = s.alloc(&d_oy, (size_t)N * C)) ||
+      (rc = sbk_integral(h, d_c, N, Hh, Ww, C, d_x, d_y, d_ox, d_oy)) ||
+      (rc = s.to_host(x_hat, d_ox, (size_t)N * C)) || (rc = s.to_host(y_hat, d_oy, (size_t)N * C)))
+    return rc;
+  return s.sync();
 }
 
 int sb_find_offsets_local_direction(sb_handle_t h, const float* patches, int N, float delta,
@@ -379,14 +310,14 @@ int sb_find_offsets_local_direction(sb_handle_t h, const float* patches, int N, 
   if (!h) return sb_fail(nullptr, SB_ERR_INVALID, "null handle");
   if (N <= 0) return SB_OK;
   SB_CUDA(h, cudaSetDevice(h->device));
+  SbScratch s(h);
+  const float* d_p;
+  float* d_o;
   int rc;
-  DevBuf d_p, d_o;
-  if ((rc = d_p.alloc(h, (size_t)N * 9 * 4)) || (rc = d_o.alloc(h, (size_t)N * 2 * 4))) return rc;
-  H2D(h, d_p.p, patches, (size_t)N * 9 * 4);
-  if ((rc = sbk_local_dir(h, d_p.as<float>(), N, delta, d_o.as<float>()))) return rc;
-  D2H(h, out_offsets, d_o.p, (size_t)N * 2 * 4);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  if ((rc = s.upload(patches, (size_t)N * 9, &d_p)) || (rc = s.alloc(&d_o, (size_t)N * 2)) ||
+      (rc = sbk_local_dir(h, d_p, N, delta, d_o)) || (rc = s.to_host(out_offsets, d_o, (size_t)N * 2)))
+    return rc;
+  return s.sync();
 }
 
 int sb_linear_sum_assignment_batch(sb_handle_t h, const float* scores, const int32_t* n_src,
@@ -401,24 +332,21 @@ int sb_linear_sum_assignment_batch(sb_handle_t h, const float* scores, const int
     if (n_src[p] > max_k || n_dst[p] > max_k) return sb_fail(h, SB_ERR_INVALID, "problem %d exceeds max_k", p);
     total = std::max(total, (size_t)offsets[p] + (size_t)n_src[p] * n_dst[p]);
   }
-  int rc;
-  DevBuf d_sc, d_ns, d_nd, d_of, d_r, d_c, d_s, d_n;
+  SbScratch s(h);
+  const float* d_sc;
+  const int *d_ns, *d_nd, *d_of;
+  int *d_r, *d_c, *d_n;
+  float* d_s;
   const size_t np = (size_t)n_problems;
-  if ((rc = d_sc.alloc(h, total * sizeof(float))) || (rc = d_ns.alloc(h, np * 4)) || (rc = d_nd.alloc(h, np * 4)) ||
-      (rc = d_of.alloc(h, np * 4)) || (rc = d_r.alloc(h, np * max_k * 4)) || (rc = d_c.alloc(h, np * max_k * 4)) ||
-      (rc = d_s.alloc(h, np * max_k * 4)) || (rc = d_n.alloc(h, np * 4))) return rc;
-  H2D(h, d_sc.p, scores, total * sizeof(float));
-  H2D(h, d_ns.p, n_src, np * 4);
-  H2D(h, d_nd.p, n_dst, np * 4);
-  H2D(h, d_of.p, offsets, np * 4);
-  if ((rc = sbk_lsap_batch(h, d_sc.as<float>(), d_ns.as<int>(), d_nd.as<int>(), d_of.as<int>(), n_problems, max_k,
-                           d_r.as<int>(), d_c.as<int>(), d_s.as<float>(), d_n.as<int>()))) return rc;
-  D2H(h, out_rows, d_r.p, np * max_k * 4);
-  D2H(h, out_cols, d_c.p, np * max_k * 4);
-  D2H(h, out_scores, d_s.p, np * max_k * 4);
-  D2H(h, out_counts, d_n.p, np * 4);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  int rc;
+  if ((rc = s.upload(scores, total, &d_sc)) || (rc = s.upload(n_src, np, &d_ns)) || (rc = s.upload(n_dst, np, &d_nd)) ||
+      (rc = s.upload(offsets, np, &d_of)) || (rc = s.alloc(&d_r, np * max_k)) || (rc = s.alloc(&d_c, np * max_k)) ||
+      (rc = s.alloc(&d_s, np * max_k)) || (rc = s.alloc(&d_n, np)) ||
+      (rc = sbk_lsap_batch(h, d_sc, d_ns, d_nd, d_of, n_problems, max_k, d_r, d_c, d_s, d_n)) ||
+      (rc = s.to_host(out_rows, d_r, np * max_k)) || (rc = s.to_host(out_cols, d_c, np * max_k)) ||
+      (rc = s.to_host(out_scores, d_s, np * max_k)) || (rc = s.to_host(out_counts, d_n, np)))
+    return rc;
+  return s.sync();
 }
 
 int sb_group_instances_batch(sb_handle_t h, int B, int n_nodes, const float* peaks,
@@ -445,10 +373,10 @@ int sb_group_instances_batch(sb_handle_t h, int B, int n_nodes, const float* pea
       K = std::max(K, ++ecnt[(size_t)b * n_edges + e]);
       K = std::max(K, std::max(match_src_peak_inds[m], match_dst_peak_inds[m]) + 1);
     }
-  WsGuard g;
-  int rc = sb_post_ws_alloc(h, g.ws, B, 1, 1, n_nodes, MP, K, max_instances, n_edges);
-  if (rc) return rc;
-  if ((rc = upload_peaks(h, g.ws, B, n_nodes, peaks, peak_vals, peak_channel_inds, peak_offsets))) return rc;
+  SbScratch s(h);
+  SbPostWs& ws = s.ws;
+  int rc = sb_post_ws_alloc(h, ws, B, 1, 1, n_nodes, MP, K, max_instances, n_edges);
+  if (rc || (rc = upload_peaks(s, B, n_nodes, peaks, peak_vals, peak_channel_inds, peak_offsets))) return rc;
   std::vector<int> msrc((size_t)B * n_edges * K, 0), mdst((size_t)B * n_edges * K, 0);
   std::vector<float> msc((size_t)B * n_edges * K, 0.f);
   std::fill(ecnt.begin(), ecnt.end(), 0);
@@ -462,22 +390,20 @@ int sb_group_instances_batch(sb_handle_t h, int B, int n_nodes, const float* pea
       msc[o] = match_line_scores[m];
       ++k;
     }
-  H2D(h, g.ws.match_cnt, ecnt.data(), ecnt.size() * 4);
-  H2D(h, g.ws.match_src, msrc.data(), msrc.size() * 4);
-  H2D(h, g.ws.match_dst, mdst.data(), mdst.size() * 4);
-  H2D(h, g.ws.match_score, msc.data(), msc.size() * 4);
-  H2D(h, g.ws.edges_dev, edge_types, (size_t)n_edges * 2 * 4);
+  if ((rc = s.to_dev(ws.match_cnt, ecnt.data(), ecnt.size())) || (rc = s.to_dev(ws.match_src, msrc.data(), msrc.size())) ||
+      (rc = s.to_dev(ws.match_dst, mdst.data(), mdst.size())) || (rc = s.to_dev(ws.match_score, msc.data(), msc.size())) ||
+      (rc = s.to_dev(ws.edges_dev, edge_types, (size_t)n_edges * 2)))
+    return rc;
   if (n_sorted > n_edges) return sb_fail(h, SB_ERR_INVALID, "n_sorted > n_edges");
-  if (n_sorted > 0) H2D(h, g.ws.sorted_edges_dev, sorted_edge_inds, (size_t)n_sorted * 4);
-  g.ws.n_sorted = n_sorted;
+  if (n_sorted > 0 && (rc = s.to_dev(ws.sorted_edges_dev, sorted_edge_inds, (size_t)n_sorted))) return rc;
+  ws.n_sorted = n_sorted;
   // Note: stage-level peaks lists hold *all* peaks of a node, so node_cnt >= every local index.
-  if ((rc = sbk_group(h, B, n_nodes, min_instance_peaks, min_line_scores, 1.0f, g.ws))) return rc;
-  D2H(h, out_instances, g.ws.inst_peaks, (size_t)B * max_instances * n_nodes * 2 * 4);
-  D2H(h, out_peak_scores, g.ws.inst_vals, (size_t)B * max_instances * n_nodes * 4);
-  D2H(h, out_instance_scores, g.ws.inst_scores, (size_t)B * max_instances * 4);
-  D2H(h, out_n_instances, g.ws.n_inst, (size_t)B * 4);
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return SB_OK;
+  const size_t I = max_instances;
+  if ((rc = sbk_group(h, B, n_nodes, min_instance_peaks, min_line_scores, 1.0f, ws)) ||
+      (rc = s.to_host(out_instances, ws.inst_peaks, B * I * n_nodes * 2)) || (rc = s.to_host(out_peak_scores, ws.inst_vals, B * I * n_nodes)) ||
+      (rc = s.to_host(out_instance_scores, ws.inst_scores, B * I)) || (rc = s.to_host(out_n_instances, ws.n_inst, (size_t)B)))
+    return rc;
+  return s.sync();
 }
 
 }  // extern "C"

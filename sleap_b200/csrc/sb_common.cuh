@@ -153,10 +153,10 @@ struct SbPeakParams {
   float input_scale;   // != 1: then / input_scale + 0.5 (centroid / single-instance paths)
 };
 
-int sbk_local_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const float* offsets,
-                    int B, int H, int W, int C, const SbPeakParams& p, SbPostWs& ws);
-int sbk_global_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const float* offsets,
-                     int B, int H, int W, int C, const SbPeakParams& p,
+// Confidence maps (and learned offsets) are fp32 NHWC: head outputs are always fp32.
+int sbk_local_peaks(sb_handle_s* h, const float* cms, const float* offsets, int B, int H, int W, int C,
+                    const SbPeakParams& p, SbPostWs& ws);
+int sbk_global_peaks(sb_handle_s* h, const float* cms, const float* offsets, int B, int H, int W, int C, const SbPeakParams& p,
                      const float* crop_off_dev, float* part_buf, int n_chunks, int rows_per_chunk,
                      float* out_points, float* out_vals);
 int sbk_score_match(sb_handle_s* h, const float* pafs, int B, int Hp, int Wp, int C2,
@@ -186,6 +186,88 @@ int sbk_local_dir(sb_handle_s* h, const float* patches, int N, float delta, floa
 int sb_post_ws_alloc(sb_handle_s* h, SbPostWs& ws, int B, int H, int W, int C, int max_peaks,
                      int max_node_peaks, int max_instances, int n_edges);
 void sb_post_ws_free(SbPostWs& ws);
+
+// Global-peak scratch for B frames of (H, C) maps: the partial maxima of ceil(2 * SMs / B) row chunks per frame, the
+// points, values and crop offsets (sb_model.cu)
+struct SbGlobalScratch {
+  float *part = nullptr, *points = nullptr, *vals = nullptr, *crop_off = nullptr;
+  int rpc = 1, chunks = 1;   // rows per chunk of the partial maxima, chunks per frame
+};
+int sb_global_scratch_alloc(sb_handle_s* h, SbGlobalScratch& g, int B, int H, int C);
+void sb_global_scratch_free(SbGlobalScratch& g);
+
+// Copies the peak lists of ws's first B frames into caller arrays, concatenated in frame order: points, values, channel
+// indices (NULL: not wanted) and frame indices; per-frame flags (NULL: not wanted); *out_n = the number of peaks (sb_api.cu)
+int sb_peaks_to_host(sb_handle_s* h, const SbPostWs& ws, int B, float* out_points, float* out_vals, int32_t* out_channel_inds,
+                     int32_t* out_sample_inds, int32_t* out_n, int32_t* out_flags);
+
+// Host copies of ws's per-frame PAF candidates (sb_model.cu): peak counts [B], node counts [B][C], node lists [B][C][K]
+// and score matrices [B][E][K*K].  sb_graph_download needs the work that wrote them finished.
+struct SbGraphHost {
+  std::vector<int> n_peaks, node_cnt, node_peaks;
+  std::vector<float> score_mat;
+};
+int sb_graph_download(sb_handle_s* h, const SbPostWs& ws, int B, SbGraphHost& g);
+// The candidates in (frame, edge, src, dst) order: edge index, (src, dst) peak indices within the frame and line score each;
+// cand_offsets[B + 1] the first candidate of every frame
+int sb_graph_flatten(sb_handle_s* h, const SbPostWs& ws, const SbGraphHost& g, const int* edges_host, int B, int cap,
+                     int32_t* edge_inds, int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets);
+
+// The scratch of a call that takes or returns caller (host) arrays, freed when the call returns: a post-processing
+// workspace, a global-peak scratch and device buffers.  Copies are queued on the handle's stream.
+struct SbScratch {
+  sb_handle_s* h;
+  SbPostWs ws;
+  SbGlobalScratch gs;
+  std::vector<void*> bufs;
+  explicit SbScratch(sb_handle_s* handle) : h(handle) {}
+  SbScratch(const SbScratch&) = delete;
+  SbScratch& operator=(const SbScratch&) = delete;
+  ~SbScratch() {
+    sb_post_ws_free(ws);
+    sb_global_scratch_free(gs);
+    for (void* q : bufs) cudaFree(q);
+  }
+  template <typename T> int alloc(T** dev, size_t n) {      // a device buffer of n elements
+    void* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, n * sizeof(T) + 16);
+    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc(%zu): %s", n * sizeof(T), cudaGetErrorString(e));
+    bufs.push_back(q);
+    *dev = (T*)q;
+    return 0;
+  }
+  // a device copy of n elements of `host`; an optional input that is NULL: *dev = NULL
+  template <typename T> int upload(const T* host, size_t n, const T** dev, bool optional = false) {
+    *dev = nullptr;
+    T* q;
+    if (optional && !host) return 0;
+    if (const int rc = alloc(&q, n)) return rc;
+    *dev = q;
+    return to_dev(q, host, n);
+  }
+  template <typename T> int to_dev(T* dev, const T* host, size_t n) {
+    SB_CUDA(h, cudaMemcpyAsync(dev, host, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+    return 0;
+  }
+  // an optional output that is NULL: nothing
+  template <typename T> int to_host(T* host, const T* dev, size_t n, bool optional = false) {
+    if (!optional || host) SB_CUDA(h, cudaMemcpyAsync(host, dev, n * sizeof(T), cudaMemcpyDeviceToHost, h->stream));
+    return 0;
+  }
+  int sync() {
+    SB_CUDA(h, cudaStreamSynchronize(h->stream));
+    return 0;
+  }
+};
+
+// Splits B fixed-width per-frame records into caller arrays: the float fields in record order (destination, floats per
+// frame), then one float per frame for each int field, cast to int32.  A NULL destination skips its field (sb_model.cu).
+struct SbRecField {
+  float* dst;
+  size_t n;
+};
+void sb_split_records(const float* rec, int B, size_t width, std::initializer_list<SbRecField> floats,
+                      std::initializer_list<int32_t*> ints);
 
 // ---- frame preprocessing shared by k_preprocess and the fused first-layer / stem view kernels ----
 // caffe mean of BGR channel c (resnet.py imagenet_preproc_v1)

@@ -26,12 +26,23 @@ int grid_for(size_t total, int sm) {
 
 int build_programs(sb_handle_s* h, SbModel* m);   // the last step of sb_model_configure (below, with the op slots)
 
-void global_scratch_free(SbGlobalScratch& g) {
+}  // namespace
+
+void sb_global_scratch_free(SbGlobalScratch& g) {
   for (float* p : {g.part, g.points, g.vals, g.crop_off}) if (p) cudaFree(p);
   g = SbGlobalScratch();
 }
 
-}  // namespace
+int sb_global_scratch_alloc(sb_handle_s* h, SbGlobalScratch& g, int B, int H, int C) {
+  const int target = (2 * h->sm_count + B - 1) / B;
+  g.rpc = std::max(1, (H + target - 1) / target);
+  g.chunks = (H + g.rpc - 1) / g.rpc;
+  SB_CUDA(h, cudaMalloc((void**)&g.part, (size_t)B * g.chunks * C * 3 * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.points, (size_t)B * C * 2 * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.vals, (size_t)B * C * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.crop_off, (size_t)B * 2 * 4));
+  return 0;
+}
 
 void sb_models_free(sb_handle_s* h) {
   for (SbModel* m : h->models) {
@@ -40,7 +51,7 @@ void sb_models_free(sb_handle_s* h) {
     if (m->weights_dev) cudaFree(m->weights_dev);
     if (m->weights_tc_dev) cudaFree(m->weights_tc_dev);
     if (m->frames_dev) cudaFree(m->frames_dev);
-    global_scratch_free(m->gs);
+    sb_global_scratch_free(m->gs);
     if (m->rec_host) cudaFreeHost(m->rec_host);
     if (m->trk_dev) cudaFree(m->trk_dev);
     for (int i = 0; i < 3; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
@@ -91,7 +102,7 @@ static int chain_drop(sb_handle_s* h, SbModel* m) {
   sb_pipeline_slots_free(m);                     // staging is sized from the chain's record width
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes)
   m->trk = nullptr;                              // its checks (nodes, instance capacity) were made against the old chain
-  global_scratch_free(m->gs);
+  sb_global_scratch_free(m->gs);
   sb_topdown_free(m);
   m->chain = SB_CHAIN_NONE;
   ++m->chain_gen;
@@ -587,6 +598,57 @@ static int check_class_params(sb_handle_s* h, const sb_multiclass_params* p) {
   return 0;
 }
 
+// ---- host copies of the results (sb_common.cuh) ----
+void sb_split_records(const float* rec, int B, size_t width, std::initializer_list<SbRecField> floats,
+                      std::initializer_list<int32_t*> ints) {
+  for (int b = 0; b < B; ++b) {
+    const float* r = rec + (size_t)b * width;
+    for (const SbRecField& f : floats) {
+      if (f.dst) memcpy(f.dst + (size_t)b * f.n, r, f.n * sizeof(float));
+      r += f.n;
+    }
+    for (int32_t* d : ints) {
+      if (d) d[b] = (int32_t)*r;
+      ++r;
+    }
+  }
+}
+
+int sb_graph_download(sb_handle_s* h, const SbPostWs& ws, int B, SbGraphHost& g) {
+  const size_t nodes = (size_t)B * ws.C, K = ws.max_node_peaks;
+  g.n_peaks.resize(B); g.node_cnt.resize(nodes); g.node_peaks.resize(nodes * K);
+  g.score_mat.resize((size_t)B * ws.n_edges * K * K);
+  SB_CUDA(h, cudaMemcpy(g.n_peaks.data(), ws.n_peaks, (size_t)B * 4, cudaMemcpyDeviceToHost));
+  SB_CUDA(h, cudaMemcpy(g.node_cnt.data(), ws.node_cnt, g.node_cnt.size() * 4, cudaMemcpyDeviceToHost));
+  SB_CUDA(h, cudaMemcpy(g.node_peaks.data(), ws.node_peaks, g.node_peaks.size() * 4, cudaMemcpyDeviceToHost));
+  SB_CUDA(h, cudaMemcpy(g.score_mat.data(), ws.score_mat, g.score_mat.size() * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int sb_graph_flatten(sb_handle_s* h, const SbPostWs& ws, const SbGraphHost& g, const int* edges_host, int B, int cap,
+                     int32_t* edge_inds, int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets) {
+  const int C = ws.C, K = ws.max_node_peaks, E = ws.n_edges;
+  int tc = 0;
+  for (int b = 0; b < B; ++b) {
+    cand_offsets[b] = tc;
+    for (int e = 0; e < E; ++e) {
+      const int sn = edges_host[2 * e], dn = edges_host[2 * e + 1];
+      const int ns = std::min(g.node_cnt[(size_t)b * C + sn], K), nd = std::min(g.node_cnt[(size_t)b * C + dn], K);
+      for (int i = 0; i < ns; ++i)
+        for (int j = 0; j < nd; ++j) {
+          if (tc >= cap) return sb_fail(h, SB_ERR_INVALID, "candidate capacity %d exceeded", cap);
+          edge_inds[tc] = e;
+          edge_peak_inds[2 * tc] = g.node_peaks[((size_t)b * C + sn) * K + i];
+          edge_peak_inds[2 * tc + 1] = g.node_peaks[((size_t)b * C + dn) * K + j];
+          line_scores[tc] = g.score_mat[((size_t)b * E + e) * K * K + (size_t)i * nd + j];
+          ++tc;
+        }
+    }
+  }
+  cand_offsets[B] = tc;
+  return SB_OK;
+}
+
 extern "C" {
 
 int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params* p) {
@@ -661,17 +723,12 @@ static int check_exchange(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
-static void unpack_records(const SbModel* m, const float* rec, int B, float* out_instance_peaks, float* out_instance_peak_vals,
-                           float* out_instance_scores, int32_t* out_n_valid, int32_t* out_flags) {
-  const size_t I = m->bu.max_instances, C = m->bu.n_nodes, w = sb_record_width((int)I, (int)C);
-  for (int b = 0; b < B; ++b) {
-    const float* r = rec + (size_t)b * w;
-    memcpy(out_instance_peaks + (size_t)b * I * C * 2, r, I * C * 2 * sizeof(float));
-    memcpy(out_instance_peak_vals + (size_t)b * I * C, r + I * C * 2, I * C * sizeof(float));
-    memcpy(out_instance_scores + (size_t)b * I, r + I * C * 3, I * sizeof(float));
-    out_n_valid[b] = (int32_t)r[I * C * 3 + I];
-    if (out_flags) out_flags[b] = (int32_t)r[I * C * 3 + I + 1];
-  }
+// A PAF-chain record: peaks | peak values | instance scores | n_valid | flags
+static void split_paf_records(const SbModel* m, const float* rec, int B, float* out_instance_peaks, float* out_instance_peak_vals,
+                              float* out_instance_scores, int32_t* out_n_valid, int32_t* out_flags) {
+  const size_t I = m->bu.max_instances, C = m->bu.n_nodes;
+  sb_split_records(rec, B, record_width(m), {{out_instance_peaks, I * C * 2}, {out_instance_peak_vals, I * C}, {out_instance_scores, I}},
+                   {out_n_valid, out_flags});
 }
 
 // The PAF chain: local peaks, PAF scoring and matching, grouping into ws's instance arrays and records (and, gx given,
@@ -679,7 +736,7 @@ static void unpack_records(const SbModel* m, const float* rec, int B, float* out
 static int bottomup_post_kernels(sb_handle_s* h, const sb_bottomup_params& p, SbPostWs& ws, const SbMap& cms, const SbMap& pafs,
                                  const float* off, int B, const SbGatherDev* gx = nullptr) {
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
-  int rc = sbk_local_peaks(h, cms.dev, 0, off, B, cms.H, cms.W, cms.C, pp, ws);
+  int rc = sbk_local_peaks(h, cms.dev, off, B, cms.H, cms.W, cms.C, pp, ws);
   if (rc) return rc;
   const float max_len = p.max_edge_length_ratio * (float)std::max(std::max(pafs.H, pafs.W), pafs.C) * (float)p.paf_output_stride;
   if ((rc = sbk_score_match(h, pafs.dev, B, pafs.H, pafs.W, pafs.C, p.n_line_points, p.paf_output_stride, max_len,
@@ -691,7 +748,7 @@ static int bottomup_post_kernels(sb_handle_s* h, const sb_bottomup_params& p, Sb
 static int multiclass_post_kernels(sb_handle_s* h, const sb_multiclass_params& p, SbPostWs& ws, const SbMap& cms,
                                    const SbMap& cls, const float* off, int B) {
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.cm_output_stride, 1.0f};
-  int rc = sbk_local_peaks(h, cms.dev, 0, off, B, cms.H, cms.W, cms.C, pp, ws);
+  int rc = sbk_local_peaks(h, cms.dev, off, B, cms.H, cms.W, cms.C, pp, ws);
   if (rc) return rc;
   return sbk_class_group(h, cls.dev, B, cls.H, cls.W, cls.C, (float)p.class_maps_output_stride, p.input_scale, ws);
 }
@@ -720,16 +777,12 @@ static int step_post_kernels(sb_handle_s* h, SbModel* m, int B) {
                         m->trk_cut, m->trk_h, m->trk_w, m->trk_dev);
 }
 
-static void unpack_class_records(const float* rec, size_t w, int B, int n_classes, int n_nodes, float* out_points,
-                                 float* out_vals, float* out_class_probs, int32_t* out_flags) {
-  const size_t n1 = (size_t)n_classes * n_nodes;
-  for (int b = 0; b < B; ++b) {
-    const float* r = rec + (size_t)b * w;
-    memcpy(out_points + (size_t)b * n1 * 2, r, n1 * 2 * sizeof(float));
-    memcpy(out_vals + (size_t)b * n1, r + n1 * 2, n1 * sizeof(float));
-    memcpy(out_class_probs + (size_t)b * n1, r + n1 * 3, n1 * sizeof(float));
-    if (out_flags) out_flags[b] = (int32_t)r[n1 * 4];
-  }
+// A multi-class record: points | values | class probabilities | flags
+static void split_class_records(const sb_multiclass_params& p, const float* rec, int B, float* out_points, float* out_vals,
+                                float* out_class_probs, int32_t* out_flags) {
+  const size_t n1 = (size_t)p.n_classes * p.n_nodes;
+  sb_split_records(rec, B, sb_class_record_width(p.n_classes, p.n_nodes), {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, n1}},
+                   {out_flags});
 }
 
 // The track records of a batch go to the host with its result records, on the same stream.
@@ -797,7 +850,7 @@ int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, i
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
   if (!m) return SB_ERR_INVALID;
   if (const int rc = step_sync(h, m, frames_host, 1, B)) return rc;
-  unpack_records(m, own_slice(m, m->rec_host, B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
+  split_paf_records(m, own_slice(m, m->rec_host, B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
   return SB_OK;
 }
 
@@ -807,7 +860,7 @@ int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, in
   if (!m) return SB_ERR_INVALID;
   if (!frames_host || !out_points || !out_vals || !out_class_probs) return sb_fail(h, SB_ERR_INVALID, "sb_infer_multiclass: null argument");
   if (const int rc = step_sync(h, m, frames_host, frames_are_u8 ? 1 : 0, B)) return rc;
-  unpack_class_records(m->rec_host, record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals, out_class_probs, out_flags);
+  split_class_records(m->mc, m->rec_host, B, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -884,7 +937,8 @@ int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
   if (!m) return SB_ERR_INVALID;
   if (const int rc = step_collect(h, m, slot, B)) return rc;
-  unpack_records(m, own_slice(m, m->stage_host[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
+  split_paf_records(m, own_slice(m, m->stage_host[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid,
+                    out_flags);
   return SB_OK;
 }
 
@@ -898,8 +952,7 @@ int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* o
   SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
   if (!m) return SB_ERR_INVALID;
   if (const int rc = step_collect(h, m, slot, B)) return rc;
-  unpack_class_records(m->stage_host[slot], record_width(m), B, m->mc.n_classes, m->mc.n_nodes, out_points, out_vals,
-                       out_class_probs, out_flags);
+  split_class_records(m->mc, m->stage_host[slot], B, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -985,46 +1038,29 @@ int sb_bottomup_device_records(sb_handle_t h, int model_id, float** records_dev)
   return SB_OK;
 }
 
+// The peaks and PAF candidates of the step that wrote ws, flattened per frame into the caller's arrays
 static int fetch_graph_ws(sb_handle_s* h, const SbPostWs& ws, const int* edges_host, int B, int cap_peaks, float* peaks,
                           float* peak_vals, int32_t* peak_channel_inds, int32_t* peak_offsets, int cap_cands,
                           int32_t* edge_inds, int32_t* edge_peak_inds, float* line_scores, int32_t* cand_offsets) {
-  const int C = ws.C, K = ws.max_node_peaks, E = ws.n_edges, MP = ws.max_peaks;
-  std::vector<int> np(B), ncnt((size_t)B * C), nlist((size_t)B * C * K);
-  std::vector<float> mat((size_t)B * E * K * K);
+  SbGraphHost g;
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->post_stream));
-  SB_CUDA(h, cudaMemcpy(np.data(), ws.n_peaks, (size_t)B * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(h, cudaMemcpy(ncnt.data(), ws.node_cnt, ncnt.size() * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(h, cudaMemcpy(nlist.data(), ws.node_peaks, nlist.size() * 4, cudaMemcpyDeviceToHost));
-  SB_CUDA(h, cudaMemcpy(mat.data(), ws.score_mat, mat.size() * 4, cudaMemcpyDeviceToHost));
-  int tp = 0, tc = 0;
+  if (const int rc = sb_graph_download(h, ws, B, g)) return rc;
+  const int MP = ws.max_peaks;
+  int tp = 0;
   for (int b = 0; b < B; ++b) {
+    const int n = g.n_peaks[b];
     peak_offsets[b] = tp;
-    cand_offsets[b] = tc;
-    if (tp + np[b] > cap_peaks) return sb_fail(h, SB_ERR_INVALID, "peak capacity exceeded");
-    if (np[b] > 0) {
-      SB_CUDA(h, cudaMemcpy(peaks + 2 * (size_t)tp, ws.peaks + (size_t)b * MP * 2, (size_t)np[b] * 8, cudaMemcpyDeviceToHost));
-      SB_CUDA(h, cudaMemcpy(peak_vals + tp, ws.peak_vals + (size_t)b * MP, (size_t)np[b] * 4, cudaMemcpyDeviceToHost));
-      SB_CUDA(h, cudaMemcpy(peak_channel_inds + tp, ws.peak_ch + (size_t)b * MP, (size_t)np[b] * 4, cudaMemcpyDeviceToHost));
+    if (tp + n > cap_peaks) return sb_fail(h, SB_ERR_INVALID, "peak capacity exceeded");
+    if (n > 0) {
+      SB_CUDA(h, cudaMemcpy(peaks + 2 * (size_t)tp, ws.peaks + (size_t)b * MP * 2, (size_t)n * 8, cudaMemcpyDeviceToHost));
+      SB_CUDA(h, cudaMemcpy(peak_vals + tp, ws.peak_vals + (size_t)b * MP, (size_t)n * 4, cudaMemcpyDeviceToHost));
+      SB_CUDA(h, cudaMemcpy(peak_channel_inds + tp, ws.peak_ch + (size_t)b * MP, (size_t)n * 4, cudaMemcpyDeviceToHost));
     }
-    tp += np[b];
-    for (int e = 0; e < E; ++e) {
-      const int sn = edges_host[2 * e], dn = edges_host[2 * e + 1];
-      const int ns = std::min(ncnt[(size_t)b * C + sn], K), nd = std::min(ncnt[(size_t)b * C + dn], K);
-      for (int i = 0; i < ns; ++i)
-        for (int j = 0; j < nd; ++j) {
-          if (tc >= cap_cands) return sb_fail(h, SB_ERR_INVALID, "candidate capacity exceeded");
-          edge_inds[tc] = e;
-          edge_peak_inds[2 * tc] = nlist[((size_t)b * C + sn) * K + i];
-          edge_peak_inds[2 * tc + 1] = nlist[((size_t)b * C + dn) * K + j];
-          line_scores[tc] = mat[((size_t)b * E + e) * K * K + (size_t)i * nd + j];
-          ++tc;
-        }
-    }
+    tp += n;
   }
   peak_offsets[B] = tp;
-  cand_offsets[B] = tc;
-  return SB_OK;
+  return sb_graph_flatten(h, ws, g, edges_host, B, cap_cands, edge_inds, edge_peak_inds, line_scores, cand_offsets);
 }
 
 int sb_bottomup_fetch_graph(sb_handle_t h, int model_id, int B, int cap_peaks, float* peaks, float* peak_vals,
@@ -1036,28 +1072,6 @@ int sb_bottomup_fetch_graph(sb_handle_t h, int model_id, int B, int cap_peaks, f
   return fetch_graph_ws(h, m->ws, m->bu_edges.data(), B, cap_peaks, peaks, peak_vals, peak_channel_inds, peak_offsets,
                         cap_cands, edge_inds, edge_peak_inds, line_scores, cand_offsets);
 }
-
-// The scratch of a *_from_maps call, freed when it returns: its workspace and device copies of the caller's maps.
-struct MapsScratch {
-  SbPostWs ws;
-  std::vector<void*> bufs;
-  ~MapsScratch() {
-    sb_post_ws_free(ws);
-    for (void* q : bufs) cudaFree(q);
-  }
-  // queues the upload of n floats from `host` on the handle's stream; host NULL (no such map): *dev = NULL
-  int upload(sb_handle_s* h, const float* host, size_t n, const float** dev) {
-    *dev = nullptr;
-    if (!host) return 0;
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, n * 4 + 16);
-    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "cudaMalloc: %s", cudaGetErrorString(e));
-    bufs.push_back(q);
-    *dev = (const float*)q;
-    SB_CUDA(h, cudaMemcpyAsync(q, host, n * 4, cudaMemcpyHostToDevice, h->stream));
-    return 0;
-  }
-};
 
 int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const float* cms_host, int B, int H, int W,
                           const float* pafs_host, int Hp, int Wp, const float* offsets_host,
@@ -1073,26 +1087,23 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const floa
   if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, C2 = 2 * p->n_edges;
-  MapsScratch s;
+  SbScratch s(h);
   if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges))) return rc;
   SbMap cms{nullptr, H, W, C}, pafs{nullptr, Hp, Wp, C2};
   const float* off = nullptr;
   const size_t ncm = (size_t)B * H * W * C;
-  if ((rc = s.upload(h, cms_host, ncm, &cms.dev)) || (rc = s.upload(h, pafs_host, (size_t)B * Hp * Wp * C2, &pafs.dev)) ||
-      (rc = s.upload(h, offsets_host, 2 * ncm, &off)))
+  if ((rc = s.upload(cms_host, ncm, &cms.dev)) || (rc = s.upload(pafs_host, (size_t)B * Hp * Wp * C2, &pafs.dev)) ||
+      (rc = s.upload(offsets_host, 2 * ncm, &off, true)) || (rc = s.to_dev(s.ws.edges_dev, p->edges, (size_t)p->n_edges * 2)))
     return rc;
-  SB_CUDA(h, cudaMemcpyAsync(s.ws.edges_dev, p->edges, (size_t)p->n_edges * 8, cudaMemcpyHostToDevice, h->stream));
-  if (p->n_sorted > 0) SB_CUDA(h, cudaMemcpyAsync(s.ws.sorted_edges_dev, p->sorted_edge_inds, (size_t)p->n_sorted * 4, cudaMemcpyHostToDevice, h->stream));
+  if (p->n_sorted > 0 && (rc = s.to_dev(s.ws.sorted_edges_dev, p->sorted_edge_inds, (size_t)p->n_sorted))) return rc;
   s.ws.n_sorted = p->n_sorted;
   if ((rc = bottomup_post_kernels(h, *p, s.ws, cms, pafs, off, B))) return rc;
   const SbPostWs& ws = s.ws;
   const size_t I = p->max_instances;
-  SB_CUDA(h, cudaMemcpyAsync(out_instance_peaks, ws.inst_peaks, (size_t)B * I * C * 8, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(out_instance_peak_vals, ws.inst_vals, (size_t)B * I * C * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(out_instance_scores, ws.inst_scores, (size_t)B * I * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(out_n_valid, ws.n_inst, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-  if (out_flags) SB_CUDA(h, cudaMemcpyAsync(out_flags, ws.flags, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
+  if ((rc = s.to_host(out_instance_peaks, ws.inst_peaks, B * I * C * 2)) || (rc = s.to_host(out_instance_peak_vals, ws.inst_vals, B * I * C)) ||
+      (rc = s.to_host(out_instance_scores, ws.inst_scores, B * I)) || (rc = s.to_host(out_n_valid, ws.n_inst, (size_t)B)) ||
+      (rc = s.to_host(out_flags, ws.flags, (size_t)B, true)) || (rc = s.sync()))
+    return rc;
   if (peaks)
     return fetch_graph_ws(h, ws, p->edges, B, cap_peaks, peaks, peak_vals, peak_channel_inds, peak_offsets, cap_cands,
                           edge_inds, edge_peak_inds, line_scores, cand_offsets);
@@ -1110,22 +1121,19 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
   if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, NC = p->n_classes;
-  MapsScratch s;
+  SbScratch s(h);
   if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0))) return rc;
   s.ws.node_lists = true;
-  const size_t w = sb_class_record_width(NC, C);
-  if ((rc = sb_dev_alloc(h, &s.ws.records, (size_t)B * w))) return rc;
+  std::vector<float> rec((size_t)B * sb_class_record_width(NC, C));
+  if ((rc = sb_dev_alloc(h, &s.ws.records, rec.size()))) return rc;
   SbMap cms{nullptr, H, W, C}, cls{nullptr, Hc, Wc, NC};
   const float* off = nullptr;
   const size_t ncm = (size_t)B * H * W * C;
-  if ((rc = s.upload(h, cms_host, ncm, &cms.dev)) || (rc = s.upload(h, class_logits_host, (size_t)B * Hc * Wc * NC, &cls.dev)) ||
-      (rc = s.upload(h, offsets_host, 2 * ncm, &off)))
+  if ((rc = s.upload(cms_host, ncm, &cms.dev)) || (rc = s.upload(class_logits_host, (size_t)B * Hc * Wc * NC, &cls.dev)) ||
+      (rc = s.upload(offsets_host, 2 * ncm, &off, true)) || (rc = multiclass_post_kernels(h, *p, s.ws, cms, cls, off, B)) ||
+      (rc = s.to_host(rec.data(), s.ws.records, rec.size())) || (rc = s.sync()))
     return rc;
-  if ((rc = multiclass_post_kernels(h, *p, s.ws, cms, cls, off, B))) return rc;
-  std::vector<float> rec((size_t)B * w);
-  SB_CUDA(h, cudaMemcpyAsync(rec.data(), s.ws.records, rec.size() * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  unpack_class_records(rec.data(), w, B, NC, C, out_points, out_vals, out_class_probs, out_flags);
+  split_class_records(*p, rec.data(), B, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -1139,15 +1147,8 @@ int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* p) 
   if (p->offsets_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad offsets buffer");
   const SbBuffer& cb = m->buffers[p->cms_buffer];
   if (cb.C > 256) return sb_fail(h, SB_ERR_UNSUPPORTED, "more than 256 confidence-map channels");
-  if (const int rc = chain_drop(h, m)) return rc;
-  SbGlobalScratch& g = m->gs;
-  const int target = (2 * h->sm_count + m->B - 1) / m->B;
-  g.rpc = std::max(1, (cb.H + target - 1) / target);
-  g.chunks = (cb.H + g.rpc - 1) / g.rpc;
-  SB_CUDA(h, cudaMalloc((void**)&g.part, (size_t)m->B * g.chunks * cb.C * 3 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&g.points, (size_t)m->B * cb.C * 2 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&g.vals, (size_t)m->B * cb.C * 4));
-  SB_CUDA(h, cudaMalloc((void**)&g.crop_off, (size_t)m->B * 2 * 4));
+  int rc = chain_drop(h, m);
+  if (rc || (rc = sb_global_scratch_alloc(h, m->gs, m->B, cb.H, cb.C))) return rc;
   m->gl = *p;
   m->chain = SB_CHAIN_GLOBAL;
   return SB_OK;
@@ -1167,7 +1168,7 @@ int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int im
   const sb_global_params& p = m->gl;
   SbBuffer& cb = m->buffers[p.cms_buffer];
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-  if ((rc = sbk_global_peaks(h, cb.dev, 0, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp,
+  if ((rc = sbk_global_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp,
                              crop_offsets_host ? g.crop_off : nullptr, g.part, g.chunks, g.rpc, g.points, g.vals))) return rc;
   SB_CUDA(h, cudaMemcpyAsync(out_points, g.points, (size_t)B * cb.C * 8, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaMemcpyAsync(out_vals, g.vals, (size_t)B * cb.C * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1205,24 +1206,8 @@ int sb_infer_centroids(sb_handle_t h, int model_id, const void* images_host, int
   const sb_centroid_params& p = m->ce;
   SbBuffer& cb = m->buffers[p.cms_buffer];
   SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-  if ((rc = sbk_local_peaks(h, cb.dev, 0, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, m->ws))) return rc;
-  std::vector<int> cnt(B), fl(B);
-  SB_CUDA(h, cudaMemcpyAsync(cnt.data(), m->ws.n_peaks, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(fl.data(), m->ws.flags, (size_t)B * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  int total = 0;
-  for (int b = 0; b < B; ++b) {
-    if (cnt[b] > 0) {
-      SB_CUDA(h, cudaMemcpyAsync(out_centroids + 2 * (size_t)total, m->ws.peaks + (size_t)b * m->ws.max_peaks * 2, (size_t)cnt[b] * 8, cudaMemcpyDeviceToHost, h->stream));
-      SB_CUDA(h, cudaMemcpyAsync(out_vals + total, m->ws.peak_vals + (size_t)b * m->ws.max_peaks, (size_t)cnt[b] * 4, cudaMemcpyDeviceToHost, h->stream));
-      for (int i = 0; i < cnt[b]; ++i) out_sample_inds[total + i] = b;
-    }
-    total += cnt[b];
-    if (out_flags) out_flags[b] = fl[b];
-  }
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
-  *out_n = total;
-  return SB_OK;
+  if ((rc = sbk_local_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, m->ws))) return rc;
+  return sb_peaks_to_host(h, m->ws, B, out_centroids, out_vals, nullptr, out_sample_inds, out_n, out_flags);
 }
 
 }  // extern "C"

@@ -104,12 +104,6 @@ struct SbEntryPlan {
 // pipeline is a layer over a centroid chain and a global chain, valid while neither model's chain_gen moves.
 enum { SB_CHAIN_ANY = -1, SB_CHAIN_NONE = 0, SB_CHAIN_PAF, SB_CHAIN_CLASS, SB_CHAIN_GLOBAL, SB_CHAIN_CENTROID };
 
-// Global-peak scratch of the global chain (per frame of the configured batch)
-struct SbGlobalScratch {
-  float *part = nullptr, *points = nullptr, *vals = nullptr, *crop_off = nullptr;
-  int rpc = 1, chunks = 1;   // rows per chunk of the partial maxima, chunks per frame
-};
-
 struct SbModel {
   int precision = 0;  // 0: fp16 activations + tensor-core convs; 1: fp32 CUDA-core path
   std::vector<SbOp> ops;

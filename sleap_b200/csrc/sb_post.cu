@@ -23,15 +23,13 @@
 namespace {
 
 __device__ __forceinline__ float ldf(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float ldf(const __half* p) { return __half2float(__ldg(p)); }
 
 // ------------------------------------------------------------------------------------------
 // tf.image.crop_and_resize(bilinear) of a p x p patch centred on integer pixel (px, py) of one
 // channel plane of an NHWC map, followed by integral regression or the local-direction offset.
 // Restates, op for op in f32: make_centered_bboxes -> normalize_bboxes -> crop_and_resize.
 // ------------------------------------------------------------------------------------------
-template <typename T>
-__device__ void refine_offset(const T* __restrict__ plane /* &cms[b][0][0][c] */, int H, int W,
+__device__ void refine_offset(const float* __restrict__ plane /* &cms[b][0][0][c] */, int H, int W,
                               int C, float px, float py, int mode, int p, float* dx, float* dy) {
   const float Hm1 = (float)(H - 1), Wm1 = (float)(W - 1);
   const float half = (float)(p - 1) * 0.5f;
@@ -97,8 +95,7 @@ __device__ void refine_offset(const T* __restrict__ plane /* &cms[b][0][0][c] */
 // strict 8-neighbour NMS (out-of-image taps skipped, centre-1 tap) + strict threshold; ordered
 // compaction of (flat index, value) into the chunk's list.
 // ------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) k_local_scan(const T* __restrict__ cms, int H, int W, int C,
+__global__ void __launch_bounds__(256) k_local_scan(const float* __restrict__ cms, int H, int W, int C,
                                                     int rows_per_chunk, int chunk_cap,
                                                     float threshold, int* __restrict__ chunk_cnt,
                                                     uint2* __restrict__ chunk_items) {
@@ -106,7 +103,7 @@ __global__ void __launch_bounds__(256) k_local_scan(const T* __restrict__ cms, i
   const int y0 = chunk * rows_per_chunk;
   const int y1 = min(H, y0 + rows_per_chunk);
   const int rowlen = W * C;
-  const T* base = cms + (size_t)b * H * rowlen;
+  const float* base = cms + (size_t)b * H * rowlen;
   const int f0 = y0 * rowlen, f1 = y1 * rowlen;
   uint2* items = chunk_items + ((size_t)b * n_chunks + chunk) * chunk_cap;
   __shared__ int warp_tot[8];
@@ -126,7 +123,7 @@ __global__ void __launch_bounds__(256) k_local_scan(const T* __restrict__ cms, i
         const int x = r / C;
         float m = v - 1.0f;  // centre tap: v + (-1)
         const bool up = y > 0, dn = y < H - 1, lf = x > 0, rt = x < W - 1;
-        const T* q = base + f;
+        const float* q = base + f;
         if (up) {
           if (lf) m = fmaxf(m, ldf(q - rowlen - C));
           m = fmaxf(m, ldf(q - rowlen));
@@ -236,8 +233,7 @@ __global__ void __launch_bounds__(256) k_local_scan_v(const float* __restrict__ 
 // loads), then every lane replays the SAME sequential accumulation over the samples (shuffle broadcast), i.e. the
 // float operations and their order are those of refine_offset -- results are bit-identical to it.
 // ------------------------------------------------------------------------------------------
-template <typename T>
-__device__ void refine_offset_warp(const T* __restrict__ plane, int H, int W, int C, float px, float py, int mode, int p,
+__device__ void refine_offset_warp(const float* __restrict__ plane, int H, int W, int C, float px, float py, int mode, int p,
                                    int lane, float* dx, float* dy) {
   const float Hm1 = (float)(H - 1), Wm1 = (float)(W - 1);
   const float half = (float)(p - 1) * 0.5f;
@@ -305,9 +301,8 @@ __device__ void refine_offset_warp(const T* __restrict__ plane, int H, int W, in
 // ------------------------------------------------------------------------------------------
 constexpr int EMIT_THREADS = 512;
 
-template <typename T>
 __global__ void __launch_bounds__(EMIT_THREADS) k_local_emit(
-    const T* __restrict__ cms, const float* __restrict__ offsets, int H, int W, int C, int n_chunks,
+    const float* __restrict__ cms, const float* __restrict__ offsets, int H, int W, int C, int n_chunks,
     int chunk_cap, int refinement, int patch, float scale, float input_scale, int max_peaks,
     int max_node_peaks, const int* __restrict__ chunk_cnt, const uint2* __restrict__ chunk_items,
     uint2* __restrict__ sorted_items /*[B][max_peaks]*/, float* __restrict__ peaks, float* __restrict__ peak_vals,
@@ -344,7 +339,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_local_emit(
   const int n = min(total, max_peaks);
   int flag = (total > max_peaks) ? SB_FLAG_PEAKS_TRUNCATED : 0;
   const int rowlen = W * C;
-  const T* base = cms + (size_t)b * H * rowlen;
+  const float* base = cms + (size_t)b * H * rowlen;
   float* pk = peaks + (size_t)b * max_peaks * 2;
   float* pv = peak_vals + (size_t)b * max_peaks;
   int* pc = peak_ch + (size_t)b * max_peaks;
@@ -386,8 +381,8 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_local_emit(
     } else if (refinement != SB_REFINE_NONE) {
       float dx, dy;
       const int pp = refinement == SB_REFINE_INTEGRAL ? patch : 3;
-      if (pp * pp <= 128) refine_offset_warp<T>(base + c, H, W, C, fx, fy, refinement, pp, lane, &dx, &dy);
-      else refine_offset<T>(base + c, H, W, C, fx, fy, refinement, pp, &dx, &dy);
+      if (pp * pp <= 128) refine_offset_warp(base + c, H, W, C, fx, fy, refinement, pp, lane, &dx, &dy);
+      else refine_offset(base + c, H, W, C, fx, fy, refinement, pp, &dx, &dy);
       fx = fx + dx;
       fy = fy + dy;
     }
@@ -444,14 +439,13 @@ __device__ __forceinline__ void gmax_merge(GMax& a, float v, int y, int x) {
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) k_global_partial(const T* __restrict__ cms, int H, int W,
+__global__ void __launch_bounds__(256) k_global_partial(const float* __restrict__ cms, int H, int W,
                                                         int C, int rows_per_chunk,
                                                         float* __restrict__ part /*[B][chunks][C][3]*/) {
   const int chunk = blockIdx.x, b = blockIdx.y, n_chunks = gridDim.x;
   const int y0 = chunk * rows_per_chunk, y1 = min(H, y0 + rows_per_chunk);
   const int rowlen = W * C;
-  const T* base = cms + (size_t)b * H * rowlen;
+  const float* base = cms + (size_t)b * H * rowlen;
   const int per = max(1, 256 / C);           // pixels handled per sweep
   const int active = per * C;                // threads that own a (pixel slot, channel)
   extern __shared__ float s_red[];           // [active][3]
@@ -490,8 +484,7 @@ struct GlobalFix {
   int has_crop_off;   // + crop_offsets[b] / input_scale
 };
 
-template <typename T>
-__global__ void k_global_final(const T* __restrict__ cms, const float* __restrict__ offsets, int H,
+__global__ void k_global_final(const float* __restrict__ cms, const float* __restrict__ offsets, int H,
                                int W, int C, int n_chunks, const float* __restrict__ part,
                                float threshold, int refinement, int patch, GlobalFix fix,
                                const float* __restrict__ crop_off, float* __restrict__ out_points,
@@ -505,7 +498,7 @@ __global__ void k_global_final(const T* __restrict__ cms, const float* __restric
       gmax_merge(a, o[0], __float_as_int(o[1]), __float_as_int(o[2]));
     }
     const int row = min(max(a.y, 0), H - 1), col = min(max(a.x, 0), W - 1);
-    const T* plane = cms + (size_t)b * H * W * C + c;
+    const float* plane = cms + (size_t)b * H * W * C + c;
     const float val = ldf(plane + ((size_t)row * W + col) * C);
     float fx = (float)col, fy = (float)row;
     if (val < threshold) {
@@ -516,8 +509,7 @@ __global__ void k_global_final(const T* __restrict__ cms, const float* __restric
         fx = fx + o[0]; fy = fy + o[1];
       } else if (refinement != SB_REFINE_NONE) {
         float dx, dy;
-        refine_offset<T>(plane, H, W, C, fx, fy, refinement,
-                         refinement == SB_REFINE_INTEGRAL ? patch : 3, &dx, &dy);
+        refine_offset(plane, H, W, C, fx, fy, refinement, refinement == SB_REFINE_INTEGRAL ? patch : 3, &dx, &dy);
         fx = fx + dx; fy = fy + dy;
       }
       fx = fx * fix.scale; fy = fy * fix.scale;
@@ -1141,44 +1133,33 @@ void sb_post_ws_free(SbPostWs& ws) {
   ws = SbPostWs();
 }
 
-int sbk_local_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const float* offsets, int B,
-                    int H, int W, int C, const SbPeakParams& p, SbPostWs& ws) {
+int sbk_local_peaks(sb_handle_s* h, const float* cms, const float* offsets, int B, int H, int W, int C,
+                    const SbPeakParams& p, SbPostWs& ws) {
   if (B > ws.B || H != ws.H || W != ws.W || C != ws.C)
     return sb_fail(h, SB_ERR_INVALID, "local peaks: workspace shape mismatch");
   dim3 g(ws.n_chunks, B);
   // zero the per-chunk append counters and the per-frame overflow flags (one memset node each, same stream)
   SB_CUDA(h, cudaMemsetAsync(ws.chunk_cnt, 0, (size_t)ws.B * ws.n_chunks * sizeof(int), h->stream));
   SB_CUDA(h, cudaMemsetAsync(ws.flags, 0, (size_t)ws.B * sizeof(int), h->stream));
-  const bool vec_ok = !cms_is_half && ((W * C) % 4 == 0) && ((reinterpret_cast<uintptr_t>(cms) & 15) == 0) &&
-                      !getenv("SB_DISABLE_SCAN_V");
-  if (cms_is_half)
-    k_local_scan<__half><<<g, 256, 0, h->stream>>>((const __half*)cms, H, W, C, ws.rows_per_chunk,
-                                                   ws.chunk_cap, p.threshold, ws.chunk_cnt, ws.chunk_items);
-  else if (vec_ok)
-    k_local_scan_v<4><<<g, 256, 0, h->stream>>>((const float*)cms, H, W, C, ws.rows_per_chunk, ws.chunk_cap, p.threshold,
+  const bool vec_ok = ((W * C) % 4 == 0) && ((reinterpret_cast<uintptr_t>(cms) & 15) == 0) && !getenv("SB_DISABLE_SCAN_V");
+  if (vec_ok)
+    k_local_scan_v<4><<<g, 256, 0, h->stream>>>(cms, H, W, C, ws.rows_per_chunk, ws.chunk_cap, p.threshold,
                                                 ws.chunk_cnt, ws.chunk_items);
   else
-    k_local_scan<float><<<g, 256, 0, h->stream>>>((const float*)cms, H, W, C, ws.rows_per_chunk,
-                                                  ws.chunk_cap, p.threshold, ws.chunk_cnt, ws.chunk_items);
+    k_local_scan<<<g, 256, 0, h->stream>>>(cms, H, W, C, ws.rows_per_chunk, ws.chunk_cap, p.threshold, ws.chunk_cnt,
+                                           ws.chunk_items);
   SB_CHECK_LAUNCH(h);
   const size_t sm = (size_t)(ws.n_chunks + 1) * sizeof(int);
   int* ncnt = ws.node_lists ? ws.node_cnt : nullptr;
-  if (cms_is_half)
-    k_local_emit<__half><<<B, EMIT_THREADS, sm, h->stream>>>(
-        (const __half*)cms, offsets, H, W, C, ws.n_chunks, ws.chunk_cap, p.refinement, p.patch,
-        p.scale, p.input_scale, ws.max_peaks, ws.max_node_peaks, ws.chunk_cnt, ws.chunk_items, ws.sorted_items, ws.peaks,
-        ws.peak_vals, ws.peak_ch, ws.n_peaks, ws.total_peaks, ncnt, ws.node_peaks, ws.flags);
-  else
-    k_local_emit<float><<<B, EMIT_THREADS, sm, h->stream>>>(
-        (const float*)cms, offsets, H, W, C, ws.n_chunks, ws.chunk_cap, p.refinement, p.patch,
-        p.scale, p.input_scale, ws.max_peaks, ws.max_node_peaks, ws.chunk_cnt, ws.chunk_items, ws.sorted_items, ws.peaks,
-        ws.peak_vals, ws.peak_ch, ws.n_peaks, ws.total_peaks, ncnt, ws.node_peaks, ws.flags);
+  k_local_emit<<<B, EMIT_THREADS, sm, h->stream>>>(
+      cms, offsets, H, W, C, ws.n_chunks, ws.chunk_cap, p.refinement, p.patch,
+      p.scale, p.input_scale, ws.max_peaks, ws.max_node_peaks, ws.chunk_cnt, ws.chunk_items, ws.sorted_items, ws.peaks,
+      ws.peak_vals, ws.peak_ch, ws.n_peaks, ws.total_peaks, ncnt, ws.node_peaks, ws.flags);
   SB_CHECK_LAUNCH(h);
   return 0;
 }
 
-int sbk_global_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const float* offsets,
-                     int B, int H, int W, int C, const SbPeakParams& p,
+int sbk_global_peaks(sb_handle_s* h, const float* cms, const float* offsets, int B, int H, int W, int C, const SbPeakParams& p,
                      const float* crop_off_dev, float* part_buf, int n_chunks, int rows_per_chunk,
                      float* out_points, float* out_vals) {
   if (C > 256) return sb_fail(h, SB_ERR_UNSUPPORTED, "global peaks: C > 256");
@@ -1187,19 +1168,10 @@ int sbk_global_peaks(sb_handle_s* h, const void* cms, int cms_is_half, const flo
   const size_t sm = (size_t)per * C * 3 * sizeof(float);
   GlobalFix fix;
   fix.scale = p.scale; fix.input_scale = p.input_scale; fix.has_crop_off = crop_off_dev != nullptr;
-  if (cms_is_half) {
-    k_global_partial<__half><<<g, 256, sm, h->stream>>>((const __half*)cms, H, W, C, rows_per_chunk, part_buf);
-    SB_CHECK_LAUNCH(h);
-    k_global_final<__half><<<B, 64, 0, h->stream>>>((const __half*)cms, offsets, H, W, C, n_chunks, part_buf,
-                                                    p.threshold, p.refinement, p.patch, fix, crop_off_dev,
-                                                    out_points, out_vals);
-  } else {
-    k_global_partial<float><<<g, 256, sm, h->stream>>>((const float*)cms, H, W, C, rows_per_chunk, part_buf);
-    SB_CHECK_LAUNCH(h);
-    k_global_final<float><<<B, 64, 0, h->stream>>>((const float*)cms, offsets, H, W, C, n_chunks, part_buf,
-                                                   p.threshold, p.refinement, p.patch, fix, crop_off_dev,
-                                                   out_points, out_vals);
-  }
+  k_global_partial<<<g, 256, sm, h->stream>>>(cms, H, W, C, rows_per_chunk, part_buf);
+  SB_CHECK_LAUNCH(h);
+  k_global_final<<<B, 64, 0, h->stream>>>(cms, offsets, H, W, C, n_chunks, part_buf, p.threshold, p.refinement, p.patch, fix,
+                                          crop_off_dev, out_points, out_vals);
   SB_CHECK_LAUNCH(h);
   return 0;
 }

@@ -192,7 +192,7 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
   SbBuffer& cb = mc->buffers[cp.cms_buffer];
   const float* coff = cp.offsets_buffer >= 0 ? (const float*)mc->buffers[cp.offsets_buffer].dev : nullptr;
   SbPeakParams pc{cp.peak_threshold, cp.refinement, cp.integral_patch_size, (float)cp.output_stride, cp.input_scale};
-  if ((rc = sbk_local_peaks(h, cb.dev, 0, coff, B, cb.H, cb.W, cb.C, pc, mc->ws))) return rc;
+  if ((rc = sbk_local_peaks(h, (const float*)cb.dev, coff, B, cb.H, cb.W, cb.C, pc, mc->ws))) return rc;
   k_td_select<<<B, 128, 0, s>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->sel_cent,
                                 t->sel_val, t->sel_count, mc->ws.flags);
   SB_CHECK_LAUNCH(h);
@@ -214,7 +214,7 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
     if ((rc = sbk_crop(h, mc->frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
                        cs, cs, t->crops, frames_are_u8))) return rc;
     if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n))) return rc;
-    if ((rc = sbk_global_peaks(h, ib.dev, 0, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
+    if ((rc = sbk_global_peaks(h, (const float*)ib.dev, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
                                t->ipts + (size_t)c0 * t->nodes * 2, t->ivals + (size_t)c0 * t->nodes))) return rc;
   }
   k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags, t->record,
@@ -228,15 +228,9 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
             t2 - t1, t3 - t2);
   }
   const size_t K = t->K, nd = t->nodes;
-  for (int b = 0; b < B; ++b) {
-    const float* r = t->record_host + (size_t)b * t->width;
-    memcpy(out_centroids + (size_t)b * K * 2, r, K * 2 * 4);
-    memcpy(out_centroid_vals + (size_t)b * K, r + K * 2, K * 4);
-    memcpy(out_instance_peaks + (size_t)b * K * nd * 2, r + K * 3, K * nd * 2 * 4);
-    memcpy(out_instance_peak_vals + (size_t)b * K * nd, r + K * 3 + K * nd * 2, K * nd * 4);
-    out_n_valid[b] = (int32_t)r[K * 3 + K * nd * 3];
-    if (out_flags) out_flags[b] = (int32_t)r[K * 3 + K * nd * 3 + 1];
-  }
+  sb_split_records(t->record_host, B, t->width,
+                   {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
+                   {out_n_valid, out_flags});
   return SB_OK;
 }
 

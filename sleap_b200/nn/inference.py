@@ -95,6 +95,9 @@ class InferenceLayer:
     """sleap/nn/inference.py:897-967: owns the device model and the preprocessing parameters.
     (uint8 -> float, gray/rgb, resize by input_scale and pad_to_stride run inside the device op-list.)"""
 
+    CHAIN = None        # configure call of the layer's post-processing chain; ``params()`` returns its parameters
+    _keep = ()          # the arrays the pointer fields of those parameters point to
+
     def __init__(self, keras_model: DeviceModel, input_scale: float = 1.0, pad_to_stride: int = 1,
                  ensure_grayscale: Optional[bool] = None, ensure_float: bool = True):
         self.keras_model = keras_model      # attribute name kept from the reference
@@ -114,6 +117,13 @@ class InferenceLayer:
             imgs = np.ascontiguousarray(imgs, dtype=np.float32)
         return imgs
 
+    def _configure(self, B, H, W, C):
+        """The device model for batches of up to B frames of (H, W, C), then the layer's chain (``CHAIN``)."""
+        m = self.keras_model
+        if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
+            m.configure(B, H, W, C)
+        m.configure_chain(self.CHAIN, self.params(), *self._keep)
+
 
 def _find_head(model: DeviceModel, name: str):
     if name not in model.cm.head_buffers:
@@ -121,11 +131,17 @@ def _find_head(model: DeviceModel, name: str):
     return model.cm.head_buffers[name]
 
 
+def head_channels(model: DeviceModel, name: str) -> int:
+    """Output channels of head ``name`` in the model's spec."""
+    return next(h["channels"] for h in model.spec["heads"] if h["name"] == name)
+
+
 # ------------------------------------------------------------------------------------------
 class SingleInstanceInferenceLayer(InferenceLayer):
     """sleap/nn/inference.py:1229-1380."""
 
     HEAD = "SingleInstanceConfmapsHead"
+    CHAIN = "sb_global_configure"
 
     def __init__(self, keras_model, input_scale=1.0, pad_to_stride=1, output_stride=None, peak_threshold=0.2,
                  refinement="local", integral_patch_size=5, return_confmaps=False, confmaps_ind=None,
@@ -148,18 +164,12 @@ class SingleInstanceInferenceLayer(InferenceLayer):
                             int(self.output_stride), float(self.peak_threshold), REFINE.get(self.refinement, 0),
                             int(self.integral_patch_size), float(self.input_scale))
 
-    def _configure(self, B, H, W, C):
-        m = self.keras_model
-        if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
-            m.configure(B, H, W, C)
-        m.configure_chain("sb_global_configure", self.params())
-
     def call(self, data, crop_offsets=None):
         imgs = self._prep(_images_of(data))
         B, H, W, C = imgs.shape
         self._configure(B, H, W, C)
         m = self.keras_model
-        n_nodes = next(h["channels"] for h in m.spec["heads"] if h["name"] == self.HEAD)
+        n_nodes = head_channels(m, self.HEAD)
         pts = np.zeros((B, n_nodes, 2), np.float32)
         vals = np.zeros((B, n_nodes), np.float32)
         co = None if crop_offsets is None else f32(crop_offsets).reshape(B, 2)
@@ -284,7 +294,7 @@ class FindInstancePeaks(SingleInstanceInferenceLayer):
             samples, sinds = n, np.arange(n)
         co = inputs.get("crop_offsets")
         m = self.keras_model
-        n_nodes = next(h["channels"] for h in m.spec["heads"] if h["name"] == self.HEAD)
+        n_nodes = head_channels(m, self.HEAD)
         pts = np.zeros((n, n_nodes, 2), np.float32)
         vals = np.zeros((n, n_nodes), np.float32)
         for i in range(0, n, self.max_crops_per_call):
@@ -423,7 +433,7 @@ class TopDownInferenceModel(InferenceModel):
             mc.configured_for = (cap, H, W, C)
             mi.configured_for = (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C)
             mc.chain = mi.chain = record
-        n_nodes = next(h["channels"] for h in mi.spec["heads"] if h["name"] == fp.HEAD)
+        n_nodes = head_channels(mi, fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
@@ -446,7 +456,7 @@ class TopDownInferenceModel(InferenceModel):
         if isinstance(self.instance_peaks, FindInstancePeaksGroundTruth):
             n_nodes = max([p.shape[1] for p in peaks_out["instance_peaks"] if p.ndim == 3] + [0])
         else:
-            n_nodes = next(h["channels"] for h in self.instance_peaks.keras_model.spec["heads"] if h["name"] == self.instance_peaks.HEAD)
+            n_nodes = head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
         ip, nv = _ragged_to_dense(peaks_out["instance_peaks"], (n_nodes, 2))
         iv, _ = _ragged_to_dense(peaks_out["instance_peak_vals"], (n_nodes,))
         ce, _ = _ragged_to_dense(peaks_out["centroids"], (2,))
@@ -461,6 +471,8 @@ class TopDownInferenceModel(InferenceModel):
 class BottomUpInferenceLayer(InferenceLayer):
     """sleap/nn/inference.py:2737-3003: net -> local peaks -> PAF scoring -> matching -> grouping,
     executed as one device pipeline (``sb_infer_bottomup``)."""
+
+    CHAIN = "sb_bottomup_configure"
 
     def __init__(self, keras_model, paf_scorer, input_scale=1.0, pad_to_stride=1, cm_output_stride=None,
                  paf_output_stride=None, peak_threshold=0.2, refinement="local", integral_patch_size=5,
@@ -487,7 +499,6 @@ class BottomUpInferenceLayer(InferenceLayer):
         self.max_peaks_per_sample = max_peaks_per_sample
         self.max_node_peaks = max_node_peaks
         self.max_instances = max_instances
-        self._keep = None
         # a Tracker with track_device, run by k_track inside each step (BottomUpPredictor.predict sets it for its span),
         # and the predictor's max_instances cut of the instance list (-1: none)
         self.tracker = None
@@ -529,12 +540,6 @@ class BottomUpInferenceLayer(InferenceLayer):
             self.input_scale, self.max_peaks_per_sample, self.max_node_peaks, self.max_instances)
         return p
 
-    def _configure(self, B, H, W, C):
-        m = self.keras_model
-        if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
-            m.configure(B, H, W, C)
-        m.configure_chain("sb_bottomup_configure", self.params(), *self._keep)
-
     def call(self, data):
         raw = _images_of(data)
         imgs = self._prep(raw)
@@ -570,17 +575,24 @@ class BottomUpInferenceLayer(InferenceLayer):
 
     def fetch_graph(self, B):
         m = self.keras_model
-        cp = B * self.max_peaks_per_sample
-        cc = B * self.paf_scorer.n_edges * self.max_node_peaks ** 2
-        peaks = np.zeros((cp, 2), np.float32); pv = np.zeros((cp,), np.float32); pc = np.zeros((cp,), np.int32)
-        po = np.zeros((B + 1,), np.int32)
-        ei = np.zeros((cc,), np.int32); epi = np.zeros((cc, 2), np.int32); ls = np.zeros((cc,), np.float32)
-        co = np.zeros((B + 1,), np.int32)
-        m.handle.call("sb_bottomup_fetch_graph", m.model_id, B, cp, ptr(peaks), ptr(pv), ptr(pc), ptr(po), cc, ptr(ei),
-                      ptr(epi), ptr(ls), ptr(co))
-        rows = lambda a, o: [a[o[b]:o[b + 1]].copy() for b in range(B)]
-        return {"peaks": rows(peaks, po), "peak_vals": rows(pv, po), "peak_channel_inds": rows(pc, po),
-                "edge_inds": rows(ei, co), "edge_peak_inds": rows(epi, co), "line_scores": rows(ls, co)}
+        pks, cands = _paf_graph_arrays(B, self.max_peaks_per_sample, self.paf_scorer.n_edges, self.max_node_peaks)
+        m.handle.call("sb_bottomup_fetch_graph", m.model_id, B, len(pks[0]), *map(ptr, pks), len(cands[0]), *map(ptr, cands))
+        return _paf_graph_rows(pks, cands)
+
+
+def _paf_graph_arrays(B, max_peaks_per_sample, n_edges, max_node_peaks):
+    """Host arrays of B frames' PAF graph: (peaks, values, channels, offsets), (edges, edge peaks, line scores, offsets)."""
+    cp, cc = B * max_peaks_per_sample, B * n_edges * max_node_peaks ** 2
+    return ((np.zeros((cp, 2), np.float32), np.zeros((cp,), np.float32), np.zeros((cp,), np.int32), np.zeros((B + 1,), np.int32)),
+            (np.zeros((cc,), np.int32), np.zeros((cc, 2), np.int32), np.zeros((cc,), np.float32), np.zeros((B + 1,), np.int32)))
+
+
+def _paf_graph_rows(pks, cands):
+    """The PAF-graph arrays split into one row per frame at their offsets."""
+    (peaks, pv, pc, po), (ei, epi, ls, co) = pks, cands
+    rows = lambda a, o: [a[o[b]:o[b + 1]].copy() for b in range(len(o) - 1)]
+    return {"peaks": rows(peaks, po), "peak_vals": rows(pv, po), "peak_channel_inds": rows(pc, po),
+            "edge_inds": rows(ei, co), "edge_peak_inds": rows(epi, co), "line_scores": rows(ls, co)}
 
 
 def paf_params(ps, buffers, cm_output_stride, paf_output_stride, peak_threshold, refinement, integral_patch_size, input_scale,
@@ -614,23 +626,16 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
     I, N = max_instances, ps.n_nodes
     ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32); isc = np.zeros((B, I), np.float32)
     nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
-    cp = B * max_peaks_per_sample
-    cc = B * ps.n_edges * max_node_peaks ** 2
-    peaks = np.zeros((cp, 2), np.float32); pv = np.zeros((cp,), np.float32); pc = np.zeros((cp,), np.int32)
-    po = np.zeros((B + 1,), np.int32)
-    ei = np.zeros((cc,), np.int32); epi = np.zeros((cc, 2), np.int32); ls = np.zeros((cc,), np.float32)
-    co = np.zeros((B + 1,), np.int32)
+    pks, cands = _paf_graph_arrays(B, max_peaks_per_sample, ps.n_edges, max_node_peaks)
     off = None if offsets is None else f32(offsets)
     h.call("sb_bottomup_from_maps", byref(p), ptr(cms), B, H, W, ptr(pafs), Hp, Wp, ptr(off), ptr(ip), ptr(iv), ptr(isc),
-           ptr(nv), ptr(fl), cp, ptr(peaks) if return_paf_graph else None, ptr(pv), ptr(pc), ptr(po), cc, ptr(ei),
-           ptr(epi), ptr(ls), ptr(co))
+           ptr(nv), ptr(fl), len(pks[0]), ptr(pks[0]) if return_paf_graph else None, *map(ptr, pks[1:]), len(cands[0]),
+           *map(ptr, cands))
     out = {"instance_peaks": [ip[b, :nv[b]].copy() for b in range(B)],
            "instance_peak_vals": [iv[b, :nv[b]].copy() for b in range(B)],
            "instance_scores": [isc[b, :nv[b]].copy() for b in range(B)], "n_valid": nv, "flags": fl}
     if return_paf_graph:
-        rows = lambda a, o: [a[o[b]:o[b + 1]].copy() for b in range(B)]
-        out.update({"peaks": rows(peaks, po), "peak_vals": rows(pv, po), "peak_channel_inds": rows(pc, po),
-                    "edge_inds": rows(ei, co), "edge_peak_inds": rows(epi, co), "line_scores": rows(ls, co)})
+        out.update(_paf_graph_rows(pks, cands))
     return out
 
 
@@ -711,6 +716,7 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
     each (frame, node) assignment of peaks to classes, as ``identity.classify_peaks_from_maps`` does on the host."""
 
     CMS, CLASS_MAPS, OFFSETS = "MultiInstanceConfmapsHead", "ClassMapsHead", "OffsetRefinementHead"
+    CHAIN = "sb_multiclass_configure"
 
     def __init__(self, keras_model, input_scale=1.0, pad_to_stride=1, cm_output_stride=None, class_maps_output_stride=None,
                  peak_threshold=0.2, refinement="integral", integral_patch_size=5, return_confmaps=False,
@@ -731,8 +737,7 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
         self.return_class_maps = return_class_maps
         self.max_peaks_per_sample = max_peaks_per_sample
         self.max_node_peaks = max_node_peaks
-        channels = {h["name"]: h["channels"] for h in keras_model.spec["heads"]}
-        self.n_nodes, self.n_classes = int(channels[self.CMS]), int(channels[self.CLASS_MAPS])
+        self.n_nodes, self.n_classes = int(head_channels(keras_model, self.CMS)), int(head_channels(keras_model, self.CLASS_MAPS))
 
     def params(self) -> MultiClassParams:
         heads = self.keras_model.cm.head_buffers
@@ -740,12 +745,6 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
                             self.cm_output_stride, self.class_maps_output_stride, self.peak_threshold, self.refinement,
                             self.integral_patch_size, self.n_nodes, self.n_classes, self.input_scale, self.max_peaks_per_sample,
                             self.max_node_peaks)
-
-    def _configure(self, B, H, W, C):
-        m = self.keras_model
-        if not (m.configured_for and m.configured_for[0] >= B and m.configured_for[1:] == (H, W, C)):
-            m.configure(B, H, W, C)
-        m.configure_chain("sb_multiclass_configure", self.params())
 
     def _outputs(self, B):
         K, N = self.n_classes, self.n_nodes
@@ -876,8 +875,7 @@ class TopDownMultiClassFindPeaks(InferenceLayer):
         else:
             samples, sinds = n, np.arange(n, dtype=np.int32)
         m = self.keras_model
-        n_nodes = next(h["channels"] for h in m.spec["heads"] if h["name"] == self.HEAD)
-        n_classes = next(h["channels"] for h in m.spec["heads"] if h["name"] == "ClassVectorsHead")
+        n_nodes, n_classes = head_channels(m, self.HEAD), head_channels(m, "ClassVectorsHead")
         pts = np.zeros((n, n_nodes, 2), np.float32)
         vals = np.zeros((n, n_nodes), np.float32)
         probs = np.zeros((n, n_classes), np.float32)
