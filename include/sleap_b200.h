@@ -370,6 +370,56 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
                      float* out_centroids, float* out_centroid_vals, float* out_instance_peaks,
                      float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
 
+/* ---- top-down multi-class (identity) step ---------------------------------------------------------
+ * sleap/nn/inference.py:4139-4210 TopDownMultiClassInferenceModel.call = CentroidCrop.call -> TopDownMultiClassFindPeaks.call
+ * (:3863-4136), as ONE device pipeline: the sb_infer_topdown pipeline up to the instance network, then after every chunk
+ * of crops the global peaks (+ crop offsets) and the class-vector head (ClassVectorsHead, sleap/nn/heads.py:431-460:
+ * global max pool or Flatten of the tapped feature map -> num_fc_layers x (Dense + ReLU) -> Dense -> softmax), and after
+ * the last chunk one SciPy assignment of the frame's crops to the classes on -probability per frame, a match kept only
+ * where its probability is the crop's best (sleap/nn/identity.py:182-254 classify_peaks_from_vectors).
+ * Head arithmetic (the definition, DESIGN.md 5.14): every unit is the float64 sum of (double)x_i * (double)W_ij in input
+ * order plus (double)b_j, rounded once to float32, then ReLU; the softmax runs in float64 over the float32 logits
+ * (max subtracted, exp, divided by the sum) and is rounded once to float32.  A split-precision tap [lo | hi | hi] is read
+ * as float(lo) + float(hi), one fp32 add.
+ * The tap is the feature map the head reads: op-list buffer, physical channel offset, its C channels, and planes (1, or 3
+ * for the [lo | hi | hi] planes of a precision-2 fp16 tensor).  dense_weights: float32, Keras layout, packed in order
+ * pre_classification{i}_fc kernel (n_in, num_fc_units) + bias for i < num_fc_layers, then the ClassVectorsHead kernel
+ * (n_in, n_classes) + bias; n_in of the first layer is C with global_pool, else tap H * W * C (Flatten in H, W, C
+ * order).  The weights are copied at configure time and owned by the pipeline.
+ * Caps, checked at configure time (SB_ERR_UNSUPPORTED): n_classes <= SB_MAX_CLASSES; num_fc_units and, with global_pool,
+ * the tap's C <= SB_MAX_DENSE_WIDTH (the vectors kept in shared memory).  A Flatten input is read from global memory and
+ * has no cap.
+ * Outputs, class-indexed and NaN where no crop was assigned: out_points (B,n_classes,n_nodes,2), out_vals
+ * (B,n_classes,n_nodes), out_class_probs (B,n_classes); then as sb_infer_topdown: out_centroids (B,K,2),
+ * out_centroid_vals (B,K), out_n_valid (B) crops per frame, out_flags (B).  out_class_vectors (B,K,n_classes): every
+ * crop's class probabilities in crop order, NaN padded (may be NULL).
+ * sb_infer_topdown refuses a multi-class pipeline and sb_infer_topdown_multiclass a plain one; the chain rules of
+ * sb_topdown_configure hold.  Not covered: instance models trained at an input scale != 1. */
+#define SB_MAX_DENSE_WIDTH 4096
+typedef struct sb_topdown_multiclass_params {
+  sb_topdown_params topdown;        /* as sb_topdown_configure */
+  int32_t tap_buffer, tap_channel_offset, tap_channels, tap_planes;
+  int32_t n_classes, num_fc_layers, num_fc_units, global_pool;
+  const float* dense_weights;
+  int64_t n_dense_weights;
+} sb_topdown_multiclass_params;
+int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_params* params, int max_batch, int H, int W,
+                                    int C_in);
+int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
+                                float* out_centroids, float* out_centroid_vals, float* out_points, float* out_vals,
+                                float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors);
+/* The same post-processing on caller-supplied crops (no network): confidence maps (n_crops,H,W,n_nodes), optional learned
+ * offsets (n_crops,H,W,2*n_nodes), float32 feature maps (n_crops,Hf,Wf,Cf) read as the tap, optional crop offsets
+ * (n_crops,2), crop_sample_inds (n_crops) non-decreasing in [0, B).  Uses params->topdown.instance and the head fields;
+ * the model ids, the centroid stage and the tap fields are ignored.  Outputs as sb_infer_topdown_multiclass without the
+ * centroids: out_points, out_vals, out_class_probs (B,...); out_class_vectors (n_crops,n_classes) and out_features
+ * (n_crops, n_in of the first dense layer: the pooled or flattened feature vector) may be NULL. */
+int sb_topdown_multiclass_from_features(sb_handle_t h, const sb_topdown_multiclass_params* params, const float* cms_host,
+                                        int n_crops, int H, int W, int n_nodes, const float* offsets_host,
+                                        const float* features_host, int Hf, int Wf, int Cf, const float* crop_offsets_host,
+                                        const int32_t* crop_sample_inds, int B, float* out_points, float* out_vals,
+                                        float* out_class_probs, float* out_class_vectors, float* out_features);
+
 /* ---- flow shift for the optical-flow trackers ----------------------------------------------
  * sleap/nn/tracking.py:262-360 FlowCandidateMaker.flow_shift_instances = cv2.calcOpticalFlowPyrLK(prev, next,
  * pts, winSize=(window, window), maxLevel=max_levels, criteria=(EPS|COUNT, 30, 0.01)) on gray (cv2.COLOR_BGR2GRAY)

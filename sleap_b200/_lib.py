@@ -75,6 +75,15 @@ class TopdownParams(ctypes.Structure):
                 ("max_crops_per_call", c_int32)]
 
 
+class TopdownMultiClassParams(ctypes.Structure):
+    _fields_ = [("topdown", TopdownParams), ("tap_buffer", c_int32), ("tap_channel_offset", c_int32), ("tap_channels", c_int32),
+                ("tap_planes", c_int32), ("n_classes", c_int32), ("num_fc_layers", c_int32), ("num_fc_units", c_int32),
+                ("global_pool", c_int32), ("dense_weights", c_void_p), ("n_dense_weights", c_int64)]
+
+
+MAX_DENSE_WIDTH = 4096      # SB_MAX_DENSE_WIDTH (include/sleap_b200.h)
+
+
 class TrackerParams(ctypes.Structure):
     _fields_ = [("maker", c_int32), ("similarity", c_int32), ("match", c_int32), ("track_window", c_int32),
                 ("max_tracks", c_int32), ("max_tracking", c_int32), ("min_match_points", c_int32),
@@ -150,6 +159,12 @@ _SIGS = {
     "sb_infer_global": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "sb_topdown_configure": [c_void_p, POINTER(TopdownParams), c_int, c_int, c_int, c_int],
     "sb_infer_topdown": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_topdown_multiclass_configure": [c_void_p, POINTER(TopdownMultiClassParams), c_int, c_int, c_int, c_int],
+    "sb_infer_topdown_multiclass": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p],
+    "sb_topdown_multiclass_from_features": [c_void_p, POINTER(TopdownMultiClassParams), c_void_p, c_int, c_int, c_int, c_int,
+                                            c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p],
     "sb_centroid_configure": [c_void_p, c_int, POINTER(CentroidParams)],
     "sb_infer_centroids": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p],

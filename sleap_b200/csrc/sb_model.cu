@@ -117,6 +117,19 @@ static SbModel* configure_target(sb_handle_s* h, int id, const void* p) {
   return m;
 }
 
+int sb_net_size(sb_handle_s* h, const SbModel* m, int H, int W, int* Hres, int* Wres, int* Hnet, int* Wnet) {
+  const SbOp* pre = nullptr;
+  for (auto& op : m->ops) if (op.kind() == SB_OPK_PREPROCESS) { pre = &op; break; }
+  if (!pre) return sb_fail(h, SB_ERR_INVALID, "model has no preprocess op");
+  const float input_scale = pre->input_scale();
+  const int pad_stride = std::max(1, pre->pad_stride());
+  *Hres = H; *Wres = W;
+  if (input_scale != 1.0f) { *Wres = (int)((float)W * input_scale); *Hres = (int)((float)H * input_scale); }
+  *Hnet = ((*Hres + pad_stride - 1) / pad_stride) * pad_stride;
+  *Wnet = ((*Wres + pad_stride - 1) / pad_stride) * pad_stride;
+  return 0;
+}
+
 extern "C" {
 
 int sb_load_model(sb_handle_t h, const int32_t* ops, int n_ops, const float* weights, int64_t n_weights,
@@ -186,16 +199,8 @@ int sb_model_configure(sb_handle_t h, int model_id, int max_batch, int H, int W,
   if (!m) return SB_ERR_INVALID;
   if (max_batch <= 0 || H <= 0 || W <= 0 || (C_in != 1 && C_in != 3)) return sb_fail(h, SB_ERR_INVALID, "sb_model_configure: bad shape");
   SB_CUDA(h, cudaSetDevice(h->device));
-  // preprocess op defines the net input size
-  const SbOp* pre = nullptr;
-  for (auto& op : m->ops) if (op.kind() == SB_OPK_PREPROCESS) { pre = &op; break; }
-  if (!pre) return sb_fail(h, SB_ERR_INVALID, "model has no preprocess op");
-  const float input_scale = pre->input_scale();
-  const int pad_stride = std::max(1, pre->pad_stride());
-  int Hres = H, Wres = W;
-  if (input_scale != 1.0f) { Wres = (int)((float)W * input_scale); Hres = (int)((float)H * input_scale); }
-  const int Hnet = ((Hres + pad_stride - 1) / pad_stride) * pad_stride;
-  const int Wnet = ((Wres + pad_stride - 1) / pad_stride) * pad_stride;
+  int Hres, Wres, Hnet, Wnet;                  // the preprocess op defines the net input size
+  if (const int rc = sb_net_size(h, m, H, W, &Hres, &Wres, &Hnet, &Wnet)) return rc;
   for (auto& b : m->buffers) {
     if (Hnet % b.stride_den || Wnet % b.stride_den)
       return sb_fail(h, SB_ERR_INVALID, "net input %dx%d not divisible by stride %d (pad_to_stride too small)", Hnet, Wnet, b.stride_den);

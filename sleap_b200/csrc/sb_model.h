@@ -159,6 +159,10 @@ struct SbModel {
   double* trk_host[3] = {nullptr, nullptr, nullptr};   // pinned: collect slots 0 / 1, sb_infer_bottomup
 };
 
+// The network input of H x W frames as sb_model_configure plans it: resized by the PREPROCESS op's input_scale
+// (Hres x Wres), then padded to its pad_to_stride (Hnet x Wnet).  Fails for a model without a PREPROCESS op.
+int sb_net_size(sb_handle_s* h, const SbModel* m, int H, int W, int* Hres, int* Wres, int* Hnet, int* Wnet);
+
 // one forward pass: the production program, or the all-stores one
 int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B, bool all_stores = false);
 

@@ -1,19 +1,29 @@
 // Fused top-down pipeline on the device: frames -> centroid network -> local peaks -> per-frame top-k ->
 // crops of the RESIDENT frames -> centered-instance network -> global peaks (+ crop offsets) -> dense per-frame record.
 // One H2D copy of the frames and one D2H copy of the results per batch (+ a 4-byte crop count).
+// The multi-class (identity) form runs the class-vector head after every chunk's global peaks (k_class_vectors) and, after
+// the last chunk, one assignment of each frame's crops to the classes (k_td_class_assign) in place of k_td_pack.
 //
 // Reference: TopDownInferenceModel.call (sleap/nn/inference.py:2273-2311) = CentroidCrop.call (:1747-1966: network,
 // find_local_peaks, /input_scale + 0.5, tf.math.top_k(max_instances) :1879-1894, crop_bboxes on the full frames :1918-1927)
-// followed by FindInstancePeaks.call (:2059-2200: network on the crops, find_global_peaks, + crop_offsets).
+// followed by FindInstancePeaks.call (:2059-2200: network on the crops, find_global_peaks, + crop_offsets);
+// TopDownMultiClassInferenceModel.call (:4139-4210) with TopDownMultiClassFindPeaks.call (:3863-4136), ClassVectorsHead
+// (sleap/nn/heads.py:431-460) and classify_peaks_from_vectors (sleap/nn/identity.py:182-254).
 // Round 1 ran these as separate host-facing calls: centroids D2H -> host top-k -> frames H2D again -> crops D2H ->
 // crops H2D -> instance network (sleap_b200/nn/inference.py CentroidCrop / FindInstancePeaks, kept for the stage-level
 // surface and for models that need a pre-crop resize).
+//
+// The head's float64 sums use __dmul_rn / __dadd_rn: this file is built with multiply-add contraction on, and a fused
+// product would round differently from the definition (include/sleap_b200.h).
 #include <algorithm>
+#include <functional>
+#include <limits>
 #include <time.h>
 
 #include <math_constants.h>
 
 #include "sb_common.cuh"
+#include "sb_lsap.cuh"
 #include "sb_model.h"
 
 namespace {
@@ -74,6 +84,14 @@ __global__ void __launch_bounds__(256) k_td_flatten(const float* __restrict__ se
   }
 }
 
+// The frame's K centroid slots of a record: [K][2] centroids | [K] values, NaN past the frame's count (sel_cent NULL: all NaN)
+__device__ void td_write_centroids(const float* __restrict__ sel_cent, const float* __restrict__ sel_val, int b, int cnt, int K,
+                                   float* __restrict__ rc) {
+  float* rv = rc + K * 2;
+  for (int t = threadIdx.x; t < K * 2; t += blockDim.x) rc[t] = (sel_cent && t / 2 < cnt) ? sel_cent[(size_t)b * K * 2 + t] : CUDART_NAN_F;
+  for (int t = threadIdx.x; t < K; t += blockDim.x) rv[t] = (sel_val && t < cnt) ? sel_val[(size_t)b * K + t] : CUDART_NAN_F;
+}
+
 // Dense per-frame record: [K][2] centroids | [K] centroid values | [K][nodes][2] peaks | [K][nodes] peak values | n_valid | flags
 __global__ void __launch_bounds__(128) k_td_pack(const float* __restrict__ sel_cent, const float* __restrict__ sel_val,
                                                  const int* __restrict__ sel_count, const int* __restrict__ offsets,
@@ -82,12 +100,9 @@ __global__ void __launch_bounds__(128) k_td_pack(const float* __restrict__ sel_c
   const int b = blockIdx.x;
   const int cnt = sel_count[b], o = offsets[b];
   float* r = record + (size_t)b * width;
-  float* rc = r;
-  float* rv = rc + K * 2;
-  float* rp = rv + K;
+  float* rp = r + K * 3;
   float* rq = rp + (size_t)K * nodes * 2;
-  for (int t = threadIdx.x; t < K * 2; t += blockDim.x) rc[t] = (t / 2 < cnt) ? sel_cent[(size_t)b * K * 2 + t] : CUDART_NAN_F;
-  for (int t = threadIdx.x; t < K; t += blockDim.x) rv[t] = (t < cnt) ? sel_val[(size_t)b * K + t] : CUDART_NAN_F;
+  td_write_centroids(sel_cent, sel_val, b, cnt, K, r);
   for (int t = threadIdx.x; t < K * nodes * 2; t += blockDim.x) {
     const int k = t / (nodes * 2);
     rp[t] = (k < cnt) ? ipts[(size_t)(o + k) * nodes * 2 + (t - k * nodes * 2)] : CUDART_NAN_F;
@@ -102,24 +117,230 @@ __global__ void __launch_bounds__(128) k_td_pack(const float* __restrict__ sel_c
   }
 }
 
+// The class-vector head's shape: the tap (H x W x C logical channels), pooling, the dense stack and its packed weights
+struct TdHead {
+  int H, W, C;          // tap
+  int global_pool;      // 1: max over H x W; 0: Flatten in (H, W, C) order
+  int n_fc, units, n_classes;
+  int n_in;             // inputs of the first dense layer: C or H * W * C
+  int wmax;             // widest vector kept in shared memory (even)
+  const float* w;       // packed dense weights (include/sleap_b200.h)
+};
+
+__device__ __forceinline__ float tap_value(const float* q, int) { return q[0]; }
+__device__ __forceinline__ float tap_value(const __half* q, int hi) {
+  // split-precision planes [lo | hi | hi]: lo + hi, one fp32 add (DeviceModel._class_vectors)
+  return hi ? __fadd_rn(__half2float(q[0]), __half2float(q[hi])) : __half2float(q[0]);
+}
+
+// ------------------------------------------------------------------------------------------
+// ClassVectorsHead on the tap of n crops, one CTA per crop: pooled (or flattened) features, num_fc_layers x (Dense + ReLU),
+// Dense, softmax -> probs [n][n_classes].  Arithmetic as defined in include/sleap_b200.h.  tap: the crop-0 element of the
+// buffer at the tap's channel offset; pitch = the buffer's physical channels; hi = the channel distance of the hi plane
+// (0: one plane).  features_out (may be NULL): the first dense layer's input vector of every crop, [n][n_in].
+// ------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(128) k_class_vectors(const T* __restrict__ tap, int pitch, int hi, TdHead d,
+                                                       float* __restrict__ probs, float* __restrict__ features_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float* s_x = reinterpret_cast<float*>(smem_raw);       // [wmax] layer input
+  float* s_y = s_x + d.wmax;                             // [wmax] layer output
+  double* s_e = reinterpret_cast<double*>(s_y + d.wmax); // [n_classes] exp terms, then [n_classes] = their sum
+  __shared__ double s_sum;
+  const int crop = blockIdx.x, HW = d.H * d.W;
+  const T* base = tap + (size_t)crop * HW * pitch;
+  auto feat = [&](int i) -> float {                      // flat input i = (p, c), Flatten order
+    const int p = i / d.C, c = i - p * d.C;
+    return tap_value(base + (size_t)p * pitch + c, hi);
+  };
+  if (d.global_pool) {
+    for (int c = threadIdx.x; c < d.C; c += blockDim.x) {
+      float m = tap_value(base + c, hi);
+      for (int p = 1; p < HW; ++p) {                     // np.max: a NaN propagates
+        const float v = tap_value(base + (size_t)p * pitch + c, hi);
+        m = (v > m || v != v) ? v : m;
+      }
+      s_x[c] = m;
+      if (features_out) features_out[(size_t)crop * d.n_in + c] = m;
+    }
+  } else if (features_out) {
+    for (int i = threadIdx.x; i < d.n_in; i += blockDim.x) features_out[(size_t)crop * d.n_in + i] = feat(i);
+  }
+  __syncthreads();
+  const float* w = d.w;
+  int n_in = d.n_in;
+  for (int l = 0; l <= d.n_fc; ++l) {
+    const bool last = l == d.n_fc;
+    const int n_out = last ? d.n_classes : d.units;
+    const float* kern = w;
+    const float* bias = w + (size_t)n_in * n_out;
+    const bool flat_in = l == 0 && !d.global_pool;       // a Flatten input is read from the tap, not staged
+    for (int j = threadIdx.x; j < n_out; j += blockDim.x) {
+      double acc = 0.0;
+      for (int i = 0; i < n_in; ++i) {
+        const float x = flat_in ? feat(i) : s_x[i];
+        acc = __dadd_rn(acc, __dmul_rn((double)x, (double)kern[(size_t)i * n_out + j]));
+      }
+      const float z = __double2float_rn(__dadd_rn(acc, (double)bias[j]));
+      s_y[j] = (last || !(z < 0.f)) ? z : 0.f;            // ReLU as np.maximum(z, 0): NaN and -0 pass
+    }
+    __syncthreads();
+    float* t = s_x; s_x = s_y; s_y = t;
+    w = bias + n_out;
+    n_in = n_out;
+  }
+  // softmax in float64 over the float32 logits s_x[0..n_classes)
+  const int NC = d.n_classes;
+  float zmax = s_x[0];
+  for (int j = 1; j < NC; ++j) zmax = (s_x[j] > zmax || s_x[j] != s_x[j]) ? s_x[j] : zmax;
+  for (int j = threadIdx.x; j < NC; j += blockDim.x) s_e[j] = exp(__dadd_rn((double)s_x[j], -(double)zmax));
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int j = 0; j < NC; ++j) s = __dadd_rn(s, s_e[j]);
+    s_sum = s;
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < NC; j += blockDim.x) probs[(size_t)crop * NC + j] = __double2float_rn(__ddiv_rn(s_e[j], s_sum));
+}
+
+// ------------------------------------------------------------------------------------------
+// Identity grouping of the top-down multi-class step: one CTA per frame.  Its crops (rows, crop order) are assigned to
+// the classes (columns) by SciPy's assignment on -probability; a match is kept only where its probability is the crop's
+// best over all classes (group_class_peaks), whatever its peaks.  Record per frame: points [NC][nodes][2] | peak values
+// [NC][nodes] | class probabilities [NC] | centroids [K][2] | centroid values [K] | crop count | flags, padded to 4 floats.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) k_td_class_assign(const float* __restrict__ sel_cent, const float* __restrict__ sel_val,
+                                                         const int* __restrict__ sel_count, const int* __restrict__ offsets,
+                                                         const float* __restrict__ ipts, const float* __restrict__ ivals,
+                                                         const float* __restrict__ probs, int K, int nodes, int NC,
+                                                         const int* __restrict__ flags, float* __restrict__ record, int width) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int b = blockIdx.x;
+  const int cnt = sel_count[b], o = offsets[b];
+  const int L = max(K, NC), M = min(K, NC);
+  int* s_rows = reinterpret_cast<int*>(smem_raw + ((lsap_scratch_bytes(L) + 15) & ~(size_t)15));
+  int* s_cols = s_rows + M;
+  float* rp = record + (size_t)b * width;
+  float* rv = rp + (size_t)NC * nodes * 2;
+  float* rpr = rv + (size_t)NC * nodes;
+  float* rc = rpr + NC;
+  float* tail = rc + 3 * K;
+  for (int t = threadIdx.x; t < NC * nodes * 3 + NC; t += blockDim.x) rp[t] = CUDART_NAN_F;
+  td_write_centroids(sel_cent, sel_val, b, cnt, K, rc);
+  if (threadIdx.x == 0) {
+    tail[0] = (float)cnt;
+    tail[1] = flags ? (float)flags[b] : 0.f;
+    for (float* q = tail + 2; q < record + (size_t)(b + 1) * width; ++q) *q = 0.f;   // padding
+  }
+  __syncthreads();                       // NaN fill ordered before thread 0's stores
+  if (threadIdx.x != 0 || cnt == 0) return;
+  const float* P = probs + (size_t)o * NC;
+  LsapScratch s = carve_lsap(smem_raw, L);
+  const int nm = lsap_solve_cost([P, NC](int i, int k) { return -(double)P[(size_t)i * NC + k]; }, cnt, NC, s, s_rows, s_cols);
+  for (int q = 0; q < nm; ++q) {
+    const int i = s_rows[q], k = s_cols[q];
+    const float p = P[(size_t)i * NC + k];
+    float best = P[(size_t)i * NC];
+    for (int j = 1; j < NC; ++j) {       // np.max: a NaN propagates
+      const float v = P[(size_t)i * NC + j];
+      best = (v > best || v != v) ? v : best;
+    }
+    if (!(p == best)) continue;
+    for (int t = 0; t < nodes * 2; ++t) rp[(size_t)k * nodes * 2 + t] = ipts[(size_t)(o + i) * nodes * 2 + t];
+    for (int t = 0; t < nodes; ++t) rv[(size_t)k * nodes + t] = ivals[(size_t)(o + i) * nodes + t];
+    rpr[k] = p;
+  }
+}
+
+size_t td_class_record_width(int NC, int nodes, int K) {
+  return (((size_t)NC * nodes * 3 + NC + 3 * (size_t)K + 2) + 3) & ~(size_t)3;
+}
+
+size_t class_vectors_smem(const TdHead& d) { return (size_t)2 * d.wmax * sizeof(float) + (size_t)d.n_classes * sizeof(double); }
+
+// k_class_vectors on n crops of a tap in fp32 or fp16 storage
+int launch_class_vectors(sb_handle_s* h, const void* tap, bool half, int pitch, int hi, const TdHead& d, int n, float* probs,
+                         float* features_out) {
+  if (n <= 0) return 0;
+  const size_t sm = class_vectors_smem(d);
+  if (half)
+    k_class_vectors<__half><<<n, 128, sm, h->stream>>>((const __half*)tap, pitch, hi, d, probs, features_out);
+  else
+    k_class_vectors<float><<<n, 128, sm, h->stream>>>((const float*)tap, pitch, hi, d, probs, features_out);
+  SB_CHECK_LAUNCH(h);
+  return 0;
+}
+
+int launch_class_assign(sb_handle_s* h, const float* sel_cent, const float* sel_val, const int* sel_count, const int* offsets,
+                        const float* ipts, const float* ivals, const float* probs, int B, int K, int nodes, int NC, const int* flags,
+                        float* record) {
+  const int L = std::max(K, NC), M = std::min(K, NC);
+  const size_t sm = ((lsap_scratch_bytes(L) + 15) & ~(size_t)15) + 2 * (size_t)M * sizeof(int);
+  if (sm > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(k_td_class_assign, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
+    if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "class assignment smem %zu: %s", sm, cudaGetErrorString(e));
+  }
+  k_td_class_assign<<<B, 128, sm, h->stream>>>(sel_cent, sel_val, sel_count, offsets, ipts, ivals, probs, K, nodes, NC, flags, record,
+                                               (int)td_class_record_width(NC, nodes, K));
+  SB_CHECK_LAUNCH(h);
+  return 0;
+}
+
+// The head fields of the parameters (everything but the tap's storage), checked against the tap's logical shape H x W x C:
+// caps, layer sizes and the length of the packed weights.
+int head_from_params(sb_handle_s* h, const sb_topdown_multiclass_params* p, int H, int W, int C, TdHead& d) {
+  if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES)
+    return sb_fail(h, SB_ERR_UNSUPPORTED, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
+  if (p->num_fc_layers < 0 || (p->num_fc_layers > 0 && p->num_fc_units < 1) || H <= 0 || W <= 0 || C <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "class-vector head: bad layer sizes");
+  if (p->num_fc_units > SB_MAX_DENSE_WIDTH || (p->global_pool && C > SB_MAX_DENSE_WIDTH))
+    return sb_fail(h, SB_ERR_UNSUPPORTED, "class-vector head: dense width above %d", SB_MAX_DENSE_WIDTH);
+  d.H = H; d.W = W; d.C = C;
+  d.global_pool = p->global_pool != 0;
+  d.n_fc = p->num_fc_layers; d.units = d.n_fc > 0 ? p->num_fc_units : 0; d.n_classes = p->n_classes;
+  d.n_in = d.global_pool ? C : H * W * C;
+  d.wmax = std::max(std::max(d.global_pool ? C : 0, d.units), d.n_classes);
+  d.wmax += d.wmax & 1;                                     // keeps the float64 exp terms 8-byte aligned
+  d.w = nullptr;
+  int64_t need = 0, n_in = d.n_in;
+  for (int l = 0; l <= d.n_fc; ++l) {
+    const int64_t n_out = l == d.n_fc ? d.n_classes : d.units;
+    need += n_in * n_out + n_out;
+    n_in = n_out;
+  }
+  if (!p->dense_weights || p->n_dense_weights != need)
+    return sb_fail(h, SB_ERR_INVALID, "class-vector head: %lld dense weights given, %lld expected", (long long)p->n_dense_weights,
+                   (long long)need);
+  return 0;
+}
+
 }  // namespace
 
 struct SbTopdown {
   sb_topdown_params p{};
   SbModel* inst = nullptr;
   unsigned gen_c = 0, gen_i = 0;    // chain_gen of the centroid and the instance model when it was configured
-  int K = 0, nodes = 0, width = 0, Bmax = 0, crop_elem = 1;
+  int K = 0, nodes = 0, width = 0, Bmax = 0;
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
   void* crops = nullptr;
   float* record_host = nullptr;
   int* total_host = nullptr;
+  // multi-class form (sb_topdown_multiclass_configure)
+  bool multiclass = false;
+  TdHead head{};
+  int tap_buf = -1, tap_coff = 0, tap_hi = 0;
+  bool tap_half = false, all_stores = false;   // fp16 storage; the production program elides the tap buffer
+  float* dense = nullptr;                      // packed dense weights
+  float* probs = nullptr;                      // [Bmax * K][n_classes] per-crop class probabilities
 };
 
 void sb_topdown_free(SbModel* m) {
   SbTopdown* t = m->td;
   if (!t) return;
-  void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample, t->offsets, t->total, t->crops};
+  void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
+                 t->offsets, t->total, t->crops, t->dense, t->probs};
   for (void* p : dev) if (p) cudaFree(p);
   if (t->record_host) cudaFreeHost(t->record_host);
   if (t->total_host) cudaFreeHost(t->total_host);
@@ -127,30 +348,39 @@ void sb_topdown_free(SbModel* m) {
   m->td = nullptr;
 }
 
-extern "C" {
+namespace {
 
-int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in) {
-  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: null argument");
+// The arguments both top-down configure calls check before anything is dropped
+int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, SbModel** mc, SbModel** mi) {
   static const char* const bad_ids = "sb_topdown_configure: bad model ids";
-  SbModel* mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
-  SbModel* mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
-  if (!mc || !mi || mc == mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
+  *mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
+  *mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
+  if (!*mc || !*mi || *mc == *mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
   if (p->crop_size <= 0 || p->max_centroids_per_frame <= 0 || p->max_crops_per_call <= 0 || max_batch <= 0)
     return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: bad sizes");
   if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_configure: more than 1024 frames per batch");
+  const int nb = (int)(*mi)->buffers.size();
+  if (p->instance.cms_buffer < 0 || p->instance.cms_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
+  return 0;
+}
+
+// Configures both networks and their chains, then the pipeline with a record of `width` floats per frame (the centroid
+// configure drops the previous pipeline).  On success mc->td is the new pipeline.
+int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in, SbModel* mc, SbModel* mi,
+                  int n_classes) {
   SB_CUDA(h, cudaSetDevice(h->device));
   int rc;
   if ((rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in))) return rc;
   if ((rc = sb_model_configure(h, p->instance_model, p->max_crops_per_call, p->crop_size, p->crop_size, C_in))) return rc;
   if ((rc = sb_centroid_configure(h, p->centroid_model, &p->centroid))) return rc;
   if ((rc = sb_global_configure(h, p->instance_model, &p->instance))) return rc;
-  SbTopdown* t = new SbTopdown();           // the centroid configure dropped the previous one
+  SbTopdown* t = new SbTopdown();
   mc->td = t;
   t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
   t->gen_c = mc->chain_gen; t->gen_i = mi->chain_gen;
   t->nodes = mi->buffers[p->instance.cms_buffer].C;
-  t->width = t->K * (3 + t->nodes * 3) + 2;
-  t->crop_elem = 1;                                                    // uint8 frames (float frames: 4, decided per call)
+  t->multiclass = n_classes > 0;
+  t->width = t->multiclass ? (int)td_class_record_width(n_classes, t->nodes, t->K) : t->K * (3 + t->nodes * 3) + 2;
   const size_t N = (size_t)max_batch * t->K;
   auto A = [&](void** q, size_t bytes) { return cudaMalloc(q, bytes + 16) == cudaSuccess; };
   const bool ok = A((void**)&t->sel_cent, N * 2 * 4) && A((void**)&t->sel_val, N * 4) && A((void**)&t->sel_count, (size_t)max_batch * 4) &&
@@ -158,7 +388,8 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batc
                   A((void**)&t->offsets, ((size_t)max_batch + 1) * 4) && A((void**)&t->total, 4) &&
                   A((void**)&t->ipts, N * t->nodes * 2 * 4) && A((void**)&t->ivals, N * t->nodes * 4) &&
                   A((void**)&t->record, (size_t)max_batch * t->width * 4) &&
-                  A(&t->crops, (size_t)p->max_crops_per_call * p->crop_size * p->crop_size * C_in * 4);
+                  A(&t->crops, (size_t)p->max_crops_per_call * p->crop_size * p->crop_size * C_in * 4) &&
+                  (!t->multiclass || A((void**)&t->probs, N * n_classes * 4));
   if (!ok || cudaHostAlloc((void**)&t->record_host, (size_t)max_batch * t->width * 4, cudaHostAllocDefault) != cudaSuccess ||
       cudaHostAlloc((void**)&t->total_host, 4, cudaHostAllocDefault) != cudaSuccess) {
     sb_topdown_free(mc);
@@ -167,16 +398,34 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batc
   return SB_OK;
 }
 
-int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B, float* out_centroids,
-                     float* out_centroid_vals, float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid,
-                     int32_t* out_flags) {
-  SbModel* mc = chain_model(h, centroid_model_id, SB_CHAIN_ANY, "top-down pipeline not configured");
-  if (!mc || !mc->td) return sb_fail(h, SB_ERR_INVALID, "top-down pipeline not configured");
+// The pipeline of centroid model `id` when it is of the wanted form and neither model was reconfigured since
+SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass) {
+  static const char* const none = "top-down pipeline not configured";
+  SbModel* mc = chain_model(h, id, SB_CHAIN_ANY, none);
+  if (!mc) return nullptr;
   SbTopdown* t = mc->td;
+  if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
+  if (t->multiclass != multiclass) {
+    sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_infer_topdown"
+                                          : "top-down pipeline is multi-class: call sb_infer_topdown_multiclass");
+    return nullptr;
+  }
   SbModel* mi = t->inst;
-  // a configure call on either model outside sb_topdown_configure moved its chain_gen (sb_model_configure included)
-  if (mc->chain != SB_CHAIN_CENTROID || mc->chain_gen != t->gen_c || mi->chain != SB_CHAIN_GLOBAL || mi->chain_gen != t->gen_i)
-    return sb_fail(h, SB_ERR_INVALID, "top-down pipeline: a model was reconfigured; call sb_topdown_configure again");
+  // a configure call on either model outside the pipeline's configure moved its chain_gen (sb_model_configure included)
+  if (mc->chain != SB_CHAIN_CENTROID || mc->chain_gen != t->gen_c || mi->chain != SB_CHAIN_GLOBAL || mi->chain_gen != t->gen_i) {
+    sb_fail(h, SB_ERR_INVALID, "top-down pipeline: a model was reconfigured; call %s again",
+            multiclass ? "sb_topdown_multiclass_configure" : "sb_topdown_configure");
+    return nullptr;
+  }
+  return t;
+}
+
+// One batch through the pipeline: frames up, centroid network, local peaks, top-k, crop list (the one mid-pipeline sync,
+// for the crop count), then per chunk of crops the crop kernel, the instance network, the global peaks and chunk(c0, n);
+// then pack() writes the records, which come back into t->record_host.
+int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_host, int frames_are_u8, int B, bool all_stores,
+                const std::function<int(int c0, int n)>& chunk, const std::function<int()>& pack) {
+  SbModel* mi = t->inst;
   if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
   SB_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
@@ -213,13 +462,12 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
     // crops of the frames already resident in HBM (uint8 frames: float -> uint8 truncation, as tf.cast in crop_bboxes)
     if ((rc = sbk_crop(h, mc->frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
                        cs, cs, t->crops, frames_are_u8))) return rc;
-    if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n))) return rc;
+    if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n, all_stores))) return rc;
     if ((rc = sbk_global_peaks(h, (const float*)ib.dev, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
                                t->ipts + (size_t)c0 * t->nodes * 2, t->ivals + (size_t)c0 * t->nodes))) return rc;
+    if ((rc = chunk(c0, n))) return rc;
   }
-  k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags, t->record,
-                              t->width);
-  SB_CHECK_LAUNCH(h);
+  if ((rc = pack())) return rc;
   SB_CUDA(h, cudaMemcpyAsync(t->record_host, t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, s));
   SB_CUDA(h, cudaStreamSynchronize(s));
   if (dbg) {
@@ -227,10 +475,170 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
     fprintf(stderr, "[sb_infer_topdown] B=%d crops=%d: H2D %.3f ms, centroid stage %.3f ms, instance stage + D2H %.3f ms\n", B, total, t1 - t0,
             t2 - t1, t3 - t2);
   }
+  return SB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in) {
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: null argument");
+  SbModel *mc, *mi;
+  if (const int rc = check_topdown(h, p, max_batch, &mc, &mi)) return rc;
+  return topdown_setup(h, p, max_batch, H, W, C_in, mc, mi, 0);
+}
+
+int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B, float* out_centroids,
+                     float* out_centroid_vals, float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid,
+                     int32_t* out_flags) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+  if (!t) return SB_ERR_INVALID;
+  SbModel* mc = h->models[centroid_model_id];
+  auto pack = [&]() {
+    k_td_pack<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags,
+                                        t->record, t->width);
+    SB_CHECK_LAUNCH(h);
+    return 0;
+  };
+  const int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, false, [](int, int) { return 0; }, pack);
+  if (rc) return rc;
   const size_t K = t->K, nd = t->nodes;
   sb_split_records(t->record_host, B, t->width,
                    {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
                    {out_n_valid, out_flags});
+  return SB_OK;
+}
+
+int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_params* p, int max_batch, int H, int W, int C_in) {
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_configure: null argument");
+  SbModel *mc, *mi;
+  int rc = check_topdown(h, &p->topdown, max_batch, &mc, &mi);
+  if (rc) return rc;
+  // the tap: a buffer of the instance network holding C logical channels at the offset, in one plane or [lo | hi | hi]
+  if (p->tap_buffer < 0 || p->tap_buffer >= (int)mi->buffers.size() || p->tap_channels <= 0 || p->tap_channel_offset < 0 ||
+      (p->tap_planes != 1 && p->tap_planes != 3))
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_configure: bad class-vector tap");
+  const SbBuffer& tb = mi->buffers[p->tap_buffer];
+  const bool half = !(tb.f32 || mi->precision == 1);
+  if (p->tap_channel_offset + p->tap_planes * p->tap_channels > tb.C || (p->tap_planes == 3 && !(half && mi->precision == 2)))
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_configure: the tap does not fit its buffer's storage");
+  int Hres, Wres, Hnet, Wnet;
+  if ((rc = sb_net_size(h, mi, p->topdown.crop_size, p->topdown.crop_size, &Hres, &Wres, &Hnet, &Wnet))) return rc;
+  if (Hnet % tb.stride_den || Wnet % tb.stride_den) return sb_fail(h, SB_ERR_INVALID, "crop size not divisible by the tap's stride");
+  TdHead d;
+  if ((rc = head_from_params(h, p, Hnet / tb.stride_den, Wnet / tb.stride_den, p->tap_channels, d))) return rc;
+  // arguments checked: from here the previous chains are dropped
+  if ((rc = topdown_setup(h, &p->topdown, max_batch, H, W, C_in, mc, mi, p->n_classes))) return rc;
+  SbTopdown* t = mc->td;
+  t->head = d;
+  t->tap_buf = p->tap_buffer; t->tap_coff = p->tap_channel_offset; t->tap_hi = p->tap_planes == 3 ? p->tap_channels : 0;
+  t->tap_half = half;
+  t->all_stores = mi->buf_elided[p->tap_buffer] != 0;       // the rule sb_model_forward follows
+  if (cudaMalloc((void**)&t->dense, (size_t)p->n_dense_weights * 4) != cudaSuccess ||
+      cudaMemcpy(t->dense, p->dense_weights, (size_t)p->n_dense_weights * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
+    sb_topdown_free(mc);
+    return sb_fail(h, SB_ERR_CUDA, "sb_topdown_multiclass_configure: dense weights");
+  }
+  t->head.w = t->dense;
+  return SB_OK;
+}
+
+int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
+                                float* out_centroids, float* out_centroid_vals, float* out_points, float* out_vals,
+                                float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, true);
+  if (!t) return SB_ERR_INVALID;
+  SbModel* mc = h->models[centroid_model_id];
+  const SbBuffer& tb = t->inst->buffers[t->tap_buf];
+  const int NC = t->head.n_classes;
+  const size_t esz = t->tap_half ? 2 : 4;
+  auto chunk = [&](int c0, int n) {
+    return launch_class_vectors(h, (const char*)tb.dev + (size_t)t->tap_coff * esz, t->tap_half, tb.C, t->tap_hi, t->head, n,
+                                t->probs + (size_t)c0 * NC, nullptr);
+  };
+  auto pack = [&]() {
+    return launch_class_assign(h, t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->probs, B, t->K, t->nodes,
+                               NC, mc->ws.flags, t->record);
+  };
+  int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, t->all_stores, chunk, pack);
+  if (rc) return rc;
+  const size_t K = t->K, n1 = (size_t)NC * t->nodes;
+  if (out_class_vectors) {                                   // the crops' probabilities, scattered to (frame, slot)
+    const int total = *t->total_host;
+    std::vector<float> pr((size_t)total * NC);
+    if (total > 0) SB_CUDA(h, cudaMemcpy(pr.data(), t->probs, pr.size() * 4, cudaMemcpyDeviceToHost));
+    int o = 0;
+    for (int b = 0; b < B; ++b) {
+      const int cnt = (int)t->record_host[(size_t)b * t->width + n1 * 3 + NC + 3 * K];
+      float* dst = out_class_vectors + (size_t)b * K * NC;
+      std::fill(dst, dst + K * NC, std::numeric_limits<float>::quiet_NaN());
+      std::copy(pr.begin() + (size_t)o * NC, pr.begin() + (size_t)(o + cnt) * NC, dst);
+      o += cnt;
+    }
+  }
+  sb_split_records(t->record_host, B, t->width,
+                   {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}, {out_centroids, K * 2}, {out_centroid_vals, K}},
+                   {out_n_valid, out_flags});
+  return SB_OK;
+}
+
+int sb_topdown_multiclass_from_features(sb_handle_t h, const sb_topdown_multiclass_params* p, const float* cms_host, int n_crops, int H,
+                                        int W, int n_nodes, const float* offsets_host, const float* features_host, int Hf, int Wf,
+                                        int Cf, const float* crop_offsets_host, const int32_t* crop_sample_inds, int B,
+                                        float* out_points, float* out_vals, float* out_class_probs, float* out_class_vectors,
+                                        float* out_features) {
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "null handle / params");
+  if ((n_crops > 0 && (!cms_host || !features_host || !crop_sample_inds)) || !out_points || !out_vals || !out_class_probs)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_from_features: null argument");
+  if (n_crops < 0 || B <= 0 || H <= 0 || W <= 0 || n_nodes <= 0 || n_nodes > 256)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_from_features: bad shape");
+  TdHead d;
+  int rc = head_from_params(h, p, Hf, Wf, Cf, d);
+  if (rc) return rc;
+  std::vector<int> count(B, 0), offsets(B + 1, 0);
+  for (int i = 0; i < n_crops; ++i) {
+    const int b = crop_sample_inds[i];
+    if (b < 0 || b >= B || (i > 0 && b < crop_sample_inds[i - 1]))
+      return sb_fail(h, SB_ERR_INVALID, "crop sample indices must be non-decreasing in [0, B)");
+    ++count[b];
+  }
+  int K = 1;
+  for (int b = 0; b < B; ++b) { offsets[b + 1] = offsets[b] + count[b]; K = std::max(K, count[b]); }
+  SB_CUDA(h, cudaSetDevice(h->device));
+  const int NC = d.n_classes, nc = std::max(n_crops, 1);
+  SbScratch s(h);
+  const float *cms = nullptr, *off = nullptr, *feats = nullptr, *coff = nullptr, *dense = nullptr;
+  const int *d_count = nullptr, *d_offsets = nullptr;
+  float *pts, *vals, *probs, *rec, *fout = nullptr;
+  const size_t width = td_class_record_width(NC, n_nodes, K);
+  const size_t ncm = (size_t)n_crops * H * W * n_nodes;
+  if ((rc = sb_global_scratch_alloc(h, s.gs, nc, H, n_nodes)) || (rc = s.alloc(&pts, (size_t)nc * n_nodes * 2)) ||
+      (rc = s.alloc(&vals, (size_t)nc * n_nodes)) || (rc = s.alloc(&probs, (size_t)nc * NC)) || (rc = s.alloc(&rec, (size_t)B * width)) ||
+      (out_features && (rc = s.alloc(&fout, (size_t)nc * d.n_in))) ||
+      (rc = s.upload(p->dense_weights, (size_t)p->n_dense_weights, &dense)) || (rc = s.upload(count.data(), (size_t)B, &d_count)) ||
+      (rc = s.upload(offsets.data(), (size_t)B + 1, &d_offsets)))
+    return rc;
+  d.w = dense;
+  if (n_crops > 0) {
+    if ((rc = s.upload(cms_host, ncm, &cms)) || (rc = s.upload(offsets_host, 2 * ncm, &off, true)) ||
+        (rc = s.upload(features_host, (size_t)n_crops * Hf * Wf * Cf, &feats)) ||
+        (rc = s.upload(crop_offsets_host, (size_t)n_crops * 2, &coff, true)))
+      return rc;
+    const sb_global_params& gp = p->topdown.instance;
+    SbPeakParams pp{gp.peak_threshold, gp.refinement, gp.integral_patch_size, (float)gp.output_stride, gp.input_scale};
+    if ((rc = sbk_global_peaks(h, cms, off, n_crops, H, W, n_nodes, pp, coff, s.gs.part, s.gs.chunks, s.gs.rpc, pts, vals)) ||
+        (rc = launch_class_vectors(h, feats, false, Cf, 0, d, n_crops, probs, fout)))
+      return rc;
+  }
+  if ((rc = launch_class_assign(h, nullptr, nullptr, d_count, d_offsets, pts, vals, probs, B, K, n_nodes, NC, nullptr, rec))) return rc;
+  std::vector<float> rec_host((size_t)B * width);
+  if ((rc = s.to_host(rec_host.data(), rec, rec_host.size())) ||
+      (n_crops > 0 && (rc = s.to_host(out_class_vectors, probs, (size_t)n_crops * NC, true))) ||
+      (n_crops > 0 && (rc = s.to_host(out_features, (const float*)fout, (size_t)n_crops * d.n_in, true))) || (rc = s.sync()))
+    return rc;
+  const size_t n1 = (size_t)NC * n_nodes;
+  sb_split_records(rec_host.data(), B, width, {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}}, {});
   return SB_OK;
 }
 

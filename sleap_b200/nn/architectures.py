@@ -404,7 +404,8 @@ def spec_from_config(model_cfg: dict, skeleton_nodes=None, skeleton_edges=None):
             raise ValueError("Classes must be provided when the head configuration is incomplete.")
         heads.append(dict(name="CenteredInstanceConfmapsHead", channels=len(part_names), output_stride=cm["output_stride"]))
         # ClassVectorsHead (heads.py:431-460): global max pool / flatten -> Dense + ReLU x num_fc_layers -> Dense + softmax.
-        # Not a convolution: the engine exposes the feature map it taps ("vector" head), the few dense layers run on the host
+        # Not a convolution: the engine exposes the feature map it taps ("vector" head); its dense layers run in the fused
+        # top-down multi-class step (k_class_vectors), or on the host after DeviceModel.forward
         heads.append(dict(name="ClassVectorsHead", channels=len(classes), output_stride=cv["output_stride"], vector=True,
                           num_fc_layers=int(cv.get("num_fc_layers", 1)), num_fc_units=int(cv.get("num_fc_units", 64)),
                           global_pool=bool(cv.get("global_pool", True))))

@@ -19,10 +19,12 @@ from typing import Dict, List, Optional
 import numpy as np
 
 from sleap_b200 import _lib
-from sleap_b200._lib import BottomUpParams, CentroidParams, GlobalParams, MultiClassParams, TopdownParams, f32, i32, ptr
+from sleap_b200._lib import (BottomUpParams, CentroidParams, GlobalParams, MultiClassParams, TopdownMultiClassParams, TopdownParams,
+                             f32, i32, ptr)
 from sleap_b200.nn import architectures as arch
 from sleap_b200.nn import paf_grouping, peak_finding
-from sleap_b200.nn.model import DeviceModel, PRECISION_FP16, PRECISION_FP32, chain_key, load_weights, load_weights_npz
+from sleap_b200.nn.model import (DeviceModel, PRECISION_FP16, PRECISION_FP32, chain_key, head_spec, load_weights, load_weights_npz,
+                                 pack_dense_weights)
 
 REFINE = peak_finding.REFINE
 
@@ -400,6 +402,31 @@ class CentroidInferenceModel(InferenceModel):
         return res
 
 
+def _topdown_params(cc, fp):
+    """TopdownParams of the fused pipeline over centroid layer ``cc`` and instance layer ``fp``, and its K (centroids kept
+    per frame)."""
+    K = int(cc.max_instances) if cc.max_instances else int(cc.max_peaks_per_sample)
+    return TopdownParams(cc.keras_model.model_id, fp.keras_model.model_id, cc.params(), fp.params(), int(cc.crop_size),
+                         int(cc.max_instances or 0), K, int(fp.max_crops_per_call)), K
+
+
+def _configure_topdown(cc, fp, fn_name, p, shape, *arrays):
+    """Configures the fused top-down pipeline with ``fn_name`` (``sb_topdown_configure`` or
+    ``sb_topdown_multiclass_configure``) for frames of ``shape`` (B, H, W, C) unless both models already run it with these
+    parameters; ``arrays`` are the ones the pointer fields of ``p`` point to."""
+    B, H, W, C = shape
+    mc, mi = cc.keras_model, fp.keras_model
+    # the pipeline's record on both models: a staged call on either one reconfigures its own chain, and this one again
+    record = (fn_name, chain_key(p, *arrays))
+    cap = max(B, mc.configured_for[0]) if mc.chain == record else B
+    if mc.chain != record or mi.chain != record or mc.configured_for != (cap, H, W, C):
+        mc.chain = mi.chain = None
+        mc.handle.call(fn_name, byref(p), cap, H, W, C)
+        mc.configured_for = (cap, H, W, C)
+        mi.configured_for = (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C)
+        mc.chain = mi.chain = record
+
+
 class TopDownInferenceModel(InferenceModel):
     """sleap/nn/inference.py:2246-2311."""
 
@@ -421,18 +448,8 @@ class TopDownInferenceModel(InferenceModel):
         imgs = cc._prep(imgs)
         B, H, W, C = imgs.shape
         mc, mi = cc.keras_model, fp.keras_model
-        K = int(cc.max_instances) if cc.max_instances else int(cc.max_peaks_per_sample)
-        p = TopdownParams(mc.model_id, mi.model_id, cc.params(), fp.params(), int(cc.crop_size), int(cc.max_instances or 0), K,
-                          int(fp.max_crops_per_call))
-        # the pipeline's record on both models: a staged call on either one reconfigures its own chain, and this one again
-        record = ("sb_topdown_configure", chain_key(p))
-        cap = max(B, mc.configured_for[0]) if mc.chain == record else B
-        if mc.chain != record or mi.chain != record or mc.configured_for != (cap, H, W, C):
-            mc.chain = mi.chain = None
-            mc.handle.call("sb_topdown_configure", byref(p), cap, H, W, C)
-            mc.configured_for = (cap, H, W, C)
-            mi.configured_for = (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C)
-            mc.chain = mi.chain = record
+        p, K = _topdown_params(cc, fp)
+        _configure_topdown(cc, fp, "sb_topdown_configure", p, (B, H, W, C))
         n_nodes = head_channels(mi, fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
@@ -840,9 +857,10 @@ class BottomUpMultiClassInferenceModel(InferenceModel):
 class TopDownMultiClassFindPeaks(InferenceLayer):
     """sleap/nn/inference.py:3863-4136: centered-instance confidence maps + class vectors on crops -> global peaks ->
     one instance per class and sample (``identity.classify_peaks_from_vectors``).  Confidence maps and the class-vector
-    head's feature map come from one device pass; the head's dense layers and the grouping run on the host."""
+    head's feature map come from one device pass; the head's dense layers and the grouping run on the host.  (Inside a
+    fused TopDownMultiClassInferenceModel both run on the device instead.)"""
 
-    HEAD = "CenteredInstanceConfmapsHead"
+    HEAD, CLASS_VECTORS = "CenteredInstanceConfmapsHead", "ClassVectorsHead"
 
     def __init__(self, keras_model, input_scale=1.0, output_stride=None, peak_threshold=0.2, refinement="local",
                  integral_patch_size=5, return_confmaps=False, return_class_vectors=False, optimal_grouping=True,
@@ -861,6 +879,15 @@ class TopDownMultiClassFindPeaks(InferenceLayer):
         self.return_class_vectors = return_class_vectors
         self.optimal_grouping = optimal_grouping
         self.max_crops_per_call = max_crops_per_call
+        self.class_head = head_spec(keras_model.spec, self.CLASS_VECTORS)
+        self.dense = pack_dense_weights(self.class_head, keras_model.dense_weights)     # what the fused step uploads
+
+    def params(self) -> GlobalParams:
+        """The global-peak chain of the fused top-down step (find_global_peaks, or with offsets, x output_stride)."""
+        heads = self.keras_model.cm.head_buffers
+        return GlobalParams(heads[self.HEAD], heads["OffsetRefinementHead"] if self.has_offsets else -1, int(self.output_stride),
+                            float(self.peak_threshold), REFINE.get(self.refinement, 0), int(self.integral_patch_size),
+                            float(self.input_scale))
 
     def call(self, inputs):
         from sleap_b200.nn import identity
@@ -913,16 +940,90 @@ class TopDownMultiClassFindPeaks(InferenceLayer):
         return out
 
 
+def topdown_multiclass_params(topdown, tap, head, dense):
+    """TopdownMultiClassParams over ``topdown`` (TopdownParams) for the class-vector head ``head`` (its spec entry) reading
+    ``tap`` (an entry of ``CompiledModel.vector_taps``; None: no tap) with the packed weights ``dense``, which must outlive
+    the call that takes the parameters."""
+    tap = tap or dict(buf=-1, coff=0, C=0, planes=1)
+    return TopdownMultiClassParams(topdown, int(tap["buf"]), int(tap["coff"]), int(tap["C"]), int(tap["planes"]), int(head["channels"]),
+                                   int(head.get("num_fc_layers", 1)), int(head.get("num_fc_units", 64)),
+                                   int(bool(head.get("global_pool", True))), dense.ctypes.data, int(dense.size))
+
+
+def topdown_multiclass_from_features(cms, features, crop_sample_inds, n_samples, head, dense_weights, output_stride,
+                                     peak_threshold=0.2, refinement="local", integral_patch_size=5, offsets=None, crop_offsets=None,
+                                     input_scale=1.0, handle=None):
+    """The post-processing of the fused top-down multi-class step (global peaks x output_stride + crop offsets,
+    k_class_vectors, k_td_class_assign) on caller-supplied crops: confidence maps (n_crops,H,W,n_nodes), feature maps
+    (n_crops,Hf,Wf,Cf) as the class-vector head ``head`` taps them, the head's dense weights (``{layer: {kernel, bias}}``)
+    and the crops' frames (non-decreasing) -- the parity entry point.  Returns the fused keys instance_peaks
+    (n_samples,n_classes,n_nodes,2), instance_peak_vals, instance_scores (n_samples,n_classes), plus class_vectors
+    (n_crops,n_classes) and features (n_crops, the first dense layer's input)."""
+    h = handle or _lib.default_handle()
+    cms, features = f32(cms), f32(features)
+    n, H, W, N = cms.shape
+    _, Hf, Wf, Cf = features.shape
+    dense = pack_dense_weights(head, dense_weights)
+    gp = GlobalParams(-1, -1, int(output_stride), float(peak_threshold), REFINE.get(refinement, 0), int(integral_patch_size),
+                      float(input_scale))
+    p = topdown_multiclass_params(TopdownParams(-1, -1, CentroidParams(), gp, 0, 0, 0, 0), None, head, dense)
+    B, NC = int(n_samples), p.n_classes
+    pts = np.zeros((B, NC, N, 2), np.float32); vals = np.zeros((B, NC, N), np.float32); probs = np.zeros((B, NC), np.float32)
+    cvec = np.zeros((n, NC), np.float32)
+    feats = np.zeros((n, Cf if p.global_pool else Hf * Wf * Cf), np.float32)
+    off = None if offsets is None else f32(offsets)
+    co = None if crop_offsets is None else f32(crop_offsets).reshape(n, 2)
+    h.call("sb_topdown_multiclass_from_features", byref(p), ptr(cms), n, H, W, N, ptr(off), ptr(features), Hf, Wf, Cf, ptr(co),
+           ptr(i32(crop_sample_inds)), B, ptr(pts), ptr(vals), ptr(probs), ptr(cvec), ptr(feats))
+    return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "class_vectors": cvec, "features": feats}
+
+
 class TopDownMultiClassInferenceModel(InferenceModel):
-    """sleap/nn/inference.py:4139-4210: centroid stage (model or ground truth) -> TopDownMultiClassFindPeaks."""
+    """sleap/nn/inference.py:4139-4210: centroid stage (model or ground truth) -> TopDownMultiClassFindPeaks.
+
+    With a centroid model the whole chain runs as one device step (``sb_infer_topdown_multiclass``): centroids, top-k,
+    crops, instance network, global peaks, the class-vector head (k_class_vectors) and the per-frame assignment of crops
+    to classes (k_td_class_assign).  ``fused = False`` keeps the staged path (ground-truth centroids always use it)."""
 
     def __init__(self, centroid_crop, instance_peaks: TopDownMultiClassFindPeaks):
         self.centroid_crop = centroid_crop
         self.instance_peaks = instance_peaks
+        self.fused = True
+
+    def _can_fuse(self):
+        cc, fp = self.centroid_crop, self.instance_peaks
+        return (self.fused and type(cc) is CentroidCrop and type(fp) is TopDownMultiClassFindPeaks and cc.precrop_resize == 1.0 and
+                cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and fp.optimal_grouping and fp.input_scale == 1.0
+                and fp.keras_model.input_scale == 1.0 and cc.keras_model.handle is fp.keras_model.handle)
+
+    def _call_fused(self, imgs):
+        """sb_infer_topdown_multiclass: frames up once, one record per frame back (include/sleap_b200.h)."""
+        cc, fp = self.centroid_crop, self.instance_peaks
+        imgs = cc._prep(imgs)
+        B, H, W, C = imgs.shape
+        mc, mi = cc.keras_model, fp.keras_model
+        td, K = _topdown_params(cc, fp)
+        p = topdown_multiclass_params(td, mi.cm.vector_taps[fp.CLASS_VECTORS], fp.class_head, fp.dense)
+        _configure_topdown(cc, fp, "sb_topdown_multiclass_configure", p, (B, H, W, C), fp.dense)
+        NC, N = p.n_classes, head_channels(mi, fp.HEAD)
+        ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
+        pts = np.zeros((B, NC, N, 2), np.float32); vals = np.zeros((B, NC, N), np.float32); probs = np.zeros((B, NC), np.float32)
+        nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
+        cvec = np.zeros((B, K, NC), np.float32) if fp.return_class_vectors else None
+        mc.handle.call("sb_infer_topdown_multiclass", mc.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(ce), ptr(cv), ptr(pts),
+                       ptr(vals), ptr(probs), ptr(nv), ptr(fl), ptr(cvec))
+        n = int(nv.max()) if B else 0
+        out = {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "centroids": ce[:, :n].copy(),
+               "centroid_vals": cv[:, :n].copy(), "flags": fl}
+        if cvec is not None:
+            out["class_vectors"] = np.concatenate([cvec[b, :nv[b]] for b in range(B)])
+        return out
 
     def call(self, example):
         if isinstance(example, np.ndarray):
             example = dict(image=example)
+        if self._can_fuse():
+            return self._call_fused(_images_of(example))
         crop_out = self.centroid_crop.call(example)
         out = self.instance_peaks.call(crop_out)
         res = {k: out[k] for k in ("instance_peaks", "instance_peak_vals", "instance_scores")}

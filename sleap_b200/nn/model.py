@@ -27,7 +27,8 @@ class DeviceModel:
         self.input_scale = float(input_scale)
         self.cm = arch.compile_model(spec, input_channels, input_scale, pad_to_stride, split=(precision == PRECISION_SPLIT))
         blob = self.cm.pack_weights(weights)
-        # dense layers of "vector" heads stay on the host (heads.py:431-460)
+        # dense layers of "vector" heads (heads.py:431-460): run on the host by forward(), packed for the device by the
+        # top-down multi-class step (pack_dense_weights)
         self.dense_weights = {k: {kk: np.asarray(vv, np.float32) for kk, vv in v.items()} for k, v in weights.items()
                               if k.startswith("pre_classification") or k in self.cm.vector_taps}
         ops = self.cm.ops_array()
@@ -108,6 +109,20 @@ class DeviceModel:
             feat = buf[..., c0:c0 + Cl]
         head = next(h for h in self.spec["heads"] if h["name"] == name)
         return class_vectors_from_features(feat, head, self.dense_weights)
+
+
+def head_spec(spec, name):
+    """The entry of head ``name`` in a model spec."""
+    return next(h for h in spec["heads"] if h["name"] == name)
+
+
+def pack_dense_weights(head, weights):
+    """The dense layers of "vector" head ``head`` in the layout the device's class-vector head reads (include/sleap_b200.h,
+    sb_topdown_multiclass_params.dense_weights): float32, Keras layout, ``pre_classification{i}_fc`` kernel (n_in, units)
+    then bias for each fc layer, then the head's own kernel and bias."""
+    names = [f"pre_classification{i}_fc" for i in range(int(head.get("num_fc_layers", 1)))] + [head["name"]]
+    return np.ascontiguousarray(np.concatenate([np.asarray(weights[n][k], np.float32).reshape(-1) for n in names
+                                                for k in ("kernel", "bias")]))
 
 
 def chain_key(params, *arrays):

@@ -2,7 +2,7 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [--steps K] [--c5-batch B]
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [--steps K] [--c5-batch B]
   (C5 default: 16 frames per GPU and step)
 
 r50: ResNet50 bottom-up (ImageNet-preprocessed "frozen" weights, upsampling stack to stride 4 with k4 transposed convs,
@@ -26,6 +26,14 @@ the trained fixture model (min_tracks_2node, 1024x1024 at input scale 0.5, 2 nod
 C4-sized UNet with 13 nodes and 4 classes at stride 4 (synthetic weights, confidence head calibrated to ~5 detections
 per node as bench.py does), 1024x1024, B=8.  The line reports frames/s per arm and whether the arms agree (assignments
 identical, points, values and class probabilities bit for bit).
+
+topdown_multiclass: the top-down multi-class (identity) predictor, two arms alternating on the same frames in one process:
+the staged path (TopDownMultiClassInferenceModel with fused = False: centroid stage, crops to the host, instance network
+with the class-vector head's dense layers and the grouping on the host) and the fused step (sb_infer_topdown_multiclass),
+both through predict_on_batch.  Workload: the C3 pair (centroid UNet at input scale 0.5, centered-instance UNet on 160x160
+crops, max 5 animals, B=16) with a ClassVectorsHead of 4 classes and 3 x 64 fc units on the stride-16 features.  The line
+reports frames/s per arm and whether they agree (centroids and points bit for bit, identical assignments, the largest
+class-probability difference).
 """
 import json
 import os
@@ -297,9 +305,9 @@ def _mc_host_arm(layer, batch):
     return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": cp}
 
 
-def _mc_agree(a, b):
+def _mc_agree(a, b, keys=("instance_peaks", "instance_peak_vals", "instance_scores")):
     """Assignments identical (NaN pattern) and every value bit for bit."""
-    for k in ("instance_peaks", "instance_peak_vals", "instance_scores"):
+    for k in keys:
         x, y = np.asarray(a[k], np.float32), np.asarray(b[k], np.float32)
         if x.shape != y.shape or not np.array_equal(np.isnan(x), np.isnan(y)):
             return False
@@ -380,6 +388,64 @@ def multiclass_bench(steps):
     return out
 
 
+def topdown_multiclass_bench(steps):
+    """The C3 pair of topdown() with the instance model given a ClassVectorsHead (4 classes, 3 x 64 fc units, global max
+    pool of the stride-16 features): the staged TopDownMultiClassInferenceModel (fused = False) and the fused step, both
+    through predict_on_batch, alternating on the same frames."""
+    from sleap_b200.nn.inference import TopDownMultiClassPredictor
+    classes = ["c0", "c1", "c2", "c3"]
+    cspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="centroid", part_names=None, edges=None,
+                 heads=[dict(name="CentroidConfmapsHead", channels=1, output_stride=2)])
+    ispec = dict(backbone="unet", backbone_cfg=dict(unet(24, 16, 4), up_interpolate=False), head_type="multi_class_topdown",
+                 part_names=FLIES13, edges=None, classes=classes,
+                 heads=[dict(name="CenteredInstanceConfmapsHead", channels=13, output_stride=4),
+                        dict(name="ClassVectorsHead", channels=len(classes), output_stride=16, vector=True, num_fc_layers=3,
+                             num_fc_units=64, global_pool=True)])
+    B = 16
+    fr = frames(B, 1024, 1024, 1, 3)
+    icm = A.compile_model(ispec, 1)
+    iw = A.make_synthetic_weights(icm, 1004)
+    rng = np.random.default_rng(1005)
+    dims = [icm.vector_taps["ClassVectorsHead"]["C"], 64, 64, 64, len(classes)]
+    for i in range(4):                                                    # He-normal dense layers, small biases
+        iw["ClassVectorsHead" if i == 3 else f"pre_classification{i}_fc"] = dict(
+            kernel=(rng.normal(0, 1, dims[i:i + 2]) * np.sqrt(2.0 / dims[i])).astype(np.float32),
+            bias=rng.normal(0, 0.1, dims[i + 1]).astype(np.float32))
+
+    def arm(fused):
+        # each arm owns its two device models: a staged call reconfigures the chains the fused pipeline needs
+        cm_model, _, _ = model_for(cspec, 1, 1003, input_scale=0.5)
+        cms = cm_model.forward(fr[:2])[0]                                # ~5 animals per frame, as topdown() calibrates
+        thr = float(np.sort(cms.reshape(-1))[-(5 * 2 * 6)])
+        pred = TopDownMultiClassPredictor(cm_model, DeviceModel(ispec, iw, input_channels=1, precision=0), crop_size=160,
+                                          peak_threshold=thr, integral_refinement=True, batch_size=B, max_instances=5)
+        pred.inference_model.instance_peaks.peak_threshold = 0.0
+        pred.inference_model.fused = fused
+        return lambda: pred.inference_model.predict_on_batch(fr)
+
+    arms = {"staged predict_on_batch (fused = False)": arm(False), "fused predict_on_batch": arm(True)}
+    outs = {k: f() for k, f in arms.items()}                             # warm-up, and the outputs compared
+    reps = max(3, steps)
+    times = {k: [] for k in arms}
+    for _ in range(reps):                                                # arms alternate
+        for k, f in arms.items():
+            t0 = time.perf_counter()
+            f()
+            times[k].append(time.perf_counter() - t0)
+    a, b = (outs[k] for k in arms)
+    same_assignments = np.array_equal(np.isnan(a["instance_scores"]), np.isnan(b["instance_scores"]))
+    return {"config": "topdown_multiclass: C3 top-down pair, instance model with a ClassVectorsHead (4 classes, 3 x 64 fc units, "
+                      "stride-16 tap), 1024x1024, max 5 animals, B=16", "gpu": gpu_identity(),
+            "metric": "frames/s (median of alternating repetitions; host frames in, results on the host)", "repetitions": reps,
+            "frames_per_s": {k: B / float(np.median(v)) for k, v in times.items()},
+            "frames_per_s_spread": {k: [B / max(v), B / min(v)] for k, v in times.items()},
+            "mean_crops_per_frame": float(np.isfinite(b["centroid_vals"]).sum() / B),
+            "agree_centroids_bitwise": _mc_agree(a, b, ("centroids", "centroid_vals")), "agree_assignments": bool(same_assignments),
+            "agree_points_bitwise": _mc_agree(a, b, ("instance_peaks", "instance_peak_vals")),
+            "class_probability_max_abs_diff": float(np.nanmax(np.abs(a["instance_scores"] - b["instance_scores"])))
+            if np.isfinite(a["instance_scores"]).any() else 0.0}
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -396,6 +462,8 @@ if __name__ == "__main__":
             r = track_bench()
         elif c == "multiclass":
             r = multiclass_bench(steps)
+        elif c == "topdown_multiclass":
+            r = topdown_multiclass_bench(steps)
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
