@@ -476,6 +476,7 @@ int sb_flow_destroy(sb_handle_t h, int flow_id);
 #define SB_TRACK_OKS_REF 1
 #define SB_TRACK_OKS_UNION 2
 #define SB_TRACK_INFEASIBLE 1
+#define SB_TRACK_OVER_CAPACITY 3
 typedef struct sb_tracker_params {
   int32_t maker, similarity, match;         /* SB_TRACK_* */
   int32_t track_window;
@@ -504,13 +505,26 @@ int sb_track_instances(sb_handle_t h, int tracker_id, int B, int I, const double
  * t = the host's _next_t.  The tracker must live on the model's handle, have its n_nodes and at least its
  * max_instances, and the record exchange must not be connected (one rank).  The per-frame track records
  * ([B][2 + 3 I] doubles, I = the tracker's max_instances: n, flag, order[I] (index into that instance list), track
- * id[I], tracking score[I]; flag != 0: the frame was not tracked -- SB_TRACK_INFEASIBLE, or 2 = queue table full)
+ * id[I], tracking score[I]; flag != 0: the frame was not tracked -- SB_TRACK_INFEASIBLE, 2 = queue table full, or
+ * SB_TRACK_OVER_CAPACITY, which only the top-down step can meet)
  * are a separate buffer: the result records and record_width do not change.  They come back with the result copy:
  * sb_bottomup_tracks(slot 0 / 1 after sb_bottomup_collect, -1 after sb_infer_bottomup); sb_bottomup_device_tracks
  * copies the last step's records after sb_infer_bottomup_dev. */
 int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int max_instances, double img_h, double img_w);
 int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks);
 int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tracks);
+/* The tracker inside the top-down step.  sb_topdown_attach_tracker(tracker_id = -1 detaches): every later
+ * sb_infer_topdown call runs k_track on the handle's stream after the record kernel, on the instance list
+ * Predictor._frames_from_example builds from each frame of a top-down batch: the frame's crops in order, rows whose
+ * points are all NaN skipped, score = the centroid value, no max_instances cut; with the frame size img_h x img_w
+ * (normalized_instance) and t = the host's _next_t.  A frame whose list is longer than the tracker's max_instances
+ * stops the batch's tracking there: its record and every later one carry flag SB_TRACK_OVER_CAPACITY, which stays set
+ * until sb_tracker_reset (as a full queue table does).  The pipeline must be a plain one (sb_topdown_configure), and the
+ * tracker must live on its handle and have its instance model's node count; img_h, img_w > 0.  The attachment lives
+ * with the pipeline: a configure call on either model drops it.  sb_topdown_tracks copies the track records of the last
+ * sb_infer_topdown (the bottom-up format above); sb_infer_topdown's outputs do not change. */
+int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w);
+int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_tracks);
 
 #ifdef __cplusplus
 }

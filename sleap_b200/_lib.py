@@ -179,6 +179,8 @@ _SIGS = {
     "sb_bottomup_attach_tracker": [c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double],
     "sb_bottomup_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
     "sb_bottomup_device_tracks": [c_void_p, c_int, c_int, c_void_p],
+    "sb_topdown_attach_tracker": [c_void_p, c_int, c_int, ctypes.c_double, ctypes.c_double],
+    "sb_topdown_tracks": [c_void_p, c_int, c_int, c_void_p],
     "sb_tracker_destroy": [c_void_p, c_int],
     "sb_track_instances": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), POINTER(c_int32)],

@@ -115,7 +115,7 @@ int sb_fail(sb_handle_s* h, int code, const char* fmt, ...);
 void sb_models_free(sb_handle_s* h);
 void sb_flows_free(sb_handle_s* h);
 void sb_trackers_free(sb_handle_s* h);
-// ---- device tracker (sb_track.cu) inside the bottom-up step ----
+// ---- device tracker (sb_track.cu) inside the bottom-up and top-down steps ----
 SbTracker* sb_tracker_get(sb_handle_s* h, int id);
 int sb_tracker_max_instances(const SbTracker* t);
 int sb_tracker_nodes(const SbTracker* t);
@@ -124,6 +124,10 @@ static __host__ __device__ inline size_t sb_track_record_width(int I) { return 2
 int sbk_track_step(sb_handle_s* h, SbTracker* tr, int B, const float* inst_peaks, const float* inst_vals,
                    const float* inst_scores, const int* n_inst, int I_src, int max_instances, double img_h, double img_w,
                    double* out_records);
+// k_track on the crops of a top-down batch (points / values per crop, centroid values [B][K], crops per frame and
+// their frame offsets), then one track record per frame into out_records
+int sbk_track_topdown(sb_handle_s* h, SbTracker* tr, int B, const float* ipts, const float* ivals, const float* sel_val,
+                      const int* sel_count, const int* offsets, int K, double img_h, double img_w, double* out_records);
 
 #define SB_CUDA(h, expr)                                                              \
   do {                                                                                \

@@ -109,6 +109,19 @@ static int chain_drop(sb_handle_s* h, SbModel* m) {
   return 0;
 }
 
+int sb_track_records_alloc(sb_handle_s* h, SbModel* m, int B, int I) {
+  if (m->trk_B >= B && m->trk_I == I) return SB_OK;
+  cudaFree(m->trk_dev); m->trk_dev = nullptr;
+  for (int i = 0; i < 3; ++i) { cudaFreeHost(m->trk_host[i]); m->trk_host[i] = nullptr; }
+  m->trk_B = 0;
+  const size_t n = (size_t)B * sb_track_record_width(I);
+  int rc;
+  if ((rc = sb_dev_alloc(h, &m->trk_dev, n))) return rc;
+  for (int i = 0; i < 3; ++i) SB_CUDA(h, cudaHostAlloc((void**)&m->trk_host[i], n * sizeof(double), cudaHostAllocDefault));
+  m->trk_B = B; m->trk_I = I;
+  return SB_OK;
+}
+
 // The model a per-model configure call sets up: a valid id, non-null params and a configured network
 static SbModel* configure_target(sb_handle_s* h, int id, const void* p) {
   SbModel* m = chain_model(h, id, SB_CHAIN_ANY, "bad model id / params");
@@ -1000,17 +1013,7 @@ int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int 
     return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_attach_tracker: tracker of %d nodes / %d instances, predictor of %d / %d",
                    sb_tracker_nodes(t), sb_tracker_max_instances(t), m->bu.n_nodes, m->bu.max_instances);
   if (!(img_h > 0) || !(img_w > 0)) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_attach_tracker: image %g x %g", img_h, img_w);
-  const int I = sb_tracker_max_instances(t);
-  if (m->trk_B < m->B || m->trk_I != I) {
-    cudaFree(m->trk_dev); m->trk_dev = nullptr;
-    for (int i = 0; i < 3; ++i) { cudaFreeHost(m->trk_host[i]); m->trk_host[i] = nullptr; }
-    m->trk_B = 0;
-    const size_t n = (size_t)m->B * sb_track_record_width(I);
-    int rc;
-    if ((rc = sb_dev_alloc(h, &m->trk_dev, n))) return rc;
-    for (int i = 0; i < 3; ++i) SB_CUDA(h, cudaHostAlloc((void**)&m->trk_host[i], n * sizeof(double), cudaHostAllocDefault));
-    m->trk_B = m->B; m->trk_I = I;
-  }
+  if (const int rc = sb_track_records_alloc(h, m, m->B, sb_tracker_max_instances(t))) return rc;
   m->trk = t; m->trk_cut = max_instances < 0 ? -1 : max_instances; m->trk_h = img_h; m->trk_w = img_w;
   return SB_OK;
 }

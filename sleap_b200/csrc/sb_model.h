@@ -150,7 +150,8 @@ struct SbModel {
   SbTopdown* td = nullptr;                 // fused top-down pipeline (sb_topdown_configure), held by its centroid model
   SbEntryPlan entry;                       // input stage (sb_entry.cu)
   SbGather gather;                         // peer-memory exchange of the result records (sb_gather.cu)
-  // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu); its per-frame track records
+  // device tracker run after the grouping kernel (sb_bottomup_attach_tracker, sb_track.cu) or, on a top-down pipeline's
+  // centroid model, after its record kernel (sb_topdown_attach_tracker); its per-frame track records
   // ([B][sb_track_record_width] doubles) live beside the result records and travel with the result copy
   SbTracker* trk = nullptr;
   int trk_B = 0, trk_I = 0, trk_cut = -1;
@@ -170,6 +171,9 @@ int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_ar
 SbModel* chain_model(sb_handle_s* h, int id, int kind, const char* what);
 
 void sb_topdown_free(SbModel* m);        // sb_topdown.cu
+
+// Sizes the model's track records (trk_dev, trk_host) for B frames of a tracker of I instances; keeps larger ones
+int sb_track_records_alloc(sb_handle_s* h, SbModel* m, int B, int I);
 
 // record exchange (sb_gather.cu)
 SbGatherDev sb_gather_dev(const SbModel* m, unsigned long long step);

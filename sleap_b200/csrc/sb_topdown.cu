@@ -346,6 +346,7 @@ void sb_topdown_free(SbModel* m) {
   if (t->total_host) cudaFreeHost(t->total_host);
   delete t;
   m->td = nullptr;
+  m->trk = nullptr;                              // an attached tracker lives with the pipeline
 }
 
 namespace {
@@ -499,6 +500,13 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
     k_td_pack<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags,
                                         t->record, t->width);
     SB_CHECK_LAUNCH(h);
+    if (!mc->trk) return 0;
+    // the attached tracker on the frames' instance lists; its records come back before the step's final sync
+    if (const int rc = sbk_track_topdown(h, mc->trk, B, t->ipts, t->ivals, t->sel_val, t->sel_count, t->offsets, t->K, mc->trk_h,
+                                         mc->trk_w, mc->trk_dev))
+      return rc;
+    SB_CUDA(h, cudaMemcpyAsync(mc->trk_host[2], mc->trk_dev, (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double),
+                               cudaMemcpyDeviceToHost, h->stream));
     return 0;
   };
   const int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, false, [](int, int) { return 0; }, pack);
@@ -507,6 +515,33 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
   sb_split_records(t->record_host, B, t->width,
                    {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
                    {out_n_valid, out_flags});
+  return SB_OK;
+}
+
+int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+  if (!t) return SB_ERR_INVALID;
+  SbModel* mc = h->models[centroid_model_id];
+  if (tracker_id < 0) { mc->trk = nullptr; return SB_OK; }
+  SbTracker* tr = sb_tracker_get(h, tracker_id);
+  if (!tr) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_attach_tracker: no tracker %d on this handle", tracker_id);
+  if (sb_tracker_nodes(tr) != t->nodes)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_attach_tracker: tracker of %d nodes, instance model of %d", sb_tracker_nodes(tr),
+                   t->nodes);
+  if (!(img_h > 0) || !(img_w > 0)) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_attach_tracker: image %g x %g", img_h, img_w);
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if (const int rc = sb_track_records_alloc(h, mc, t->Bmax, sb_tracker_max_instances(tr))) return rc;
+  mc->trk = tr; mc->trk_h = img_h; mc->trk_w = img_w;
+  return SB_OK;
+}
+
+int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_tracks) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+  if (!t) return SB_ERR_INVALID;
+  const SbModel* mc = h->models[centroid_model_id];
+  if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
+  if (B <= 0 || B > t->Bmax || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad batch");
+  memcpy(out_tracks, mc->trk_host[2], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
   return SB_OK;
 }
 

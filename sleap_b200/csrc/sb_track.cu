@@ -46,7 +46,8 @@ struct TrackCfg {
 struct TrackState {
   long long next_t;
   int n_spawned, head, len, n_table;            // head / len: the simple maker's ring of frames
-  int status, n_done;                           // status: 0, SB_TRACK_INFEASIBLE, or 2 = queue table full
+  int status, n_done;                           // status: 0, SB_TRACK_INFEASIBLE, 2 = queue table full, or
+                                                // SB_TRACK_OVER_CAPACITY
 };
 
 struct TrackBufs {
@@ -274,6 +275,10 @@ __global__ void __launch_bounds__(kTrackThreads) k_track(TrackCfg c, TrackBufs b
   if (st->status) return;                        // a full queue table stays an error until sb_tracker_reset
   for (int b = 0; b < B; ++b) {
     const int n = bf.count[b];
+    if (n > I) {                                 // a list longer than the capacity: frames b.. stay untracked
+      if (tid == 0) { st->status = SB_TRACK_OVER_CAPACITY; st->n_done = b; }
+      return;
+    }
     const double* P = bf.pts + (size_t)b * I * C * 2;
     const double* PC = bf.conf + (size_t)b * I * C;
     const double* SC = bf.score + (size_t)b * I;
@@ -539,8 +544,46 @@ __global__ void k_track_prep(const float* __restrict__ ip, const float* __restri
   for (int i = threadIdx.x; i < k; i += blockDim.x) score[(size_t)b * I + i] = (double)S[s_keep[i]];
 }
 
+// The instance list the predictors build from one frame of a top-down batch: the frame's crops offsets[b] + j,
+// j < sel_count[b], in crop order, rows with every point NaN skipped; score = the centroid value sel_val[b * K + j].  No
+// max_instances cut (top-down caps centroids only).  count[b] is the full length of the list, which may exceed I: only
+// the first I rows are written, and k_track stops at such a frame.  One CTA per frame.
+__global__ void k_track_prep_td(const float* __restrict__ ipts, const float* __restrict__ ivals, const float* __restrict__ sel_val,
+                                const int* __restrict__ sel_count, const int* __restrict__ offsets, int K, int C, double img_h,
+                                double img_w, int I, double* pts, double* conf, double* score, int* count, double* hw,
+                                long long* t) {
+  __shared__ int s_keep[kTrackMaxInstances];
+  __shared__ int s_n;
+  const int b = blockIdx.x;
+  const int o = offsets[b];
+  if (threadIdx.x == 0) {
+    const int n = sel_count[b];
+    int k = 0;
+    for (int j = 0; j < n; ++j) {
+      const float* p = ipts + (size_t)(o + j) * C * 2;
+      bool all_nan = true;
+      for (int q = 0; q < 2 * C && all_nan; ++q) all_nan = p[q] != p[q];
+      if (all_nan) continue;
+      if (k < I) s_keep[k] = j;                  // I <= kTrackMaxInstances
+      ++k;
+    }
+    s_n = min(k, I);
+    count[b] = k; hw[2 * b] = img_h; hw[2 * b + 1] = img_w; t[b] = -1;
+  }
+  __syncthreads();
+  const int k = s_n;
+  for (int e = threadIdx.x; e < k * C; e += blockDim.x) {
+    const int i = e / C, q = e - i * C;
+    const size_t src = (size_t)(o + s_keep[i]) * C + q;
+    pts[((size_t)b * I + i) * C * 2 + 2 * q] = (double)ipts[src * 2];
+    pts[((size_t)b * I + i) * C * 2 + 2 * q + 1] = (double)ipts[src * 2 + 1];
+    conf[((size_t)b * I + i) * C + q] = (double)ivals[src];
+  }
+  for (int i = threadIdx.x; i < k; i += blockDim.x) score[(size_t)b * I + i] = (double)sel_val[(size_t)b * K + s_keep[i]];
+}
+
 // Per-frame track record: [n, flag, order[I], track id[I], tracking score[I]] (doubles; flag 0 = tracked, else the
-// tracker's status: SB_TRACK_INFEASIBLE, 2 = queue table full).  One CTA per frame.
+// tracker's status: SB_TRACK_INFEASIBLE, 2 = queue table full, SB_TRACK_OVER_CAPACITY).  One CTA per frame.
 __global__ void k_track_pack(const TrackState* st, const int* on, const int* oidx, const int* otid,
                              const double* oscore, int I, double* rec) {
   const int b = blockIdx.x;
@@ -643,6 +686,16 @@ int tracker_clear(sb_handle_s* h, SbTracker* t) {
   return SB_OK;
 }
 
+// k_track on the B instance lists a step's prep wrote into io, then one track record per frame into out_records
+int track_and_pack(sb_handle_s* h, SbTracker* tr, int B, const TrackIo& io, double* out_records) {
+  const TrackCfg& c = tr->cfg;
+  k_track<<<1, kTrackThreads, 0, h->stream>>>(c, call_bufs(tr, io, true), B);
+  SB_CHECK_LAUNCH(h);
+  k_track_pack<<<B, 128, 0, h->stream>>>(tr->bf.st, io.on, io.oidx, io.otid, io.oscore, c.I, out_records);
+  SB_CHECK_LAUNCH(h);
+  return SB_OK;
+}
+
 }  // namespace
 
 int sbk_track_step(sb_handle_s* h, SbTracker* tr, int B, const float* inst_peaks, const float* inst_vals,
@@ -655,11 +708,19 @@ int sbk_track_step(sb_handle_s* h, SbTracker* tr, int B, const float* inst_peaks
   k_track_prep<<<B, 128, 0, h->stream>>>(inst_peaks, inst_vals, inst_scores, n_inst, I_src, c.C, max_instances, img_h,
                                          img_w, c.I, io.pts, io.conf, io.score, io.count, io.hw, io.t);
   SB_CHECK_LAUNCH(h);
-  k_track<<<1, kTrackThreads, 0, h->stream>>>(c, call_bufs(tr, io, true), B);
+  return track_and_pack(h, tr, B, io, out_records);
+}
+
+int sbk_track_topdown(sb_handle_s* h, SbTracker* tr, int B, const float* ipts, const float* ivals, const float* sel_val,
+                      const int* sel_count, const int* offsets, int K, double img_h, double img_w, double* out_records) {
+  TrackIo io;
+  int rc;
+  if ((rc = tracker_io(h, tr, B, io))) return rc;
+  const TrackCfg& c = tr->cfg;
+  k_track_prep_td<<<B, 128, 0, h->stream>>>(ipts, ivals, sel_val, sel_count, offsets, K, c.C, img_h, img_w, c.I, io.pts, io.conf,
+                                            io.score, io.count, io.hw, io.t);
   SB_CHECK_LAUNCH(h);
-  k_track_pack<<<B, 128, 0, h->stream>>>(tr->bf.st, io.on, io.oidx, io.otid, io.oscore, c.I, out_records);
-  SB_CHECK_LAUNCH(h);
-  return SB_OK;
+  return track_and_pack(h, tr, B, io, out_records);
 }
 
 extern "C" {

@@ -127,6 +127,16 @@ class InferenceLayer:
         m.configure_chain(self.CHAIN, self.params(), *self._keep)
 
 
+def _track_fields(rec):
+    """Per-frame track records ([B][2 + 3 I] doubles: n, flag, order[I], track id[I], tracking score[I]) as batch-dict
+    fields: track_order / track_ids / tracking_scores (B, I) (order = index into the frame's instance list, -1 padded),
+    track_n and track_flags (B)."""
+    I = (rec.shape[1] - 2) // 3
+    return {"track_n": rec[:, 0].astype(np.int64), "track_flags": rec[:, 1].astype(np.int64),
+            "track_order": rec[:, 2:2 + I].astype(np.int64), "track_ids": rec[:, 2 + I:2 + 2 * I].astype(np.int64),
+            "tracking_scores": rec[:, 2 + 2 * I:].copy()}
+
+
 def _find_head(model: DeviceModel, name: str):
     if name not in model.cm.head_buffers:
         return None
@@ -434,6 +444,13 @@ class TopDownInferenceModel(InferenceModel):
         self.centroid_crop = centroid_crop
         self.instance_peaks = instance_peaks
         self.fused = True            # one device pipeline (sb_infer_topdown) when both stages are device models
+        # a Tracker with track_device, run by k_track inside each fused step (TopDownPredictor.predict sets it for its span)
+        self.tracker = None
+
+    def detach_tracker(self):
+        mc = self.centroid_crop.keras_model
+        if getattr(self.tracker, "_device", None) is not None and mc.chain and mc.chain[0] == "sb_topdown_configure":
+            mc.handle.call("sb_topdown_attach_tracker", mc.model_id, -1, 1.0, 1.0)
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
@@ -451,14 +468,22 @@ class TopDownInferenceModel(InferenceModel):
         p, K = _topdown_params(cc, fp)
         _configure_topdown(cc, fp, "sb_topdown_configure", p, (B, H, W, C))
         n_nodes = head_channels(mi, fp.HEAD)
+        if self.tracker is not None:     # the raw frame size, as the predictor's image_hw; default capacity, not K
+            dev = self.tracker._device_tracker(n_nodes, handle=mc.handle)
+            mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
         mc.handle.call("sb_infer_topdown", mc.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(ce), ptr(cv), ptr(ip), ptr(iv),
                        ptr(nv), ptr(fl))
         n = int(nv.max()) if B else 0
-        return {"centroids": ce[:, :n].copy(), "centroid_vals": cv[:, :n].copy(), "instance_peaks": ip[:, :n].copy(),
-                "instance_peak_vals": iv[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
+        out = {"centroids": ce[:, :n].copy(), "centroid_vals": cv[:, :n].copy(), "instance_peaks": ip[:, :n].copy(),
+               "instance_peak_vals": iv[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
+        if self.tracker is not None:
+            rec = np.zeros((B, 2 + 3 * self.tracker._device.max_instances), np.float64)
+            mc.handle.call("sb_topdown_tracks", mc.model_id, B, ptr(rec))
+            out.update(_track_fields(rec))
+        return out
 
     def call(self, example):
         if isinstance(example, np.ndarray):
@@ -536,18 +561,14 @@ class BottomUpInferenceLayer(InferenceLayer):
             m.handle.call("sb_bottomup_attach_tracker", m.model_id, -1, -1, 1.0, 1.0)
 
     def track_fields(self, slot, B):
-        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields:
-        track_order / track_ids / tracking_scores (B, I) (order = index into the frame's instance list, -1 padded),
-        track_n and track_flags (B)."""
+        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields
+        (``_track_fields``)."""
         if self.tracker is None:
             return {}
-        I = self.tracker._device.max_instances
-        rec = np.zeros((B, 2 + 3 * I), np.float64)
+        rec = np.zeros((B, 2 + 3 * self.tracker._device.max_instances), np.float64)
         m = self.keras_model
         m.handle.call("sb_bottomup_tracks", m.model_id, slot, B, ptr(rec))
-        return {"track_n": rec[:, 0].astype(np.int64), "track_flags": rec[:, 1].astype(np.int64),
-                "track_order": rec[:, 2:2 + I].astype(np.int64), "track_ids": rec[:, 2 + I:2 + 2 * I].astype(np.int64),
-                "tracking_scores": rec[:, 2 + 2 * I:].copy()}
+        return _track_fields(rec)
 
     def params(self) -> BottomUpParams:
         """The chain's parameters; their edge arrays stay alive in ``self._keep``."""
@@ -1358,12 +1379,29 @@ class Predictor:
             self.tracker.final_pass(frames)
         return frames
 
+    def _step_tracker(self, model, make_labels):
+        """The tracker to run inside the device step of ``model`` (a Tracker with ``track_device``), or None when the
+        step runs without one.  The tracker's GPU must be the model's, and the run must be on one rank."""
+        tr = self.tracker
+        if tr is None or getattr(tr, "track_device", None) is None or tr.candidate_maker is None:
+            return None
+        if int(str(tr.track_device).split(":")[-1]) != model.handle.device_id:
+            raise ValueError(f"the tracker's track_device {tr.track_device!r} is not the model's GPU ({model.handle.device_id})")
+        if getattr(model, "peer_gather", None) is not None or int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            raise ValueError("a device tracker tracks one rank's frames: run the multi-rank prediction without track_device")
+        if not make_labels:                          # no labeled frames, nothing to track (as with the host tracker)
+            return None
+        return tr
+
     def _apply_device_tracks(self, ex, new):
-        """The frames' tracked lists from the track records of their step (BottomUpPredictor with a device tracker)."""
+        """The frames' tracked lists from the track records of their step (a predictor with a device tracker)."""
         for k, lf in enumerate(new):
             flag = int(ex["track_flags"][k])
             if flag == 1:
                 raise ValueError("cost matrix is infeasible")
+            if flag == 3:                                # SB_TRACK_OVER_CAPACITY
+                raise _lib.SleapB200Error(f"frame {lf.frame_idx} has {len(lf.instances)} instances, more than the device tracker's "
+                                          f"capacity of {self.tracker._device.max_instances} (Tracker.device_max_instances)")
             if flag:
                 raise _lib.SleapB200Error(f"the device tracker's track queue table is full (frame {lf.frame_idx})")
             n = int(ex["track_n"][k])
@@ -1481,6 +1519,25 @@ class TopDownPredictor(Predictor):
     def uses_ground_truth(self):
         return self.centroid_model is None or self.confmap_model is None
 
+    def predict(self, data, make_labels: bool = True):
+        """As Predictor.predict.  On the fused step (frames in, not ``Labels``), a tracker with ``track_device`` runs
+        inside each step (k_track after the record kernel, on the model's GPU); the consumer thread only maps its track
+        ids to ``Track`` objects before ``final_pass``.  The tracker's GPU must be the model's, and the run must be on
+        one rank.  Other inputs track on the consumer thread."""
+        from sleap_b200.io.labels import Labels, LabelsReader
+        im = self.inference_model
+        if not im._can_fuse() or isinstance(data, (Labels, LabelsReader)):
+            return super().predict(data, make_labels)
+        tr = self._step_tracker(im.centroid_crop.keras_model, make_labels)
+        if tr is None:
+            return super().predict(data, make_labels)
+        im.tracker = tr
+        try:
+            return super().predict(data, make_labels)
+        finally:
+            im.detach_tracker()
+            im.tracker = None
+
     @classmethod
     def from_trained_models(cls, centroid_model_path=None, confmap_model_path=None, batch_size=4, peak_threshold=0.2,
                             integral_refinement=True, integral_patch_size=5, resize_input_layer=True,
@@ -1529,16 +1586,9 @@ class BottomUpPredictor(Predictor):
         """As Predictor.predict.  A tracker with ``track_device`` runs inside each bottom-up step (k_track after the
         grouping kernel, on the model's GPU); the consumer thread only maps its track ids to ``Track`` objects before
         ``final_pass``.  The tracker's GPU must be the model's, and the run must be on one rank."""
-        tr = self.tracker
-        if tr is None or getattr(tr, "track_device", None) is None or tr.candidate_maker is None:
-            return super().predict(data, make_labels)
         layer = self.inference_model.bottomup_layer
-        m = layer.keras_model
-        if int(str(tr.track_device).split(":")[-1]) != m.handle.device_id:
-            raise ValueError(f"the tracker's track_device {tr.track_device!r} is not the model's GPU ({m.handle.device_id})")
-        if getattr(m, "peer_gather", None) is not None or int(os.environ.get("WORLD_SIZE", "1")) > 1:
-            raise ValueError("a device tracker tracks one rank's frames: run the multi-rank prediction without track_device")
-        if not make_labels:                          # no labeled frames, nothing to track (as with the host tracker)
+        tr = self._step_tracker(layer.keras_model, make_labels)
+        if tr is None:
             return super().predict(data, make_labels)
         layer.tracker, layer.tracker_cut = tr, -1 if self.max_instances is None else int(self.max_instances)
         try:

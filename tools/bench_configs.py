@@ -2,7 +2,8 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [--steps K] [--c5-batch B]
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_track] [--steps K]
+                               [--c5-batch B]
   (C5 default: 16 frames per GPU and step)
 
 r50: ResNet50 bottom-up (ImageNet-preprocessed "frozen" weights, upsampling stack to stride 4 with k4 transposed convs,
@@ -34,6 +35,13 @@ both through predict_on_batch.  Workload: the C3 pair (centroid UNet at input sc
 crops, max 5 animals, B=16) with a ClassVectorsHead of 4 classes and 3 x 64 fc units on the stride-16 features.  The line
 reports frames/s per arm and whether they agree (centroids and points bit for bit, identical assignments, the largest
 class-probability difference).
+
+topdown_track: the top-down predictor with a tracker, four arms alternating in one process: TopDownPredictor.predict
+(labels made) of the C3 pair on 256 gray tracking-clip frames, B=16, the centroid threshold calibrated on clip frames to
+about 5 animals per frame; no tracker, the host simple tracker, the device simple tracker inside the fused step
+(sb_topdown_attach_tracker) and the device simple tracker on the per-frame route (fused = False).  The line reports
+frames/s and instances per frame per arm, and whether the device tracks equal the host's, with numpy's greedy ties and
+with the device's stable ones.
 """
 import json
 import os
@@ -446,6 +454,70 @@ def topdown_multiclass_bench(steps):
             if np.isfinite(a["instance_scores"]).any() else 0.0}
 
 
+def topdown_track_bench(steps):
+    """TopDownPredictor.predict (labels made) of the C3 pair of topdown() on 256 tracking-clip frames (gray), B = 16, the
+    centroid threshold calibrated on clip frames to about 5 animals per frame.  Four arms alternate in one process: no
+    tracker, the host simple tracker, the device simple tracker inside the fused step, and the device simple tracker on
+    the per-frame route (fused = False, one sb_track_instances call per frame)."""
+    import torch
+    from scipy.ndimage import maximum_filter
+    from sleap_b200.nn import tracking as T
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from flow_clip import clip_frames
+    n, B = 256, 16
+    gray = torch.from_numpy(np.ascontiguousarray(clip_frames(n)[:, :, :, :1])).pin_memory().numpy()
+    cspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="centroid", part_names=None, edges=None,
+                 heads=[dict(name="CentroidConfmapsHead", channels=1, output_stride=2)])
+    ispec = dict(backbone="unet", backbone_cfg=dict(unet(24, 16, 4), up_interpolate=False), head_type="centered_instance",
+                 part_names=FLIES13, edges=None, heads=[dict(name="CenteredInstanceConfmapsHead", channels=13, output_stride=4)])
+
+    def predictor(fused):
+        # the per-frame arm owns its two device models: its staged calls reconfigure the chains the fused pipeline needs
+        cm_model, _, _ = model_for(cspec, 1, 1003, input_scale=0.5)
+        cms = np.concatenate([cm_model.forward(gray[i:i + B])[0][..., 0] for i in range(0, 4 * B, B)])
+        fifth = [np.sort(c[c == maximum_filter(c, size=3, mode="constant", cval=-np.inf)])[-5] for c in cms]
+        pred = TopDownPredictor(cm_model, model_for(ispec, 1, 1004)[0], crop_size=160, peak_threshold=float(np.median(fifth)),
+                                integral_refinement=True, batch_size=B, max_instances=5)
+        pred.inference_model.instance_peaks.peak_threshold = 0.0
+        pred.inference_model.fused = fused
+        return pred
+
+    fused_pred, frame_pred = predictor(True), predictor(False)
+    simple = dict(tracker="simple", similarity="instance", match="greedy")
+    arms = {"no tracker": (fused_pred, lambda: None),
+            "simple host": (fused_pred, lambda: T.Tracker.make_tracker_by_name(**simple)),
+            "simple device, fused step": (fused_pred, lambda: T.Tracker.make_tracker_by_name(track_device=0, **simple)),
+            "simple device, per-frame route (fused = False)": (frame_pred, lambda: T.Tracker.make_tracker_by_name(track_device=0, **simple))}
+
+    def run(name, frames):
+        pred, mk = arms[name]
+        pred.tracker = mk()
+        return pred.predict(frames)
+
+    outs = {k: run(k, gray) for k in arms}                              # warm-up, and the outputs compared
+    from track_cases import host_twin                                   # the host tracker with the device's greedy tie rule
+    fused_pred.tracker = host_twin(**simple)
+    stable = fused_pred.predict(gray)
+    reps = max(3, steps)
+    times = {k: [] for k in arms}
+    for _ in range(reps):                                                # arms alternate
+        for k in arms:
+            t0 = time.perf_counter()
+            run(k, gray)
+            times[k].append(time.perf_counter() - t0)
+    names = lambda frames: [[x.track.name if x.track else None for x in lf.instances] for lf in frames]
+    return {"config": "topdown_track: C3 top-down pair, TopDownPredictor.predict with labels, 256 tracking-clip frames "
+                      "(1024x1024 gray), max 5 animals, B=16", "gpu": gpu_identity(),
+            "metric": "frames/s (median of alternating repetitions; host frames in, labeled frames out)", "repetitions": reps,
+            "frames_per_s": {k: n / float(np.median(v)) for k, v in times.items()},
+            "frames_per_s_spread": {k: [n / max(v), n / min(v)] for k, v in times.items()},
+            "instances_per_frame": {k: float(np.mean([len(lf.instances) for lf in v])) for k, v in outs.items()},
+            "tracks": {k: len({x.track.name for lf in v for x in lf.instances if x.track}) for k, v in outs.items()},
+            "device_tracks_equal_host": names(outs["simple device, fused step"]) == names(outs["simple host"]),
+            "device_tracks_equal_host_stable_ties": names(outs["simple device, fused step"]) == names(stable),
+            "routes_agree": names(outs["simple device, fused step"]) == names(outs["simple device, per-frame route (fused = False)"])}
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -464,6 +536,8 @@ if __name__ == "__main__":
             r = multiclass_bench(steps)
         elif c == "topdown_multiclass":
             r = topdown_multiclass_bench(steps)
+        elif c == "topdown_track":
+            r = topdown_track_bench(steps)
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
