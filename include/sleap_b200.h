@@ -168,7 +168,7 @@ int sb_model_profile_ops(sb_handle_t h, int model_id, const uint8_t* frames_dev,
                          float* out_ms, int32_t* out_kind, double* out_flops, int32_t* out_n_ops);
 
 /* Live timing of the network part of every step: while enabled, each forward pass (whatever entry point runs it:
- * sb_model_forward, sb_infer_*, sb_bottomup_submit, sb_infer_topdown) is bracketed by a pair of CUDA events on the
+ * sb_model_forward, sb_infer_*, the *_submit calls and the top-down collects, sb_infer_topdown) is bracketed by a pair of CUDA events on the
  * launching stream.  A call synchronises that stream, returns the milliseconds of the passes recorded since the last
  * call (at most cap, at most 1024 are kept), clears them, and switches the recording on / off.  bench.py derives
  * `roofline.achieved` from the passes of its timed region.  Replaces nothing in the reference (it has no device
@@ -331,6 +331,10 @@ typedef struct sb_global_params {
 int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* params);
 int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int images_are_u8,
                     int B, const float* crop_offsets_host, float* out_points, float* out_vals);
+/* The double-buffered form, as sb_bottomup_submit / sb_bottomup_collect (uint8 frames, no crop offsets): the global
+ * peaks run on the post-processing stream and the points | values block comes back in one copy per batch. */
+int sb_global_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
+int sb_global_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals);
 
 /* sleap/nn/inference.py:1638-1966 CentroidCrop.call: net -> local peaks -> * output_stride ->
  * /input_scale + 0.5; returns flat centroid list ordered by (sample, y, x) like the reference
@@ -369,6 +373,22 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* params, int max
 int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
                      float* out_centroids, float* out_centroid_vals, float* out_instance_peaks,
                      float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
+/* The double-buffered form (uint8 frames; arguments as sb_bottomup_submit / _collect, outputs as sb_infer_topdown).  A
+ * step is a centroid stage (network, peaks, top-k, crop list, the crop count's copy to the host) and an instance stage
+ * (crops, instance network, peaks, records, tracker, the records' copy).  sb_topdown_submit queues the batch's upload on
+ * a copy stream into slot `slot`, then the instance stage of the batch submitted before it (waiting on the host for that
+ * batch's crop count, which its centroid stage produced while the GPU ran it), then the batch's own centroid stage.
+ * sb_topdown_collect queues the batch's instance stage if no submit did, and blocks until its records are on the host.
+ * Refused (SB_ERR_INVALID): a submit into a slot whose batch was not collected; a collect of a slot that holds no batch,
+ * with another B, or before the batch submitted earlier; sb_infer_topdown*, sb_infer_centroids on the centroid model and
+ * sb_topdown_attach_tracker while a batch is submitted and not collected; a submit or collect of the other pipeline form.
+ * A configure call on either model drops the submitted batches (after their work has finished); collecting one then fails.
+ * A batch's instance stage, and with it the attached tracker's step, is queued by the next submit or by its collect:
+ * sb_tracker_reset between a batch's submit and that point applies before the batch is tracked, and the attached tracker
+ * must not be destroyed while a batch is submitted. */
+int sb_topdown_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot);
+int sb_topdown_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+                       float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
 
 /* ---- top-down multi-class (identity) step ---------------------------------------------------------
  * sleap/nn/inference.py:4139-4210 TopDownMultiClassInferenceModel.call = CentroidCrop.call -> TopDownMultiClassFindPeaks.call
@@ -408,6 +428,12 @@ int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_p
 int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
                                 float* out_centroids, float* out_centroid_vals, float* out_points, float* out_vals,
                                 float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors);
+/* The double-buffered form, with the rules of sb_topdown_submit / sb_topdown_collect; outputs as
+ * sb_infer_topdown_multiclass (out_class_vectors may be NULL). */
+int sb_topdown_multiclass_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot);
+int sb_topdown_multiclass_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids,
+                                  float* out_centroid_vals, float* out_points, float* out_vals, float* out_class_probs,
+                                  int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors);
 /* The same post-processing on caller-supplied crops (no network): confidence maps (n_crops,H,W,n_nodes), optional learned
  * offsets (n_crops,H,W,2*n_nodes), float32 feature maps (n_crops,Hf,Wf,Cf) read as the tap, optional crop offsets
  * (n_crops,2), crop_sample_inds (n_crops) non-decreasing in [0, B).  Uses params->topdown.instance and the head fields;
@@ -522,9 +548,12 @@ int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tr
  * until sb_tracker_reset (as a full queue table does).  The pipeline must be a plain one (sb_topdown_configure), and the
  * tracker must live on its handle and have its instance model's node count; img_h, img_w > 0.  The attachment lives
  * with the pipeline: a configure call on either model drops it.  sb_topdown_tracks copies the track records of the last
- * sb_infer_topdown (the bottom-up format above); sb_infer_topdown's outputs do not change. */
+ * sb_infer_topdown (the bottom-up format above); sb_infer_topdown's outputs do not change.  Streamed batches are tracked
+ * in submit order; sb_topdown_slot_tracks copies the track records of the batch last collected from slot 0 / 1 (B must
+ * be that batch's frame count). */
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w);
 int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_tracks);
+int sb_topdown_slot_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks);
 
 #ifdef __cplusplus
 }

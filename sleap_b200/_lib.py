@@ -157,11 +157,18 @@ _SIGS = {
     "sb_gather_close": [c_void_p, c_int],
     "sb_global_configure": [c_void_p, c_int, POINTER(GlobalParams)],
     "sb_infer_global": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "sb_global_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
+    "sb_global_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
     "sb_topdown_configure": [c_void_p, POINTER(TopdownParams), c_int, c_int, c_int, c_int],
     "sb_infer_topdown": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sb_topdown_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
+    "sb_topdown_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sb_topdown_multiclass_configure": [c_void_p, POINTER(TopdownMultiClassParams), c_int, c_int, c_int, c_int],
     "sb_infer_topdown_multiclass": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p],
+    "sb_topdown_multiclass_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
+    "sb_topdown_multiclass_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_void_p],
     "sb_topdown_multiclass_from_features": [c_void_p, POINTER(TopdownMultiClassParams), c_void_p, c_int, c_int, c_int, c_int,
                                             c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
                                             c_void_p, c_void_p, c_void_p, c_void_p],
@@ -181,6 +188,7 @@ _SIGS = {
     "sb_bottomup_device_tracks": [c_void_p, c_int, c_int, c_void_p],
     "sb_topdown_attach_tracker": [c_void_p, c_int, c_int, ctypes.c_double, ctypes.c_double],
     "sb_topdown_tracks": [c_void_p, c_int, c_int, c_void_p],
+    "sb_topdown_slot_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
     "sb_tracker_destroy": [c_void_p, c_int],
     "sb_track_instances": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), POINTER(c_int32)],

@@ -29,7 +29,7 @@ int build_programs(sb_handle_s* h, SbModel* m);   // the last step of sb_model_c
 }  // namespace
 
 void sb_global_scratch_free(SbGlobalScratch& g) {
-  for (float* p : {g.part, g.points, g.vals, g.crop_off}) if (p) cudaFree(p);
+  for (float* p : {g.part, g.points, g.crop_off}) if (p) cudaFree(p);    // vals lives in the points block
   g = SbGlobalScratch();
 }
 
@@ -38,8 +38,8 @@ int sb_global_scratch_alloc(sb_handle_s* h, SbGlobalScratch& g, int B, int H, in
   g.rpc = std::max(1, (H + target - 1) / target);
   g.chunks = (H + g.rpc - 1) / g.rpc;
   SB_CUDA(h, cudaMalloc((void**)&g.part, (size_t)B * g.chunks * C * 3 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&g.points, (size_t)B * C * 2 * 4));
-  SB_CUDA(h, cudaMalloc((void**)&g.vals, (size_t)B * C * 4));
+  SB_CUDA(h, cudaMalloc((void**)&g.points, (size_t)B * C * 3 * 4));
+  g.vals = g.points + (size_t)B * C * 2;
   SB_CUDA(h, cudaMalloc((void**)&g.crop_off, (size_t)B * 2 * 4));
   return 0;
 }
@@ -576,7 +576,10 @@ static int post_guard_op(const SbModel* m, int b0, int b1, int b2) {
   return -1;
 }
 
+// Floats per frame of the chain's result block: its records, or for the global chain points and values (the block is
+// [B][C][2] points | [B][C] values at the configured B, one copy of the whole block)
 static size_t record_width(const SbModel* m) {
+  if (m->chain == SB_CHAIN_GLOBAL) return (size_t)m->buffers[m->gl.cms_buffer].C * 3;
   return m->chain == SB_CHAIN_CLASS ? sb_class_record_width(m->mc.n_classes, m->mc.n_nodes) : sb_record_width(m->bu.max_instances, m->bu.n_nodes);
 }
 
@@ -667,6 +670,25 @@ int sb_graph_flatten(sb_handle_s* h, const SbPostWs& ws, const SbGraphHost& g, c
   return SB_OK;
 }
 
+int sb_slot_upload(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot) {
+  if (!m->copy_stream) {
+    SB_CUDA(h, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i) {
+      SB_CUDA(h, cudaEventCreateWithFlags(&m->h2d_done_ev[i], cudaEventDisableTiming));
+      SB_CUDA(h, cudaEventCreateWithFlags(&m->frames_free_ev[i], cudaEventDisableTiming));
+      SB_CUDA(h, cudaEventCreateWithFlags(&m->result_ev[i], cudaEventDisableTiming));
+    }
+  }
+  const size_t fbytes = (size_t)m->B * m->Hin * m->Win * m->Cin;
+  for (int i = 0; i < 2; ++i)
+    if (!m->frames_slot[i]) SB_CUDA(h, cudaMalloc(&m->frames_slot[i], fbytes));
+  // H2D on the copy stream (after the work that last read this slot's frames has finished)
+  if (m->slot_used[slot]) SB_CUDA(h, cudaStreamWaitEvent(m->copy_stream, m->frames_free_ev[slot], 0));
+  SB_CUDA(h, cudaMemcpyAsync(m->frames_slot[slot], frames_host, (size_t)B * m->Hin * m->Win * m->Cin, cudaMemcpyHostToDevice, m->copy_stream));
+  SB_CUDA(h, cudaEventRecord(m->h2d_done_ev[slot], m->copy_stream));
+  return 0;
+}
+
 extern "C" {
 
 int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params* p) {
@@ -725,7 +747,10 @@ static size_t stage_floats(const SbModel* m) {          // [world][B][width] whe
 static int queue_result_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, float* dst, int counts_slot) {
   if (m->gather.connected)
     return sb_gather_queue_collect(h, m, m->gather.step - 1, B, dst, m->gather.counts_dev + counts_slot * SB_GATHER_MAX_WORLD, rs);
-  SB_CUDA(h, cudaMemcpyAsync(dst, m->ws.records, (size_t)B * record_width(m) * sizeof(float), cudaMemcpyDeviceToHost, rs));
+  // the global chain's values sit at the configured batch's offset of its block, so the whole block comes over (B <= m->B)
+  const bool global = m->chain == SB_CHAIN_GLOBAL;
+  SB_CUDA(h, cudaMemcpyAsync(dst, global ? m->gs.points : m->ws.records, (global ? m->B : B) * record_width(m) * sizeof(float),
+                             cudaMemcpyDeviceToHost, rs));
   return 0;
 }
 static const float* own_slice(const SbModel* m, const float* staged, int B) {
@@ -774,6 +799,14 @@ static int multiclass_post_kernels(sb_handle_s* h, const sb_multiclass_params& p
 // The step's chain on the head buffers: the multi-class one, or the PAF one with the record exchange pushed from k_group's
 // epilogue when connected, else the attached tracker after it.
 static int step_post_kernels(sb_handle_s* h, SbModel* m, int B) {
+  if (m->chain == SB_CHAIN_GLOBAL) {
+    const sb_global_params& p = m->gl;
+    const SbBuffer& cb = m->buffers[p.cms_buffer];
+    const SbGlobalScratch& g = m->gs;
+    SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
+    return sbk_global_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, nullptr, g.part,
+                            g.chunks, g.rpc, g.points, g.vals);
+  }
   if (m->chain == SB_CHAIN_CLASS) {
     const sb_multiclass_params& p = m->mc;
     return multiclass_post_kernels(h, p, m->ws, head_map(m, p.cms_buffer), head_map(m, p.class_maps_buffer),
@@ -906,25 +939,12 @@ int sb_get_post_stream(sb_handle_t h, void** out_stream) {
 static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot) {
   if (slot < 0 || slot > 1 || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
   SB_CUDA(h, cudaSetDevice(h->device));
-  if (!m->copy_stream) {
-    SB_CUDA(h, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->h2d_done_ev[i], cudaEventDisableTiming));
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->frames_free_ev[i], cudaEventDisableTiming));
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->result_ev[i], cudaEventDisableTiming));
-    }
-  }
-  const size_t fbytes = (size_t)m->B * m->Hin * m->Win * m->Cin;
-  for (int i = 0; i < 2; ++i) {
-    if (!m->frames_slot[i]) SB_CUDA(h, cudaMalloc(&m->frames_slot[i], fbytes));
+  int rc = sb_slot_upload(h, m, frames_host, B, slot);
+  if (rc) return rc;
+  for (int i = 0; i < 2; ++i)
     if (!m->stage_host[i]) SB_CUDA(h, cudaHostAlloc((void**)&m->stage_host[i], stage_floats(m) * sizeof(float), cudaHostAllocDefault));
-  }
-  // H2D on the copy stream (after the network that last read this slot's frames has finished)
-  if (m->slot_used[slot]) SB_CUDA(h, cudaStreamWaitEvent(m->copy_stream, m->frames_free_ev[slot], 0));
-  SB_CUDA(h, cudaMemcpyAsync(m->frames_slot[slot], frames_host, (size_t)B * m->Hin * m->Win * m->Cin, cudaMemcpyHostToDevice, m->copy_stream));
-  SB_CUDA(h, cudaEventRecord(m->h2d_done_ev[slot], m->copy_stream));
   SB_CUDA(h, cudaStreamWaitEvent(h->stream, m->h2d_done_ev[slot], 0));
-  int rc = sb_run_ops(h, m, m->frames_slot[slot], 1, B);
+  rc = sb_run_ops(h, m, m->frames_slot[slot], 1, B);
   if (rc) return rc;
   SB_CUDA(h, cudaEventRecord(m->frames_free_ev[slot], h->stream));
   if ((rc = bottomup_post(h, m, B))) return rc;
@@ -1146,6 +1166,8 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
 }
 
 // ---------------------------------- global peaks (single / centered instance) ----------------
+static const char* const kNoGlobal = "global-peak predictor not configured";
+
 int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* p) {
   SbModel* m = configure_target(h, model_id, p);
   if (!m) return SB_ERR_INVALID;
@@ -1158,16 +1180,21 @@ int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* p) 
   int rc = chain_drop(h, m);
   if (rc || (rc = sb_global_scratch_alloc(h, m->gs, m->B, cb.H, cb.C))) return rc;
   m->gl = *p;
+  m->guard_op = post_guard_op(m, p->cms_buffer, p->cms_buffer, p->offsets_buffer);
   m->chain = SB_CHAIN_GLOBAL;
   return SB_OK;
 }
 
 int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int images_are_u8, int B,
                     const float* crop_offsets_host, float* out_points, float* out_vals) {
-  SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, "global-peak predictor not configured");
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
   if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
+  if (h->post_pending) {             // a streamed batch's peaks and result copy may still use the scratch
+    SB_CUDA(h, cudaStreamSynchronize(h->post_stream));
+    h->post_pending = false;
+  }
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
   if (rc) return rc;
   const SbGlobalScratch& g = m->gs;
@@ -1181,6 +1208,24 @@ int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int im
   SB_CUDA(h, cudaMemcpyAsync(out_points, g.points, (size_t)B * cb.C * 8, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaMemcpyAsync(out_vals, g.vals, (size_t)B * cb.C * 4, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
+  return SB_OK;
+}
+
+// The double-buffered form of sb_infer_global (uint8 frames, no crop offsets): the chain's global peaks run on the
+// post-processing stream, as the bottom-up chains do, and the points | values block comes back in one copy.
+int sb_global_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
+  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
+}
+
+int sb_global_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals) {
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
+  if (!m) return SB_ERR_INVALID;
+  if (!out_points || !out_vals) return sb_fail(h, SB_ERR_INVALID, "sb_global_collect: null argument");
+  if (const int rc = step_collect(h, m, slot, B)) return rc;
+  const size_t C = m->buffers[m->gl.cms_buffer].C;
+  memcpy(out_points, m->stage_host[slot], (size_t)B * C * 2 * sizeof(float));
+  memcpy(out_vals, m->stage_host[slot] + (size_t)m->B * C * 2, (size_t)B * C * sizeof(float));
   return SB_OK;
 }
 
@@ -1208,6 +1253,8 @@ int sb_infer_centroids(sb_handle_t h, int model_id, const void* images_host, int
   if (!m) return SB_ERR_INVALID;
   SB_CUDA(h, cudaSetDevice(h->device));
   if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
+  if (sb_topdown_busy(m))      // the pending instance stage reads this workspace's flags
+    return sb_fail(h, SB_ERR_INVALID, "sb_infer_centroids: a top-down batch was submitted and not collected; collect it first");
   int rc = upload_frames(h, m, images_host, images_are_u8, B);
   if (rc) return rc;
   if ((rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B))) return rc;

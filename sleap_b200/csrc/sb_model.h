@@ -136,7 +136,8 @@ struct SbModel {
   std::vector<int> bu_edges;
   sb_multiclass_params mc{};
   int guard_op = -1;
-  // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect, sb_multiclass_submit / _collect)
+  // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect, sb_multiclass_submit / _collect,
+  // sb_global_submit / _collect; the top-down submit uses the frame slots, the copy stream and the events of its centroid model)
   void* frames_slot[2] = {nullptr, nullptr};
   float* stage_host[2] = {nullptr, nullptr};     // pinned result staging (per-frame records)
   int slot_B[2] = {0, 0}, rec_B = 0;            // frames of the batch last staged in each slot / in rec_host
@@ -171,6 +172,7 @@ int sb_run_ops(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_ar
 SbModel* chain_model(sb_handle_s* h, int id, int kind, const char* what);
 
 void sb_topdown_free(SbModel* m);        // sb_topdown.cu
+bool sb_topdown_busy(const SbModel* m);  // the model's top-down pipeline holds a submitted batch not yet collected
 
 // Sizes the model's track records (trk_dev, trk_host) for B frames of a tracker of I instances; keeps larger ones
 int sb_track_records_alloc(sb_handle_s* h, SbModel* m, int B, int I);
@@ -181,6 +183,10 @@ void sb_gather_free(SbModel* m);
 // queues on `s`: wait for every rank's records of `step`, copy the [world][B][width] window to host_dst, acknowledge
 int sb_gather_queue_collect(sb_handle_s* h, SbModel* m, long long step, int B, float* host_dst, int* counts_dev, cudaStream_t s);
 void sb_pipeline_slots_free(SbModel* m);
+// The frame half of a streamed submit into `slot`: the copy stream and slot events (created once), the two device frame
+// slots ([m->B] uint8 frames), and the batch's H2D copy on the copy stream into frames_slot[slot] once the work that last
+// read that slot is done (frames_free_ev); h2d_done_ev[slot] marks its end.  The caller makes its stream wait on it.
+int sb_slot_upload(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot);
 
 // tensor-core conv path (sb_conv_tc.cu)
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m);      // after buffers are allocated

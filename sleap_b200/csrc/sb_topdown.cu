@@ -16,7 +16,6 @@
 // The head's float64 sums use __dmul_rn / __dadd_rn: this file is built with multiply-add contraction on, and a fused
 // product would round differently from the definition (include/sleap_b200.h).
 #include <algorithm>
-#include <functional>
 #include <limits>
 #include <time.h>
 
@@ -334,6 +333,16 @@ struct SbTopdown {
   bool tap_half = false, all_stores = false;   // fp16 storage; the production program elides the tap buffer
   float* dense = nullptr;                      // packed dense weights
   float* probs = nullptr;                      // [Bmax * K][n_classes] per-crop class probabilities
+  // streaming (sb_topdown_submit / _collect), allocated at the first submit: per slot the pinned crop count and its
+  // event, the pinned record staging, multi-class the pinned class probabilities of its crops, the frames of the batch it
+  // holds (0: none) with its submit number, and the frames of the batch last collected from it (0: none); `pending` is the
+  // slot whose instance stage is not queued yet (-1: none).  The frames live in the centroid model's frame slots.
+  int* count_host = nullptr;                   // [2]
+  float* stage[2] = {nullptr, nullptr};
+  float* probs_stage[2] = {nullptr, nullptr};  // [Bmax * K][n_classes]
+  cudaEvent_t count_ev[2] = {nullptr, nullptr};
+  int slot_B[2] = {0, 0}, done_B[2] = {0, 0}, pending = -1;
+  unsigned long long slot_seq[2] = {0, 0}, seq = 0;
 };
 
 void sb_topdown_free(SbModel* m) {
@@ -342,8 +351,10 @@ void sb_topdown_free(SbModel* m) {
   void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
                  t->offsets, t->total, t->crops, t->dense, t->probs};
   for (void* p : dev) if (p) cudaFree(p);
-  if (t->record_host) cudaFreeHost(t->record_host);
-  if (t->total_host) cudaFreeHost(t->total_host);
+  for (void* p : {(void*)t->record_host, (void*)t->total_host, (void*)t->count_host, (void*)t->stage[0], (void*)t->stage[1],
+                  (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
+    if (p) cudaFreeHost(p);
+  for (cudaEvent_t e : t->count_ev) if (e) cudaEventDestroy(e);
   delete t;
   m->td = nullptr;
   m->trk = nullptr;                              // an attached tracker lives with the pipeline
@@ -399,16 +410,21 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   return SB_OK;
 }
 
-// The pipeline of centroid model `id` when it is of the wanted form and neither model was reconfigured since
-SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass) {
+// The pipeline of centroid model `id` when it is of the wanted form and neither model was reconfigured since.  `streamed`:
+// the refusal of the wrong form names the submit call rather than the synchronous one.
+SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = false) {
   static const char* const none = "top-down pipeline not configured";
   SbModel* mc = chain_model(h, id, SB_CHAIN_ANY, none);
   if (!mc) return nullptr;
   SbTopdown* t = mc->td;
   if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
   if (t->multiclass != multiclass) {
-    sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_infer_topdown"
-                                          : "top-down pipeline is multi-class: call sb_infer_topdown_multiclass");
+    if (streamed)
+      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_submit"
+                                            : "top-down pipeline is multi-class: call sb_topdown_multiclass_submit");
+    else
+      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_infer_topdown"
+                                            : "top-down pipeline is multi-class: call sb_infer_topdown_multiclass");
     return nullptr;
   }
   SbModel* mi = t->inst;
@@ -421,22 +437,19 @@ SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass) {
   return t;
 }
 
-// One batch through the pipeline: frames up, centroid network, local peaks, top-k, crop list (the one mid-pipeline sync,
-// for the crop count), then per chunk of crops the crop kernel, the instance network, the global peaks and chunk(c0, n);
-// then pack() writes the records, which come back into t->record_host.
-int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_host, int frames_are_u8, int B, bool all_stores,
-                const std::function<int(int c0, int n)>& chunk, const std::function<int()>& pack) {
-  SbModel* mi = t->inst;
-  if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
-  SB_CUDA(h, cudaSetDevice(h->device));
+// Refuses a call that would overwrite the single selection, crop and record buffers while a streamed batch holds them
+int check_idle(sb_handle_s* h, const SbTopdown* t, const char* what) {
+  if (t->slot_B[0] || t->slot_B[1])
+    return sb_fail(h, SB_ERR_INVALID, "%s: a batch was submitted and not collected; collect it first", what);
+  return 0;
+}
+
+// The centroid stage of B frames resident at frames_dev: centroid network, local peaks, top-k, the flat crop list, then
+// the crop count's copy into *count_host and, given, count_ev.
+int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int* count_host,
+                   cudaEvent_t count_ev) {
   cudaStream_t s = h->stream;
-  const size_t esz = frames_are_u8 ? 1 : 4;
-  static const bool dbg = getenv("SB_DEBUG_TD") != nullptr;      // stage timing (host clock around stream syncs), profiling only
-  auto now = []() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; };
-  double t0 = now(), t1 = 0, t2 = 0, t3 = 0;
-  SB_CUDA(h, cudaMemcpyAsync(mc->frames_dev, frames_host, (size_t)B * mc->Hin * mc->Win * mc->Cin * esz, cudaMemcpyHostToDevice, s));
-  if (dbg) { cudaStreamSynchronize(s); t1 = now(); }
-  int rc = sb_run_ops(h, mc, mc->frames_dev, frames_are_u8, B);
+  int rc = sb_run_ops(h, mc, frames_dev, frames_are_u8, B);
   if (rc) return rc;
   const sb_centroid_params& cp = mc->ce;
   SbBuffer& cb = mc->buffers[cp.cms_buffer];
@@ -449,27 +462,83 @@ int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_ho
   k_td_flatten<<<1, 256, 0, s>>>(t->sel_cent, t->sel_count, B, t->K, (float)t->p.crop_size * 0.5f, t->flat_cent, t->flat_off,
                                  t->flat_sample, t->offsets, t->total);
   SB_CHECK_LAUNCH(h);
-  SB_CUDA(h, cudaMemcpyAsync(t->total_host, t->total, 4, cudaMemcpyDeviceToHost, s));
-  SB_CUDA(h, cudaStreamSynchronize(s));                     // the one mid-pipeline sync: how many crops the instance net runs on
-  const int total = *t->total_host;
-  if (dbg) t2 = now();
+  SB_CUDA(h, cudaMemcpyAsync(count_host, t->total, 4, cudaMemcpyDeviceToHost, s));
+  if (count_ev) SB_CUDA(h, cudaEventRecord(count_ev, s));
+  return 0;
+}
+
+// The instance stage of the batch the centroid stage left in the selection buffers (`total` crops of the B frames at
+// frames_dev): per chunk of crops the crop kernel, the instance network, the global peaks and, multi-class, the class
+// vectors; frames_free (given) after the last crop kernel; then the records -- k_td_class_assign, or k_td_pack and the
+// attached tracker -- copied into rec_host, the track records into trk_host and, given, the crops' class probabilities
+// into probs_host.
+int instance_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int total,
+                   float* rec_host, double* trk_host, float* probs_host, cudaEvent_t frames_free) {
+  cudaStream_t s = h->stream;
+  SbModel* mi = t->inst;
   const sb_global_params& gp = mi->gl;
   SbBuffer& ib = mi->buffers[gp.cms_buffer];
   const float* ioff = gp.offsets_buffer >= 0 ? (const float*)mi->buffers[gp.offsets_buffer].dev : nullptr;
   SbPeakParams pi{gp.peak_threshold, gp.refinement, gp.integral_patch_size, (float)gp.output_stride, gp.input_scale};
-  const int cs = t->p.crop_size;
+  const int cs = t->p.crop_size, NC = t->head.n_classes;
+  const SbBuffer* tb = t->multiclass ? &mi->buffers[t->tap_buf] : nullptr;
+  int rc;
   for (int c0 = 0; c0 < total; c0 += mi->B) {
     const int n = std::min(mi->B, total - c0);
     // crops of the frames already resident in HBM (uint8 frames: float -> uint8 truncation, as tf.cast in crop_bboxes)
-    if ((rc = sbk_crop(h, mc->frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
+    if ((rc = sbk_crop(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
                        cs, cs, t->crops, frames_are_u8))) return rc;
-    if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n, all_stores))) return rc;
+    if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n, t->all_stores))) return rc;
     if ((rc = sbk_global_peaks(h, (const float*)ib.dev, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
                                t->ipts + (size_t)c0 * t->nodes * 2, t->ivals + (size_t)c0 * t->nodes))) return rc;
-    if ((rc = chunk(c0, n))) return rc;
+    if (tb && (rc = launch_class_vectors(h, (const char*)tb->dev + (size_t)t->tap_coff * (t->tap_half ? 2 : 4), t->tap_half, tb->C,
+                                         t->tap_hi, t->head, n, t->probs + (size_t)c0 * NC, nullptr)))
+      return rc;
   }
-  if ((rc = pack())) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(t->record_host, t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, s));
+  if (frames_free) SB_CUDA(h, cudaEventRecord(frames_free, s));
+  if (t->multiclass) {
+    if ((rc = launch_class_assign(h, t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->probs, B, t->K, t->nodes,
+                                  NC, mc->ws.flags, t->record)))
+      return rc;
+    if (probs_host && total > 0)
+      SB_CUDA(h, cudaMemcpyAsync(probs_host, t->probs, (size_t)total * NC * 4, cudaMemcpyDeviceToHost, s));
+  } else {
+    k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags,
+                                t->record, t->width);
+    SB_CHECK_LAUNCH(h);
+    if (mc->trk) {
+      // the attached tracker on the frames' instance lists; its records come back with the step's records
+      if ((rc = sbk_track_topdown(h, mc->trk, B, t->ipts, t->ivals, t->sel_val, t->sel_count, t->offsets, t->K, mc->trk_h, mc->trk_w,
+                                  mc->trk_dev)))
+        return rc;
+      SB_CUDA(h, cudaMemcpyAsync(trk_host, mc->trk_dev, (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double),
+                                 cudaMemcpyDeviceToHost, s));
+    }
+  }
+  SB_CUDA(h, cudaMemcpyAsync(rec_host, t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, s));
+  return 0;
+}
+
+// One synchronous batch: frames up, the centroid stage, the one mid-pipeline sync (how many crops the instance network
+// runs on), the instance stage, the final sync.  The records land in t->record_host.
+int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_host, int frames_are_u8, int B, const char* what) {
+  if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
+  if (const int rc = check_idle(h, t, what)) return rc;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  const size_t esz = frames_are_u8 ? 1 : 4;
+  static const bool dbg = getenv("SB_DEBUG_TD") != nullptr;      // stage timing (host clock around stream syncs), profiling only
+  auto now = []() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; };
+  double t0 = now(), t1 = 0, t2 = 0, t3 = 0;
+  SB_CUDA(h, cudaMemcpyAsync(mc->frames_dev, frames_host, (size_t)B * mc->Hin * mc->Win * mc->Cin * esz, cudaMemcpyHostToDevice, s));
+  if (dbg) { cudaStreamSynchronize(s); t1 = now(); }
+  int rc = centroid_stage(h, mc, t, mc->frames_dev, frames_are_u8, B, t->total_host, nullptr);
+  if (rc) return rc;
+  SB_CUDA(h, cudaStreamSynchronize(s));
+  const int total = *t->total_host;
+  if (dbg) t2 = now();
+  if ((rc = instance_stage(h, mc, t, mc->frames_dev, frames_are_u8, B, total, t->record_host, mc->trk_host[2], nullptr, nullptr)))
+    return rc;
   SB_CUDA(h, cudaStreamSynchronize(s));
   if (dbg) {
     t3 = now();
@@ -479,7 +548,111 @@ int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_ho
   return SB_OK;
 }
 
+// Queues the instance stage of the pending streamed batch (its count event waited for on the host) behind whatever the
+// handle's stream holds.  The slot is dropped when it fails.
+int queue_pending_instance(sb_handle_s* h, SbModel* mc, SbTopdown* t) {
+  const int k = t->pending;
+  t->pending = -1;
+  cudaError_t e = cudaEventSynchronize(t->count_ev[k]);
+  int rc = e == cudaSuccess ? 0 : sb_fail(h, SB_ERR_CUDA, "crop count: %s", cudaGetErrorString(e));
+  if (!rc) {
+    rc = instance_stage(h, mc, t, mc->frames_slot[k], 1, t->slot_B[k], t->count_host[k], t->stage[k], mc->trk_host[k],
+                        t->probs_stage[k], mc->frames_free_ev[k]);
+  }
+  if (!rc) {
+    e = cudaEventRecord(mc->result_ev[k], h->stream);
+    if (e != cudaSuccess) rc = sb_fail(h, SB_ERR_CUDA, "event record: %s", cudaGetErrorString(e));
+  }
+  if (rc) t->slot_B[k] = 0;
+  return rc;
+}
+
+// The streaming staging of the pipeline, allocated once at its first submit (synchronous users never pay for it)
+int stream_alloc(sb_handle_s* h, SbTopdown* t) {
+  if (t->count_host) return 0;
+  const size_t rec_bytes = (size_t)t->Bmax * t->width * 4, probs_bytes = (size_t)t->Bmax * t->K * t->head.n_classes * 4;
+  for (int i = 0; i < 2; ++i) {
+    if (!t->stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&t->stage[i], rec_bytes, cudaHostAllocDefault));
+    if (t->multiclass && !t->probs_stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&t->probs_stage[i], probs_bytes, cudaHostAllocDefault));
+    if (!t->count_ev[i]) SB_CUDA(h, cudaEventCreateWithFlags(&t->count_ev[i], cudaEventDisableTiming));
+  }
+  SB_CUDA(h, cudaHostAlloc((void**)&t->count_host, 2 * sizeof(int), cudaHostAllocDefault));   // last: marks it complete
+  return 0;
+}
+
+// Streamed batch into `slot`: (1) its upload on the copy stream into the slot's frames, once the crops of the batch that
+// last used them have run; (2) the instance stage of the batch submitted before it, if no collect queued it yet;
+// (3) its own centroid stage.  The stream order instance(k) -> centroid(k + 1) lets one set of selection buffers serve.
+int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, int slot, bool multiclass) {
+  SbTopdown* t = topdown_of(h, id, multiclass, true);
+  if (!t) return SB_ERR_INVALID;
+  SbModel* mc = h->models[id];
+  if (slot < 0 || slot > 1 || !frames_host || B <= 0 || B > t->Bmax || B > mc->B)
+    return sb_fail(h, SB_ERR_INVALID, "top-down submit: bad slot / batch");
+  if (t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "top-down submit: slot %d holds a batch that was not collected", slot);
+  SB_CUDA(h, cudaSetDevice(h->device));
+  int rc = stream_alloc(h, t);
+  if (rc || (rc = sb_slot_upload(h, mc, frames_host, B, slot))) return rc;
+  if (t->pending >= 0 && (rc = queue_pending_instance(h, mc, t))) return rc;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, mc->h2d_done_ev[slot], 0));
+  if ((rc = centroid_stage(h, mc, t, mc->frames_slot[slot], 1, B, t->count_host + slot, t->count_ev[slot]))) return rc;
+  mc->slot_used[slot] = true;
+  t->slot_B[slot] = B; t->done_B[slot] = 0; t->slot_seq[slot] = ++t->seq; t->pending = slot;
+  return SB_OK;
+}
+
+// The streamed batch of `slot` in its pinned staging: its instance stage queued if still pending, then its record event
+// waited for.  The slot is free again afterwards.
+int topdown_collect(sb_handle_s* h, SbModel* mc, SbTopdown* t, int slot, int B) {
+  if (slot < 0 || slot > 1 || !t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d holds no submitted batch", slot);
+  if (B != t->slot_B[slot])
+    return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d holds a batch of %d frames, not %d", slot, t->slot_B[slot], B);
+  const int other = 1 - slot;
+  if (t->slot_B[other] && t->slot_seq[other] < t->slot_seq[slot])
+    return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d was submitted first; collect batches in submit order", other);
+  SB_CUDA(h, cudaSetDevice(h->device));
+  int rc = t->pending == slot ? queue_pending_instance(h, mc, t) : 0;
+  if (rc) return rc;
+  t->slot_B[slot] = 0;
+  SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
+  t->done_B[slot] = B;
+  return SB_OK;
+}
+
+// A plain record's fields into the caller's arrays
+void split_topdown(const SbTopdown* t, const float* rec, int B, float* out_centroids, float* out_centroid_vals, float* out_instance_peaks,
+                   float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags) {
+  const size_t K = t->K, nd = t->nodes;
+  sb_split_records(rec, B, t->width,
+                   {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
+                   {out_n_valid, out_flags});
+}
+
+// A multi-class record's fields into the caller's arrays, and the crops' class probabilities (pr: the batch's crops in
+// order, on the host) scattered to (frame, slot)
+void split_topdown_multiclass(const SbTopdown* t, const float* rec, const float* pr, int B, float* out_centroids,
+                              float* out_centroid_vals, float* out_points, float* out_vals, float* out_class_probs, int32_t* out_n_valid,
+                              int32_t* out_flags, float* out_class_vectors) {
+  const int NC = t->head.n_classes;
+  const size_t K = t->K, n1 = (size_t)NC * t->nodes;
+  if (out_class_vectors) {
+    int o = 0;
+    for (int b = 0; b < B; ++b) {
+      const int cnt = (int)rec[(size_t)b * t->width + n1 * 3 + NC + 3 * K];
+      float* dst = out_class_vectors + (size_t)b * K * NC;
+      std::fill(dst, dst + K * NC, std::numeric_limits<float>::quiet_NaN());
+      std::copy(pr + (size_t)o * NC, pr + (size_t)(o + cnt) * NC, dst);
+      o += cnt;
+    }
+  }
+  sb_split_records(rec, B, t->width,
+                   {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}, {out_centroids, K * 2}, {out_centroid_vals, K}},
+                   {out_n_valid, out_flags});
+}
+
 }  // namespace
+
+bool sb_topdown_busy(const SbModel* m) { return m->td && (m->td->slot_B[0] || m->td->slot_B[1]); }
 
 extern "C" {
 
@@ -496,25 +669,21 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
   SbTopdown* t = topdown_of(h, centroid_model_id, false);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[centroid_model_id];
-  auto pack = [&]() {
-    k_td_pack<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags,
-                                        t->record, t->width);
-    SB_CHECK_LAUNCH(h);
-    if (!mc->trk) return 0;
-    // the attached tracker on the frames' instance lists; its records come back before the step's final sync
-    if (const int rc = sbk_track_topdown(h, mc->trk, B, t->ipts, t->ivals, t->sel_val, t->sel_count, t->offsets, t->K, mc->trk_h,
-                                         mc->trk_w, mc->trk_dev))
-      return rc;
-    SB_CUDA(h, cudaMemcpyAsync(mc->trk_host[2], mc->trk_dev, (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double),
-                               cudaMemcpyDeviceToHost, h->stream));
-    return 0;
-  };
-  const int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, false, [](int, int) { return 0; }, pack);
-  if (rc) return rc;
-  const size_t K = t->K, nd = t->nodes;
-  sb_split_records(t->record_host, B, t->width,
-                   {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
-                   {out_n_valid, out_flags});
+  if (const int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, "sb_infer_topdown")) return rc;
+  split_topdown(t, t->record_host, B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
+  return SB_OK;
+}
+
+int sb_topdown_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot) {
+  return topdown_submit(h, centroid_model_id, frames_host, B, slot, false);
+}
+
+int sb_topdown_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+                       float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
+  if (!t) return SB_ERR_INVALID;
+  if (const int rc = topdown_collect(h, h->models[centroid_model_id], t, slot, B)) return rc;
+  split_topdown(t, t->stage[slot], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
   return SB_OK;
 }
 
@@ -522,6 +691,7 @@ int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_
   SbTopdown* t = topdown_of(h, centroid_model_id, false);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[centroid_model_id];
+  if (const int rc = check_idle(h, t, "sb_topdown_attach_tracker")) return rc;
   if (tracker_id < 0) { mc->trk = nullptr; return SB_OK; }
   SbTracker* tr = sb_tracker_get(h, tracker_id);
   if (!tr) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_attach_tracker: no tracker %d on this handle", tracker_id);
@@ -542,6 +712,19 @@ int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_t
   if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
   if (B <= 0 || B > t->Bmax || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad batch");
   memcpy(out_tracks, mc->trk_host[2], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
+  return SB_OK;
+}
+
+int sb_topdown_slot_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
+  if (!t) return SB_ERR_INVALID;
+  const SbModel* mc = h->models[centroid_model_id];
+  if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: no tracker attached");
+  if (slot < 0 || slot > 1 || B <= 0 || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: bad slot / batch");
+  if (t->done_B[slot] != B)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: slot %d holds no collected batch of %d frames", slot, B);
+  SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
+  memcpy(out_tracks, mc->trk_host[slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
   return SB_OK;
 }
 
@@ -584,37 +767,26 @@ int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void
                                 float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors) {
   SbTopdown* t = topdown_of(h, centroid_model_id, true);
   if (!t) return SB_ERR_INVALID;
-  SbModel* mc = h->models[centroid_model_id];
-  const SbBuffer& tb = t->inst->buffers[t->tap_buf];
-  const int NC = t->head.n_classes;
-  const size_t esz = t->tap_half ? 2 : 4;
-  auto chunk = [&](int c0, int n) {
-    return launch_class_vectors(h, (const char*)tb.dev + (size_t)t->tap_coff * esz, t->tap_half, tb.C, t->tap_hi, t->head, n,
-                                t->probs + (size_t)c0 * NC, nullptr);
-  };
-  auto pack = [&]() {
-    return launch_class_assign(h, t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->probs, B, t->K, t->nodes,
-                               NC, mc->ws.flags, t->record);
-  };
-  int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, t->all_stores, chunk, pack);
-  if (rc) return rc;
-  const size_t K = t->K, n1 = (size_t)NC * t->nodes;
-  if (out_class_vectors) {                                   // the crops' probabilities, scattered to (frame, slot)
-    const int total = *t->total_host;
-    std::vector<float> pr((size_t)total * NC);
-    if (total > 0) SB_CUDA(h, cudaMemcpy(pr.data(), t->probs, pr.size() * 4, cudaMemcpyDeviceToHost));
-    int o = 0;
-    for (int b = 0; b < B; ++b) {
-      const int cnt = (int)t->record_host[(size_t)b * t->width + n1 * 3 + NC + 3 * K];
-      float* dst = out_class_vectors + (size_t)b * K * NC;
-      std::fill(dst, dst + K * NC, std::numeric_limits<float>::quiet_NaN());
-      std::copy(pr.begin() + (size_t)o * NC, pr.begin() + (size_t)(o + cnt) * NC, dst);
-      o += cnt;
-    }
-  }
-  sb_split_records(t->record_host, B, t->width,
-                   {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}, {out_centroids, K * 2}, {out_centroid_vals, K}},
-                   {out_n_valid, out_flags});
+  if (const int rc = topdown_run(h, h->models[centroid_model_id], t, frames_host, frames_are_u8, B, "sb_infer_topdown_multiclass")) return rc;
+  std::vector<float> pr(out_class_vectors ? (size_t)*t->total_host * t->head.n_classes : 0);
+  if (!pr.empty()) SB_CUDA(h, cudaMemcpy(pr.data(), t->probs, pr.size() * 4, cudaMemcpyDeviceToHost));
+  split_topdown_multiclass(t, t->record_host, pr.data(), B, out_centroids, out_centroid_vals, out_points, out_vals, out_class_probs,
+                           out_n_valid, out_flags, out_class_vectors);
+  return SB_OK;
+}
+
+int sb_topdown_multiclass_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot) {
+  return topdown_submit(h, centroid_model_id, frames_host, B, slot, true);
+}
+
+int sb_topdown_multiclass_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+                                  float* out_points, float* out_vals, float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags,
+                                  float* out_class_vectors) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, true, true);
+  if (!t) return SB_ERR_INVALID;
+  if (const int rc = topdown_collect(h, h->models[centroid_model_id], t, slot, B)) return rc;
+  split_topdown_multiclass(t, t->stage[slot], t->probs_stage[slot], B, out_centroids, out_centroid_vals, out_points, out_vals,
+                           out_class_probs, out_n_valid, out_flags, out_class_vectors);
   return SB_OK;
 }
 

@@ -201,6 +201,37 @@ class SingleInstanceInferenceModel(InferenceModel):
     def call(self, example):
         return self.single_instance_layer.call(example)
 
+    def predict_batches(self, data, batch_size: int = 4):
+        """Generator over per-batch result dicts, double-buffered as BottomUpInferenceModel.predict_batches
+        (sb_global_submit / sb_global_collect): the upload of batch i+1 overlaps the compute of batch i (uint8 frames
+        without return_confmaps; otherwise one predict_on_batch per batch)."""
+        layer = self.single_instance_layer
+        imgs = _images_of(data)
+        n = len(imgs)
+        if n == 0:
+            return
+        first = layer._prep(np.asarray(imgs[0:min(n, batch_size)]))
+        if first.dtype != np.uint8 or layer.return_confmaps:
+            for i in range(0, n, batch_size):        # generic (synchronous) path
+                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
+            return
+        _, H, W, C = first.shape
+        layer._configure(batch_size, H, W, C)
+        m = layer.keras_model
+        n_nodes = head_channels(m, layer.HEAD)
+
+        def collect(slot, B):
+            pts = np.zeros((B, n_nodes, 2), np.float32)
+            vals = np.zeros((B, n_nodes), np.float32)
+            m.handle.call("sb_global_collect", m.model_id, slot, B, ptr(pts), ptr(vals))
+            return {"instance_peaks": pts[:, None], "instance_peak_vals": vals[:, None]}
+
+        yield from _pipelined_batches(layer, imgs, batch_size, "sb_global_submit", collect)
+
+    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
+        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
+        return _merge_batches(list(self.predict_batches(data, batch_size)))
+
 
 # ------------------------------------------------------------------------------------------
 class CentroidCrop(InferenceLayer):
@@ -458,32 +489,67 @@ class TopDownInferenceModel(InferenceModel):
                 cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and cc.keras_model.handle is fp.keras_model.handle
                 and fp.keras_model.input_scale == 1.0)
 
-    def _call_fused(self, imgs):
-        """sb_infer_topdown: frames up once, centroid peaks / top-k / crops / instance network / peaks on the device, one
-        dense record back (include/sleap_b200.h)."""
+    def _configure_fused(self, B, H, W, C):
+        """The fused pipeline for batches of up to B frames of (H, W, C), with ``self.tracker`` attached (the raw frame
+        size, as the predictor's image_hw; default capacity, not K).  Returns K."""
         cc, fp = self.centroid_crop, self.instance_peaks
-        imgs = cc._prep(imgs)
-        B, H, W, C = imgs.shape
-        mc, mi = cc.keras_model, fp.keras_model
+        mc = cc.keras_model
         p, K = _topdown_params(cc, fp)
         _configure_topdown(cc, fp, "sb_topdown_configure", p, (B, H, W, C))
-        n_nodes = head_channels(mi, fp.HEAD)
-        if self.tracker is not None:     # the raw frame size, as the predictor's image_hw; default capacity, not K
-            dev = self.tracker._device_tracker(n_nodes, handle=mc.handle)
+        if self.tracker is not None:
+            dev = self.tracker._device_tracker(head_channels(fp.keras_model, fp.HEAD), handle=mc.handle)
             mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
+        return K
+
+    def _run_fused(self, B, K, fn, *args, tracks=("sb_topdown_tracks",)):
+        """One fused call ``fn(model id, *args, <outputs>)`` into dense arrays of B frames, as a batch dict; the track
+        records through ``tracks`` (call name and leading arguments after the model id)."""
+        mc, n_nodes = self.centroid_crop.keras_model, head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
-        mc.handle.call("sb_infer_topdown", mc.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(ce), ptr(cv), ptr(ip), ptr(iv),
-                       ptr(nv), ptr(fl))
+        mc.handle.call(fn, mc.model_id, *args, B, ptr(ce), ptr(cv), ptr(ip), ptr(iv), ptr(nv), ptr(fl))
         n = int(nv.max()) if B else 0
         out = {"centroids": ce[:, :n].copy(), "centroid_vals": cv[:, :n].copy(), "instance_peaks": ip[:, :n].copy(),
                "instance_peak_vals": iv[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
         if self.tracker is not None:
             rec = np.zeros((B, 2 + 3 * self.tracker._device.max_instances), np.float64)
-            mc.handle.call("sb_topdown_tracks", mc.model_id, B, ptr(rec))
+            mc.handle.call(tracks[0], mc.model_id, *tracks[1:], B, ptr(rec))
             out.update(_track_fields(rec))
         return out
+
+    def _call_fused(self, imgs):
+        """sb_infer_topdown: frames up once, centroid peaks / top-k / crops / instance network / peaks on the device, one
+        dense record back (include/sleap_b200.h)."""
+        imgs = self.centroid_crop._prep(imgs)
+        B, H, W, C = imgs.shape
+        K = self._configure_fused(B, H, W, C)
+        return self._run_fused(B, K, "sb_infer_topdown", ptr(imgs), int(imgs.dtype == np.uint8))
+
+    def predict_batches(self, data, batch_size: int = 4):
+        """Generator over per-batch result dicts, double-buffered (sb_topdown_submit / sb_topdown_collect): the upload
+        of batch i+1 and its centroid stage are queued before batch i is collected.  Frames that are not uint8, and a
+        model that cannot run the fused step, take one predict_on_batch per batch."""
+        imgs = _images_of(data)
+        n = len(imgs)
+        if n == 0:
+            return
+        cc = self.centroid_crop
+        first = cc._prep(np.asarray(imgs[0:min(n, batch_size)])) if self._can_fuse() else None
+        if first is None or first.dtype != np.uint8:
+            for i in range(0, n, batch_size):        # generic (synchronous) path
+                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
+            return
+        K = self._configure_fused(batch_size, *first.shape[1:])
+
+        def collect(slot, B):
+            return self._run_fused(B, K, "sb_topdown_collect", slot, tracks=("sb_topdown_slot_tracks", slot))
+
+        yield from _pipelined_batches(cc, imgs, batch_size, "sb_topdown_submit", collect)
+
+    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
+        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
+        return _merge_batches(list(self.predict_batches(data, batch_size)))
 
     def call(self, example):
         if isinstance(example, np.ndarray):
@@ -678,9 +744,10 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
 
 
 def _pipelined_batches(layer, imgs, batch_size, submit_fn, collect):
-    """The double-buffered batch loop of the bottom-up models (uint8 frames, chain configured): batch i+1 is submitted
+    """The double-buffered batch loop of the streaming models (uint8 frames, chain configured): batch i+1 is submitted
     (``submit_fn``: its upload on the copy stream, network and post-processing queued) into slot (i+1) % 2 before
-    ``collect(slot, B)`` waits for batch i and returns its result dict."""
+    ``collect(slot, B)`` waits for batch i and returns its result dict.  A consumer that stops early (an exception, a
+    closed generator) leaves no batch submitted: the rest are collected and dropped."""
     m = layer.keras_model
     starts = list(range(0, len(imgs), batch_size))
     keep = {}
@@ -691,11 +758,19 @@ def _pipelined_batches(layer, imgs, batch_size, submit_fn, collect):
         m.handle.call(submit_fn, m.model_id, ptr(batch), batch.shape[0], k % 2)
         return batch.shape[0]
 
-    sizes = {0: submit(0)}
-    for k in range(len(starts)):
-        if k + 1 < len(starts):
-            sizes[k + 1] = submit(k + 1)
-        yield collect(k % 2, sizes.pop(k))
+    sizes = {}
+    try:
+        sizes[0] = submit(0)
+        for k in range(len(starts)):
+            if k + 1 < len(starts):
+                sizes[k + 1] = submit(k + 1)
+            yield collect(k % 2, sizes.pop(k))
+    finally:
+        for k in sorted(sizes):
+            try:
+                collect(k % 2, sizes[k])
+            except _lib.SleapB200Error:
+                pass                                  # already failed: the error that stopped the loop is the one to see
 
 
 class BottomUpInferenceModel(InferenceModel):
@@ -1017,28 +1092,60 @@ class TopDownMultiClassInferenceModel(InferenceModel):
                 cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and fp.optimal_grouping and fp.input_scale == 1.0
                 and fp.keras_model.input_scale == 1.0 and cc.keras_model.handle is fp.keras_model.handle)
 
+    def _configure_fused(self, B, H, W, C):
+        """The fused pipeline for batches of up to B frames of (H, W, C).  Returns (K, n_classes)."""
+        cc, fp = self.centroid_crop, self.instance_peaks
+        td, K = _topdown_params(cc, fp)
+        p = topdown_multiclass_params(td, fp.keras_model.cm.vector_taps[fp.CLASS_VECTORS], fp.class_head, fp.dense)
+        _configure_topdown(cc, fp, "sb_topdown_multiclass_configure", p, (B, H, W, C), fp.dense)
+        return K, p.n_classes
+
     def _call_fused(self, imgs):
         """sb_infer_topdown_multiclass: frames up once, one record per frame back (include/sleap_b200.h)."""
-        cc, fp = self.centroid_crop, self.instance_peaks
-        imgs = cc._prep(imgs)
+        imgs = self.centroid_crop._prep(imgs)
         B, H, W, C = imgs.shape
-        mc, mi = cc.keras_model, fp.keras_model
-        td, K = _topdown_params(cc, fp)
-        p = topdown_multiclass_params(td, mi.cm.vector_taps[fp.CLASS_VECTORS], fp.class_head, fp.dense)
-        _configure_topdown(cc, fp, "sb_topdown_multiclass_configure", p, (B, H, W, C), fp.dense)
-        NC, N = p.n_classes, head_channels(mi, fp.HEAD)
+        K, NC = self._configure_fused(B, H, W, C)
+        return self._run_fused(B, K, NC, "sb_infer_topdown_multiclass", ptr(imgs), int(imgs.dtype == np.uint8))
+
+    def _run_fused(self, B, K, NC, fn, *args):
+        """One fused call ``fn(model id, *args, <outputs>)`` into dense arrays of B frames, as a batch dict."""
+        fp, mc = self.instance_peaks, self.centroid_crop.keras_model
+        N = head_channels(fp.keras_model, fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         pts = np.zeros((B, NC, N, 2), np.float32); vals = np.zeros((B, NC, N), np.float32); probs = np.zeros((B, NC), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
         cvec = np.zeros((B, K, NC), np.float32) if fp.return_class_vectors else None
-        mc.handle.call("sb_infer_topdown_multiclass", mc.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(ce), ptr(cv), ptr(pts),
-                       ptr(vals), ptr(probs), ptr(nv), ptr(fl), ptr(cvec))
+        mc.handle.call(fn, mc.model_id, *args, B, ptr(ce), ptr(cv), ptr(pts), ptr(vals), ptr(probs), ptr(nv), ptr(fl), ptr(cvec))
         n = int(nv.max()) if B else 0
         out = {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "centroids": ce[:, :n].copy(),
                "centroid_vals": cv[:, :n].copy(), "flags": fl}
         if cvec is not None:
             out["class_vectors"] = np.concatenate([cvec[b, :nv[b]] for b in range(B)])
         return out
+
+    def predict_batches(self, data, batch_size: int = 4):
+        """Generator over per-batch result dicts, double-buffered as TopDownInferenceModel.predict_batches
+        (sb_topdown_multiclass_submit / _collect)."""
+        imgs = _images_of(data)
+        n = len(imgs)
+        if n == 0:
+            return
+        cc = self.centroid_crop
+        first = cc._prep(np.asarray(imgs[0:min(n, batch_size)])) if self._can_fuse() else None
+        if first is None or first.dtype != np.uint8:
+            for i in range(0, n, batch_size):        # generic (synchronous) path
+                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
+            return
+        K, NC = self._configure_fused(batch_size, *first.shape[1:])
+
+        def collect(slot, B):
+            return self._run_fused(B, K, NC, "sb_topdown_multiclass_collect", slot)
+
+        yield from _pipelined_batches(cc, imgs, batch_size, "sb_topdown_multiclass_submit", collect)
+
+    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
+        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
+        return _merge_batches(list(self.predict_batches(data, batch_size)))
 
     def call(self, example):
         if isinstance(example, np.ndarray):
@@ -1320,9 +1427,12 @@ class Predictor:
     def predict(self, data, make_labels: bool = True):
         """:496-531."""
         gen = self._with_progress(self._predict_generator(data), self._n_total(data))
-        if make_labels:
-            return self._make_labeled_frames_from_generator(gen, data)
-        return list(gen)
+        try:
+            if make_labels:
+                return self._make_labeled_frames_from_generator(gen, data)
+            return list(gen)
+        finally:
+            gen.close()           # a streamed batch loop stopped by an error collects what it submitted before this returns
 
     def skeleton(self):
         """Skeleton of the loaded model(s): node names (+ edges for bottom-up models), as the reference takes them

@@ -2,7 +2,8 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_track] [--steps K]
+  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_track] [pipeline]
+                               [--steps K]
                                [--c5-batch B]
   (C5 default: 16 frames per GPU and step)
 
@@ -42,6 +43,13 @@ about 5 animals per frame; no tracker, the host simple tracker, the device simpl
 (sb_topdown_attach_tracker) and the device simple tracker on the per-frame route (fused = False).  The line reports
 frames/s and instances per frame per arm, and whether the device tracks equal the host's, with numpy's greedy ties and
 with the device's stable ones.
+
+pipeline: the per-batch loop (predict_on_batch) against the double-buffered loop (predict_batches: submit / collect) of
+the same inference model, alternating in one process on the same 128 pinned gray tracking-clip frames (1024x1024), B=16,
+outputs compared batch by batch, bit for bit.  Workloads: a single-instance UNet as single() builds it (13 nodes); the C3
+top-down pair of topdown_track (about 5 animals per frame) without a tracker and with the device simple tracker; the C3
+identity pair of topdown_multiclass.  The line reports per workload the median frames/s of each loop over the
+repetitions, their spread, and the agreement.
 """
 import json
 import os
@@ -518,6 +526,101 @@ def topdown_track_bench(steps):
             "routes_agree": names(outs["simple device, fused step"]) == names(outs["simple device, per-frame route (fused = False)"])}
 
 
+def pipeline_bench(steps):
+    """predict_on_batch per batch against predict_batches on the same frames, alternating (see the module docstring)."""
+    import torch
+    from scipy.ndimage import maximum_filter
+    from sleap_b200.nn import tracking as T
+    from sleap_b200.nn.inference import TopDownMultiClassPredictor
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from flow_clip import clip_frames
+    n, B = 128, 16
+    gray = torch.from_numpy(np.ascontiguousarray(clip_frames(n)[:, :, :, :1])).pin_memory().numpy()
+    cspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="centroid", part_names=None, edges=None,
+                 heads=[dict(name="CentroidConfmapsHead", channels=1, output_stride=2)])
+    ihead = dict(name="CenteredInstanceConfmapsHead", channels=13, output_stride=4)
+    ispec = dict(backbone="unet", backbone_cfg=dict(unet(24, 16, 4), up_interpolate=False), head_type="centered_instance",
+                 part_names=FLIES13, edges=None, heads=[ihead])
+    classes = ["c0", "c1", "c2", "c3"]
+    mspec = dict(ispec, head_type="multi_class_topdown", classes=classes,
+                 heads=[ihead, dict(name="ClassVectorsHead", channels=len(classes), output_stride=16, vector=True, num_fc_layers=3,
+                                    num_fc_units=64, global_pool=True)])
+    sspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="single_instance", part_names=FLIES13, edges=None,
+                 heads=[dict(name="SingleInstanceConfmapsHead", channels=13, output_stride=2)])
+
+    def centroid_model():
+        m = model_for(cspec, 1, 1003, input_scale=0.5)[0]
+        cms = np.concatenate([m.forward(gray[i:i + B])[0][..., 0] for i in range(0, 4 * B, B)])
+        fifth = [np.sort(c[c == maximum_filter(c, size=3, mode="constant", cval=-np.inf)])[-5] for c in cms]
+        return m, float(np.median(fifth))
+
+    def topdown_model():
+        cm, thr = centroid_model()
+        pred = TopDownPredictor(cm, model_for(ispec, 1, 1004)[0], crop_size=160, peak_threshold=thr, integral_refinement=True,
+                                batch_size=B, max_instances=5)
+        pred.inference_model.instance_peaks.peak_threshold = 0.0
+        return pred.inference_model
+
+    def identity_model():
+        cm, thr = centroid_model()
+        icm = A.compile_model(mspec, 1)
+        iw = A.make_synthetic_weights(icm, 1004)
+        rng = np.random.default_rng(1005)
+        dims = [icm.vector_taps["ClassVectorsHead"]["C"], 64, 64, 64, len(classes)]
+        for i in range(4):
+            iw["ClassVectorsHead" if i == 3 else f"pre_classification{i}_fc"] = dict(
+                kernel=(rng.normal(0, 1, dims[i:i + 2]) * np.sqrt(2.0 / dims[i])).astype(np.float32),
+                bias=rng.normal(0, 0.1, dims[i + 1]).astype(np.float32))
+        pred = TopDownMultiClassPredictor(cm, DeviceModel(mspec, iw, input_channels=1, precision=0), crop_size=160, peak_threshold=thr,
+                                          integral_refinement=True, batch_size=B, max_instances=5)
+        pred.inference_model.instance_peaks.peak_threshold = 0.0
+        return pred.inference_model
+
+    single_im = SingleInstancePredictor(model_for(sspec, 1, 1001)[0], peak_threshold=0.2, integral_refinement=True,
+                                        batch_size=B).inference_model
+    td_im, td_trk_im = topdown_model(), topdown_model()
+    simple = dict(tracker="simple", similarity="instance", match="greedy")
+    workloads = {"single-instance UNet 1024x1024x1, 13 nodes": (single_im, None),
+                 "C3 top-down pair, max 5 animals": (td_im, None),
+                 "C3 top-down pair, max 5 animals, device simple tracker": (td_trk_im, simple),
+                 "C3 identity pair (4 classes, 3 x 64 fc units), max 5 animals": (identity_model(), None)}
+
+    def arm(im, trk, streamed):
+        im.tracker = T.Tracker.make_tracker_by_name(track_device=0, **trk) if trk else None   # a fresh tracker per run
+        try:
+            if streamed:
+                return list(im.predict_batches(gray, B))
+            return [im.predict_on_batch(gray[i:i + B]) for i in range(0, n, B)]
+        finally:
+            if trk:
+                im.detach_tracker()
+                im.tracker = None
+
+    def same(a, b):
+        return len(a) == len(b) and all(sorted(x) == sorted(y) and all(np.asarray(x[k]).tobytes() == np.asarray(y[k]).tobytes() for k in x)
+                                        for x, y in zip(a, b))
+
+    reps = max(10, steps)
+    res = {}
+    for name, (im, trk) in workloads.items():
+        outs = {s: arm(im, trk, s) for s in (False, True)}                # warm-up, and the outputs compared
+        times = {False: [], True: []}
+        for _ in range(reps):                                            # the two loops alternate
+            for s in (False, True):
+                t0 = time.perf_counter()
+                arm(im, trk, s)
+                times[s].append(time.perf_counter() - t0)
+        res[name] = {"per_batch_frames_per_s": n / float(np.median(times[False])),
+                     "streamed_frames_per_s": n / float(np.median(times[True])),
+                     "per_batch_spread": [n / max(times[False]), n / min(times[False])],
+                     "streamed_spread": [n / max(times[True]), n / min(times[True])],
+                     "speedup": float(np.median(times[False]) / np.median(times[True])),
+                     "outputs_equal": same(outs[False], outs[True])}
+    return {"config": "pipeline: predict_on_batch per batch vs predict_batches, 128 pinned gray clip frames 1024x1024, B=16",
+            "gpu": gpu_identity(), "metric": "frames/s (median of alternating repetitions; host frames in, result dicts out)",
+            "repetitions": reps, "post_overlap": not os.environ.get("SB_DISABLE_POST_OVERLAP"), "workloads": res}
+
+
 if __name__ == "__main__":
     which = [a for a in sys.argv[1:] if not a.startswith("--")] or ["c1", "c2", "c3", "c5"]
     steps = int(sys.argv[sys.argv.index("--steps") + 1]) if "--steps" in sys.argv else 10
@@ -538,6 +641,8 @@ if __name__ == "__main__":
             r = topdown_multiclass_bench(steps)
         elif c == "topdown_track":
             r = topdown_track_bench(steps)
+        elif c == "pipeline":
+            r = pipeline_bench(steps)
         else:
             b5 = int(sys.argv[sys.argv.index("--c5-batch") + 1]) if "--c5-batch" in sys.argv else 16
             r = hourglass(max(3, steps // 3), b5)
