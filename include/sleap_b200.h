@@ -197,8 +197,8 @@ typedef struct sb_bottomup_params {
 int sb_bottomup_configure(sb_handle_t h, int model_id, const sb_bottomup_params* params);
 
 /* frames: (B,H,W,C_in) uint8.  *_host variant copies H2D / D2H inside; *_dev takes frames
- * already resident in HBM and leaves results on the device (pointers returned through
- * sb_bottomup_device_outputs).  Outputs: instance_peaks (B,max_instances,n_nodes,2),
+ * already resident in HBM and leaves results on the device (the records of
+ * sb_bottomup_device_records).  Outputs: instance_peaks (B,max_instances,n_nodes,2),
  * instance_peak_vals (B,max_instances,n_nodes), instance_scores (B,max_instances),
  * n_valid (B), flags (B). */
 int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B,
@@ -217,13 +217,8 @@ int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out
 
 /* sb_infer_bottomup_dev returns as soon as the work is queued: the network runs on the handle's
  * stream and the post-processing on a second stream, so that it overlaps the network of the next
- * call.  sb_bottomup_wait_results makes the handle's stream wait (device side) for the results of
- * the last call; sb_get_post_stream exposes the post-processing stream; sb_synchronize joins both. */
-int sb_bottomup_wait_results(sb_handle_t h, int model_id);
+ * call.  sb_get_post_stream exposes the post-processing stream; sb_synchronize joins both. */
 int sb_get_post_stream(sb_handle_t h, void** out_stream);
-int sb_bottomup_device_outputs(sb_handle_t h, int model_id, float** instance_peaks_dev,
-                               float** instance_peak_vals_dev, float** instance_scores_dev,
-                               int32_t** n_valid_dev, int32_t** flags_dev);
 /* Device pointer of the contiguous per-frame result records the grouping kernel writes ([max_batch][width] float32,
  * width = ceil4(max_instances*n_nodes*3 + max_instances + 2): peaks | peak values | instance scores | n_valid | flags). */
 int sb_bottomup_device_records(sb_handle_t h, int model_id, float** records_dev);
@@ -547,13 +542,12 @@ int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tr
  * stops the batch's tracking there: its record and every later one carry flag SB_TRACK_OVER_CAPACITY, which stays set
  * until sb_tracker_reset (as a full queue table does).  The pipeline must be a plain one (sb_topdown_configure), and the
  * tracker must live on its handle and have its instance model's node count; img_h, img_w > 0.  The attachment lives
- * with the pipeline: a configure call on either model drops it.  sb_topdown_tracks copies the track records of the last
- * sb_infer_topdown (the bottom-up format above); sb_infer_topdown's outputs do not change.  Streamed batches are tracked
- * in submit order; sb_topdown_slot_tracks copies the track records of the batch last collected from slot 0 / 1 (B must
- * be that batch's frame count). */
+ * with the pipeline: a configure call on either model drops it.  sb_infer_topdown's outputs do not change.  Streamed
+ * batches are tracked in submit order.  sb_topdown_tracks copies track records in the bottom-up format above, as
+ * sb_bottomup_tracks does: slot -1, those of the last sb_infer_topdown; slot 0 / 1, those of the batch last collected
+ * from that slot (B must be that batch's frame count). */
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w);
-int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_tracks);
-int sb_topdown_slot_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks);
+int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks);
 
 #ifdef __cplusplus
 }

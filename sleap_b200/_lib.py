@@ -130,10 +130,7 @@ _SIGS = {
     "sb_infer_bottomup_dev": [c_void_p, c_int, c_void_p, c_int],
     "sb_bottomup_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
     "sb_bottomup_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sb_bottomup_wait_results": [c_void_p, c_int],
     "sb_get_post_stream": [c_void_p, POINTER(c_void_p)],
-    "sb_bottomup_device_outputs": [c_void_p, c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
-                                   POINTER(c_void_p), POINTER(c_void_p)],
     "sb_bottomup_device_records": [c_void_p, c_int, POINTER(c_void_p)],
     "sb_bottomup_fetch_graph": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                 c_void_p, c_void_p, c_void_p, c_void_p],
@@ -187,8 +184,7 @@ _SIGS = {
     "sb_bottomup_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
     "sb_bottomup_device_tracks": [c_void_p, c_int, c_int, c_void_p],
     "sb_topdown_attach_tracker": [c_void_p, c_int, c_int, ctypes.c_double, ctypes.c_double],
-    "sb_topdown_tracks": [c_void_p, c_int, c_int, c_void_p],
-    "sb_topdown_slot_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
+    "sb_topdown_tracks": [c_void_p, c_int, c_int, c_int, c_void_p],
     "sb_tracker_destroy": [c_void_p, c_int],
     "sb_track_instances": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int32), POINTER(c_int32)],

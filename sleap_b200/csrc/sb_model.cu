@@ -915,15 +915,6 @@ int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, in
   return SB_OK;
 }
 
-// Makes the handle's main stream wait (on the device, no host sync) for the post-processing of the
-// last sb_infer_bottomup_dev call, e.g. before recording an end-of-work event or reading the results.
-int sb_bottomup_wait_results(sb_handle_t h, int model_id) {
-  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
-  if (!m) return SB_ERR_INVALID;
-  if (h->post_pending) SB_CUDA(h, cudaStreamWaitEvent(h->stream, h->post_done_ev, 0));
-  return SB_OK;
-}
-
 // The stream post-processing runs on (consumers such as the NCCL gather can be queued behind it).
 int sb_get_post_stream(sb_handle_t h, void** out_stream) {
   if (!h || !out_stream) return sb_fail(h, SB_ERR_INVALID, "null argument");
@@ -1004,18 +995,6 @@ int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* ou
   memcpy(out_records, src, (size_t)m->gather.world * B * sb_record_width(m->bu.max_instances, m->bu.n_nodes) * sizeof(float));
   if (out_counts)
     for (int r = 0; r < m->gather.world; ++r) out_counts[r] = m->gather.counts_host[(slot < 0 ? 3 : 1 + slot) * SB_GATHER_MAX_WORLD + r];
-  return SB_OK;
-}
-
-int sb_bottomup_device_outputs(sb_handle_t h, int model_id, float** instance_peaks_dev, float** instance_peak_vals_dev,
-                               float** instance_scores_dev, int32_t** n_valid_dev, int32_t** flags_dev) {
-  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
-  if (!m) return SB_ERR_INVALID;
-  if (instance_peaks_dev) *instance_peaks_dev = m->ws.inst_peaks;
-  if (instance_peak_vals_dev) *instance_peak_vals_dev = m->ws.inst_vals;
-  if (instance_scores_dev) *instance_scores_dev = m->ws.inst_scores;
-  if (n_valid_dev) *n_valid_dev = m->ws.n_inst;
-  if (flags_dev) *flags_dev = m->ws.flags;
   return SB_OK;
 }
 

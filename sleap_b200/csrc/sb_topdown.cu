@@ -705,26 +705,20 @@ int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_
   return SB_OK;
 }
 
-int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int B, double* out_tracks) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+// slot -1: the records of the last sb_infer_topdown; slot 0 / 1: those of the batch last collected from that slot.
+int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, slot >= 0);
   if (!t) return SB_ERR_INVALID;
   const SbModel* mc = h->models[centroid_model_id];
   if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
-  if (B <= 0 || B > t->Bmax || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad batch");
-  memcpy(out_tracks, mc->trk_host[2], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
-  return SB_OK;
-}
-
-int sb_topdown_slot_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
-  if (!t) return SB_ERR_INVALID;
-  const SbModel* mc = h->models[centroid_model_id];
-  if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: no tracker attached");
-  if (slot < 0 || slot > 1 || B <= 0 || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: bad slot / batch");
-  if (t->done_B[slot] != B)
-    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_slot_tracks: slot %d holds no collected batch of %d frames", slot, B);
-  SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
-  memcpy(out_tracks, mc->trk_host[slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
+  if (slot < -1 || slot > 1 || B <= 0 || B > t->Bmax || !out_tracks)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad slot / batch");
+  if (slot >= 0) {
+    if (t->done_B[slot] != B)
+      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: slot %d holds no collected batch of %d frames", slot, B);
+    SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
+  }
+  memcpy(out_tracks, mc->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
   return SB_OK;
 }
 

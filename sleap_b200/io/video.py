@@ -203,7 +203,7 @@ class FrameFeeder:
     ``hold`` batches past it, so the last ``hold`` batches returned stay valid (the double-buffered
     device pipeline still reads batch k while it asks for k + 1).
 
-    Sequence protocol (what ``BottomUpInferenceModel.predict_batches`` needs): ``len(feeder)`` frames,
+    Sequence protocol (what ``InferenceModel.predict_batches`` needs): ``len(feeder)`` frames,
     ``feeder[a:b]`` for consecutive batch-aligned slices.  ``for inds, batch in feeder.batches()`` is
     the generator form.
     """

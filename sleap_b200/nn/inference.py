@@ -8,6 +8,7 @@ Kept surface (same names / attributes / dict contract, NumPy in and out):
   BottomUpPredictor (:3055-3349), load_model (:4865).
 All tensor work runs on the GPU through libsleapb200 (C-ABI); this file is orchestration only.
 """
+import contextlib
 import ctypes
 import json
 import os
@@ -65,9 +66,28 @@ class InferenceModel:
 
     def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
         """:989-1045: iterate batches and concatenate (NaN-padding to the widest batch)."""
-        imgs = np.asarray(_images_of(data))
-        chunks = [self.predict_on_batch(imgs[i:i + batch_size]) for i in range(0, len(imgs), batch_size)]
-        return _merge_batches(chunks)
+        return _merge_batches(list(self.predict_batches(data, batch_size)))
+
+    def predict_batches(self, data, batch_size: int = 4):
+        """Generator over per-batch result dicts (the Predictor batch loop, :377-420).  When the model's device step
+        takes these frames (``_stream``), the loop is double-buffered: the upload of batch i+1 overlaps the compute of
+        batch i.  Otherwise one predict_on_batch per batch."""
+        imgs = _images_of(data)
+        n = len(imgs)
+        if n == 0:
+            return
+        stream = self._stream(InferenceLayer._prep(np.asarray(imgs[0:min(n, batch_size)])), batch_size)
+        if stream is None:
+            for i in range(0, n, batch_size):
+                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
+            return
+        yield from _pipelined_batches(imgs, batch_size, *stream)
+
+    def _stream(self, first, batch_size):
+        """The streamed step for batches of up to ``batch_size`` frames like ``first`` (the first batch, prepped), set
+        up for them: (device model, submit call, ``collect(slot, B)`` returning the batch dict), or None for the
+        per-batch route."""
+        return None
 
 
 def _merge_batches(chunks):
@@ -137,6 +157,16 @@ def _track_fields(rec):
             "tracking_scores": rec[:, 2 + 2 * I:].copy()}
 
 
+def _step_tracks(m, fn, tracker, slot, B):
+    """The track fields of the B frames a step of model ``m`` returned, read with ``fn`` (sb_bottomup_tracks or
+    sb_topdown_tracks) from slot 0 / 1 or, with -1, from the synchronous call; none without ``tracker``."""
+    if tracker is None:
+        return {}
+    rec = np.zeros((B, 2 + 3 * tracker._device.max_instances), np.float64)
+    m.handle.call(fn, m.model_id, slot, B, ptr(rec))
+    return _track_fields(rec)
+
+
 def _find_head(model: DeviceModel, name: str):
     if name not in model.cm.head_buffers:
         return None
@@ -180,16 +210,21 @@ class SingleInstanceInferenceLayer(InferenceLayer):
         imgs = self._prep(_images_of(data))
         B, H, W, C = imgs.shape
         self._configure(B, H, W, C)
+        co = None if crop_offsets is None else f32(crop_offsets).reshape(B, 2)
+        out = self._run_step(B, "sb_infer_global", ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(co))
+        if self.return_confmaps:
+            out["confmaps"] = self.keras_model.forward(imgs, [self.HEAD])[0]
+        return out
+
+    def _run_step(self, B, fn, *args):
+        """One call ``fn(model id, *args, <outputs>)`` (sb_infer_global or sb_global_collect) into B frames' peaks, as a
+        batch dict.  ``args`` run up to the outputs, B included: sb_infer_global takes the crop offsets after B."""
         m = self.keras_model
         n_nodes = head_channels(m, self.HEAD)
         pts = np.zeros((B, n_nodes, 2), np.float32)
         vals = np.zeros((B, n_nodes), np.float32)
-        co = None if crop_offsets is None else f32(crop_offsets).reshape(B, 2)
-        m.handle.call("sb_infer_global", m.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(co), ptr(pts), ptr(vals))
-        out = {"instance_peaks": pts[:, None], "instance_peak_vals": vals[:, None]}
-        if self.return_confmaps:
-            out["confmaps"] = m.forward(imgs, [self.HEAD])[0]
-        return out
+        m.handle.call(fn, m.model_id, *args, ptr(pts), ptr(vals))
+        return {"instance_peaks": pts[:, None], "instance_peak_vals": vals[:, None]}
 
 
 class SingleInstanceInferenceModel(InferenceModel):
@@ -201,36 +236,13 @@ class SingleInstanceInferenceModel(InferenceModel):
     def call(self, example):
         return self.single_instance_layer.call(example)
 
-    def predict_batches(self, data, batch_size: int = 4):
-        """Generator over per-batch result dicts, double-buffered as BottomUpInferenceModel.predict_batches
-        (sb_global_submit / sb_global_collect): the upload of batch i+1 overlaps the compute of batch i (uint8 frames
-        without return_confmaps; otherwise one predict_on_batch per batch)."""
+    def _stream(self, first, batch_size):
+        """sb_global_submit / sb_global_collect: uint8 frames without return_confmaps."""
         layer = self.single_instance_layer
-        imgs = _images_of(data)
-        n = len(imgs)
-        if n == 0:
-            return
-        first = layer._prep(np.asarray(imgs[0:min(n, batch_size)]))
         if first.dtype != np.uint8 or layer.return_confmaps:
-            for i in range(0, n, batch_size):        # generic (synchronous) path
-                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
-            return
-        _, H, W, C = first.shape
-        layer._configure(batch_size, H, W, C)
-        m = layer.keras_model
-        n_nodes = head_channels(m, layer.HEAD)
-
-        def collect(slot, B):
-            pts = np.zeros((B, n_nodes, 2), np.float32)
-            vals = np.zeros((B, n_nodes), np.float32)
-            m.handle.call("sb_global_collect", m.model_id, slot, B, ptr(pts), ptr(vals))
-            return {"instance_peaks": pts[:, None], "instance_peak_vals": vals[:, None]}
-
-        yield from _pipelined_batches(layer, imgs, batch_size, "sb_global_submit", collect)
-
-    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
-        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
-        return _merge_batches(list(self.predict_batches(data, batch_size)))
+            return None
+        layer._configure(batch_size, *first.shape[1:])
+        return layer.keras_model, "sb_global_submit", lambda slot, B: layer._run_step(B, "sb_global_collect", slot, B)
 
 
 # ------------------------------------------------------------------------------------------
@@ -501,9 +513,9 @@ class TopDownInferenceModel(InferenceModel):
             mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
         return K
 
-    def _run_fused(self, B, K, fn, *args, tracks=("sb_topdown_tracks",)):
-        """One fused call ``fn(model id, *args, <outputs>)`` into dense arrays of B frames, as a batch dict; the track
-        records through ``tracks`` (call name and leading arguments after the model id)."""
+    def _run_fused(self, B, K, fn, *args, slot=-1):
+        """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown or sb_topdown_collect) into dense arrays
+        of B frames, as a batch dict; with a tracker, the track records of ``slot`` (-1: sb_infer_topdown)."""
         mc, n_nodes = self.centroid_crop.keras_model, head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
@@ -512,10 +524,7 @@ class TopDownInferenceModel(InferenceModel):
         n = int(nv.max()) if B else 0
         out = {"centroids": ce[:, :n].copy(), "centroid_vals": cv[:, :n].copy(), "instance_peaks": ip[:, :n].copy(),
                "instance_peak_vals": iv[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
-        if self.tracker is not None:
-            rec = np.zeros((B, 2 + 3 * self.tracker._device.max_instances), np.float64)
-            mc.handle.call(tracks[0], mc.model_id, *tracks[1:], B, ptr(rec))
-            out.update(_track_fields(rec))
+        out.update(_step_tracks(mc, "sb_topdown_tracks", self.tracker, slot, B))
         return out
 
     def _call_fused(self, imgs):
@@ -526,30 +535,14 @@ class TopDownInferenceModel(InferenceModel):
         K = self._configure_fused(B, H, W, C)
         return self._run_fused(B, K, "sb_infer_topdown", ptr(imgs), int(imgs.dtype == np.uint8))
 
-    def predict_batches(self, data, batch_size: int = 4):
-        """Generator over per-batch result dicts, double-buffered (sb_topdown_submit / sb_topdown_collect): the upload
-        of batch i+1 and its centroid stage are queued before batch i is collected.  Frames that are not uint8, and a
-        model that cannot run the fused step, take one predict_on_batch per batch."""
-        imgs = _images_of(data)
-        n = len(imgs)
-        if n == 0:
-            return
-        cc = self.centroid_crop
-        first = cc._prep(np.asarray(imgs[0:min(n, batch_size)])) if self._can_fuse() else None
-        if first is None or first.dtype != np.uint8:
-            for i in range(0, n, batch_size):        # generic (synchronous) path
-                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
-            return
+    def _stream(self, first, batch_size):
+        """sb_topdown_submit / sb_topdown_collect (the upload of batch i+1 and its centroid stage are queued before batch
+        i is collected): uint8 frames and a model that can run the fused step."""
+        if not self._can_fuse() or first.dtype != np.uint8:
+            return None
         K = self._configure_fused(batch_size, *first.shape[1:])
-
-        def collect(slot, B):
-            return self._run_fused(B, K, "sb_topdown_collect", slot, tracks=("sb_topdown_slot_tracks", slot))
-
-        yield from _pipelined_batches(cc, imgs, batch_size, "sb_topdown_submit", collect)
-
-    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
-        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
-        return _merge_batches(list(self.predict_batches(data, batch_size)))
+        return (self.centroid_crop.keras_model, "sb_topdown_submit",
+                lambda slot, B: self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot))
 
     def call(self, example):
         if isinstance(example, np.ndarray):
@@ -627,14 +620,8 @@ class BottomUpInferenceLayer(InferenceLayer):
             m.handle.call("sb_bottomup_attach_tracker", m.model_id, -1, -1, 1.0, 1.0)
 
     def track_fields(self, slot, B):
-        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields
-        (``_track_fields``)."""
-        if self.tracker is None:
-            return {}
-        rec = np.zeros((B, 2 + 3 * self.tracker._device.max_instances), np.float64)
-        m = self.keras_model
-        m.handle.call("sb_bottomup_tracks", m.model_id, slot, B, ptr(rec))
-        return _track_fields(rec)
+        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields."""
+        return _step_tracks(self.keras_model, "sb_bottomup_tracks", self.tracker, slot, B)
 
     def params(self) -> BottomUpParams:
         """The chain's parameters; their edge arrays stay alive in ``self._keep``."""
@@ -645,28 +632,14 @@ class BottomUpInferenceLayer(InferenceLayer):
         return p
 
     def call(self, data):
-        raw = _images_of(data)
-        imgs = self._prep(raw)
+        imgs = self._prep(_images_of(data))
         if imgs.dtype != np.uint8:
             raise ValueError("BottomUpInferenceLayer expects uint8 frames (the fused path reads raw frames).")
         B, H, W, C = imgs.shape
         self._configure(B, H, W, C)
-        self.attach_tracker(np.asarray(raw[0]).shape[:2])
+        self.attach_tracker((H, W))
         m = self.keras_model
-        I, N = self.max_instances, self.paf_scorer.n_nodes
-        ip = np.zeros((B, I, N, 2), np.float32)
-        iv = np.zeros((B, I, N), np.float32)
-        isc = np.zeros((B, I), np.float32)
-        nv = np.zeros((B,), np.int32)
-        fl = np.zeros((B,), np.int32)
-        m.handle.call("sb_infer_bottomup", m.model_id, ptr(imgs), B, ptr(ip), ptr(iv), ptr(isc), ptr(nv), ptr(fl))
-        n = int(nv.max()) if B else 0
-        out = {"instance_peaks": ip[:, :n].copy(), "instance_peak_vals": iv[:, :n].copy(),
-               "instance_scores": isc[:, :n].copy(), "n_valid": nv.astype(np.int64), "flags": fl}
-        out.update(self.track_fields(-1, B))
-        pg = getattr(m, "peer_gather", None)
-        if pg is not None:          # multi-GPU: this call was one exchange step; the window came over with the result copy
-            out["gathered_records"], out["gathered_counts"] = pg.gathered(-1, B, I, N)
+        out = self._run_step(B, "sb_infer_bottomup", ptr(imgs))
         if self.return_confmaps or self.return_pafs:
             cms, pafs = m.forward(imgs, ["MultiInstanceConfmapsHead", "PartAffinityFieldsHead"])
             if self.return_confmaps:
@@ -675,6 +648,24 @@ class BottomUpInferenceLayer(InferenceLayer):
                 out["part_affinity_fields"] = pafs
         if self.return_paf_graph:
             out.update(self.fetch_graph(B))
+        return out
+
+    def _run_step(self, B, fn, *args, slot=-1):
+        """One call ``fn(model id, *args, B, <outputs>)`` (sb_infer_bottomup or sb_bottomup_collect) into B frames'
+        instances, as a batch dict; the track records and, with the multi-GPU exchange, every rank's records of this step
+        (they came over with the result copy) from ``slot`` (-1: sb_infer_bottomup)."""
+        m = self.keras_model
+        I, N = self.max_instances, self.paf_scorer.n_nodes
+        ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32)
+        isc = np.zeros((B, I), np.float32); nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
+        m.handle.call(fn, m.model_id, *args, B, ptr(ip), ptr(iv), ptr(isc), ptr(nv), ptr(fl))
+        n = int(nv.max()) if B else 0
+        out = {"instance_peaks": ip[:, :n], "instance_peak_vals": iv[:, :n], "instance_scores": isc[:, :n],
+               "n_valid": nv.astype(np.int64), "flags": fl}
+        out.update(self.track_fields(slot, B))
+        pg = getattr(m, "peer_gather", None)
+        if pg is not None:
+            out["gathered_records"], out["gathered_counts"] = pg.gathered(slot, B, I, N)
         return out
 
     def fetch_graph(self, B):
@@ -743,17 +734,16 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
     return out
 
 
-def _pipelined_batches(layer, imgs, batch_size, submit_fn, collect):
+def _pipelined_batches(imgs, batch_size, m, submit_fn, collect):
     """The double-buffered batch loop of the streaming models (uint8 frames, chain configured): batch i+1 is submitted
-    (``submit_fn``: its upload on the copy stream, network and post-processing queued) into slot (i+1) % 2 before
-    ``collect(slot, B)`` waits for batch i and returns its result dict.  A consumer that stops early (an exception, a
-    closed generator) leaves no batch submitted: the rest are collected and dropped."""
-    m = layer.keras_model
+    (``submit_fn`` of device model ``m``: its upload on the copy stream, network and post-processing queued) into slot
+    (i+1) % 2 before ``collect(slot, B)`` waits for batch i and returns its result dict.  A consumer that stops early (an
+    exception, a closed generator) leaves no batch submitted: the rest are collected and dropped."""
     starts = list(range(0, len(imgs), batch_size))
     keep = {}
 
     def submit(k):
-        batch = layer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
+        batch = InferenceLayer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
         keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
         m.handle.call(submit_fn, m.model_id, ptr(batch), batch.shape[0], k % 2)
         return batch.shape[0]
@@ -782,43 +772,16 @@ class BottomUpInferenceModel(InferenceModel):
     def call(self, example):
         return self.bottomup_layer.call(example)
 
-    def predict_batches(self, data, batch_size: int = 4):
-        """Generator over per-batch result dicts for a stack of uint8 frames (the Predictor batch loop,
-        inference.py:377-420), double-buffered: the upload of batch i+1 overlaps the compute of batch i."""
+    def _stream(self, first, batch_size):
+        """sb_bottomup_submit / sb_bottomup_collect: uint8 frames without return_confmaps, return_pafs or
+        return_paf_graph."""
         layer = self.bottomup_layer
-        imgs = _images_of(data)
-        n = len(imgs)
-        if n == 0:
-            return
-        first = layer._prep(np.asarray(imgs[0:min(n, batch_size)]))
         if first.dtype != np.uint8 or layer.return_confmaps or layer.return_pafs or layer.return_paf_graph:
-            for i in range(0, n, batch_size):        # generic (synchronous) path
-                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
-            return
-        _, H, W, C = first.shape
-        layer._configure(batch_size, H, W, C)
-        layer.attach_tracker(np.asarray(imgs[0]).shape[:2])
-        m = layer.keras_model
-        I, N = layer.max_instances, layer.paf_scorer.n_nodes
-
-        def collect(slot, B):
-            ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32)
-            isc = np.zeros((B, I), np.float32); nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
-            m.handle.call("sb_bottomup_collect", m.model_id, slot, B, ptr(ip), ptr(iv), ptr(isc), ptr(nv), ptr(fl))
-            w = int(nv.max()) if B else 0
-            out = {"instance_peaks": ip[:, :w], "instance_peak_vals": iv[:, :w], "instance_scores": isc[:, :w],
-                   "n_valid": nv.astype(np.int64), "flags": fl}
-            out.update(layer.track_fields(slot, B))
-            pg = getattr(m, "peer_gather", None)
-            if pg is not None:      # multi-GPU: every rank's records of this step came over with the result copy (sb_gather_*)
-                out["gathered_records"], out["gathered_counts"] = pg.gathered(slot, B, I, N)
-            return out
-
-        yield from _pipelined_batches(layer, imgs, batch_size, "sb_bottomup_submit", collect)
-
-    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
-        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
-        return _merge_batches(list(self.predict_batches(data, batch_size)))
+            return None
+        layer._configure(batch_size, *first.shape[1:])
+        layer.attach_tracker(first.shape[1:3])
+        return (layer.keras_model, "sb_bottomup_submit",
+                lambda slot, B: layer._run_step(B, "sb_bottomup_collect", slot, slot=slot))
 
 
 # ------------------------------------------------------------------------------------------
@@ -864,19 +827,23 @@ class BottomUpMultiClassInferenceLayer(InferenceLayer):
         return (np.zeros((B, K, N, 2), np.float32), np.zeros((B, K, N), np.float32), np.zeros((B, K, N), np.float32),
                 np.zeros((B,), np.int32))
 
+    def _run_step(self, B, fn, *args):
+        """One call ``fn(model id, *args, B, <outputs>)`` (sb_infer_multiclass or sb_multiclass_collect) into B frames'
+        instances, one per class, as a batch dict."""
+        m = self.keras_model
+        pts, vals, probs, fl = self._outputs(B)
+        m.handle.call(fn, m.model_id, *args, B, ptr(pts), ptr(vals), ptr(probs), ptr(fl))
+        return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+
     def call(self, data):
         """:3530-3589."""
         from sleap_b200.nn import identity
         imgs = self._prep(_images_of(data))
         B, H, W, C = imgs.shape
         self._configure(B, H, W, C)
-        m = self.keras_model
-        pts, vals, probs, fl = self._outputs(B)
-        m.handle.call("sb_infer_multiclass", m.model_id, ptr(imgs), int(imgs.dtype == np.uint8), B, ptr(pts), ptr(vals),
-                      ptr(probs), ptr(fl))
-        out = {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
+        out = self._run_step(B, "sb_infer_multiclass", ptr(imgs), int(imgs.dtype == np.uint8))
         if self.return_confmaps or self.return_class_maps:
-            cms, logits = m.forward(imgs, [self.CMS, self.CLASS_MAPS])
+            cms, logits = self.keras_model.forward(imgs, [self.CMS, self.CLASS_MAPS])
             if self.return_confmaps:
                 out["confmaps"] = cms
             if self.return_class_maps:
@@ -921,33 +888,13 @@ class BottomUpMultiClassInferenceModel(InferenceModel):
     def call(self, example):
         return self.inference_layer.call(example)
 
-    def predict_batches(self, data, batch_size: int = 4):
-        """Generator over per-batch result dicts, double-buffered as BottomUpInferenceModel.predict_batches: the upload
-        of batch i+1 overlaps the compute of batch i (uint8 frames; otherwise one predict_on_batch per batch)."""
+    def _stream(self, first, batch_size):
+        """sb_multiclass_submit / sb_multiclass_collect: uint8 frames without return_confmaps or return_class_maps."""
         layer = self.inference_layer
-        imgs = _images_of(data)
-        n = len(imgs)
-        if n == 0:
-            return
-        first = layer._prep(np.asarray(imgs[0:min(n, batch_size)]))
         if first.dtype != np.uint8 or layer.return_confmaps or layer.return_class_maps:
-            for i in range(0, n, batch_size):        # generic (synchronous) path
-                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
-            return
-        _, H, W, C = first.shape
-        layer._configure(batch_size, H, W, C)
-        m = layer.keras_model
-
-        def collect(slot, B):
-            pts, vals, probs, fl = layer._outputs(B)
-            m.handle.call("sb_multiclass_collect", m.model_id, slot, B, ptr(pts), ptr(vals), ptr(probs), ptr(fl))
-            return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "flags": fl}
-
-        yield from _pipelined_batches(layer, imgs, batch_size, "sb_multiclass_submit", collect)
-
-    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
-        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
-        return _merge_batches(list(self.predict_batches(data, batch_size)))
+            return None
+        layer._configure(batch_size, *first.shape[1:])
+        return layer.keras_model, "sb_multiclass_submit", lambda slot, B: layer._run_step(B, "sb_multiclass_collect", slot)
 
 
 class TopDownMultiClassFindPeaks(InferenceLayer):
@@ -1108,7 +1055,8 @@ class TopDownMultiClassInferenceModel(InferenceModel):
         return self._run_fused(B, K, NC, "sb_infer_topdown_multiclass", ptr(imgs), int(imgs.dtype == np.uint8))
 
     def _run_fused(self, B, K, NC, fn, *args):
-        """One fused call ``fn(model id, *args, <outputs>)`` into dense arrays of B frames, as a batch dict."""
+        """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown_multiclass or
+        sb_topdown_multiclass_collect) into dense arrays of B frames, as a batch dict."""
         fp, mc = self.instance_peaks, self.centroid_crop.keras_model
         N = head_channels(fp.keras_model, fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
@@ -1123,29 +1071,14 @@ class TopDownMultiClassInferenceModel(InferenceModel):
             out["class_vectors"] = np.concatenate([cvec[b, :nv[b]] for b in range(B)])
         return out
 
-    def predict_batches(self, data, batch_size: int = 4):
-        """Generator over per-batch result dicts, double-buffered as TopDownInferenceModel.predict_batches
-        (sb_topdown_multiclass_submit / _collect)."""
-        imgs = _images_of(data)
-        n = len(imgs)
-        if n == 0:
-            return
-        cc = self.centroid_crop
-        first = cc._prep(np.asarray(imgs[0:min(n, batch_size)])) if self._can_fuse() else None
-        if first is None or first.dtype != np.uint8:
-            for i in range(0, n, batch_size):        # generic (synchronous) path
-                yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
-            return
+    def _stream(self, first, batch_size):
+        """sb_topdown_multiclass_submit / _collect, as TopDownInferenceModel's: uint8 frames and a model that can run the
+        fused step."""
+        if not self._can_fuse() or first.dtype != np.uint8:
+            return None
         K, NC = self._configure_fused(batch_size, *first.shape[1:])
-
-        def collect(slot, B):
-            return self._run_fused(B, K, NC, "sb_topdown_multiclass_collect", slot)
-
-        yield from _pipelined_batches(cc, imgs, batch_size, "sb_topdown_multiclass_submit", collect)
-
-    def predict(self, data, numpy: bool = True, batch_size: int = 4, **kwargs):
-        """sleap/nn/inference.py:989-1045 with the pipelined batch loop."""
-        return _merge_batches(list(self.predict_batches(data, batch_size)))
+        return (self.centroid_crop.keras_model, "sb_topdown_multiclass_submit",
+                lambda slot, B: self._run_fused(B, K, NC, "sb_topdown_multiclass_collect", slot))
 
     def call(self, example):
         if isinstance(example, np.ndarray):
@@ -1289,22 +1222,8 @@ class Predictor:
                 batch["centroids"] = [e["centroids"] for e in exs]
             yield batch
 
-    def _batches(self, data):
-        from sleap_b200.io.video import FrameFeeder
-        imgs = _images_of(data)
-        if isinstance(imgs, FrameFeeder):
-            i = 0
-            for _, batch in imgs.batches():
-                yield i, batch
-                i += len(batch)
-            return
-        n = len(imgs)
-        for i in range(0, n, self.batch_size):
-            batch = np.stack([np.asarray(imgs[j]) for j in range(i, min(n, i + self.batch_size))])
-            yield i, batch
-
     def _predict_generator(self, data):
-        """:377-420: one predict_on_batch per batch (+ frame indices)."""
+        """:377-420: the inference model's batch loop (+ frame indices)."""
         from sleap_b200.io.labels import Labels, LabelsReader
         from sleap_b200.io.video import FrameFeeder
         if isinstance(data, Labels):
@@ -1324,29 +1243,18 @@ class Predictor:
         feeder = data if isinstance(data, FrameFeeder) else None
         frame_inds = (lambda a, b: np.asarray(feeder.inds[a:b])) if feeder is not None else (lambda a, b: np.arange(a, b))
         try:
-            if hasattr(self.inference_model, "predict_batches"):      # pipelined device loop (upload i+1 || compute i)
-                i0 = 0
-                want_img = self.tracker is not None and getattr(self.tracker, "uses_image", False)   # flow trackers (:2664-2671)
-                imgs_all = _images_of(data)
-                hw = tuple(np.asarray(imgs_all[0]).shape[:2]) if len(imgs_all) else (1, 1)
-                for ex in self.inference_model.predict_batches(imgs_all, self.batch_size):
-                    n = len(ex["instance_peaks"])
-                    ex["frame_ind"] = frame_inds(i0, i0 + n)
-                    ex["video_ind"] = np.zeros(n, np.int64)
-                    ex["image_hw"] = hw
-                    if want_img:
-                        ex["image"] = np.stack([np.asarray(imgs_all[j]) for j in range(i0, i0 + n)])
-                    i0 += n
-                    self._check_flags(ex)
-                    yield ex
-                return
-            for i0, batch in self._batches(data):
-                ex = self.inference_model.predict_on_batch(batch)
-                ex["frame_ind"] = frame_inds(i0, i0 + len(batch))
-                ex["video_ind"] = np.zeros(len(batch), np.int64)
-                ex["image_hw"] = tuple(batch.shape[1:3])
-                if self.tracker is not None and getattr(self.tracker, "uses_image", False):
-                    ex["image"] = batch
+            i0 = 0
+            want_img = self.tracker is not None and getattr(self.tracker, "uses_image", False)   # flow trackers (:2664-2671)
+            imgs_all = _images_of(data)
+            hw = tuple(np.asarray(imgs_all[0]).shape[:2]) if len(imgs_all) else (1, 1)
+            for ex in self.inference_model.predict_batches(imgs_all, self.batch_size):
+                n = len(ex["instance_peaks"])
+                ex["frame_ind"] = frame_inds(i0, i0 + n)
+                ex["video_ind"] = np.zeros(n, np.int64)
+                ex["image_hw"] = hw
+                if want_img:
+                    ex["image"] = np.stack([np.asarray(imgs_all[j]) for j in range(i0, i0 + n)])
+                i0 += n
                 self._check_flags(ex)
                 yield ex
         finally:
@@ -1503,6 +1411,21 @@ class Predictor:
             return None
         return tr
 
+    @contextlib.contextmanager
+    def _tracking_in_step(self, owner, model, make_labels):
+        """For the span of the block, the step tracker (``_step_tracker``) set as ``owner.tracker`` (the layer or model
+        whose device step of ``model`` runs it), detached from the step after."""
+        tr = self._step_tracker(model, make_labels)
+        if tr is None:
+            yield
+            return
+        owner.tracker = tr
+        try:
+            yield
+        finally:
+            owner.detach_tracker()
+            owner.tracker = None
+
     def _apply_device_tracks(self, ex, new):
         """The frames' tracked lists from the track records of their step (a predictor with a device tracker)."""
         for k, lf in enumerate(new):
@@ -1638,15 +1561,8 @@ class TopDownPredictor(Predictor):
         im = self.inference_model
         if not im._can_fuse() or isinstance(data, (Labels, LabelsReader)):
             return super().predict(data, make_labels)
-        tr = self._step_tracker(im.centroid_crop.keras_model, make_labels)
-        if tr is None:
+        with self._tracking_in_step(im, im.centroid_crop.keras_model, make_labels):
             return super().predict(data, make_labels)
-        im.tracker = tr
-        try:
-            return super().predict(data, make_labels)
-        finally:
-            im.detach_tracker()
-            im.tracker = None
 
     @classmethod
     def from_trained_models(cls, centroid_model_path=None, confmap_model_path=None, batch_size=4, peak_threshold=0.2,
@@ -1697,15 +1613,9 @@ class BottomUpPredictor(Predictor):
         grouping kernel, on the model's GPU); the consumer thread only maps its track ids to ``Track`` objects before
         ``final_pass``.  The tracker's GPU must be the model's, and the run must be on one rank."""
         layer = self.inference_model.bottomup_layer
-        tr = self._step_tracker(layer.keras_model, make_labels)
-        if tr is None:
+        layer.tracker_cut = -1 if self.max_instances is None else int(self.max_instances)
+        with self._tracking_in_step(layer, layer.keras_model, make_labels):
             return super().predict(data, make_labels)
-        layer.tracker, layer.tracker_cut = tr, -1 if self.max_instances is None else int(self.max_instances)
-        try:
-            return super().predict(data, make_labels)
-        finally:
-            layer.detach_tracker()
-            layer.tracker = None
 
     def _initialize_inference_model(self):
         """:3119-3150."""

@@ -219,8 +219,8 @@ def test_topdown_refusals(pair):
     clean()
 
 
-def test_slot_tracks_refusals(pair):
-    """sb_topdown_slot_tracks reads only the track records of the batch last collected from the slot, with its B."""
+def test_topdown_tracks_slot_refusals(pair):
+    """sb_topdown_tracks from a slot reads only the track records of the batch last collected from it, with its B."""
     from sleap_b200.nn.inference import _topdown_params
     _, _, gray, _ = pair
     im = td_predictor(pair, 4).inference_model
@@ -236,12 +236,12 @@ def test_slot_tracks_refusals(pair):
 
     def slot_tracks(slot, B, msg):
         with pytest.raises(_lib.SleapB200Error, match=msg):
-            h.call("sb_topdown_slot_tracks", mid, slot, B, _lib.ptr(rec))
+            h.call("sb_topdown_tracks", mid, slot, B, _lib.ptr(rec))
 
     slot_tracks(1, 4, "slot 1 holds no collected batch of 4 frames")
     h.call("sb_topdown_submit", mid, _lib.ptr(b0), 4, 0)
     slot_tracks(0, 4, "slot 0 holds no collected batch of 4 frames")
-    out = im._run_fused(4, K, "sb_topdown_collect", 0, tracks=("sb_topdown_slot_tracks", 0))
+    out = im._run_fused(4, K, "sb_topdown_collect", 0, slot=0)
     assert out["track_n"].sum() > 0
     slot_tracks(0, 3, "slot 0 holds no collected batch of 3 frames")
     im.detach_tracker()

@@ -163,7 +163,7 @@ def test_over_capacity_raises_at_first_frame(pair):
         pred.predict(gray)
 
 
-def test_abi(pair):
+def test_track_abi(pair):
     _, imodel, gray, _, _ = pair
     pred = _predictor(pair, 8)
     im = pred.inference_model
@@ -179,7 +179,7 @@ def test_abi(pair):
     im.detach_tracker()
     im.tracker = None
     with pytest.raises(_lib.SleapB200Error):         # nothing attached
-        mc.handle.call("sb_topdown_tracks", mc.model_id, 8, _lib.ptr(rec))
+        mc.handle.call("sb_topdown_tracks", mc.model_id, -1, 8, _lib.ptr(rec))
     other = T.DeviceTracker(0, dict(tr.device_params, n_nodes=len(NODES) - 1, max_instances=8, track_table=16), handle=mc.handle)
     with pytest.raises(_lib.SleapB200Error):         # other node count than the instance model's
         mc.handle.call("sb_topdown_attach_tracker", mc.model_id, other.id, 1024.0, 1024.0)
