@@ -82,6 +82,15 @@ int sb_crop_centered(sb_handle_t h, const void* images_host, int images_are_u8, 
                      int W, int C, const float* centroids, const int32_t* sample_inds, int n,
                      int crop_h, int crop_w, void* out_crops);
 
+/* CentroidCrop.call with precrop_resize = scale (sleap/nn/inference.py:1836-1841, :1918-1927): the crops of
+ * resize_image(images, scale) (sleap/nn/data/resizing.py:71-106: int(float32(W) * scale) x int(float32(H) * scale),
+ * bilinear with half-pixel centres, no antialias, cast back to the frame dtype -- uint8 by truncation), byte for byte;
+ * centroids are in resized-frame coordinates.  The resized frames are computed on the fly and never stored.
+ * SB_ERR_INVALID: a scale that is not finite and positive, or that gives a resized frame with a zero extent. */
+int sb_crop_centered_resized(sb_handle_t h, const void* images_host, int images_are_u8, int B, int H, int W, int C,
+                             const float* centroids, const int32_t* sample_inds, int n, int crop_h, int crop_w,
+                             float scale, void* out_crops);
+
 /* ---- stage level: PAF grouping (host buffers) --------------------------------------------
  * sleap/nn/paf_grouping.py:406-550 score_paf_lines_batch (:82-142 candidates, :145-275 line
  * sampling, :278-403 scoring).  pafs (B,Hp,Wp,2E) f32; peaks (N,2) image px, peak_channel_inds
@@ -354,7 +363,10 @@ int sb_infer_centroids(sb_handle_t h, int model_id, const void* images_host, int
  * Outputs are dense and NaN padded: centroids (B,K,2), centroid_vals (B,K), instance_peaks (B,K,n_nodes,2),
  * instance_peak_vals (B,K,n_nodes) with K = max_centroids_per_frame; n_valid (B); flags (B).  The instance network is
  * configured for max_crops_per_call crops of crop_size x crop_size and runs as often as the batch's crop count needs.
- * Not covered (use the stage-level calls): instance models trained at an input scale != 1 (pre-crop resize). */
+ * An instance model trained at an input scale s != 1 (CentroidCrop.precrop_resize, :1836-1843): the centroids are
+ * multiplied by s (one float32 multiply, before the top-k) and the crops are cut from the frames resized by s, as
+ * sb_crop_centered_resized cuts them, without storing the resized frames; the returned centroids are in resized-frame
+ * coordinates, the instance peaks in frame coordinates (/ s + 0.5, + crop offset / s, with instance.input_scale = s). */
 typedef struct sb_topdown_params {
   int32_t centroid_model, instance_model;
   sb_centroid_params centroid;      /* as sb_centroid_configure */
@@ -363,6 +375,8 @@ typedef struct sb_topdown_params {
   int32_t max_instances;            /* top-k per frame by centroid confidence; <= 0: keep every centroid */
   int32_t max_centroids_per_frame;  /* K */
   int32_t max_crops_per_call;       /* batch the instance network is planned for */
+  float precrop_resize;             /* s: resize the frames by s before cropping; 1 or 0: no resize.  SB_ERR_INVALID at
+                                       configure time: negative, NaN or infinite, or a resized frame with a zero extent */
 } sb_topdown_params;
 int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* params, int max_batch, int H, int W, int C_in);
 int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
@@ -409,7 +423,8 @@ int sb_topdown_collect(sb_handle_t h, int centroid_model_id, int slot, int B, fl
  * out_centroid_vals (B,K), out_n_valid (B) crops per frame, out_flags (B).  out_class_vectors (B,K,n_classes): every
  * crop's class probabilities in crop order, NaN padded (may be NULL).
  * sb_infer_topdown refuses a multi-class pipeline and sb_infer_topdown_multiclass a plain one; the chain rules of
- * sb_topdown_configure hold.  Not covered: instance models trained at an input scale != 1. */
+ * sb_topdown_configure hold.  Instance models trained at an input scale != 1 are not covered: a precrop_resize other
+ * than 0 or 1 is refused (SB_ERR_UNSUPPORTED). */
 #define SB_MAX_DENSE_WIDTH 4096
 typedef struct sb_topdown_multiclass_params {
   sb_topdown_params topdown;        /* as sb_topdown_configure */

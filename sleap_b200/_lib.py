@@ -72,7 +72,7 @@ class CentroidParams(ctypes.Structure):
 class TopdownParams(ctypes.Structure):
     _fields_ = [("centroid_model", c_int32), ("instance_model", c_int32), ("centroid", CentroidParams), ("instance", GlobalParams),
                 ("crop_size", c_int32), ("max_instances", c_int32), ("max_centroids_per_frame", c_int32),
-                ("max_crops_per_call", c_int32)]
+                ("max_crops_per_call", c_int32), ("precrop_resize", c_float)]
 
 
 class TopdownMultiClassParams(ctypes.Structure):
@@ -107,6 +107,8 @@ _SIGS = {
                              c_void_p, c_void_p],
     "sb_crop_centered": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                          c_int, c_int, c_void_p],
+    "sb_crop_centered_resized": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                 c_int, c_int, c_float, c_void_p],
     "sb_score_paf_lines_batch": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                  c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_int, c_void_p,
                                  c_void_p, c_void_p, c_void_p],

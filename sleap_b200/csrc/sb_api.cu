@@ -122,6 +122,29 @@ int sb_peaks_to_host(sb_handle_s* h, const SbPostWs& ws, int B, float* out_point
   return s.sync();
 }
 
+// sb_crop_centered (resized: false) and sb_crop_centered_resized (the frames resized to Hr x Wr) on host arrays
+static int crop_centered(sb_handle_s* h, const void* images_host, int images_are_u8, int B, int H, int W, int C,
+                         const float* centroids, const int32_t* sample_inds, int n, int crop_h, int crop_w, bool resized, int Hr,
+                         int Wr, void* out_crops) {
+  if (n <= 0) return SB_OK;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  const size_t esz = images_are_u8 ? 1 : 4;
+  const size_t nimg = (size_t)B * H * W * C * esz, nout = (size_t)n * crop_h * crop_w * C * esz;
+  SbScratch s(h);
+  const uint8_t* d_img;
+  const float* d_c;
+  const int* d_s;
+  uint8_t* d_out;
+  int rc;
+  if ((rc = s.upload((const uint8_t*)images_host, nimg, &d_img)) || (rc = s.upload(centroids, (size_t)n * 2, &d_c)) ||
+      (rc = s.upload(sample_inds, (size_t)n, &d_s)) || (rc = s.alloc(&d_out, nout)) ||
+      (rc = resized ? sbk_crop_resized(h, d_img, images_are_u8, B, H, W, C, Hr, Wr, d_c, d_s, n, crop_h, crop_w, d_out)
+                    : sbk_crop(h, d_img, images_are_u8, B, H, W, C, d_c, d_s, n, crop_h, crop_w, d_out, images_are_u8)) ||
+      (rc = s.to_host((uint8_t*)out_crops, d_out, nout)))
+    return rc;
+  return s.sync();
+}
+
 extern "C" {
 
 int sb_find_local_peaks(sb_handle_t h, const float* cms_host, int B, int H, int W, int C,
@@ -167,22 +190,17 @@ int sb_crop_centered(sb_handle_t h, const void* images_host, int images_are_u8, 
                      int C, const float* centroids, const int32_t* sample_inds, int n, int crop_h,
                      int crop_w, void* out_crops) {
   if (!h) return sb_fail(nullptr, SB_ERR_INVALID, "null handle");
-  if (n <= 0) return SB_OK;
-  SB_CUDA(h, cudaSetDevice(h->device));
-  const size_t esz = images_are_u8 ? 1 : 4;
-  const size_t nimg = (size_t)B * H * W * C * esz, nout = (size_t)n * crop_h * crop_w * C * esz;
-  SbScratch s(h);
-  const uint8_t* d_img;
-  const float* d_c;
-  const int* d_s;
-  uint8_t* d_out;
-  int rc;
-  if ((rc = s.upload((const uint8_t*)images_host, nimg, &d_img)) || (rc = s.upload(centroids, (size_t)n * 2, &d_c)) ||
-      (rc = s.upload(sample_inds, (size_t)n, &d_s)) || (rc = s.alloc(&d_out, nout)) ||
-      (rc = sbk_crop(h, d_img, images_are_u8, B, H, W, C, d_c, d_s, n, crop_h, crop_w, d_out, images_are_u8)) ||
-      (rc = s.to_host((uint8_t*)out_crops, d_out, nout)))
-    return rc;
-  return s.sync();
+  return crop_centered(h, images_host, images_are_u8, B, H, W, C, centroids, sample_inds, n, crop_h, crop_w, false, H, W, out_crops);
+}
+
+int sb_crop_centered_resized(sb_handle_t h, const void* images_host, int images_are_u8, int B, int H, int W, int C,
+                             const float* centroids, const int32_t* sample_inds, int n, int crop_h, int crop_w, float scale,
+                             void* out_crops) {
+  if (!h) return sb_fail(nullptr, SB_ERR_INVALID, "null handle");
+  int Hr, Wr;
+  if (sb_resized_size(H, W, scale, &Hr, &Wr))
+    return sb_fail(h, SB_ERR_INVALID, "sb_crop_centered_resized: scale %g of %d x %d frames", scale, H, W);
+  return crop_centered(h, images_host, images_are_u8, B, H, W, C, centroids, sample_inds, n, crop_h, crop_w, true, Hr, Wr, out_crops);
 }
 
 // Builds the per-node ascending peak lists on the host (stable argsort by channel,

@@ -178,6 +178,19 @@ int sbk_lsap_batch(sb_handle_s* h, const float* scores, const int* n_src, const 
 int sbk_crop(sb_handle_s* h, const void* images, int img_is_u8, int B, int H, int W, int C,
              const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w,
              void* out, int out_is_u8_trunc);
+// The size resize_image gives H x W frames at `scale`: int(float32(H) * scale) x int(float32(W) * scale), as sb_net_size
+// and FrameResizer compute it.  Nonzero (no size) when scale is not finite and positive or an extent is below 1.
+static inline int sb_resized_size(int H, int W, float scale, int* Hr, int* Wr) {
+  const float fh = (float)H * scale, fw = (float)W * scale;
+  if (!(scale > 0.f) || !(fh >= 1.f && fh < 2147483648.f) || !(fw >= 1.f && fw < 2147483648.f)) return 1;
+  *Hr = (int)fh;
+  *Wr = (int)fw;
+  return 0;
+}
+// sbk_crop of the frames resized to Hr x Wr (resize_image, uint8 frames cast back by truncation) without storing them;
+// centroids in resized-frame coordinates
+int sbk_crop_resized(sb_handle_s* h, const void* images, int img_is_u8, int B, int H, int W, int C, int Hr, int Wr,
+                     const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w, void* out);
 
 int sbk_lines(sb_handle_s* h, const float* pafs, int Hp, int Wp, int C2, const float* lines_in,
               const float* peaks, const int* edge_peak_inds, const int* edge_inds, int n, int P,
@@ -273,7 +286,24 @@ struct SbRecField {
 void sb_split_records(const float* rec, int B, size_t width, std::initializer_list<SbRecField> floats,
                       std::initializer_list<int32_t*> ints);
 
-// ---- frame preprocessing shared by k_preprocess and the fused first-layer / stem view kernels ----
+// ---- frame preprocessing shared by k_preprocess, the fused first-layer / stem view kernels and the resized crops ----
+// Pixel (oy, ox) of an Hin x Win image resized to Hres x Wres: bilinear, half-pixel centres, no antialias
+// (tf.image.resize); fetch(y, x) is one source texel as a float.  Explicitly rounded, so that every caller computes the
+// same value whatever the contraction setting of its file.
+template <typename Fetch>
+__device__ __forceinline__ float sb_resize_sample(const Fetch& fetch, int oy, int ox, int Hin, int Win, int Hres, int Wres) {
+  const float scy = (float)Hin / (float)Hres, scx = (float)Win / (float)Wres;
+  const float sy = __fadd_rn(__fmul_rn(__fadd_rn((float)oy, 0.5f), scy), -0.5f);
+  const float sx = __fadd_rn(__fmul_rn(__fadd_rn((float)ox, 0.5f), scx), -0.5f);
+  const float fy = floorf(sy), fx = floorf(sx);
+  const int y0 = max((int)fy, 0), y1 = min((int)ceilf(sy), Hin - 1);
+  const int x0 = max((int)fx, 0), x1 = min((int)ceilf(sx), Win - 1);
+  const float ly = __fsub_rn(sy, fy), lx = __fsub_rn(sx, fx);
+  const float tl = fetch(y0, x0), tr = fetch(y0, x1), bl = fetch(y1, x0), br = fetch(y1, x1);
+  const float tp = __fadd_rn(tl, __fmul_rn(__fadd_rn(tr, -tl), lx));
+  const float bt = __fadd_rn(bl, __fmul_rn(__fadd_rn(br, -bl), lx));
+  return __fadd_rn(tp, __fmul_rn(__fadd_rn(bt, -tp), ly));
+}
 // caffe mean of BGR channel c (resnet.py imagenet_preproc_v1)
 __device__ __forceinline__ float sb_imagenet_caffe_mean(int c) { return c == 0 ? 103.939f : (c == 1 ? 116.779f : 123.68f); }
 // ensure_grayscale of one RGB pixel as a [0, 1] float (u8: truncating round trip like tf.image.rgb_to_grayscale)

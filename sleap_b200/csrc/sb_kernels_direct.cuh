@@ -291,21 +291,7 @@ __global__ void k_preprocess(const TI* __restrict__ in, int Hin, int Win, int Ci
         }
         return f;
       };
-      if (!resize) {
-        v = fetch(oy, ox);
-      } else {
-        const float scy = (float)Hin / (float)Hres, scx = (float)Win / (float)Wres;
-        const float sy = __fadd_rn(__fmul_rn(__fadd_rn((float)oy, 0.5f), scy), -0.5f);
-        const float sx = __fadd_rn(__fmul_rn(__fadd_rn((float)ox, 0.5f), scx), -0.5f);
-        const float fy = floorf(sy), fx = floorf(sx);
-        const int y0 = max((int)fy, 0), y1 = min((int)ceilf(sy), Hin - 1);
-        const int x0 = max((int)fx, 0), x1 = min((int)ceilf(sx), Win - 1);
-        const float ly = sy - fy, lx = sx - fx;
-        const float tl = fetch(y0, x0), tr = fetch(y0, x1), bl = fetch(y1, x0), br = fetch(y1, x1);
-        const float tp = __fadd_rn(tl, __fmul_rn(__fadd_rn(tr, -tl), lx));
-        const float bt = __fadd_rn(bl, __fmul_rn(__fadd_rn(br, -bl), lx));
-        v = __fadd_rn(tp, __fmul_rn(__fadd_rn(bt, -tp), ly));
-      }
+      v = resize ? sb_resize_sample(fetch, oy, ox, Hin, Win, Hres, Wres) : fetch(oy, ox);
     }
     if (imagenet) v = __fsub_rn(__fmul_rn(v, 255.f), sb_imagenet_caffe_mean(c));
     st(out + t, v);

@@ -938,10 +938,31 @@ __global__ void __launch_bounds__(128) k_class_group(
 }
 
 // ------------------------------------------------------------------------------------------
-// Centred bilinear crops (top-down): crop_bboxes(make_centered_bboxes(centroid, h, w)).
+// Centred bilinear crops (top-down): crop_bboxes(make_centered_bboxes(centroid, h, w)) of the H x W frames a texel
+// source reads: the frames themselves, or the frames resized on the fly (resize_image before the crop, for instance
+// models trained at an input scale != 1), which is never stored.
 // ------------------------------------------------------------------------------------------
-template <typename TI, typename TO, bool TRUNC_U8>
-__global__ void k_crop(const TI* __restrict__ images, int H, int W, int C,
+template <typename TI>
+struct SbFrameTexels {                      // channel c of pixel (y, x) of frame b
+  const TI* __restrict__ img;
+  int H, W, C;
+  __device__ __forceinline__ float operator()(int b, int y, int x, int c) const {
+    return (float)img[(size_t)b * H * W * C + ((size_t)y * W + x) * C + c];
+  }
+};
+template <typename TI, bool TRUNC_U8>
+struct SbResizedTexels {                    // channel c of pixel (y, x) of frame b resized from H x W to Hr x Wr
+  const TI* __restrict__ img;
+  int H, W, C, Hr, Wr;
+  __device__ __forceinline__ float operator()(int b, int y, int x, int c) const {
+    const TI* f = img + (size_t)b * H * W * C + c;
+    const float v = sb_resize_sample([&](int sy, int sx) { return (float)f[((size_t)sy * W + sx) * C]; }, y, x, H, W, Hr, Wr);
+    return TRUNC_U8 ? truncf(fminf(fmaxf(v, 0.f), 255.f)) : v;    // tf.cast back to the frame dtype
+  }
+};
+
+template <typename Src, typename TO, bool TRUNC_U8>
+__global__ void k_crop(Src img, int H, int W, int C,
                        const float* __restrict__ centroids, const int* __restrict__ sample_inds,
                        int crop_h, int crop_w, TO* __restrict__ out) {
   const int n = blockIdx.y;
@@ -954,7 +975,6 @@ __global__ void k_crop(const TI* __restrict__ images, int H, int W, int C,
   const float x2 = (cx + (float)(crop_w - 1) * 0.5f) / Wm1;
   const float hs = (crop_h > 1) ? ((y2 - y1) * Hm1) / (float)(crop_h - 1) : 0.f;
   const float wsx = (crop_w > 1) ? ((x2 - x1) * Wm1) / (float)(crop_w - 1) : 0.f;
-  const TI* img = images + (size_t)b * H * W * C;
   const int total = crop_h * crop_w * C;
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
     const int c = t % C;
@@ -967,10 +987,7 @@ __global__ void k_crop(const TI* __restrict__ images, int H, int W, int C,
       const int ty = (int)floorf(in_y), by = (int)ceilf(in_y);
       const int lx = (int)floorf(in_x), rx = (int)ceilf(in_x);
       const float ly = in_y - (float)ty, xl = in_x - (float)lx;
-      const float tl = (float)img[((size_t)ty * W + lx) * C + c];
-      const float tr = (float)img[((size_t)ty * W + rx) * C + c];
-      const float bl = (float)img[((size_t)by * W + lx) * C + c];
-      const float br = (float)img[((size_t)by * W + rx) * C + c];
+      const float tl = img(b, ty, lx, c), tr = img(b, ty, rx, c), bl = img(b, by, lx, c), br = img(b, by, rx, c);
       const float tp = tl + (tr - tl) * xl;
       const float bt = bl + (br - bl) * xl;
       v = tp + (bt - tp) * ly;
@@ -1245,21 +1262,39 @@ int sbk_lsap_batch(sb_handle_s* h, const float* scores, const int* n_src, const 
   return 0;
 }
 
-int sbk_crop(sb_handle_s* h, const void* images, int img_is_u8, int B, int H, int W, int C,
-             const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w, void* out,
-             int out_is_u8_trunc) {
+// k_crop of n crops of the H x W frames `src` reads: uint8 frames give uint8 crops (float -> uint8 truncation, as tf.cast in
+// crop_bboxes), float frames float crops
+template <template <typename> class Src>
+static int launch_crop(sb_handle_s* h, Src<unsigned char> src_u8, Src<float> src_f32, int img_is_u8, int H, int W, int C,
+                       const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w, void* out) {
   if (n <= 0) return 0;
   const int total = crop_h * crop_w * C;
   dim3 g((total + 255) / 256, n);
   if (g.x > 64) g.x = 64;
   if (img_is_u8)
-    k_crop<unsigned char, unsigned char, true><<<g, 256, 0, h->stream>>>(
-        (const unsigned char*)images, H, W, C, centroids, sample_inds, crop_h, crop_w, (unsigned char*)out);
+    k_crop<Src<unsigned char>, unsigned char, true><<<g, 256, 0, h->stream>>>(src_u8, H, W, C, centroids, sample_inds, crop_h,
+                                                                             crop_w, (unsigned char*)out);
   else
-    k_crop<float, float, false><<<g, 256, 0, h->stream>>>((const float*)images, H, W, C, centroids,
-                                                           sample_inds, crop_h, crop_w, (float*)out);
+    k_crop<Src<float>, float, false><<<g, 256, 0, h->stream>>>(src_f32, H, W, C, centroids, sample_inds, crop_h, crop_w,
+                                                               (float*)out);
   SB_CHECK_LAUNCH(h);
   return 0;
+}
+
+template <typename TI>
+using SbResizedFrameTexels = SbResizedTexels<TI, sizeof(TI) == 1>;
+
+int sbk_crop(sb_handle_s* h, const void* images, int img_is_u8, int B, int H, int W, int C,
+             const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w, void* out,
+             int out_is_u8_trunc) {
+  return launch_crop<SbFrameTexels>(h, {(const unsigned char*)images, H, W, C}, {(const float*)images, H, W, C}, img_is_u8, H, W,
+                                    C, centroids, sample_inds, n, crop_h, crop_w, out);
+}
+
+int sbk_crop_resized(sb_handle_s* h, const void* images, int img_is_u8, int B, int H, int W, int C, int Hr, int Wr,
+                     const float* centroids, const int* sample_inds, int n, int crop_h, int crop_w, void* out) {
+  return launch_crop<SbResizedFrameTexels>(h, {(const unsigned char*)images, H, W, C, Hr, Wr}, {(const float*)images, H, W, C, Hr, Wr},
+                                           img_is_u8, Hr, Wr, C, centroids, sample_inds, n, crop_h, crop_w, out);
 }
 
 int sbk_lines(sb_handle_s* h, const float* pafs, int Hp, int Wp, int C2, const float* lines_in,

@@ -11,7 +11,8 @@
 // (sleap/nn/heads.py:431-460) and classify_peaks_from_vectors (sleap/nn/identity.py:182-254).
 // Round 1 ran these as separate host-facing calls: centroids D2H -> host top-k -> frames H2D again -> crops D2H ->
 // crops H2D -> instance network (sleap_b200/nn/inference.py CentroidCrop / FindInstancePeaks, kept for the stage-level
-// surface and for models that need a pre-crop resize).
+// surface).  A pre-crop resize (CentroidCrop.precrop_resize, :1836-1843) scales the kept centroids in k_td_select and cuts
+// the crops from the resident frames resized on the fly (sbk_crop_resized).
 //
 // The head's float64 sums use __dmul_rn / __dadd_rn: this file is built with multiply-add contraction on, and a fused
 // product would round differently from the definition (include/sleap_b200.h).
@@ -28,9 +29,11 @@
 namespace {
 
 // Per frame: keep all centroids in tf.where order, or -- more than max_instances -- the max_instances most confident ones
-// in tf.math.top_k order (descending value, ties: lower index first).  K = capacity of the dense outputs.
+// in tf.math.top_k order (descending value, ties: lower index first).  K = capacity of the dense outputs.  The kept
+// centroids are multiplied by the pre-crop resize `scale` (1: unchanged), rounded on its own: the crop offsets subtract
+// half the crop size from the product.
 __global__ void __launch_bounds__(128) k_td_select(const float* __restrict__ peaks, const float* __restrict__ peak_vals,
-                                                   const int* __restrict__ n_peaks, int max_peaks, int max_instances, int K,
+                                                   const int* __restrict__ n_peaks, int max_peaks, int max_instances, int K, float scale,
                                                    float* __restrict__ sel_cent, float* __restrict__ sel_val, int* __restrict__ sel_count,
                                                    int* __restrict__ flags) {
   const int b = blockIdx.x;
@@ -48,8 +51,8 @@ __global__ void __launch_bounds__(128) k_td_select(const float* __restrict__ pea
       pos = rank;
     }
     if (pos < keep && pos < K) {
-      sel_cent[((size_t)b * K + pos) * 2] = pk[2 * i];
-      sel_cent[((size_t)b * K + pos) * 2 + 1] = pk[2 * i + 1];
+      sel_cent[((size_t)b * K + pos) * 2] = __fmul_rn(pk[2 * i], scale);
+      sel_cent[((size_t)b * K + pos) * 2 + 1] = __fmul_rn(pk[2 * i + 1], scale);
       sel_val[(size_t)b * K + pos] = pv[i];
     }
   }
@@ -321,6 +324,8 @@ struct SbTopdown {
   SbModel* inst = nullptr;
   unsigned gen_c = 0, gen_i = 0;    // chain_gen of the centroid and the instance model when it was configured
   int K = 0, nodes = 0, width = 0, Bmax = 0;
+  float scale = 1.f;                // pre-crop resize (1: none) and the resized frame the crops are cut from
+  int Hr = 0, Wr = 0;
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
   void* crops = nullptr;
@@ -362,8 +367,16 @@ void sb_topdown_free(SbModel* m) {
 
 namespace {
 
+// The pre-crop resize of the parameters (0: 1) and the size of the H x W frames resized by it
+int precrop_size(sb_handle_s* h, const sb_topdown_params* p, int H, int W, float* s, int* Hr, int* Wr) {
+  *s = p->precrop_resize == 0.f ? 1.f : p->precrop_resize;
+  if (sb_resized_size(H, W, *s, Hr, Wr))
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: precrop_resize %g of %d x %d frames", p->precrop_resize, H, W);
+  return 0;
+}
+
 // The arguments both top-down configure calls check before anything is dropped
-int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, SbModel** mc, SbModel** mi) {
+int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, SbModel** mc, SbModel** mi) {
   static const char* const bad_ids = "sb_topdown_configure: bad model ids";
   *mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
   *mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
@@ -373,7 +386,9 @@ int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, SbM
   if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_configure: more than 1024 frames per batch");
   const int nb = (int)(*mi)->buffers.size();
   if (p->instance.cms_buffer < 0 || p->instance.cms_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
-  return 0;
+  float s;
+  int Hr, Wr;
+  return precrop_size(h, p, H, W, &s, &Hr, &Wr);
 }
 
 // Configures both networks and their chains, then the pipeline with a record of `width` floats per frame (the centroid
@@ -390,6 +405,7 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   mc->td = t;
   t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
   t->gen_c = mc->chain_gen; t->gen_i = mi->chain_gen;
+  precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by check_topdown
   t->nodes = mi->buffers[p->instance.cms_buffer].C;
   t->multiclass = n_classes > 0;
   t->width = t->multiclass ? (int)td_class_record_width(n_classes, t->nodes, t->K) : t->K * (3 + t->nodes * 3) + 2;
@@ -456,7 +472,7 @@ int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
   const float* coff = cp.offsets_buffer >= 0 ? (const float*)mc->buffers[cp.offsets_buffer].dev : nullptr;
   SbPeakParams pc{cp.peak_threshold, cp.refinement, cp.integral_patch_size, (float)cp.output_stride, cp.input_scale};
   if ((rc = sbk_local_peaks(h, (const float*)cb.dev, coff, B, cb.H, cb.W, cb.C, pc, mc->ws))) return rc;
-  k_td_select<<<B, 128, 0, s>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->sel_cent,
+  k_td_select<<<B, 128, 0, s>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->scale, t->sel_cent,
                                 t->sel_val, t->sel_count, mc->ws.flags);
   SB_CHECK_LAUNCH(h);
   k_td_flatten<<<1, 256, 0, s>>>(t->sel_cent, t->sel_count, B, t->K, (float)t->p.crop_size * 0.5f, t->flat_cent, t->flat_off,
@@ -485,9 +501,14 @@ int instance_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
   int rc;
   for (int c0 = 0; c0 < total; c0 += mi->B) {
     const int n = std::min(mi->B, total - c0);
-    // crops of the frames already resident in HBM (uint8 frames: float -> uint8 truncation, as tf.cast in crop_bboxes)
-    if ((rc = sbk_crop(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->flat_cent + 2 * (size_t)c0, t->flat_sample + c0, n,
-                       cs, cs, t->crops, frames_are_u8))) return rc;
+    // crops of the frames already resident in HBM (uint8 frames: float -> uint8 truncation, as tf.cast in crop_bboxes),
+    // with a pre-crop resize of those frames resized on the fly
+    const float* cent = t->flat_cent + 2 * (size_t)c0;
+    if ((rc = t->scale != 1.f ? sbk_crop_resized(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->Hr, t->Wr, cent,
+                                                 t->flat_sample + c0, n, cs, cs, t->crops)
+                              : sbk_crop(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, cent, t->flat_sample + c0, n, cs, cs,
+                                         t->crops, frames_are_u8)))
+      return rc;
     if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n, t->all_stores))) return rc;
     if ((rc = sbk_global_peaks(h, (const float*)ib.dev, ioff, n, ib.H, ib.W, ib.C, pi, t->flat_off + 2 * (size_t)c0, mi->gs.part, mi->gs.chunks, mi->gs.rpc,
                                t->ipts + (size_t)c0 * t->nodes * 2, t->ivals + (size_t)c0 * t->nodes))) return rc;
@@ -659,7 +680,7 @@ extern "C" {
 int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: null argument");
   SbModel *mc, *mi;
-  if (const int rc = check_topdown(h, p, max_batch, &mc, &mi)) return rc;
+  if (const int rc = check_topdown(h, p, max_batch, H, W, &mc, &mi)) return rc;
   return topdown_setup(h, p, max_batch, H, W, C_in, mc, mi, 0);
 }
 
@@ -725,8 +746,11 @@ int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, dou
 int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_params* p, int max_batch, int H, int W, int C_in) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_configure: null argument");
   SbModel *mc, *mi;
-  int rc = check_topdown(h, &p->topdown, max_batch, &mc, &mi);
+  int rc = check_topdown(h, &p->topdown, max_batch, H, W, &mc, &mi);
   if (rc) return rc;
+  if (p->topdown.precrop_resize != 0.f && p->topdown.precrop_resize != 1.f)
+    return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_multiclass_configure: instance models trained at an input scale != 1 (precrop_resize %g)",
+                   p->topdown.precrop_resize);
   // the tap: a buffer of the instance network holding C logical channels at the offset, in one plane or [lo | hi | hi]
   if (p->tap_buffer < 0 || p->tap_buffer >= (int)mi->buffers.size() || p->tap_channels <= 0 || p->tap_channel_offset < 0 ||
       (p->tap_planes != 1 && p->tap_planes != 3))

@@ -460,7 +460,7 @@ def _topdown_params(cc, fp):
     per frame)."""
     K = int(cc.max_instances) if cc.max_instances else int(cc.max_peaks_per_sample)
     return TopdownParams(cc.keras_model.model_id, fp.keras_model.model_id, cc.params(), fp.params(), int(cc.crop_size),
-                         int(cc.max_instances or 0), K, int(fp.max_crops_per_call)), K
+                         int(cc.max_instances or 0), K, int(fp.max_crops_per_call), float(cc.precrop_resize)), K
 
 
 def _configure_topdown(cc, fp, fn_name, p, shape, *arrays):
@@ -497,7 +497,7 @@ class TopDownInferenceModel(InferenceModel):
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
-        return (self.fused and type(cc) is CentroidCrop and type(fp) is FindInstancePeaks and cc.precrop_resize == 1.0 and
+        return (self.fused and type(cc) is CentroidCrop and type(fp) is FindInstancePeaks and
                 cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and cc.keras_model.handle is fp.keras_model.handle
                 and fp.keras_model.input_scale == 1.0)
 

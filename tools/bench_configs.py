@@ -2,8 +2,8 @@
 JSON line each (frames/s end to end with host frames, CUDA-event timed device loop where available).
 Secondary to bench.py (C4).
 
-  python tools/bench_configs.py [c1] [c2] [c3] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_track] [pipeline]
-                               [--steps K]
+  python tools/bench_configs.py [c1] [c2] [c3 | topdown] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_scaled]
+                               [topdown_track] [pipeline] [--steps K]
                                [--c5-batch B]
   (C5 default: 16 frames per GPU and step)
 
@@ -36,6 +36,12 @@ both through predict_on_batch.  Workload: the C3 pair (centroid UNet at input sc
 crops, max 5 animals, B=16) with a ClassVectorsHead of 4 classes and 3 x 64 fc units on the stride-16 features.  The line
 reports frames/s per arm and whether they agree (centroids and points bit for bit, identical assignments, the largest
 class-probability difference).
+
+topdown_scaled: the C3 pair with the centered-instance UNet trained at input scale 0.5 (96x96 crops of the frame resized
+to 512x512 before cropping), three arms alternating in one process on the same 128 pinned frames, B=16: the staged route
+(fused = False: centroids to the host, the frames resized by FrameResizer, crops through host memory), the fused step
+(predict_on_batch: resize and crop inside the step) and the double-buffered loop (predict_batches).  The line reports
+frames/s per arm (median and range over the repetitions) and whether all arms agree bit for bit.
 
 topdown_track: the top-down predictor with a tracker, four arms alternating in one process: TopDownPredictor.predict
 (labels made) of the C3 pair on 256 gray tracking-clip frames, B=16, the centroid threshold calibrated on clip frames to
@@ -462,6 +468,58 @@ def topdown_multiclass_bench(steps):
             if np.isfinite(a["instance_scores"]).any() else 0.0}
 
 
+def topdown_scaled_bench(steps):
+    """The C3 pair of topdown() with the instance UNet trained at input scale 0.5 (96x96 crops of the half-size frame, as
+    a model with input_scaling 0.5 loads): three arms alternating on the same 128 pinned frames, B = 16 -- the staged route
+    (fused = False: centroids to the host, FrameResizer, crops through host memory), the fused step per batch
+    (predict_on_batch) and the double-buffered loop (predict_batches)."""
+    n, B = 128, 16
+    fr = frames(n, 1024, 1024, 1, 3)
+    cspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="centroid", part_names=None, edges=None,
+                 heads=[dict(name="CentroidConfmapsHead", channels=1, output_stride=2)])
+    ispec = dict(backbone="unet", backbone_cfg=dict(unet(24, 16, 4), up_interpolate=False), head_type="centered_instance",
+                 part_names=FLIES13, edges=None, heads=[dict(name="CenteredInstanceConfmapsHead", channels=13, output_stride=4)])
+
+    def inference_model(fused):
+        # the staged arm owns its two device models: its calls reconfigure the chains the fused pipeline needs
+        cm_model, _, _ = model_for(cspec, 1, 1003, input_scale=0.5)
+        cms = cm_model.forward(fr[:2])[0]                                # ~5 animals per frame, as topdown() calibrates
+        thr = float(np.sort(cms.reshape(-1))[-(5 * 2 * 6)])
+        im_model = model_for(ispec, 1, 1004)[0]
+        im_model.config_input_scale = 0.5                                # what Predictor._load(..., resize_in_graph=False) sets
+        pred = TopDownPredictor(cm_model, im_model, crop_size=96, peak_threshold=thr, integral_refinement=True, batch_size=B,
+                                max_instances=5)
+        pred.inference_model.instance_peaks.peak_threshold = 0.0
+        pred.inference_model.fused = fused
+        return pred.inference_model
+
+    staged, fused = inference_model(False), inference_model(True)
+    assert not staged._can_fuse() and fused._can_fuse()
+    arms = {"staged predict_on_batch (fused = False)": lambda: [staged.predict_on_batch(fr[i:i + B]) for i in range(0, n, B)],
+            "fused predict_on_batch": lambda: [fused.predict_on_batch(fr[i:i + B]) for i in range(0, n, B)],
+            "streamed predict_batches": lambda: list(fused.predict_batches(fr, B))}
+    outs = {k: f() for k, f in arms.items()}                             # warm-up, and the outputs compared
+    reps = max(5, steps)
+    times = {k: [] for k in arms}
+    for _ in range(reps):                                                # arms alternate
+        for k, f in arms.items():
+            t0 = time.perf_counter()
+            f()
+            times[k].append(time.perf_counter() - t0)
+    keys = ("n_valid", "centroids", "centroid_vals", "instance_peaks", "instance_peak_vals")
+    ref = outs["staged predict_on_batch (fused = False)"]
+    agree = all(len(o) == len(ref) and all(np.asarray(x[k]).shape == np.asarray(y[k]).shape and
+                                           np.asarray(x[k]).tobytes() == np.asarray(y[k]).tobytes() for x, y in zip(o, ref) for k in keys)
+                for o in outs.values())
+    return {"config": "topdown_scaled: C3 top-down pair, instance UNet at input scale 0.5 (96x96 crops of the 512x512 resized frame), "
+                      "1024x1024, max 5 animals, B=16, 128 pinned frames", "gpu": gpu_identity(),
+            "metric": "frames/s (median of alternating repetitions; host frames in, result dicts out)", "repetitions": reps,
+            "frames_per_s": {k: n / float(np.median(v)) for k, v in times.items()},
+            "frames_per_s_range": {k: [n / max(v), n / min(v)] for k, v in times.items()},
+            "mean_instances_per_frame": float(np.mean(np.concatenate([o["n_valid"] for o in ref]))),
+            "arms_agree_bitwise": bool(agree)}
+
+
 def topdown_track_bench(steps):
     """TopDownPredictor.predict (labels made) of the C3 pair of topdown() on 256 tracking-clip frames (gray), B = 16, the
     centroid threshold calibrated on clip frames to about 5 animals per frame.  Four arms alternate in one process: no
@@ -629,8 +687,10 @@ if __name__ == "__main__":
             r = single("C1 single-instance UNet 256x256x1, 5 nodes, B=1", 256, list("abcde"), 1, steps)
         elif c == "c2":
             r = single("C2 single-instance UNet 512x512x1, 13 nodes, B=32", 512, FLIES13, 32, steps)
-        elif c == "c3":
+        elif c in ("c3", "topdown"):
             r = topdown(steps)
+        elif c == "topdown_scaled":
+            r = topdown_scaled_bench(steps)
         elif c == "r50":
             r = resnet50(steps)
         elif c == "track":
