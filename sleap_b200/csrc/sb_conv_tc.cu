@@ -632,12 +632,12 @@ __global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(con
 
 // Halo form (form 2): persistent, weights resident, for 3x3 stride-1 convs with C_in <= 64 (one K chunk) and one N tile of
 // <= 64 channels in the epi_mode == 1 shape (fp16 out, no BN, no residual).  A work item is a 16 x 8 BY-pixel tile of one
-// frame, cut into 2 x BY blocks of 8x8 pixels (one m64 each).  Warpgroup 0 (all 128 threads) stages the item's
-// (8 BY + 2) x 18-pixel halo patch as KC / 8 non-swizzled 8-channel planes [rows][18][8 ch] (16 bytes per pixel; zero
-// outside the image and beyond C_in) with 16-byte cp.async into a ring of patch slots (stage_halo_patch).  Every tap
-// (ky, kx) of a block is then the same K-major operand at start offset (ky * 18 + kx) * 16 bytes (LBO = one plane, SBO =
-// one patch row): one load serves all nine taps.  Consumer warpgroups 1 and 2 take alternate items (ping-pong), so one
-// warpgroup's epilogue overlaps the other's wgmma.
+// frame, cut into 2 x BY blocks of 8x8 pixels (one m64 each).  Lane 0 of the producer warp (warp 8) loads the item's
+// (8 BY + 2) x 18-pixel halo patch as one TMA box of the 5-D patch map (encode_patches) into a ring of patch slots: KC / 8
+// non-swizzled 8-channel planes [rows][18][8 ch] (16 bytes per pixel; TMA zero fill outside the image and beyond C_in).
+// Every tap (ky, kx) of a block is then the same K-major operand at start offset (ky * 18 + kx) * 16 bytes (LBO = one
+// plane, SBO = one patch row): one load serves all nine taps.  Consumer warpgroups 0 and 1 take alternate items
+// (ping-pong), so one warpgroup's epilogue overlaps the other's wgmma.
 // The epilogue runs from registers (halo_block_epilogue): a thread's two accumulator rows are vertically adjacent pixels.  Every
 // output element gets the wgmma products of k_conv_wg -- the same m64nNk16 shape, (filter column, tap, k-step) order and
 // operand values -- and the bias / ReLU / fp16 rounding / 2x2 max of tc_epilogue_cols_fast in the same order, so the
@@ -646,30 +646,6 @@ constexpr int kHaloCols = 18;                                  // 16 output colu
 // 8x8 blocks along y per item: 16x16 px where N <= 32 and N x KC <= 1024, else 16x8 (ptxas: 16x16 at N = 32, KC = 64 spills)
 constexpr int halo_by(int n, int kc) { return n <= 32 && n * kc <= 1024 ? 2 : 1; }
 constexpr int halo_plane(int n, int kc) { return (8 * halo_by(n, kc) + 2) * kHaloCols * 16; }
-// one producer warpgroup (the patch loaders and the bank's TMA) + two consumer warpgroups
-constexpr int kHaloThreads = 384;
-
-// Patch loader of the halo forms (2 and 3): loader thread `lid` of `n_loaders` issues its share of the 16-byte cp.async
-// that stage one halo patch -- the rows x 18 pixels of frame b from (ys, xs) (zero outside the image), channels
-// [c0, c0 + 8 NP) as NP planes [rows][18][8 ch] of `plane` bytes from shared address `dst` (zero beyond C_in).  Piece
-// (patch pixel p, plane pl) is taken by the thread with lid = (NP p + pl) mod n_loaders, plane fastest: a warp instruction
-// reads 32 / NP whole pixels.  n_loaders must be a multiple of NP, so each thread keeps one plane.  Completion is the
-// caller's: one cp.async.mbarrier.arrive per loader thread.
-template <int NP>
-__device__ __forceinline__ void stage_halo_patch(const TcParams& P, uint32_t dst, int plane, int rows, int c0, int b, int ys, int xs,
-                                                 int lid, int n_loaders) {
-  const __half* in = reinterpret_cast<const __half*>(P.in);
-  const int pl = lid % NP, c = c0 + pl * 8;
-  const bool c_ok = c < P.in_C;
-  const __half* in_c = in + (size_t)b * P.H * P.W * P.in_Ctot + c;
-  const uint32_t d = dst + (uint32_t)(pl * plane);
-  for (int p = lid / NP; p < rows * kHaloCols; p += n_loaders / NP) {
-    const int y = ys + p / kHaloCols, x = xs + p % kHaloCols;
-    const bool ok = c_ok && y >= 0 && y < P.H && x >= 0 && x < P.W;
-    const __half* src = ok ? in_c + ((size_t)y * P.W + x) * P.in_Ctot : in;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d + (uint32_t)(p * 16)), "l"(src), "r"(ok ? 16 : 0) : "memory");
-  }
-}
 
 // lane t of each quad holds piece k of chunks 0..3 in v[k]; afterwards it holds pieces 0..3 of chunk t (two xor stages)
 __device__ __forceinline__ void quad_transpose(uint32_t& v0, uint32_t& v1, uint32_t& v2, uint32_t& v3, int t) {
@@ -765,13 +741,11 @@ __device__ __forceinline__ void halo_block_epilogue(const TcParams& P, const flo
 }
 
 template <int KSTEPS, int N>
-__global__ void __launch_bounds__(kHaloThreads, 1) k_conv_wg_h(const __grid_constant__ CUtensorMap mapA,
+__global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_constant__ CUtensorMap mapA,
                                                                const __grid_constant__ CUtensorMap mapB,
                                                                const __grid_constant__ TcParams P) {
   constexpr int BY = halo_by(N, 16 * KSTEPS), NB = 2 * BY;                  // blocks per item: 2 along x, BY along y
-  constexpr int NP = 2 * KSTEPS;                               // 8-channel planes of the chunk
-  constexpr int PH = 8 * BY + 2, PW = kHaloCols, PLANE = halo_plane(N, 16 * KSTEPS), SLOT = NP * PLANE;
-  constexpr int kLoaders = kHaloThreads - kConsumerThreads;
+  constexpr int PW = kHaloCols, PLANE = halo_plane(N, 16 * KSTEPS), SLOT = 2 * KSTEPS * PLANE;   // KC / 8 planes
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* bank = base;                                        // 9 weight slices, swizzled as in k_conv_wg_p
@@ -786,39 +760,39 @@ __global__ void __launch_bounds__(kHaloThreads, 1) k_conv_wg_h(const __grid_cons
   const int n_work = n_tiles * P.batch;
   for (int i = threadIdx.x; i < N; i += blockDim.x) s_bias[i] = (P.bias && i < P.Cout) ? P.bias[i] : 0.f;
   if (threadIdx.x == 0) {
-    // full: one cp.async arrival per loader thread; empty: one arrival per warp of the consuming warpgroup
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(full + i), kLoaders); mbar_init(smem_u32(empty + i), 4); }
+    // full: the producer's expect_tx arrival + the box's bytes; empty: one arrival per warp of the consuming warpgroup
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(full + i), 1); mbar_init(smem_u32(empty + i), 4); }
     mbar_init(smem_u32(fullB), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
   }
   __syncthreads();
 
-  if (warp < kLoaders / 32) {
-    // ------------------------------ producer warpgroup ------------------------------
-    if (threadIdx.x == 0) {
+  if (warp == kConsumerThreads / 32) {
+    // ------------------------------ producer warp ------------------------------
+    if (lane == 0) {
       // weights are static: load the bank (slice kx * 3 + ky = filter tap (ky, kx)) while the predecessor drains
       mbar_expect_tx(smem_u32(fullB), (uint32_t)(9 * P.b_tx_bytes));
       for (int kx = 0; kx < 3; ++kx)
         for (int ky = 0; ky < 3; ++ky)
           tma_load_3d(smem_u32(bank + (size_t)(kx * 3 + ky) * P.b_slot_bytes), &mapB, smem_u32(fullB), 0, 0, ky * 3 + kx);
+      griddep_wait();                                          // activations come from the previous kernel of the stream
+      for (int i = 0, w = blockIdx.x; w < n_work; ++i, w += gridDim.x) {
+        if (w + (int)gridDim.x >= n_work) griddep_launch();    // last item of this CTA
+        const int s = i % P.n_a_slots;
+        mbar_wait(smem_u32(empty + s), ((i / P.n_a_slots) & 1) ^ 1);
+        const int tile = w % n_tiles, b = w / n_tiles;
+        mbar_expect_tx(smem_u32(full + s), (uint32_t)SLOT);      // zero-filled bytes count too
+        tma_load_5d(smem_u32(ring + (size_t)s * SLOT), &mapA, smem_u32(full + s), 0, (tile % tiles_x) * 16 - 1,
+                    (tile / tiles_x) * (8 * BY) - 1, 0, b);
+      }
     }
-    griddep_wait();                                            // activations come from the previous kernel of the stream
-    for (int i = 0, w = blockIdx.x; w < n_work; ++i, w += gridDim.x) {
-      if (w + (int)gridDim.x >= n_work) griddep_launch();      // last item of this CTA
-      const int s = i % P.n_a_slots;
-      mbar_wait(smem_u32(empty + s), ((i / P.n_a_slots) & 1) ^ 1);
-      const int tile = w % n_tiles, b = w / n_tiles;
-      stage_halo_patch<NP>(P, smem_u32(ring + (size_t)s * SLOT), PLANE, PH, 0, b, (tile / tiles_x) * (8 * BY) - 1,
-                           (tile % tiles_x) * 16 - 1, threadIdx.x, kLoaders);
-      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(full + s)) : "memory");
-    }
-    asm volatile("cp.async.wait_all;" ::: "memory");
     return;
   }
 
   // ------------------------------ consumers: warpgroup wg takes the CTA's items wg, wg + 2, ... ------------------------------
-  const int wg = (warp >> 2) - 1, q = warp & 3, g = lane >> 2, t = lane & 3;
+  const int wg = warp >> 2, q = warp & 3, g = lane >> 2, t = lane & 3;
   const float lo = P.relu ? 0.f : -INFINITY;
   const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
   const uint64_t desc_b = make_desc(0, P.row_bytes, P.layout_type);
@@ -828,7 +802,6 @@ __global__ void __launch_bounds__(kHaloThreads, 1) k_conv_wg_h(const __grid_cons
   for (int i = wg, w = blockIdx.x + wg * (int)gridDim.x; w < n_work; i += 2, w += 2 * (int)gridDim.x) {
     const int s = i % P.n_a_slots;
     mbar_wait(smem_u32(full + s), (i / P.n_a_slots) & 1);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async writes (generic proxy) -> wgmma operand reads
     const uint32_t a_base = smem_u32(ring + (size_t)s * SLOT);
     wgmma_fence();
 #pragma unroll
@@ -868,23 +841,21 @@ __global__ void __launch_bounds__(kHaloThreads, 1) k_conv_wg_h(const __grid_cons
 // here a work item is 16 x 8 BY output pixels x one N tile (N <= 128) x one frame, cut into 2 x BY blocks of 8x8 pixels,
 // and both consumer warpgroups (BY blocks each) read every weight slice, so one L2 read of a slice feeds 256 (N > 64) or
 // 512 (N <= 64) pixels.  K = 9 taps x C_in runs in chunks of 64 input channels (the last zero-filled beyond C_in).
-//   warpgroup 0 (registers cut to 56): warps 0, 2, 3 stage one halo patch per (item, chunk) in form 2's layout (8 non-swizzled
-//     8-channel planes [8 BY + 2][18][8], 16-byte cp.async, zero outside the image and beyond C_in; form 2's loader,
-//     stage_halo_patch) into a ring of patch slots; lane 0 of warp 1 streams the [N x 64] weight slices (SW128, TMA) in
-//     (chunk, filter column, tap) order into a ring of weight slots.  The weights never wait on the grid dependency, so the first ring is in flight while the
-//     predecessor drains.
+//   warpgroup 0 (registers cut to 56): lane 0 of warp 0 loads one halo patch per (item, chunk) in form 2's layout (8
+//     non-swizzled 8-channel planes [8 BY + 2][18][8], one TMA box of the 5-D patch map, zero outside the image and beyond
+//     C_in) into a ring of patch slots; lane 0 of warp 1 streams the [N x 64] weight slices (SW128, TMA) in (chunk, filter
+//     column, tap) order into a ring of weight slots.  The weights never wait on the grid dependency, so the first ring is
+//     in flight while the predecessor drains.
 //   warpgroups 1, 2 (registers raised to 224): per weight slice, m64nNk16 wgmma over all k-steps and the warpgroup's
 //     blocks as one group; a slice's slot is released (one arrival per consumer warp, 8 in all) once the next slice's
 //     group is issued and its own has completed, a patch slot after the chunk's last slice.  Then the register epilogue of
 //     form 2 (halo_block_epilogue), for channels [n0, n0 + N).
 // Every output element gets the wgmma products of k_conv_wg -- the (chunk, filter column, tap, k-step) order on the same
 // operand values -- and form 2's epilogue arithmetic, so the outputs are bit-identical to forms 0, 1 and 2.
-// The CTA starts with 168 registers per thread (the cap for 384 threads); the consumers can only take what the producer
-// warpgroup gives back: 128 x (168 - 56) = 256 x (224 - 168).  (56 / 224 rather than 40 / 232: at 40 the patch loader spills.)
+// The 128 accumulators of a consumer thread need more than the 168 registers per thread that any CTA of more than 8 warps
+// gets at one CTA per SM (a quarter of the register file holds at most 3 warps of 170).  So the CTA is three warpgroups,
+// and the consumers take what the producer warpgroup gives back: 128 x (168 - 56) = 256 x (224 - 168).
 constexpr int kWideThreads = 384;
-// threads of the producer warpgroup that stage patches (warps 0, 2 and 3; one warp alone issues the ~2600 16-byte
-// copies of a 64-channel patch too slowly to keep up with the MMAs)
-constexpr int kWidePatchLoaders = 96;
 constexpr int wide_by(int n) { return n <= 64 ? 4 : 2; }       // 8x8 block rows per item: 128 accumulators per consumer thread
 constexpr int wide_plane(int n) { return (8 * wide_by(n) + 2) * kHaloCols * 16; }
 
@@ -892,7 +863,7 @@ template <int N>
 __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_constant__ CUtensorMap mapA,
                                                                 const __grid_constant__ CUtensorMap mapB,
                                                                 const __grid_constant__ TcParams P) {
-  constexpr int BY = wide_by(N), NP = 8, PH = 8 * BY + 2, PW = kHaloCols, PLANE = wide_plane(N), SLOT = NP * PLANE;
+  constexpr int BY = wide_by(N), PW = kHaloCols, PLANE = wide_plane(N), SLOT = 8 * PLANE;
   constexpr int WSLOT = N * 128;                               // one [N x 64-channel] weight slice
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -910,10 +881,11 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
   const int n_nt = P.Cout / N, n_work = n_nt * n_pt * P.batch;
   for (int i = threadIdx.x; i < P.Cout; i += blockDim.x) s_bias[i] = P.bias ? P.bias[i] : 0.f;
   if (threadIdx.x == 0) {
-    // full: one cp.async arrival per patch loader thread / one TMA transaction; empty: one arrival per consumer warp
-    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(pfull + i), kWidePatchLoaders); mbar_init(smem_u32(pempty + i), 8); }
+    // full: the producer's expect_tx arrival + the box's bytes; empty: one arrival per consumer warp
+    for (int i = 0; i < P.n_a_slots; ++i) { mbar_init(smem_u32(pfull + i), 1); mbar_init(smem_u32(pempty + i), 8); }
     for (int i = 0; i < P.n_b_slots; ++i) { mbar_init(smem_u32(wfull + i), 1); mbar_init(smem_u32(wempty + i), 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
   }
   __syncthreads();
@@ -921,9 +893,8 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
   if (warp < 4) {
     // ------------------------------ producer warpgroup ------------------------------
     setmaxnreg_dec<56>();
-    if (warp != 1) {
+    if (warp == 0 && lane == 0) {
       griddep_wait();                                          // activations come from the previous kernel of the stream
-      const int pid = (warp == 0 ? 0 : 32 * (warp - 1)) + lane;   // patch loader thread 0..95 (warps 0, 2, 3)
       for (int i = 0, w = blockIdx.x; w < n_work; w += gridDim.x) {
         if (w + (int)gridDim.x >= n_work) griddep_launch();    // last item of this CTA
         const int pt = (w / n_nt) % n_pt, b = w / (n_nt * n_pt);
@@ -931,12 +902,10 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
         for (int ch = 0; ch < P.n_chunks; ++ch, ++i) {
           const int s = i % P.n_a_slots;
           mbar_wait(smem_u32(pempty + s), ((i / P.n_a_slots) & 1) ^ 1);
-          // a warp instruction reads four whole 128-byte pixel runs
-          stage_halo_patch<NP>(P, smem_u32(pring + (size_t)s * SLOT), PLANE, PH, ch * 64, b, ys, xs, pid, kWidePatchLoaders);
-          asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(pfull + s)) : "memory");
+          mbar_expect_tx(smem_u32(pfull + s), (uint32_t)SLOT);   // zero-filled bytes count too
+          tma_load_5d(smem_u32(pring + (size_t)s * SLOT), &mapA, smem_u32(pfull + s), 0, xs, ys, ch * 8, b);
         }
       }
-      asm volatile("cp.async.wait_all;" ::: "memory");
     } else if (warp == 1 && lane == 0) {
       // weights are static: no grid-dependency wait
       for (int j = 0, w = blockIdx.x; w < n_work; w += gridDim.x) {
@@ -968,7 +937,6 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
     int rel_w = -1, rel_p = -1;
     for (int ch = 0; ch < P.n_chunks; ++ch) {
       mbar_wait(smem_u32(pfull + ps), pph);
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async writes (generic proxy) -> wgmma operand reads
       const uint32_t a_base = p_base + (uint32_t)(ps * SLOT);
 #pragma unroll
       for (int kx = 0; kx < 3; ++kx)
@@ -1367,7 +1335,8 @@ struct TcForm {
   int max_ctas;                // persistent forms: CTAs the GPU holds at once
   int n_items;                 // persistent forms: work items per frame
   TcParams P;                  // the launch's parameters with this form's ring sizes and N
-  CUtensorMap mapA, mapB;      // form 3: a [64, N, 1] weight box; form 4: a [64, 16, 17, 1] activation box too
+  // forms 2 and 3: a halo-patch box (encode_patches); form 3: a [64, N, 1] weight box; form 4: a [64, 16, 17, 1] activation box
+  CUtensorMap mapA, mapB;
   TcPhases Q;                  // form 4: the four phases' filter columns and taps
 };
 
@@ -1556,7 +1525,7 @@ static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
     fit_ctas(h, F, 3);
   }
   if (TcForm& F = L.forms[2]; form_kernel(2, P.KC, P.N) && halo_eligible(L)) {
-    F.threads = kHaloThreads;
+    F.threads = kConvThreads;
     for (int na = 8; na >= 4 && !F.ok; --na)
       if (conv_smem_halo(P, na) <= kMaxDynSmem) { F.ok = 1; F.P.n_a_slots = na; F.P.n_b_slots = 9; F.smem = conv_smem_halo(P, na); }
     const int by = halo_by(P.N, P.KC);
@@ -1597,6 +1566,19 @@ static CUresult encode_weights(EncodeTiledFn enc, const SbConvTcPlan* plan, int 
   cuuint32_t es[3] = {1, 1, 1};
   return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)plan->w16, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
              swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// Forms 2 and 3: the input slice as a 5-D map {8 channels, W, H, C_in / 8, frames}, byte strides {C_tot 2, W C_tot 2, 16,
+// H W C_tot 2}, whose box {8, 18, rows, KC / 8, 1} at (0, x - 1, y - 1, c0 / 8, b) is one halo patch: it lands as the
+// KC / 8 planes [rows][18][8 ch] of a patch slot.  Pixels outside the image (SAME padding) and planes beyond C_in (the
+// chunk's zero fill) are out of bounds of the map and zero-filled by TMA.
+static CUresult encode_patches(EncodeTiledFn enc, const TcParams& P, int frames, int rows, CUtensorMap* map) {
+  cuuint64_t dims[5] = {8, (cuuint64_t)P.W, (cuuint64_t)P.H, (cuuint64_t)(P.in_C / 8), (cuuint64_t)frames};
+  cuuint64_t strides[4] = {(cuuint64_t)P.in_Ctot * 2, (cuuint64_t)P.W * P.in_Ctot * 2, 16, (cuuint64_t)P.H * P.W * P.in_Ctot * 2};
+  cuuint32_t box[5] = {8, kHaloCols, (cuuint32_t)rows, (cuuint32_t)(P.KC / 8), 1};
+  cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(P.in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
@@ -1691,9 +1673,15 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   P.n_tiles = (int)L.grid.x;
   setup_forms(h, L, total_steps);
-  if (L.forms[3].ok)
+  if (L.forms[2].ok)
+    if (CUresult r = encode_patches(enc, P, m->B, 8 * halo_by(P.N, KC) + 2, &L.forms[2].mapA); r != CUDA_SUCCESS)
+      return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(patches, halo form) failed: %d", (int)r);
+  if (L.forms[3].ok) {
+    if (CUresult r = encode_patches(enc, P, m->B, 8 * wide_by(L.forms[3].P.N) + 2, &L.forms[3].mapA); r != CUDA_SUCCESS)
+      return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(patches, wide form) failed: %d", (int)r);
     if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, L.forms[3].P.N, &L.forms[3].mapB); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, wide form) failed: %d", (int)r);
+  }
   (dst ? *dst : plan->launches).push_back(L);
   return 0;
 }
