@@ -396,8 +396,31 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
  * sb_tracker_reset between a batch's submit and that point applies before the batch is tracked, and the attached tracker
  * must not be destroyed while a batch is submitted. */
 int sb_topdown_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot);
-int sb_topdown_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+/* model_id: the pipeline's owner -- the centroid model, or the instance model of a ground-truth pipeline. */
+int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                        float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
+
+/* ---- ground-truth centroids ------------------------------------------------------------------------
+ * sleap/nn/inference.py:743-809 CentroidCropGroundTruth.call -> FindInstancePeaks.call (or TopDownMultiClassFindPeaks.call):
+ * the instance step above on centroids the caller supplies.  sb_topdown_configure and sb_topdown_multiclass_configure with
+ * params.centroid_model = -1 configure it: the pipeline belongs to the instance model and is addressed by its id;
+ * `centroid` and `max_instances` are ignored (no top-k); max_centroids_per_frame (K) is the per-frame capacity;
+ * precrop_resize is CentroidCropGroundTruth.input_scale (the multi-class form refuses one other than 0 or 1, as above).
+ * A batch holds at most max_batch x K crops, so the instance network is configured for min(max_crops_per_call,
+ * max_batch x K) crops per chunk.
+ * The pipeline owns two slots of max_batch uint8 frames of H x W x C_in, allocated at configure time.  A configure call
+ * on the instance model drops the pipeline and its submitted batches.
+ * sb_topdown_gt_submit queues one whole step into slot 0 / 1 without waiting on the host: the frames and the centroid
+ * table (B,K,2) (frame coordinates, float32, rows past a frame's count ignored, NaN allowed) with counts (B), each in
+ * [0, K], are copied on a copy stream; the centroids are multiplied by precrop_resize (one float32 multiply), their
+ * values are 1, and the crops, instance network, peaks and records follow as in sb_topdown_submit.  Refused
+ * (SB_ERR_INVALID, nothing queued, the slot stays free): a count outside [0, K], a bad slot or B, a slot whose batch was
+ * not collected.  Results come back through sb_topdown_collect or sb_topdown_multiclass_collect with the instance model's
+ * id (outputs as there, flags all zero), under their rules.  On a ground-truth pipeline sb_infer_topdown*,
+ * sb_topdown_submit, sb_topdown_multiclass_submit and sb_topdown_attach_tracker are refused (SB_ERR_INVALID), and
+ * sb_topdown_gt_submit is refused on a pipeline with a centroid model. */
+int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* frames_host, const float* centroids_host,
+                         const int32_t* counts_host, int B, int slot);
 
 /* ---- top-down multi-class (identity) step ---------------------------------------------------------
  * sleap/nn/inference.py:4139-4210 TopDownMultiClassInferenceModel.call = CentroidCrop.call -> TopDownMultiClassFindPeaks.call
@@ -441,7 +464,8 @@ int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void
 /* The double-buffered form, with the rules of sb_topdown_submit / sb_topdown_collect; outputs as
  * sb_infer_topdown_multiclass (out_class_vectors may be NULL). */
 int sb_topdown_multiclass_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, int B, int slot);
-int sb_topdown_multiclass_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids,
+/* model_id of sb_topdown_multiclass_collect: the pipeline's owner, as for sb_topdown_collect. */
+int sb_topdown_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids,
                                   float* out_centroid_vals, float* out_points, float* out_vals, float* out_class_probs,
                                   int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors);
 /* The same post-processing on caller-supplied crops (no network): confidence maps (n_crops,H,W,n_nodes), optional learned

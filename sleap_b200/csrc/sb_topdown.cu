@@ -13,6 +13,9 @@
 // crops H2D -> instance network (sleap_b200/nn/inference.py CentroidCrop / FindInstancePeaks, kept for the stage-level
 // surface).  A pre-crop resize (CentroidCrop.precrop_resize, :1836-1843) scales the kept centroids in k_td_select and cuts
 // the crops from the resident frames resized on the fly (sbk_crop_resized).
+// Ground-truth centroids (CentroidCropGroundTruth.call, :743-809; centroid_model = -1): the host's centroid table stands
+// in for the centroid stage (k_td_gt_select), and the rest of the step is the same instance stage.  The crop count is
+// known on the host, so sb_topdown_gt_submit queues a whole step without a mid-step synchronise.
 //
 // The head's float64 sums use __dmul_rn / __dadd_rn: this file is built with multiply-add contraction on, and a fused
 // product would round differently from the definition (include/sleap_b200.h).
@@ -59,6 +62,23 @@ __global__ void __launch_bounds__(128) k_td_select(const float* __restrict__ pea
   if (threadIdx.x == 0) {
     sel_count[b] = min(keep, K);
     if (keep > K) atomicOr(&flags[b], SB_FLAG_INSTANCES_TRUNCATED);
+  }
+}
+
+// Ground-truth centroids (CentroidCropGroundTruth.call, :743-809): the first count[b] rows of frame b's K-row table (the
+// host checked count <= K), multiplied by the pre-crop resize `scale` (1: unchanged) with one explicitly rounded
+// multiply, as the layer's float32 multiply; value 1; no top-k, so no truncation flag.
+__global__ void __launch_bounds__(128) k_td_gt_select(const float* __restrict__ table, const int* __restrict__ count, int K, float scale,
+                                                      float* __restrict__ sel_cent, float* __restrict__ sel_val, int* __restrict__ sel_count,
+                                                      int* __restrict__ flags) {
+  const int b = blockIdx.x;
+  const int n = count[b];
+  const size_t o = (size_t)b * K;
+  for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) sel_cent[2 * o + i] = __fmul_rn(table[2 * o + i], scale);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) sel_val[o + i] = 1.f;
+  if (threadIdx.x == 0) {
+    sel_count[b] = n;
+    flags[b] = 0;
   }
 }
 
@@ -348,14 +368,34 @@ struct SbTopdown {
   cudaEvent_t count_ev[2] = {nullptr, nullptr};
   int slot_B[2] = {0, 0}, done_B[2] = {0, 0}, pending = -1;
   unsigned long long slot_seq[2] = {0, 0}, seq = 0;
+  // ground-truth form (sb_topdown_params.centroid_model = -1), held by its instance model.  `frames` stands in for the
+  // centroid model as the step's frame source: a model without a network whose B x H x W x C uint8 frame slots, copy
+  // stream, slot events and per-frame flags (all zero) are allocated at configure time.  gt_cent / gt_count: per slot
+  // the device copy of the batch's centroid table and counts, which k_td_gt_select reads.
+  SbModel* frames = nullptr;
+  float* gt_cent[2] = {nullptr, nullptr};      // [Bmax][K][2]
+  int* gt_count[2] = {nullptr, nullptr};       // [Bmax]
 };
+
+// A ground-truth pipeline's frame source with everything it holds
+static void gt_frames_free(SbModel* f) {
+  if (!f) return;
+  for (int i = 0; i < 2; ++i) {
+    if (f->frames_slot[i]) cudaFree(f->frames_slot[i]);
+    for (cudaEvent_t e : {f->h2d_done_ev[i], f->frames_free_ev[i], f->result_ev[i]}) if (e) cudaEventDestroy(e);
+  }
+  if (f->copy_stream) cudaStreamDestroy(f->copy_stream);
+  if (f->ws.flags) cudaFree(f->ws.flags);
+  delete f;
+}
 
 void sb_topdown_free(SbModel* m) {
   SbTopdown* t = m->td;
   if (!t) return;
   void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
-                 t->offsets, t->total, t->crops, t->dense, t->probs};
+                 t->offsets, t->total, t->crops, t->dense, t->probs, t->gt_cent[0], t->gt_cent[1], t->gt_count[0], t->gt_count[1]};
   for (void* p : dev) if (p) cudaFree(p);
+  gt_frames_free(t->frames);
   for (void* p : {(void*)t->record_host, (void*)t->total_host, (void*)t->count_host, (void*)t->stage[0], (void*)t->stage[1],
                   (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
     if (p) cudaFreeHost(p);
@@ -375,12 +415,14 @@ int precrop_size(sb_handle_s* h, const sb_topdown_params* p, int H, int W, float
   return 0;
 }
 
-// The arguments both top-down configure calls check before anything is dropped
+// The arguments both top-down configure calls check before anything is dropped.  *mc is NULL in the ground-truth form
+// (centroid_model = -1).
 int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, SbModel** mc, SbModel** mi) {
   static const char* const bad_ids = "sb_topdown_configure: bad model ids";
-  *mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
+  const bool gt = p->centroid_model == -1;
+  *mc = gt ? nullptr : chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
   *mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
-  if (!*mc || !*mi || *mc == *mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
+  if ((!gt && !*mc) || !*mi || *mc == *mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
   if (p->crop_size <= 0 || p->max_centroids_per_frame <= 0 || p->max_crops_per_call <= 0 || max_batch <= 0)
     return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: bad sizes");
   if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_configure: more than 1024 frames per batch");
@@ -391,20 +433,48 @@ int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   return precrop_size(h, p, H, W, &s, &Hr, &Wr);
 }
 
+// The ground-truth form's frame source (SbTopdown::frames) and centroid staging for batches of up to Bmax frames
+int gt_alloc(sb_handle_s* h, SbTopdown* t, int H, int W, int C_in) {
+  SbModel* f = t->frames = new SbModel();
+  f->B = t->Bmax; f->Hin = H; f->Win = W; f->Cin = C_in;
+  SB_CUDA(h, cudaStreamCreateWithFlags(&f->copy_stream, cudaStreamNonBlocking));
+  int rc = sb_dev_alloc(h, &f->ws.flags, (size_t)t->Bmax);
+  for (int i = 0; i < 2 && !rc; ++i) {
+    for (cudaEvent_t* e : {&f->h2d_done_ev[i], &f->frames_free_ev[i], &f->result_ev[i]})
+      SB_CUDA(h, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    uint8_t* fr = nullptr;
+    if ((rc = sb_dev_alloc(h, &fr, (size_t)t->Bmax * H * W * C_in)) || (rc = sb_dev_alloc(h, &t->gt_cent[i], (size_t)t->Bmax * t->K * 2)) ||
+        (rc = sb_dev_alloc(h, &t->gt_count[i], (size_t)t->Bmax)))
+      break;
+    f->frames_slot[i] = fr;
+  }
+  return rc;
+}
+
 // Configures both networks and their chains, then the pipeline with a record of `width` floats per frame (the centroid
-// configure drops the previous pipeline).  On success mc->td is the new pipeline.
+// configure drops the previous pipeline).  On success mc->td is the new pipeline; in the ground-truth form (mc NULL), with
+// the instance network only, mi->td (the global configure dropped the previous one).
 int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in, SbModel* mc, SbModel* mi,
                   int n_classes) {
   SB_CUDA(h, cudaSetDevice(h->device));
   int rc;
-  if ((rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in))) return rc;
-  if ((rc = sb_model_configure(h, p->instance_model, p->max_crops_per_call, p->crop_size, p->crop_size, C_in))) return rc;
-  if ((rc = sb_centroid_configure(h, p->centroid_model, &p->centroid))) return rc;
+  if (mc && (rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in))) return rc;
+  // the instance network runs chunks of up to max_crops_per_call crops; a ground-truth batch has at most max_batch x K
+  // crops, so that form plans it for no more than those
+  const int chunk = mc ? p->max_crops_per_call
+                       : (int)std::min<long long>(p->max_crops_per_call, (long long)max_batch * p->max_centroids_per_frame);
+  if ((rc = sb_model_configure(h, p->instance_model, chunk, p->crop_size, p->crop_size, C_in))) return rc;
+  if (mc && (rc = sb_centroid_configure(h, p->centroid_model, &p->centroid))) return rc;
   if ((rc = sb_global_configure(h, p->instance_model, &p->instance))) return rc;
   SbTopdown* t = new SbTopdown();
-  mc->td = t;
+  SbModel* owner = mc ? mc : mi;
+  owner->td = t;
   t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
-  t->gen_c = mc->chain_gen; t->gen_i = mi->chain_gen;
+  t->gen_c = mc ? mc->chain_gen : 0; t->gen_i = mi->chain_gen;
+  if (!mc && (rc = gt_alloc(h, t, H, W, C_in))) {
+    sb_topdown_free(owner);
+    return rc;
+  }
   precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by check_topdown
   t->nodes = mi->buffers[p->instance.cms_buffer].C;
   t->multiclass = n_classes > 0;
@@ -416,24 +486,45 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
                   A((void**)&t->offsets, ((size_t)max_batch + 1) * 4) && A((void**)&t->total, 4) &&
                   A((void**)&t->ipts, N * t->nodes * 2 * 4) && A((void**)&t->ivals, N * t->nodes * 4) &&
                   A((void**)&t->record, (size_t)max_batch * t->width * 4) &&
-                  A(&t->crops, (size_t)p->max_crops_per_call * p->crop_size * p->crop_size * C_in * 4) &&
+                  A(&t->crops, (size_t)chunk * p->crop_size * p->crop_size * C_in * 4) &&
                   (!t->multiclass || A((void**)&t->probs, N * n_classes * 4));
   if (!ok || cudaHostAlloc((void**)&t->record_host, (size_t)max_batch * t->width * 4, cudaHostAllocDefault) != cudaSuccess ||
       cudaHostAlloc((void**)&t->total_host, 4, cudaHostAllocDefault) != cudaSuccess) {
-    sb_topdown_free(mc);
+    sb_topdown_free(owner);
     return sb_fail(h, SB_ERR_CUDA, "sb_topdown_configure: allocation failed");
   }
   return SB_OK;
 }
 
-// The pipeline of centroid model `id` when it is of the wanted form and neither model was reconfigured since.  `streamed`:
-// the refusal of the wrong form names the submit call rather than the synchronous one.
-SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = false) {
+// The centroid sources a call takes: a centroid model, ground-truth centroids (sb_topdown_gt_submit)
+enum { TD_MODEL = 1, TD_GT = 2 };
+
+// The pipeline of model `id` (its centroid model, or the instance model of a ground-truth pipeline) when it is of the
+// wanted form and no model of it was reconfigured since.  `streamed`: the refusal of the wrong form names the submit
+// call rather than the synchronous one.  `sources`: the TD_* forms the call takes.
+SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = false, int sources = TD_MODEL) {
   static const char* const none = "top-down pipeline not configured";
   SbModel* mc = chain_model(h, id, SB_CHAIN_ANY, none);
   if (!mc) return nullptr;
   SbTopdown* t = mc->td;
   if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
+  if (!(sources & (t->frames ? TD_GT : TD_MODEL))) {
+    if (t->frames)
+      sb_fail(h, SB_ERR_INVALID, "top-down pipeline takes ground-truth centroids: call sb_topdown_gt_submit");
+    else
+      sb_fail(h, SB_ERR_INVALID, "top-down pipeline runs a centroid model: call %s",
+              multiclass ? "sb_topdown_multiclass_submit" : "sb_topdown_submit");
+    return nullptr;
+  }
+  if (t->frames) {
+    // the instance model holds the pipeline: a configure call on it dropped the pipeline with its chain
+    if (t->multiclass != multiclass) {
+      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_collect"
+                                            : "top-down pipeline is multi-class: call sb_topdown_multiclass_collect");
+      return nullptr;
+    }
+    return t;
+  }
   if (t->multiclass != multiclass) {
     if (streamed)
       sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_submit"
@@ -460,6 +551,14 @@ int check_idle(sb_handle_s* h, const SbTopdown* t, const char* what) {
   return 0;
 }
 
+// The flat crop list and crop offsets of the B frames' selected centroids, on the handle's stream
+int flatten(sb_handle_s* h, SbTopdown* t, int B) {
+  k_td_flatten<<<1, 256, 0, h->stream>>>(t->sel_cent, t->sel_count, B, t->K, (float)t->p.crop_size * 0.5f, t->flat_cent, t->flat_off,
+                                         t->flat_sample, t->offsets, t->total);
+  SB_CHECK_LAUNCH(h);
+  return 0;
+}
+
 // The centroid stage of B frames resident at frames_dev: centroid network, local peaks, top-k, the flat crop list, then
 // the crop count's copy into *count_host and, given, count_ev.
 int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int* count_host,
@@ -475,9 +574,7 @@ int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
   k_td_select<<<B, 128, 0, s>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->scale, t->sel_cent,
                                 t->sel_val, t->sel_count, mc->ws.flags);
   SB_CHECK_LAUNCH(h);
-  k_td_flatten<<<1, 256, 0, s>>>(t->sel_cent, t->sel_count, B, t->K, (float)t->p.crop_size * 0.5f, t->flat_cent, t->flat_off,
-                                 t->flat_sample, t->offsets, t->total);
-  SB_CHECK_LAUNCH(h);
+  if ((rc = flatten(h, t, B))) return rc;
   SB_CUDA(h, cudaMemcpyAsync(count_host, t->total, 4, cudaMemcpyDeviceToHost, s));
   if (count_ev) SB_CUDA(h, cudaEventRecord(count_ev, s));
   return 0;
@@ -622,6 +719,45 @@ int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, in
   return SB_OK;
 }
 
+// Streamed batch with ground-truth centroids into `slot`, the whole step queued at once (the host knows the crop count):
+// the frames, then the centroid table and counts, on the frame source's copy stream into the slot; k_td_gt_select and
+// the crop list behind that copy on the handle's stream; then the instance stage.  The table has its own per-slot
+// staging: the batch before may still be reading the selection buffers when the copy lands.
+int topdown_gt_submit(sb_handle_s* h, SbTopdown* t, const uint8_t* frames_host, const float* centroids_host, const int32_t* counts_host,
+                      int B, int slot) {
+  SbModel* f = t->frames;
+  if (slot < 0 || slot > 1 || !frames_host || !centroids_host || !counts_host || B <= 0 || B > t->Bmax)
+    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: bad slot / batch");
+  if (t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: slot %d holds a batch that was not collected", slot);
+  int total = 0;
+  for (int b = 0; b < B; ++b) {
+    if (counts_host[b] < 0 || counts_host[b] > t->K)
+      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: frame %d has %d centroids, not 0 to %d (max_centroids_per_frame)", b,
+                     counts_host[b], t->K);
+    total += counts_host[b];
+  }
+  SB_CUDA(h, cudaSetDevice(h->device));
+  int rc = stream_alloc(h, t);
+  if (rc || (rc = sb_slot_upload(h, f, frames_host, B, slot))) return rc;
+  SB_CUDA(h, cudaMemcpyAsync(t->gt_cent[slot], centroids_host, (size_t)B * t->K * 2 * sizeof(float), cudaMemcpyHostToDevice, f->copy_stream));
+  SB_CUDA(h, cudaMemcpyAsync(t->gt_count[slot], counts_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, f->copy_stream));
+  SB_CUDA(h, cudaEventRecord(f->h2d_done_ev[slot], f->copy_stream));
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, f->h2d_done_ev[slot], 0));
+  k_td_gt_select<<<B, 128, 0, h->stream>>>(t->gt_cent[slot], t->gt_count[slot], t->K, t->scale, t->sel_cent, t->sel_val, t->sel_count,
+                                           f->ws.flags);
+  SB_CHECK_LAUNCH(h);
+  if ((rc = flatten(h, t, B)) ||
+      (rc = instance_stage(h, f, t, f->frames_slot[slot], 1, B, total, t->stage[slot], nullptr, t->probs_stage[slot], f->frames_free_ev[slot])))
+    return rc;
+  SB_CUDA(h, cudaEventRecord(f->result_ev[slot], h->stream));
+  f->slot_used[slot] = true;
+  t->slot_B[slot] = B; t->done_B[slot] = 0; t->slot_seq[slot] = ++t->seq;
+  return SB_OK;
+}
+
+// The model whose frame slots and slot events a streamed batch of pipeline `t` (held by model `id`) uses
+SbModel* step_frames(sb_handle_s* h, int id, SbTopdown* t) { return t->frames ? t->frames : h->models[id]; }
+
 // The streamed batch of `slot` in its pinned staging: its instance stage queued if still pending, then its record event
 // waited for.  The slot is free again afterwards.
 int topdown_collect(sb_handle_s* h, SbModel* mc, SbTopdown* t, int slot, int B) {
@@ -699,13 +835,22 @@ int sb_topdown_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frame
   return topdown_submit(h, centroid_model_id, frames_host, B, slot, false);
 }
 
-int sb_topdown_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                        float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
+  SbTopdown* t = topdown_of(h, model_id, false, true, TD_MODEL | TD_GT);
   if (!t) return SB_ERR_INVALID;
-  if (const int rc = topdown_collect(h, h->models[centroid_model_id], t, slot, B)) return rc;
+  if (const int rc = topdown_collect(h, step_frames(h, model_id, t), t, slot, B)) return rc;
   split_topdown(t, t->stage[slot], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
   return SB_OK;
+}
+
+int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* frames_host, const float* centroids_host,
+                         const int32_t* counts_host, int B, int slot) {
+  const SbModel* mi = chain_model(h, instance_model_id, SB_CHAIN_ANY, "top-down pipeline not configured");
+  if (!mi) return SB_ERR_INVALID;
+  SbTopdown* t = topdown_of(h, instance_model_id, mi->td && mi->td->multiclass, true, TD_GT);
+  if (!t) return SB_ERR_INVALID;
+  return topdown_gt_submit(h, t, frames_host, centroids_host, counts_host, B, slot);
 }
 
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w) {
@@ -766,14 +911,15 @@ int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_p
   if ((rc = head_from_params(h, p, Hnet / tb.stride_den, Wnet / tb.stride_den, p->tap_channels, d))) return rc;
   // arguments checked: from here the previous chains are dropped
   if ((rc = topdown_setup(h, &p->topdown, max_batch, H, W, C_in, mc, mi, p->n_classes))) return rc;
-  SbTopdown* t = mc->td;
+  SbModel* owner = mc ? mc : mi;
+  SbTopdown* t = owner->td;
   t->head = d;
   t->tap_buf = p->tap_buffer; t->tap_coff = p->tap_channel_offset; t->tap_hi = p->tap_planes == 3 ? p->tap_channels : 0;
   t->tap_half = half;
   t->all_stores = mi->buf_elided[p->tap_buffer] != 0;       // the rule sb_model_forward follows
   if (cudaMalloc((void**)&t->dense, (size_t)p->n_dense_weights * 4) != cudaSuccess ||
       cudaMemcpy(t->dense, p->dense_weights, (size_t)p->n_dense_weights * 4, cudaMemcpyHostToDevice) != cudaSuccess) {
-    sb_topdown_free(mc);
+    sb_topdown_free(owner);
     return sb_fail(h, SB_ERR_CUDA, "sb_topdown_multiclass_configure: dense weights");
   }
   t->head.w = t->dense;
@@ -797,12 +943,12 @@ int sb_topdown_multiclass_submit(sb_handle_t h, int centroid_model_id, const uin
   return topdown_submit(h, centroid_model_id, frames_host, B, slot, true);
 }
 
-int sb_topdown_multiclass_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+int sb_topdown_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                                   float* out_points, float* out_vals, float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags,
                                   float* out_class_vectors) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, true, true);
+  SbTopdown* t = topdown_of(h, model_id, true, true, TD_MODEL | TD_GT);
   if (!t) return SB_ERR_INVALID;
-  if (const int rc = topdown_collect(h, h->models[centroid_model_id], t, slot, B)) return rc;
+  if (const int rc = topdown_collect(h, step_frames(h, model_id, t), t, slot, B)) return rc;
   split_topdown_multiclass(t, t->stage[slot], t->probs_stage[slot], B, out_centroids, out_centroid_vals, out_points, out_vals,
                            out_class_probs, out_n_valid, out_flags, out_class_vectors);
   return SB_OK;

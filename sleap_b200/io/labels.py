@@ -370,11 +370,19 @@ class LabelsReader:
     def videos(self):
         return self.labels.videos
 
+    def _instances(self, lf):
+        return lf.user_instances if self.user_instances_only else lf.instances
+
+    def max_instance_count(self) -> int:
+        """The most instances (= ground-truth centroids) of any frame the reader yields, read from the labels alone:
+        no frame is decoded."""
+        return max([len(self._instances(self.labels[i])) for i in self.indices()] + [0])
+
     def example(self, ind: int) -> dict:
         lf = self.labels[ind]
         video = self.labels.video(lf.video, self.video_search)
         img = video.get_frame(lf.frame_idx)
-        insts = lf.user_instances if self.user_instances_only else lf.instances
+        insts = self._instances(lf)
         n_nodes = len(self.labels.skeleton) if self.labels.skeletons else (insts[0].points.shape[0] if insts else 0)
         pts = np.stack([i.numpy() for i in insts]) if insts else np.zeros((0, n_nodes, 2), np.float32)
         ex = {"image": img, "raw_image_size": np.asarray(img.shape, np.int32), "example_ind": np.int64(ind),

@@ -8,6 +8,7 @@ Kept surface (same names / attributes / dict contract, NumPy in and out):
   BottomUpPredictor (:3055-3349), load_model (:4865).
 All tensor work runs on the GPU through libsleapb200 (C-ABI); this file is orchestration only.
 """
+import collections
 import contextlib
 import ctypes
 import json
@@ -81,12 +82,50 @@ class InferenceModel:
             for i in range(0, n, batch_size):
                 yield self.predict_on_batch(np.asarray(imgs[i:i + batch_size]))
             return
-        yield from _pipelined_batches(imgs, batch_size, *stream)
+        batches = ((InferenceLayer._prep(np.asarray(imgs[i:i + batch_size])),) for i in range(0, n, batch_size))
+        yield from _pipelined_batches(batches, *stream)
 
     def _stream(self, first, batch_size):
         """The streamed step for batches of up to ``batch_size`` frames like ``first`` (the first batch, prepped), set
         up for them: (device model, submit call, ``collect(slot, B)`` returning the batch dict), or None for the
         per-batch route."""
+        return None
+
+    def predict_examples(self, examples, batch_size: int, max_centroids: int):
+        """Generator over (example, result dict) for batches of labels examples (dicts with the frames ``image`` and the
+        ground-truth ``centroids``, at most ``max_centroids`` per frame): the batch loop of a predictor fed labels.  A run
+        of batches whose frames the model's ground-truth step takes (``_stream_ground_truth``) is double-buffered as
+        predict_batches is; other batches take one predict_on_batch each."""
+        it = iter(examples)
+        ex = next(it, None)
+        while ex is not None:
+            first = InferenceLayer._prep(ex["image"])
+            got = self._stream_ground_truth(first, batch_size, max_centroids)
+            if got is None:
+                yield ex, self.predict_on_batch(ex)
+                ex = next(it, None)
+                continue
+            stream, K = got
+            order, rest = collections.deque(), []
+
+            def run(ex=ex):                   # the examples up to the first with other frames, as submit arguments
+                while ex is not None:
+                    imgs = InferenceLayer._prep(ex["image"])
+                    if imgs.shape[1:] != first.shape[1:] or imgs.dtype != first.dtype:
+                        rest.append(ex)
+                        return
+                    order.append(ex)
+                    yield (imgs,) + _centroid_table(ex["centroids"], K)
+                    ex = next(it, None)
+
+            for out in _pipelined_batches(run(), *stream):
+                yield order.popleft(), out
+            ex = rest[0] if rest else None
+
+    def _stream_ground_truth(self, first, batch_size, max_centroids):
+        """The streamed ground-truth step for batches of up to ``batch_size`` labels examples with frames like ``first``
+        (prepped) and up to ``max_centroids`` centroids per frame, set up for them: ((device model, submit call,
+        ``collect(slot, B)``), K of the centroid tables it takes), or None for the per-batch route."""
         return None
 
 
@@ -377,6 +416,7 @@ class CentroidCropGroundTruth:
         self.input_scale = input_scale
         self.handle = handle
         self._resizer = None
+        self._pipeline = None        # the fused step's pipeline (_configure_ground_truth)
 
     def call(self, example_gt):
         from sleap_b200 import _lib
@@ -480,6 +520,61 @@ def _configure_topdown(cc, fp, fn_name, p, shape, *arrays):
         mc.chain = mi.chain = record
 
 
+def _centroid_table(centroids, K):
+    """The ragged ground-truth centroids of a batch (one (n, 2) array per frame) as sb_topdown_gt_submit takes them: the
+    (B, K, 2) float32 table, NaN past each frame's count, and the (B,) int32 counts.  A frame with more than K centroids
+    keeps its count, so the submit refuses the batch rather than dropping centroids."""
+    cents = [f32(c).reshape(-1, 2) for c in centroids]
+    counts = np.asarray([len(c) for c in cents], np.int32)
+    table = np.full((len(cents), K, 2), np.nan, np.float32)
+    for b, c in enumerate(cents):
+        table[b, :len(c)] = c[:K]
+    return table, counts
+
+
+def _call_ground_truth(im, example):
+    """One batch of top-down model ``im`` with ground-truth centroids (uint8 ``image`` and ``centroids``) through its fused
+    step: the table packed for the pipeline's K (grown to the batch's largest count if needed), sb_topdown_gt_submit into
+    slot 0, then the collect."""
+    imgs = InferenceLayer._prep(example["image"])
+    B = imgs.shape[0]
+    n = max([len(f32(c).reshape(-1, 2)) for c in example["centroids"]] + [0])
+    K = im._configure_ground_truth(B, n, imgs.shape[1:])
+    table, counts = _centroid_table(example["centroids"], K)
+    m = im.instance_peaks.keras_model
+    m.handle.call("sb_topdown_gt_submit", m.model_id, ptr(imgs), ptr(table), ptr(counts), B, 0)
+    return im._run_ground_truth(B, K, 0)
+
+
+def _configure_ground_truth(cc, fp, fn_name, make_params, B, K, shape, *arrays):
+    """Configures the ground-truth top-down pipeline (``make_params(K)``: the parameters with centroid_model -1, for
+    ``fn_name``) of ground-truth layer ``cc`` on instance layer ``fp`` for batches of up to B frames of ``shape``
+    (H, W, C) with up to K centroids each, unless it already runs with at least these capacities: B and K grow only when a
+    batch exceeds them.  ``arrays`` are the ones the pointer fields of the parameters point to.  Returns the pipeline's K."""
+    mi = fp.keras_model
+    what = (fn_name, chain_key(make_params(0), *arrays), tuple(shape))     # the pipeline apart from its capacities
+    have = cc._pipeline                      # (what, B, K, the instance model's chain record) of the last configure
+    if have is not None and have[0] == what and mi.chain is have[3]:
+        if B <= have[1] and K <= have[2]:
+            return have[2]
+        B, K = max(B, have[1]), max(K, have[2])
+    K = max(K, 1)
+    p = make_params(K)
+    mi.chain = None                          # a refused call may have dropped the previous chain
+    mi.handle.call(fn_name, byref(p), B, *shape)
+    # the instance network's plan: chunks of max_crops_per_call crops, but no more than a batch's B x K (include/sleap_b200.h)
+    mi.configured_for = (min(fp.max_crops_per_call, B * K), cc.crop_size, cc.crop_size, shape[2])
+    mi.chain = (fn_name, chain_key(p, *arrays))
+    cc._pipeline = (what, B, K, mi.chain)
+    return K
+
+
+def _ground_truth_params(cc, fp, K):
+    """TopdownParams of the ground-truth pipeline of layer ``cc`` on instance layer ``fp`` with K centroids per frame."""
+    return TopdownParams(-1, fp.keras_model.model_id, CentroidParams(), fp.params(), int(cc.crop_size), 0, int(K),
+                         int(fp.max_crops_per_call), float(cc.input_scale))
+
+
 class TopDownInferenceModel(InferenceModel):
     """sleap/nn/inference.py:2246-2311."""
 
@@ -497,9 +592,22 @@ class TopDownInferenceModel(InferenceModel):
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
-        return (self.fused and type(cc) is CentroidCrop and type(fp) is FindInstancePeaks and
-                cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and cc.keras_model.handle is fp.keras_model.handle
-                and fp.keras_model.input_scale == 1.0)
+        if not (self.fused and type(fp) is FindInstancePeaks and not fp.return_confmaps and fp.keras_model.input_scale == 1.0):
+            return False
+        if type(cc) is CentroidCropGroundTruth:
+            return cc.handle is fp.keras_model.handle
+        return (type(cc) is CentroidCrop and cc.return_crops and not cc.return_confmaps
+                and cc.keras_model.handle is fp.keras_model.handle)
+
+    @property
+    def ground_truth(self):
+        """Centroids come from the labels (CentroidCropGroundTruth), not from a centroid model."""
+        return isinstance(self.centroid_crop, CentroidCropGroundTruth)
+
+    def _owner(self):
+        """The device model that holds the fused pipeline: the centroid model, or with ground-truth centroids the
+        instance model."""
+        return self.instance_peaks.keras_model if self.ground_truth else self.centroid_crop.keras_model
 
     def _configure_fused(self, B, H, W, C):
         """The fused pipeline for batches of up to B frames of (H, W, C), with ``self.tracker`` attached (the raw frame
@@ -516,7 +624,7 @@ class TopDownInferenceModel(InferenceModel):
     def _run_fused(self, B, K, fn, *args, slot=-1):
         """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown or sb_topdown_collect) into dense arrays
         of B frames, as a batch dict; with a tracker, the track records of ``slot`` (-1: sb_infer_topdown)."""
-        mc, n_nodes = self.centroid_crop.keras_model, head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
+        mc, n_nodes = self._owner(), head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
@@ -537,18 +645,35 @@ class TopDownInferenceModel(InferenceModel):
 
     def _stream(self, first, batch_size):
         """sb_topdown_submit / sb_topdown_collect (the upload of batch i+1 and its centroid stage are queued before batch
-        i is collected): uint8 frames and a model that can run the fused step."""
-        if not self._can_fuse() or first.dtype != np.uint8:
+        i is collected): uint8 frames and a model that can run the fused step with a centroid model."""
+        if not self._can_fuse() or self.ground_truth or first.dtype != np.uint8:
             return None
         K = self._configure_fused(batch_size, *first.shape[1:])
         return (self.centroid_crop.keras_model, "sb_topdown_submit",
                 lambda slot, B: self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot))
 
+    def _configure_ground_truth(self, B, K, shape):
+        cc, fp = self.centroid_crop, self.instance_peaks
+        return _configure_ground_truth(cc, fp, "sb_topdown_configure", lambda k: _ground_truth_params(cc, fp, k), B, K, shape)
+
+    def _stream_ground_truth(self, first, batch_size, max_centroids):
+        """sb_topdown_gt_submit / sb_topdown_collect: uint8 frames and a model that can run the fused step with
+        ground-truth centroids.  The whole step is queued at the submit."""
+        if not (self._can_fuse() and self.ground_truth) or first.dtype != np.uint8:
+            return None
+        K = self._configure_ground_truth(batch_size, max_centroids, first.shape[1:])
+        return (self.instance_peaks.keras_model, "sb_topdown_gt_submit", lambda slot, B: self._run_ground_truth(B, K, slot)), K
+
+    def _run_ground_truth(self, B, K, slot):
+        return self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot)
+
     def call(self, example):
         if isinstance(example, np.ndarray):
             example = dict(image=example)
-        if self._can_fuse():
+        if self._can_fuse() and not self.ground_truth:
             return self._call_fused(_images_of(example))
+        if self._can_fuse() and "centroids" in example and np.asarray(example["image"]).dtype == np.uint8:
+            return _call_ground_truth(self, example)
         crop_out = self.centroid_crop.call(example)
         if isinstance(self.instance_peaks, FindInstancePeaksGroundTruth):                 # :2300-2304
             peaks_out = self.instance_peaks.call(example, crop_out)
@@ -734,27 +859,33 @@ def bottomup_from_maps(cms, pafs, paf_scorer, cm_output_stride, peak_threshold=0
     return out
 
 
-def _pipelined_batches(imgs, batch_size, m, submit_fn, collect):
+def _pipelined_batches(batches, m, submit_fn, collect):
     """The double-buffered batch loop of the streaming models (uint8 frames, chain configured): batch i+1 is submitted
     (``submit_fn`` of device model ``m``: its upload on the copy stream, network and post-processing queued) into slot
-    (i+1) % 2 before ``collect(slot, B)`` waits for batch i and returns its result dict.  A consumer that stops early (an
-    exception, a closed generator) leaves no batch submitted: the rest are collected and dropped."""
-    starts = list(range(0, len(imgs), batch_size))
-    keep = {}
+    (i+1) % 2 before ``collect(slot, B)`` waits for batch i and returns its result dict.  ``batches`` yields each batch's
+    arrays the submit takes before B: its prepped frames and, for sb_topdown_gt_submit, its centroid table and counts;
+    they are kept alive until the batch is collected.  A batch is drawn from ``batches`` only when it is submitted.  A
+    consumer that stops early (an exception, a closed generator) leaves no batch submitted: the rest are collected and
+    dropped."""
+    it = iter(batches)
+    keep, sizes = {}, {}
 
     def submit(k):
-        batch = InferenceLayer._prep(np.asarray(imgs[starts[k]:starts[k] + batch_size]))
-        keep[k % 2] = batch                       # the async copy reads this host buffer until collect()
-        m.handle.call(submit_fn, m.model_id, ptr(batch), batch.shape[0], k % 2)
-        return batch.shape[0]
+        arrays = next(it, None)
+        if arrays is None:
+            return
+        keep[k % 2] = arrays                      # the async copies read these host buffers until collect()
+        B = arrays[0].shape[0]
+        m.handle.call(submit_fn, m.model_id, *[ptr(a) for a in arrays], B, k % 2)
+        sizes[k] = B
 
-    sizes = {}
     try:
-        sizes[0] = submit(0)
-        for k in range(len(starts)):
-            if k + 1 < len(starts):
-                sizes[k + 1] = submit(k + 1)
+        submit(0)
+        k = 0
+        while k in sizes:
+            submit(k + 1)
             yield collect(k % 2, sizes.pop(k))
+            k += 1
     finally:
         for k in sorted(sizes):
             try:
@@ -1035,9 +1166,16 @@ class TopDownMultiClassInferenceModel(InferenceModel):
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
-        return (self.fused and type(cc) is CentroidCrop and type(fp) is TopDownMultiClassFindPeaks and cc.precrop_resize == 1.0 and
-                cc.return_crops and not cc.return_confmaps and not fp.return_confmaps and fp.optimal_grouping and fp.input_scale == 1.0
-                and fp.keras_model.input_scale == 1.0 and cc.keras_model.handle is fp.keras_model.handle)
+        if not (self.fused and type(fp) is TopDownMultiClassFindPeaks and not fp.return_confmaps and fp.optimal_grouping and
+                fp.input_scale == 1.0 and fp.keras_model.input_scale == 1.0):
+            return False
+        if type(cc) is CentroidCropGroundTruth:
+            return cc.input_scale == 1.0 and cc.handle is fp.keras_model.handle
+        return (type(cc) is CentroidCrop and cc.precrop_resize == 1.0 and cc.return_crops and not cc.return_confmaps
+                and cc.keras_model.handle is fp.keras_model.handle)
+
+    ground_truth = TopDownInferenceModel.ground_truth
+    _owner = TopDownInferenceModel._owner
 
     def _configure_fused(self, B, H, W, C):
         """The fused pipeline for batches of up to B frames of (H, W, C).  Returns (K, n_classes)."""
@@ -1057,7 +1195,7 @@ class TopDownMultiClassInferenceModel(InferenceModel):
     def _run_fused(self, B, K, NC, fn, *args):
         """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown_multiclass or
         sb_topdown_multiclass_collect) into dense arrays of B frames, as a batch dict."""
-        fp, mc = self.instance_peaks, self.centroid_crop.keras_model
+        fp, mc = self.instance_peaks, self._owner()
         N = head_channels(fp.keras_model, fp.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         pts = np.zeros((B, NC, N, 2), np.float32); vals = np.zeros((B, NC, N), np.float32); probs = np.zeros((B, NC), np.float32)
@@ -1073,18 +1211,37 @@ class TopDownMultiClassInferenceModel(InferenceModel):
 
     def _stream(self, first, batch_size):
         """sb_topdown_multiclass_submit / _collect, as TopDownInferenceModel's: uint8 frames and a model that can run the
-        fused step."""
-        if not self._can_fuse() or first.dtype != np.uint8:
+        fused step with a centroid model."""
+        if not self._can_fuse() or self.ground_truth or first.dtype != np.uint8:
             return None
         K, NC = self._configure_fused(batch_size, *first.shape[1:])
         return (self.centroid_crop.keras_model, "sb_topdown_multiclass_submit",
                 lambda slot, B: self._run_fused(B, K, NC, "sb_topdown_multiclass_collect", slot))
 
+    def _configure_ground_truth(self, B, K, shape):
+        cc, fp = self.centroid_crop, self.instance_peaks
+        tap = fp.keras_model.cm.vector_taps[fp.CLASS_VECTORS]
+        return _configure_ground_truth(cc, fp, "sb_topdown_multiclass_configure",
+                                       lambda k: topdown_multiclass_params(_ground_truth_params(cc, fp, k), tap, fp.class_head, fp.dense),
+                                       B, K, shape, fp.dense)
+
+    def _run_ground_truth(self, B, K, slot):
+        return self._run_fused(B, K, head_channels(self.instance_peaks.keras_model, "ClassVectorsHead"), "sb_topdown_multiclass_collect", slot)
+
+    def _stream_ground_truth(self, first, batch_size, max_centroids):
+        """sb_topdown_gt_submit / sb_topdown_multiclass_collect, as TopDownInferenceModel's."""
+        if not (self._can_fuse() and self.ground_truth) or first.dtype != np.uint8:
+            return None
+        K = self._configure_ground_truth(batch_size, max_centroids, first.shape[1:])
+        return (self.instance_peaks.keras_model, "sb_topdown_gt_submit", lambda slot, B: self._run_ground_truth(B, K, slot)), K
+
     def call(self, example):
         if isinstance(example, np.ndarray):
             example = dict(image=example)
-        if self._can_fuse():
+        if self._can_fuse() and not self.ground_truth:
             return self._call_fused(_images_of(example))
+        if self._can_fuse() and "centroids" in example and np.asarray(example["image"]).dtype == np.uint8:
+            return _call_ground_truth(self, example)
         crop_out = self.centroid_crop.call(example)
         out = self.instance_peaks.call(crop_out)
         res = {k: out[k] for k in ("instance_peaks", "instance_peak_vals", "instance_scores")}
@@ -1229,15 +1386,19 @@ class Predictor:
         if isinstance(data, Labels):
             data = LabelsReader(data, with_centroids=True, center_on_part=getattr(self, "anchor_part", None))
         if isinstance(data, LabelsReader):
-            for batch in self._label_examples(data):
-                use_gt = getattr(self, "uses_ground_truth", False)
-                ex = self.inference_model.predict_on_batch(batch if use_gt else batch["image"])
-                ex["frame_ind"], ex["video_ind"] = batch["frame_ind"], batch["video_ind"]
-                ex["image_hw"] = tuple(batch["image"].shape[1:3])
-                if self.tracker is not None and getattr(self.tracker, "uses_image", False):
-                    ex["image"] = batch["image"]
-                self._check_flags(ex)
-                yield ex
+            batches = self._label_examples(data)
+            if getattr(self, "uses_ground_truth", False):     # streamed where the model's ground-truth step takes them
+                results = self.inference_model.predict_examples(batches, self.batch_size, data.max_instance_count())
+            else:
+                results = ((b, self.inference_model.predict_on_batch(b["image"])) for b in batches)
+            with contextlib.closing(results):
+                for batch, ex in results:
+                    ex["frame_ind"], ex["video_ind"] = batch["frame_ind"], batch["video_ind"]
+                    ex["image_hw"] = tuple(batch["image"].shape[1:3])
+                    if self.tracker is not None and getattr(self.tracker, "uses_image", False):
+                        ex["image"] = batch["image"]
+                    self._check_flags(ex)
+                    yield ex
             return
         data = self._as_frames(data)
         feeder = data if isinstance(data, FrameFeeder) else None
@@ -1556,10 +1717,10 @@ class TopDownPredictor(Predictor):
         """As Predictor.predict.  On the fused step (frames in, not ``Labels``), a tracker with ``track_device`` runs
         inside each step (k_track after the record kernel, on the model's GPU); the consumer thread only maps its track
         ids to ``Track`` objects before ``final_pass``.  The tracker's GPU must be the model's, and the run must be on
-        one rank.  Other inputs track on the consumer thread."""
+        one rank.  Other inputs, and ground-truth centroids, track on the consumer thread."""
         from sleap_b200.io.labels import Labels, LabelsReader
         im = self.inference_model
-        if not im._can_fuse() or isinstance(data, (Labels, LabelsReader)):
+        if not im._can_fuse() or im.ground_truth or isinstance(data, (Labels, LabelsReader)):
             return super().predict(data, make_labels)
         with self._tracking_in_step(im, im.centroid_crop.keras_model, make_labels):
             return super().predict(data, make_labels)

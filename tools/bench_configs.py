@@ -3,7 +3,7 @@ JSON line each (frames/s end to end with host frames, CUDA-event timed device lo
 Secondary to bench.py (C4).
 
   python tools/bench_configs.py [c1] [c2] [c3 | topdown] [c5] [r50] [track] [multiclass] [topdown_multiclass] [topdown_scaled]
-                               [topdown_track] [pipeline] [--steps K]
+                               [topdown_gt] [topdown_track] [pipeline] [--steps K]
                                [--c5-batch B]
   (C5 default: 16 frames per GPU and step)
 
@@ -42,6 +42,14 @@ to 512x512 before cropping), three arms alternating in one process on the same 1
 (fused = False: centroids to the host, the frames resized by FrameResizer, crops through host memory), the fused step
 (predict_on_batch: resize and crop inside the step) and the double-buffered loop (predict_batches).  The line reports
 frames/s per arm (median and range over the repetitions) and whether all arms agree bit for bit.
+
+topdown_gt: a top-down predictor with ground-truth centroids (no centroid model: CentroidCropGroundTruth) on synthetic
+labels of 128 frames of 1024x1024 uint8, 5 instances of 13 nodes each, B=16; the instance UNet of the C3 pair at input
+scale 1 (160x160 crops) and at 0.5 (96x96 crops of the half-size frame).  Three arms alternate in one process on the same
+decoded label batches: the staged route (fused = False: FrameResizer, crops through host memory, one synchronous
+sb_infer_global per chunk), the fused step per batch (predict_on_batch: sb_topdown_gt_submit + collect) and the
+double-buffered loop predict runs on labels (predict_examples).  The line reports the card and its power limit, frames/s
+per arm (median and range over the repetitions) and whether all arms agree bit for bit.
 
 topdown_track: the top-down predictor with a tracker, four arms alternating in one process: TopDownPredictor.predict
 (labels made) of the C3 pair on 256 gray tracking-clip frames, B=16, the centroid threshold calibrated on clip frames to
@@ -520,6 +528,64 @@ def topdown_scaled_bench(steps):
             "arms_agree_bitwise": bool(agree)}
 
 
+def topdown_gt_bench(steps):
+    """Ground-truth centroids through the three routes of a TopDownPredictor built from an instance model only (see the
+    module docstring), at input scales 1 and 0.5."""
+    from sleap_b200.io.labels import Instance, LabeledFrame, Labels, LabelsReader, Skeleton
+    from sleap_b200.io.video import Video
+    n, B, animals = 128, 16, 5
+    fr = frames(n, 1024, 1024, 1, 5)
+    rng = np.random.default_rng(7)
+    sk = Skeleton(FLIES13, [])
+    lfs = [LabeledFrame(0, i, [Instance((rng.uniform(80, 944, 2) + rng.normal(0, 20, (13, 2))).astype(np.float32), sk)
+                                for _ in range(animals)]) for i in range(n)]
+    labels = Labels(lfs, [{}], [sk])
+    labels.set_video(0, Video.from_numpy(fr))
+    ispec = dict(backbone="unet", backbone_cfg=dict(unet(24, 16, 4), up_interpolate=False), head_type="centered_instance",
+                 part_names=FLIES13, edges=None, heads=[dict(name="CenteredInstanceConfmapsHead", channels=13, output_stride=4)])
+    keys = ("n_valid", "centroids", "centroid_vals", "instance_peaks", "instance_peak_vals")
+    res = {}
+    for scale, crop in ((1.0, 160), (0.5, 96)):
+        def inference_model(fused):
+            # each arm owns its device model: the staged calls reconfigure the chain the fused pipeline needs
+            im_model = model_for(ispec, 1, 1004)[0]
+            im_model.config_input_scale = scale                          # what Predictor._load(..., resize_in_graph=False) sets
+            pred = TopDownPredictor(None, im_model, crop_size=crop, batch_size=B)
+            pred.inference_model.instance_peaks.peak_threshold = 0.0
+            pred.inference_model.fused = fused
+            return pred
+
+        staged, fused = inference_model(False), inference_model(True)
+        assert not staged.inference_model._can_fuse() and fused.inference_model._can_fuse()
+        reader = LabelsReader(labels, with_centroids=True)
+        batches = list(fused._label_examples(reader))
+        K = reader.max_instance_count()
+        sim, fim = staged.inference_model, fused.inference_model
+        arms = {"staged predict_on_batch (fused = False)": lambda: [sim.predict_on_batch(b) for b in batches],
+                "fused predict_on_batch": lambda: [fim.predict_on_batch(b) for b in batches],
+                "streamed predict_examples": lambda: [o for _, o in fim.predict_examples(batches, B, K)]}
+        outs = {k: f() for k, f in arms.items()}                         # warm-up, and the outputs compared
+        reps = max(5, steps)
+        times = {k: [] for k in arms}
+        for _ in range(reps):                                            # arms alternate
+            for k, f in arms.items():
+                t0 = time.perf_counter()
+                f()
+                times[k].append(time.perf_counter() - t0)
+        ref = outs["staged predict_on_batch (fused = False)"]
+        agree = all(len(o) == len(ref) and all(np.asarray(x[k]).shape == np.asarray(y[k]).shape and
+                                               np.asarray(x[k]).tobytes() == np.asarray(y[k]).tobytes() for x, y in zip(o, ref) for k in keys)
+                    for o in outs.values())
+        assert agree, f"the routes disagree at input scale {scale}"
+        res[f"s={scale:g}, {crop}x{crop} crops"] = {
+            "repetitions": reps, "frames_per_s": {k: n / float(np.median(v)) for k, v in times.items()},
+            "frames_per_s_range": {k: [n / max(v), n / min(v)] for k, v in times.items()},
+            "mean_instances_per_frame": float(np.mean(np.concatenate([o["n_valid"] for o in ref]))), "arms_agree_bitwise": agree}
+    return {"config": "topdown_gt: ground-truth centroids + C3 instance UNet, synthetic labels of 128 1024x1024 uint8 frames, "
+                      "5 instances each, B=16", "gpu": gpu_identity(),
+            "metric": "frames/s (median of alternating repetitions; decoded label batches in, result dicts out)", "workloads": res}
+
+
 def topdown_track_bench(steps):
     """TopDownPredictor.predict (labels made) of the C3 pair of topdown() on 256 tracking-clip frames (gray), B = 16, the
     centroid threshold calibrated on clip frames to about 5 animals per frame.  Four arms alternate in one process: no
@@ -691,6 +757,8 @@ if __name__ == "__main__":
             r = topdown(steps)
         elif c == "topdown_scaled":
             r = topdown_scaled_bench(steps)
+        elif c == "topdown_gt":
+            r = topdown_gt_bench(steps)
         elif c == "r50":
             r = resnet50(steps)
         elif c == "track":
