@@ -214,11 +214,18 @@ int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, i
                       float* out_instance_peaks, float* out_instance_peak_vals,
                       float* out_instance_scores, int32_t* out_n_valid, int32_t* out_flags);
 int sb_infer_bottomup_dev(sb_handle_t h, int model_id, const uint8_t* frames_dev, int B);
-/* Streaming form of sb_infer_bottomup for many batches (sleap/nn/inference.py:377-420, the
+/* Streamed steps.  Streaming form of sb_infer_bottomup for many batches (sleap/nn/inference.py:377-420, the
  * Predictor batch loop): sb_bottomup_submit queues the H2D copy (copy stream), the network and the
  * post-processing of one batch into slot 0/1 and returns; sb_bottomup_collect blocks until that
  * slot's results are in host memory.  Submitting batch i+1 before collecting batch i overlaps its
- * upload with the compute of batch i.  frames_host should be pinned for a truly asynchronous copy. */
+ * upload with the compute of batch i.  frames_host should be pinned for a truly asynchronous copy.
+ * Every *_submit / *_collect pair below (bottom-up, multi-class, global, top-down, top-down identity, ground-truth
+ * top-down) follows these rules.  Refused (SB_ERR_INVALID, nothing queued): a submit with a slot other than 0 / 1 or B
+ * outside [1, max batch]; a submit into a slot whose batch was not collected; a collect of a slot that holds no
+ * batch, with another B than its submit, or before the batch submitted earlier into the other slot.  A slot read
+ * (sb_bottomup_tracks, sb_bottomup_gathered, sb_topdown_tracks with slot 0 / 1) takes only the batch last collected
+ * from that slot, with its B.  A configure call on the model (or either model of a top-down pipeline) drops the
+ * submitted batches after their work has finished; collecting one then fails. */
 int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
 int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out_instance_peaks,
                         float* out_instance_peak_vals, float* out_instance_scores,
@@ -278,7 +285,7 @@ int sb_multiclass_configure(sb_handle_t h, int model_id, const sb_multiclass_par
  * out_class_probs (B,n_classes,n_nodes), out_flags (B) SB_FLAG_* (may be NULL). */
 int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B,
                         float* out_points, float* out_vals, float* out_class_probs, int32_t* out_flags);
-/* The double-buffered form, as sb_bottomup_submit / sb_bottomup_collect (uint8 frames). */
+/* The streamed form, as sb_bottomup_submit / sb_bottomup_collect, with the rules of the streamed steps (uint8 frames). */
 int sb_multiclass_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
 int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals,
                           float* out_class_probs, int32_t* out_flags);
@@ -335,7 +342,7 @@ typedef struct sb_global_params {
 int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* params);
 int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int images_are_u8,
                     int B, const float* crop_offsets_host, float* out_points, float* out_vals);
-/* The double-buffered form, as sb_bottomup_submit / sb_bottomup_collect (uint8 frames, no crop offsets): the global
+/* The streamed form, as sb_bottomup_submit / sb_bottomup_collect (rules, uint8 frames, no crop offsets): the global
  * peaks run on the post-processing stream and the points | values block comes back in one copy per batch. */
 int sb_global_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
 int sb_global_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals);
@@ -382,16 +389,14 @@ int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* params, int max
 int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
                      float* out_centroids, float* out_centroid_vals, float* out_instance_peaks,
                      float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags);
-/* The double-buffered form (uint8 frames; arguments as sb_bottomup_submit / _collect, outputs as sb_infer_topdown).  A
+/* The streamed form (uint8 frames; arguments and rules as sb_bottomup_submit / _collect, outputs as sb_infer_topdown).  A
  * step is a centroid stage (network, peaks, top-k, crop list, the crop count's copy to the host) and an instance stage
  * (crops, instance network, peaks, records, tracker, the records' copy).  sb_topdown_submit queues the batch's upload on
  * a copy stream into slot `slot`, then the instance stage of the batch submitted before it (waiting on the host for that
  * batch's crop count, which its centroid stage produced while the GPU ran it), then the batch's own centroid stage.
  * sb_topdown_collect queues the batch's instance stage if no submit did, and blocks until its records are on the host.
- * Refused (SB_ERR_INVALID): a submit into a slot whose batch was not collected; a collect of a slot that holds no batch,
- * with another B, or before the batch submitted earlier; sb_infer_topdown*, sb_infer_centroids on the centroid model and
+ * Also refused (SB_ERR_INVALID): sb_infer_topdown*, sb_infer_centroids on the centroid model and
  * sb_topdown_attach_tracker while a batch is submitted and not collected; a submit or collect of the other pipeline form.
- * A configure call on either model drops the submitted batches (after their work has finished); collecting one then fails.
  * A batch's instance stage, and with it the attached tracker's step, is queued by the next submit or by its collect:
  * sb_tracker_reset between a batch's submit and that point applies before the batch is tracked, and the attached tracker
  * must not be destroyed while a batch is submitted. */
@@ -408,14 +413,13 @@ int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_
  * precrop_resize is CentroidCropGroundTruth.input_scale (the multi-class form refuses one other than 0 or 1, as above).
  * A batch holds at most max_batch x K crops, so the instance network is configured for min(max_crops_per_call,
  * max_batch x K) crops per chunk.
- * The pipeline owns two slots of max_batch uint8 frames of H x W x C_in, allocated at configure time.  A configure call
+ * The pipeline owns two slots of max_batch uint8 frames of H x W x C_in, allocated at its first submit.  A configure call
  * on the instance model drops the pipeline and its submitted batches.
  * sb_topdown_gt_submit queues one whole step into slot 0 / 1 without waiting on the host: the frames and the centroid
  * table (B,K,2) (frame coordinates, float32, rows past a frame's count ignored, NaN allowed) with counts (B), each in
  * [0, K], are copied on a copy stream; the centroids are multiplied by precrop_resize (one float32 multiply), their
  * values are 1, and the crops, instance network, peaks and records follow as in sb_topdown_submit.  Refused
- * (SB_ERR_INVALID, nothing queued, the slot stays free): a count outside [0, K], a bad slot or B, a slot whose batch was
- * not collected.  Results come back through sb_topdown_collect or sb_topdown_multiclass_collect with the instance model's
+ * (SB_ERR_INVALID, nothing queued, the slot stays free): a count outside [0, K], and as every streamed submit.  Results come back through sb_topdown_collect or sb_topdown_multiclass_collect with the instance model's
  * id (outputs as there, flags all zero), under their rules.  On a ground-truth pipeline sb_infer_topdown*,
  * sb_topdown_submit, sb_topdown_multiclass_submit and sb_topdown_attach_tracker are refused (SB_ERR_INVALID), and
  * sb_topdown_gt_submit is refused on a pipeline with a centroid model. */

@@ -163,7 +163,8 @@ int sb_gather_connect(sb_handle_t h, int model_id, const void* all_ipc_handles) 
   g.connected = true;
   g.step = 0;
   g.consumed = 0;
-  sb_pipeline_slots_free(m);                       // host staging now holds [world][B][width] windows
+  m->slots.release();                              // host staging now holds [world][B][width] windows
+  if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
   return SB_OK;
 }
 

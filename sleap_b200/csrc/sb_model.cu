@@ -55,14 +55,7 @@ void sb_models_free(sb_handle_s* h) {
     if (m->rec_host) cudaFreeHost(m->rec_host);
     if (m->trk_dev) cudaFree(m->trk_dev);
     for (int i = 0; i < 3; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
-    for (int i = 0; i < 2; ++i) {
-      if (m->frames_slot[i]) cudaFree(m->frames_slot[i]);
-      if (m->stage_host[i]) cudaFreeHost(m->stage_host[i]);
-      if (m->h2d_done_ev[i]) cudaEventDestroy(m->h2d_done_ev[i]);
-      if (m->frames_free_ev[i]) cudaEventDestroy(m->frames_free_ev[i]);
-      if (m->result_ev[i]) cudaEventDestroy(m->result_ev[i]);
-    }
-    if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
+    m->slots.release();
     for (auto& e : m->fwd_events) cudaEventDestroy(e);
     sb_post_ws_free(m->ws);
     sb_gather_free(m);
@@ -73,17 +66,6 @@ void sb_models_free(sb_handle_s* h) {
     delete m;
   }
   h->models.clear();
-}
-
-// pinned staging + device frame slots of the submit/collect pipeline are sized from (B, H, W, C, max_instances,
-// n_nodes) at first use: any configure call that may change one of those drops them (re-created lazily)
-void sb_pipeline_slots_free(SbModel* m) {
-  for (int i = 0; i < 2; ++i) {
-    if (m->frames_slot[i]) { cudaFree(m->frames_slot[i]); m->frames_slot[i] = nullptr; }
-    if (m->stage_host[i]) { cudaFreeHost(m->stage_host[i]); m->stage_host[i] = nullptr; }
-    m->slot_used[i] = false;
-  }
-  if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
 }
 
 SbModel* chain_model(sb_handle_s* h, int id, int kind, const char* what) {
@@ -99,7 +81,8 @@ static int chain_drop(sb_handle_s* h, SbModel* m) {
   SB_CUDA(h, cudaDeviceSynchronize());
   h->post_pending = false;
   sb_post_ws_free(m->ws);
-  sb_pipeline_slots_free(m);                     // staging is sized from the chain's record width
+  m->slots.release();                            // staging is sized from the chain's record width
+  if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes)
   m->trk = nullptr;                              // its checks (nodes, instance capacity) were made against the old chain
   sb_global_scratch_free(m->gs);
@@ -670,23 +653,62 @@ int sb_graph_flatten(sb_handle_s* h, const SbPostWs& ws, const SbGraphHost& g, c
   return SB_OK;
 }
 
-int sb_slot_upload(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot) {
-  if (!m->copy_stream) {
-    SB_CUDA(h, cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->h2d_done_ev[i], cudaEventDisableTiming));
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->frames_free_ev[i], cudaEventDisableTiming));
-      SB_CUDA(h, cudaEventCreateWithFlags(&m->result_ev[i], cudaEventDisableTiming));
-    }
+// ---------------------------------- the slots of the streamed steps ----------------------------
+int SbSlots::alloc(sb_handle_s* h, size_t frame_bytes, size_t stage_floats) {
+  if (!copy_stream) SB_CUDA(h, cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; ++i) {
+    for (cudaEvent_t* e : {&h2d_done[i], &frames_free[i], &result[i]})
+      if (!*e) SB_CUDA(h, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    if (!frames[i]) SB_CUDA(h, cudaMalloc(&frames[i], frame_bytes));
+    if (!stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&stage[i], stage_floats * sizeof(float), cudaHostAllocDefault));
   }
-  const size_t fbytes = (size_t)m->B * m->Hin * m->Win * m->Cin;
-  for (int i = 0; i < 2; ++i)
-    if (!m->frames_slot[i]) SB_CUDA(h, cudaMalloc(&m->frames_slot[i], fbytes));
-  // H2D on the copy stream (after the work that last read this slot's frames has finished)
-  if (m->slot_used[slot]) SB_CUDA(h, cudaStreamWaitEvent(m->copy_stream, m->frames_free_ev[slot], 0));
-  SB_CUDA(h, cudaMemcpyAsync(m->frames_slot[slot], frames_host, (size_t)B * m->Hin * m->Win * m->Cin, cudaMemcpyHostToDevice, m->copy_stream));
-  SB_CUDA(h, cudaEventRecord(m->h2d_done_ev[slot], m->copy_stream));
   return 0;
+}
+
+int SbSlots::check_submit(sb_handle_s* h, const char* what, int slot, int B, int max_B, const void* frames_host) const {
+  if (slot < 0 || slot > 1 || !frames_host || B <= 0 || B > max_B) return sb_fail(h, SB_ERR_INVALID, "%s: bad slot / batch", what);
+  if (slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "%s: slot %d holds a batch that was not collected", what, slot);
+  return 0;
+}
+
+int SbSlots::upload(sb_handle_s* h, int slot, const void* frames_host, size_t bytes, std::initializer_list<Copy> more) {
+  if (slot_seq[slot]) SB_CUDA(h, cudaStreamWaitEvent(copy_stream, frames_free[slot], 0));
+  SB_CUDA(h, cudaMemcpyAsync(frames[slot], frames_host, bytes, cudaMemcpyHostToDevice, copy_stream));
+  for (const Copy& c : more) SB_CUDA(h, cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyHostToDevice, copy_stream));
+  SB_CUDA(h, cudaEventRecord(h2d_done[slot], copy_stream));
+  return 0;
+}
+
+int SbSlots::check_collect(sb_handle_s* h, const char* what, int slot, int B) const {
+  if (slot < 0 || slot > 1 || !slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "%s: slot %d holds no submitted batch", what, slot);
+  if (B != slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "%s: slot %d holds a batch of %d frames, not %d", what, slot, slot_B[slot], B);
+  if (slot_B[1 - slot] && slot_seq[1 - slot] < slot_seq[slot])
+    return sb_fail(h, SB_ERR_INVALID, "%s: slot %d was submitted first; collect batches in submit order", what, 1 - slot);
+  return 0;
+}
+
+int SbSlots::collect(sb_handle_s* h, int slot) {
+  const int B = slot_B[slot];
+  slot_B[slot] = 0;
+  SB_CUDA(h, cudaEventSynchronize(result[slot]));
+  done_B[slot] = B;
+  return 0;
+}
+
+int SbSlots::check_read(sb_handle_s* h, const char* what, int slot, int B) const {
+  if (slot < 0 || slot > 1 || B <= 0 || done_B[slot] != B)
+    return sb_fail(h, SB_ERR_INVALID, "%s: slot %d holds no collected batch of %d frames", what, slot, B);
+  return 0;
+}
+
+void SbSlots::release() {
+  for (int i = 0; i < 2; ++i) {
+    if (frames[i]) cudaFree(frames[i]);
+    if (stage[i]) cudaFreeHost(stage[i]);
+    for (cudaEvent_t e : {h2d_done[i], frames_free[i], result[i]}) if (e) cudaEventDestroy(e);
+  }
+  if (copy_stream) cudaStreamDestroy(copy_stream);
+  *this = SbSlots();
 }
 
 extern "C" {
@@ -922,42 +944,40 @@ int sb_get_post_stream(sb_handle_t h, void** out_stream) {
   return SB_OK;
 }
 
-// Splits the per-frame result records (written by k_group's epilogue, ONE D2H copy per batch) into the caller's arrays.
-// Asynchronous, double-buffered variant of sb_infer_bottomup for streaming many batches: submit
-// batch i+1 (its H2D copy runs on a copy stream) while batch i computes, then collect batch i.
-// Layout of the pinned staging record per slot: peaks | vals | scores | n_valid | flags.
+// The streamed form of the chain's synchronous step: submit batch i + 1 (its upload runs on the slots' copy stream) while
+// batch i computes, then collect batch i; ONE D2H copy per batch brings the per-frame records into the slot's staging.
 
-static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot) {
-  if (slot < 0 || slot > 1 || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
+static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot, const char* what) {
+  SbSlots& sl = m->slots;
+  int rc = sl.check_submit(h, what, slot, B, m->B, frames_host);
+  if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
-  int rc = sb_slot_upload(h, m, frames_host, B, slot);
+  if ((rc = sl.alloc(h, (size_t)m->B * m->Hin * m->Win * m->Cin, stage_floats(m))) ||
+      (rc = sl.upload(h, slot, frames_host, (size_t)B * m->Hin * m->Win * m->Cin)))
+    return rc;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
+  rc = sb_run_ops(h, m, sl.frames[slot], 1, B);
   if (rc) return rc;
-  for (int i = 0; i < 2; ++i)
-    if (!m->stage_host[i]) SB_CUDA(h, cudaHostAlloc((void**)&m->stage_host[i], stage_floats(m) * sizeof(float), cudaHostAllocDefault));
-  SB_CUDA(h, cudaStreamWaitEvent(h->stream, m->h2d_done_ev[slot], 0));
-  rc = sb_run_ops(h, m, m->frames_slot[slot], 1, B);
-  if (rc) return rc;
-  SB_CUDA(h, cudaEventRecord(m->frames_free_ev[slot], h->stream));
+  SB_CUDA(h, cudaEventRecord(sl.frames_free[slot], h->stream));
   if ((rc = bottomup_post(h, m, B))) return rc;
   cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
-  if ((rc = queue_result_copy(h, m, B, rs, m->stage_host[slot], 1 + slot))) return rc;
+  if ((rc = queue_result_copy(h, m, B, rs, sl.stage[slot], 1 + slot))) return rc;
   if ((rc = queue_track_copy(h, m, B, rs, slot))) return rc;
-  m->slot_B[slot] = B;
-  SB_CUDA(h, cudaEventRecord(m->result_ev[slot], rs));
-  m->slot_used[slot] = true;
+  SB_CUDA(h, cudaEventRecord(sl.result[slot], rs));
+  sl.submitted(slot, B);
   return SB_OK;
 }
 
 // Blocks until the records of the batch submitted into `slot` are in its pinned staging.
-static int step_collect(sb_handle_s* h, SbModel* m, int slot, int B) {
-  if (slot < 0 || slot > 1 || !m->slot_used[slot] || B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad slot / batch");
-  SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
+static int step_collect(sb_handle_s* h, SbModel* m, int slot, int B, const char* what) {
+  int rc = m->slots.check_collect(h, what, slot, B);
+  if (rc || (rc = m->slots.collect(h, slot))) return rc;
   return check_exchange(h, m);
 }
 
 int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
-  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
+  return m ? step_submit(h, m, frames_host, B, slot, "sb_bottomup_submit") : SB_ERR_INVALID;
 }
 
 int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out_instance_peaks,
@@ -965,23 +985,23 @@ int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out
                         int32_t* out_flags) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
   if (!m) return SB_ERR_INVALID;
-  if (const int rc = step_collect(h, m, slot, B)) return rc;
-  split_paf_records(m, own_slice(m, m->stage_host[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid,
-                    out_flags);
+  if (const int rc = step_collect(h, m, slot, B, "sb_bottomup_collect")) return rc;
+  split_paf_records(m, own_slice(m, m->slots.stage[slot], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores,
+                    out_n_valid, out_flags);
   return SB_OK;
 }
 
 int sb_multiclass_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
-  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
+  return m ? step_submit(h, m, frames_host, B, slot, "sb_multiclass_submit") : SB_ERR_INVALID;
 }
 
 int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals,
                           float* out_class_probs, int32_t* out_flags) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
   if (!m) return SB_ERR_INVALID;
-  if (const int rc = step_collect(h, m, slot, B)) return rc;
-  split_class_records(m->mc, m->stage_host[slot], B, out_points, out_vals, out_class_probs, out_flags);
+  if (const int rc = step_collect(h, m, slot, B, "sb_multiclass_collect")) return rc;
+  split_class_records(m->mc, m->slots.stage[slot], B, out_points, out_vals, out_class_probs, out_flags);
   return SB_OK;
 }
 
@@ -989,9 +1009,11 @@ int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* ou
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_gathered: exchange not connected");
   if (!m || !m->gather.connected) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: exchange not connected");
   if (slot < -1 || slot > 1 || !out_records) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: bad slot");
-  const float* src = slot < 0 ? m->rec_host : m->stage_host[slot];
-  const int have = slot < 0 ? m->rec_B : m->slot_B[slot];
-  if (!src || have != B) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: no collected batch of %d frames in that slot", B);
+  if (slot < 0 && (!m->rec_host || m->rec_B != B))
+    return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: no collected batch of %d frames in that slot", B);
+  if (slot >= 0)
+    if (const int rc = m->slots.check_read(h, "sb_bottomup_gathered", slot, B)) return rc;
+  const float* src = slot < 0 ? m->rec_host : m->slots.stage[slot];
   memcpy(out_records, src, (size_t)m->gather.world * B * sb_record_width(m->bu.max_instances, m->bu.n_nodes) * sizeof(float));
   if (out_counts)
     for (int r = 0; r < m->gather.world; ++r) out_counts[r] = m->gather.counts_host[(slot < 0 ? 3 : 1 + slot) * SB_GATHER_MAX_WORLD + r];
@@ -1021,7 +1043,8 @@ int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_tracks: no tracker attached");
   if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: no tracker attached");
   if (slot < -1 || slot > 1 || B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: bad slot / batch");
-  if (slot >= 0) SB_CUDA(h, cudaEventSynchronize(m->result_ev[slot]));
+  if (slot >= 0)
+    if (const int rc = m->slots.check_read(h, "sb_bottomup_tracks", slot, B)) return rc;
   memcpy(out_tracks, m->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double));
   return SB_OK;
 }
@@ -1194,17 +1217,17 @@ int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int im
 // post-processing stream, as the bottom-up chains do, and the points | values block comes back in one copy.
 int sb_global_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
-  return m ? step_submit(h, m, frames_host, B, slot) : SB_ERR_INVALID;
+  return m ? step_submit(h, m, frames_host, B, slot, "sb_global_submit") : SB_ERR_INVALID;
 }
 
 int sb_global_collect(sb_handle_t h, int model_id, int slot, int B, float* out_points, float* out_vals) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
   if (!m) return SB_ERR_INVALID;
   if (!out_points || !out_vals) return sb_fail(h, SB_ERR_INVALID, "sb_global_collect: null argument");
-  if (const int rc = step_collect(h, m, slot, B)) return rc;
+  if (const int rc = step_collect(h, m, slot, B, "sb_global_collect")) return rc;
   const size_t C = m->buffers[m->gl.cms_buffer].C;
-  memcpy(out_points, m->stage_host[slot], (size_t)B * C * 2 * sizeof(float));
-  memcpy(out_vals, m->stage_host[slot] + (size_t)m->B * C * 2, (size_t)B * C * sizeof(float));
+  memcpy(out_points, m->slots.stage[slot], (size_t)B * C * 2 * sizeof(float));
+  memcpy(out_vals, m->slots.stage[slot] + (size_t)m->B * C * 2, (size_t)B * C * sizeof(float));
   return SB_OK;
 }
 

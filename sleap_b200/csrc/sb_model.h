@@ -2,6 +2,7 @@
 // The int32 record layout must match sleap_b200/nn/oplist.py.
 #pragma once
 #include <functional>
+#include <initializer_list>
 #include <vector>
 
 #include "sb_common.cuh"
@@ -104,6 +105,35 @@ struct SbEntryPlan {
 // pipeline is a layer over a centroid chain and a global chain, valid while neither model's chain_gen moves.
 enum { SB_CHAIN_ANY = -1, SB_CHAIN_NONE = 0, SB_CHAIN_PAF, SB_CHAIN_CLASS, SB_CHAIN_GLOBAL, SB_CHAIN_CENTROID };
 
+// The two slots of a streamed (submit / collect) step and the rules of the streamed steps (include/sleap_b200.h): a
+// submit goes into a slot that holds no batch; a collect takes a slot's batch with its B, oldest first; a slot read
+// takes the batch last collected from that slot with its B.  A check that fails returns SB_ERR_INVALID with `what`
+// before its message and changes nothing.  Buffers, stream and events are allocated by the first submit after release().
+struct SbSlots {
+  cudaStream_t copy_stream = nullptr;
+  void* frames[2] = {nullptr, nullptr};            // device uint8 frames of the slot's batch
+  float* stage[2] = {nullptr, nullptr};            // pinned result staging
+  // h2d_done: the slot's upload landed; frames_free: the last read of its frames is done; result: its results are staged
+  cudaEvent_t h2d_done[2] = {nullptr, nullptr}, frames_free[2] = {nullptr, nullptr}, result[2] = {nullptr, nullptr};
+  int slot_B[2] = {0, 0};                          // frames of the batch the slot holds (submitted, not collected; 0: none)
+  int done_B[2] = {0, 0};                          // frames of the batch last collected from the slot (0: none)
+  unsigned long long slot_seq[2] = {0, 0}, seq = 0;   // submit number of the slot's last batch (0: none since allocation)
+
+  int alloc(sb_handle_s* h, size_t frame_bytes, size_t stage_floats);
+  int check_submit(sb_handle_s* h, const char* what, int slot, int B, int max_B, const void* frames_host) const;
+  // The batch's frames (`bytes`), then the copies `more`, into `slot` on the copy stream once the work that last read
+  // the slot's frames is done; h2d_done[slot] marks their end.  The caller makes its stream wait on it.
+  struct Copy { void* dst; const void* src; size_t bytes; };
+  int upload(sb_handle_s* h, int slot, const void* frames_host, size_t bytes, std::initializer_list<Copy> more = {});
+  void submitted(int slot, int B) { slot_B[slot] = B; done_B[slot] = 0; slot_seq[slot] = ++seq; }
+  void drop(int slot) { slot_B[slot] = 0; }        // a submitted batch whose work could not be queued
+  int check_collect(sb_handle_s* h, const char* what, int slot, int B) const;
+  int collect(sb_handle_s* h, int slot);           // waits for result[slot]; the slot is free again
+  int check_read(sb_handle_s* h, const char* what, int slot, int B) const;
+  bool busy() const { return slot_B[0] || slot_B[1]; }
+  void release();
+};
+
 struct SbModel {
   int precision = 0;  // 0: fp16 activations + tensor-core convs; 1: fp32 CUDA-core path
   std::vector<SbOp> ops;
@@ -135,16 +165,11 @@ struct SbModel {
   sb_bottomup_params bu{};
   std::vector<int> bu_edges;
   sb_multiclass_params mc{};
-  int guard_op = -1;
-  // double-buffered asynchronous pipeline (sb_bottomup_submit / sb_bottomup_collect, sb_multiclass_submit / _collect,
-  // sb_global_submit / _collect; the top-down submit uses the frame slots, the copy stream and the events of its centroid model)
-  void* frames_slot[2] = {nullptr, nullptr};
-  float* stage_host[2] = {nullptr, nullptr};     // pinned result staging (per-frame records)
-  int slot_B[2] = {0, 0}, rec_B = 0;            // frames of the batch last staged in each slot / in rec_host
+  int guard_op = -1;                       // first op that overwrites a head buffer the post-processing stream may still read
+  // the streamed steps of the chain (sb_bottomup_*, sb_multiclass_*, sb_global_*), staging the chain's records
+  SbSlots slots;
   float* rec_host = nullptr;                     // pinned staging of the synchronous sb_infer_bottomup
-  cudaEvent_t h2d_done_ev[2] = {nullptr, nullptr}, frames_free_ev[2] = {nullptr, nullptr}, result_ev[2] = {nullptr, nullptr};
-  bool slot_used[2] = {false, false};
-  cudaStream_t copy_stream = nullptr;      // first op that overwrites a head buffer the post-processing stream may still read
+  int rec_B = 0;                                 // frames of the batch in rec_host
   sb_global_params gl{};
   SbGlobalScratch gs;
   sb_centroid_params ce{};
@@ -182,11 +207,6 @@ SbGatherDev sb_gather_dev(const SbModel* m, unsigned long long step);
 void sb_gather_free(SbModel* m);
 // queues on `s`: wait for every rank's records of `step`, copy the [world][B][width] window to host_dst, acknowledge
 int sb_gather_queue_collect(sb_handle_s* h, SbModel* m, long long step, int B, float* host_dst, int* counts_dev, cudaStream_t s);
-void sb_pipeline_slots_free(SbModel* m);
-// The frame half of a streamed submit into `slot`: the copy stream and slot events (created once), the two device frame
-// slots ([m->B] uint8 frames), and the batch's H2D copy on the copy stream into frames_slot[slot] once the work that last
-// read that slot is done (frames_free_ev); h2d_done_ev[slot] marks its end.  The caller makes its stream wait on it.
-int sb_slot_upload(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot);
 
 // tensor-core conv path (sb_conv_tc.cu)
 int sb_conv_tc_prepare(sb_handle_s* h, SbModel* m);      // after buffers are allocated

@@ -344,8 +344,10 @@ struct SbTopdown {
   SbModel* inst = nullptr;
   unsigned gen_c = 0, gen_i = 0;    // chain_gen of the centroid and the instance model when it was configured
   int K = 0, nodes = 0, width = 0, Bmax = 0;
+  int H = 0, W = 0, C = 0;          // the uint8 or float frames of a batch
   float scale = 1.f;                // pre-crop resize (1: none) and the resized frame the crops are cut from
   int Hr = 0, Wr = 0;
+  int* flags = nullptr;             // per-frame flags: the centroid model's ws.flags, or gt_flags
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
   void* crops = nullptr;
@@ -358,46 +360,32 @@ struct SbTopdown {
   bool tap_half = false, all_stores = false;   // fp16 storage; the production program elides the tap buffer
   float* dense = nullptr;                      // packed dense weights
   float* probs = nullptr;                      // [Bmax * K][n_classes] per-crop class probabilities
-  // streaming (sb_topdown_submit / _collect), allocated at the first submit: per slot the pinned crop count and its
-  // event, the pinned record staging, multi-class the pinned class probabilities of its crops, the frames of the batch it
-  // holds (0: none) with its submit number, and the frames of the batch last collected from it (0: none); `pending` is the
-  // slot whose instance stage is not queued yet (-1: none).  The frames live in the centroid model's frame slots.
+  // streaming (sb_topdown_submit / _collect, sb_topdown_gt_submit), allocated at the first submit: the slots (frames,
+  // record staging), and per slot the pinned crop count and its event and, multi-class, the pinned class probabilities of
+  // its crops; `pending` is the slot whose instance stage is not queued yet (-1: none)
+  SbSlots slots;
   int* count_host = nullptr;                   // [2]
-  float* stage[2] = {nullptr, nullptr};
   float* probs_stage[2] = {nullptr, nullptr};  // [Bmax * K][n_classes]
   cudaEvent_t count_ev[2] = {nullptr, nullptr};
-  int slot_B[2] = {0, 0}, done_B[2] = {0, 0}, pending = -1;
-  unsigned long long slot_seq[2] = {0, 0}, seq = 0;
-  // ground-truth form (sb_topdown_params.centroid_model = -1), held by its instance model.  `frames` stands in for the
-  // centroid model as the step's frame source: a model without a network whose B x H x W x C uint8 frame slots, copy
-  // stream, slot events and per-frame flags (all zero) are allocated at configure time.  gt_cent / gt_count: per slot
-  // the device copy of the batch's centroid table and counts, which k_td_gt_select reads.
-  SbModel* frames = nullptr;
+  int pending = -1;
+  // ground-truth form (sb_topdown_params.centroid_model = -1), held by its instance model.  gt_flags: the per-frame flags,
+  // which k_td_gt_select zeroes; gt_cent / gt_count: per slot the device copy of the batch's centroid table and counts,
+  // which k_td_gt_select reads.
+  bool gt = false;
+  int* gt_flags = nullptr;                     // [Bmax]
   float* gt_cent[2] = {nullptr, nullptr};      // [Bmax][K][2]
   int* gt_count[2] = {nullptr, nullptr};       // [Bmax]
 };
-
-// A ground-truth pipeline's frame source with everything it holds
-static void gt_frames_free(SbModel* f) {
-  if (!f) return;
-  for (int i = 0; i < 2; ++i) {
-    if (f->frames_slot[i]) cudaFree(f->frames_slot[i]);
-    for (cudaEvent_t e : {f->h2d_done_ev[i], f->frames_free_ev[i], f->result_ev[i]}) if (e) cudaEventDestroy(e);
-  }
-  if (f->copy_stream) cudaStreamDestroy(f->copy_stream);
-  if (f->ws.flags) cudaFree(f->ws.flags);
-  delete f;
-}
 
 void sb_topdown_free(SbModel* m) {
   SbTopdown* t = m->td;
   if (!t) return;
   void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
-                 t->offsets, t->total, t->crops, t->dense, t->probs, t->gt_cent[0], t->gt_cent[1], t->gt_count[0], t->gt_count[1]};
+                 t->offsets, t->total, t->crops, t->dense, t->probs, t->gt_flags, t->gt_cent[0], t->gt_cent[1], t->gt_count[0],
+                 t->gt_count[1]};
   for (void* p : dev) if (p) cudaFree(p);
-  gt_frames_free(t->frames);
-  for (void* p : {(void*)t->record_host, (void*)t->total_host, (void*)t->count_host, (void*)t->stage[0], (void*)t->stage[1],
-                  (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
+  t->slots.release();
+  for (void* p : {(void*)t->record_host, (void*)t->total_host, (void*)t->count_host, (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
     if (p) cudaFreeHost(p);
   for (cudaEvent_t e : t->count_ev) if (e) cudaEventDestroy(e);
   delete t;
@@ -433,24 +421,6 @@ int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   return precrop_size(h, p, H, W, &s, &Hr, &Wr);
 }
 
-// The ground-truth form's frame source (SbTopdown::frames) and centroid staging for batches of up to Bmax frames
-int gt_alloc(sb_handle_s* h, SbTopdown* t, int H, int W, int C_in) {
-  SbModel* f = t->frames = new SbModel();
-  f->B = t->Bmax; f->Hin = H; f->Win = W; f->Cin = C_in;
-  SB_CUDA(h, cudaStreamCreateWithFlags(&f->copy_stream, cudaStreamNonBlocking));
-  int rc = sb_dev_alloc(h, &f->ws.flags, (size_t)t->Bmax);
-  for (int i = 0; i < 2 && !rc; ++i) {
-    for (cudaEvent_t* e : {&f->h2d_done_ev[i], &f->frames_free_ev[i], &f->result_ev[i]})
-      SB_CUDA(h, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-    uint8_t* fr = nullptr;
-    if ((rc = sb_dev_alloc(h, &fr, (size_t)t->Bmax * H * W * C_in)) || (rc = sb_dev_alloc(h, &t->gt_cent[i], (size_t)t->Bmax * t->K * 2)) ||
-        (rc = sb_dev_alloc(h, &t->gt_count[i], (size_t)t->Bmax)))
-      break;
-    f->frames_slot[i] = fr;
-  }
-  return rc;
-}
-
 // Configures both networks and their chains, then the pipeline with a record of `width` floats per frame (the centroid
 // configure drops the previous pipeline).  On success mc->td is the new pipeline; in the ground-truth form (mc NULL), with
 // the instance network only, mi->td (the global configure dropped the previous one).
@@ -471,10 +441,7 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   owner->td = t;
   t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
   t->gen_c = mc ? mc->chain_gen : 0; t->gen_i = mi->chain_gen;
-  if (!mc && (rc = gt_alloc(h, t, H, W, C_in))) {
-    sb_topdown_free(owner);
-    return rc;
-  }
+  t->H = H; t->W = W; t->C = C_in; t->gt = !mc;
   precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by check_topdown
   t->nodes = mi->buffers[p->instance.cms_buffer].C;
   t->multiclass = n_classes > 0;
@@ -487,7 +454,9 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
                   A((void**)&t->ipts, N * t->nodes * 2 * 4) && A((void**)&t->ivals, N * t->nodes * 4) &&
                   A((void**)&t->record, (size_t)max_batch * t->width * 4) &&
                   A(&t->crops, (size_t)chunk * p->crop_size * p->crop_size * C_in * 4) &&
-                  (!t->multiclass || A((void**)&t->probs, N * n_classes * 4));
+                  (!t->multiclass || A((void**)&t->probs, N * n_classes * 4)) &&
+                  (mc || A((void**)&t->gt_flags, (size_t)max_batch * 4));
+  t->flags = mc ? mc->ws.flags : t->gt_flags;
   if (!ok || cudaHostAlloc((void**)&t->record_host, (size_t)max_batch * t->width * 4, cudaHostAllocDefault) != cudaSuccess ||
       cudaHostAlloc((void**)&t->total_host, 4, cudaHostAllocDefault) != cudaSuccess) {
     sb_topdown_free(owner);
@@ -508,15 +477,15 @@ SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = f
   if (!mc) return nullptr;
   SbTopdown* t = mc->td;
   if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
-  if (!(sources & (t->frames ? TD_GT : TD_MODEL))) {
-    if (t->frames)
+  if (!(sources & (t->gt ? TD_GT : TD_MODEL))) {
+    if (t->gt)
       sb_fail(h, SB_ERR_INVALID, "top-down pipeline takes ground-truth centroids: call sb_topdown_gt_submit");
     else
       sb_fail(h, SB_ERR_INVALID, "top-down pipeline runs a centroid model: call %s",
               multiclass ? "sb_topdown_multiclass_submit" : "sb_topdown_submit");
     return nullptr;
   }
-  if (t->frames) {
+  if (t->gt) {
     // the instance model holds the pipeline: a configure call on it dropped the pipeline with its chain
     if (t->multiclass != multiclass) {
       sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_collect"
@@ -546,7 +515,7 @@ SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = f
 
 // Refuses a call that would overwrite the single selection, crop and record buffers while a streamed batch holds them
 int check_idle(sb_handle_s* h, const SbTopdown* t, const char* what) {
-  if (t->slot_B[0] || t->slot_B[1])
+  if (t->slots.busy())
     return sb_fail(h, SB_ERR_INVALID, "%s: a batch was submitted and not collected; collect it first", what);
   return 0;
 }
@@ -583,9 +552,9 @@ int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
 // The instance stage of the batch the centroid stage left in the selection buffers (`total` crops of the B frames at
 // frames_dev): per chunk of crops the crop kernel, the instance network, the global peaks and, multi-class, the class
 // vectors; frames_free (given) after the last crop kernel; then the records -- k_td_class_assign, or k_td_pack and the
-// attached tracker -- copied into rec_host, the track records into trk_host and, given, the crops' class probabilities
-// into probs_host.
-int instance_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int total,
+// attached tracker of the centroid model mc (NULL in the ground-truth form) -- copied into rec_host, the track records into
+// trk_host and, given, the crops' class probabilities into probs_host.
+int instance_stage(sb_handle_s* h, const SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int total,
                    float* rec_host, double* trk_host, float* probs_host, cudaEvent_t frames_free) {
   cudaStream_t s = h->stream;
   SbModel* mi = t->inst;
@@ -601,9 +570,9 @@ int instance_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
     // crops of the frames already resident in HBM (uint8 frames: float -> uint8 truncation, as tf.cast in crop_bboxes),
     // with a pre-crop resize of those frames resized on the fly
     const float* cent = t->flat_cent + 2 * (size_t)c0;
-    if ((rc = t->scale != 1.f ? sbk_crop_resized(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, t->Hr, t->Wr, cent,
+    if ((rc = t->scale != 1.f ? sbk_crop_resized(h, frames_dev, frames_are_u8, B, t->H, t->W, t->C, t->Hr, t->Wr, cent,
                                                  t->flat_sample + c0, n, cs, cs, t->crops)
-                              : sbk_crop(h, frames_dev, frames_are_u8, B, mc->Hin, mc->Win, mc->Cin, cent, t->flat_sample + c0, n, cs, cs,
+                              : sbk_crop(h, frames_dev, frames_are_u8, B, t->H, t->W, t->C, cent, t->flat_sample + c0, n, cs, cs,
                                          t->crops, frames_are_u8)))
       return rc;
     if ((rc = sb_run_ops(h, mi, t->crops, frames_are_u8, n, t->all_stores))) return rc;
@@ -616,15 +585,15 @@ int instance_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
   if (frames_free) SB_CUDA(h, cudaEventRecord(frames_free, s));
   if (t->multiclass) {
     if ((rc = launch_class_assign(h, t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->probs, B, t->K, t->nodes,
-                                  NC, mc->ws.flags, t->record)))
+                                  NC, t->flags, t->record)))
       return rc;
     if (probs_host && total > 0)
       SB_CUDA(h, cudaMemcpyAsync(probs_host, t->probs, (size_t)total * NC * 4, cudaMemcpyDeviceToHost, s));
   } else {
-    k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, mc->ws.flags,
+    k_td_pack<<<B, 128, 0, s>>>(t->sel_cent, t->sel_val, t->sel_count, t->offsets, t->ipts, t->ivals, t->K, t->nodes, t->flags,
                                 t->record, t->width);
     SB_CHECK_LAUNCH(h);
-    if (mc->trk) {
+    if (mc && mc->trk) {
       // the attached tracker on the frames' instance lists; its records come back with the step's records
       if ((rc = sbk_track_topdown(h, mc->trk, B, t->ipts, t->ivals, t->sel_val, t->sel_count, t->offsets, t->K, mc->trk_h, mc->trk_w,
                                   mc->trk_dev)))
@@ -668,31 +637,34 @@ int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_ho
 
 // Queues the instance stage of the pending streamed batch (its count event waited for on the host) behind whatever the
 // handle's stream holds.  The slot is dropped when it fails.
-int queue_pending_instance(sb_handle_s* h, SbModel* mc, SbTopdown* t) {
+int queue_pending_instance(sb_handle_s* h, const SbModel* mc, SbTopdown* t) {
   const int k = t->pending;
+  SbSlots& sl = t->slots;
   t->pending = -1;
   cudaError_t e = cudaEventSynchronize(t->count_ev[k]);
   int rc = e == cudaSuccess ? 0 : sb_fail(h, SB_ERR_CUDA, "crop count: %s", cudaGetErrorString(e));
   if (!rc) {
-    rc = instance_stage(h, mc, t, mc->frames_slot[k], 1, t->slot_B[k], t->count_host[k], t->stage[k], mc->trk_host[k],
-                        t->probs_stage[k], mc->frames_free_ev[k]);
+    rc = instance_stage(h, mc, t, sl.frames[k], 1, sl.slot_B[k], t->count_host[k], sl.stage[k], mc->trk_host[k], t->probs_stage[k],
+                        sl.frames_free[k]);
   }
   if (!rc) {
-    e = cudaEventRecord(mc->result_ev[k], h->stream);
+    e = cudaEventRecord(sl.result[k], h->stream);
     if (e != cudaSuccess) rc = sb_fail(h, SB_ERR_CUDA, "event record: %s", cudaGetErrorString(e));
   }
-  if (rc) t->slot_B[k] = 0;
+  if (rc) sl.drop(k);
   return rc;
 }
 
-// The streaming staging of the pipeline, allocated once at its first submit (synchronous users never pay for it)
+// The streaming buffers of the pipeline, allocated at its first submit (synchronous users never pay for them)
 int stream_alloc(sb_handle_s* h, SbTopdown* t) {
-  if (t->count_host) return 0;
-  const size_t rec_bytes = (size_t)t->Bmax * t->width * 4, probs_bytes = (size_t)t->Bmax * t->K * t->head.n_classes * 4;
+  int rc = t->slots.alloc(h, (size_t)t->Bmax * t->H * t->W * t->C, (size_t)t->Bmax * t->width);
+  if (rc || t->count_host) return rc;
+  const size_t probs_bytes = (size_t)t->Bmax * t->K * t->head.n_classes * 4;
   for (int i = 0; i < 2; ++i) {
-    if (!t->stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&t->stage[i], rec_bytes, cudaHostAllocDefault));
     if (t->multiclass && !t->probs_stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&t->probs_stage[i], probs_bytes, cudaHostAllocDefault));
     if (!t->count_ev[i]) SB_CUDA(h, cudaEventCreateWithFlags(&t->count_ev[i], cudaEventDisableTiming));
+    if (t->gt && !t->gt_cent[i] && (rc = sb_dev_alloc(h, &t->gt_cent[i], (size_t)t->Bmax * t->K * 2))) return rc;
+    if (t->gt && !t->gt_count[i] && (rc = sb_dev_alloc(h, &t->gt_count[i], (size_t)t->Bmax))) return rc;
   }
   SB_CUDA(h, cudaHostAlloc((void**)&t->count_host, 2 * sizeof(int), cudaHostAllocDefault));   // last: marks it complete
   return 0;
@@ -705,30 +677,28 @@ int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, in
   SbTopdown* t = topdown_of(h, id, multiclass, true);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[id];
-  if (slot < 0 || slot > 1 || !frames_host || B <= 0 || B > t->Bmax || B > mc->B)
-    return sb_fail(h, SB_ERR_INVALID, "top-down submit: bad slot / batch");
-  if (t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "top-down submit: slot %d holds a batch that was not collected", slot);
+  SbSlots& sl = t->slots;
+  int rc = sl.check_submit(h, "top-down submit", slot, B, t->Bmax, frames_host);
+  if (rc) return rc;
   SB_CUDA(h, cudaSetDevice(h->device));
-  int rc = stream_alloc(h, t);
-  if (rc || (rc = sb_slot_upload(h, mc, frames_host, B, slot))) return rc;
+  if ((rc = stream_alloc(h, t)) || (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C))) return rc;
   if (t->pending >= 0 && (rc = queue_pending_instance(h, mc, t))) return rc;
-  SB_CUDA(h, cudaStreamWaitEvent(h->stream, mc->h2d_done_ev[slot], 0));
-  if ((rc = centroid_stage(h, mc, t, mc->frames_slot[slot], 1, B, t->count_host + slot, t->count_ev[slot]))) return rc;
-  mc->slot_used[slot] = true;
-  t->slot_B[slot] = B; t->done_B[slot] = 0; t->slot_seq[slot] = ++t->seq; t->pending = slot;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
+  if ((rc = centroid_stage(h, mc, t, sl.frames[slot], 1, B, t->count_host + slot, t->count_ev[slot]))) return rc;
+  sl.submitted(slot, B);
+  t->pending = slot;
   return SB_OK;
 }
 
 // Streamed batch with ground-truth centroids into `slot`, the whole step queued at once (the host knows the crop count):
-// the frames, then the centroid table and counts, on the frame source's copy stream into the slot; k_td_gt_select and
-// the crop list behind that copy on the handle's stream; then the instance stage.  The table has its own per-slot
-// staging: the batch before may still be reading the selection buffers when the copy lands.
+// the frames, then the centroid table and counts, on the copy stream into the slot; k_td_gt_select and the crop list
+// behind that copy on the handle's stream; then the instance stage.  The table has its own per-slot staging: the batch
+// before may still be reading the selection buffers when the copy lands.
 int topdown_gt_submit(sb_handle_s* h, SbTopdown* t, const uint8_t* frames_host, const float* centroids_host, const int32_t* counts_host,
                       int B, int slot) {
-  SbModel* f = t->frames;
-  if (slot < 0 || slot > 1 || !frames_host || !centroids_host || !counts_host || B <= 0 || B > t->Bmax)
-    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: bad slot / batch");
-  if (t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: slot %d holds a batch that was not collected", slot);
+  SbSlots& sl = t->slots;
+  int rc = sl.check_submit(h, "sb_topdown_gt_submit", slot, B, t->Bmax, centroids_host && counts_host ? frames_host : nullptr);
+  if (rc) return rc;
   int total = 0;
   for (int b = 0; b < B; ++b) {
     if (counts_host[b] < 0 || counts_host[b] > t->K)
@@ -737,43 +707,31 @@ int topdown_gt_submit(sb_handle_s* h, SbTopdown* t, const uint8_t* frames_host, 
     total += counts_host[b];
   }
   SB_CUDA(h, cudaSetDevice(h->device));
-  int rc = stream_alloc(h, t);
-  if (rc || (rc = sb_slot_upload(h, f, frames_host, B, slot))) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(t->gt_cent[slot], centroids_host, (size_t)B * t->K * 2 * sizeof(float), cudaMemcpyHostToDevice, f->copy_stream));
-  SB_CUDA(h, cudaMemcpyAsync(t->gt_count[slot], counts_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, f->copy_stream));
-  SB_CUDA(h, cudaEventRecord(f->h2d_done_ev[slot], f->copy_stream));
-  SB_CUDA(h, cudaStreamWaitEvent(h->stream, f->h2d_done_ev[slot], 0));
+  if ((rc = stream_alloc(h, t)) ||
+      (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C,
+                      {{t->gt_cent[slot], centroids_host, (size_t)B * t->K * 2 * sizeof(float)},
+                       {t->gt_count[slot], counts_host, (size_t)B * sizeof(int32_t)}})))
+    return rc;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
   k_td_gt_select<<<B, 128, 0, h->stream>>>(t->gt_cent[slot], t->gt_count[slot], t->K, t->scale, t->sel_cent, t->sel_val, t->sel_count,
-                                           f->ws.flags);
+                                           t->gt_flags);
   SB_CHECK_LAUNCH(h);
   if ((rc = flatten(h, t, B)) ||
-      (rc = instance_stage(h, f, t, f->frames_slot[slot], 1, B, total, t->stage[slot], nullptr, t->probs_stage[slot], f->frames_free_ev[slot])))
+      (rc = instance_stage(h, nullptr, t, sl.frames[slot], 1, B, total, sl.stage[slot], nullptr, t->probs_stage[slot], sl.frames_free[slot])))
     return rc;
-  SB_CUDA(h, cudaEventRecord(f->result_ev[slot], h->stream));
-  f->slot_used[slot] = true;
-  t->slot_B[slot] = B; t->done_B[slot] = 0; t->slot_seq[slot] = ++t->seq;
+  SB_CUDA(h, cudaEventRecord(sl.result[slot], h->stream));
+  sl.submitted(slot, B);
   return SB_OK;
 }
 
-// The model whose frame slots and slot events a streamed batch of pipeline `t` (held by model `id`) uses
-SbModel* step_frames(sb_handle_s* h, int id, SbTopdown* t) { return t->frames ? t->frames : h->models[id]; }
-
-// The streamed batch of `slot` in its pinned staging: its instance stage queued if still pending, then its record event
-// waited for.  The slot is free again afterwards.
-int topdown_collect(sb_handle_s* h, SbModel* mc, SbTopdown* t, int slot, int B) {
-  if (slot < 0 || slot > 1 || !t->slot_B[slot]) return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d holds no submitted batch", slot);
-  if (B != t->slot_B[slot])
-    return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d holds a batch of %d frames, not %d", slot, t->slot_B[slot], B);
-  const int other = 1 - slot;
-  if (t->slot_B[other] && t->slot_seq[other] < t->slot_seq[slot])
-    return sb_fail(h, SB_ERR_INVALID, "top-down collect: slot %d was submitted first; collect batches in submit order", other);
-  SB_CUDA(h, cudaSetDevice(h->device));
-  int rc = t->pending == slot ? queue_pending_instance(h, mc, t) : 0;
+// The streamed batch of `slot` of the pipeline held by model `id` in its pinned staging: its instance stage queued if
+// still pending, then its record event waited for.  The slot is free again afterwards.
+int topdown_collect(sb_handle_s* h, int id, SbTopdown* t, int slot, int B) {
+  int rc = t->slots.check_collect(h, "top-down collect", slot, B);
   if (rc) return rc;
-  t->slot_B[slot] = 0;
-  SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
-  t->done_B[slot] = B;
-  return SB_OK;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if (t->pending == slot && (rc = queue_pending_instance(h, h->models[id], t))) return rc;
+  return t->slots.collect(h, slot);
 }
 
 // A plain record's fields into the caller's arrays
@@ -809,7 +767,7 @@ void split_topdown_multiclass(const SbTopdown* t, const float* rec, const float*
 
 }  // namespace
 
-bool sb_topdown_busy(const SbModel* m) { return m->td && (m->td->slot_B[0] || m->td->slot_B[1]); }
+bool sb_topdown_busy(const SbModel* m) { return m->td && m->td->slots.busy(); }
 
 extern "C" {
 
@@ -839,8 +797,8 @@ int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_
                        float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags) {
   SbTopdown* t = topdown_of(h, model_id, false, true, TD_MODEL | TD_GT);
   if (!t) return SB_ERR_INVALID;
-  if (const int rc = topdown_collect(h, step_frames(h, model_id, t), t, slot, B)) return rc;
-  split_topdown(t, t->stage[slot], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
+  if (const int rc = topdown_collect(h, model_id, t, slot, B)) return rc;
+  split_topdown(t, t->slots.stage[slot], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
   return SB_OK;
 }
 
@@ -879,11 +837,8 @@ int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, dou
   if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
   if (slot < -1 || slot > 1 || B <= 0 || B > t->Bmax || !out_tracks)
     return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad slot / batch");
-  if (slot >= 0) {
-    if (t->done_B[slot] != B)
-      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: slot %d holds no collected batch of %d frames", slot, B);
-    SB_CUDA(h, cudaEventSynchronize(mc->result_ev[slot]));
-  }
+  if (slot >= 0)
+    if (const int rc = t->slots.check_read(h, "sb_topdown_tracks", slot, B)) return rc;
   memcpy(out_tracks, mc->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
   return SB_OK;
 }
@@ -948,8 +903,8 @@ int sb_topdown_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, 
                                   float* out_class_vectors) {
   SbTopdown* t = topdown_of(h, model_id, true, true, TD_MODEL | TD_GT);
   if (!t) return SB_ERR_INVALID;
-  if (const int rc = topdown_collect(h, step_frames(h, model_id, t), t, slot, B)) return rc;
-  split_topdown_multiclass(t, t->stage[slot], t->probs_stage[slot], B, out_centroids, out_centroid_vals, out_points, out_vals,
+  if (const int rc = topdown_collect(h, model_id, t, slot, B)) return rc;
+  split_topdown_multiclass(t, t->slots.stage[slot], t->probs_stage[slot], B, out_centroids, out_centroid_vals, out_points, out_vals,
                            out_class_probs, out_n_valid, out_flags, out_class_vectors);
   return SB_OK;
 }

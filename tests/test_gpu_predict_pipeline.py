@@ -268,7 +268,9 @@ def test_single_instance_trained(precision, monkeypatch):
     assert frames_summary(streamed) == frames_summary(batched) == frames_summary(via_video)
 
 
-def test_single_instance_refusals():
+def test_single_instance_stream_refusals():
+    """A batch above the configured B, a collect of a slot that holds no submitted batch and a call of another chain are
+    refused; the stream runs afterwards."""
     from sleap_b200.nn.inference import Predictor
     imgs, _ = rm.frames("robot")
     im = Predictor.from_model_paths([rm.model_dir("minimal_robot.single_instance")], precision=1).inference_model
@@ -279,7 +281,7 @@ def test_single_instance_refusals():
     pts, vals = np.zeros((2, 4, 2), np.float32), np.zeros((2, 4), np.float32)
     with pytest.raises(_lib.SleapB200Error, match="bad slot / batch"):
         m.handle.call("sb_global_submit", m.model_id, _lib.ptr(imgs), 3, 0)
-    with pytest.raises(_lib.SleapB200Error, match="bad slot / batch"):
+    with pytest.raises(_lib.SleapB200Error, match="slot 1 holds no submitted batch"):
         m.handle.call("sb_global_collect", m.model_id, 1, 2, _lib.ptr(pts), _lib.ptr(vals))
     with pytest.raises(_lib.SleapB200Error, match="bottom-up predictor not configured"):
         m.handle.call("sb_bottomup_submit", m.model_id, _lib.ptr(imgs), 2, 0)
