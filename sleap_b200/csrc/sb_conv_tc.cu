@@ -633,10 +633,11 @@ __global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(con
 // Halo form (form 2): persistent, weights resident, for 3x3 stride-1 convs with C_in <= 64 (one K chunk) and one N tile of
 // <= 64 channels in the epi_mode == 1 shape (fp16 out, no BN, no residual).  A work item is a 16 x 8 BY-pixel tile of one
 // frame, cut into 2 x BY blocks of 8x8 pixels (one m64 each).  Lane 0 of the producer warp (warp 8) loads the item's
-// (8 BY + 2) x 18-pixel halo patch as one TMA box of the 5-D patch map (encode_patches) into a ring of patch slots: KC / 8
-// non-swizzled 8-channel planes [rows][18][8 ch] (16 bytes per pixel; TMA zero fill outside the image and beyond C_in).
-// Every tap (ky, kx) of a block is then the same K-major operand at start offset (ky * 18 + kx) * 16 bytes (LBO = one
-// plane, SBO = one patch row): one load serves all nine taps.  Consumer warpgroups 0 and 1 take alternate items
+// (8 BY + 2) x 18-pixel halo patch as one TMA box of the patch map (encode_patches) into a ring of patch slots: pixel rows
+// [rows][18][KC ch] of KC * 2 bytes, swizzled at the row width (SW128 / SW64 / SW32 for KC 64 / 32 / 16; TMA zero fill
+// outside the image and beyond C_in).  Every tap (ky, kx) of a block is then the same swizzled K-major operand at start
+// offset (ky * 18 + kx) * KC * 2 bytes (SBO = one patch row): one load serves all nine taps.  Consumer warpgroups 0 and 1
+// take alternate items
 // (ping-pong), so one warpgroup's epilogue overlaps the other's wgmma.
 // The epilogue runs from registers (halo_block_epilogue): a thread's two accumulator rows are vertically adjacent pixels.  Every
 // output element gets the wgmma products of k_conv_wg -- the same m64nNk16 shape, (filter column, tap, k-step) order and
@@ -645,7 +646,11 @@ __global__ void __launch_bounds__(kConvThreads, N <= 64 ? 2 : 1) k_conv_wg_p(con
 constexpr int kHaloCols = 18;                                  // 16 output columns + 2
 // 8x8 blocks along y per item: 16x16 px where N <= 32 and N x KC <= 1024, else 16x8 (ptxas: 16x16 at N = 32, KC = 64 spills)
 constexpr int halo_by(int n, int kc) { return n <= 32 && n * kc <= 1024 ? 2 : 1; }
-constexpr int halo_plane(int n, int kc) { return (8 * halo_by(n, kc) + 2) * kHaloCols * 16; }
+// A patch of `rows` x 18 pixels of KC channels (forms 2 and 3): the bytes of its TMA box, and its slot in a patch ring,
+// rounded up to the swizzle pattern (8 rows of KC * 2 bytes) so that every slot starts on one.
+constexpr int patch_box_bytes(int rows, int kc) { return rows * kHaloCols * kc * 2; }
+constexpr int patch_slot_bytes(int rows, int kc) { return (patch_box_bytes(rows, kc) + 16 * kc - 1) / (16 * kc) * (16 * kc); }
+constexpr int patch_layout(int kc) { return kc == 64 ? 1 : (kc == 32 ? 2 : 3); }   // wgmma descriptor: SW128 / SW64 / SW32
 
 // lane t of each quad holds piece k of chunks 0..3 in v[k]; afterwards it holds pieces 0..3 of chunk t (two xor stages)
 __device__ __forceinline__ void quad_transpose(uint32_t& v0, uint32_t& v1, uint32_t& v2, uint32_t& v3, int t) {
@@ -744,8 +749,8 @@ template <int KSTEPS, int N>
 __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_constant__ CUtensorMap mapA,
                                                                const __grid_constant__ CUtensorMap mapB,
                                                                const __grid_constant__ TcParams P) {
-  constexpr int BY = halo_by(N, 16 * KSTEPS), NB = 2 * BY;                  // blocks per item: 2 along x, BY along y
-  constexpr int PW = kHaloCols, PLANE = halo_plane(N, 16 * KSTEPS), SLOT = 2 * KSTEPS * PLANE;   // KC / 8 planes
+  constexpr int KC = 16 * KSTEPS, BY = halo_by(N, KC), NB = 2 * BY;        // blocks per item: 2 along x, BY along y
+  constexpr int PW = kHaloCols, RB = 2 * KC, BOX = patch_box_bytes(8 * BY + 2, KC), SLOT = patch_slot_bytes(8 * BY + 2, KC);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* bank = base;                                        // 9 weight slices, swizzled as in k_conv_wg_p
@@ -783,9 +788,9 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
         const int s = i % P.n_a_slots;
         mbar_wait(smem_u32(empty + s), ((i / P.n_a_slots) & 1) ^ 1);
         const int tile = w % n_tiles, b = w / n_tiles;
-        mbar_expect_tx(smem_u32(full + s), (uint32_t)SLOT);      // zero-filled bytes count too
-        tma_load_5d(smem_u32(ring + (size_t)s * SLOT), &mapA, smem_u32(full + s), 0, (tile % tiles_x) * 16 - 1,
-                    (tile / tiles_x) * (8 * BY) - 1, 0, b);
+        mbar_expect_tx(smem_u32(full + s), (uint32_t)BOX);       // zero-filled bytes count too
+        tma_load_4d(smem_u32(ring + (size_t)s * SLOT), &mapA, smem_u32(full + s), 0, (tile % tiles_x) * 16 - 1,
+                    (tile / tiles_x) * (8 * BY) - 1, b);
       }
     }
     return;
@@ -794,7 +799,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
   // ------------------------------ consumers: warpgroup wg takes the CTA's items wg, wg + 2, ... ------------------------------
   const int wg = warp >> 2, q = warp & 3, g = lane >> 2, t = lane & 3;
   const float lo = P.relu ? 0.f : -INFINITY;
-  const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
+  const uint64_t desc_a = make_desc(0, RB, patch_layout(KC), PW * RB);
   const uint64_t desc_b = make_desc(0, P.row_bytes, P.layout_type);
   const uint32_t b_base = smem_u32(bank);
   mbar_wait(smem_u32(fullB), 0);
@@ -815,7 +820,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
           const uint64_t db = desc_b + (uint64_t)((b_base + (uint32_t)((kx * 3 + ky) * P.b_slot_bytes)) >> 4) + 2 * k;
 #pragma unroll
           for (int bk = 0; bk < NB; ++bk) {
-            const uint32_t a = a_base + (uint32_t)(((8 * (bk >> 1) + ky) * PW + 8 * (bk & 1) + kx) * 16 + 2 * k * PLANE);
+            const uint32_t a = a_base + (uint32_t)(((8 * (bk >> 1) + ky) * PW + 8 * (bk & 1) + kx) * RB + 32 * k);
             wgmma_f16<N>(acc[bk], desc_a + (uint64_t)(a >> 4), db, (kx | ky | k) ? 1u : 0u);
           }
         }
@@ -841,8 +846,8 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
 // here a work item is 16 x 8 BY output pixels x one N tile (N <= 128) x one frame, cut into 2 x BY blocks of 8x8 pixels,
 // and both consumer warpgroups (BY blocks each) read every weight slice, so one L2 read of a slice feeds 256 (N > 64) or
 // 512 (N <= 64) pixels.  K = 9 taps x C_in runs in chunks of 64 input channels (the last zero-filled beyond C_in).
-//   warpgroup 0 (registers cut to 56): lane 0 of warp 0 loads one halo patch per (item, chunk) in form 2's layout (8
-//     non-swizzled 8-channel planes [8 BY + 2][18][8], one TMA box of the 5-D patch map, zero outside the image and beyond
+//   warpgroup 0 (registers cut to 56): lane 0 of warp 0 loads one halo patch per (item, chunk) in form 2's layout (128B-
+//     swizzled 64-channel pixel rows [8 BY + 2][18][64], one TMA box of the patch map, zero outside the image and beyond
 //     C_in) into a ring of patch slots; lane 0 of warp 1 streams the [N x 64] weight slices (SW128, TMA) in (chunk, filter
 //     column, tap) order into a ring of weight slots.  The weights never wait on the grid dependency, so the first ring is
 //     in flight while the predecessor drains.
@@ -857,13 +862,14 @@ __global__ void __launch_bounds__(kConvThreads, 1) k_conv_wg_h(const __grid_cons
 // and the consumers take what the producer warpgroup gives back: 128 x (168 - 56) = 256 x (224 - 168).
 constexpr int kWideThreads = 384;
 constexpr int wide_by(int n) { return n <= 64 ? 4 : 2; }       // 8x8 block rows per item: 128 accumulators per consumer thread
-constexpr int wide_plane(int n) { return (8 * wide_by(n) + 2) * kHaloCols * 16; }
+constexpr int wide_rows(int n) { return 8 * wide_by(n) + 2; }
 
 template <int N>
 __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_constant__ CUtensorMap mapA,
                                                                 const __grid_constant__ CUtensorMap mapB,
                                                                 const __grid_constant__ TcParams P) {
-  constexpr int BY = wide_by(N), PW = kHaloCols, PLANE = wide_plane(N), SLOT = 8 * PLANE;
+  constexpr int BY = wide_by(N), PW = kHaloCols, RB = 128, BOX = patch_box_bytes(wide_rows(N), 64),
+                SLOT = patch_slot_bytes(wide_rows(N), 64);
   constexpr int WSLOT = N * 128;                               // one [N x 64-channel] weight slice
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -902,8 +908,8 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
         for (int ch = 0; ch < P.n_chunks; ++ch, ++i) {
           const int s = i % P.n_a_slots;
           mbar_wait(smem_u32(pempty + s), ((i / P.n_a_slots) & 1) ^ 1);
-          mbar_expect_tx(smem_u32(pfull + s), (uint32_t)SLOT);   // zero-filled bytes count too
-          tma_load_5d(smem_u32(pring + (size_t)s * SLOT), &mapA, smem_u32(pfull + s), 0, xs, ys, ch * 8, b);
+          mbar_expect_tx(smem_u32(pfull + s), (uint32_t)BOX);    // zero-filled bytes count too
+          tma_load_4d(smem_u32(pring + (size_t)s * SLOT), &mapA, smem_u32(pfull + s), ch * 64, xs, ys, b);
         }
       }
     } else if (warp == 1 && lane == 0) {
@@ -927,9 +933,9 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
   setmaxnreg_inc<224>();
   const int cw = (warp >> 2) - 1, q = warp & 3, g = lane >> 2, t = lane & 3;
   const float lo = P.relu ? 0.f : -INFINITY;
-  const uint64_t desc_a = make_desc_interleave(0, PLANE, PW * 16);
+  const uint64_t desc_a = make_desc(0, RB, 1, PW * RB);
   const uint64_t desc_b = make_desc(0, 128, 1);
-  const uint32_t p_base = smem_u32(pring) + (uint32_t)(cw * (BY / 2) * 8 * PW * 16), w_base = smem_u32(wring);
+  const uint32_t p_base = smem_u32(pring) + (uint32_t)(cw * (BY / 2) * 8 * PW * RB), w_base = smem_u32(wring);
   float acc[BY][N / 2];
   int ps = 0, ws = 0;
   uint32_t pph = 0, wph = 0;
@@ -951,7 +957,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_conv_wg_hw(const __grid_con
           for (int k = 0; k < 4; ++k)
 #pragma unroll
             for (int i = 0; i < BY; ++i) {
-              const uint32_t a = a_base + (uint32_t)(((8 * (i >> 1) + ky) * PW + 8 * (i & 1) + kx) * 16 + 2 * k * PLANE);
+              const uint32_t a = a_base + (uint32_t)(((8 * (i >> 1) + ky) * PW + 8 * (i & 1) + kx) * RB + 32 * k);
               wgmma_f16<N>(acc[i], desc_a + (uint64_t)(a >> 4), db + 2 * k, (ch | kx | ky | k) ? 1u : 0u);
             }
           wgmma_commit();
@@ -1452,7 +1458,8 @@ static size_t conv_smem_resident(const TcParams& P, int n_a, int bank) {
 
 // shared memory of a k_conv_wg_h launch: weight bank (9 slices), n_a patch slots, 2 n_a + 1 barriers
 static size_t conv_smem_halo(const TcParams& P, int n_a) {
-  return 1024 /*align slack*/ + (size_t)9 * P.b_slot_bytes + (size_t)n_a * (P.KC / 8) * halo_plane(P.N, P.KC) + (size_t)(2 * n_a + 1) * 8 +
+  return 1024 /*align slack*/ + (size_t)9 * P.b_slot_bytes + (size_t)n_a * patch_slot_bytes(8 * halo_by(P.N, P.KC) + 2, P.KC) +
+         (size_t)(2 * n_a + 1) * 8 +
          (size_t)P.N * sizeof(float);
 }
 
@@ -1519,7 +1526,7 @@ static void setup_forms(sb_handle_s* h, TcLaunch& L, int total_steps) {
   if (TcForm& F = L.forms[3]; form_kernel(3, P.KC, wide_n(P)) && wide_eligible(P)) {
     F.threads = kWideThreads;
     F.P.N = wide_n(P);
-    fit_weight_ring(F, 2, (size_t)8 * wide_plane(F.P.N));
+    fit_weight_ring(F, 2, (size_t)patch_slot_bytes(wide_rows(F.P.N), 64));
     const int by = wide_by(F.P.N);
     F.n_items = (P.Cout / F.P.N) * ((P.W + 15) / 16) * ((P.H + 8 * by - 1) / (8 * by));
     fit_ctas(h, F, 3);
@@ -1568,17 +1575,17 @@ static CUresult encode_weights(EncodeTiledFn enc, const SbConvTcPlan* plan, int 
              swz_for(KC), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// Forms 2 and 3: the input slice as a 5-D map {8 channels, W, H, C_in / 8, frames}, byte strides {C_tot 2, W C_tot 2, 16,
-// H W C_tot 2}, whose box {8, 18, rows, KC / 8, 1} at (0, x - 1, y - 1, c0 / 8, b) is one halo patch: it lands as the
-// KC / 8 planes [rows][18][8 ch] of a patch slot.  Pixels outside the image (SAME padding) and planes beyond C_in (the
-// chunk's zero fill) are out of bounds of the map and zero-filled by TMA.
+// Forms 2 and 3: the input slice as a 4-D map {C_in, W, H, frames}, byte strides {C_tot 2, W C_tot 2, H W C_tot 2},
+// whose box {KC, 18, rows, 1} at (c0, x - 1, y - 1, b) is one halo patch: it lands as the swizzled pixel rows
+// [rows][18][KC ch] of a patch slot.  Pixels outside the image (SAME padding) and channels beyond C_in (the chunk's zero
+// fill) are out of bounds of the map and zero-filled by TMA.
 static CUresult encode_patches(EncodeTiledFn enc, const TcParams& P, int frames, int rows, CUtensorMap* map) {
-  cuuint64_t dims[5] = {8, (cuuint64_t)P.W, (cuuint64_t)P.H, (cuuint64_t)(P.in_C / 8), (cuuint64_t)frames};
-  cuuint64_t strides[4] = {(cuuint64_t)P.in_Ctot * 2, (cuuint64_t)P.W * P.in_Ctot * 2, 16, (cuuint64_t)P.H * P.W * P.in_Ctot * 2};
-  cuuint32_t box[5] = {8, kHaloCols, (cuuint32_t)rows, (cuuint32_t)(P.KC / 8), 1};
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(P.in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  cuuint64_t dims[4] = {(cuuint64_t)P.in_C, (cuuint64_t)P.W, (cuuint64_t)P.H, (cuuint64_t)frames};
+  cuuint64_t strides[3] = {(cuuint64_t)P.in_Ctot * 2, (cuuint64_t)P.W * P.in_Ctot * 2, (cuuint64_t)P.H * P.W * P.in_Ctot * 2};
+  cuuint32_t box[4] = {(cuuint32_t)P.KC, kHaloCols, (cuuint32_t)rows, 1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(P.in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             swz_for(P.KC), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan* plan, int n_groups,
@@ -1677,7 +1684,7 @@ static int make_launch(sb_handle_s* h, SbModel* m, const SbOp& op, SbConvTcPlan*
     if (CUresult r = encode_patches(enc, P, m->B, 8 * halo_by(P.N, KC) + 2, &L.forms[2].mapA); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(patches, halo form) failed: %d", (int)r);
   if (L.forms[3].ok) {
-    if (CUresult r = encode_patches(enc, P, m->B, 8 * wide_by(L.forms[3].P.N) + 2, &L.forms[3].mapA); r != CUDA_SUCCESS)
+    if (CUresult r = encode_patches(enc, P, m->B, wide_rows(L.forms[3].P.N), &L.forms[3].mapA); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(patches, wide form) failed: %d", (int)r);
     if (CUresult r = encode_weights(enc, plan, Cin, n_wtaps, KC, L.forms[3].P.N, &L.forms[3].mapB); r != CUDA_SUCCESS)
       return sb_fail(h, SB_ERR_CUDA, "cuTensorMapEncodeTiled(B, wide form) failed: %d", (int)r);

@@ -39,33 +39,20 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3,
-                                            int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
-}
 
 // K-major swizzled wgmma shared-memory matrix descriptor (sm_90 GMMA descriptor bit layout):
 //   [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1),
-//   [32,46) stride byte offset >> 4 = 8 rows x row_bytes, [62,64) layout: 1 = SW128, 2 = SW64, 3 = SW32.
-// Advancing K by 16 fp16 elements (32 bytes) inside the swizzle atom adds 2 to the start-address field.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, int row_bytes, int layout_type) {
+//   [32,46) stride byte offset >> 4 = distance between successive 8-row groups (default 8 rows x row_bytes),
+//   [49,52) matrix base offset (left 0), [62,64) layout: 1 = SW128, 2 = SW64, 3 = SW32.
+// Advancing K by 16 fp16 elements (32 bytes) inside the swizzle atom adds 2 to the start-address field.  The swizzle is
+// applied to the operand's shared-memory addresses, as TMA applies it when it writes: any start offset by whole rows from
+// a pattern-aligned base reads what TMA wrote there, with base offset 0 (tools/wgmma_rate.cu checks this bit for bit).
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, int row_bytes, int layout_type, uint32_t sbo = 0) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(((8 * row_bytes) >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)(((sbo ? sbo : 8 * row_bytes) >> 4) & 0x3FFF) << 32;
   d |= (uint64_t)layout_type << 62;
-  return d;
-}
-// Non-swizzled K-major descriptor (layout type 0) with explicit offsets.  The operand is built from 8-row x 16-byte core
-// matrices whose rows are 16 bytes apart; lbo = distance between the two core matrices of one K = 16 step, sbo = distance
-// between successive 8-row groups along M / N.  The start address only needs 16-byte alignment.
-__device__ __forceinline__ uint64_t make_desc_interleave(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
   return d;
 }
 
