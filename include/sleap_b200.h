@@ -223,9 +223,14 @@ int sb_infer_bottomup_dev(sb_handle_t h, int model_id, const uint8_t* frames_dev
  * top-down) follows these rules.  Refused (SB_ERR_INVALID, nothing queued): a submit with a slot other than 0 / 1 or B
  * outside [1, max batch]; a submit into a slot whose batch was not collected; a collect of a slot that holds no
  * batch, with another B than its submit, or before the batch submitted earlier into the other slot.  A slot read
- * (sb_bottomup_tracks, sb_bottomup_gathered, sb_topdown_tracks with slot 0 / 1) takes only the batch last collected
- * from that slot, with its B.  A configure call on the model (or either model of a top-down pipeline) drops the
- * submitted batches after their work has finished; collecting one then fails. */
+ * (sb_bottomup_tracks, sb_bottomup_gathered, sb_topdown_tracks; slot 0 / 1) takes only the batch last collected from
+ * that slot, with its B.  A configure call on the model (or either model of a top-down pipeline) drops the submitted
+ * batches after their work has finished; collecting one then fails.
+ * The synchronous call of each form (sb_infer_bottomup, sb_infer_multiclass, sb_infer_global, sb_infer_topdown,
+ * sb_infer_topdown_multiclass) runs its batch as a submit into slot 0 and its collect: it is refused (SB_ERR_INVALID,
+ * nothing queued) while a batch is submitted and not collected, and its batch is then the one last collected from slot
+ * 0.  The slots are allocated by the first submit or synchronous call: two of max_batch uint8 frames and pinned record
+ * staging per model (per pipeline for the top-down forms). */
 int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot);
 int sb_bottomup_collect(sb_handle_t h, int model_id, int slot, int B, float* out_instance_peaks,
                         float* out_instance_peak_vals, float* out_instance_scores,
@@ -323,8 +328,8 @@ int sb_gather_collect(sb_handle_t h, int model_id, int64_t step, int B, float* o
 int sb_gather_status(sb_handle_t h, int model_id, int32_t* out_status, int64_t* out_steps_pushed, int64_t* out_steps_consumed);
 /* With the exchange connected, sb_infer_bottomup / sb_bottomup_submit wait (on the device, behind the post-processing) for
  * every rank's records of their step and bring the WHOLE gather window to the host in the one result copy they do anyway
- * (their own outputs are the rank's slice of it).  sb_bottomup_gathered returns that copy: slot 0 / 1 after
- * sb_bottomup_collect(slot), slot -1 after sb_infer_bottomup.  out_records [world][B][width], out_counts [world]. */
+ * (their own outputs are the rank's slice of it).  sb_bottomup_gathered returns the copy of the batch last collected from
+ * slot 0 / 1 (slot 0 after sb_infer_bottomup).  out_records [world][B][width], out_counts [world]. */
 int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* out_records, int32_t* out_counts);
 int sb_gather_close(sb_handle_t h, int model_id);
 
@@ -395,8 +400,8 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
  * a copy stream into slot `slot`, then the instance stage of the batch submitted before it (waiting on the host for that
  * batch's crop count, which its centroid stage produced while the GPU ran it), then the batch's own centroid stage.
  * sb_topdown_collect queues the batch's instance stage if no submit did, and blocks until its records are on the host.
- * Also refused (SB_ERR_INVALID): sb_infer_topdown*, sb_infer_centroids on the centroid model and
- * sb_topdown_attach_tracker while a batch is submitted and not collected; a submit or collect of the other pipeline form.
+ * Also refused (SB_ERR_INVALID): sb_infer_centroids on the centroid model and sb_topdown_attach_tracker while a batch
+ * is submitted and not collected; a submit or collect of the other pipeline form.
  * A batch's instance stage, and with it the attached tracker's step, is queued by the next submit or by its collect:
  * sb_tracker_reset between a batch's submit and that point applies before the batch is tracked, and the attached tracker
  * must not be destroyed while a batch is submitted. */
@@ -572,7 +577,7 @@ int sb_track_instances(sb_handle_t h, int tracker_id, int B, int I, const double
  * id[I], tracking score[I]; flag != 0: the frame was not tracked -- SB_TRACK_INFEASIBLE, 2 = queue table full, or
  * SB_TRACK_OVER_CAPACITY, which only the top-down step can meet)
  * are a separate buffer: the result records and record_width do not change.  They come back with the result copy:
- * sb_bottomup_tracks(slot 0 / 1 after sb_bottomup_collect, -1 after sb_infer_bottomup); sb_bottomup_device_tracks
+ * sb_bottomup_tracks(slot 0 / 1, as every slot read; slot 0 after sb_infer_bottomup); sb_bottomup_device_tracks
  * copies the last step's records after sb_infer_bottomup_dev. */
 int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int max_instances, double img_h, double img_w);
 int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks);
@@ -587,8 +592,8 @@ int sb_bottomup_device_tracks(sb_handle_t h, int model_id, int B, double* out_tr
  * tracker must live on its handle and have its instance model's node count; img_h, img_w > 0.  The attachment lives
  * with the pipeline: a configure call on either model drops it.  sb_infer_topdown's outputs do not change.  Streamed
  * batches are tracked in submit order.  sb_topdown_tracks copies track records in the bottom-up format above, as
- * sb_bottomup_tracks does: slot -1, those of the last sb_infer_topdown; slot 0 / 1, those of the batch last collected
- * from that slot (B must be that batch's frame count). */
+ * sb_bottomup_tracks does: those of the batch last collected from slot 0 / 1 (slot 0 after sb_infer_topdown; B must be
+ * that batch's frame count). */
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w);
 int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks);
 

@@ -132,7 +132,7 @@ int sb_gather_init(sb_handle_t h, int model_id, int rank, int world, int generat
   SB_CUDA(h, cudaMalloc(&g.local, win_bytes(g)));
   SB_CUDA(h, cudaMemset(g.local, 0, win_bytes(g)));
   SB_CUDA(h, cudaHostAlloc((void**)&g.status_host, sizeof(int), cudaHostAllocMapped));
-  SB_CUDA(h, cudaHostAlloc((void**)&g.counts_host, sizeof(int) * SB_GATHER_MAX_WORLD * 4, cudaHostAllocMapped));   // [collect | slot 0 | slot 1 | sync]
+  SB_CUDA(h, cudaHostAlloc((void**)&g.counts_host, sizeof(int) * SB_GATHER_MAX_WORLD * 3, cudaHostAllocMapped));   // [collect | slot 0 | slot 1]
   *g.status_host = 0;
   SB_CUDA(h, cudaHostGetDevicePointer((void**)&g.status_dev, g.status_host, 0));
   SB_CUDA(h, cudaHostGetDevicePointer((void**)&g.counts_dev, g.counts_host, 0));
@@ -164,7 +164,6 @@ int sb_gather_connect(sb_handle_t h, int model_id, const void* all_ipc_handles) 
   g.step = 0;
   g.consumed = 0;
   m->slots.release();                              // host staging now holds [world][B][width] windows
-  if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
   return SB_OK;
 }
 

@@ -52,9 +52,8 @@ void sb_models_free(sb_handle_s* h) {
     if (m->weights_tc_dev) cudaFree(m->weights_tc_dev);
     if (m->frames_dev) cudaFree(m->frames_dev);
     sb_global_scratch_free(m->gs);
-    if (m->rec_host) cudaFreeHost(m->rec_host);
     if (m->trk_dev) cudaFree(m->trk_dev);
-    for (int i = 0; i < 3; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
+    for (int i = 0; i < 2; ++i) if (m->trk_host[i]) cudaFreeHost(m->trk_host[i]);
     m->slots.release();
     for (auto& e : m->fwd_events) cudaEventDestroy(e);
     sb_post_ws_free(m->ws);
@@ -82,7 +81,6 @@ static int chain_drop(sb_handle_s* h, SbModel* m) {
   h->post_pending = false;
   sb_post_ws_free(m->ws);
   m->slots.release();                            // staging is sized from the chain's record width
-  if (m->rec_host) { cudaFreeHost(m->rec_host); m->rec_host = nullptr; }
   sb_gather_free(m);                             // window sizes depend on (B, max_instances, n_nodes)
   m->trk = nullptr;                              // its checks (nodes, instance capacity) were made against the old chain
   sb_global_scratch_free(m->gs);
@@ -95,12 +93,12 @@ static int chain_drop(sb_handle_s* h, SbModel* m) {
 int sb_track_records_alloc(sb_handle_s* h, SbModel* m, int B, int I) {
   if (m->trk_B >= B && m->trk_I == I) return SB_OK;
   cudaFree(m->trk_dev); m->trk_dev = nullptr;
-  for (int i = 0; i < 3; ++i) { cudaFreeHost(m->trk_host[i]); m->trk_host[i] = nullptr; }
+  for (int i = 0; i < 2; ++i) { cudaFreeHost(m->trk_host[i]); m->trk_host[i] = nullptr; }
   m->trk_B = 0;
   const size_t n = (size_t)B * sb_track_record_width(I);
   int rc;
   if ((rc = sb_dev_alloc(h, &m->trk_dev, n))) return rc;
-  for (int i = 0; i < 3; ++i) SB_CUDA(h, cudaHostAlloc((void**)&m->trk_host[i], n * sizeof(double), cudaHostAllocDefault));
+  for (int i = 0; i < 2; ++i) SB_CUDA(h, cudaHostAlloc((void**)&m->trk_host[i], n * sizeof(double), cudaHostAllocDefault));
   m->trk_B = B; m->trk_I = I;
   return SB_OK;
 }
@@ -701,6 +699,11 @@ int SbSlots::check_read(sb_handle_s* h, const char* what, int slot, int B) const
   return 0;
 }
 
+int SbSlots::check_idle(sb_handle_s* h, const char* what) const {
+  if (busy()) return sb_fail(h, SB_ERR_INVALID, "%s: a batch was submitted and not collected; collect it first", what);
+  return 0;
+}
+
 void SbSlots::release() {
   for (int i = 0; i < 2; ++i) {
     if (frames[i]) cudaFree(frames[i]);
@@ -818,15 +821,16 @@ static int multiclass_post_kernels(sb_handle_s* h, const sb_multiclass_params& p
   return sbk_class_group(h, cls.dev, B, cls.H, cls.W, cls.C, (float)p.class_maps_output_stride, p.input_scale, ws);
 }
 
-// The step's chain on the head buffers: the multi-class one, or the PAF one with the record exchange pushed from k_group's
-// epilogue when connected, else the attached tracker after it.
-static int step_post_kernels(sb_handle_s* h, SbModel* m, int B) {
+// The step's chain on the head buffers: the global peaks (plus the device crop offsets crop_off, when given), the
+// multi-class one, or the PAF one with the record exchange pushed from k_group's epilogue when connected, else the
+// attached tracker after it.
+static int step_post_kernels(sb_handle_s* h, SbModel* m, int B, const float* crop_off) {
   if (m->chain == SB_CHAIN_GLOBAL) {
     const sb_global_params& p = m->gl;
     const SbBuffer& cb = m->buffers[p.cms_buffer];
     const SbGlobalScratch& g = m->gs;
     SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-    return sbk_global_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, nullptr, g.part,
+    return sbk_global_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp, crop_off, g.part,
                             g.chunks, g.rpc, g.points, g.vals);
   }
   if (m->chain == SB_CHAIN_CLASS) {
@@ -872,12 +876,12 @@ static int queue_track_copy(sb_handle_s* h, SbModel* m, int B, cudaStream_t rs, 
 // (run_ops waits on post_done_ev right before it overwrites a head buffer).  Without the overlap
 // (SB_DISABLE_POST_OVERLAP: no guard op) it still runs there, so that work a caller queues on the
 // post-processing stream stays behind it, and the handle's stream waits for it at once.
-static int bottomup_post(sb_handle_s* h, SbModel* m, int B) {
+static int bottomup_post(sb_handle_s* h, SbModel* m, int B, const float* crop_off = nullptr) {
   cudaStream_t main_stream = h->stream;
   SB_CUDA(h, cudaEventRecord(h->fwd_done_ev, main_stream));
   SB_CUDA(h, cudaStreamWaitEvent(h->post_stream, h->fwd_done_ev, 0));
   h->stream = h->post_stream;
-  int rc = step_post_kernels(h, m, B);
+  int rc = step_post_kernels(h, m, B, crop_off);
   cudaError_t e = cudaEventRecord(h->post_done_ev, h->post_stream);
   h->stream = main_stream;
   if (rc) return rc;
@@ -899,67 +903,22 @@ int sb_infer_bottomup_dev(sb_handle_t h, int model_id, const uint8_t* frames_dev
   return bottomup_post(h, m, B);
 }
 
-// One synchronous step of the configured chain: upload, network, post-processing, one result copy into rec_host.
-static int step_sync(sb_handle_s* h, SbModel* m, const void* frames_host, int frames_are_u8, int B) {
-  SB_CUDA(h, cudaSetDevice(h->device));
-  if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
-  int rc = upload_frames(h, m, frames_host, frames_are_u8, B);
-  if (rc) return rc;
-  if ((rc = sb_run_ops(h, m, m->frames_dev, frames_are_u8, B))) return rc;
-  if ((rc = bottomup_post(h, m, B))) return rc;
-  cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
-  if (!m->rec_host) SB_CUDA(h, cudaHostAlloc((void**)&m->rec_host, stage_floats(m) * sizeof(float), cudaHostAllocDefault));
-  if ((rc = queue_result_copy(h, m, B, rs, m->rec_host, 3))) return rc;
-  if ((rc = queue_track_copy(h, m, B, rs, 2))) return rc;
-  SB_CUDA(h, cudaStreamSynchronize(rs));
-  h->post_pending = false;
-  m->rec_B = B;
-  return check_exchange(h, m);
+// The streamed steps of the chain: submit batch i + 1 (its upload runs on the slots' copy stream) while batch i computes,
+// then collect batch i; ONE D2H copy per batch brings the per-frame records into the slot's staging.  A synchronous call
+// is one step into slot 0 and its collect.
+
+static int slots_alloc(sb_handle_s* h, SbModel* m) {
+  return m->slots.alloc(h, (size_t)m->B * m->Hin * m->Win * m->Cin, stage_floats(m));
 }
 
-int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, float* out_instance_peaks,
-                      float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
-                      int32_t* out_flags) {
-  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
-  if (!m) return SB_ERR_INVALID;
-  if (const int rc = step_sync(h, m, frames_host, 1, B)) return rc;
-  split_paf_records(m, own_slice(m, m->rec_host, B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores, out_n_valid, out_flags);
-  return SB_OK;
-}
-
-int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B, float* out_points,
-                        float* out_vals, float* out_class_probs, int32_t* out_flags) {
-  SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
-  if (!m) return SB_ERR_INVALID;
-  if (!frames_host || !out_points || !out_vals || !out_class_probs) return sb_fail(h, SB_ERR_INVALID, "sb_infer_multiclass: null argument");
-  if (const int rc = step_sync(h, m, frames_host, frames_are_u8 ? 1 : 0, B)) return rc;
-  split_class_records(m->mc, m->rec_host, B, out_points, out_vals, out_class_probs, out_flags);
-  return SB_OK;
-}
-
-// The stream post-processing runs on (consumers such as the NCCL gather can be queued behind it).
-int sb_get_post_stream(sb_handle_t h, void** out_stream) {
-  if (!h || !out_stream) return sb_fail(h, SB_ERR_INVALID, "null argument");
-  *out_stream = (void*)h->post_stream;
-  return SB_OK;
-}
-
-// The streamed form of the chain's synchronous step: submit batch i + 1 (its upload runs on the slots' copy stream) while
-// batch i computes, then collect batch i; ONE D2H copy per batch brings the per-frame records into the slot's staging.
-
-static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot, const char* what) {
+// Queues the step of B frames at frames_dev into `slot`: network, post-processing (crop_off: the global chain's device
+// crop offsets, or nullptr), the result and track copies into the slot's staging, its events.  The batch is then submitted.
+static int queue_step(sb_handle_s* h, SbModel* m, const void* frames_dev, int frames_are_u8, int B, int slot, const float* crop_off) {
   SbSlots& sl = m->slots;
-  int rc = sl.check_submit(h, what, slot, B, m->B, frames_host);
-  if (rc) return rc;
-  SB_CUDA(h, cudaSetDevice(h->device));
-  if ((rc = sl.alloc(h, (size_t)m->B * m->Hin * m->Win * m->Cin, stage_floats(m))) ||
-      (rc = sl.upload(h, slot, frames_host, (size_t)B * m->Hin * m->Win * m->Cin)))
-    return rc;
-  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
-  rc = sb_run_ops(h, m, sl.frames[slot], 1, B);
+  int rc = sb_run_ops(h, m, frames_dev, frames_are_u8, B);
   if (rc) return rc;
   SB_CUDA(h, cudaEventRecord(sl.frames_free[slot], h->stream));
-  if ((rc = bottomup_post(h, m, B))) return rc;
+  if ((rc = bottomup_post(h, m, B, crop_off))) return rc;
   cudaStream_t rs = h->post_pending ? h->post_stream : h->stream;
   if ((rc = queue_result_copy(h, m, B, rs, sl.stage[slot], 1 + slot))) return rc;
   if ((rc = queue_track_copy(h, m, B, rs, slot))) return rc;
@@ -968,11 +927,64 @@ static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, i
   return SB_OK;
 }
 
+static int step_submit(sb_handle_s* h, SbModel* m, const uint8_t* frames_host, int B, int slot, const char* what) {
+  SbSlots& sl = m->slots;
+  int rc = sl.check_submit(h, what, slot, B, m->B, frames_host);
+  if (rc) return rc;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if ((rc = slots_alloc(h, m)) || (rc = sl.upload(h, slot, frames_host, (size_t)B * m->Hin * m->Win * m->Cin))) return rc;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
+  return queue_step(h, m, sl.frames[slot], 1, B, slot, nullptr);
+}
+
 // Blocks until the records of the batch submitted into `slot` are in its pinned staging.
 static int step_collect(sb_handle_s* h, SbModel* m, int slot, int B, const char* what) {
   int rc = m->slots.check_collect(h, what, slot, B);
   if (rc || (rc = m->slots.collect(h, slot))) return rc;
   return check_exchange(h, m);
+}
+
+// A synchronous call: the uint8 or float32 frames (and the global chain's crop offsets, when given) uploaded on the
+// handle's stream into frames_dev, the step queued into slot 0, then slot 0 collected.
+static int step_call(sb_handle_s* h, SbModel* m, const void* frames_host, int frames_are_u8, int B, const float* crop_off_host,
+                     const char* what) {
+  if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "%s: bad batch", what);
+  int rc = m->slots.check_idle(h, what);
+  if (rc) return rc;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if ((rc = slots_alloc(h, m)) || (rc = upload_frames(h, m, frames_host, frames_are_u8, B))) return rc;
+  if (crop_off_host)
+    SB_CUDA(h, cudaMemcpyAsync(m->gs.crop_off, crop_off_host, (size_t)B * 2 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  if ((rc = queue_step(h, m, m->frames_dev, frames_are_u8, B, 0, crop_off_host ? m->gs.crop_off : nullptr))) return rc;
+  return step_collect(h, m, 0, B, what);
+}
+
+int sb_infer_bottomup(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, float* out_instance_peaks,
+                      float* out_instance_peak_vals, float* out_instance_scores, int32_t* out_n_valid,
+                      int32_t* out_flags) {
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, kNoPaf);
+  if (!m) return SB_ERR_INVALID;
+  if (const int rc = step_call(h, m, frames_host, 1, B, nullptr, "sb_infer_bottomup")) return rc;
+  split_paf_records(m, own_slice(m, m->slots.stage[0], B), B, out_instance_peaks, out_instance_peak_vals, out_instance_scores,
+                    out_n_valid, out_flags);
+  return SB_OK;
+}
+
+int sb_infer_multiclass(sb_handle_t h, int model_id, const void* frames_host, int frames_are_u8, int B, float* out_points,
+                        float* out_vals, float* out_class_probs, int32_t* out_flags) {
+  SbModel* m = chain_model(h, model_id, SB_CHAIN_CLASS, kNoClass);
+  if (!m) return SB_ERR_INVALID;
+  if (!frames_host || !out_points || !out_vals || !out_class_probs) return sb_fail(h, SB_ERR_INVALID, "sb_infer_multiclass: null argument");
+  if (const int rc = step_call(h, m, frames_host, frames_are_u8 ? 1 : 0, B, nullptr, "sb_infer_multiclass")) return rc;
+  split_class_records(m->mc, m->slots.stage[0], B, out_points, out_vals, out_class_probs, out_flags);
+  return SB_OK;
+}
+
+// The stream post-processing runs on (consumers such as the NCCL gather can be queued behind it).
+int sb_get_post_stream(sb_handle_t h, void** out_stream) {
+  if (!h || !out_stream) return sb_fail(h, SB_ERR_INVALID, "null argument");
+  *out_stream = (void*)h->post_stream;
+  return SB_OK;
 }
 
 int sb_bottomup_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
@@ -1008,15 +1020,11 @@ int sb_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* o
 int sb_bottomup_gathered(sb_handle_t h, int model_id, int slot, int B, float* out_records, int32_t* out_counts) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_gathered: exchange not connected");
   if (!m || !m->gather.connected) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: exchange not connected");
-  if (slot < -1 || slot > 1 || !out_records) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: bad slot");
-  if (slot < 0 && (!m->rec_host || m->rec_B != B))
-    return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: no collected batch of %d frames in that slot", B);
-  if (slot >= 0)
-    if (const int rc = m->slots.check_read(h, "sb_bottomup_gathered", slot, B)) return rc;
-  const float* src = slot < 0 ? m->rec_host : m->slots.stage[slot];
-  memcpy(out_records, src, (size_t)m->gather.world * B * sb_record_width(m->bu.max_instances, m->bu.n_nodes) * sizeof(float));
+  if (!out_records) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_gathered: bad slot");
+  if (const int rc = m->slots.check_read(h, "sb_bottomup_gathered", slot, B)) return rc;
+  memcpy(out_records, m->slots.stage[slot], (size_t)m->gather.world * B * sb_record_width(m->bu.max_instances, m->bu.n_nodes) * sizeof(float));
   if (out_counts)
-    for (int r = 0; r < m->gather.world; ++r) out_counts[r] = m->gather.counts_host[(slot < 0 ? 3 : 1 + slot) * SB_GATHER_MAX_WORLD + r];
+    for (int r = 0; r < m->gather.world; ++r) out_counts[r] = m->gather.counts_host[(1 + slot) * SB_GATHER_MAX_WORLD + r];
   return SB_OK;
 }
 
@@ -1042,10 +1050,9 @@ int sb_bottomup_attach_tracker(sb_handle_t h, int model_id, int tracker_id, int 
 int sb_bottomup_tracks(sb_handle_t h, int model_id, int slot, int B, double* out_tracks) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_PAF, "sb_bottomup_tracks: no tracker attached");
   if (!m || !m->trk) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: no tracker attached");
-  if (slot < -1 || slot > 1 || B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: bad slot / batch");
-  if (slot >= 0)
-    if (const int rc = m->slots.check_read(h, "sb_bottomup_tracks", slot, B)) return rc;
-  memcpy(out_tracks, m->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double));
+  if (slot < 0 || slot > 1 || B <= 0 || B > m->trk_B || !out_tracks) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_tracks: bad slot / batch");
+  if (const int rc = m->slots.check_read(h, "sb_bottomup_tracks", slot, B)) return rc;
+  memcpy(out_tracks, m->trk_host[slot], (size_t)B * sb_track_record_width(m->trk_I) * sizeof(double));
   return SB_OK;
 }
 
@@ -1170,6 +1177,13 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
 // ---------------------------------- global peaks (single / centered instance) ----------------
 static const char* const kNoGlobal = "global-peak predictor not configured";
 
+// The points and values of the first B frames of the global chain's block staged in `slot`
+static void split_global(const SbModel* m, int slot, int B, float* out_points, float* out_vals) {
+  const size_t C = m->buffers[m->gl.cms_buffer].C;
+  memcpy(out_points, m->slots.stage[slot], (size_t)B * C * 2 * sizeof(float));
+  memcpy(out_vals, m->slots.stage[slot] + (size_t)m->B * C * 2, (size_t)B * C * sizeof(float));
+}
+
 int sb_global_configure(sb_handle_t h, int model_id, const sb_global_params* p) {
   SbModel* m = configure_target(h, model_id, p);
   if (!m) return SB_ERR_INVALID;
@@ -1191,30 +1205,13 @@ int sb_infer_global(sb_handle_t h, int model_id, const void* images_host, int im
                     const float* crop_offsets_host, float* out_points, float* out_vals) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
   if (!m) return SB_ERR_INVALID;
-  SB_CUDA(h, cudaSetDevice(h->device));
-  if (B <= 0 || B > m->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
-  if (h->post_pending) {             // a streamed batch's peaks and result copy may still use the scratch
-    SB_CUDA(h, cudaStreamSynchronize(h->post_stream));
-    h->post_pending = false;
-  }
-  int rc = upload_frames(h, m, images_host, images_are_u8, B);
-  if (rc) return rc;
-  const SbGlobalScratch& g = m->gs;
-  if (crop_offsets_host) SB_CUDA(h, cudaMemcpyAsync(g.crop_off, crop_offsets_host, (size_t)B * 8, cudaMemcpyHostToDevice, h->stream));
-  if ((rc = sb_run_ops(h, m, m->frames_dev, images_are_u8, B))) return rc;
-  const sb_global_params& p = m->gl;
-  SbBuffer& cb = m->buffers[p.cms_buffer];
-  SbPeakParams pp{p.peak_threshold, p.refinement, p.integral_patch_size, (float)p.output_stride, p.input_scale};
-  if ((rc = sbk_global_peaks(h, (const float*)cb.dev, head_offsets(m, p.offsets_buffer), B, cb.H, cb.W, cb.C, pp,
-                             crop_offsets_host ? g.crop_off : nullptr, g.part, g.chunks, g.rpc, g.points, g.vals))) return rc;
-  SB_CUDA(h, cudaMemcpyAsync(out_points, g.points, (size_t)B * cb.C * 8, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(out_vals, g.vals, (size_t)B * cb.C * 4, cudaMemcpyDeviceToHost, h->stream));
-  SB_CUDA(h, cudaStreamSynchronize(h->stream));
+  if (const int rc = step_call(h, m, images_host, images_are_u8 ? 1 : 0, B, crop_offsets_host, "sb_infer_global")) return rc;
+  split_global(m, 0, B, out_points, out_vals);
   return SB_OK;
 }
 
-// The double-buffered form of sb_infer_global (uint8 frames, no crop offsets): the chain's global peaks run on the
-// post-processing stream, as the bottom-up chains do, and the points | values block comes back in one copy.
+// The double-buffered form of sb_infer_global (uint8 frames, no crop offsets): the points | values block comes back in
+// one copy.
 int sb_global_submit(sb_handle_t h, int model_id, const uint8_t* frames_host, int B, int slot) {
   SbModel* m = chain_model(h, model_id, SB_CHAIN_GLOBAL, kNoGlobal);
   return m ? step_submit(h, m, frames_host, B, slot, "sb_global_submit") : SB_ERR_INVALID;
@@ -1225,9 +1222,7 @@ int sb_global_collect(sb_handle_t h, int model_id, int slot, int B, float* out_p
   if (!m) return SB_ERR_INVALID;
   if (!out_points || !out_vals) return sb_fail(h, SB_ERR_INVALID, "sb_global_collect: null argument");
   if (const int rc = step_collect(h, m, slot, B, "sb_global_collect")) return rc;
-  const size_t C = m->buffers[m->gl.cms_buffer].C;
-  memcpy(out_points, m->slots.stage[slot], (size_t)B * C * 2 * sizeof(float));
-  memcpy(out_vals, m->slots.stage[slot] + (size_t)m->B * C * 2, (size_t)B * C * sizeof(float));
+  split_global(m, slot, B, out_points, out_vals);
   return SB_OK;
 }
 

@@ -107,8 +107,10 @@ enum { SB_CHAIN_ANY = -1, SB_CHAIN_NONE = 0, SB_CHAIN_PAF, SB_CHAIN_CLASS, SB_CH
 
 // The two slots of a streamed (submit / collect) step and the rules of the streamed steps (include/sleap_b200.h): a
 // submit goes into a slot that holds no batch; a collect takes a slot's batch with its B, oldest first; a slot read
-// takes the batch last collected from that slot with its B.  A check that fails returns SB_ERR_INVALID with `what`
-// before its message and changes nothing.  Buffers, stream and events are allocated by the first submit after release().
+// takes the batch last collected from that slot with its B; a synchronous call runs one batch into slot 0 and collects it,
+// and is refused while a batch is submitted and not collected.  A check that fails returns SB_ERR_INVALID with `what`
+// before its message and changes nothing.  Buffers, stream and events are allocated by the first submit or synchronous
+// call after release().
 struct SbSlots {
   cudaStream_t copy_stream = nullptr;
   void* frames[2] = {nullptr, nullptr};            // device uint8 frames of the slot's batch
@@ -131,6 +133,7 @@ struct SbSlots {
   int collect(sb_handle_s* h, int slot);           // waits for result[slot]; the slot is free again
   int check_read(sb_handle_s* h, const char* what, int slot, int B) const;
   bool busy() const { return slot_B[0] || slot_B[1]; }
+  int check_idle(sb_handle_s* h, const char* what) const;   // refuses a synchronous call while busy()
   void release();
 };
 
@@ -166,10 +169,9 @@ struct SbModel {
   std::vector<int> bu_edges;
   sb_multiclass_params mc{};
   int guard_op = -1;                       // first op that overwrites a head buffer the post-processing stream may still read
-  // the streamed steps of the chain (sb_bottomup_*, sb_multiclass_*, sb_global_*), staging the chain's records
+  // the steps of the chain (sb_infer_bottomup / _multiclass / _global into slot 0, and the streamed sb_bottomup_*,
+  // sb_multiclass_*, sb_global_*), staging the chain's records
   SbSlots slots;
-  float* rec_host = nullptr;                     // pinned staging of the synchronous sb_infer_bottomup
-  int rec_B = 0;                                 // frames of the batch in rec_host
   sb_global_params gl{};
   SbGlobalScratch gs;
   sb_centroid_params ce{};
@@ -183,7 +185,7 @@ struct SbModel {
   int trk_B = 0, trk_I = 0, trk_cut = -1;
   double trk_h = 1.0, trk_w = 1.0;
   double* trk_dev = nullptr;
-  double* trk_host[3] = {nullptr, nullptr, nullptr};   // pinned: collect slots 0 / 1, sb_infer_bottomup
+  double* trk_host[2] = {nullptr, nullptr};   // pinned: slots 0 / 1
 };
 
 // The network input of H x W frames as sb_model_configure plans it: resized by the PREPROCESS op's input_scale

@@ -21,7 +21,6 @@
 // product would round differently from the definition (include/sleap_b200.h).
 #include <algorithm>
 #include <limits>
-#include <time.h>
 
 #include <math_constants.h>
 
@@ -351,8 +350,6 @@ struct SbTopdown {
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
   void* crops = nullptr;
-  float* record_host = nullptr;
-  int* total_host = nullptr;
   // multi-class form (sb_topdown_multiclass_configure)
   bool multiclass = false;
   TdHead head{};
@@ -360,13 +357,15 @@ struct SbTopdown {
   bool tap_half = false, all_stores = false;   // fp16 storage; the production program elides the tap buffer
   float* dense = nullptr;                      // packed dense weights
   float* probs = nullptr;                      // [Bmax * K][n_classes] per-crop class probabilities
-  // streaming (sb_topdown_submit / _collect, sb_topdown_gt_submit), allocated at the first submit: the slots (frames,
-  // record staging), and per slot the pinned crop count and its event and, multi-class, the pinned class probabilities of
-  // its crops; `pending` is the slot whose instance stage is not queued yet (-1: none)
+  // the steps (sb_topdown_submit / _collect, sb_topdown_gt_submit, and sb_infer_topdown* into slot 0), allocated at the
+  // first of them: the slots (frames, record staging), and per slot the pinned crop count and its event, the frames its
+  // crops are cut from and, multi-class, the pinned class probabilities of its crops; `pending` is the slot whose instance
+  // stage is not queued yet (-1: none)
   SbSlots slots;
   int* count_host = nullptr;                   // [2]
   float* probs_stage[2] = {nullptr, nullptr};  // [Bmax * K][n_classes]
   cudaEvent_t count_ev[2] = {nullptr, nullptr};
+  struct { const void* dev; int is_u8; } src[2] = {};   // the slot's frames, or a synchronous call's frames_dev
   int pending = -1;
   // ground-truth form (sb_topdown_params.centroid_model = -1), held by its instance model.  gt_flags: the per-frame flags,
   // which k_td_gt_select zeroes; gt_cent / gt_count: per slot the device copy of the batch's centroid table and counts,
@@ -385,7 +384,7 @@ void sb_topdown_free(SbModel* m) {
                  t->gt_count[1]};
   for (void* p : dev) if (p) cudaFree(p);
   t->slots.release();
-  for (void* p : {(void*)t->record_host, (void*)t->total_host, (void*)t->count_host, (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
+  for (void* p : {(void*)t->count_host, (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
     if (p) cudaFreeHost(p);
   for (cudaEvent_t e : t->count_ev) if (e) cudaEventDestroy(e);
   delete t;
@@ -457,8 +456,7 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
                   (!t->multiclass || A((void**)&t->probs, N * n_classes * 4)) &&
                   (mc || A((void**)&t->gt_flags, (size_t)max_batch * 4));
   t->flags = mc ? mc->ws.flags : t->gt_flags;
-  if (!ok || cudaHostAlloc((void**)&t->record_host, (size_t)max_batch * t->width * 4, cudaHostAllocDefault) != cudaSuccess ||
-      cudaHostAlloc((void**)&t->total_host, 4, cudaHostAllocDefault) != cudaSuccess) {
+  if (!ok) {
     sb_topdown_free(owner);
     return sb_fail(h, SB_ERR_CUDA, "sb_topdown_configure: allocation failed");
   }
@@ -513,13 +511,6 @@ SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = f
   return t;
 }
 
-// Refuses a call that would overwrite the single selection, crop and record buffers while a streamed batch holds them
-int check_idle(sb_handle_s* h, const SbTopdown* t, const char* what) {
-  if (t->slots.busy())
-    return sb_fail(h, SB_ERR_INVALID, "%s: a batch was submitted and not collected; collect it first", what);
-  return 0;
-}
-
 // The flat crop list and crop offsets of the B frames' selected centroids, on the handle's stream
 int flatten(sb_handle_s* h, SbTopdown* t, int B) {
   k_td_flatten<<<1, 256, 0, h->stream>>>(t->sel_cent, t->sel_count, B, t->K, (float)t->p.crop_size * 0.5f, t->flat_cent, t->flat_off,
@@ -552,10 +543,10 @@ int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
 // The instance stage of the batch the centroid stage left in the selection buffers (`total` crops of the B frames at
 // frames_dev): per chunk of crops the crop kernel, the instance network, the global peaks and, multi-class, the class
 // vectors; frames_free (given) after the last crop kernel; then the records -- k_td_class_assign, or k_td_pack and the
-// attached tracker of the centroid model mc (NULL in the ground-truth form) -- copied into rec_host, the track records into
+// attached tracker of the centroid model mc (NULL in the ground-truth form) -- copied into rec_dst, the track records into
 // trk_host and, given, the crops' class probabilities into probs_host.
 int instance_stage(sb_handle_s* h, const SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int total,
-                   float* rec_host, double* trk_host, float* probs_host, cudaEvent_t frames_free) {
+                   float* rec_dst, double* trk_host, float* probs_host, cudaEvent_t frames_free) {
   cudaStream_t s = h->stream;
   SbModel* mi = t->inst;
   const sb_global_params& gp = mi->gl;
@@ -602,41 +593,12 @@ int instance_stage(sb_handle_s* h, const SbModel* mc, SbTopdown* t, const void* 
                                  cudaMemcpyDeviceToHost, s));
     }
   }
-  SB_CUDA(h, cudaMemcpyAsync(rec_host, t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, s));
+  SB_CUDA(h, cudaMemcpyAsync(rec_dst, t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, s));
   return 0;
 }
 
-// One synchronous batch: frames up, the centroid stage, the one mid-pipeline sync (how many crops the instance network
-// runs on), the instance stage, the final sync.  The records land in t->record_host.
-int topdown_run(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_host, int frames_are_u8, int B, const char* what) {
-  if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
-  if (const int rc = check_idle(h, t, what)) return rc;
-  SB_CUDA(h, cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
-  const size_t esz = frames_are_u8 ? 1 : 4;
-  static const bool dbg = getenv("SB_DEBUG_TD") != nullptr;      // stage timing (host clock around stream syncs), profiling only
-  auto now = []() { timespec t; clock_gettime(CLOCK_MONOTONIC, &t); return t.tv_sec * 1e3 + t.tv_nsec * 1e-6; };
-  double t0 = now(), t1 = 0, t2 = 0, t3 = 0;
-  SB_CUDA(h, cudaMemcpyAsync(mc->frames_dev, frames_host, (size_t)B * mc->Hin * mc->Win * mc->Cin * esz, cudaMemcpyHostToDevice, s));
-  if (dbg) { cudaStreamSynchronize(s); t1 = now(); }
-  int rc = centroid_stage(h, mc, t, mc->frames_dev, frames_are_u8, B, t->total_host, nullptr);
-  if (rc) return rc;
-  SB_CUDA(h, cudaStreamSynchronize(s));
-  const int total = *t->total_host;
-  if (dbg) t2 = now();
-  if ((rc = instance_stage(h, mc, t, mc->frames_dev, frames_are_u8, B, total, t->record_host, mc->trk_host[2], nullptr, nullptr)))
-    return rc;
-  SB_CUDA(h, cudaStreamSynchronize(s));
-  if (dbg) {
-    t3 = now();
-    fprintf(stderr, "[sb_infer_topdown] B=%d crops=%d: H2D %.3f ms, centroid stage %.3f ms, instance stage + D2H %.3f ms\n", B, total, t1 - t0,
-            t2 - t1, t3 - t2);
-  }
-  return SB_OK;
-}
-
-// Queues the instance stage of the pending streamed batch (its count event waited for on the host) behind whatever the
-// handle's stream holds.  The slot is dropped when it fails.
+// Queues the instance stage of the pending batch (its count event waited for on the host) behind whatever the handle's
+// stream holds.  The slot is dropped when it fails.
 int queue_pending_instance(sb_handle_s* h, const SbModel* mc, SbTopdown* t) {
   const int k = t->pending;
   SbSlots& sl = t->slots;
@@ -644,8 +606,8 @@ int queue_pending_instance(sb_handle_s* h, const SbModel* mc, SbTopdown* t) {
   cudaError_t e = cudaEventSynchronize(t->count_ev[k]);
   int rc = e == cudaSuccess ? 0 : sb_fail(h, SB_ERR_CUDA, "crop count: %s", cudaGetErrorString(e));
   if (!rc) {
-    rc = instance_stage(h, mc, t, sl.frames[k], 1, sl.slot_B[k], t->count_host[k], sl.stage[k], mc->trk_host[k], t->probs_stage[k],
-                        sl.frames_free[k]);
+    rc = instance_stage(h, mc, t, t->src[k].dev, t->src[k].is_u8, sl.slot_B[k], t->count_host[k], sl.stage[k], mc->trk_host[k],
+                        t->probs_stage[k], sl.frames_free[k]);
   }
   if (!rc) {
     e = cudaEventRecord(sl.result[k], h->stream);
@@ -655,7 +617,7 @@ int queue_pending_instance(sb_handle_s* h, const SbModel* mc, SbTopdown* t) {
   return rc;
 }
 
-// The streaming buffers of the pipeline, allocated at its first submit (synchronous users never pay for them)
+// The slot buffers of the pipeline, allocated at its first step
 int stream_alloc(sb_handle_s* h, SbTopdown* t) {
   int rc = t->slots.alloc(h, (size_t)t->Bmax * t->H * t->W * t->C, (size_t)t->Bmax * t->width);
   if (rc || t->count_host) return rc;
@@ -668,6 +630,16 @@ int stream_alloc(sb_handle_s* h, SbTopdown* t) {
   }
   SB_CUDA(h, cudaHostAlloc((void**)&t->count_host, 2 * sizeof(int), cudaHostAllocDefault));   // last: marks it complete
   return 0;
+}
+
+// The centroid stage of B frames at frames_dev queued as the batch of `slot`; its instance stage is queued by the next
+// submit or by the slot's collect.
+int queue_centroids(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int slot) {
+  if (const int rc = centroid_stage(h, mc, t, frames_dev, frames_are_u8, B, t->count_host + slot, t->count_ev[slot])) return rc;
+  t->slots.submitted(slot, B);
+  t->src[slot] = {frames_dev, frames_are_u8};
+  t->pending = slot;
+  return SB_OK;
 }
 
 // Streamed batch into `slot`: (1) its upload on the copy stream into the slot's frames, once the crops of the batch that
@@ -684,10 +656,7 @@ int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, in
   if ((rc = stream_alloc(h, t)) || (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C))) return rc;
   if (t->pending >= 0 && (rc = queue_pending_instance(h, mc, t))) return rc;
   SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
-  if ((rc = centroid_stage(h, mc, t, sl.frames[slot], 1, B, t->count_host + slot, t->count_ev[slot]))) return rc;
-  sl.submitted(slot, B);
-  t->pending = slot;
-  return SB_OK;
+  return queue_centroids(h, mc, t, sl.frames[slot], 1, B, slot);
 }
 
 // Streamed batch with ground-truth centroids into `slot`, the whole step queued at once (the host knows the crop count):
@@ -732,6 +701,21 @@ int topdown_collect(sb_handle_s* h, int id, SbTopdown* t, int slot, int B) {
   SB_CUDA(h, cudaSetDevice(h->device));
   if (t->pending == slot && (rc = queue_pending_instance(h, h->models[id], t))) return rc;
   return t->slots.collect(h, slot);
+}
+
+// A synchronous batch of the pipeline held by centroid model `id`: the uint8 or float32 frames uploaded on the handle's
+// stream into the model's frames_dev, the step queued into slot 0, then slot 0 collected.
+int topdown_call(sb_handle_s* h, int id, SbTopdown* t, const void* frames_host, int frames_are_u8, int B, const char* what) {
+  SbModel* mc = h->models[id];
+  if (B <= 0 || B > t->Bmax || B > mc->B) return sb_fail(h, SB_ERR_INVALID, "bad batch");
+  int rc = t->slots.check_idle(h, what);
+  if (rc) return rc;
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if ((rc = stream_alloc(h, t))) return rc;
+  SB_CUDA(h, cudaMemcpyAsync(mc->frames_dev, frames_host, (size_t)B * mc->Hin * mc->Win * mc->Cin * (frames_are_u8 ? 1 : 4),
+                             cudaMemcpyHostToDevice, h->stream));
+  if ((rc = queue_centroids(h, mc, t, mc->frames_dev, frames_are_u8, B, 0))) return rc;
+  return topdown_collect(h, id, t, 0, B);
 }
 
 // A plain record's fields into the caller's arrays
@@ -783,9 +767,8 @@ int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_ho
                      int32_t* out_flags) {
   SbTopdown* t = topdown_of(h, centroid_model_id, false);
   if (!t) return SB_ERR_INVALID;
-  SbModel* mc = h->models[centroid_model_id];
-  if (const int rc = topdown_run(h, mc, t, frames_host, frames_are_u8, B, "sb_infer_topdown")) return rc;
-  split_topdown(t, t->record_host, B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
+  if (const int rc = topdown_call(h, centroid_model_id, t, frames_host, frames_are_u8, B, "sb_infer_topdown")) return rc;
+  split_topdown(t, t->slots.stage[0], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
   return SB_OK;
 }
 
@@ -815,7 +798,7 @@ int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_
   SbTopdown* t = topdown_of(h, centroid_model_id, false);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[centroid_model_id];
-  if (const int rc = check_idle(h, t, "sb_topdown_attach_tracker")) return rc;
+  if (const int rc = t->slots.check_idle(h, "sb_topdown_attach_tracker")) return rc;
   if (tracker_id < 0) { mc->trk = nullptr; return SB_OK; }
   SbTracker* tr = sb_tracker_get(h, tracker_id);
   if (!tr) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_attach_tracker: no tracker %d on this handle", tracker_id);
@@ -829,17 +812,15 @@ int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_
   return SB_OK;
 }
 
-// slot -1: the records of the last sb_infer_topdown; slot 0 / 1: those of the batch last collected from that slot.
 int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, slot >= 0);
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
   if (!t) return SB_ERR_INVALID;
   const SbModel* mc = h->models[centroid_model_id];
   if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
-  if (slot < -1 || slot > 1 || B <= 0 || B > t->Bmax || !out_tracks)
+  if (slot < 0 || slot > 1 || B <= 0 || B > t->Bmax || !out_tracks)
     return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: bad slot / batch");
-  if (slot >= 0)
-    if (const int rc = t->slots.check_read(h, "sb_topdown_tracks", slot, B)) return rc;
-  memcpy(out_tracks, mc->trk_host[slot < 0 ? 2 : slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
+  if (const int rc = t->slots.check_read(h, "sb_topdown_tracks", slot, B)) return rc;
+  memcpy(out_tracks, mc->trk_host[slot], (size_t)B * sb_track_record_width(mc->trk_I) * sizeof(double));
   return SB_OK;
 }
 
@@ -886,11 +867,9 @@ int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void
                                 float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors) {
   SbTopdown* t = topdown_of(h, centroid_model_id, true);
   if (!t) return SB_ERR_INVALID;
-  if (const int rc = topdown_run(h, h->models[centroid_model_id], t, frames_host, frames_are_u8, B, "sb_infer_topdown_multiclass")) return rc;
-  std::vector<float> pr(out_class_vectors ? (size_t)*t->total_host * t->head.n_classes : 0);
-  if (!pr.empty()) SB_CUDA(h, cudaMemcpy(pr.data(), t->probs, pr.size() * 4, cudaMemcpyDeviceToHost));
-  split_topdown_multiclass(t, t->record_host, pr.data(), B, out_centroids, out_centroid_vals, out_points, out_vals, out_class_probs,
-                           out_n_valid, out_flags, out_class_vectors);
+  if (const int rc = topdown_call(h, centroid_model_id, t, frames_host, frames_are_u8, B, "sb_infer_topdown_multiclass")) return rc;
+  split_topdown_multiclass(t, t->slots.stage[0], t->probs_stage[0], B, out_centroids, out_centroid_vals, out_points, out_vals,
+                           out_class_probs, out_n_valid, out_flags, out_class_vectors);
   return SB_OK;
 }
 
@@ -958,13 +937,13 @@ int sb_topdown_multiclass_from_features(sb_handle_t h, const sb_topdown_multicla
       return rc;
   }
   if ((rc = launch_class_assign(h, nullptr, nullptr, d_count, d_offsets, pts, vals, probs, B, K, n_nodes, NC, nullptr, rec))) return rc;
-  std::vector<float> rec_host((size_t)B * width);
-  if ((rc = s.to_host(rec_host.data(), rec, rec_host.size())) ||
+  std::vector<float> records((size_t)B * width);
+  if ((rc = s.to_host(records.data(), rec, records.size())) ||
       (n_crops > 0 && (rc = s.to_host(out_class_vectors, probs, (size_t)n_crops * NC, true))) ||
       (n_crops > 0 && (rc = s.to_host(out_features, (const float*)fout, (size_t)n_crops * d.n_in, true))) || (rc = s.sync()))
     return rc;
   const size_t n1 = (size_t)NC * n_nodes;
-  sb_split_records(rec_host.data(), B, width, {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}}, {});
+  sb_split_records(records.data(), B, width, {{out_points, n1 * 2}, {out_vals, n1}, {out_class_probs, (size_t)NC}}, {});
   return SB_OK;
 }
 

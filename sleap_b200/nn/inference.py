@@ -198,7 +198,7 @@ def _track_fields(rec):
 
 def _step_tracks(m, fn, tracker, slot, B):
     """The track fields of the B frames a step of model ``m`` returned, read with ``fn`` (sb_bottomup_tracks or
-    sb_topdown_tracks) from slot 0 / 1 or, with -1, from the synchronous call; none without ``tracker``."""
+    sb_topdown_tracks) from slot 0 / 1 (slot 0 after the synchronous call); none without ``tracker``."""
     if tracker is None:
         return {}
     rec = np.zeros((B, 2 + 3 * tracker._device.max_instances), np.float64)
@@ -621,9 +621,9 @@ class TopDownInferenceModel(InferenceModel):
             mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
         return K
 
-    def _run_fused(self, B, K, fn, *args, slot=-1):
+    def _run_fused(self, B, K, fn, *args, slot=0):
         """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown or sb_topdown_collect) into dense arrays
-        of B frames, as a batch dict; with a tracker, the track records of ``slot`` (-1: sb_infer_topdown)."""
+        of B frames, as a batch dict; with a tracker, the track records of ``slot`` (0 after sb_infer_topdown)."""
         mc, n_nodes = self._owner(), head_channels(self.instance_peaks.keras_model, self.instance_peaks.HEAD)
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         ip = np.zeros((B, K, n_nodes, 2), np.float32); iv = np.zeros((B, K, n_nodes), np.float32)
@@ -745,7 +745,7 @@ class BottomUpInferenceLayer(InferenceLayer):
             m.handle.call("sb_bottomup_attach_tracker", m.model_id, -1, -1, 1.0, 1.0)
 
     def track_fields(self, slot, B):
-        """The track records of the batch just collected (slot 0 / 1, -1: sb_infer_bottomup) as batch-dict fields."""
+        """The track records of the batch just collected (slot 0 / 1; 0 after sb_infer_bottomup) as batch-dict fields."""
         return _step_tracks(self.keras_model, "sb_bottomup_tracks", self.tracker, slot, B)
 
     def params(self) -> BottomUpParams:
@@ -775,10 +775,10 @@ class BottomUpInferenceLayer(InferenceLayer):
             out.update(self.fetch_graph(B))
         return out
 
-    def _run_step(self, B, fn, *args, slot=-1):
+    def _run_step(self, B, fn, *args, slot=0):
         """One call ``fn(model id, *args, B, <outputs>)`` (sb_infer_bottomup or sb_bottomup_collect) into B frames'
         instances, as a batch dict; the track records and, with the multi-GPU exchange, every rank's records of this step
-        (they came over with the result copy) from ``slot`` (-1: sb_infer_bottomup)."""
+        (they came over with the result copy) from ``slot`` (0 after sb_infer_bottomup)."""
         m = self.keras_model
         I, N = self.max_instances, self.paf_scorer.n_nodes
         ip = np.zeros((B, I, N, 2), np.float32); iv = np.zeros((B, I, N), np.float32)

@@ -119,9 +119,9 @@ class PeerGather:
 
     ``model``: a configured bottom-up ``DeviceModel`` (``sb_bottomup_configure`` done).  After construction every
     ``sb_infer_bottomup*`` / ``sb_bottomup_submit`` call of that model is one exchange *step*.  The host-facing calls
-    (``sb_infer_bottomup``, ``sb_bottomup_submit`` / ``collect``) consume their own step: the whole gather window rides on
-    the result copy they do anyway (``gathered``); the device-resident call (``sb_infer_bottomup_dev``) leaves consumption
-    to ``consume_next_dev``.  A producer blocks only when it is ``generations`` steps ahead of the slowest consumer."""
+    (``sb_bottomup_submit`` / ``collect``, and ``sb_infer_bottomup``, which is a submit into slot 0 and its collect)
+    consume their own step: the whole gather window rides on the result copy they do anyway (``gathered``); the
+    device-resident call (``sb_infer_bottomup_dev``) leaves consumption to ``consume_next_dev``.  A producer blocks only when it is ``generations`` steps ahead of the slowest consumer."""
 
     def __init__(self, model, generations: int = 8, group=None):
         import ctypes
@@ -182,7 +182,7 @@ class PeerGather:
         return p.value, n.value
 
     def gathered(self, slot: int, B: int, max_instances: int, n_nodes: int):
-        """Every rank's records of the batch last collected from ``slot`` (0 / 1: sb_bottomup_collect, -1: the synchronous
+        """Every rank's records of the batch last collected from ``slot`` (0 / 1; 0 after the synchronous
         sb_infer_bottomup): (world*B, width) in rank-major (= frame) order + frames pushed per rank.  Host memory only: the
         window came over with the batch's own result copy."""
         from sleap_b200._lib import ptr

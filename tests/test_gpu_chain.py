@@ -151,7 +151,7 @@ def test_configure_detaches_the_tracker(frames):
         assert out["track_n"].shape == (B,)
         drop()
         with pytest.raises(SleapB200Error, match="no tracker attached"):
-            layer.track_fields(-1, B)
+            layer.track_fields(0, B)
         m.chain = None
     layer.tracker = None
 

@@ -6,7 +6,11 @@ Each refusal is SB_ERR_INVALID with its message and queues nothing: a bad slot o
 batch, a collect of an empty slot, with another B or out of submit order, a second collect of a slot, and (bottom-up and
 top-down with a device tracker) a tracks read of a slot before its collect or with another B.  After the refusals the
 in-order collects still equal predict_on_batch bit for bit, and a configure call between a submit and its collect makes
-the collect fail cleanly while the next stream runs."""
+the collect fail cleanly while the next stream runs.
+
+The synchronous call of a form (predict_on_batch: sb_infer_global, sb_infer_bottomup, sb_infer_multiclass,
+sb_infer_topdown, sb_infer_topdown_multiclass) is a submit into slot 0 and its collect: it is refused while a batch is
+submitted and not collected, and its track records are then slot 0's (slot -1 is refused)."""
 import numpy as np
 import pytest
 
@@ -208,3 +212,27 @@ def test_reconfigure_between_submit_and_collect(form):
         got.append(collect(k % 2, B))
     for k, (g, w) in enumerate(zip(got, form.want)):
         _same(g, w, f"batch {k}")
+
+
+def test_sync_call_is_a_slot_0_step(form):
+    if form.gt:
+        pytest.skip("the ground-truth forms have no synchronous call")
+    m, fn, collect, args = form.stream()
+    keep = args(form.batches[0])
+    m.handle.call(fn, m.model_id, *[_lib.ptr(a) for a in keep], B, 0)
+    with pytest.raises(_lib.SleapB200Error, match="a batch was submitted and not collected; collect it first"):
+        form.im.predict_on_batch(form.batches[1])
+    _same(collect(0, B), form.want[0], "batch 0")
+    if not form.tracks:
+        return
+    form.layer.tracker = T.Tracker.make_tracker_by_name(track_device=0, **SIMPLE)
+    try:
+        out = form.im.predict_on_batch(form.batches[1])
+        _same(out, form.want[1], "batch 1 with a tracker")
+        rec = np.full((B, 2 + 3 * form.layer.tracker._device.max_instances), -1.0)
+        m.handle.call(form.tracks, m.model_id, 0, B, _lib.ptr(rec))
+        assert (rec[:, 0] >= 0).all() and np.array_equal(rec[:, 0].astype(np.int64), out["track_n"])
+        with pytest.raises(_lib.SleapB200Error, match="bad slot / batch"):
+            m.handle.call(form.tracks, m.model_id, -1, B, _lib.ptr(rec))
+    finally:
+        form.untrack()

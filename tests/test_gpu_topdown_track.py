@@ -179,7 +179,7 @@ def test_track_abi(pair):
     im.detach_tracker()
     im.tracker = None
     with pytest.raises(_lib.SleapB200Error):         # nothing attached
-        mc.handle.call("sb_topdown_tracks", mc.model_id, -1, 8, _lib.ptr(rec))
+        mc.handle.call("sb_topdown_tracks", mc.model_id, 0, 8, _lib.ptr(rec))
     other = T.DeviceTracker(0, dict(tr.device_params, n_nodes=len(NODES) - 1, max_instances=8, track_table=16), handle=mc.handle)
     with pytest.raises(_lib.SleapB200Error):         # other node count than the instance model's
         mc.handle.call("sb_topdown_attach_tracker", mc.model_id, other.id, 1024.0, 1024.0)
