@@ -272,7 +272,13 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* params, const
  * configure calls drops the model's previous chain, with its tracker and record exchange, and so does
  * sb_model_configure.  A call for another chain than the model's is refused.  A configure call refused for its
  * arguments leaves the previous chain in place.  The fused top-down pipeline must be configured again
- * (sb_topdown_configure) after either of its models is reconfigured. */
+ * (sb_topdown_configure) after either of its models is reconfigured.
+ * Caps: n_classes <= SB_MAX_CLASSES (SB_ERR_INVALID).  The grouping kernels keep a node's peaks, their class
+ * probabilities and the assignment's scratch in shared memory, about 4 * max_node_peaks * n_classes bytes plus 42 bytes
+ * per row or column of the assignment; sb_multiclass_configure and sb_multiclass_from_maps refuse (SB_ERR_UNSUPPORTED) a
+ * max_node_peaks that would need more than the device's opt-in shared memory per block (227 KB on an H100: up to 408
+ * peaks per node with 128 classes).  sb_bottomup_configure and sb_bottomup_from_maps do the same for the PAF chain,
+ * whose matching keeps a max_node_peaks^2 score matrix (up to 235 peaks per node on an H100). */
 #define SB_MAX_CLASSES 128
 typedef struct sb_multiclass_params {
   int32_t cms_buffer, class_maps_buffer, offsets_buffer; /* op-list buffer ids (offsets: -1 if none) */
@@ -448,8 +454,8 @@ int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* fr
  * (n_in, n_classes) + bias; n_in of the first layer is C with global_pool, else tap H * W * C (Flatten in H, W, C
  * order).  The weights are copied at configure time and owned by the pipeline.
  * Caps, checked at configure time (SB_ERR_UNSUPPORTED): n_classes <= SB_MAX_CLASSES; num_fc_units and, with global_pool,
- * the tap's C <= SB_MAX_DENSE_WIDTH (the vectors kept in shared memory).  A Flatten input is read from global memory and
- * has no cap.
+ * the tap's C <= SB_MAX_DENSE_WIDTH (the vectors kept in shared memory; 33 KB at both caps, under the 48 KB every
+ * device gives without opt-in).  A Flatten input is read from global memory and has no cap.
  * Outputs, class-indexed and NaN where no crop was assigned: out_points (B,n_classes,n_nodes,2), out_vals
  * (B,n_classes,n_nodes), out_class_probs (B,n_classes); then as sb_infer_topdown: out_centroids (B,K,2),
  * out_centroid_vals (B,K), out_n_valid (B) crops per frame, out_flags (B).  out_class_vectors (B,K,n_classes): every

@@ -172,6 +172,14 @@ int sbk_group(sb_handle_s* h, int B, int n_nodes, int min_instance_peaks, float 
 // one record per frame into ws.records (sb_class_record_width); ws must have node_lists and records
 int sbk_class_group(sb_handle_s* h, const float* class_maps, int B, int Hc, int Wc, int n_classes, float class_stride,
                     float input_scale, SbPostWs& ws);
+// Dynamic shared memory of k_score_match, k_group and k_class_group: the launchers size their launches by these, and
+// the chains' configure calls refuse (SB_ERR_UNSUPPORTED) a max_node_peaks / n_classes whose kernels would not fit in
+// the device's opt-in shared memory per block, so a configured chain never fails a step at launch.
+size_t sb_score_match_smem(int K);
+size_t sb_group_smem(int n_nodes, int n_edges, int K);
+size_t sb_class_group_smem(int K, int n_classes);
+int sb_check_paf_smem(sb_handle_s* h, int n_nodes, int n_edges, int K);
+int sb_check_class_smem(sb_handle_s* h, int K, int n_classes);
 int sbk_lsap_batch(sb_handle_s* h, const float* scores, const int* n_src, const int* n_dst,
                    const int* offsets, int n_problems, int max_k, int* out_rows, int* out_cols,
                    float* out_scores, int* out_counts);

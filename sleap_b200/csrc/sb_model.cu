@@ -580,24 +580,26 @@ static bool f32_head(const SbModel* m, int buf, int C) {
   return buf >= 0 && buf < (int)m->buffers.size() && m->buffers[buf].f32 && m->buffers[buf].C == C;
 }
 
-// The PAF chain's parameters, checked by sb_bottomup_configure and sb_bottomup_from_maps alike (not the buffer ids)
+// The PAF chain's parameters, checked by sb_bottomup_configure and sb_bottomup_from_maps alike (not the buffer ids),
+// with the shared memory max_node_peaks gives its kernels (on the handle's device, which must be current)
 static int check_paf_params(sb_handle_s* h, const sb_bottomup_params* p) {
   if (p->n_nodes <= 0 || p->n_edges <= 0 || !p->edges) return sb_fail(h, SB_ERR_INVALID, "bad skeleton");
   if (p->n_sorted > p->n_edges || p->max_peaks_per_sample <= 0 || p->max_node_peaks <= 0 || p->max_instances <= 0)
     return sb_fail(h, SB_ERR_INVALID, "bad capacities");
   for (int e = 0; e < 2 * p->n_edges; ++e)
     if (p->edges[e] < 0 || p->edges[e] >= p->n_nodes) return sb_fail(h, SB_ERR_INVALID, "edge node index out of range");
-  return 0;
+  return sb_check_paf_smem(h, p->n_nodes, p->n_edges, p->max_node_peaks);
 }
 
-// The multi-class chain's parameters, checked by sb_multiclass_configure and sb_multiclass_from_maps alike
+// The multi-class chain's parameters, checked by sb_multiclass_configure and sb_multiclass_from_maps alike, with the
+// shared memory max_node_peaks and n_classes give k_class_group (on the handle's device, which must be current)
 static int check_class_params(sb_handle_s* h, const sb_multiclass_params* p) {
   if (p->n_classes < 1 || p->n_classes > SB_MAX_CLASSES)
     return sb_fail(h, SB_ERR_INVALID, "%d classes (1 to %d)", p->n_classes, SB_MAX_CLASSES);
   if (p->cm_output_stride <= 0 || p->class_maps_output_stride <= 0 || !(p->input_scale > 0.f) || p->max_peaks_per_sample <= 0 ||
       p->max_node_peaks <= 0)
     return sb_fail(h, SB_ERR_INVALID, "bad strides / input scale / capacities");
-  return 0;
+  return sb_check_class_smem(h, p->max_node_peaks, p->n_classes);
 }
 
 // ---- host copies of the results (sb_common.cuh) ----
@@ -1120,9 +1122,9 @@ int sb_bottomup_from_maps(sb_handle_t h, const sb_bottomup_params* p, const floa
   if (!cms_host || !pafs_host || !out_instance_peaks || !out_instance_peak_vals || !out_instance_scores || !out_n_valid)
     return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_from_maps: null argument");
   if (B <= 0 || H <= 0 || W <= 0 || Hp <= 0 || Wp <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_bottomup_from_maps: bad shape");
+  SB_CUDA(h, cudaSetDevice(h->device));
   int rc = check_paf_params(h, p);
   if (rc) return rc;
-  SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, C2 = 2 * p->n_edges;
   SbScratch s(h);
   if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, p->max_instances, p->n_edges))) return rc;
@@ -1154,9 +1156,9 @@ int sb_multiclass_from_maps(sb_handle_t h, const sb_multiclass_params* p, const 
   if (!cms_host || !class_logits_host || !out_points || !out_vals || !out_class_probs)
     return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: null argument");
   if (B <= 0 || H <= 0 || W <= 0 || Hc <= 0 || Wc <= 0 || p->n_nodes <= 0) return sb_fail(h, SB_ERR_INVALID, "sb_multiclass_from_maps: bad shape");
+  SB_CUDA(h, cudaSetDevice(h->device));
   int rc = check_class_params(h, p);
   if (rc) return rc;
-  SB_CUDA(h, cudaSetDevice(h->device));
   const int C = p->n_nodes, NC = p->n_classes;
   SbScratch s(h);
   if ((rc = sb_post_ws_alloc(h, s.ws, B, H, W, C, p->max_peaks_per_sample, p->max_node_peaks, 1, 0))) return rc;

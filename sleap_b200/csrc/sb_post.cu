@@ -17,6 +17,7 @@
 #include "sb_common.cuh"
 
 #include <algorithm>
+#include <cstdio>
 #include <math_constants.h>
 #include "sb_lsap.cuh"
 
@@ -1193,10 +1194,50 @@ int sbk_global_peaks(sb_handle_s* h, const float* cms, const float* offsets, int
   return 0;
 }
 
+size_t sb_score_match_smem(int K) { return (((size_t)K * K * sizeof(float) + 15) & ~(size_t)15) + lsap_scratch_bytes(K); }
+
+size_t sb_group_smem(int n_nodes, int n_edges, int K) {
+  return ((size_t)3 * n_nodes * K + n_nodes + n_edges + 3 * (size_t)n_edges * K + 3 * (size_t)n_edges) * sizeof(int);
+}
+
+size_t sb_class_group_smem(int K, int n_classes) {
+  const int L = std::max(K, n_classes), M = std::min(K, n_classes);
+  return ((lsap_scratch_bytes(L) + 15) & ~(size_t)15) + ((size_t)K * n_classes + 2 * (size_t)K) * sizeof(float) +
+         ((size_t)K + 2 * (size_t)M) * sizeof(int);
+}
+
+// SB_ERR_UNSUPPORTED unless `kernel` can be launched with `bytes` of dynamic shared memory on the handle's device: the
+// opt-in limit per block less the kernel's static shared memory
+template <typename Kern>
+static int smem_fits(sb_handle_s* h, Kern* kernel, const char* what, const char* cap, size_t bytes) {
+  int optin = 0;
+  SB_CUDA(h, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+  cudaFuncAttributes a;
+  SB_CUDA(h, cudaFuncGetAttributes(&a, kernel));
+  const size_t limit = (size_t)optin > a.sharedSizeBytes ? (size_t)optin - a.sharedSizeBytes : 0;
+  if (bytes > limit)
+    return sb_fail(h, SB_ERR_UNSUPPORTED, "%s: %s needs %zu B of shared memory per block, above the device's limit of %zu B",
+                   cap, what, bytes, limit);
+  return 0;
+}
+
+int sb_check_paf_smem(sb_handle_s* h, int n_nodes, int n_edges, int K) {
+  char cap[64];
+  snprintf(cap, sizeof(cap), "max_node_peaks %d", K);
+  if (int rc = smem_fits(h, k_score_match, "PAF scoring and matching", cap, sb_score_match_smem(K))) return rc;
+  return smem_fits(h, k_group, "grouping", cap, sb_group_smem(n_nodes, n_edges, K));
+}
+
+int sb_check_class_smem(sb_handle_s* h, int K, int n_classes) {
+  char cap[64];
+  snprintf(cap, sizeof(cap), "max_node_peaks %d with %d classes", K, n_classes);
+  return smem_fits(h, k_class_group, "class grouping", cap, sb_class_group_smem(K, n_classes));
+}
+
 int sbk_score_match(sb_handle_s* h, const float* pafs, int B, int Hp, int Wp, int C2, int n_points,
                     int pafs_stride, float max_edge_length, float dist_penalty_weight, SbPostWs& ws) {
   const int K = ws.max_node_peaks, E = ws.n_edges;
-  const size_t sm = (((size_t)K * K * sizeof(float) + 15) & ~(size_t)15) + lsap_scratch_bytes(K);
+  const size_t sm = sb_score_match_smem(K);
   if (sm > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_score_match, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "score_match smem %zu: %s", sm, cudaGetErrorString(e));
@@ -1216,7 +1257,7 @@ int sbk_group(sb_handle_s* h, int B, int n_nodes, int min_instance_peaks, float 
   if (gather) gx = *gather; else memset(&gx, 0, sizeof(gx));
   const int K = ws.max_node_peaks;
   const int E = ws.n_edges;
-  const size_t sm = ((size_t)3 * n_nodes * K + n_nodes + E + 3 * (size_t)E * K + 3 * E) * sizeof(int);
+  const size_t sm = sb_group_smem(n_nodes, E, K);
   if (sm > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "group smem %zu: %s", sm, cudaGetErrorString(e));
@@ -1233,9 +1274,8 @@ int sbk_group(sb_handle_s* h, int B, int n_nodes, int min_instance_peaks, float 
 int sbk_class_group(sb_handle_s* h, const float* class_maps, int B, int Hc, int Wc, int n_classes, float class_stride,
                     float input_scale, SbPostWs& ws) {
   if (!ws.node_lists || !ws.records || B > ws.B) return sb_fail(h, SB_ERR_INVALID, "class grouping: workspace not sized for it");
-  const int K = ws.max_node_peaks, L = std::max(K, n_classes), M = std::min(K, n_classes);
-  const size_t sm = ((lsap_scratch_bytes(L) + 15) & ~(size_t)15) + ((size_t)K * n_classes + 2 * (size_t)K) * sizeof(float) +
-                    ((size_t)K + 2 * (size_t)M) * sizeof(int);
+  const int K = ws.max_node_peaks;
+  const size_t sm = sb_class_group_smem(K, n_classes);
   if (sm > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(k_class_group, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm);
     if (e != cudaSuccess) return sb_fail(h, SB_ERR_CUDA, "class group smem %zu: %s", sm, cudaGetErrorString(e));
