@@ -502,7 +502,9 @@ int sb_topdown_multiclass_from_features(sb_handle_t h, const sb_topdown_multicla
  * frames on the device, keyed by frame index t, so that every frame's pyramid is built once however many later
  * frames shift points out of it.  Gray conversion, resize, pyramid and derivatives are bit-exact with OpenCV; the
  * LK iteration agrees with it to the size of its stopping step.
- *   window: 3..41; max_levels >= 0; img_scale: 1 or 0.5 (others return SB_ERR_UNSUPPORTED); ring: 2..64.
+ *   window: 3..41; max_levels >= 0; img_scale: 1 or 0.5 (others return SB_ERR_UNSUPPORTED); ring >= 2, with no
+ * upper cap: the ring's pyramids are one device allocation, sized at the first frame, and a ring the device cannot
+ * hold fails there with SB_ERR_CUDA.
  * frame_host: uint8 (H, W, C), C = 1 or 3 (3 = BGR order, as the reference calls cvtColor).  A frame of another
  * size than the ring holds empties the ring.  replace = 0 keeps a frame already held under t and skips the upload.
  * When every slot is taken, the slot used least recently (added or read by a shift) is replaced.

@@ -11,7 +11,8 @@
 //   Scharr   dx = [3 10 3]^T x [-1 0 1], dy = [-1 0 1]^T x [3 10 3], reflect-101, int16
 //   levels   after level l, stop when ((w+1)/2 <= win || (h+1)/2 <= win)
 // Every level is stored with a border of `win` pixels (image: reflect-101, derivatives: 0), as OpenCV pads its
-// pyramid, so the window reads of the LK kernel need no bounds checks.
+// pyramid, so the window reads of the LK kernel need no bounds checks.  The ring's pyramids are one allocation for the
+// images and one for the derivatives, slot s at s times a fixed slot stride, so the ring has no size cap of its own.
 //
 // The LK iteration follows OpenCV's tracker: 14-bit fixed-point bilinear weights, image samples kept with 5
 // fractional bits and derivative samples with none, sums scaled by 2^-20, the min-eigenvalue / determinant test,
@@ -29,9 +30,13 @@
 namespace {
 
 constexpr int kFlowMaxLevels = 16;
-constexpr int kFlowMaxRing = 64;
 constexpr int kFlowMaxWin = 41;
 constexpr int kFlowWarps = 4;                  // points per LK block
+// k_flow_lk sums each lane's share of the window in 32-bit ints.  The largest term is b1's |J - I| * |Ix|: image
+// samples carry 5 fraction bits (|J - I| <= 255 * 32) and a Scharr derivative of uint8 pixels is at most 16 * 255.
+constexpr long long kFlowLanePixels = (kFlowMaxWin * kFlowMaxWin + 31) / 32;
+static_assert(kFlowLanePixels * (255 * 32) * (16 * 255) < (1ll << 31),
+              "k_flow_lk's per-lane int sums could overflow at kFlowMaxWin");
 
 struct FlowLevel {
   int w, h;                                     // interior size
@@ -40,10 +45,6 @@ struct FlowLevel {
 struct FlowGeom {
   int win, n_levels;
   FlowLevel lv[kFlowMaxLevels];
-};
-struct FlowSlots {                              // by-value kernel argument: every slot's pyramid
-  const uint8_t* img[kFlowMaxRing];
-  const short2* der[kFlowMaxRing];
 };
 struct FlowIn { float x, y; int slot, pad; };
 struct FlowOut { float x, y, err; int status; };
@@ -141,7 +142,9 @@ __device__ __forceinline__ void bilinear_weights(float a, float b, int& w00, int
 
 // One warp per point; lanes stride over the win x win window.  Every lane reduces to the same sums (integer
 // butterfly), so all control flow below is warp-uniform.
-__global__ void __launch_bounds__(kFlowWarps * 32) k_flow_lk(FlowGeom g, FlowSlots s, int cur_slot,
+__global__ void __launch_bounds__(kFlowWarps * 32) k_flow_lk(FlowGeom g, const uint8_t* __restrict__ img,
+                                                              const short2* __restrict__ der, long long img_stride,
+                                                              long long der_stride, int cur_slot,
                                                               const FlowIn* __restrict__ in, FlowOut* __restrict__ out,
                                                               int n) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -152,9 +155,9 @@ __global__ void __launch_bounds__(kFlowWarps * 32) k_flow_lk(FlowGeom g, FlowSlo
   short* Iw = (short*)smem_raw + (size_t)warp * area2;                                  // I patch, 5 fraction bits
   short2* dIw = (short2*)((short*)smem_raw + (size_t)kFlowWarps * area2) + (size_t)warp * area;   // (Ix, Iy) patch
   const FlowIn p = in[pt];
-  const uint8_t* Ibase = s.img[p.slot];
-  const short2* Dbase = s.der[p.slot];
-  const uint8_t* Jbase = s.img[cur_slot];
+  const uint8_t* Ibase = img + p.slot * img_stride;
+  const short2* Dbase = der + p.slot * der_stride;
+  const uint8_t* Jbase = img + cur_slot * img_stride;
   const float halfw = (win - 1) * 0.5f;
   const float FLT_SCALE = 1.f / (1 << 20);
   int status = 1;
@@ -253,9 +256,9 @@ struct SbFlow {
   int win = 0, max_levels = 0, half = 0, ring = 0;
   int H = 0, W = 0;                               // frame size the ring holds
   FlowGeom geom{};
-  long long img_elems = 0, der_elems = 0;         // per slot
-  std::vector<uint8_t*> img;
-  std::vector<short2*> der;
+  long long img_elems = 0, der_elems = 0;         // per slot: the slot stride of img and der
+  uint8_t* img = nullptr;                         // ring * img_elems
+  short2* der = nullptr;                          // ring * der_elems
   std::vector<long long> slot_t, stamp;           // frame index (-1: empty) and last use of every slot
   long long clock = 0;
   uint8_t* frame_dev = nullptr;
@@ -265,11 +268,13 @@ struct SbFlow {
   int cap = 0;
 
   void free_ring() {
-    for (auto* p : img) cudaFree(p);
-    for (auto* p : der) cudaFree(p);
-    img.clear(); der.clear(); slot_t.clear(); stamp.clear();
+    cudaFree(img); cudaFree(der);
+    img = nullptr; der = nullptr;
+    slot_t.clear(); stamp.clear();
     H = W = 0;
   }
+  uint8_t* slot_img(int slot) const { return img + slot * img_elems; }
+  short2* slot_der(int slot) const { return der + slot * der_elems; }
   ~SbFlow() {
     free_ring();
     cudaFree(frame_dev); cudaFree(in_dev); cudaFree(out_dev);
@@ -312,17 +317,11 @@ int flow_alloc_ring(sb_handle_s* h, SbFlow* f, int H, int W) {
     if (w <= g.win || hh <= g.win) break;
   }
   f->img_elems = io; f->der_elems = dof;
-  for (int i = 0; i < f->ring; ++i) {
-    uint8_t* a = nullptr;
-    short2* d = nullptr;
-    int rc;
-    if ((rc = sb_dev_alloc(h, &a, io))) return rc;
-    f->img.push_back(a);
-    if ((rc = sb_dev_alloc(h, &d, dof))) return rc;
-    f->der.push_back(d);
-    SB_CUDA(h, cudaMemsetAsync(d, 0, dof * sizeof(short2), h->stream));
-    f->slot_t.push_back(-1); f->stamp.push_back(-1);
-  }
+  const size_t n_img = (size_t)io * f->ring, n_der = (size_t)dof * f->ring;
+  int rc;
+  if ((rc = sb_dev_alloc(h, &f->img, n_img)) || (rc = sb_dev_alloc(h, &f->der, n_der))) return rc;
+  SB_CUDA(h, cudaMemsetAsync(f->der, 0, n_der * sizeof(short2), h->stream));
+  f->slot_t.assign(f->ring, -1); f->stamp.assign(f->ring, -1);
   f->H = H; f->W = W;
   return SB_OK;
 }
@@ -337,7 +336,7 @@ int sb_flow_create(sb_handle_t h, int window, int max_levels, float img_scale, i
   if (max_levels < 0) return sb_fail(h, SB_ERR_INVALID, "sb_flow_create: max_levels %d < 0", max_levels);
   if (img_scale != 1.f && img_scale != 0.5f)
     return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_flow_create: img_scale %g (the device flow resizes by 1 or 0.5)", img_scale);
-  if (ring < 2 || ring > kFlowMaxRing) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_flow_create: ring %d outside 2..%d", ring, kFlowMaxRing);
+  if (ring < 2) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_flow_create: ring %d < 2", ring);
   SbFlow* f = new SbFlow();
   f->win = window; f->max_levels = max_levels; f->half = img_scale == 0.5f; f->ring = ring;
   h->flows.push_back(f);
@@ -387,14 +386,15 @@ int sb_flow_add_frame(sb_handle_t h, int flow_id, int64_t t, const uint8_t* fram
   const FlowGeom& g = f->geom;
   const dim3 blk(32, 8);
   auto grid = [&](int w, int hh) { return dim3((w + 31) / 32, (hh + 7) / 8); };
-  k_flow_level0<<<grid(g.lv[0].w, g.lv[0].h), blk, 0, h->stream>>>(f->frame_dev, H, W, C, f->half, g, f->img[slot]);
+  k_flow_level0<<<grid(g.lv[0].w, g.lv[0].h), blk, 0, h->stream>>>(f->frame_dev, H, W, C, f->half, g, f->slot_img(slot));
   SB_CHECK_LAUNCH(h);
   for (int l = 0; l < g.n_levels; ++l) {
     if (l > 0) {
-      k_flow_pyrdown<<<grid(g.lv[l].w, g.lv[l].h), blk, 0, h->stream>>>(g, l, f->img[slot]);
+      k_flow_pyrdown<<<grid(g.lv[l].w, g.lv[l].h), blk, 0, h->stream>>>(g, l, f->slot_img(slot));
       SB_CHECK_LAUNCH(h);
     }
-    k_flow_finish<<<grid(g.lv[l].w + 2 * g.win, g.lv[l].h + 2 * g.win), blk, 0, h->stream>>>(g, l, f->img[slot], f->der[slot]);
+    k_flow_finish<<<grid(g.lv[l].w + 2 * g.win, g.lv[l].h + 2 * g.win), blk, 0, h->stream>>>(g, l, f->slot_img(slot),
+                                                                                          f->slot_der(slot));
     SB_CHECK_LAUNCH(h);
   }
   f->slot_t[slot] = t;
@@ -430,13 +430,11 @@ int sb_flow_shift(sb_handle_t h, int flow_id, int64_t t, int n, const int64_t* r
     f->stamp[s] = f->clock;
     f->in_host[i] = FlowIn{pts[2 * i], pts[2 * i + 1], s, 0};
   }
-  FlowSlots slots{};
-  for (int i = 0; i < f->ring; ++i) { slots.img[i] = f->img[i]; slots.der[i] = f->der[i]; }
   const int area2 = (f->win * f->win + 1) & ~1;
   const size_t smem = (size_t)kFlowWarps * (area2 * sizeof(short) + f->win * f->win * sizeof(short2));
   SB_CUDA(h, cudaMemcpyAsync(f->in_dev, f->in_host, n * sizeof(FlowIn), cudaMemcpyHostToDevice, h->stream));
-  k_flow_lk<<<(n + kFlowWarps - 1) / kFlowWarps, kFlowWarps * 32, smem, h->stream>>>(f->geom, slots, cur, f->in_dev,
-                                                                                    f->out_dev, n);
+  k_flow_lk<<<(n + kFlowWarps - 1) / kFlowWarps, kFlowWarps * 32, smem, h->stream>>>(
+      f->geom, f->img, f->der, f->img_elems, f->der_elems, cur, f->in_dev, f->out_dev, n);
   SB_CHECK_LAUNCH(h);
   SB_CUDA(h, cudaMemcpyAsync(f->out_host, f->out_dev, n * sizeof(FlowOut), cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -463,9 +461,9 @@ int sb_flow_fetch_level(sb_handle_t h, int flow_id, int64_t t, int level, uint8_
   const FlowLevel L = g.lv[level];
   const size_t pw = L.w + 2 * g.win, first = (size_t)g.win * pw + g.win;
   if (img_out)
-    SB_CUDA(h, cudaMemcpy2DAsync(img_out, L.w, f->img[slot] + L.img_off + first, pw, L.w, L.h, cudaMemcpyDeviceToHost, h->stream));
+    SB_CUDA(h, cudaMemcpy2DAsync(img_out, L.w, f->slot_img(slot) + L.img_off + first, pw, L.w, L.h, cudaMemcpyDeviceToHost, h->stream));
   if (deriv_out)
-    SB_CUDA(h, cudaMemcpy2DAsync(deriv_out, L.w * sizeof(short2), f->der[slot] + L.der_off + first, pw * sizeof(short2),
+    SB_CUDA(h, cudaMemcpy2DAsync(deriv_out, L.w * sizeof(short2), f->slot_der(slot) + L.der_off + first, pw * sizeof(short2),
                                  L.w * sizeof(short2), L.h, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaStreamSynchronize(h->stream));
   if (out_H) *out_H = L.h;

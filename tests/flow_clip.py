@@ -35,8 +35,8 @@ def clip_labeled_frames(n: int) -> list:
                                 for j in range(counts[t])]) for t in range(n)]
 
 
-def track_clip(tracker: str, save: bool, n: int, frames: np.ndarray, **kw) -> list:
-    tr = T.Tracker.make_tracker_by_name(tracker=tracker, similarity="instance", match="greedy", track_window=5, max_tracks=2,
+def track_clip(tracker: str, save: bool, n: int, frames: np.ndarray, track_window: int = 5, **kw) -> list:
+    tr = T.Tracker.make_tracker_by_name(tracker=tracker, similarity="instance", match="greedy", track_window=track_window, max_tracks=2,
                                         max_tracking=tracker == "flowmaxtracks", save_shifted_instances=save, **kw)
     return T.run_tracker(clip_labeled_frames(n), tr, images=lambda t: frames[t])
 

@@ -1,5 +1,6 @@
 """Shared by the device-tracker tests: the host tracker with its greedy ties made stable, seeded synthetic frames and
 the comparison of a host and a device tracking run."""
+import contextlib
 import math
 
 import numpy as np
@@ -62,6 +63,47 @@ def synthetic_frames(seed: int, n_frames: int = 300, max_instances: int = 32, n_
             insts.append(PredictedInstance.from_numpy(p, conf, float(rng.uniform(0.1, 5.0))))
         frames.append(LabeledFrame(0, t, insts))
     return frames
+
+
+def counted_frames(seed: int, shown: list, n_nodes: int = 13, hw=(1024, 1024), score_levels: int = 0) -> list:
+    """One frame per entry of ``shown``: an int k shows animals 0..k-1, a list shows those animal ids; each frame's
+    order is shuffled.  Animals persist: each keeps its skeleton and walks 1.5 px per frame, so one that leaves and
+    comes back can be matched again.  About 15 % of the nodes are NaN, never all of an instance's (no all-NaN
+    similarity rows, which SciPy's Hungarian matcher rejects).  Scores are distinct, or with ``score_levels`` > 0
+    drawn from that many values, so that most scores are tied."""
+    rng = np.random.default_rng(seed)
+    ids = [np.arange(s) if np.isscalar(s) else np.asarray(s) for s in shown]
+    n_animals = 1 + max(int(i.max()) for i in ids if len(i))
+    side = int(np.ceil(np.sqrt(n_animals)))                  # a jittered grid: neighbours 60+ px apart at 1024^2
+    cell = np.array([hw[1], hw[0]], np.float64) / side
+    pos = (np.stack([np.arange(n_animals) % side, np.arange(n_animals) // side], -1) + 0.5) * cell
+    pos += rng.uniform(-0.15, 0.15, pos.shape) * cell
+    shape = rng.normal(0, 0.12 * cell.min(), (n_animals, n_nodes, 2))
+    frames = []
+    for t, a_ids in enumerate(ids):
+        pos += rng.normal(0, 1.5, pos.shape)
+        insts = []
+        for a in rng.permutation(a_ids):
+            p = pos[a] + shape[a] + rng.normal(0, 0.7, (n_nodes, 2))
+            lost = rng.random(n_nodes) < 0.15
+            lost[rng.integers(n_nodes)] = False
+            p[lost] = np.nan
+            score = rng.integers(score_levels) / score_levels if score_levels else rng.uniform(0.1, 5.0)
+            insts.append(PredictedInstance.from_numpy(p, rng.uniform(0.2, 1.0, n_nodes), float(score)))
+        frames.append(LabeledFrame(0, t, insts))
+    return frames
+
+
+@contextlib.contextmanager
+def stable_argsort():
+    """Every np.argsort stable while the block runs: the host's nms_fast then orders equal scores as the device's
+    pre-cull does (the default sort leaves that order to the implementation)."""
+    argsort = np.argsort
+    np.argsort = lambda a, axis=-1, kind=None, order=None: argsort(a, axis=axis, kind="stable", order=order)
+    try:
+        yield
+    finally:
+        np.argsort = argsort
 
 
 def _close(a: float, b: float) -> bool:
