@@ -437,6 +437,38 @@ int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_
 int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* frames_host, const float* centroids_host,
                          const int32_t* counts_host, int B, int slot);
 
+/* ---- ground-truth instances ------------------------------------------------------------------------
+ * sleap/nn/inference.py:1747-1966 CentroidCrop.call -> :812-893 FindInstancePeaksGroundTruth.call: the centroid stage of
+ * sb_topdown_submit, then every kept centroid gets the labelled instance whose nearest visible node is closest to it, as
+ * ONE device step with no instance model.  sb_topdown_gt_instances_configure: params.instance_model must be -1 and
+ * params.centroid_model a configured model; `centroid`, `max_instances`, max_centroids_per_frame (K) and precrop_resize
+ * as in sb_topdown_configure; `instance`, crop_size and max_crops_per_call are ignored.  The table holds up to
+ * max_instances_per_frame (N) instances of n_nodes nodes per frame.  The pipeline belongs to the centroid model and is
+ * addressed by its id; a configure call on that model drops the pipeline and its submitted batches.  It owns two slots of
+ * max_batch uint8 frames of H x W x C_in and two instance tables, allocated at its first submit.
+ * sb_topdown_gt_instances_submit queues one whole step into slot 0 / 1 without waiting on the host: the frames, the
+ * instance table (B,N,n_nodes,2) (frame coordinates, float32, NaN allowed, rows past a frame's count ignored) and the
+ * counts (B), each in [0, N], are copied on a copy stream; the centroid network, local peaks, (/ input_scale + 0.5) and
+ * the per-frame top-k run as in sb_topdown_submit; then per centroid d[j] = min over the non-NaN nodes of sqrtf((x - cx)^2
+ * + (y - cy)^2) in float32, each operation rounded on its own (NaN: an instance without a visible node).  A centroid
+ * whose d is all NaN is dropped; otherwise it takes instance 0 unless a later one is strictly nearer (ties: the lower
+ * index; an all-NaN instance 0 is kept).  The kept rows, in centroid order, carry the instance's points unchanged
+ * (NaN included) with values 1.  Refused (SB_ERR_INVALID, nothing queued, the slot stays free): a count outside [0, N],
+ * and as every streamed submit.
+ * sb_topdown_gt_instances_collect, under the rules of the streamed steps: out_centroids (B,K,2), out_centroid_vals (B,K),
+ * out_n_centroids (B), out_instance_peaks (B,K,n_nodes,2), out_instance_peak_vals (B,K,n_nodes), out_n_rows (B) (row i
+ * is not centroid i: unmatched centroids have no row), out_flags (B) as sb_infer_topdown's; NaN padded.
+ * On this pipeline sb_infer_topdown*, sb_topdown_submit / _collect, sb_topdown_gt_submit, sb_topdown_multiclass_*,
+ * sb_topdown_attach_tracker and sb_topdown_tracks are refused (SB_ERR_INVALID); the other pipeline forms refuse these
+ * two calls. */
+int sb_topdown_gt_instances_configure(sb_handle_t h, const sb_topdown_params* params, int n_nodes, int max_instances_per_frame,
+                                      int max_batch, int H, int W, int C_in);
+int sb_topdown_gt_instances_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, const float* instances_host,
+                                   const int32_t* counts_host, int B, int slot);
+int sb_topdown_gt_instances_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids,
+                                    float* out_centroid_vals, int32_t* out_n_centroids, float* out_instance_peaks,
+                                    float* out_instance_peak_vals, int32_t* out_n_rows, int32_t* out_flags);
+
 /* ---- top-down multi-class (identity) step ---------------------------------------------------------
  * sleap/nn/inference.py:4139-4210 TopDownMultiClassInferenceModel.call = CentroidCrop.call -> TopDownMultiClassFindPeaks.call
  * (:3863-4136), as ONE device pipeline: the sb_infer_topdown pipeline up to the instance network, then after every chunk

@@ -163,6 +163,10 @@ _SIGS = {
     "sb_topdown_submit": [c_void_p, c_int, c_void_p, c_int, c_int],
     "sb_topdown_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sb_topdown_gt_submit": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int],
+    "sb_topdown_gt_instances_configure": [c_void_p, POINTER(TopdownParams), c_int, c_int, c_int, c_int, c_int, c_int],
+    "sb_topdown_gt_instances_submit": [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int],
+    "sb_topdown_gt_instances_collect": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p],
     "sb_topdown_multiclass_configure": [c_void_p, POINTER(TopdownMultiClassParams), c_int, c_int, c_int, c_int],
     "sb_infer_topdown_multiclass": [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p],

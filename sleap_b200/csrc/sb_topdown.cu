@@ -138,6 +138,78 @@ __global__ void __launch_bounds__(128) k_td_pack(const float* __restrict__ sel_c
   }
 }
 
+// Ground-truth instances (FindInstancePeaksGroundTruth.call, :812-893), one CTA per frame: every selected centroid gets
+// the labelled instance whose nearest visible node is closest to it.  d[c, j] = min over the non-NaN nodes k of
+// sqrtf((x - cx)^2 + (y - cy)^2), each operation rounded on its own as numpy rounds it (NaN: no visible node).  A
+// centroid whose d[c, :] is all NaN (no instance, or none with a visible node) is dropped; otherwise the pick starts at
+// instance 0 and moves on a strict "<" only, so ties go to the lower index and an all-NaN instance 0 is kept.  One warp
+// per centroid, lanes over the instances; `match` ([K] per frame) holds each centroid's pick (-1: dropped), then the
+// picks of the kept rows in centroid order.
+// Record per frame: [K][2] centroids | [K] centroid values | [K][nodes][2] points | [K][nodes] values (1) | centroid count |
+// row count | flags.
+__global__ void __launch_bounds__(128) k_td_gt_match(const float* __restrict__ sel_cent, const float* __restrict__ sel_val,
+                                                     const int* __restrict__ sel_count, const float* __restrict__ inst,
+                                                     const int* __restrict__ inst_count, int N, int nodes, int K,
+                                                     const int* __restrict__ flags, int* __restrict__ match, float* __restrict__ record,
+                                                     int width) {
+  __shared__ int s_rows;
+  const int b = blockIdx.x;
+  const int cnt = sel_count[b], ni = inst_count[b];
+  const float* cent = sel_cent + (size_t)b * K * 2;
+  const float* ins = inst + (size_t)b * N * nodes * 2;
+  int* mt = match + (size_t)b * K;
+  float* r = record + (size_t)b * width;
+  float* rp = r + K * 3;
+  float* rq = rp + (size_t)K * nodes * 2;
+  td_write_centroids(sel_cent, sel_val, b, cnt, K, r);
+  const int lane = threadIdx.x & 31;
+  for (int c = threadIdx.x >> 5; c < cnt; c += blockDim.x >> 5) {
+    const float cx = cent[2 * c], cy = cent[2 * c + 1];
+    float bv = 0.f, d0 = CUDART_NAN_F;
+    int bj = -1;                                         // the lane's first smallest non-NaN distance (-1: none)
+    for (int j = lane; j < ni; j += 32) {
+      const float* p = ins + (size_t)j * nodes * 2;
+      // np.nanmin over the nodes of the rounded roots: a correctly rounded sqrtf is monotone, so the root of the smallest
+      // square is the smallest root, bit for bit (the picks below still compare roots)
+      float q = CUDART_NAN_F;
+      for (int k = 0; k < nodes; ++k) {
+        const float dx = __fsub_rn(p[2 * k], cx), dy = __fsub_rn(p[2 * k + 1], cy);
+        const float s = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
+        if (s < q || q != q) q = s;
+      }
+      const float m = __fsqrt_rn(q);
+      if (j == 0) d0 = m;
+      if (m == m && (bj < 0 || m < bv)) { bv = m; bj = j; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_down_sync(0xffffffffu, bv, o);
+      const int oj = __shfl_down_sync(0xffffffffu, bj, o);
+      if (oj >= 0 && (bj < 0 || ov < bv || (ov == bv && oj < bj))) { bv = ov; bj = oj; }
+    }
+    // lane 0 ran instance 0: a NaN there is never left by a "<", whatever the others hold
+    if (lane == 0) mt[c] = bj < 0 ? -1 : (d0 != d0 ? 0 : bj);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int rows = 0;
+    for (int c = 0; c < cnt; ++c)
+      if (mt[c] >= 0) mt[rows++] = mt[c];
+    s_rows = rows;
+  }
+  __syncthreads();
+  const int rows = s_rows;
+  for (int t = threadIdx.x; t < K * nodes * 2; t += blockDim.x) {
+    const int k = t / (nodes * 2);
+    rp[t] = (k < rows) ? ins[(size_t)mt[k] * nodes * 2 + (t - k * nodes * 2)] : CUDART_NAN_F;
+  }
+  for (int t = threadIdx.x; t < K * nodes; t += blockDim.x) rq[t] = (t / nodes < rows) ? 1.f : CUDART_NAN_F;
+  if (threadIdx.x == 0) {
+    rq[(size_t)K * nodes] = (float)cnt;
+    rq[(size_t)K * nodes + 1] = (float)rows;
+    rq[(size_t)K * nodes + 2] = (float)flags[b];
+  }
+}
+
 // The class-vector head's shape: the tap (H x W x C logical channels), pooling, the dense stack and its packed weights
 struct TdHead {
   int H, W, C;          // tap
@@ -374,6 +446,14 @@ struct SbTopdown {
   int* gt_flags = nullptr;                     // [Bmax]
   float* gt_cent[2] = {nullptr, nullptr};      // [Bmax][K][2]
   int* gt_count[2] = {nullptr, nullptr};       // [Bmax]
+  // ground-truth instances form (sb_topdown_gt_instances_configure: no instance model), held by its centroid model.
+  // gi_inst / gi_count: per slot the device copy of the batch's instance table and counts, which k_td_gt_match reads;
+  // gi_match: its per-centroid picks.
+  bool gti = false;
+  int N = 0;                                   // instances per frame of the table
+  float* gi_inst[2] = {nullptr, nullptr};      // [Bmax][N][nodes][2]
+  int* gi_count[2] = {nullptr, nullptr};       // [Bmax]
+  int* gi_match = nullptr;                     // [Bmax][K]
 };
 
 void sb_topdown_free(SbModel* m) {
@@ -381,7 +461,7 @@ void sb_topdown_free(SbModel* m) {
   if (!t) return;
   void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
                  t->offsets, t->total, t->crops, t->dense, t->probs, t->gt_flags, t->gt_cent[0], t->gt_cent[1], t->gt_count[0],
-                 t->gt_count[1]};
+                 t->gt_count[1], t->gi_inst[0], t->gi_inst[1], t->gi_count[0], t->gi_count[1], t->gi_match};
   for (void* p : dev) if (p) cudaFree(p);
   t->slots.release();
   for (void* p : {(void*)t->count_host, (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
@@ -463,8 +543,36 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   return SB_OK;
 }
 
-// The centroid sources a call takes: a centroid model, ground-truth centroids (sb_topdown_gt_submit)
-enum { TD_MODEL = 1, TD_GT = 2 };
+// Configures the centroid network and its chain, then the ground-truth instances pipeline on the centroid model mc:
+// frames -> centroid stage -> k_td_gt_match against a table of N instances of n_nodes nodes per frame.
+int gt_instances_setup(sb_handle_s* h, const sb_topdown_params* p, int n_nodes, int N, int max_batch, int H, int W, int C_in,
+                       SbModel* mc) {
+  SB_CUDA(h, cudaSetDevice(h->device));
+  int rc;
+  if ((rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in)) || (rc = sb_centroid_configure(h, p->centroid_model, &p->centroid)))
+    return rc;
+  SbTopdown* t = new SbTopdown();
+  mc->td = t;
+  t->p = *p; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
+  t->gen_c = mc->chain_gen;
+  t->H = H; t->W = W; t->C = C_in; t->gti = true; t->N = N;
+  precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by the caller
+  t->nodes = n_nodes;
+  t->width = t->K * (3 + n_nodes * 3) + 3;
+  t->flags = mc->ws.flags;
+  const size_t KB = (size_t)max_batch * t->K;
+  if ((rc = sb_dev_alloc(h, &t->sel_cent, KB * 2)) || (rc = sb_dev_alloc(h, &t->sel_val, KB)) ||
+      (rc = sb_dev_alloc(h, &t->sel_count, (size_t)max_batch)) || (rc = sb_dev_alloc(h, &t->gi_match, KB)) ||
+      (rc = sb_dev_alloc(h, &t->record, (size_t)max_batch * t->width))) {
+    sb_topdown_free(mc);
+    return rc;
+  }
+  return SB_OK;
+}
+
+// The centroid sources a call takes: a centroid model, ground-truth centroids (sb_topdown_gt_submit), a centroid model
+// with ground-truth instances (sb_topdown_gt_instances_submit)
+enum { TD_MODEL = 1, TD_GT = 2, TD_GTI = 4 };
 
 // The pipeline of model `id` (its centroid model, or the instance model of a ground-truth pipeline) when it is of the
 // wanted form and no model of it was reconfigured since.  `streamed`: the refusal of the wrong form names the submit
@@ -475,14 +583,19 @@ SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = f
   if (!mc) return nullptr;
   SbTopdown* t = mc->td;
   if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
-  if (!(sources & (t->gt ? TD_GT : TD_MODEL))) {
-    if (t->gt)
+  if (!(sources & (t->gti ? TD_GTI : t->gt ? TD_GT : TD_MODEL))) {
+    if (t->gti)
+      sb_fail(h, SB_ERR_INVALID,
+              "top-down pipeline takes ground-truth instances: call sb_topdown_gt_instances_submit / sb_topdown_gt_instances_collect");
+    else if (t->gt)
       sb_fail(h, SB_ERR_INVALID, "top-down pipeline takes ground-truth centroids: call sb_topdown_gt_submit");
     else
       sb_fail(h, SB_ERR_INVALID, "top-down pipeline runs a centroid model: call %s",
               multiclass ? "sb_topdown_multiclass_submit" : "sb_topdown_submit");
     return nullptr;
   }
+  // the centroid model holds the pipeline, and a configure call on it dropped the pipeline with its chain
+  if (t->gti) return t;
   if (t->gt) {
     // the instance model holds the pipeline: a configure call on it dropped the pipeline with its chain
     if (t->multiclass != multiclass) {
@@ -519,11 +632,8 @@ int flatten(sb_handle_s* h, SbTopdown* t, int B) {
   return 0;
 }
 
-// The centroid stage of B frames resident at frames_dev: centroid network, local peaks, top-k, the flat crop list, then
-// the crop count's copy into *count_host and, given, count_ev.
-int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int* count_host,
-                   cudaEvent_t count_ev) {
-  cudaStream_t s = h->stream;
+// The centroids of B frames resident at frames_dev in the selection buffers: centroid network, local peaks, top-k
+int select_centroids(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B) {
   int rc = sb_run_ops(h, mc, frames_dev, frames_are_u8, B);
   if (rc) return rc;
   const sb_centroid_params& cp = mc->ce;
@@ -531,10 +641,19 @@ int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames
   const float* coff = cp.offsets_buffer >= 0 ? (const float*)mc->buffers[cp.offsets_buffer].dev : nullptr;
   SbPeakParams pc{cp.peak_threshold, cp.refinement, cp.integral_patch_size, (float)cp.output_stride, cp.input_scale};
   if ((rc = sbk_local_peaks(h, (const float*)cb.dev, coff, B, cb.H, cb.W, cb.C, pc, mc->ws))) return rc;
-  k_td_select<<<B, 128, 0, s>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->scale, t->sel_cent,
-                                t->sel_val, t->sel_count, mc->ws.flags);
+  k_td_select<<<B, 128, 0, h->stream>>>(mc->ws.peaks, mc->ws.peak_vals, mc->ws.n_peaks, mc->ws.max_peaks, t->p.max_instances, t->K, t->scale,
+                                        t->sel_cent, t->sel_val, t->sel_count, mc->ws.flags);
   SB_CHECK_LAUNCH(h);
-  if ((rc = flatten(h, t, B))) return rc;
+  return 0;
+}
+
+// The centroid stage of B frames resident at frames_dev: centroid network, local peaks, top-k, the flat crop list, then
+// the crop count's copy into *count_host and, given, count_ev.
+int centroid_stage(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frames_dev, int frames_are_u8, int B, int* count_host,
+                   cudaEvent_t count_ev) {
+  cudaStream_t s = h->stream;
+  int rc;
+  if ((rc = select_centroids(h, mc, t, frames_dev, frames_are_u8, B)) || (rc = flatten(h, t, B))) return rc;
   SB_CUDA(h, cudaMemcpyAsync(count_host, t->total, 4, cudaMemcpyDeviceToHost, s));
   if (count_ev) SB_CUDA(h, cudaEventRecord(count_ev, s));
   return 0;
@@ -627,6 +746,8 @@ int stream_alloc(sb_handle_s* h, SbTopdown* t) {
     if (!t->count_ev[i]) SB_CUDA(h, cudaEventCreateWithFlags(&t->count_ev[i], cudaEventDisableTiming));
     if (t->gt && !t->gt_cent[i] && (rc = sb_dev_alloc(h, &t->gt_cent[i], (size_t)t->Bmax * t->K * 2))) return rc;
     if (t->gt && !t->gt_count[i] && (rc = sb_dev_alloc(h, &t->gt_count[i], (size_t)t->Bmax))) return rc;
+    if (t->gti && !t->gi_inst[i] && (rc = sb_dev_alloc(h, &t->gi_inst[i], (size_t)t->Bmax * t->N * t->nodes * 2))) return rc;
+    if (t->gti && !t->gi_count[i] && (rc = sb_dev_alloc(h, &t->gi_count[i], (size_t)t->Bmax))) return rc;
   }
   SB_CUDA(h, cudaHostAlloc((void**)&t->count_host, 2 * sizeof(int), cudaHostAllocDefault));   // last: marks it complete
   return 0;
@@ -688,6 +809,37 @@ int topdown_gt_submit(sb_handle_s* h, SbTopdown* t, const uint8_t* frames_host, 
   if ((rc = flatten(h, t, B)) ||
       (rc = instance_stage(h, nullptr, t, sl.frames[slot], 1, B, total, sl.stage[slot], nullptr, t->probs_stage[slot], sl.frames_free[slot])))
     return rc;
+  SB_CUDA(h, cudaEventRecord(sl.result[slot], h->stream));
+  sl.submitted(slot, B);
+  return SB_OK;
+}
+
+// Streamed batch with ground-truth instances into `slot`, the whole step queued at once (nothing in it waits on the
+// host): the frames, then the instance table and counts, on the copy stream into the slot; the centroid stage behind
+// that copy on the handle's stream; k_td_gt_match; the records' copy.  The table has its own per-slot staging, free
+// again once the slot's frames are (frames_free, recorded after the match).
+int topdown_gt_instances_submit(sb_handle_s* h, SbModel* mc, SbTopdown* t, const uint8_t* frames_host, const float* instances_host,
+                                const int32_t* counts_host, int B, int slot) {
+  SbSlots& sl = t->slots;
+  int rc = sl.check_submit(h, "sb_topdown_gt_instances_submit", slot, B, t->Bmax, instances_host && counts_host ? frames_host : nullptr);
+  if (rc) return rc;
+  for (int b = 0; b < B; ++b)
+    if (counts_host[b] < 0 || counts_host[b] > t->N)
+      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_instances_submit: frame %d has %d instances, not 0 to %d (max_instances_per_frame)",
+                     b, counts_host[b], t->N);
+  SB_CUDA(h, cudaSetDevice(h->device));
+  if ((rc = stream_alloc(h, t)) ||
+      (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C,
+                      {{t->gi_inst[slot], instances_host, (size_t)B * t->N * t->nodes * 2 * sizeof(float)},
+                       {t->gi_count[slot], counts_host, (size_t)B * sizeof(int32_t)}})))
+    return rc;
+  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
+  if ((rc = select_centroids(h, mc, t, sl.frames[slot], 1, B))) return rc;
+  k_td_gt_match<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->gi_inst[slot], t->gi_count[slot], t->N, t->nodes, t->K,
+                                          t->flags, t->gi_match, t->record, t->width);
+  SB_CHECK_LAUNCH(h);
+  SB_CUDA(h, cudaEventRecord(sl.frames_free[slot], h->stream));
+  SB_CUDA(h, cudaMemcpyAsync(sl.stage[slot], t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, h->stream));
   SB_CUDA(h, cudaEventRecord(sl.result[slot], h->stream));
   sl.submitted(slot, B);
   return SB_OK;
@@ -792,6 +944,42 @@ int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* fr
   SbTopdown* t = topdown_of(h, instance_model_id, mi->td && mi->td->multiclass, true, TD_GT);
   if (!t) return SB_ERR_INVALID;
   return topdown_gt_submit(h, t, frames_host, centroids_host, counts_host, B, slot);
+}
+
+int sb_topdown_gt_instances_configure(sb_handle_t h, const sb_topdown_params* p, int n_nodes, int max_instances_per_frame, int max_batch,
+                                      int H, int W, int C_in) {
+  static const char* const what = "sb_topdown_gt_instances_configure";
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "%s: null argument", what);
+  if (p->instance_model != -1) return sb_fail(h, SB_ERR_INVALID, "%s: instance_model must be -1", what);
+  SbModel* mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, "sb_topdown_gt_instances_configure: bad centroid model id");
+  if (!mc) return SB_ERR_INVALID;
+  if (p->max_centroids_per_frame <= 0 || n_nodes <= 0 || max_instances_per_frame <= 0 || max_batch <= 0)
+    return sb_fail(h, SB_ERR_INVALID, "%s: bad sizes", what);
+  if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "%s: more than 1024 frames per batch", what);
+  float s;
+  int Hr, Wr;
+  if (const int rc = precrop_size(h, p, H, W, &s, &Hr, &Wr)) return rc;
+  return gt_instances_setup(h, p, n_nodes, max_instances_per_frame, max_batch, H, W, C_in, mc);
+}
+
+int sb_topdown_gt_instances_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, const float* instances_host,
+                                   const int32_t* counts_host, int B, int slot) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, true, TD_GTI);
+  if (!t) return SB_ERR_INVALID;
+  return topdown_gt_instances_submit(h, h->models[centroid_model_id], t, frames_host, instances_host, counts_host, B, slot);
+}
+
+int sb_topdown_gt_instances_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
+                                    int32_t* out_n_centroids, float* out_instance_peaks, float* out_instance_peak_vals,
+                                    int32_t* out_n_rows, int32_t* out_flags) {
+  SbTopdown* t = topdown_of(h, centroid_model_id, false, true, TD_GTI);
+  if (!t) return SB_ERR_INVALID;
+  if (const int rc = topdown_collect(h, centroid_model_id, t, slot, B)) return rc;
+  const size_t K = t->K, nd = t->nodes;
+  sb_split_records(t->slots.stage[slot], B, t->width,
+                   {{out_centroids, K * 2}, {out_centroid_vals, K}, {out_instance_peaks, K * nd * 2}, {out_instance_peak_vals, K * nd}},
+                   {out_n_centroids, out_n_rows, out_flags});
+  return SB_OK;
 }
 
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w) {

@@ -93,14 +93,14 @@ class InferenceModel:
 
     def predict_examples(self, examples, batch_size: int, max_centroids: int):
         """Generator over (example, result dict) for batches of labels examples (dicts with the frames ``image`` and the
-        ground-truth ``centroids``, at most ``max_centroids`` per frame): the batch loop of a predictor fed labels.  A run
-        of batches whose frames the model's ground-truth step takes (``_stream_ground_truth``) is double-buffered as
-        predict_batches is; other batches take one predict_on_batch each."""
+        ground-truth ``centroids`` and ``instances``, at most ``max_centroids`` of each per frame): the batch loop of a
+        predictor fed labels.  A run of batches whose frames the model's ground-truth step takes (``_stream_ground_truth``)
+        is double-buffered as predict_batches is; other batches take one predict_on_batch each."""
         it = iter(examples)
         ex = next(it, None)
         while ex is not None:
             first = InferenceLayer._prep(ex["image"])
-            got = self._stream_ground_truth(first, batch_size, max_centroids)
+            got = self._stream_ground_truth(first, batch_size, max_centroids, ex)
             if got is None:
                 yield ex, self.predict_on_batch(ex)
                 ex = next(it, None)
@@ -111,22 +111,31 @@ class InferenceModel:
             def run(ex=ex):                   # the examples up to the first with other frames, as submit arguments
                 while ex is not None:
                     imgs = InferenceLayer._prep(ex["image"])
-                    if imgs.shape[1:] != first.shape[1:] or imgs.dtype != first.dtype:
+                    table = None
+                    if imgs.shape[1:] == first.shape[1:] and imgs.dtype == first.dtype:
+                        table = self._ground_truth_table(ex, K)
+                    if table is None:
                         rest.append(ex)
                         return
                     order.append(ex)
-                    yield (imgs,) + _centroid_table(ex["centroids"], K)
+                    yield (imgs,) + table
                     ex = next(it, None)
 
             for out in _pipelined_batches(run(), *stream):
                 yield order.popleft(), out
             ex = rest[0] if rest else None
 
-    def _stream_ground_truth(self, first, batch_size, max_centroids):
-        """The streamed ground-truth step for batches of up to ``batch_size`` labels examples with frames like ``first``
-        (prepped) and up to ``max_centroids`` centroids per frame, set up for them: ((device model, submit call,
-        ``collect(slot, B)``), K of the centroid tables it takes), or None for the per-batch route."""
+    def _stream_ground_truth(self, first, batch_size, max_centroids, ex=None):
+        """The streamed ground-truth step for batches of up to ``batch_size`` labels examples like ``ex`` with frames like
+        ``first`` (prepped) and up to ``max_centroids`` centroids (or labelled instances) per frame, set up for them:
+        ((device model, submit call, ``collect(slot, B)``), the capacity of the tables it takes), or None for the
+        per-batch route."""
         return None
+
+    def _ground_truth_table(self, ex, K):
+        """The arrays the ground-truth submit takes after the frames of labels example ``ex``, for tables of capacity K:
+        the centroid table and counts; None when the streamed step cannot take the example."""
+        return _centroid_table(ex["centroids"], K)
 
 
 def _merge_batches(chunks):
@@ -575,6 +584,37 @@ def _ground_truth_params(cc, fp, K):
                          int(fp.max_crops_per_call), float(cc.input_scale))
 
 
+def _instance_nodes(instances):
+    """The node count of a batch's ground-truth instances (one (n, nodes, 2) array per frame) as the host route's batch
+    dict has it (the most nodes of any frame's array), or None when the fused step cannot take them: no nodes, or a
+    frame with instances of another shape."""
+    arrs = [np.asarray(a) for a in instances]
+    nodes = max([a.shape[1] for a in arrs if a.ndim == 3] + [0])
+    if nodes == 0 or any(len(a) and (a.ndim != 3 or a.shape[1:] != (nodes, 2)) for a in arrs):
+        return None
+    return nodes
+
+
+def _instance_table(instances, N, nodes):
+    """The ground-truth instances of a batch (one (n, nodes, 2) array per frame) as sb_topdown_gt_instances_submit takes
+    them: the (B, N, nodes, 2) float32 table, NaN past each frame's count, and the (B,) int32 counts.  A frame with more
+    than N instances keeps its count, so the submit refuses the batch rather than dropping instances."""
+    arrs = [f32(a) for a in instances]
+    counts = np.asarray([len(a) for a in arrs], np.int32)
+    table = np.full((len(arrs), N, nodes, 2), np.nan, np.float32)
+    for b, a in enumerate(arrs):
+        if len(a):
+            table[b, :len(a)] = a[:N]
+    return table, counts
+
+
+def _gt_instances_params(cc):
+    """TopdownParams of the ground-truth instances pipeline of centroid layer ``cc`` (no instance model), and its K."""
+    K = int(cc.max_instances) if cc.max_instances else int(cc.max_peaks_per_sample)
+    return TopdownParams(cc.keras_model.model_id, -1, cc.params(), GlobalParams(), int(cc.crop_size), int(cc.max_instances or 0), K, 1,
+                         float(cc.precrop_resize)), K
+
+
 class TopDownInferenceModel(InferenceModel):
     """sleap/nn/inference.py:2246-2311."""
 
@@ -584,6 +624,7 @@ class TopDownInferenceModel(InferenceModel):
         self.fused = True            # one device pipeline (sb_infer_topdown) when both stages are device models
         # a Tracker with track_device, run by k_track inside each fused step (TopDownPredictor.predict sets it for its span)
         self.tracker = None
+        self._gt_instances = None    # (what, B, N, the centroid model's chain record) of the last ground-truth instances configure
 
     def detach_tracker(self):
         mc = self.centroid_crop.keras_model
@@ -603,6 +644,58 @@ class TopDownInferenceModel(InferenceModel):
     def ground_truth(self):
         """Centroids come from the labels (CentroidCropGroundTruth), not from a centroid model."""
         return isinstance(self.centroid_crop, CentroidCropGroundTruth)
+
+    def _fuses_instances(self):
+        """A centroid model with ground-truth instances (FindInstancePeaksGroundTruth) runs as one device step
+        (sb_topdown_gt_instances_submit) on uint8 labels examples."""
+        cc = self.centroid_crop
+        return (self.fused and type(self.instance_peaks) is FindInstancePeaksGroundTruth and type(cc) is CentroidCrop
+                and not cc.return_confmaps and (cc.max_instances is None or cc.max_instances > 0))
+
+    def _configure_gt_instances(self, B, N, nodes, shape):
+        """The ground-truth instances pipeline of the centroid model for batches of up to B frames of ``shape`` (H, W, C)
+        with tables of up to N instances of ``nodes`` nodes, unless it already runs with at least these capacities: B and
+        N grow only when a batch exceeds them.  Returns (K, N) of the pipeline."""
+        cc = self.centroid_crop
+        mc = cc.keras_model
+        p, K = _gt_instances_params(cc)
+        what = (chain_key(p), int(nodes), tuple(shape))
+        have = self._gt_instances
+        if have is not None and have[0] == what and mc.chain is have[3]:
+            if B <= have[1] and N <= have[2]:
+                return K, have[2]
+            B, N = max(B, have[1]), max(N, have[2])
+        N = max(N, 1)
+        mc.chain = None                          # a refused call may have dropped the previous chain
+        mc.handle.call("sb_topdown_gt_instances_configure", byref(p), int(nodes), N, B, *shape)
+        mc.configured_for = (B,) + tuple(shape)
+        mc.chain = ("sb_topdown_gt_instances_configure", chain_key(p))
+        self._gt_instances = (what, B, N, mc.chain)
+        return K, N
+
+    def _run_gt_instances(self, B, K, nodes, slot):
+        """sb_topdown_gt_instances_collect of ``slot`` into the batch dict of the host route: the centroids padded to the
+        batch's most centroids, the matched instances to its most rows (``n_valid``)."""
+        mc = self.centroid_crop.keras_model
+        ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
+        ip = np.zeros((B, K, nodes, 2), np.float32); iv = np.zeros((B, K, nodes), np.float32)
+        nc = np.zeros((B,), np.int32); nr = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
+        mc.handle.call("sb_topdown_gt_instances_collect", mc.model_id, slot, B, ptr(ce), ptr(cv), ptr(nc), ptr(ip), ptr(iv), ptr(nr),
+                       ptr(fl))
+        c, r = int(nc.max()), int(nr.max())
+        return {"centroids": ce[:, :c].copy(), "centroid_vals": cv[:, :c].copy(), "instance_peaks": ip[:, :r].copy(),
+                "instance_peak_vals": iv[:, :r].copy(), "n_valid": nr.astype(np.int64), "flags": fl}
+
+    def _call_gt_instances(self, example, imgs, nodes):
+        """One batch through the ground-truth instances step: the table packed for the pipeline's N (grown to the batch's
+        most instances if needed), a submit into slot 0, then its collect."""
+        B = imgs.shape[0]
+        n = max([len(a) for a in example["instances"]] + [0])
+        K, N = self._configure_gt_instances(B, n, nodes, imgs.shape[1:])
+        table, counts = _instance_table(example["instances"], N, nodes)
+        mc = self.centroid_crop.keras_model
+        mc.handle.call("sb_topdown_gt_instances_submit", mc.model_id, ptr(imgs), ptr(table), ptr(counts), B, 0)
+        return self._run_gt_instances(B, K, nodes, 0)
 
     def _owner(self):
         """The device model that holds the fused pipeline: the centroid model, or with ground-truth centroids the
@@ -656,13 +749,29 @@ class TopDownInferenceModel(InferenceModel):
         cc, fp = self.centroid_crop, self.instance_peaks
         return _configure_ground_truth(cc, fp, "sb_topdown_configure", lambda k: _ground_truth_params(cc, fp, k), B, K, shape)
 
-    def _stream_ground_truth(self, first, batch_size, max_centroids):
+    def _stream_ground_truth(self, first, batch_size, max_centroids, ex=None):
         """sb_topdown_gt_submit / sb_topdown_collect: uint8 frames and a model that can run the fused step with
-        ground-truth centroids.  The whole step is queued at the submit."""
-        if not (self._can_fuse() and self.ground_truth) or first.dtype != np.uint8:
+        ground-truth centroids; or sb_topdown_gt_instances_submit / _collect: uint8 frames and ground-truth instances
+        (``ex``) for a centroid model, tables of ``max_centroids`` instances.  The whole step is queued at the submit."""
+        if first.dtype != np.uint8:
+            return None
+        if self._fuses_instances():
+            nodes = _instance_nodes(ex["instances"]) if ex is not None and "instances" in ex else None
+            if nodes is None:
+                return None
+            K, N = self._configure_gt_instances(batch_size, max_centroids, nodes, first.shape[1:])
+            return (self.centroid_crop.keras_model, "sb_topdown_gt_instances_submit",
+                    lambda slot, B: self._run_gt_instances(B, K, nodes, slot)), N
+        if not (self._can_fuse() and self.ground_truth):
             return None
         K = self._configure_ground_truth(batch_size, max_centroids, first.shape[1:])
         return (self.instance_peaks.keras_model, "sb_topdown_gt_submit", lambda slot, B: self._run_ground_truth(B, K, slot)), K
+
+    def _ground_truth_table(self, ex, K):
+        if not self._fuses_instances():
+            return super()._ground_truth_table(ex, K)
+        nodes = self._gt_instances[0][1]
+        return _instance_table(ex["instances"], K, nodes) if _instance_nodes(ex["instances"]) == nodes else None
 
     def _run_ground_truth(self, B, K, slot):
         return self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot)
@@ -670,6 +779,11 @@ class TopDownInferenceModel(InferenceModel):
     def call(self, example):
         if isinstance(example, np.ndarray):
             example = dict(image=example)
+        if self._fuses_instances() and "instances" in example:
+            imgs = InferenceLayer._prep(example["image"])
+            nodes = _instance_nodes(example["instances"])
+            if imgs.dtype == np.uint8 and nodes is not None:
+                return self._call_gt_instances(example, imgs, nodes)
         if self._can_fuse() and not self.ground_truth:
             return self._call_fused(_images_of(example))
         if self._can_fuse() and "centroids" in example and np.asarray(example["image"]).dtype == np.uint8:
@@ -1228,7 +1342,7 @@ class TopDownMultiClassInferenceModel(InferenceModel):
     def _run_ground_truth(self, B, K, slot):
         return self._run_fused(B, K, head_channels(self.instance_peaks.keras_model, "ClassVectorsHead"), "sb_topdown_multiclass_collect", slot)
 
-    def _stream_ground_truth(self, first, batch_size, max_centroids):
+    def _stream_ground_truth(self, first, batch_size, max_centroids, ex=None):
         """sb_topdown_gt_submit / sb_topdown_multiclass_collect, as TopDownInferenceModel's."""
         if not (self._can_fuse() and self.ground_truth) or first.dtype != np.uint8:
             return None

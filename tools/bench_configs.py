@@ -51,6 +51,15 @@ sb_infer_global per chunk), the fused step per batch (predict_on_batch: sb_topdo
 double-buffered loop predict runs on labels (predict_examples).  The line reports the card and its power limit, frames/s
 per arm (median and range over the repetitions) and whether all arms agree bit for bit.
 
+topdown_gt_instances: a top-down predictor built from the C3 centroid UNet (input scale 0.5) alone, ground-truth
+instances standing in for the instance model (FindInstancePeaksGroundTruth), on labels of 128 gray tracking-clip frames
+with 5 synthetic instances of 13 nodes each (some nodes invisible), B=16, the centroid threshold calibrated to about 5
+animals per frame.  Three arms alternate in one process on the same decoded label batches: the host route (fused = False:
+the centroid list to the host, the match in numpy), the fused step per batch (predict_on_batch:
+sb_topdown_gt_instances_submit + collect) and the double-buffered loop predict runs on labels (predict_examples).  The
+line reports the card and its power limit, frames/s per arm (median and range over the repetitions) and whether all arms
+agree bit for bit.
+
 topdown_track: the top-down predictor with a tracker, four arms alternating in one process: TopDownPredictor.predict
 (labels made) of the C3 pair on 256 gray tracking-clip frames, B=16, the centroid threshold calibrated on clip frames to
 about 5 animals per frame; no tracker, the host simple tracker, the device simple tracker inside the fused step
@@ -586,6 +595,76 @@ def topdown_gt_bench(steps):
             "metric": "frames/s (median of alternating repetitions; decoded label batches in, result dicts out)", "workloads": res}
 
 
+def topdown_gt_instances_bench(steps):
+    """A centroid model with ground-truth instances (FindInstancePeaksGroundTruth, no instance model) through its three
+    routes (see the module docstring): the C3 centroid UNet at input scale 0.5 on 128 gray tracking-clip frames, B = 16,
+    the threshold calibrated to about 5 animals per frame, and 5 synthetic labelled instances of 13 nodes per frame."""
+    import torch
+    from scipy.ndimage import maximum_filter
+    from sleap_b200.io.labels import Instance, LabeledFrame, Labels, LabelsReader, Skeleton
+    from sleap_b200.io.video import Video
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from flow_clip import clip_frames
+    n, B, animals = 128, 16, 5
+    gray = torch.from_numpy(np.ascontiguousarray(clip_frames(n)[:, :, :, :1])).pin_memory().numpy()
+    H, W = gray.shape[1:3]
+    rng = np.random.default_rng(7)
+    sk = Skeleton(FLIES13, [])
+    lfs = []
+    for i in range(n):
+        pts = [(rng.uniform(80, [W - 80, H - 80]) + rng.normal(0, 20, (13, 2))).astype(np.float32) for _ in range(animals)]
+        for p in pts:
+            p[rng.random(13) < 0.1] = np.nan                                # some invisible nodes
+        lfs.append(LabeledFrame(0, i, [Instance(p, sk) for p in pts]))
+    labels = Labels(lfs, [{}], [sk])
+    labels.set_video(0, Video.from_numpy(gray))
+    cspec = dict(backbone="unet", backbone_cfg=unet(16, 16, 2), head_type="centroid", part_names=None, edges=None,
+                 heads=[dict(name="CentroidConfmapsHead", channels=1, output_stride=2)])
+
+    def predictor(fused):
+        # each arm owns its device model: the host route's centroid calls reconfigure the chain the fused pipeline needs
+        cm_model, _, _ = model_for(cspec, 1, 1003, input_scale=0.5)
+        cms = np.concatenate([cm_model.forward(gray[i:i + B])[0][..., 0] for i in range(0, 4 * B, B)])
+        fifth = [np.sort(c[c == maximum_filter(c, size=3, mode="constant", cval=-np.inf)])[-5] for c in cms]
+        pred = TopDownPredictor(cm_model, None, peak_threshold=float(np.median(fifth)), integral_refinement=True, batch_size=B)
+        pred.inference_model.fused = fused
+        return pred
+
+    host, fused = predictor(False), predictor(True)
+    reader = LabelsReader(labels, with_centroids=True)
+    batches = list(fused._label_examples(reader))
+    N = reader.max_instance_count()
+    him, fim = host.inference_model, fused.inference_model
+    arms = {"host route (fused = False)": lambda: [him.predict_on_batch(b) for b in batches],
+            "fused predict_on_batch": lambda: [fim.predict_on_batch(b) for b in batches],
+            "streamed predict_examples": lambda: [o for _, o in fim.predict_examples(batches, B, N)]}
+    outs = {k: f() for k, f in arms.items()}                             # warm-up, and the outputs compared
+    reps = max(5, steps)
+    times = {k: [] for k in arms}
+    for _ in range(reps):                                                # arms alternate
+        for k, f in arms.items():
+            t0 = time.perf_counter()
+            f()
+            times[k].append(time.perf_counter() - t0)
+    keys = ("n_valid", "flags", "centroids", "centroid_vals", "instance_peaks", "instance_peak_vals")
+    ref = outs["host route (fused = False)"]
+
+    def same(x, y):                                                      # NaN positions, not NaN payloads
+        x, y = np.asarray(x), np.asarray(y)
+        return x.dtype == y.dtype and x.shape == y.shape and bool(np.array_equal(x, y, equal_nan=x.dtype.kind == "f"))
+
+    agree = all(len(o) == len(ref) and all(same(x[k], y[k]) for x, y in zip(o, ref) for k in keys) for o in outs.values())
+    assert agree, "the routes disagree"
+    return {"config": "topdown_gt_instances: C3 centroid UNet (input scale 0.5) + ground-truth instances, 128 tracking-clip "
+                      "frames (1024x1024 gray), about 5 animals, 5 labelled instances of 13 nodes per frame, B=16",
+            "gpu": gpu_identity(),
+            "metric": "frames/s (median of alternating repetitions; decoded label batches in, result dicts out)", "repetitions": reps,
+            "frames_per_s": {k: n / float(np.median(v)) for k, v in times.items()},
+            "frames_per_s_range": {k: [n / max(v), n / min(v)] for k, v in times.items()},
+            "mean_centroids_per_frame": float(np.mean(np.concatenate([np.isfinite(o["centroid_vals"]).sum(1) for o in ref]))),
+            "mean_rows_per_frame": float(np.mean(np.concatenate([o["n_valid"] for o in ref]))), "arms_agree": agree}
+
+
 def topdown_track_bench(steps):
     """TopDownPredictor.predict (labels made) of the C3 pair of topdown() on 256 tracking-clip frames (gray), B = 16, the
     centroid threshold calibrated on clip frames to about 5 animals per frame.  Four arms alternate in one process: no
@@ -759,6 +838,8 @@ if __name__ == "__main__":
             r = topdown_scaled_bench(steps)
         elif c == "topdown_gt":
             r = topdown_gt_bench(steps)
+        elif c == "topdown_gt_instances":
+            r = topdown_gt_instances_bench(steps)
         elif c == "r50":
             r = resnet50(steps)
         elif c == "track":
