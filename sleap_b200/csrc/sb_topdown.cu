@@ -408,11 +408,17 @@ int head_from_params(sb_handle_s* h, const sb_topdown_multiclass_params* p, int 
   return 0;
 }
 
+// The forms of the pipeline by their centroid source: a centroid model (sb_topdown_configure, held by the centroid
+// model), ground-truth centroids (centroid_model = -1, held by the instance model), a centroid model with ground-truth
+// instances (sb_topdown_gt_instances_configure, no instance model, held by the centroid model).  A call takes a mask.
+enum { TD_MODEL = 1, TD_GT = 2, TD_GTI = 4 };
+
 }  // namespace
 
 struct SbTopdown {
   sb_topdown_params p{};
-  SbModel* inst = nullptr;
+  int form = TD_MODEL;
+  SbModel* inst = nullptr;          // the instance model (NULL in the TD_GTI form)
   unsigned gen_c = 0, gen_i = 0;    // chain_gen of the centroid and the instance model when it was configured
   int K = 0, nodes = 0, width = 0, Bmax = 0;
   int H = 0, W = 0, C = 0;          // the uint8 or float frames of a batch
@@ -421,7 +427,7 @@ struct SbTopdown {
   int* flags = nullptr;             // per-frame flags: the centroid model's ws.flags, or gt_flags
   float *sel_cent = nullptr, *sel_val = nullptr, *flat_cent = nullptr, *flat_off = nullptr, *ipts = nullptr, *ivals = nullptr, *record = nullptr;
   int *sel_count = nullptr, *flat_sample = nullptr, *offsets = nullptr, *total = nullptr;
-  void* crops = nullptr;
+  float* crops = nullptr;           // one chunk of float or uint8 crops
   // multi-class form (sb_topdown_multiclass_configure)
   bool multiclass = false;
   TdHead head{};
@@ -439,29 +445,22 @@ struct SbTopdown {
   cudaEvent_t count_ev[2] = {nullptr, nullptr};
   struct { const void* dev; int is_u8; } src[2] = {};   // the slot's frames, or a synchronous call's frames_dev
   int pending = -1;
-  // ground-truth form (sb_topdown_params.centroid_model = -1), held by its instance model.  gt_flags: the per-frame flags,
-  // which k_td_gt_select zeroes; gt_cent / gt_count: per slot the device copy of the batch's centroid table and counts,
-  // which k_td_gt_select reads.
-  bool gt = false;
-  int* gt_flags = nullptr;                     // [Bmax]
-  float* gt_cent[2] = {nullptr, nullptr};      // [Bmax][K][2]
-  int* gt_count[2] = {nullptr, nullptr};       // [Bmax]
-  // ground-truth instances form (sb_topdown_gt_instances_configure: no instance model), held by its centroid model.
-  // gi_inst / gi_count: per slot the device copy of the batch's instance table and counts, which k_td_gt_match reads;
-  // gi_match: its per-centroid picks.
-  bool gti = false;
-  int N = 0;                                   // instances per frame of the table
-  float* gi_inst[2] = {nullptr, nullptr};      // [Bmax][N][nodes][2]
-  int* gi_count[2] = {nullptr, nullptr};       // [Bmax]
-  int* gi_match = nullptr;                     // [Bmax][K]
+  // the table-fed forms (TD_GT, TD_GTI): per slot the device copy of the batch's host table and its counts -- the
+  // ground-truth centroids [Bmax][K][2], which k_td_gt_select reads, or the ground-truth instances [Bmax][N][nodes][2],
+  // which k_td_gt_match reads -- allocated at the first step; a frame's floats and row cap (K or N) of the table.
+  float* table[2] = {nullptr, nullptr};
+  int* table_count[2] = {nullptr, nullptr};    // [Bmax]
+  int table_floats = 0, table_rows = 0;
+  int* gt_flags = nullptr;                     // TD_GT: [Bmax] the per-frame flags, which k_td_gt_select zeroes
+  int* match = nullptr;                        // TD_GTI: [Bmax][K] k_td_gt_match's per-centroid picks
 };
 
 void sb_topdown_free(SbModel* m) {
   SbTopdown* t = m->td;
   if (!t) return;
   void* dev[] = {t->sel_cent, t->sel_val, t->flat_cent, t->flat_off, t->ipts, t->ivals, t->record, t->sel_count, t->flat_sample,
-                 t->offsets, t->total, t->crops, t->dense, t->probs, t->gt_flags, t->gt_cent[0], t->gt_cent[1], t->gt_count[0],
-                 t->gt_count[1], t->gi_inst[0], t->gi_inst[1], t->gi_count[0], t->gi_count[1], t->gi_match};
+                 t->offsets, t->total, t->crops, t->dense, t->probs, t->table[0], t->table[1], t->table_count[0], t->table_count[1],
+                 t->gt_flags, t->match};
   for (void* p : dev) if (p) cudaFree(p);
   t->slots.release();
   for (void* p : {(void*)t->count_host, (void*)t->probs_stage[0], (void*)t->probs_stage[1]})
@@ -482,29 +481,32 @@ int precrop_size(sb_handle_s* h, const sb_topdown_params* p, int H, int W, float
   return 0;
 }
 
-// The arguments both top-down configure calls check before anything is dropped.  *mc is NULL in the ground-truth form
-// (centroid_model = -1).
-int check_topdown(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, SbModel** mc, SbModel** mi) {
-  static const char* const bad_ids = "sb_topdown_configure: bad model ids";
-  const bool gt = p->centroid_model == -1;
-  *mc = gt ? nullptr : chain_model(h, p->centroid_model, SB_CHAIN_ANY, bad_ids);
-  *mi = chain_model(h, p->instance_model, SB_CHAIN_ANY, bad_ids);
-  if ((!gt && !*mc) || !*mi || *mc == *mi) return sb_fail(h, SB_ERR_INVALID, bad_ids);
-  if (p->crop_size <= 0 || p->max_centroids_per_frame <= 0 || p->max_crops_per_call <= 0 || max_batch <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: bad sizes");
-  if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_configure: more than 1024 frames per batch");
-  const int nb = (int)(*mi)->buffers.size();
-  if (p->instance.cms_buffer < 0 || p->instance.cms_buffer >= nb) return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
+// The arguments every top-down configure call checks before anything is dropped, for the pipeline of `form`; *mc is NULL
+// in the TD_GT form, *mi in the TD_GTI form, which has no instance model and ignores `instance`, crop_size and
+// max_crops_per_call but takes a table of N rows of n_nodes nodes per frame.
+int check_topdown(sb_handle_s* h, const char* what, const sb_topdown_params* p, int form, int max_batch, int H, int W, int n_nodes,
+                  int N, SbModel** mc, SbModel** mi) {
+  const bool has_c = form != TD_GT, has_i = form != TD_GTI;
+  if (!has_i && p->instance_model != -1) return sb_fail(h, SB_ERR_INVALID, "%s: instance_model must be -1", what);
+  *mc = has_c ? chain_model(h, p->centroid_model, SB_CHAIN_ANY, "bad model ids") : nullptr;
+  *mi = has_i ? chain_model(h, p->instance_model, SB_CHAIN_ANY, "bad model ids") : nullptr;
+  if ((has_c && !*mc) || (has_i && !*mi) || *mc == *mi) return sb_fail(h, SB_ERR_INVALID, "%s: bad model ids", what);
+  if (p->max_centroids_per_frame <= 0 || max_batch <= 0 || (has_i && (p->crop_size <= 0 || p->max_crops_per_call <= 0)) ||
+      (!has_i && (n_nodes <= 0 || N <= 0)))
+    return sb_fail(h, SB_ERR_INVALID, "%s: bad sizes", what);
+  if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "%s: more than 1024 frames per batch", what);
+  if (has_i && (p->instance.cms_buffer < 0 || p->instance.cms_buffer >= (int)(*mi)->buffers.size()))
+    return sb_fail(h, SB_ERR_INVALID, "bad cms buffer");
   float s;
   int Hr, Wr;
   return precrop_size(h, p, H, W, &s, &Hr, &Wr);
 }
 
-// Configures both networks and their chains, then the pipeline with a record of `width` floats per frame (the centroid
-// configure drops the previous pipeline).  On success mc->td is the new pipeline; in the ground-truth form (mc NULL), with
-// the instance network only, mi->td (the global configure dropped the previous one).
-int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in, SbModel* mc, SbModel* mi,
-                  int n_classes) {
+// Configures the networks of the form and their chains, then the pipeline of the form: on success the new pipeline is
+// the td of its owner, the centroid model (whose configure dropped the previous one) or in the TD_GT form the instance
+// model (whose global configure did).  n_classes > 0: the multi-class record; n_nodes and N: the TD_GTI table.
+int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int form, int max_batch, int H, int W, int C_in, SbModel* mc, SbModel* mi,
+                  int n_classes, int n_nodes, int N) {
   SB_CUDA(h, cudaSetDevice(h->device));
   int rc;
   if (mc && (rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in))) return rc;
@@ -512,113 +514,87 @@ int topdown_setup(sb_handle_s* h, const sb_topdown_params* p, int max_batch, int
   // crops, so that form plans it for no more than those
   const int chunk = mc ? p->max_crops_per_call
                        : (int)std::min<long long>(p->max_crops_per_call, (long long)max_batch * p->max_centroids_per_frame);
-  if ((rc = sb_model_configure(h, p->instance_model, chunk, p->crop_size, p->crop_size, C_in))) return rc;
+  if (mi && (rc = sb_model_configure(h, p->instance_model, chunk, p->crop_size, p->crop_size, C_in))) return rc;
   if (mc && (rc = sb_centroid_configure(h, p->centroid_model, &p->centroid))) return rc;
-  if ((rc = sb_global_configure(h, p->instance_model, &p->instance))) return rc;
+  if (mi && (rc = sb_global_configure(h, p->instance_model, &p->instance))) return rc;
   SbTopdown* t = new SbTopdown();
   SbModel* owner = mc ? mc : mi;
   owner->td = t;
-  t->p = *p; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
-  t->gen_c = mc ? mc->chain_gen : 0; t->gen_i = mi->chain_gen;
-  t->H = H; t->W = W; t->C = C_in; t->gt = !mc;
+  t->p = *p; t->form = form; t->inst = mi; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
+  t->gen_c = mc ? mc->chain_gen : 0; t->gen_i = mi ? mi->chain_gen : 0;
+  t->H = H; t->W = W; t->C = C_in;
   precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by check_topdown
-  t->nodes = mi->buffers[p->instance.cms_buffer].C;
+  t->nodes = mi ? mi->buffers[p->instance.cms_buffer].C : n_nodes;
   t->multiclass = n_classes > 0;
-  t->width = t->multiclass ? (int)td_class_record_width(n_classes, t->nodes, t->K) : t->K * (3 + t->nodes * 3) + 2;
-  const size_t N = (size_t)max_batch * t->K;
-  auto A = [&](void** q, size_t bytes) { return cudaMalloc(q, bytes + 16) == cudaSuccess; };
-  const bool ok = A((void**)&t->sel_cent, N * 2 * 4) && A((void**)&t->sel_val, N * 4) && A((void**)&t->sel_count, (size_t)max_batch * 4) &&
-                  A((void**)&t->flat_cent, N * 2 * 4) && A((void**)&t->flat_off, N * 2 * 4) && A((void**)&t->flat_sample, N * 4) &&
-                  A((void**)&t->offsets, ((size_t)max_batch + 1) * 4) && A((void**)&t->total, 4) &&
-                  A((void**)&t->ipts, N * t->nodes * 2 * 4) && A((void**)&t->ivals, N * t->nodes * 4) &&
-                  A((void**)&t->record, (size_t)max_batch * t->width * 4) &&
-                  A(&t->crops, (size_t)chunk * p->crop_size * p->crop_size * C_in * 4) &&
-                  (!t->multiclass || A((void**)&t->probs, N * n_classes * 4)) &&
-                  (mc || A((void**)&t->gt_flags, (size_t)max_batch * 4));
-  t->flags = mc ? mc->ws.flags : t->gt_flags;
-  if (!ok) {
-    sb_topdown_free(owner);
-    return sb_fail(h, SB_ERR_CUDA, "sb_topdown_configure: allocation failed");
-  }
-  return SB_OK;
-}
-
-// Configures the centroid network and its chain, then the ground-truth instances pipeline on the centroid model mc:
-// frames -> centroid stage -> k_td_gt_match against a table of N instances of n_nodes nodes per frame.
-int gt_instances_setup(sb_handle_s* h, const sb_topdown_params* p, int n_nodes, int N, int max_batch, int H, int W, int C_in,
-                       SbModel* mc) {
-  SB_CUDA(h, cudaSetDevice(h->device));
-  int rc;
-  if ((rc = sb_model_configure(h, p->centroid_model, max_batch, H, W, C_in)) || (rc = sb_centroid_configure(h, p->centroid_model, &p->centroid)))
-    return rc;
-  SbTopdown* t = new SbTopdown();
-  mc->td = t;
-  t->p = *p; t->K = p->max_centroids_per_frame; t->Bmax = max_batch;
-  t->gen_c = mc->chain_gen;
-  t->H = H; t->W = W; t->C = C_in; t->gti = true; t->N = N;
-  precrop_size(h, p, H, W, &t->scale, &t->Hr, &t->Wr);     // checked by the caller
-  t->nodes = n_nodes;
-  t->width = t->K * (3 + n_nodes * 3) + 3;
-  t->flags = mc->ws.flags;
-  const size_t KB = (size_t)max_batch * t->K;
+  // the dense per-frame record of k_td_class_assign, k_td_pack or k_td_gt_match
+  const int K = t->K, nodes = t->nodes;
+  t->width = t->multiclass ? (int)td_class_record_width(n_classes, nodes, K) : K * (3 + nodes * 3) + (form == TD_GTI ? 3 : 2);
+  t->table_rows = form == TD_GT ? K : N;
+  t->table_floats = form == TD_GT ? K * 2 : N * nodes * 2;
+  const size_t KB = (size_t)max_batch * K;
   if ((rc = sb_dev_alloc(h, &t->sel_cent, KB * 2)) || (rc = sb_dev_alloc(h, &t->sel_val, KB)) ||
-      (rc = sb_dev_alloc(h, &t->sel_count, (size_t)max_batch)) || (rc = sb_dev_alloc(h, &t->gi_match, KB)) ||
-      (rc = sb_dev_alloc(h, &t->record, (size_t)max_batch * t->width))) {
-    sb_topdown_free(mc);
+      (rc = sb_dev_alloc(h, &t->sel_count, (size_t)max_batch)) || (rc = sb_dev_alloc(h, &t->record, (size_t)max_batch * t->width)) ||
+      (mi && ((rc = sb_dev_alloc(h, &t->flat_cent, KB * 2)) || (rc = sb_dev_alloc(h, &t->flat_off, KB * 2)) ||
+              (rc = sb_dev_alloc(h, &t->flat_sample, KB)) || (rc = sb_dev_alloc(h, &t->offsets, (size_t)max_batch + 1)) ||
+              (rc = sb_dev_alloc(h, &t->total, 1)) || (rc = sb_dev_alloc(h, &t->ipts, KB * nodes * 2)) ||
+              (rc = sb_dev_alloc(h, &t->ivals, KB * nodes)) ||
+              (rc = sb_dev_alloc(h, &t->crops, (size_t)chunk * p->crop_size * p->crop_size * C_in)))) ||
+      (t->multiclass && (rc = sb_dev_alloc(h, &t->probs, KB * n_classes))) ||
+      (form == TD_GT && (rc = sb_dev_alloc(h, &t->gt_flags, (size_t)max_batch))) ||
+      (form == TD_GTI && (rc = sb_dev_alloc(h, &t->match, KB)))) {
+    sb_topdown_free(owner);
     return rc;
   }
+  t->flags = mc ? mc->ws.flags : t->gt_flags;
   return SB_OK;
 }
 
-// The centroid sources a call takes: a centroid model, ground-truth centroids (sb_topdown_gt_submit), a centroid model
-// with ground-truth instances (sb_topdown_gt_instances_submit)
-enum { TD_MODEL = 1, TD_GT = 2, TD_GTI = 4 };
+// The calls of each form and kind: the refusals of a call on the wrong form or kind name the pipeline's own.  The
+// table-fed forms have no synchronous call: a batch is a submit and a collect.
+struct TdCalls {
+  const char *source, *submit, *collect, *sync, *configure;
+};
 
-// The pipeline of model `id` (its centroid model, or the instance model of a ground-truth pipeline) when it is of the
-// wanted form and no model of it was reconfigured since.  `streamed`: the refusal of the wrong form names the submit
-// call rather than the synchronous one.  `sources`: the TD_* forms the call takes.
-SbTopdown* topdown_of(sb_handle_s* h, int id, bool multiclass, bool streamed = false, int sources = TD_MODEL) {
+const TdCalls& td_calls(const SbTopdown* t) {
+  static const TdCalls calls[3][2] = {
+      {{"runs a centroid model", "sb_topdown_submit", "sb_topdown_collect", "sb_infer_topdown", "sb_topdown_configure"},
+       {"runs a centroid model", "sb_topdown_multiclass_submit", "sb_topdown_multiclass_collect", "sb_infer_topdown_multiclass",
+        "sb_topdown_multiclass_configure"}},
+      {{"takes ground-truth centroids", "sb_topdown_gt_submit", "sb_topdown_collect", "sb_topdown_gt_submit", "sb_topdown_configure"},
+       {"takes ground-truth centroids", "sb_topdown_gt_submit", "sb_topdown_multiclass_collect", "sb_topdown_gt_submit",
+        "sb_topdown_multiclass_configure"}},
+      {{"takes ground-truth instances", "sb_topdown_gt_instances_submit", "sb_topdown_gt_instances_collect",
+        "sb_topdown_gt_instances_submit", "sb_topdown_gt_instances_configure"},
+       {}}};                                       // no multi-class form
+  return calls[t->form == TD_MODEL ? 0 : t->form == TD_GT ? 1 : 2][t->multiclass];
+}
+
+// The pipeline of model `id` (its owner) when it is of one of the forms `sources` (a mask of TD_*) and of the kind
+// `multiclass` (-1: either), and no model of it was reconfigured since.  `streamed`: a refusal names the pipeline's submit
+// and collect calls, not its synchronous one.
+SbTopdown* topdown_of(sb_handle_s* h, int id, int sources, int multiclass, bool streamed) {
   static const char* const none = "top-down pipeline not configured";
-  SbModel* mc = chain_model(h, id, SB_CHAIN_ANY, none);
-  if (!mc) return nullptr;
-  SbTopdown* t = mc->td;
+  SbModel* owner = chain_model(h, id, SB_CHAIN_ANY, none);
+  if (!owner) return nullptr;
+  SbTopdown* t = owner->td;
   if (!t) { sb_fail(h, SB_ERR_INVALID, none); return nullptr; }
-  if (!(sources & (t->gti ? TD_GTI : t->gt ? TD_GT : TD_MODEL))) {
-    if (t->gti)
-      sb_fail(h, SB_ERR_INVALID,
-              "top-down pipeline takes ground-truth instances: call sb_topdown_gt_instances_submit / sb_topdown_gt_instances_collect");
-    else if (t->gt)
-      sb_fail(h, SB_ERR_INVALID, "top-down pipeline takes ground-truth centroids: call sb_topdown_gt_submit");
-    else
-      sb_fail(h, SB_ERR_INVALID, "top-down pipeline runs a centroid model: call %s",
-              multiclass ? "sb_topdown_multiclass_submit" : "sb_topdown_submit");
-    return nullptr;
-  }
-  // the centroid model holds the pipeline, and a configure call on it dropped the pipeline with its chain
-  if (t->gti) return t;
-  if (t->gt) {
-    // the instance model holds the pipeline: a configure call on it dropped the pipeline with its chain
-    if (t->multiclass != multiclass) {
-      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_collect"
-                                            : "top-down pipeline is multi-class: call sb_topdown_multiclass_collect");
-      return nullptr;
-    }
-    return t;
-  }
-  if (t->multiclass != multiclass) {
+  const TdCalls& c = td_calls(t);
+  const char* why = !(sources & t->form)                          ? c.source
+                    : multiclass >= 0 && t->multiclass != (multiclass != 0) ? (t->multiclass ? "is multi-class" : "is not multi-class")
+                                                                  : nullptr;
+  if (why) {
     if (streamed)
-      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_topdown_submit"
-                                            : "top-down pipeline is multi-class: call sb_topdown_multiclass_submit");
+      sb_fail(h, SB_ERR_INVALID, "top-down pipeline %s: call %s / %s", why, c.submit, c.collect);
     else
-      sb_fail(h, SB_ERR_INVALID, multiclass ? "top-down pipeline is not multi-class: call sb_infer_topdown"
-                                            : "top-down pipeline is multi-class: call sb_infer_topdown_multiclass");
+      sb_fail(h, SB_ERR_INVALID, "top-down pipeline %s: call %s", why, c.sync);
     return nullptr;
   }
-  SbModel* mi = t->inst;
-  // a configure call on either model outside the pipeline's configure moved its chain_gen (sb_model_configure included)
-  if (mc->chain != SB_CHAIN_CENTROID || mc->chain_gen != t->gen_c || mi->chain != SB_CHAIN_GLOBAL || mi->chain_gen != t->gen_i) {
-    sb_fail(h, SB_ERR_INVALID, "top-down pipeline: a model was reconfigured; call %s again",
-            multiclass ? "sb_topdown_multiclass_configure" : "sb_topdown_configure");
+  // a configure call on the owner dropped the pipeline with its chain; one on the instance model of the TD_MODEL form
+  // outside the pipeline's configure moved its chain_gen (sb_model_configure included)
+  const SbModel* mi = t->inst;
+  if (t->form == TD_MODEL && (owner->chain != SB_CHAIN_CENTROID || owner->chain_gen != t->gen_c || mi->chain != SB_CHAIN_GLOBAL ||
+                              mi->chain_gen != t->gen_i)) {
+    sb_fail(h, SB_ERR_INVALID, "top-down pipeline: a model was reconfigured; call %s again", c.configure);
     return nullptr;
   }
   return t;
@@ -744,10 +720,8 @@ int stream_alloc(sb_handle_s* h, SbTopdown* t) {
   for (int i = 0; i < 2; ++i) {
     if (t->multiclass && !t->probs_stage[i]) SB_CUDA(h, cudaHostAlloc((void**)&t->probs_stage[i], probs_bytes, cudaHostAllocDefault));
     if (!t->count_ev[i]) SB_CUDA(h, cudaEventCreateWithFlags(&t->count_ev[i], cudaEventDisableTiming));
-    if (t->gt && !t->gt_cent[i] && (rc = sb_dev_alloc(h, &t->gt_cent[i], (size_t)t->Bmax * t->K * 2))) return rc;
-    if (t->gt && !t->gt_count[i] && (rc = sb_dev_alloc(h, &t->gt_count[i], (size_t)t->Bmax))) return rc;
-    if (t->gti && !t->gi_inst[i] && (rc = sb_dev_alloc(h, &t->gi_inst[i], (size_t)t->Bmax * t->N * t->nodes * 2))) return rc;
-    if (t->gti && !t->gi_count[i] && (rc = sb_dev_alloc(h, &t->gi_count[i], (size_t)t->Bmax))) return rc;
+    if (t->form != TD_MODEL && !t->table[i] && (rc = sb_dev_alloc(h, &t->table[i], (size_t)t->Bmax * t->table_floats))) return rc;
+    if (t->form != TD_MODEL && !t->table_count[i] && (rc = sb_dev_alloc(h, &t->table_count[i], (size_t)t->Bmax))) return rc;
   }
   SB_CUDA(h, cudaHostAlloc((void**)&t->count_host, 2 * sizeof(int), cudaHostAllocDefault));   // last: marks it complete
   return 0;
@@ -767,7 +741,7 @@ int queue_centroids(sb_handle_s* h, SbModel* mc, SbTopdown* t, const void* frame
 // last used them have run; (2) the instance stage of the batch submitted before it, if no collect queued it yet;
 // (3) its own centroid stage.  The stream order instance(k) -> centroid(k + 1) lets one set of selection buffers serve.
 int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, int slot, bool multiclass) {
-  SbTopdown* t = topdown_of(h, id, multiclass, true);
+  SbTopdown* t = topdown_of(h, id, TD_MODEL, multiclass, true);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[id];
   SbSlots& sl = t->slots;
@@ -780,66 +754,50 @@ int topdown_submit(sb_handle_s* h, int id, const uint8_t* frames_host, int B, in
   return queue_centroids(h, mc, t, sl.frames[slot], 1, B, slot);
 }
 
-// Streamed batch with ground-truth centroids into `slot`, the whole step queued at once (the host knows the crop count):
-// the frames, then the centroid table and counts, on the copy stream into the slot; k_td_gt_select and the crop list
-// behind that copy on the handle's stream; then the instance stage.  The table has its own per-slot staging: the batch
-// before may still be reading the selection buffers when the copy lands.
-int topdown_gt_submit(sb_handle_s* h, SbTopdown* t, const uint8_t* frames_host, const float* centroids_host, const int32_t* counts_host,
-                      int B, int slot) {
+// Streamed batch of a table-fed form into `slot` (sb_topdown_gt_submit, sb_topdown_gt_instances_submit), the whole step
+// queued at once, since nothing in it waits on the host: the frames, the table and its counts (each in [0, table_rows])
+// on the copy stream into the slot; behind that copy on the handle's stream, the form's launches -- ground-truth
+// centroids: k_td_gt_select, the crop list and the instance stage; ground-truth instances: the centroid stage,
+// k_td_gt_match and the records' copy.  The table has its own per-slot staging: the batch before may still be reading
+// the selection buffers when the copy lands; it is free again once the slot's frames are (frames_free).
+int table_submit(sb_handle_s* h, int id, int form, const uint8_t* frames_host, const float* table_host, const int32_t* counts_host,
+                 int B, int slot) {
+  SbTopdown* t = topdown_of(h, id, form, -1, true);
+  if (!t) return SB_ERR_INVALID;
+  const char* what = td_calls(t).submit;
   SbSlots& sl = t->slots;
-  int rc = sl.check_submit(h, "sb_topdown_gt_submit", slot, B, t->Bmax, centroids_host && counts_host ? frames_host : nullptr);
+  int rc = sl.check_submit(h, what, slot, B, t->Bmax, table_host && counts_host ? frames_host : nullptr);
   if (rc) return rc;
   int total = 0;
   for (int b = 0; b < B; ++b) {
-    if (counts_host[b] < 0 || counts_host[b] > t->K)
-      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_submit: frame %d has %d centroids, not 0 to %d (max_centroids_per_frame)", b,
-                     counts_host[b], t->K);
+    if (counts_host[b] < 0 || counts_host[b] > t->table_rows)
+      return sb_fail(h, SB_ERR_INVALID, "%s: frame %d has %d %s, not 0 to %d (%s)", what, b, counts_host[b],
+                     form == TD_GT ? "centroids" : "instances", t->table_rows,
+                     form == TD_GT ? "max_centroids_per_frame" : "max_instances_per_frame");
     total += counts_host[b];
   }
   SB_CUDA(h, cudaSetDevice(h->device));
   if ((rc = stream_alloc(h, t)) ||
       (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C,
-                      {{t->gt_cent[slot], centroids_host, (size_t)B * t->K * 2 * sizeof(float)},
-                       {t->gt_count[slot], counts_host, (size_t)B * sizeof(int32_t)}})))
+                      {{t->table[slot], table_host, (size_t)B * t->table_floats * sizeof(float)},
+                       {t->table_count[slot], counts_host, (size_t)B * sizeof(int32_t)}})))
     return rc;
   SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
-  k_td_gt_select<<<B, 128, 0, h->stream>>>(t->gt_cent[slot], t->gt_count[slot], t->K, t->scale, t->sel_cent, t->sel_val, t->sel_count,
-                                           t->gt_flags);
-  SB_CHECK_LAUNCH(h);
-  if ((rc = flatten(h, t, B)) ||
-      (rc = instance_stage(h, nullptr, t, sl.frames[slot], 1, B, total, sl.stage[slot], nullptr, t->probs_stage[slot], sl.frames_free[slot])))
-    return rc;
-  SB_CUDA(h, cudaEventRecord(sl.result[slot], h->stream));
-  sl.submitted(slot, B);
-  return SB_OK;
-}
-
-// Streamed batch with ground-truth instances into `slot`, the whole step queued at once (nothing in it waits on the
-// host): the frames, then the instance table and counts, on the copy stream into the slot; the centroid stage behind
-// that copy on the handle's stream; k_td_gt_match; the records' copy.  The table has its own per-slot staging, free
-// again once the slot's frames are (frames_free, recorded after the match).
-int topdown_gt_instances_submit(sb_handle_s* h, SbModel* mc, SbTopdown* t, const uint8_t* frames_host, const float* instances_host,
-                                const int32_t* counts_host, int B, int slot) {
-  SbSlots& sl = t->slots;
-  int rc = sl.check_submit(h, "sb_topdown_gt_instances_submit", slot, B, t->Bmax, instances_host && counts_host ? frames_host : nullptr);
-  if (rc) return rc;
-  for (int b = 0; b < B; ++b)
-    if (counts_host[b] < 0 || counts_host[b] > t->N)
-      return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_instances_submit: frame %d has %d instances, not 0 to %d (max_instances_per_frame)",
-                     b, counts_host[b], t->N);
-  SB_CUDA(h, cudaSetDevice(h->device));
-  if ((rc = stream_alloc(h, t)) ||
-      (rc = sl.upload(h, slot, frames_host, (size_t)B * t->H * t->W * t->C,
-                      {{t->gi_inst[slot], instances_host, (size_t)B * t->N * t->nodes * 2 * sizeof(float)},
-                       {t->gi_count[slot], counts_host, (size_t)B * sizeof(int32_t)}})))
-    return rc;
-  SB_CUDA(h, cudaStreamWaitEvent(h->stream, sl.h2d_done[slot], 0));
-  if ((rc = select_centroids(h, mc, t, sl.frames[slot], 1, B))) return rc;
-  k_td_gt_match<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->gi_inst[slot], t->gi_count[slot], t->N, t->nodes, t->K,
-                                          t->flags, t->gi_match, t->record, t->width);
-  SB_CHECK_LAUNCH(h);
-  SB_CUDA(h, cudaEventRecord(sl.frames_free[slot], h->stream));
-  SB_CUDA(h, cudaMemcpyAsync(sl.stage[slot], t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (form == TD_GT) {
+    k_td_gt_select<<<B, 128, 0, h->stream>>>(t->table[slot], t->table_count[slot], t->K, t->scale, t->sel_cent, t->sel_val, t->sel_count,
+                                             t->flags);
+    SB_CHECK_LAUNCH(h);
+    if ((rc = flatten(h, t, B)) ||
+        (rc = instance_stage(h, nullptr, t, sl.frames[slot], 1, B, total, sl.stage[slot], nullptr, t->probs_stage[slot], sl.frames_free[slot])))
+      return rc;
+  } else {
+    if ((rc = select_centroids(h, h->models[id], t, sl.frames[slot], 1, B))) return rc;
+    k_td_gt_match<<<B, 128, 0, h->stream>>>(t->sel_cent, t->sel_val, t->sel_count, t->table[slot], t->table_count[slot], t->table_rows,
+                                            t->nodes, t->K, t->flags, t->match, t->record, t->width);
+    SB_CHECK_LAUNCH(h);
+    SB_CUDA(h, cudaEventRecord(sl.frames_free[slot], h->stream));
+    SB_CUDA(h, cudaMemcpyAsync(sl.stage[slot], t->record, (size_t)B * t->width * 4, cudaMemcpyDeviceToHost, h->stream));
+  }
   SB_CUDA(h, cudaEventRecord(sl.result[slot], h->stream));
   sl.submitted(slot, B);
   return SB_OK;
@@ -910,14 +868,15 @@ extern "C" {
 int sb_topdown_configure(sb_handle_t h, const sb_topdown_params* p, int max_batch, int H, int W, int C_in) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_configure: null argument");
   SbModel *mc, *mi;
-  if (const int rc = check_topdown(h, p, max_batch, H, W, &mc, &mi)) return rc;
-  return topdown_setup(h, p, max_batch, H, W, C_in, mc, mi, 0);
+  const int form = p->centroid_model == -1 ? TD_GT : TD_MODEL;
+  if (const int rc = check_topdown(h, "sb_topdown_configure", p, form, max_batch, H, W, 0, 0, &mc, &mi)) return rc;
+  return topdown_setup(h, p, form, max_batch, H, W, C_in, mc, mi, 0, 0, 0);
 }
 
 int sb_infer_topdown(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B, float* out_centroids,
                      float* out_centroid_vals, float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid,
                      int32_t* out_flags) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+  SbTopdown* t = topdown_of(h, centroid_model_id, TD_MODEL, 0, false);
   if (!t) return SB_ERR_INVALID;
   if (const int rc = topdown_call(h, centroid_model_id, t, frames_host, frames_are_u8, B, "sb_infer_topdown")) return rc;
   split_topdown(t, t->slots.stage[0], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
@@ -930,7 +889,7 @@ int sb_topdown_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frame
 
 int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                        float* out_instance_peaks, float* out_instance_peak_vals, int32_t* out_n_valid, int32_t* out_flags) {
-  SbTopdown* t = topdown_of(h, model_id, false, true, TD_MODEL | TD_GT);
+  SbTopdown* t = topdown_of(h, model_id, TD_MODEL | TD_GT, 0, true);
   if (!t) return SB_ERR_INVALID;
   if (const int rc = topdown_collect(h, model_id, t, slot, B)) return rc;
   split_topdown(t, t->slots.stage[slot], B, out_centroids, out_centroid_vals, out_instance_peaks, out_instance_peak_vals, out_n_valid, out_flags);
@@ -939,40 +898,28 @@ int sb_topdown_collect(sb_handle_t h, int model_id, int slot, int B, float* out_
 
 int sb_topdown_gt_submit(sb_handle_t h, int instance_model_id, const uint8_t* frames_host, const float* centroids_host,
                          const int32_t* counts_host, int B, int slot) {
-  const SbModel* mi = chain_model(h, instance_model_id, SB_CHAIN_ANY, "top-down pipeline not configured");
-  if (!mi) return SB_ERR_INVALID;
-  SbTopdown* t = topdown_of(h, instance_model_id, mi->td && mi->td->multiclass, true, TD_GT);
-  if (!t) return SB_ERR_INVALID;
-  return topdown_gt_submit(h, t, frames_host, centroids_host, counts_host, B, slot);
+  return table_submit(h, instance_model_id, TD_GT, frames_host, centroids_host, counts_host, B, slot);
 }
 
 int sb_topdown_gt_instances_configure(sb_handle_t h, const sb_topdown_params* p, int n_nodes, int max_instances_per_frame, int max_batch,
                                       int H, int W, int C_in) {
-  static const char* const what = "sb_topdown_gt_instances_configure";
-  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "%s: null argument", what);
-  if (p->instance_model != -1) return sb_fail(h, SB_ERR_INVALID, "%s: instance_model must be -1", what);
-  SbModel* mc = chain_model(h, p->centroid_model, SB_CHAIN_ANY, "sb_topdown_gt_instances_configure: bad centroid model id");
-  if (!mc) return SB_ERR_INVALID;
-  if (p->max_centroids_per_frame <= 0 || n_nodes <= 0 || max_instances_per_frame <= 0 || max_batch <= 0)
-    return sb_fail(h, SB_ERR_INVALID, "%s: bad sizes", what);
-  if (max_batch > 1024) return sb_fail(h, SB_ERR_UNSUPPORTED, "%s: more than 1024 frames per batch", what);
-  float s;
-  int Hr, Wr;
-  if (const int rc = precrop_size(h, p, H, W, &s, &Hr, &Wr)) return rc;
-  return gt_instances_setup(h, p, n_nodes, max_instances_per_frame, max_batch, H, W, C_in, mc);
+  if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_gt_instances_configure: null argument");
+  SbModel *mc, *mi;
+  if (const int rc = check_topdown(h, "sb_topdown_gt_instances_configure", p, TD_GTI, max_batch, H, W, n_nodes, max_instances_per_frame,
+                                   &mc, &mi))
+    return rc;
+  return topdown_setup(h, p, TD_GTI, max_batch, H, W, C_in, mc, nullptr, 0, n_nodes, max_instances_per_frame);
 }
 
 int sb_topdown_gt_instances_submit(sb_handle_t h, int centroid_model_id, const uint8_t* frames_host, const float* instances_host,
                                    const int32_t* counts_host, int B, int slot) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, true, TD_GTI);
-  if (!t) return SB_ERR_INVALID;
-  return topdown_gt_instances_submit(h, h->models[centroid_model_id], t, frames_host, instances_host, counts_host, B, slot);
+  return table_submit(h, centroid_model_id, TD_GTI, frames_host, instances_host, counts_host, B, slot);
 }
 
 int sb_topdown_gt_instances_collect(sb_handle_t h, int centroid_model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                                     int32_t* out_n_centroids, float* out_instance_peaks, float* out_instance_peak_vals,
                                     int32_t* out_n_rows, int32_t* out_flags) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, true, TD_GTI);
+  SbTopdown* t = topdown_of(h, centroid_model_id, TD_GTI, -1, true);
   if (!t) return SB_ERR_INVALID;
   if (const int rc = topdown_collect(h, centroid_model_id, t, slot, B)) return rc;
   const size_t K = t->K, nd = t->nodes;
@@ -983,7 +930,7 @@ int sb_topdown_gt_instances_collect(sb_handle_t h, int centroid_model_id, int sl
 }
 
 int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_id, double img_h, double img_w) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false);
+  SbTopdown* t = topdown_of(h, centroid_model_id, TD_MODEL, 0, false);
   if (!t) return SB_ERR_INVALID;
   SbModel* mc = h->models[centroid_model_id];
   if (const int rc = t->slots.check_idle(h, "sb_topdown_attach_tracker")) return rc;
@@ -1001,7 +948,7 @@ int sb_topdown_attach_tracker(sb_handle_t h, int centroid_model_id, int tracker_
 }
 
 int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, double* out_tracks) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, false, true);
+  SbTopdown* t = topdown_of(h, centroid_model_id, TD_MODEL, 0, true);
   if (!t) return SB_ERR_INVALID;
   const SbModel* mc = h->models[centroid_model_id];
   if (!mc->trk) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_tracks: no tracker attached");
@@ -1015,7 +962,8 @@ int sb_topdown_tracks(sb_handle_t h, int centroid_model_id, int slot, int B, dou
 int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_params* p, int max_batch, int H, int W, int C_in) {
   if (!h || !p) return sb_fail(h, SB_ERR_INVALID, "sb_topdown_multiclass_configure: null argument");
   SbModel *mc, *mi;
-  int rc = check_topdown(h, &p->topdown, max_batch, H, W, &mc, &mi);
+  const int form = p->topdown.centroid_model == -1 ? TD_GT : TD_MODEL;
+  int rc = check_topdown(h, "sb_topdown_multiclass_configure", &p->topdown, form, max_batch, H, W, 0, 0, &mc, &mi);
   if (rc) return rc;
   if (p->topdown.precrop_resize != 0.f && p->topdown.precrop_resize != 1.f)
     return sb_fail(h, SB_ERR_UNSUPPORTED, "sb_topdown_multiclass_configure: instance models trained at an input scale != 1 (precrop_resize %g)",
@@ -1034,7 +982,7 @@ int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_p
   TdHead d;
   if ((rc = head_from_params(h, p, Hnet / tb.stride_den, Wnet / tb.stride_den, p->tap_channels, d))) return rc;
   // arguments checked: from here the previous chains are dropped
-  if ((rc = topdown_setup(h, &p->topdown, max_batch, H, W, C_in, mc, mi, p->n_classes))) return rc;
+  if ((rc = topdown_setup(h, &p->topdown, form, max_batch, H, W, C_in, mc, mi, p->n_classes, 0, 0))) return rc;
   SbModel* owner = mc ? mc : mi;
   SbTopdown* t = owner->td;
   t->head = d;
@@ -1053,7 +1001,7 @@ int sb_topdown_multiclass_configure(sb_handle_t h, const sb_topdown_multiclass_p
 int sb_infer_topdown_multiclass(sb_handle_t h, int centroid_model_id, const void* frames_host, int frames_are_u8, int B,
                                 float* out_centroids, float* out_centroid_vals, float* out_points, float* out_vals,
                                 float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags, float* out_class_vectors) {
-  SbTopdown* t = topdown_of(h, centroid_model_id, true);
+  SbTopdown* t = topdown_of(h, centroid_model_id, TD_MODEL, 1, false);
   if (!t) return SB_ERR_INVALID;
   if (const int rc = topdown_call(h, centroid_model_id, t, frames_host, frames_are_u8, B, "sb_infer_topdown_multiclass")) return rc;
   split_topdown_multiclass(t, t->slots.stage[0], t->probs_stage[0], B, out_centroids, out_centroid_vals, out_points, out_vals,
@@ -1068,7 +1016,7 @@ int sb_topdown_multiclass_submit(sb_handle_t h, int centroid_model_id, const uin
 int sb_topdown_multiclass_collect(sb_handle_t h, int model_id, int slot, int B, float* out_centroids, float* out_centroid_vals,
                                   float* out_points, float* out_vals, float* out_class_probs, int32_t* out_n_valid, int32_t* out_flags,
                                   float* out_class_vectors) {
-  SbTopdown* t = topdown_of(h, model_id, true, true, TD_MODEL | TD_GT);
+  SbTopdown* t = topdown_of(h, model_id, TD_MODEL | TD_GT, 1, true);
   if (!t) return SB_ERR_INVALID;
   if (const int rc = topdown_collect(h, model_id, t, slot, B)) return rc;
   split_topdown_multiclass(t, t->slots.stage[slot], t->probs_stage[slot], B, out_centroids, out_centroid_vals, out_points, out_vals,

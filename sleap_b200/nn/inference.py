@@ -425,7 +425,6 @@ class CentroidCropGroundTruth:
         self.input_scale = input_scale
         self.handle = handle
         self._resizer = None
-        self._pipeline = None        # the fused step's pipeline (_configure_ground_truth)
 
     def call(self, example_gt):
         from sleap_b200 import _lib
@@ -512,23 +511,6 @@ def _topdown_params(cc, fp):
                          int(cc.max_instances or 0), K, int(fp.max_crops_per_call), float(cc.precrop_resize)), K
 
 
-def _configure_topdown(cc, fp, fn_name, p, shape, *arrays):
-    """Configures the fused top-down pipeline with ``fn_name`` (``sb_topdown_configure`` or
-    ``sb_topdown_multiclass_configure``) for frames of ``shape`` (B, H, W, C) unless both models already run it with these
-    parameters; ``arrays`` are the ones the pointer fields of ``p`` point to."""
-    B, H, W, C = shape
-    mc, mi = cc.keras_model, fp.keras_model
-    # the pipeline's record on both models: a staged call on either one reconfigures its own chain, and this one again
-    record = (fn_name, chain_key(p, *arrays))
-    cap = max(B, mc.configured_for[0]) if mc.chain == record else B
-    if mc.chain != record or mi.chain != record or mc.configured_for != (cap, H, W, C):
-        mc.chain = mi.chain = None
-        mc.handle.call(fn_name, byref(p), cap, H, W, C)
-        mc.configured_for = (cap, H, W, C)
-        mi.configured_for = (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C)
-        mc.chain = mi.chain = record
-
-
 def _centroid_table(centroids, K):
     """The ragged ground-truth centroids of a batch (one (n, 2) array per frame) as sb_topdown_gt_submit takes them: the
     (B, K, 2) float32 table, NaN past each frame's count, and the (B,) int32 counts.  A frame with more than K centroids
@@ -539,43 +521,6 @@ def _centroid_table(centroids, K):
     for b, c in enumerate(cents):
         table[b, :len(c)] = c[:K]
     return table, counts
-
-
-def _call_ground_truth(im, example):
-    """One batch of top-down model ``im`` with ground-truth centroids (uint8 ``image`` and ``centroids``) through its fused
-    step: the table packed for the pipeline's K (grown to the batch's largest count if needed), sb_topdown_gt_submit into
-    slot 0, then the collect."""
-    imgs = InferenceLayer._prep(example["image"])
-    B = imgs.shape[0]
-    n = max([len(f32(c).reshape(-1, 2)) for c in example["centroids"]] + [0])
-    K = im._configure_ground_truth(B, n, imgs.shape[1:])
-    table, counts = _centroid_table(example["centroids"], K)
-    m = im.instance_peaks.keras_model
-    m.handle.call("sb_topdown_gt_submit", m.model_id, ptr(imgs), ptr(table), ptr(counts), B, 0)
-    return im._run_ground_truth(B, K, 0)
-
-
-def _configure_ground_truth(cc, fp, fn_name, make_params, B, K, shape, *arrays):
-    """Configures the ground-truth top-down pipeline (``make_params(K)``: the parameters with centroid_model -1, for
-    ``fn_name``) of ground-truth layer ``cc`` on instance layer ``fp`` for batches of up to B frames of ``shape``
-    (H, W, C) with up to K centroids each, unless it already runs with at least these capacities: B and K grow only when a
-    batch exceeds them.  ``arrays`` are the ones the pointer fields of the parameters point to.  Returns the pipeline's K."""
-    mi = fp.keras_model
-    what = (fn_name, chain_key(make_params(0), *arrays), tuple(shape))     # the pipeline apart from its capacities
-    have = cc._pipeline                      # (what, B, K, the instance model's chain record) of the last configure
-    if have is not None and have[0] == what and mi.chain is have[3]:
-        if B <= have[1] and K <= have[2]:
-            return have[2]
-        B, K = max(B, have[1]), max(K, have[2])
-    K = max(K, 1)
-    p = make_params(K)
-    mi.chain = None                          # a refused call may have dropped the previous chain
-    mi.handle.call(fn_name, byref(p), B, *shape)
-    # the instance network's plan: chunks of max_crops_per_call crops, but no more than a batch's B x K (include/sleap_b200.h)
-    mi.configured_for = (min(fp.max_crops_per_call, B * K), cc.crop_size, cc.crop_size, shape[2])
-    mi.chain = (fn_name, chain_key(p, *arrays))
-    cc._pipeline = (what, B, K, mi.chain)
-    return K
 
 
 def _ground_truth_params(cc, fp, K):
@@ -615,8 +560,20 @@ def _gt_instances_params(cc):
                          float(cc.precrop_resize)), K
 
 
+# The last configure of a top-down pipeline (TopDownInferenceModel._configure_pipeline): its call at capacities 0 (the
+# call's name, the chain key of its parameters, the arguments after them), its capacities (B, then K or N), the chain
+# record it set and the device models it set it on.
+_Configured = collections.namedtuple("_Configured", "key caps chain models")
+
+
 class TopDownInferenceModel(InferenceModel):
-    """sleap/nn/inference.py:2246-2311."""
+    """sleap/nn/inference.py:2246-2311.  The fused pipeline takes one of three centroid sources: a centroid model, the
+    ground-truth centroids of labels (CentroidCropGroundTruth), or a centroid model matched against ground-truth instances
+    (FindInstancePeaksGroundTruth).  TopDownMultiClassInferenceModel shares the configure, the streams and the dispatch,
+    and supplies its own parameters (``_params``), calls and result builder (``_run_fused``)."""
+
+    CONFIGURE, INFER, SUBMIT, COLLECT = "sb_topdown_configure", "sb_infer_topdown", "sb_topdown_submit", "sb_topdown_collect"
+    _keep = ()          # the arrays the pointer fields of ``_params`` point to
 
     def __init__(self, centroid_crop, instance_peaks):
         self.centroid_crop = centroid_crop
@@ -624,7 +581,7 @@ class TopDownInferenceModel(InferenceModel):
         self.fused = True            # one device pipeline (sb_infer_topdown) when both stages are device models
         # a Tracker with track_device, run by k_track inside each fused step (TopDownPredictor.predict sets it for its span)
         self.tracker = None
-        self._gt_instances = None    # (what, B, N, the centroid model's chain record) of the last ground-truth instances configure
+        self._pipeline = None        # the _Configured of the last pipeline configure
 
     def detach_tracker(self):
         mc = self.centroid_crop.keras_model
@@ -652,25 +609,73 @@ class TopDownInferenceModel(InferenceModel):
         return (self.fused and type(self.instance_peaks) is FindInstancePeaksGroundTruth and type(cc) is CentroidCrop
                 and not cc.return_confmaps and (cc.max_instances is None or cc.max_instances > 0))
 
-    def _configure_gt_instances(self, B, N, nodes, shape):
-        """The ground-truth instances pipeline of the centroid model for batches of up to B frames of ``shape`` (H, W, C)
-        with tables of up to N instances of ``nodes`` nodes, unless it already runs with at least these capacities: B and
-        N grow only when a batch exceeds them.  Returns (K, N) of the pipeline."""
-        cc = self.centroid_crop
+    def _params(self, td):
+        """The parameters of ``CONFIGURE`` over TopdownParams ``td``."""
+        return td
+
+    def _configure_pipeline(self, fn, args, caps, plans, arrays=()):
+        """Configures a form of the pipeline with ``fn(byref(p), *rest)``, where (p, *rest) = ``args(*caps)``.  When the
+        last configure made the same call at capacities 0 and every model it configured still runs the chain it set, the
+        capacities ``caps`` (B, then K or N) grow to the larger of asked and held, and nothing is called while the held ones
+        suffice; otherwise the call is made at the asked ones.  ``plans(*caps)``: (device model, its configured_for) of each
+        model the pipeline uses, the one that holds it first; ``arrays``: the ones the pointer fields of p point to.
+        Returns the pipeline's capacities."""
+        p0, *rest0 = args(*(0,) * len(caps))
+        key = (fn, chain_key(p0, *arrays), tuple(rest0))
+        have = self._pipeline
+        if have is not None and have.key == key and all(m.chain is have.chain for m in have.models):
+            if all(c <= h for c, h in zip(caps, have.caps)):
+                return have.caps
+            caps = tuple(max(c, h) for c, h in zip(caps, have.caps))
+        p, *rest = args(*caps)
+        plan = plans(*caps)
+        for m, _ in plan:
+            m.chain = None                       # a refused call may have dropped the previous chain
+        plan[0][0].handle.call(fn, byref(p), *rest)
+        chain = (fn, chain_key(p, *arrays))
+        for m, configured_for in plan:
+            m.configured_for, m.chain = configured_for, chain
+        self._pipeline = _Configured(key, tuple(caps), chain, [m for m, _ in plan])
+        return self._pipeline.caps
+
+    def _configure_fused(self, B, H, W, C):
+        """The pipeline with a centroid model for batches of up to B frames of (H, W, C), with ``self.tracker`` attached
+        (the raw frame size, as the predictor's image_hw; default capacity, not K).  Returns K."""
+        cc, fp = self.centroid_crop, self.instance_peaks
         mc = cc.keras_model
+        td, K = _topdown_params(cc, fp)
+        p = self._params(td)
+        self._configure_pipeline(self.CONFIGURE, lambda b: (p, b, H, W, C), (B,),
+                                 lambda b: [(mc, (b, H, W, C)), (fp.keras_model, (fp.max_crops_per_call, cc.crop_size, cc.crop_size, C))],
+                                 self._keep)
+        if self.tracker is not None:
+            dev = self.tracker._device_tracker(head_channels(fp.keras_model, fp.HEAD), handle=mc.handle)
+            mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
+        return K
+
+    def _configure_ground_truth(self, B, K, shape):
+        """The ground-truth centroids pipeline of the instance model (sb_topdown_gt_submit) for batches of up to B frames
+        of ``shape`` (H, W, C) with up to K centroids each: B and K grow only when a batch exceeds them, and K is at least
+        1.  Returns the pipeline's K."""
+        cc, fp = self.centroid_crop, self.instance_peaks
+        shape = tuple(shape)
+        _, K = self._configure_pipeline(
+            self.CONFIGURE, lambda b, k: (self._params(_ground_truth_params(cc, fp, k)), b) + shape, (B, max(K, 1)),
+            # the instance network's plan: chunks of max_crops_per_call crops, but no more than a batch's B x K
+            # (include/sleap_b200.h)
+            lambda b, k: [(fp.keras_model, (min(fp.max_crops_per_call, b * k), cc.crop_size, cc.crop_size, shape[2]))],
+            self._keep)
+        return K
+
+    def _configure_gt_instances(self, B, N, nodes, shape):
+        """The ground-truth instances pipeline of the centroid model (sb_topdown_gt_instances_submit) for batches of up
+        to B frames of ``shape`` (H, W, C) with tables of up to N instances of ``nodes`` nodes: B and N grow only when a
+        batch exceeds them, and N is at least 1.  Returns (K, N) of the pipeline."""
+        cc = self.centroid_crop
+        shape = tuple(shape)
         p, K = _gt_instances_params(cc)
-        what = (chain_key(p), int(nodes), tuple(shape))
-        have = self._gt_instances
-        if have is not None and have[0] == what and mc.chain is have[3]:
-            if B <= have[1] and N <= have[2]:
-                return K, have[2]
-            B, N = max(B, have[1]), max(N, have[2])
-        N = max(N, 1)
-        mc.chain = None                          # a refused call may have dropped the previous chain
-        mc.handle.call("sb_topdown_gt_instances_configure", byref(p), int(nodes), N, B, *shape)
-        mc.configured_for = (B,) + tuple(shape)
-        mc.chain = ("sb_topdown_gt_instances_configure", chain_key(p))
-        self._gt_instances = (what, B, N, mc.chain)
+        _, N = self._configure_pipeline("sb_topdown_gt_instances_configure", lambda b, n: (p, int(nodes), n, b) + shape,
+                                        (B, max(N, 1)), lambda b, n: [(cc.keras_model, (b,) + shape)])
         return K, N
 
     def _run_gt_instances(self, B, K, nodes, slot):
@@ -686,33 +691,10 @@ class TopDownInferenceModel(InferenceModel):
         return {"centroids": ce[:, :c].copy(), "centroid_vals": cv[:, :c].copy(), "instance_peaks": ip[:, :r].copy(),
                 "instance_peak_vals": iv[:, :r].copy(), "n_valid": nr.astype(np.int64), "flags": fl}
 
-    def _call_gt_instances(self, example, imgs, nodes):
-        """One batch through the ground-truth instances step: the table packed for the pipeline's N (grown to the batch's
-        most instances if needed), a submit into slot 0, then its collect."""
-        B = imgs.shape[0]
-        n = max([len(a) for a in example["instances"]] + [0])
-        K, N = self._configure_gt_instances(B, n, nodes, imgs.shape[1:])
-        table, counts = _instance_table(example["instances"], N, nodes)
-        mc = self.centroid_crop.keras_model
-        mc.handle.call("sb_topdown_gt_instances_submit", mc.model_id, ptr(imgs), ptr(table), ptr(counts), B, 0)
-        return self._run_gt_instances(B, K, nodes, 0)
-
     def _owner(self):
         """The device model that holds the fused pipeline: the centroid model, or with ground-truth centroids the
         instance model."""
         return self.instance_peaks.keras_model if self.ground_truth else self.centroid_crop.keras_model
-
-    def _configure_fused(self, B, H, W, C):
-        """The fused pipeline for batches of up to B frames of (H, W, C), with ``self.tracker`` attached (the raw frame
-        size, as the predictor's image_hw; default capacity, not K).  Returns K."""
-        cc, fp = self.centroid_crop, self.instance_peaks
-        mc = cc.keras_model
-        p, K = _topdown_params(cc, fp)
-        _configure_topdown(cc, fp, "sb_topdown_configure", p, (B, H, W, C))
-        if self.tracker is not None:
-            dev = self.tracker._device_tracker(head_channels(fp.keras_model, fp.HEAD), handle=mc.handle)
-            mc.handle.call("sb_topdown_attach_tracker", mc.model_id, dev.id, float(H), float(W))
-        return K
 
     def _run_fused(self, B, K, fn, *args, slot=0):
         """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown or sb_topdown_collect) into dense arrays
@@ -729,30 +711,24 @@ class TopDownInferenceModel(InferenceModel):
         return out
 
     def _call_fused(self, imgs):
-        """sb_infer_topdown: frames up once, centroid peaks / top-k / crops / instance network / peaks on the device, one
-        dense record back (include/sleap_b200.h)."""
+        """``INFER``: frames up once, the whole step on the device, one dense record per frame back (include/sleap_b200.h)."""
         imgs = self.centroid_crop._prep(imgs)
         B, H, W, C = imgs.shape
         K = self._configure_fused(B, H, W, C)
-        return self._run_fused(B, K, "sb_infer_topdown", ptr(imgs), int(imgs.dtype == np.uint8))
+        return self._run_fused(B, K, self.INFER, ptr(imgs), int(imgs.dtype == np.uint8))
 
     def _stream(self, first, batch_size):
-        """sb_topdown_submit / sb_topdown_collect (the upload of batch i+1 and its centroid stage are queued before batch
-        i is collected): uint8 frames and a model that can run the fused step with a centroid model."""
+        """``SUBMIT`` / ``COLLECT`` (the upload of batch i+1 and its centroid stage are queued before batch i is
+        collected): uint8 frames and a model that can run the fused step with a centroid model."""
         if not self._can_fuse() or self.ground_truth or first.dtype != np.uint8:
             return None
         K = self._configure_fused(batch_size, *first.shape[1:])
-        return (self.centroid_crop.keras_model, "sb_topdown_submit",
-                lambda slot, B: self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot))
-
-    def _configure_ground_truth(self, B, K, shape):
-        cc, fp = self.centroid_crop, self.instance_peaks
-        return _configure_ground_truth(cc, fp, "sb_topdown_configure", lambda k: _ground_truth_params(cc, fp, k), B, K, shape)
+        return (self.centroid_crop.keras_model, self.SUBMIT, lambda slot, B: self._run_fused(B, K, self.COLLECT, slot, slot=slot))
 
     def _stream_ground_truth(self, first, batch_size, max_centroids, ex=None):
-        """sb_topdown_gt_submit / sb_topdown_collect: uint8 frames and a model that can run the fused step with
-        ground-truth centroids; or sb_topdown_gt_instances_submit / _collect: uint8 frames and ground-truth instances
-        (``ex``) for a centroid model, tables of ``max_centroids`` instances.  The whole step is queued at the submit."""
+        """sb_topdown_gt_submit / ``COLLECT``: uint8 frames and a model that can run the fused step with ground-truth
+        centroids; or sb_topdown_gt_instances_submit / _collect: uint8 frames and ground-truth instances (``ex``) for a
+        centroid model, tables of ``max_centroids`` instances.  The whole step is queued at the submit."""
         if first.dtype != np.uint8:
             return None
         if self._fuses_instances():
@@ -770,24 +746,30 @@ class TopDownInferenceModel(InferenceModel):
     def _ground_truth_table(self, ex, K):
         if not self._fuses_instances():
             return super()._ground_truth_table(ex, K)
-        nodes = self._gt_instances[0][1]
+        nodes = self._pipeline.key[2][0]         # the node count: the first argument after the parameters
         return _instance_table(ex["instances"], K, nodes) if _instance_nodes(ex["instances"]) == nodes else None
 
     def _run_ground_truth(self, B, K, slot):
-        return self._run_fused(B, K, "sb_topdown_collect", slot, slot=slot)
+        return self._run_fused(B, K, self.COLLECT, slot, slot=slot)
 
     def call(self, example):
         if isinstance(example, np.ndarray):
             example = dict(image=example)
-        if self._fuses_instances() and "instances" in example:
-            imgs = InferenceLayer._prep(example["image"])
-            nodes = _instance_nodes(example["instances"])
-            if imgs.dtype == np.uint8 and nodes is not None:
-                return self._call_gt_instances(example, imgs, nodes)
         if self._can_fuse() and not self.ground_truth:
             return self._call_fused(_images_of(example))
-        if self._can_fuse() and "centroids" in example and np.asarray(example["image"]).dtype == np.uint8:
-            return _call_ground_truth(self, example)
+        rows = "instances" if self._fuses_instances() else "centroids"
+        if rows in example and np.asarray(example["image"]).dtype == np.uint8:
+            # one batch through the ground-truth step: its submit into slot 0, then the collect
+            imgs = InferenceLayer._prep(example["image"])
+            B = imgs.shape[0]
+            got = self._stream_ground_truth(imgs, B, max([len(a) for a in example[rows]] + [0]), example)
+            if got is not None:
+                (m, fn, collect), cap = got
+                m.handle.call(fn, m.model_id, ptr(imgs), *map(ptr, self._ground_truth_table(example, cap)), B, 0)
+                return collect(0, B)
+        return self._call_staged(example)
+
+    def _call_staged(self, example):
         crop_out = self.centroid_crop.call(example)
         if isinstance(self.instance_peaks, FindInstancePeaksGroundTruth):                 # :2300-2304
             peaks_out = self.instance_peaks.call(example, crop_out)
@@ -1266,17 +1248,16 @@ def topdown_multiclass_from_features(cms, features, crop_sample_inds, n_samples,
     return {"instance_peaks": pts, "instance_peak_vals": vals, "instance_scores": probs, "class_vectors": cvec, "features": feats}
 
 
-class TopDownMultiClassInferenceModel(InferenceModel):
+class TopDownMultiClassInferenceModel(TopDownInferenceModel):
     """sleap/nn/inference.py:4139-4210: centroid stage (model or ground truth) -> TopDownMultiClassFindPeaks.
 
-    With a centroid model the whole chain runs as one device step (``sb_infer_topdown_multiclass``): centroids, top-k,
-    crops, instance network, global peaks, the class-vector head (k_class_vectors) and the per-frame assignment of crops
-    to classes (k_td_class_assign).  ``fused = False`` keeps the staged path (ground-truth centroids always use it)."""
+    The whole chain runs as one device step (``sb_infer_topdown_multiclass``): centroids, top-k, crops, instance network,
+    global peaks, the class-vector head (k_class_vectors) and the per-frame assignment of crops to classes
+    (k_td_class_assign); with ground-truth centroids, the same step from the crops on.  ``fused = False`` keeps the staged
+    path."""
 
-    def __init__(self, centroid_crop, instance_peaks: TopDownMultiClassFindPeaks):
-        self.centroid_crop = centroid_crop
-        self.instance_peaks = instance_peaks
-        self.fused = True
+    CONFIGURE, INFER = "sb_topdown_multiclass_configure", "sb_infer_topdown_multiclass"
+    SUBMIT, COLLECT = "sb_topdown_multiclass_submit", "sb_topdown_multiclass_collect"
 
     def _can_fuse(self):
         cc, fp = self.centroid_crop, self.instance_peaks
@@ -1288,29 +1269,19 @@ class TopDownMultiClassInferenceModel(InferenceModel):
         return (type(cc) is CentroidCrop and cc.precrop_resize == 1.0 and cc.return_crops and not cc.return_confmaps
                 and cc.keras_model.handle is fp.keras_model.handle)
 
-    ground_truth = TopDownInferenceModel.ground_truth
-    _owner = TopDownInferenceModel._owner
+    @property
+    def _keep(self):
+        return (self.instance_peaks.dense,)
 
-    def _configure_fused(self, B, H, W, C):
-        """The fused pipeline for batches of up to B frames of (H, W, C).  Returns (K, n_classes)."""
-        cc, fp = self.centroid_crop, self.instance_peaks
-        td, K = _topdown_params(cc, fp)
-        p = topdown_multiclass_params(td, fp.keras_model.cm.vector_taps[fp.CLASS_VECTORS], fp.class_head, fp.dense)
-        _configure_topdown(cc, fp, "sb_topdown_multiclass_configure", p, (B, H, W, C), fp.dense)
-        return K, p.n_classes
+    def _params(self, td):
+        fp = self.instance_peaks
+        return topdown_multiclass_params(td, fp.keras_model.cm.vector_taps[fp.CLASS_VECTORS], fp.class_head, fp.dense)
 
-    def _call_fused(self, imgs):
-        """sb_infer_topdown_multiclass: frames up once, one record per frame back (include/sleap_b200.h)."""
-        imgs = self.centroid_crop._prep(imgs)
-        B, H, W, C = imgs.shape
-        K, NC = self._configure_fused(B, H, W, C)
-        return self._run_fused(B, K, NC, "sb_infer_topdown_multiclass", ptr(imgs), int(imgs.dtype == np.uint8))
-
-    def _run_fused(self, B, K, NC, fn, *args):
+    def _run_fused(self, B, K, fn, *args, slot=0):
         """One fused call ``fn(model id, *args, B, <outputs>)`` (sb_infer_topdown_multiclass or
-        sb_topdown_multiclass_collect) into dense arrays of B frames, as a batch dict."""
+        sb_topdown_multiclass_collect) into dense arrays of B frames, as a batch dict (no tracker: ``slot`` is unused)."""
         fp, mc = self.instance_peaks, self._owner()
-        N = head_channels(fp.keras_model, fp.HEAD)
+        N, NC = head_channels(fp.keras_model, fp.HEAD), int(fp.class_head["channels"])
         ce = np.zeros((B, K, 2), np.float32); cv = np.zeros((B, K), np.float32)
         pts = np.zeros((B, NC, N, 2), np.float32); vals = np.zeros((B, NC, N), np.float32); probs = np.zeros((B, NC), np.float32)
         nv = np.zeros((B,), np.int32); fl = np.zeros((B,), np.int32)
@@ -1323,39 +1294,7 @@ class TopDownMultiClassInferenceModel(InferenceModel):
             out["class_vectors"] = np.concatenate([cvec[b, :nv[b]] for b in range(B)])
         return out
 
-    def _stream(self, first, batch_size):
-        """sb_topdown_multiclass_submit / _collect, as TopDownInferenceModel's: uint8 frames and a model that can run the
-        fused step with a centroid model."""
-        if not self._can_fuse() or self.ground_truth or first.dtype != np.uint8:
-            return None
-        K, NC = self._configure_fused(batch_size, *first.shape[1:])
-        return (self.centroid_crop.keras_model, "sb_topdown_multiclass_submit",
-                lambda slot, B: self._run_fused(B, K, NC, "sb_topdown_multiclass_collect", slot))
-
-    def _configure_ground_truth(self, B, K, shape):
-        cc, fp = self.centroid_crop, self.instance_peaks
-        tap = fp.keras_model.cm.vector_taps[fp.CLASS_VECTORS]
-        return _configure_ground_truth(cc, fp, "sb_topdown_multiclass_configure",
-                                       lambda k: topdown_multiclass_params(_ground_truth_params(cc, fp, k), tap, fp.class_head, fp.dense),
-                                       B, K, shape, fp.dense)
-
-    def _run_ground_truth(self, B, K, slot):
-        return self._run_fused(B, K, head_channels(self.instance_peaks.keras_model, "ClassVectorsHead"), "sb_topdown_multiclass_collect", slot)
-
-    def _stream_ground_truth(self, first, batch_size, max_centroids, ex=None):
-        """sb_topdown_gt_submit / sb_topdown_multiclass_collect, as TopDownInferenceModel's."""
-        if not (self._can_fuse() and self.ground_truth) or first.dtype != np.uint8:
-            return None
-        K = self._configure_ground_truth(batch_size, max_centroids, first.shape[1:])
-        return (self.instance_peaks.keras_model, "sb_topdown_gt_submit", lambda slot, B: self._run_ground_truth(B, K, slot)), K
-
-    def call(self, example):
-        if isinstance(example, np.ndarray):
-            example = dict(image=example)
-        if self._can_fuse() and not self.ground_truth:
-            return self._call_fused(_images_of(example))
-        if self._can_fuse() and "centroids" in example and np.asarray(example["image"]).dtype == np.uint8:
-            return _call_ground_truth(self, example)
+    def _call_staged(self, example):
         crop_out = self.centroid_crop.call(example)
         out = self.instance_peaks.call(crop_out)
         res = {k: out[k] for k in ("instance_peaks", "instance_peak_vals", "instance_scores")}

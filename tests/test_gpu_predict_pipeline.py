@@ -373,5 +373,5 @@ def test_multiclass_refusals():
         mc.handle.call("sb_infer_topdown_multiclass", mc.model_id, _lib.ptr(frames), 1, 2, *([None] * 8))
     with pytest.raises(_lib.SleapB200Error, match="is multi-class"):
         mc.handle.call("sb_topdown_collect", mc.model_id, 0, 2, *([None] * 6))
-    K, NC = im._configure_fused(2, *frames.shape[1:])
-    assert_same_batches([im._run_fused(2, K, NC, "sb_topdown_multiclass_collect", 0)], [want])
+    K = im._configure_fused(2, *frames.shape[1:])
+    assert_same_batches([im._run_fused(2, K, "sb_topdown_multiclass_collect", 0)], [want])

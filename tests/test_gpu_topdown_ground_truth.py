@@ -211,10 +211,10 @@ def test_results_do_not_depend_on_K(dev):
     ex = dict(image=frames, centroids=_centroids(97, 131, [2, 0, 3, 1], 7))
     im = _predictor(dev, 1, 0.5).inference_model
     a = im.predict_on_batch(ex)
-    assert im.centroid_crop._pipeline[2] == 3
+    assert im._pipeline.caps[1] == 3
     assert im._configure_ground_truth(4, 11, frames.shape[1:]) == 11
     b = im.predict_on_batch(ex)
-    assert im.centroid_crop._pipeline[2] == 11
+    assert im._pipeline.caps[1] == 11
     assert_same_batches([a], [b])
 
 
@@ -325,7 +325,7 @@ def test_refusals_keep_the_pipeline(dev):
     im = _predictor(dev, 1, 0.5).inference_model
     want = im.predict_on_batch(ex)
     m = im.instance_peaks.keras_model
-    K = im.centroid_crop._pipeline[2]
+    K = im._pipeline.caps[1]
     table, counts = _centroid_table(cents, K)
     L, h = _lib.lib(), m.handle.h
 

@@ -204,7 +204,7 @@ def test_caps_past_one_pass(dev):
         ex = dict(image=frames, instances=insts)
         out = _fused_and_host(im, ex)
         assert out["n_valid"].tolist() == [len(c) for c in cents]
-        assert im._gt_instances[2] == 40 and im._gt_instances[0][1] == 20
+        assert im._pipeline.caps[1] == 40 and im._pipeline.key[2][0] == 20      # N, and the node count
     from sleap_b200.nn.inference import _instance_table
     im.predict_on_batch(ex)                                              # the host route's centroid call dropped the pipeline
     m = im.centroid_crop.keras_model
@@ -335,7 +335,7 @@ def test_refusals_and_chain_rules(dev):
     im.predict_on_batch(ex)                                              # the host route's centroid call dropped the pipeline
     m = im.centroid_crop.keras_model
     L, h = _lib.lib(), m.handle.h
-    N = im._gt_instances[2]
+    N = im._pipeline.caps[1]
     table, counts = _instance_table(insts, N, 4)
 
     def submit(slot, c=counts):

@@ -2,9 +2,9 @@
 networks -- single-instance (sb_global_submit / _collect), bottom-up (sb_bottomup_*) plain and with an attached device
 tracker, bottom-up identity (sb_multiclass_*), top-down (sb_topdown_submit / _collect) plain, with an attached device
 tracker and with several instance chunks per batch, top-down identity (sb_topdown_multiclass_*, class vectors
-returned), and ground-truth top-down (sb_topdown_gt_submit) plain and identity -- each checked against the per-batch
-route, so that the copy stream, the deferred instance stage and the per-slot staging run under memcheck / racecheck in
-minutes.
+returned), ground-truth top-down (sb_topdown_gt_submit) plain and identity, and a centroid model with ground-truth
+instances (sb_topdown_gt_instances_*) -- each checked against the per-batch route, so that the copy stream, the
+deferred instance stage and the per-slot staging run under memcheck / racecheck in minutes.
 Usage: compute-sanitizer --tool memcheck python tools/sanitize_stream.py"""
 import os
 import sys
@@ -44,11 +44,16 @@ def same(im, frames, tracker=None, holder=None):
     return sum(len(x["instance_peaks"]) for x in streamed)
 
 
-def same_ground_truth(im, frames, seed):
-    """predict_examples (sb_topdown_gt_submit / collect) against predict_on_batch on labels of 0-3 random centroids."""
+def same_ground_truth(im, frames, seed, nodes=0):
+    """predict_examples (sb_topdown_gt_submit / collect) against predict_on_batch on labels of 0-3 random centroids; with
+    `nodes`, (sb_topdown_gt_instances_submit / _collect) on labels of 0-3 random instances of that many nodes, some NaN."""
     rng = np.random.default_rng(seed)
-    cents = [rng.uniform(0, [frames.shape[2], frames.shape[1]], (int(rng.integers(0, 4)), 2)).astype(np.float32) for _ in frames]
-    examples = [dict(image=frames[i:i + B], centroids=cents[i:i + B]) for i in range(0, len(frames), B)]
+    rows = [rng.uniform(0, [frames.shape[2], frames.shape[1]], (int(rng.integers(0, 4)),) + ((nodes, 2) if nodes else (2,)))
+            .astype(np.float32) for _ in frames]
+    for r in rows if nodes else ():
+        r[rng.random(r.shape[:2]) < 0.3] = np.nan
+    key = "instances" if nodes else "centroids"
+    examples = [{"image": frames[i:i + B], key: rows[i:i + B]} for i in range(0, len(frames), B)]
     n = 0
     for ex, a in list(im.predict_examples(iter(examples), B, 3)):      # streamed first: predict_on_batch uses slot 0
         b = im.predict_on_batch(ex)
@@ -108,6 +113,8 @@ def main():
     im.tracker = None
     gt = TopDownPredictor(None, im_model, crop_size=64, peak_threshold=0.0, batch_size=B).inference_model
     print("ground-truth top-down", same_ground_truth(gt, frames, 73), flush=True)
+    gti = TopDownPredictor(cm, None, peak_threshold=thr, batch_size=B, max_instances=4).inference_model
+    print("ground-truth instances top-down", same_ground_truth(gti, frames, 77, len(NODES)), flush=True)
 
     classes = ["c0", "c1", "c2"]
     mspec = dict(ispec, head_type="multi_class_topdown", classes=classes,
